@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Headline benchmark: batched put + get throughput of the object store on N B200 workers.
+"""Headline benchmark: batched put + get throughput of the object store on N H100 workers.
 
 Metric (BASELINE.json): batched put/get GB/s (and p50 / p99 us) at 1/2/4/8 GPU-tier workers, synthetic random-byte
 objects, device-timed, max over ranks.  One *step* = one `batch_put_device` of B objects of S bytes (fused kernel:
@@ -32,15 +32,14 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 BASELINE_GBPS = 0.233  # the only throughput figure in the reference tree (configs/worker.yaml:19, unsourced)
-NVLINK_NOMINAL_GBPS = 900.0  # BASELINE.json: per direction per GPU
+NVLINK_NOMINAL_GBPS = 450.0  # NVLink 4 (H100 SXM, 18 links): per direction per GPU
+HBM_NOMINAL_GBPS = 3350.0  # H100 SXM 80 GB HBM3
 
 
 def reference_arm() -> int:
     """The reference cannot be installed or built offline (DESIGN.md section 3 records the attempts)."""
-    why = ("blackbird-io/blackbird is a CMake C++ project with no Python package: `pip install --no-index --no-build-isolation "
-           "--find-links /opt/wheelhouse --target baseline/_ref /root/reference` fails (neither setup.py nor pyproject.toml); cmake "
-           "configure needs the network (yalantinglibs / GoogleTest FetchContent) and UCX, etcd-cpp-apiv3, glog, yaml-cpp, liburing "
-           "which are absent here and on the GPU box (profiles/r2_nvlink/ucx_probe.txt: no ucx_info, no /opt/hpcx, no libucp); "
+    why = ("blackbird-io/blackbird is a CMake C++ project with no Python package (neither setup.py nor pyproject.toml); its cmake "
+           "configure fetches yalantinglibs / GoogleTest over the network and needs UCX, etcd-cpp-apiv3, glog, yaml-cpp and liburing; "
            "src/worker/storage/cxl_memory_backend.cpp does not compile at this commit; its GPU pools are std::malloc")
     if int(os.environ.get("RANK", "0")) == 0:  # one line for the job, also when launched under torchrun
         print(json.dumps({"impl": "reference", "unavailable": why}))
@@ -72,6 +71,9 @@ def main() -> int:
                     help="N>1: ranks rendezvous per step / per put-get phase (inside the timed region)")
     ap.add_argument("--idle-odd", action="store_true", help="diagnostic: odd ranks idle (unidirectional NVLink traffic)")
     ap.add_argument("--quick", action="store_true", help="sweep config: fewer sizes")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="headline config: after the timed steps, write what the last timed step computed to DIR/<name>.npy "
+                         "(a fixed, seeded sample of the bytes its get returned, the returned sizes, the digests its put recorded)")
     args = ap.parse_args()
     if args.impl == "reference":
         return reference_arm()
@@ -110,7 +112,7 @@ def run_headline(args, world: int) -> int:
                                 preferred_classes=[_bb.StorageClass.RAM_GPU])
 
     cfg = cfg_for(algo)
-    # synthetic random-byte objects: payload (1 GiB by default) is larger than L2 (126 MB)
+    # synthetic random-byte objects: payload (4 GiB by default) is larger than L2 (50 MB)
     src = torch.empty(step_bytes, dtype=torch.uint8, device=dev)
     _bb.random_fill(src.data_ptr(), step_bytes, 0xB200 + rank, stream)
     out = torch.empty(step_bytes, dtype=torch.uint8, device=dev)
@@ -126,8 +128,9 @@ def run_headline(args, world: int) -> int:
         if world > 1:
             cl.host_barrier()
 
-    def step(tag: str, i: int, keys=None, put_ptrs=None, get_ptrs=None, c=None):
+    def step(tag: str, i: int, keys=None, put_ptrs=None, get_ptrs=None, c=None, remove=True):
         keys = keys or [f"r{rank}/{tag}{i}/o{j}" for j in range(nobj)]
+        got = None
         if args.sync != "none":
             rendezvous()  # bulk-synchronous step (checkpoint / KV hand-off pattern): all ranks put, then all ranks get
         if not idle:
@@ -136,10 +139,12 @@ def run_headline(args, world: int) -> int:
         if args.sync == "phase":
             rendezvous()
         if not idle:
-            ecs, _ = cl.client.batch_get_device(keys, get_ptrs or out_ptrs, sizes, stream)
+            ecs, got = cl.client.batch_get_device(keys, get_ptrs or out_ptrs, sizes, stream)
             assert all(e == OK for e in ecs), f"get failed: {[str(e) for e in ecs if e != OK][:3]}"
-            ecs = cl.client.batch_remove(keys)
-            assert all(e == OK for e in ecs)
+            if remove:
+                ecs = cl.client.batch_remove(keys)
+                assert all(e == OK for e in ecs)
+        return got
 
     if args.ctas:
         cl.fabric.set_max_ctas(args.ctas)
@@ -159,11 +164,14 @@ def run_headline(args, world: int) -> int:
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(args.steps):
-        step("t", i, all_keys[i])
+        # with --dump-outputs the last step's objects stay until their digests have been read (after the timed region)
+        got = step("t", i, all_keys[i], remove=not (args.dump_outputs and i + 1 == args.steps))
     e1.record()
     torch.cuda.synchronize()
     cl.barrier()
     ms = cl.max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and args.steps > 0:
+        dump_headline_outputs(args.dump_outputs, cl, rank, out, got, all_keys[-1], idle)
     launches = int(cl.sum_over_ranks(cl.fabric.launches - launches0))
     if ms < 1500:  # give nvidia-smi time to take samples under the same load (same count on every rank: steps rendezvous)
         for i in range(int(1200.0 / max(ms / args.steps, 0.05)) + 1):
@@ -380,26 +388,20 @@ def run_headline(args, world: int) -> int:
         except Exception:
             pass
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except OSError:
-            pass
         per_gpu = value / world
         if world == 1:
-            roof = {"per_gpu_GBps": round(per_gpu, 1), "denominator_GBps": round(peaks.get("hbm_gbs", 6650.0) / 2.0, 1),
-                    "denominator": "MEASURED_PEAKS.json hbm_gbs / 2 (every payload byte is read once and written once)"}
+            roof = {"per_gpu_GBps": round(per_gpu, 1), "denominator_GBps": round(HBM_NOMINAL_GBPS / 2.0, 1),
+                    "denominator": "HBM3 nominal / 2 (every payload byte is read once and written once)"}
             roof["fraction"] = round(per_gpu / roof["denominator_GBps"], 3)
         else:
             measured = comparators.get("cudaMemcpyPeerAsync_single_copy_GBps_per_rank")
             roof = {"per_gpu_GBps": round(per_gpu, 1), "denominator_GBps": NVLINK_NOMINAL_GBPS,
-                    "denominator": "NVLink 5 nominal, per direction per GPU (BASELINE.json)",
+                    "denominator": "NVLink 4 nominal, per direction per GPU",
                     "fraction": round(per_gpu / NVLINK_NOMINAL_GBPS, 3),
                     "measured_peer_copy_peak_GBps": measured,
                     "fraction_of_measured_peer_copy_peak": round(per_gpu / measured, 3) if measured else None,
                     "note": "every payload byte crosses NVLink once per put and once per get; a rank's egress carries its own puts and its neighbour's "
-                            "gets.  SM-issued traffic moves in 128-byte packets: pushes top out at ~714 GB/s and bidirectional pulls at ~672 GB/s on "
-                            "this fabric whatever the kernel (profiles/r2_nvlink/), copy engines reach ~775 GB/s with larger packets"}
+                            "gets"}
         line = {
             "metric": "batched put+get payload throughput (GB/s), %g MiB random-byte objects, GPU tier, %s fused" % (
                 args.object_mib, {"xxh3": "XXH3-64 (per 16 KiB tile) digest", "crc32c": "CRC32C digest", "bbh64": "BBH64 digest", "none": "no digest"}[args.algo]),
@@ -422,7 +424,7 @@ def run_headline(args, world: int) -> int:
                 "placement": "writer's ring neighbour (all payload crosses NVLink)" if world > 1 else "local HBM slab",
                 "checksum": args.algo,
                 "rank_sync": (args.sync + " (shared-memory rendezvous, host side)") if world > 1 else "n/a",
-                "l2_policy": "per-step payload %.2f GiB per rank >> 126 MB L2 (inputs larger than L2)" % (step_bytes / 2**30),
+                "l2_policy": "per-step payload %.2f GiB per rank >> 50 MB L2 (inputs larger than L2)" % (step_bytes / 2**30),
                 "control_plane_in_timed_region": "batch_put_start + batch_put_complete + batch_get_workers + batch_remove RPCs every step",
             },
             "kernel_only": kernel_only,
@@ -450,6 +452,36 @@ def run_headline(args, world: int) -> int:
         }
         print(json.dumps(line))
     return 0
+
+
+def dump_headline_outputs(out_dir: str, cl, rank: int, out, got_sizes, keys, idle: bool) -> None:
+    """Writes what the last timed step handed back, as float arrays a second build's run can be compared with:
+    payload_sample (uint8 values of 4 Mi bytes of the get destination per job at fixed, seeded positions), payload_sample_index
+    (those positions), get_sizes (the sizes batch_get_device returned) and put_digests (the digest the Keystone recorded
+    for every object, split into its high and low 32 bits so that float64 holds them exactly).  Then removes the objects."""
+    import numpy as np
+    import torch
+
+    from blackbird_b200 import _bb
+
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = f"_rank{rank}" if cl.world > 1 else ""
+    arrays = {}
+    if not idle:
+        n = out.numel()
+        idx = np.sort(np.random.default_rng(1234).integers(0, n, size=min(n, (4 << 20) // cl.world), dtype=np.int64))
+        sample = out[torch.from_numpy(idx).to(out.device)].cpu().numpy()
+        digests = [cl.client.get_workers(k)[0].shards[0].checksum for k in keys]
+        assert all(e == _bb.ErrorCode.OK for e in cl.client.batch_remove(keys))
+        arrays = {
+            "payload_sample": sample.astype(np.float32),
+            "payload_sample_index": idx.astype(np.float64),
+            "get_sizes": np.asarray(got_sizes, dtype=np.float64),
+            "put_digests": np.asarray([[d >> 32, d & 0xFFFFFFFF] for d in digests], dtype=np.float64),
+        }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), a)
+    assert sum(a.nbytes for a in arrays.values()) * cl.world <= 64 << 20
 
 
 # ====================================================================================================== other configs

@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
 """First-contact GPU diagnostics for the fused transfer kernel.
 
-phase=probe : impulse probes through the tcgen05 int8 MMA (dumps raw TMEM accumulators and
+phase=probe : impulse probes through the wgmma int8 MMA (dumps the raw accumulators and
               derives which (row, k) the hardware assigns to each tile-linear byte offset),
               then digest / copy correctness against the CPU BBH64 model.
 phase=perf  : single-GPU bandwidth of the fused kernel vs copy-only, SIMT copy, cudaMemcpy.
-Run under gpurun; prints to stdout (redirect into gpurun_out/).
+Prints to stdout.
 """
 import argparse
 import sys
@@ -192,7 +192,7 @@ def phase_perf():
     _bb.random_fill(src.data_ptr(), total, 7, stream())
     dst = torch.empty(total, dtype=torch.uint8, device=dev)
     items = [(src.data_ptr() + i * osz, dst.data_ptr() + i * osz, osz) for i in range(nobj)]
-    for ctas in (16, 32, 64, 96, 128, 148):
+    for ctas in (16, 32, 64, 96, 128, 132):
         eng.set_max_ctas(ctas)
         kms = []
         for _ in range(4):

@@ -7,7 +7,6 @@
 //
 //   methods : memcpy      cudaMemcpyPeerAsync (copy engines)
 //             stg         SIMT kernel, local LDG.128 -> peer STG.128 (push)
-//             stg256      same with 256-bit stores (st.global.v8.b32)
 //             ldg         SIMT kernel, peer LDG.128 -> local STG.128 (pull)
 //             bulk_push   TMA ring: cp.async.bulk local -> smem -> cp.async.bulk peer   (what bb_xfer's put does)
 //             bulk_pull   TMA ring: cp.async.bulk peer -> smem -> cp.async.bulk local   (what bb_xfer's get does)
@@ -108,19 +107,6 @@ __global__ void __launch_bounds__(512) k_copy_v4(const uint4* __restrict__ src, 
     for (int u = 0; u < UNROLL; ++u) __stcs(dst + i + u * stride, v[u]);
   }
   for (; i < n16; i += stride) dst[i] = src[i];
-}
-
-__global__ void __launch_bounds__(512) k_copy_v8(const uint4* __restrict__ src, uint4* __restrict__ dst, uint64_t n32) {
-  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * blockDim.x;
-  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n32; i += stride) {
-    uint32_t a, b, c, d, e, f, g, h;
-    asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a), "=r"(b), "=r"(c), "=r"(d), "=r"(e), "=r"(f), "=r"(g), "=r"(h)
-                 : "l"(src + 2 * i));
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst + 2 * i), "r"(a), "r"(b), "r"(c), "r"(d), "r"(e),
-                 "r"(f), "r"(g), "r"(h)
-                 : "memory");
-  }
 }
 
 __global__ void __launch_bounds__(512) k_mc_simt(const uint4* __restrict__ src, uint4* mc, uint64_t n16) {
@@ -475,8 +461,8 @@ int main(int argc, char** argv) {
     report("memcpy", pt.name, "cudaMemcpyPeerAsync",
            run(pt, [&](const Dev& me, const Dev& peer) { CK(cudaMemcpyPeerAsync(peer.dst, peer.id, me.src, me.id, bytes, me.st)); }), bytes,
            o.iters);
-    for (int ctas : {148, 296, 592}) {
-      if (o.quick && ctas != 296) continue;
+    for (int ctas : {132, 264, 528}) {
+      if (o.quick && ctas != 264) continue;
       char cfg[64];
       std::snprintf(cfg, sizeof cfg, "ctas=%d x512 unroll4", ctas);
       report("stg", pt.name, cfg, run(pt, [&](const Dev& me, const Dev& peer) {
@@ -486,22 +472,19 @@ int main(int argc, char** argv) {
                k_copy_v4<4><<<ctas, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(peer.src), reinterpret_cast<uint4*>(me.dst), bytes / 16);
              }), bytes, o.iters);
     }
-    report("stg", pt.name, "ctas=296 x512 unroll8", run(pt, [&](const Dev& me, const Dev& peer) {
-             k_copy_v4<8><<<296, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(me.src), reinterpret_cast<uint4*>(peer.dst), bytes / 16);
+    report("stg", pt.name, "ctas=264 x512 unroll8", run(pt, [&](const Dev& me, const Dev& peer) {
+             k_copy_v4<8><<<264, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(me.src), reinterpret_cast<uint4*>(peer.dst), bytes / 16);
            }), bytes, o.iters);
-    report("ldg", pt.name, "ctas=296 x512 unroll8", run(pt, [&](const Dev& me, const Dev& peer) {
-             k_copy_v4<8><<<296, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(peer.src), reinterpret_cast<uint4*>(me.dst), bytes / 16);
-           }), bytes, o.iters);
-    report("stg256", pt.name, "ctas=296 x512", run(pt, [&](const Dev& me, const Dev& peer) {
-             k_copy_v8<<<296, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(me.src), reinterpret_cast<uint4*>(peer.dst), bytes / 32);
+    report("ldg", pt.name, "ctas=264 x512 unroll8", run(pt, [&](const Dev& me, const Dev& peer) {
+             k_copy_v4<8><<<264, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(peer.src), reinterpret_cast<uint4*>(me.dst), bytes / 16);
            }), bytes, o.iters);
     struct RC {
       int ctas;
       uint32_t tile, stages, lag, inter;
     };
-    std::vector<RC> rcs = {{128, 16384, 8, 2, 0},  {128, 16384, 12, 6, 0}, {148, 16384, 12, 6, 0}, {128, 32768, 6, 3, 0},
-                           {148, 32768, 6, 3, 0},  {128, 65536, 3, 1, 0},  {64, 32768, 6, 3, 0},   {128, 16384, 12, 6, 1},
-                           {128, 8192, 24, 6, 0},  {96, 32768, 6, 3, 0},   {148, 65536, 3, 1, 0},  {128, 32768, 6, 3, 1}};
+    std::vector<RC> rcs = {{128, 16384, 8, 2, 0},  {128, 16384, 12, 6, 0}, {132, 16384, 12, 6, 0}, {128, 32768, 6, 3, 0},
+                           {132, 32768, 6, 3, 0},  {128, 65536, 3, 1, 0},  {64, 32768, 6, 3, 0},   {128, 16384, 12, 6, 1},
+                           {128, 8192, 24, 6, 0},  {96, 32768, 6, 3, 0},   {132, 65536, 3, 1, 0},  {128, 32768, 6, 3, 1}};
     if (o.quick) rcs.resize(4);
     for (const RC& rc : rcs) {
       char cfg[96];
@@ -542,7 +525,7 @@ int main(int argc, char** argv) {
       for (int d = 0; d < g; ++d) all.active.push_back(d);
       for (const Pattern* pt : {&one, &all}) {
         char cfg[96];
-        for (int ctas : {148, 296}) {
+        for (int ctas : {132, 264}) {
           std::snprintf(cfg, sizeof cfg, "group=%d ctas=%d x512", g, ctas);
           report("mc_simt", pt->name, cfg, run(*pt, [&](const Dev& me, const Dev&) {
                    k_mc_simt<<<ctas, 512, 0, me.st>>>(reinterpret_cast<const uint4*>(me.src), reinterpret_cast<uint4*>(m.mc_va), bytes / 16);
@@ -557,7 +540,7 @@ int main(int argc, char** argv) {
       }
       // verify: every member sees device 0's pattern after a 1-writer broadcast
       CK(cudaSetDevice(0));
-      k_mc_simt<<<296, 512, 0, dv[0].st>>>(reinterpret_cast<const uint4*>(dv[0].src), reinterpret_cast<uint4*>(m.mc_va), bytes / 16);
+      k_mc_simt<<<264, 512, 0, dv[0].st>>>(reinterpret_cast<const uint4*>(dv[0].src), reinterpret_cast<uint4*>(m.mc_va), bytes / 16);
       CK(cudaStreamSynchronize(dv[0].st));
       bool ok = true;
       for (int d = 0; d < g; ++d) {

@@ -1,9 +1,9 @@
-"""blackbird_b200 — a Blackwell-native tiered distributed object store.
+"""blackbird_b200 — a Hopper-native tiered distributed object store.
 
 Capabilities and API of blackbird-io/blackbird (Keystone control plane, striped + replicated
 placement, TTL / soft-pin eviction, worker tiers, client SDK) with a data plane written for
-one 8xB200 NVSwitch box: batched put/get run as hand-written sm_100a kernels that fuse the
-NVLink transfer with a tensor-core checksum (TMA -> smem -> tcgen05.mma/TMEM -> TMA).
+one 8xH100 NVSwitch box: batched put/get run as hand-written sm_90a kernels that fuse the
+NVLink transfer with a tensor-core checksum (TMA -> smem -> wgmma -> TMA).
 """
 from . import _bb  # noqa: F401  (native core; must be built in-tree: python build.py)
 from ._bb import ChecksumAlgo, ErrorCode  # noqa: F401

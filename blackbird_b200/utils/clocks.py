@@ -1,4 +1,4 @@
-"""GPU clock / throttle sampler for benchmark hygiene (B200_PROFILING.md: clocks line)."""
+"""GPU clock / throttle sampler for benchmark hygiene: a benchmark reports the clocks its numbers were taken at."""
 from __future__ import annotations
 
 import statistics

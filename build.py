@@ -2,10 +2,10 @@
 """In-tree native build for blackbird_b200.
 
 Generates build/build.ninja and runs ninja.  Produces
-  blackbird_b200/_bb<EXT_SUFFIX>   single pybind11 module: C++20 control plane + sm_100a data plane
+  blackbird_b200/_bb<EXT_SUFFIX>   single pybind11 module: C++20 control plane + sm_90a data plane
   bin/bb-keystone bin/bb-worker bin/bb-coord bin/bb-cli bin/bb-bench bin/bb-tests
 
-All CUDA is compiled for sm_100a only (`-gencode arch=compute_100a,code=sm_100a -lineinfo`);
+All CUDA is compiled for sm_90a only (`-gencode arch=compute_90a,code=sm_90a -lineinfo`);
 nvcc cross-compiles without a GPU.  cudart is linked statically and the driver API is
 resolved at runtime, so the module imports on a CPU-only box.
 """
@@ -31,7 +31,7 @@ NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")
 
 CXXFLAGS = "-std=c++20 -O2 -g1 -fPIC -Wall -Wextra -Wno-unused-parameter -Wno-missing-field-initializers -pthread"
 NVCCFLAGS = (
-    "-std=c++20 -O3 -lineinfo -gencode arch=compute_100a,code=sm_100a "
+    "-std=c++20 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a "
     "-Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v --expt-relaxed-constexpr -Wno-deprecated-gpu-targets"
 )
 

@@ -1,12 +1,12 @@
-// BBH64 ("tensor-core hash") — definition shared by the CPU reference and the sm_100a kernels.
+// BBH64 ("tensor-core hash") — definition shared by the CPU reference and the sm_90a kernels.
 //
 // The reference computes no checksum at all (error_codes.h:62-63 defines CHECKSUM_MISMATCH /
 // DATA_CORRUPTION but nothing produces them, SURVEY K11).  BBH64 is the checksum designed for
-// the Blackwell data plane: the 16 KiB tile that TMA lands in shared memory is consumed
-// *in place* as the A operand of `tcgen05.mma.kind::i8` (u8 x u8 -> s32 in TMEM) against a fixed
-// pseudo-random weight matrix, so hashing costs no register traffic and overlaps the copy.
+// the GPU data plane: the 16 KiB tile that TMA lands in shared memory is consumed *in place* as
+// the A operand of `wgmma.mma_async...s32.u8.u8` (u8 x u8 -> s32) against a fixed pseudo-random
+// weight matrix, so the payload bytes never pass through registers and hashing overlaps the copy.
 //
-//   tile   = 16384 bytes, viewed as A[128 rows][128 k] in the UMMA K-major no-swizzle
+//   tile   = 16384 bytes, viewed as A[128 rows][128 k] in the wgmma K-major no-swizzle
 //            canonical layout: linear offset o -> row m = (o/1024)*8 + (o%128)/16,
 //                                                k     = ((o%1024)/128)*16 + o%16
 //            (8-row x 16-byte core matrices; LBO = 128 B between K chunks, SBO = 1024 B
@@ -29,9 +29,9 @@
 namespace bb::tchash {
 
 constexpr uint32_t kTileBytes = 16384;
-constexpr uint32_t kRows = 128;   // UMMA M
+constexpr uint32_t kRows = 128;   // tile rows (two wgmma M=64 halves)
 constexpr uint32_t kK = 128;      // bytes per row (4 MMAs of K=32)
-constexpr uint32_t kN = 16;       // UMMA N (hash columns)
+constexpr uint32_t kN = 16;       // wgmma N (hash columns)
 constexpr uint64_t kGold = 0x9E3779B97F4A7C15ull;
 constexpr uint64_t kLenMul = 0xD6E8FEB86659FD93ull;
 

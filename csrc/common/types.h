@@ -4,7 +4,7 @@
 // placement model UcxEndpoint/MemoryLocation/FileLocation/CxlMemoryLocation/LocationDetail/
 // ShardPlacement/CopyPlacement (:97-156), WorkerConfig (:161-187), ClusterStats (:192-209),
 // KeystoneConfig (:410-444), ClientConfig (:449-459), MemoryPool (:464-493), hash<UUID> (:499-512).
-// B200-native additions: GpuSlabLocation (rank/slab/offset addressing of an exported HBM
+// GPU-native additions: GpuSlabLocation (rank/slab/offset addressing of an exported HBM
 // slab — the role the (remote_addr, rkey) pair plays for UCX), per-shard checksum, checksum /
 // fp8-pack / NVLS policy knobs, pool topology attributes that the placement engine consumes.
 #pragma once
@@ -131,7 +131,7 @@ struct WorkerConfig {
   bool enable_locality_awareness = true;
   bool prefer_contiguous = false;
   size_t min_shard_size = 4096;
-  // --- B200-native extensions
+  // --- GPU-native extensions
   ChecksumAlgo checksum = ChecksumAlgo::BBH64;
   bool pack_fp8 = false;          // store bf16 payload as block-scaled MXFP8 (E4M3 + E8M0/32)
   bool symmetric_replicas = false;  // same slab offset on every replica (NVLS multicast fan-out)

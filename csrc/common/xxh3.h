@@ -3,7 +3,7 @@
 // BASELINE.json / SURVEY K11 name "CRC32/xxhash" as the checksums to fuse into put / get; the reference only declares the
 // error codes (include/blackbird/common/error/error_codes.h:62-63) and computes nothing.  XXH3-64 (Yann Collet's xxHash
 // 0.8 specification, default secret, seed 0) over a whole object is a serial recurrence (the 8-lane accumulator is
-// scrambled after every 1 KiB block), so it cannot be evaluated tile-parallel by 148 SMs whose tiles finish in any order.
+// scrambled after every 1 KiB block), so it cannot be evaluated tile-parallel by 132 SMs whose tiles finish in any order.
 // The object digest therefore is
 //
 //   digest = mix64( ( sum over tiles t of  mix64( XXH3_64(tile_t) + (t + 1) * GOLD ) )  ^  nbytes * LENMUL )

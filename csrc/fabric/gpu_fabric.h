@@ -1,4 +1,4 @@
-// GPU fabric: the B200-native replacement of the reference's UcxEngine (SURVEY C11, §2.5).
+// GPU fabric: the GPU-native replacement of the reference's UcxEngine (SURVEY C11, §2.5).
 //
 //   reference (src/transport/ucx_engine.cpp)            here
 //   ucp_mem_map + ucp_rkey_pack of a malloc'd pool  ->  cudaMalloc'd HBM slab + cudaIpcGetMemHandle

@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(1024) crc_combine_kernel(uint32_t* arr, uint64
 bool g_crc_table_init[16] = {false};
 
 int grid_for(uint64_t work_items, int threads, int per_sm) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   uint64_t need = (work_items + threads - 1) / threads;

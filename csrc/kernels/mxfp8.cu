@@ -1,4 +1,4 @@
-// MXFP8 pack / unpack kernels (sm_100a): bf16 <-> [E4M3 payload | E8M0 block scales].
+// MXFP8 pack / unpack kernels (sm_90a): bf16 <-> [E4M3 payload | E8M0 block scales].
 // Memory-bound streaming kernels: one 16-byte load (8 bf16) per thread, 4 lanes share a 32-element
 // block (amax via two xor-shuffles), 8-byte payload store per thread.  Destination / source may be
 // peer-mapped slab memory, so the pack can write straight across NVLink.
@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(256) mxfp8_unpack_kernel(const uint2* __restri
 }
 
 int grid_for(uint64_t threads_needed) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const uint64_t blocks = (threads_needed + 255) / 256;

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the data plane uses:
-// mbarrier, TMA bulk copies (cp.async.bulk), tcgen05 (alloc / mma.kind::i8 / commit / ld),
+// Thin inline-PTX wrappers for the sm_90a features the data plane uses:
+// mbarrier, TMA bulk copies (cp.async.bulk), wgmma (u8 x u8 -> s32 warpgroup MMA from shared memory),
 // proxy fences, multimem stores, and cache-hinted vector loads/stores.
 #pragma once
 #include <cstdint>
@@ -85,63 +85,37 @@ __device__ __forceinline__ void bulk_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// Issued by all 128 threads of one warpgroup (4 consecutive warps, the first warp index a multiple of 4); the
+// accumulators live in the issuing threads' registers.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], 8-bit integer inputs, s32 accumulate.
-__device__ __forceinline__ void mma_i8_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64x16] (+)= A[64x32 smem desc] * B[32x16 smem desc]^T, u8 x u8 inputs, s32 accumulate.  Thread t of the warpgroup
+// holds d[i] = D[row][col], row = 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2), col = 2 (t % 4) + i % 2 + 8 (i / 4).
+__device__ __forceinline__ void wgmma_m64n16k32_u8(uint32_t (&d)[8], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u)
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-// mbarrier arrive when all prior tcgen05 async ops of this thread have completed.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 TMEM lanes (this warp's quadrant) x 16 consecutive 32-bit columns -> 16 registers per thread.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"): 8-row x 16-byte
-// core matrices; `lbo` = byte distance between the two 16-byte K chunks of one MMA,
-// `sbo` = byte distance between consecutive 8-row groups.  version=1 (sm_100).
-__device__ __forceinline__ uint64_t umma_desc_kmajor_noswizzle(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+// wgmma shared-memory matrix descriptor, K-major, no swizzle (interleave): 8-row x 16-byte core matrices;
+// `lbo` = byte distance between the two 16-byte K chunks of one MMA, `sbo` = byte distance between consecutive
+// 8-row groups.  Layout type 0 (bits 62-63) = no swizzle, base offset 0.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_noswizzle(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
   return d;
-}
-// kind::i8 instruction descriptor: D=s32, A=u8, B=u8, both K-major, dense.
-__host__ __device__ constexpr uint32_t umma_idesc_i8(uint32_t m, uint32_t n, bool a_signed, bool b_signed) {
-  return (2u << 4) | ((a_signed ? 1u : 0u) << 7) | ((b_signed ? 1u : 0u) << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
 }
 
 // ---------------------------------------------------------------- global memory helpers

@@ -1,4 +1,4 @@
-// Host-visible API of the sm_100a data-plane kernels (plain C++; no CUDA types leak out).
+// Host-visible API of the sm_90a data-plane kernels (plain C++; no CUDA types leak out).
 //
 // These kernels replace the reference's UCX call sites (SURVEY K1-K7): `ucp_put_nbx`
 // (blackbird_client.cpp:231-237), `ucp_get_nbx` (:315-327) and the CPU byte compare

@@ -1,4 +1,4 @@
-// bb_xfer: the fused batched put/get kernel (sm_100a).
+// bb_xfer: the fused batched put/get kernel (sm_90a).
 //
 // Replaces the reference's per-shard UCX RMA calls (blackbird_client.cpp:231-237 put,
 // :315-327 get; SURVEY K1/K4/K6/K11/K13) with ONE persistent launch per batch.  Every CTA owns
@@ -7,9 +7,6 @@
 //   warp 0  producer : descriptor lookup (32 tiles looked up in parallel), zero-pads short
 //                      tiles, `cp.async.bulk` global -> shared (TMA, mbarrier complete_tx).
 //                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).
-//   warp 1  hash     : BBH64: one elected thread issues 4x `tcgen05.mma.kind::i8` (M128 N16 K32)
-//                      that read the landed tile *in place* as the A operand against the BBH64
-//                      weight matrix; accumulators live in TMEM (16 columns per stage).
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
 //                      to an NVLS multicast address (one store, N replicas).
@@ -17,8 +14,10 @@
 //                      object that lives entirely inside this CTA's run is finalised with no
 //                      global atomics; only the <=2 objects straddling a CTA boundary use them.
 //                      Compares with the expected digest on get (CHECKSUM_MISMATCH source).
-//   warps 4-7 epilogue: BBH64: `tcgen05.ld` the 128x16 s32 accumulators -> position-dependent
-//                      64-bit row hashes -> warp sum.  CRC32C: each warp streams its 4 KiB quarter of
+//   warps 4-7 epilogue: BBH64: the warpgroup issues 2x4 `wgmma.mma_async.m64n16k32.s32.u8.u8` that
+//                      read the landed tile *in place* as the A operand against the BBH64 weight
+//                      matrix (bbh_tile.cuh); the 128x16 s32 accumulators land in registers ->
+//                      position-dependent 64-bit row hashes -> warp sum.  CRC32C: each warp streams its 4 KiB quarter of
 //                      the tile as 8 Horner chains per lane through lane-private nibble shift tables
 //                      (bank-conflict free); the chains run on across the tiles of an object and are
 //                      combined (chain / lane / quarter, GF(2) shift algebra) once per object and CTA.
@@ -38,6 +37,7 @@
 #include "common/checksum.h"
 #include "common/tchash_def.h"
 #include "common/xxh3.h"
+#include "kernels/bbh_tile.cuh"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
 
@@ -49,8 +49,6 @@ using namespace bb::ptx;
 constexpr int kStages = 8;
 constexpr int kThreads = 256;
 constexpr int kStoreLag = 2;         // stores may trail this many tiles before their stage is released
-constexpr uint32_t kTmemCols = 128;  // kStages * 16 accumulator columns
-static_assert(kStages * tchash::kN == kTmemCols);
 static_assert(kTileBytes == tchash::kTileBytes);
 
 __constant__ uint64_t c_col_mul[tchash::kN];
@@ -88,14 +86,12 @@ struct __align__(1024) SmemT {
   uint8_t tile[kStages][kTileBytes];
   uint8_t w[2048];
   uint64_t full[kStages];
-  uint64_t acc_full[kStages];
   uint64_t epi_done[kStages];
   uint64_t empty[kStages];
   StageMeta meta[kStages];
   uint64_t part[kStages][4];
   LookupEntry lk[32];
   uint32_t dirty[kStages];
-  uint32_t tmem_base;
   uint32_t crc_t[ALGO == ALGO_CRC32C ? kNumCrcTabs : 1][4][256];
   // x^(8*128) shift as 8 nibble tables with one private copy per lane ([nibble][value][lane]: lane l only ever
   // touches bank l, so the 8 lookups of a step are bank-conflict free whatever the data is).
@@ -139,16 +135,6 @@ __device__ __forceinline__ uint64_t shfl_u64(uint64_t v, int src) {
   const uint32_t lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v), src);
   const uint32_t hi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), src);
   return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-
-__device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), o);
-    uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), o);
-    v += (static_cast<uint64_t>(hi) << 32) | lo;
-  }
-  return v;
 }
 
 // s * x^(8k) mod P through the 4x256 table of distance k.
@@ -215,7 +201,6 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&s.full[i], 1);
-      mbar_init(&s.acc_full[i], 1);
       mbar_init(&s.epi_done[i], 4);
       mbar_init(&s.empty[i], kHash ? 2 : 1);  // store warp (+ finalizer)
       s.dirty[i] = kTileBytes;
@@ -223,12 +208,10 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     fence_mbar_init();
   }
   if constexpr (kBbh) {
-    // BBH64 weight matrix W[k][n] as the UMMA B operand (N=16 rows, K-major, no swizzle).
+    // BBH64 weight matrix W[k][n] as the wgmma B operand (N=16 rows, K-major, no swizzle).
     for (uint32_t o = threadIdx.x; o < 2048; o += kThreads)
       s.w[o] = static_cast<uint8_t>(tchash::weight(tchash::off_to_k(o), tchash::off_to_row(o)));
     fence_proxy_async_smem();
-    if (warp == 3) tmem_alloc<kTmemCols>(&s.tmem_base);
-    tc_fence_before();
   }
   if constexpr (kCrc) {
     uint32_t* dstt = &s.crc_t[0][0][0];
@@ -251,8 +234,6 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     }
   }
   __syncthreads();
-  if constexpr (kBbh) tc_fence_after();
-  const uint32_t tmem_base = kBbh ? s.tmem_base : 0;
 
   if (warp == 0) {
     // ================================================================ TMA producer
@@ -338,29 +319,7 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
       __syncwarp();
     }
   } else if (warp == 1) {
-    // ================================================================ tensor-core hash issuer
-    if constexpr (kBbh) {
-      constexpr uint32_t idesc = umma_idesc_i8(tchash::kRows, tchash::kN, false, false);
-      const uint32_t w_addr = smem_u32(s.w);
-      for (uint32_t it = 0; it < my_tiles; ++it) {
-        const uint32_t stage = it % kStages;
-        const uint32_t par = (it / kStages) & 1u;
-        mbar_wait(&s.full[stage], par);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t a_addr = smem_u32(s.tile[stage]);
-          const uint32_t tmem_d = tmem_base + stage * tchash::kN;
-#pragma unroll
-          for (uint32_t j = 0; j < tchash::kK / 32; ++j) {
-            // each MMA consumes K=32 bytes = two 16-byte K chunks (LBO 128 B apart)
-            mma_i8_ss(tmem_d, umma_desc_kmajor_noswizzle(a_addr + j * 256, 128, 1024),
-                      umma_desc_kmajor_noswizzle(w_addr + j * 256, 128, 1024), idesc, j > 0 ? 1u : 0u);
-          }
-          tc_commit(&s.acc_full[stage]);
-        }
-        __syncwarp();
-      }
-    }
+    // idle: the BBH64 tensor-core product is issued by the epilogue warpgroup that consumes it
   } else if (warp == 2) {
     // ================================================================ store warp
     for (uint32_t it = 0; it < my_tiles; ++it) {
@@ -519,31 +478,26 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     // ================================================================ epilogue warps 4..7
     if constexpr (kBbh) {
       const uint32_t q = warp & 3u;
-      const uint32_t row = q * 32 + lane;
+      const uint32_t w_addr = smem_u32(s.w);
       for (uint32_t it = 0; it < my_tiles; ++it) {
         const uint32_t stage = it % kStages;
         const uint32_t par = (it / kStages) & 1u;
-        mbar_wait(&s.acc_full[stage], par);
-        mbar_wait(&s.full[stage], par);  // already complete; acquires the producer's StageMeta writes
-        tc_fence_after();
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(tmem_base + ((q * 32u) << 16) + stage * tchash::kN, r);
-        tmem_ld_wait();
-        tc_fence_before();
+        mbar_wait(&s.full[stage], par);  // tile landed (TMA + the producer's fenced zero padding) and its StageMeta
+        uint32_t d[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) d[k] = 0;
+        bbh_tile_mma(smem_u32(s.tile[stage]), w_addr, d);
         // position of this tile in the hashed object (a RAW_SUM slice starts at a non-zero tile index)
         const uint32_t ti = s.meta[stage].tile_in_obj + (((s.meta[stage].ndst_flags >> 8) & XFER_RAW_SUM) ? s.meta[stage].crc_unpad : 0u);
-        uint64_t rr = 0;
-#pragma unroll
-        for (int n = 0; n < 16; ++n) rr += static_cast<uint64_t>(r[n]) * c_col_mul[n];
-        const uint64_t tot = warp_sum64(tchash::row_contrib(rr, static_cast<uint64_t>(ti) * tchash::kRows + row));
+        const uint64_t tot = bbh_tile_rows(d, c_col_mul, ti, q, lane);
         if (lane == 0) {
           s.part[stage][q] = tot;
           mbar_arrive(&s.epi_done[stage]);
         }
         if (p.debug_d) {
-          uint32_t* o = p.debug_d + (static_cast<uint64_t>(t0 + it) * tchash::kRows + row) * tchash::kN;
+          uint32_t* o = p.debug_d + static_cast<uint64_t>(t0 + it) * tchash::kRows * tchash::kN;
 #pragma unroll
-          for (int n = 0; n < 16; ++n) o[n] = r[n];
+          for (uint32_t k = 0; k < 16; ++k) o[bbh_acc_row(k, q, lane) * tchash::kN + bbh_acc_col(k, lane)] = d[k];
         }
       }
     } else if constexpr (kXxh) {
@@ -631,15 +585,6 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     }
   }
 
-  // ------------------------------------------------------------------ teardown
-  if constexpr (kBbh) tc_fence_before();
-  __syncthreads();
-  if constexpr (kBbh) {
-    if (warp == 3) {
-      tc_fence_after();
-      tmem_dealloc<kTmemCols>(tmem_base);
-    }
-  }
 }
 
 struct DeviceState {
@@ -742,7 +687,7 @@ int launch_xfer(const XferLaunch& l) {
       e = cudaMemcpyToSymbol(c_xxh_secret, xxh3::kSecret, sizeof xxh3::kSecret);
       if (e != cudaSuccess) return static_cast<int>(e);
       int n = 0;
-      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
       ds.sm_count = n;
       ds.consts = true;
     }
@@ -777,8 +722,7 @@ int launch_xfer(const XferLaunch& l) {
   p.crc_tables = ds.crc_tables;
   p.debug_d = l.debug_d;
   p.trace_d = reinterpret_cast<unsigned long long*>(l.trace_d);
-  // Measured on B200 (profiles/xfer_single_gpu.md): 96-128 persistent CTAs saturate HBM for
-  // large batches (3.2 TB/s payload); all 148 lose ~6% to DRAM contention.  BB_XFER_CTAS overrides.
+  // At most 128 persistent CTAs (one per SM, 1 CTA/SM by shared memory) for the DRAM-bound digests; BB_XFER_CTAS overrides.
   static const int env_ctas = [] { const char* e = std::getenv("BB_XFER_CTAS"); return e ? std::atoi(e) : 0; }();
   // The fused CRC32C is bound by shared-memory lookups per SM, not by DRAM: it takes every SM.
   int grid = l.max_ctas > 0 ? l.max_ctas : env_ctas > 0 ? env_ctas : l.algo == ALGO_CRC32C ? ds.sm_count : std::min(ds.sm_count, 128);

@@ -1,7 +1,7 @@
-// bb_xfer_fp8: fused MXFP8 transfer kernels (sm_100a; SURVEY K12 "fp8 pack fused into put / unpack into get").
+// bb_xfer_fp8: fused MXFP8 transfer kernels (sm_90a; SURVEY K12 "fp8 pack fused into put / unpack into get").
 //
 //   put  (PACK)   : TMA loads a 32 KiB bf16 tile -> 8 pack warps compute the E8M0 block scales and the E4M3
-//                   payload *in shared memory* -> the 16 KiB payload tile is hashed in place by tcgen05.mma
+//                   payload *in shared memory* -> the 16 KiB payload tile is hashed in place by wgmma
 //                   (BBH64, same tile hash as bb_xfer) -> TMA stores payload + 512 B of scales to the
 //                   (peer) slab -- to up to 3 replicas of the object from the one converted tile.  The bf16 data
 //                   is read from HBM once and only the 0.52x packed bytes cross NVLink (once per replica).
@@ -16,8 +16,8 @@
 // here -- in the packed object its hash tile also contains the first scale bytes, so the slice the host hashes simply
 // starts at the last whole payload tile.
 //
-// Warp roles (24 warps): 0 producer, 1 MMA issuer, 2 store, 3 accumulator, 4-7 epilogue (TMEM -> row hashes),
-// 8-23 convert (pack / unpack).  Two shared-memory rings: 3 x 32 KiB bf16 tiles and 6 x (16 KiB payload + 512 B scales).
+// Warp roles (24 warps): 0 producer, 1 idle, 2 store, 3 accumulator, 4-7 epilogue (the warpgroup issues the wgmma
+// tile product, bbh_tile.cuh, and turns its register accumulators into row hashes), 8-23 convert (pack / unpack).  Two shared-memory rings: 3 x 32 KiB bf16 tiles and 6 x (16 KiB payload + 512 B scales).
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
 #include <cuda_runtime.h>
@@ -26,6 +26,7 @@
 #include <mutex>
 
 #include "common/tchash_def.h"
+#include "kernels/bbh_tile.cuh"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
 
@@ -40,9 +41,7 @@ constexpr int kConvertWarps = 16;           // warps 8..23 (the pack side is ALU
 constexpr int kFpThreads = (8 + kConvertWarps) * 32;
 constexpr uint32_t kWideBytes = 2 * kTileBytes;  // bf16 side of one payload tile
 constexpr uint32_t kScaleBytes = kTileBytes / 32;
-constexpr uint32_t kFpTmemCols = 128;       // >= kTileStages * 16 accumulator columns (power of two)
 constexpr int kFpStoreLag = 1;
-static_assert(kTileStages * tchash::kN <= kFpTmemCols);
 
 __constant__ uint64_t c_fp_col_mul[tchash::kN];
 
@@ -77,13 +76,11 @@ struct __align__(1024) SmemFp {
   uint64_t t_empty[kTileStages];
   uint64_t w_full[kWideStages];   // wide tile ready (pack: TMA; unpack: convert warps)
   uint64_t w_empty[kWideStages];
-  uint64_t acc_full[kTileStages];
   uint64_t epi_done[kTileStages];
   FpMeta t_meta[kTileStages];
   FpMeta w_meta[kWideStages];
   uint64_t part[kTileStages][4];
   FpLookup lk[32];
-  uint32_t tmem_base;
 };
 
 struct FpParams {
@@ -93,16 +90,6 @@ struct FpParams {
   uint32_t total_tiles;
   unsigned long long* sum_ws;  // [ndesc] raw BBH64 sums of the payload tiles (zero on entry)
 };
-
-__device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), o);
-    uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), o);
-    v += (static_cast<uint64_t>(hi) << 32) | lo;
-  }
-  return v;
-}
 
 __device__ __forceinline__ __nv_bfloat162 as_bf162(uint32_t v) { return *reinterpret_cast<const __nv_bfloat162*>(&v); }
 
@@ -172,7 +159,6 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     for (int i = 0; i < kTileStages; ++i) {
       mbar_init(&s.t_full[i], UNPACK ? 1 : kConvertWarps);
       mbar_init(&s.t_empty[i], UNPACK ? kConvertWarps + 1 : 2);  // unpack: convert warps + accumulator; pack: store + accumulator
-      mbar_init(&s.acc_full[i], 1);
       mbar_init(&s.epi_done[i], 4);
     }
     for (int i = 0; i < kWideStages; ++i) {
@@ -184,11 +170,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
   for (uint32_t o = threadIdx.x; o < 2048; o += kFpThreads)
     s.w[o] = static_cast<uint8_t>(tchash::weight(tchash::off_to_k(o), tchash::off_to_row(o)));
   fence_proxy_async_smem();
-  if (warp == 3) tmem_alloc<kFpTmemCols>(&s.tmem_base);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s.tmem_base;
 
   if (warp == 0) {
     // ================================================================ TMA producer
@@ -269,24 +251,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
       __syncwarp();
     }
   } else if (warp == 1) {
-    // ================================================================ tensor-core hash issuer (payload tile)
-    constexpr uint32_t idesc = umma_idesc_i8(tchash::kRows, tchash::kN, false, false);
-    const uint32_t w_addr = smem_u32(s.w);
-    for (uint32_t it = 0; it < my_tiles; ++it) {
-      const uint32_t ts = it % kTileStages, tp = (it / kTileStages) & 1u;
-      mbar_wait(&s.t_full[ts], tp);  // pack: written by the convert warps (generic proxy, fenced); unpack: TMA
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t a_addr = smem_u32(s.tile[ts]);
-        const uint32_t tmem_d = tmem_base + ts * tchash::kN;
-#pragma unroll
-        for (uint32_t j = 0; j < tchash::kK / 32; ++j)
-          mma_i8_ss(tmem_d, umma_desc_kmajor_noswizzle(a_addr + j * 256, 128, 1024), umma_desc_kmajor_noswizzle(w_addr + j * 256, 128, 1024),
-                    idesc, j > 0 ? 1u : 0u);
-        tc_commit(&s.acc_full[ts]);
-      }
-      __syncwarp();
-    }
+    // idle: the tensor-core hash of the payload tile is issued by the epilogue warpgroup that consumes it
   } else if (warp == 2) {
     // ================================================================ store warp
     constexpr int kRing = UNPACK ? kWideStages : kTileStages;
@@ -352,23 +317,17 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     }
     if (cur_d != 0xFFFFFFFFu && lane == 0) atomicAdd(&p.sum_ws[cur_d], static_cast<unsigned long long>(acc));
   } else if (warp < 8) {
-    // ================================================================ epilogue warps 4..7: TMEM -> row hashes
+    // ================================================================ epilogue warpgroup 4..7: wgmma -> row hashes
     const uint32_t q = warp & 3u;
-    const uint32_t row = q * 32 + lane;
+    const uint32_t w_addr = smem_u32(s.w);
     for (uint32_t it = 0; it < my_tiles; ++it) {
       const uint32_t ts = it % kTileStages, tp = (it / kTileStages) & 1u;
-      mbar_wait(&s.acc_full[ts], tp);
-      mbar_wait(&s.t_full[ts], tp);  // (already complete) acquires the t_meta writes
-      tc_fence_after();
-      uint32_t r[16];
-      tmem_ld_32x32b_x16(tmem_base + ((q * 32u) << 16) + ts * tchash::kN, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      const uint32_t ti = s.t_meta[ts].tile_in_obj;
-      uint64_t rr = 0;
+      mbar_wait(&s.t_full[ts], tp);  // pack: written by the convert warps (generic proxy, fenced); unpack: TMA
+      uint32_t d[16];
 #pragma unroll
-      for (int n = 0; n < 16; ++n) rr += static_cast<uint64_t>(r[n]) * c_fp_col_mul[n];
-      const uint64_t tot = warp_sum64(tchash::row_contrib(rr, static_cast<uint64_t>(ti) * tchash::kRows + row));
+      for (int k = 0; k < 16; ++k) d[k] = 0;
+      bbh_tile_mma(smem_u32(s.tile[ts]), w_addr, d);
+      const uint64_t tot = bbh_tile_rows(d, c_fp_col_mul, s.t_meta[ts].tile_in_obj, q, lane);
       if (lane == 0) {
         s.part[ts][q] = tot;
         mbar_arrive(&s.epi_done[ts]);
@@ -419,13 +378,6 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     }
   }
 
-  // ------------------------------------------------------------------ teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 3) {
-    tc_fence_after();
-    tmem_dealloc<kFpTmemCols>(tmem_base);
-  }
 }
 
 struct FpDeviceState {
@@ -455,7 +407,7 @@ int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
       e = cudaMemcpyToSymbol(c_fp_col_mul, h, sizeof h);
       if (e != cudaSuccess) return static_cast<int>(e);
       int n = 0;
-      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
       ds.sm_count = n;
       ds.consts = true;
     }

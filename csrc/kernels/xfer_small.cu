@@ -1,8 +1,8 @@
 // bb_xfer_small: the small-object latency tier of the fused transfer (SURVEY K2, §7.4 #1).
 //
 // The reference's only end-to-end client moves a 64-byte object with one `ucp_put_nbx` + flush and one `ucp_get_nbx`
-// (clients/ucx_client.cpp:188-257).  For objects of <= 4 KiB the persistent TMA / tcgen05 pipeline of bb_xfer_kernel is
-// all set-up cost (mbarriers, TMEM allocation, weight matrix, tile padding: ~9.5 us for one 4 KiB object), so batches made
+// (clients/ucx_client.cpp:188-257).  For objects of <= 4 KiB the persistent TMA / wgmma pipeline of bb_xfer_kernel is
+// all set-up cost (mbarriers, weight matrix, tile padding), so batches made
 // of small objects only take this path instead: ONE WARP PER OBJECT, no shared-memory staging of the payload, no TMA.
 //
 //   lane l owns bytes [128 l, 128 l + 128) of the object: 8 x LDG.128 (local HBM, peer slab over NVLink, or pinned host)

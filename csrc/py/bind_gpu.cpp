@@ -1,4 +1,4 @@
-// Bindings for the sm_100a data plane: XferEngine (fused batched transfer), comparators and
+// Bindings for the sm_90a data plane: XferEngine (fused batched transfer), comparators and
 // device helpers.  Pointers cross the boundary as integers (tensor.data_ptr()), streams as
 // integers (torch.cuda.current_stream().cuda_stream).
 #include <pybind11/pybind11.h>

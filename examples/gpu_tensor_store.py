@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""GPU tier from torch (needs B200s): one process per GPU, `torchrun --nproc-per-node N examples/gpu_tensor_store.py`.
+"""GPU tier from torch (needs H100s): one process per GPU, `torchrun --nproc-per-node N examples/gpu_tensor_store.py`.
 Every rank puts activations on its ring neighbour, reads its neighbour's back, stores a KV block as MXFP8 (pack fused
 into the put kernel) and reads it back (unpack fused into the get kernel)."""
 import os

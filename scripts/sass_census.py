@@ -1,14 +1,14 @@
 #!/usr/bin/env python3
-"""SASS census of the built extension: per kernel, how many of each instruction class that matters here (tcgen05 = UTC*,
-LDTM / STTM; TMA bulk copies = UBLKCP; mbarrier = SYNCS; fences; shuffles; global loads / stores).
-  python scripts/sass_census.py [blackbird_b200/_bb*.so] > profiles/sass_census_r2.txt"""
+"""SASS census of the built extension: per kernel, how many of each instruction class that matters here (wgmma = IGMMA /
+HGMMA, WARPGROUP.*; TMA bulk copies = UBLKCP; mbarrier = SYNCS; fences; shuffles; global loads / stores).
+  python scripts/sass_census.py [blackbird_b200/_bb*.so] > profiles/sass_census.txt"""
 import collections
 import glob
 import re
 import subprocess
 import sys
 
-KEEP = ["UTCIMMA", "UTCHMMA", "UTCQMMA", "LDTM", "STTM", "UTCBAR", "UTCATOMSWS", "UTCCP", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "UTMACMDFLUSH",
+KEEP = ["IGMMA", "HGMMA", "WARPGROUP", "UBLKCP", "UTMALDG", "UTMASTG", "SYNCS", "UTMACMDFLUSH",
         "IMAD", "IDP", "SHFL", "LDS", "LDG", "STG", "ATOMG", "REDG", "MEMBAR", "CCTL", "FENCE"]
 
 
@@ -16,7 +16,7 @@ def main() -> int:
     so = sys.argv[1] if len(sys.argv) > 1 else sorted(glob.glob("blackbird_b200/_bb*.so"))[0]
     txt = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
     demangle = subprocess.run(["c++filt"], input=txt, capture_output=True, text=True).stdout
-    print(f"SASS census of {so} (cuobjdump -sass, sm_100a), final code of round 2.  Columns = instruction counts per kernel.\n")
+    print(f"SASS census of {so} (cuobjdump -sass, sm_90a).  Columns = instruction counts per kernel.\n")
     cur, counts = None, collections.OrderedDict()
     for line in demangle.splitlines():
         m = re.match(r"\s*Function : (.*)", line)

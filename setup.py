@@ -1,5 +1,5 @@
 """`pip install -e .` / `python setup.py build_ext --inplace`: the native code is built by build.py (ninja + g++ +
-nvcc for sm_100a) into blackbird_b200/_bb*.so and bin/; setuptools only packages the result."""
+nvcc for sm_90a) into blackbird_b200/_bb*.so and bin/; setuptools only packages the result."""
 import os
 import subprocess
 import sys

@@ -15,7 +15,7 @@ if PKG_ROOT != ROOT:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run with -m gpu on an H100 box)")
 
 
 def _have_module():

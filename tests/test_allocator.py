@@ -163,7 +163,7 @@ def test_range_min_shard_strict_fails_default_narrows(bb):
     with pytest.raises(bb.BlackbirdError) as e:  # reference semantics
         ra.allocate(req(bb, "small", 1024, wpc=4, min_shard=4096, strict_min_shard=True), pools)
     assert e.value.code == bb.ErrorCode.INSUFFICIENT_SPACE
-    res = ra.allocate(req(bb, "small", 1024, wpc=4, min_shard=4096), pools)  # B200 store: narrow the stripe
+    res = ra.allocate(req(bb, "small", 1024, wpc=4, min_shard=4096), pools)  # GPU store: narrow the stripe
     assert len(res.copies[0].shards) == 1 and res.copies[0].shards[0].length == 1024
     pools8 = {f"q{i}": mkpool(bb, f"q{i}", 16384) for i in range(8)}
     with pytest.raises(bb.BlackbirdError):

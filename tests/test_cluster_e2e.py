@@ -197,10 +197,11 @@ def test_multi_tier_worker_and_class_preference(bb, tmp_path):
 
 
 def test_config_files_parse(bb, tmp_path):
-    ks = bb.KeystoneConfig.from_yaml("/root/reference/configs/keystone.yaml")  # reference sample parses unchanged
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_configs")
+    ks = bb.KeystoneConfig.from_yaml(os.path.join(golden, "keystone.yaml"))  # reference sample parses unchanged
     assert ks.cluster_id == "blackbird_cluster" and ks.etcd_endpoints == "localhost:2379" and ks.high_watermark == 0.8
     assert ks.client_ttl_sec == 300 and ks.max_replicas == 3 and ks.log_level == "INFO"
-    wc = bb.WorkerServiceConfig.from_yaml("/root/reference/configs/worker.yaml")
+    wc = bb.WorkerServiceConfig.from_yaml(os.path.join(golden, "worker.yaml"))
     assert wc.worker_id == "worker-1" and wc.interconnects == ["rdma", "tcp"] and wc.heartbeat_interval_sec == 5
     assert wc.storage_pools[0].pool_id == "ram_pool_0" and wc.storage_pools[0].size_bytes == 2 << 30
     for name in ("keystone.yaml", "worker.yaml", "gpu_worker.yaml", "tiered_worker.yaml"):
@@ -557,7 +558,7 @@ def test_health_loop_compacts_pools_above_the_fragmentation_threshold(bb):
         assert c.keystone.run_compaction_once() == 0
 
 
-def test_readers_survive_concurrent_compaction_and_migration(bb):
+def test_readers_survive_concurrent_compaction_and_migration(bb, tmp_path):
     """Gets that lose a race with the Keystone moving an object (compaction, explicit migration) re-read the placements
     and succeed: no reader ever sees an error or wrong bytes while objects are being shuffled underneath."""
     import random
@@ -567,7 +568,7 @@ def test_readers_survive_concurrent_compaction_and_migration(bb):
     MiB = 1 << 20
     with LocalCluster(cluster_id="shuffle", n_workers=1, pool_bytes=24 * MiB) as c:
         c.keystone.install_data_server_mover()
-        c.add_worker("worker-disk", "node-0", [("disk-0", bb.StorageClass.HDD, 64 * MiB, "/tmp")])
+        c.add_worker("worker-disk", "node-0", [("disk-0", bb.StorageClass.HDD, 64 * MiB, str(tmp_path))])
         cl = c.client()
         cfg = bb.WorkerConfig(replication_factor=1, max_workers_per_copy=1, ttl_ms=0, preferred_classes=[bb.StorageClass.RAM_CPU])
         blobs = {f"o{i}": os.urandom(MiB // 2 + 1000 * i) for i in range(14)}

@@ -1,5 +1,5 @@
 """The device batch API of the client (batch_put_device / batch_get_device) on CPU: a HostLoopbackTransport stands in for
-the GPU fabric ("device pointers" are numpy buffers), so the logic that otherwise only runs on a B200 -- descriptors
+the GPU fabric ("device pointers" are numpy buffers), so the logic that otherwise only runs on a GPU -- descriptors
 per shard with replica fan-out, chunk pipelining, replica choice and fail-over on digest mismatch, host-staged
 fall-back for unreachable tiers, capacity checks -- is exercised by the CPU suite."""
 import os

@@ -64,7 +64,7 @@ def test_fused_batch_of_small_objects(bb, torch_cuda):
 @pytest.mark.parametrize("algo_name", ["BBH64", "CRC32C", "XXH3", "NONE"])
 def test_small_object_warp_path_matches_cpu_models_and_the_big_kernel(bb, torch_cuda, algo_name):
     """xfer_small.cu: batches made only of objects <= 4 KiB take the warp-per-object kernel; bytes and digests are
-    identical to the CPU models and to what the TMA / tcgen05 kernel produces for the same objects."""
+    identical to the CPU models and to what the TMA / wgmma kernel produces for the same objects."""
     torch = torch_cuda
     algo = getattr(bb.ChecksumAlgo, algo_name)
     eng = bb.XferEngine(0, 8192, 2)
