@@ -8,6 +8,7 @@
 #include "common/checksum.h"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
+#include "kernels/xfer_common.cuh"
 
 namespace bb::gpu {
 namespace {
@@ -66,7 +67,7 @@ struct CrcConsts {
 
 __constant__ uint32_t c_crc_table[4][256];  // slice-by-4 byte tables for the standard byte step
 
-__device__ __forceinline__ uint32_t gf2_mulmod_dev(uint32_t a, uint32_t b) {
+__device__ __forceinline__ uint32_t gf2_mulmod_simt(uint32_t a, uint32_t b) {
   uint32_t p = 0;
 #pragma unroll 1
   for (uint32_t m = 1u << 31; m; m >>= 1) {
@@ -114,22 +115,13 @@ __global__ void __launch_bounds__(1024) crc_combine_kernel(uint32_t* arr, uint64
   uint32_t L = 0;
   for (uint64_t s = 1; s < nchunks; s <<= 1, ++L) {
     for (uint64_t lo = static_cast<uint64_t>(threadIdx.x) * 2 * s; lo + s < nchunks; lo += static_cast<uint64_t>(blockDim.x) * 2 * s)
-      arr[lo] ^= gf2_mulmod_dev(arr[lo + s], k.level_xp[L]);
+      arr[lo] ^= gf2_mulmod_simt(arr[lo + s], k.level_xp[L]);
     __syncthreads();
   }
   if (threadIdx.x == 0) *out = arr[0] ^ k.init_term ^ 0xFFFFFFFFu;
 }
 
 bool g_crc_table_init[16] = {false};
-
-int grid_for(uint64_t work_items, int threads, int per_sm) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  uint64_t need = (work_items + threads - 1) / threads;
-  uint64_t cap = static_cast<uint64_t>(sms) * per_sm;
-  return static_cast<int>(need < 1 ? 1 : (need > cap ? cap : need));
-}
 
 }  // namespace
 

@@ -9,8 +9,15 @@
 
 #include "common/tchash_def.h"
 #include "kernels/ptx.cuh"
+#include "kernels/xfer_common.cuh"
 
 namespace bb::gpu {
+
+// Thread `tid` of `nthreads` writes its share of the 2 KiB BBH64 weight matrix W[k][n] as the wgmma B operand (N = 16
+// rows, K-major, no swizzle); the caller fences it for the async proxy and synchronises.
+__device__ __forceinline__ void bbh_load_weights(uint8_t* w, uint32_t tid, uint32_t nthreads) {
+  for (uint32_t o = tid; o < 2048; o += nthreads) w[o] = static_cast<uint8_t>(tchash::weight(tchash::off_to_k(o), tchash::off_to_row(o)));
+}
 
 // d[8h + i] (h = M half) follows the wgmma_m64n16k32_u8 fragment layout, with rows offset by 64 h.
 // Every thread of the warpgroup must call this (the MMAs are warpgroup-wide).
@@ -42,19 +49,14 @@ __device__ __forceinline__ uint64_t bbh_tile_rows(const uint32_t (&d)[16], const
   uint64_t part[4] = {0, 0, 0, 0};  // rows bbh_acc_row(k) for k = 0, 2, 8, 10
 #pragma unroll
   for (uint32_t k = 0; k < 16; ++k) part[2 * (k >> 3) + ((k >> 1) & 1u)] += static_cast<uint64_t>(d[k]) * col_mul[bbh_acc_col(k, lane)];
-  auto shfl_xor = [](uint64_t v, int m) {
-    const uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), m);
-    const uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), m);
-    return (static_cast<uint64_t>(hi) << 32) | lo;
-  };
   const bool b1 = (lane >> 1) & 1u, b0 = lane & 1u;
-  const uint64_t k0 = (b1 ? part[2] : part[0]) + shfl_xor(b1 ? part[0] : part[2], 2);  // M half b1
-  const uint64_t k1 = (b1 ? part[3] : part[1]) + shfl_xor(b1 ? part[1] : part[3], 2);
-  const uint64_t r = (b0 ? k1 : k0) + shfl_xor(b0 ? k0 : k1, 1);                        // row offset 8 b0
+  const uint64_t k0 = (b1 ? part[2] : part[0]) + shfl_xor_u64(b1 ? part[0] : part[2], 2);  // M half b1
+  const uint64_t k1 = (b1 ? part[3] : part[1]) + shfl_xor_u64(b1 ? part[1] : part[3], 2);
+  const uint64_t r = (b0 ? k1 : k0) + shfl_xor_u64(b0 ? k0 : k1, 1);                        // row offset 8 b0
   const uint32_t row = 64u * b1 + 16u * q + (lane >> 2) + 8u * b0;
   uint64_t v = tchash::row_contrib(r, static_cast<uint64_t>(tile_index) * tchash::kRows + row);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += shfl_xor(v, o);
+  for (int o = 16; o > 0; o >>= 1) v += shfl_xor_u64(v, o);
   return v;
 }
 

@@ -1,0 +1,167 @@
+// What the data-plane kernels share: reading the XferDesc table, the split of a batch's tiles over the CTAs, 64-bit warp
+// shuffles, the GF(2) multiply of the CRC32C combine, and the per-device state of the host launchers.
+#pragma once
+#include <cuda_runtime.h>
+
+#include <atomic>
+#include <cstddef>
+#include <cstdint>
+#include <mutex>
+
+#include "kernels/xfer.h"
+
+namespace bb::gpu {
+
+// ---------------------------------------------------------------- descriptor table
+// The 32- / 64-bit field at byte offset OFF of a descriptor read as four 16-byte words.
+template <size_t OFF>
+__device__ __forceinline__ uint32_t desc_u32(const uint4 (&w)[4]) {
+  static_assert(OFF % 4 == 0 && OFF + 4 <= sizeof(XferDesc));
+  return reinterpret_cast<const uint32_t*>(w)[OFF / 4];
+}
+template <size_t OFF>
+__device__ __forceinline__ uint64_t desc_u64(const uint4 (&w)[4]) {
+  static_assert(OFF % 8 == 0);
+  return (static_cast<uint64_t>(desc_u32<OFF + 4>(w)) << 32) | desc_u32<OFF>(w);
+}
+
+// A descriptor read as words; the field positions come from XferDesc itself.
+__device__ __forceinline__ XferDesc desc_from_words(const uint4 (&w)[4]) {
+  static_assert(sizeof(XferDesc) == sizeof(w) && kMaxDst == 3 && sizeof(void*) == 8 && sizeof(XferDesc::nbytes) == 8);
+  XferDesc d;
+  d.src = reinterpret_cast<const void*>(desc_u64<offsetof(XferDesc, src)>(w));
+  d.dst[0] = reinterpret_cast<void*>(desc_u64<offsetof(XferDesc, dst) + 0 * sizeof(void*)>(w));
+  d.dst[1] = reinterpret_cast<void*>(desc_u64<offsetof(XferDesc, dst) + 1 * sizeof(void*)>(w));
+  d.dst[2] = reinterpret_cast<void*>(desc_u64<offsetof(XferDesc, dst) + 2 * sizeof(void*)>(w));
+  d.nbytes = desc_u64<offsetof(XferDesc, nbytes)>(w);
+  d.first_tile = desc_u32<offsetof(XferDesc, first_tile)>(w);
+  d.ndst = desc_u32<offsetof(XferDesc, ndst)>(w);
+  d.expect = desc_u64<offsetof(XferDesc, expect)>(w);
+  d.flags = desc_u32<offsetof(XferDesc, flags)>(w);
+  d.reserved = desc_u32<offsetof(XferDesc, reserved)>(w);
+  return d;
+}
+
+// The descriptor table of a launch, as a copy in the kernel parameters (PARAM: plain loads, ld.global.nc is illegal on
+// the parameter space) or in device memory (read-only path).  tile_start[i] is the first tile of descriptor i and
+// tile_start[ndesc] the batch's tile count; kernels that do not split objects into tiles leave it null.
+template <bool PARAM>
+struct DescTable {
+  const XferDesc* descs;
+  const uint32_t* tile_start;
+  uint32_t ndesc;
+
+  __device__ __forceinline__ uint32_t start(uint32_t i) const { return PARAM ? tile_start[i] : __ldg(&tile_start[i]); }
+
+  // Descriptor i as four 16-byte words, for desc_from_words.
+  __device__ __forceinline__ void load(uint32_t i, uint4 (&w)[4]) const {
+    const uint4* q = reinterpret_cast<const uint4*>(&descs[i]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = PARAM ? q[k] : __ldg(q + k);
+  }
+  __device__ __forceinline__ XferDesc operator[](uint32_t i) const {
+    uint4 w[4];
+    load(i, w);
+    return desc_from_words(w);
+  }
+
+  // The descriptor holding tile t: start(i) <= t < start(i + 1).
+  __device__ __forceinline__ uint32_t desc_of_tile(uint32_t t) const {
+    uint32_t lo = 0, hi = ndesc;
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (start(mid) <= t) lo = mid; else hi = mid;
+    }
+    return lo;
+  }
+};
+
+// (t0, n): this CTA's contiguous run of tiles [t0, t0 + n) when a batch of total_tiles is split evenly over the grid.
+__device__ __forceinline__ uint2 cta_tile_run(uint32_t total_tiles) {
+  const uint32_t tpc = (total_tiles + gridDim.x - 1) / gridDim.x;
+  const uint32_t t0 = blockIdx.x * tpc;
+  return make_uint2(t0, t0 < total_tiles ? min(tpc, total_tiles - t0) : 0);
+}
+
+// ---------------------------------------------------------------- warp helpers
+__device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
+  const uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), m);
+  const uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), m);
+  return (static_cast<uint64_t>(hi) << 32) | lo;
+}
+__device__ __forceinline__ uint64_t shfl_u64(uint64_t v, int src) {
+  const uint32_t lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v), src);
+  const uint32_t hi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), src);
+  return (static_cast<uint64_t>(hi) << 32) | lo;
+}
+
+// a * b mod P in the reflected CRC32C representation (0x80000000 == 1).
+__device__ __forceinline__ uint32_t gf2_mulmod_dev(uint32_t a, uint32_t b) {
+  uint32_t p = 0;
+#pragma unroll 4
+  for (int i = 31; i >= 0; --i) {
+    p ^= ((a >> i) & 1u) ? b : 0u;
+    b = (b >> 1) ^ ((b & 1u) ? 0x82F63B78u : 0u);
+  }
+  return p;
+}
+
+// ---------------------------------------------------------------- host: per-device launcher state
+constexpr int kMaxDevices = 16;  // launchers keep their per-device state in arrays of this size
+
+// The calling thread's current device; cudaErrorInvalidDevice if it has no slot in those arrays.
+inline cudaError_t current_device(int* dev) {
+  const cudaError_t e = cudaGetDevice(dev);
+  if (e != cudaSuccess) return e;
+  return *dev >= 0 && *dev < kMaxDevices ? cudaSuccess : cudaErrorInvalidDevice;
+}
+
+// Multiprocessor count of the current device, queried once per device; 132 (an H100 SXM) if the query fails.
+inline int current_sm_count() {
+  static std::atomic<int> cache[kMaxDevices];
+  int dev = 0;
+  if (current_device(&dev) != cudaSuccess) return 132;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
+
+// Grid of a grid-stride kernel: enough blocks of `threads` for `work_items`, at most `per_sm` per SM.
+inline int grid_for(uint64_t work_items, int threads, int per_sm) {
+  const uint64_t need = (work_items + threads - 1) / threads, cap = static_cast<uint64_t>(current_sm_count()) * per_sm;
+  return static_cast<int>(need < 1 ? 1 : (need > cap ? cap : need));
+}
+
+// Raises KERNEL's dynamic shared-memory limit to `bytes` on device `dev`, once (a repeated call is harmless).
+template <auto KERNEL>
+cudaError_t set_max_dynamic_smem_once(int dev, int bytes) {
+  static std::atomic<bool> done[kMaxDevices];
+  if (done[dev].load(std::memory_order_acquire)) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) done[dev].store(true, std::memory_order_release);
+  return e;
+}
+
+// Runs a launcher's per-device set-up (its own __constant__ uploads and tables: without relocatable device code every
+// translation unit has its own copy of its constants) once per device, serialised; a failed set-up returns its error
+// and runs again on the next call.
+class PerDeviceOnce {
+ public:
+  template <class F>
+  cudaError_t run(int dev, F&& init) {
+    std::lock_guard<std::mutex> lk(mu_);
+    if (done_[dev]) return cudaSuccess;
+    const cudaError_t e = init();
+    if (e == cudaSuccess) done_[dev] = true;
+    return e;
+  }
+
+ private:
+  std::mutex mu_;
+  bool done_[kMaxDevices] = {};
+};
+
+}  // namespace bb::gpu

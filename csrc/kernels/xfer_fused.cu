@@ -4,7 +4,7 @@
 // :315-327 get; SURVEY K1/K4/K6/K11/K13) with ONE persistent launch per batch.  Every CTA owns
 // a contiguous run of 16 KiB tiles of the batch and pipelines them through 8 smem stages:
 //
-//   warp 0  producer : descriptor lookup (32 tiles looked up in parallel), zero-pads short
+//   warp 0  producer : descriptor lookup (32 tiles looked up in parallel, xfer_common.cuh), zero-pads short
 //                      tiles, `cp.async.bulk` global -> shared (TMA, mbarrier complete_tx).
 //                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
@@ -40,6 +40,7 @@
 #include "kernels/bbh_tile.cuh"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
+#include "kernels/xfer_common.cuh"
 
 namespace bb::gpu {
 namespace {
@@ -126,17 +127,6 @@ struct Params {
   XferDesc inl_descs[kInlineDescs];
 };
 
-__device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
-  const uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), m);
-  const uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), m);
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-__device__ __forceinline__ uint64_t shfl_u64(uint64_t v, int src) {
-  const uint32_t lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v), src);
-  const uint32_t hi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), src);
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-
 // s * x^(8k) mod P through the 4x256 table of distance k.
 __device__ __forceinline__ uint32_t crc_shift(const uint32_t (*t)[256], uint32_t s) {
   return t[0][s & 0xFFu] ^ t[1][(s >> 8) & 0xFFu] ^ t[2][(s >> 16) & 0xFFu] ^ t[3][s >> 24];
@@ -156,16 +146,6 @@ __device__ __forceinline__ uint32_t crc_nib_shift(uint32_t v, uint32_t nib_lane)
   return crc_nib_lookup<0>(v, nib_lane) ^ crc_nib_lookup<1>(v, nib_lane) ^ crc_nib_lookup<2>(v, nib_lane) ^
          crc_nib_lookup<3>(v, nib_lane) ^ crc_nib_lookup<4>(v, nib_lane) ^ crc_nib_lookup<5>(v, nib_lane) ^
          crc_nib_lookup<6>(v, nib_lane) ^ crc_nib_lookup<7>(v, nib_lane);
-}
-
-__device__ __forceinline__ uint32_t gf2_mulmod_dev(uint32_t a, uint32_t b) {
-  uint32_t p = 0;
-#pragma unroll 4
-  for (int i = 31; i >= 0; --i) {
-    p ^= ((a >> i) & 1u) ? b : 0u;
-    b = (b >> 1) ^ ((b & 1u) ? 0x82F63B78u : 0u);
-  }
-  return p;
 }
 
 // x^(8*16384*k) mod P, computed cooperatively by a full warp (lane j owns bit j of k).
@@ -192,10 +172,7 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
   constexpr bool kSum = kBbh || kXxh;  // digest = finalize(commutative sum of per-tile terms)
   constexpr bool kHash = kBbh || kCrc || kXxh;
 
-  // contiguous run of tiles for this CTA
-  const uint32_t tpc = (p.total_tiles + gridDim.x - 1) / gridDim.x;
-  const uint32_t t0 = blockIdx.x * tpc;
-  const uint32_t my_tiles = t0 < p.total_tiles ? min(tpc, p.total_tiles - t0) : 0;
+  const auto [t0, my_tiles] = cta_tile_run(p.total_tiles);
 
   // ------------------------------------------------------------------ setup
   if (threadIdx.x == 0) {
@@ -208,9 +185,7 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     fence_mbar_init();
   }
   if constexpr (kBbh) {
-    // BBH64 weight matrix W[k][n] as the wgmma B operand (N=16 rows, K-major, no swizzle).
-    for (uint32_t o = threadIdx.x; o < 2048; o += kThreads)
-      s.w[o] = static_cast<uint8_t>(tchash::weight(tchash::off_to_k(o), tchash::off_to_row(o)));
+    bbh_load_weights(s.w, threadIdx.x, kThreads);
     fence_proxy_async_smem();
   }
   if constexpr (kCrc) {
@@ -242,40 +217,28 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
       const uint32_t idx = base + lane;
       if (idx < my_tiles) {
         const uint32_t t = t0 + idx;
-        uint32_t lo = 0, hi = p.ndesc;  // tile_start[lo] <= t < tile_start[hi]
-        uint32_t first, next;
-        uint4 q0, q1, q2, q3;
-        if (p.use_inline) {  // table in the parameter space (plain loads: ld.global.nc is illegal there)
-          while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (p.inl_tile_start[mid] <= t) lo = mid; else hi = mid;
-          }
-          first = p.inl_tile_start[lo];
-          next = p.inl_tile_start[lo + 1];
-          const uint4* q = reinterpret_cast<const uint4*>(&p.inl_descs[lo]);
-          q0 = q[0], q1 = q[1], q2 = q[2], q3 = q[3];
+        const DescTable<true> inl{p.inl_descs, p.inl_tile_start, p.ndesc};
+        const DescTable<false> tab{p.descs, p.tile_start, p.ndesc};
+        uint32_t lo, first, next;
+        uint4 w[4];
+        if (p.use_inline) {
+          lo = inl.desc_of_tile(t), first = inl.start(lo), next = inl.start(lo + 1);
+          inl.load(lo, w);
         } else {
-          while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (__ldg(&p.tile_start[mid]) <= t) lo = mid; else hi = mid;
-          }
-          first = __ldg(&p.tile_start[lo]);
-          next = __ldg(&p.tile_start[lo + 1]);
-          const uint4* q = reinterpret_cast<const uint4*>(&p.descs[lo]);
-          q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2), q3 = __ldg(q + 3);
+          lo = tab.desc_of_tile(t), first = tab.start(lo), next = tab.start(lo + 1);
+          tab.load(lo, w);
         }
+        const XferDesc d = desc_from_words(w);
         LookupEntry& e = s.lk[lane];
-        e.src = (static_cast<uint64_t>(q0.y) << 32) | q0.x;
-        e.m.dst[0] = (static_cast<uint64_t>(q0.w) << 32) | q0.z;
-        e.m.dst[1] = (static_cast<uint64_t>(q1.y) << 32) | q1.x;
-        e.m.dst[2] = (static_cast<uint64_t>(q1.w) << 32) | q1.z;
-        e.m.nbytes = (static_cast<uint64_t>(q2.y) << 32) | q2.x;
-        e.m.expect = (static_cast<uint64_t>(q3.y) << 32) | q3.x;
+        e.src = reinterpret_cast<uint64_t>(d.src);
+        for (uint32_t r = 0; r < kMaxDst; ++r) e.m.dst[r] = reinterpret_cast<uint64_t>(d.dst[r]);
+        e.m.nbytes = d.nbytes;
+        e.m.expect = d.expect;
         e.m.desc = lo;
         e.m.tile_in_obj = t - first;
-        e.m.ndst_flags = (q2.w & 0xFFu) | (q3.z << 8);
+        e.m.ndst_flags = (d.ndst & 0xFFu) | (d.flags << 8);
         e.m.obj_ntiles = next - first;
-        e.m.crc_unpad = q3.w;
+        e.m.crc_unpad = d.reserved;
       }
       __syncwarp();
       const uint32_t cnt = min(32u, my_tiles - base);
@@ -587,23 +550,14 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
 
 }
 
-struct DeviceState {
-  bool consts = false;
-  uint32_t* crc_tables = nullptr;
-  int sm_count = 0;
-  bool attr[4] = {false, false, false, false};
-};
-DeviceState g_dev[16];
-std::mutex g_mu;
+PerDeviceOnce g_consts;      // __constant__ uploads
+PerDeviceOnce g_crc_once;    // CRC32C shift tables, on the first CRC32C launch
+uint32_t* g_crc_tables[kMaxDevices] = {};
 
 template <int ALGO>
-cudaError_t launch_t(DeviceState& ds, const Params& p, int grid, cudaStream_t st) {
-  if (!ds.attr[ALGO]) {
-    cudaError_t e = cudaFuncSetAttribute(bb_xfer_kernel<ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(sizeof(SmemT<ALGO>)));
-    if (e != cudaSuccess) return e;
-    ds.attr[ALGO] = true;
-  }
+cudaError_t launch_t(int dev, const Params& p, int grid, cudaStream_t st) {
+  const cudaError_t e = set_max_dynamic_smem_once<bb_xfer_kernel<ALGO>>(dev, static_cast<int>(sizeof(SmemT<ALGO>)));
+  if (e != cudaSuccess) return e;
   bb_xfer_kernel<ALGO><<<grid, kThreads, sizeof(SmemT<ALGO>), st>>>(p);
   return cudaGetLastError();
 }
@@ -665,44 +619,33 @@ int launch_xfer(const XferLaunch& l) {
   if (l.ndesc == 0 || l.total_tiles == 0) return 0;
   if (l.small_path && !l.debug_d && !l.trace_d) return launch_xfer_small(l);
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = current_device(&dev);
   if (e != cudaSuccess) return static_cast<int>(e);
-  if (dev < 0 || dev >= 16) return static_cast<int>(cudaErrorInvalidDevice);
-  DeviceState& ds = g_dev[dev];
-  {
-    std::lock_guard<std::mutex> lk(g_mu);
-    if (!ds.consts) {
-      uint64_t h[tchash::kN];
-      for (uint32_t n = 0; n < tchash::kN; ++n) h[n] = tchash::col_mul(n);
-      e = cudaMemcpyToSymbol(c_col_mul, h, sizeof h);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      uint32_t xp[32];
-      uint32_t b = gf2_xpow_bytes(kTileBytes);
-      for (int j = 0; j < 32; ++j) {
-        xp[j] = b;
-        b = gf2_mulmod(b, b);
-      }
-      e = cudaMemcpyToSymbol(c_xpow_tiles, xp, sizeof xp);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      e = cudaMemcpyToSymbol(c_xxh_secret, xxh3::kSecret, sizeof xxh3::kSecret);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      int n = 0;
-      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-      ds.sm_count = n;
-      ds.consts = true;
+  e = g_consts.run(dev, [] {
+    uint64_t h[tchash::kN];
+    for (uint32_t n = 0; n < tchash::kN; ++n) h[n] = tchash::col_mul(n);
+    cudaError_t e = cudaMemcpyToSymbol(c_col_mul, h, sizeof h);
+    if (e != cudaSuccess) return e;
+    uint32_t xp[32];
+    uint32_t b = gf2_xpow_bytes(kTileBytes);
+    for (int j = 0; j < 32; ++j) {
+      xp[j] = b;
+      b = gf2_mulmod(b, b);
     }
-    if (l.algo == ALGO_CRC32C && !ds.crc_tables) {
-      static uint32_t host_t[kNumCrcTabs][4][256];
-      static bool host_init = false;
-      if (!host_init) {
-        for (int t = 0; t < kNumCrcTabs; ++t) crc32c_shift_table(kCrcTabBytes[t], host_t[t]);
-        host_init = true;
-      }
-      e = cudaMalloc(reinterpret_cast<void**>(&ds.crc_tables), sizeof host_t);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      e = cudaMemcpy(ds.crc_tables, host_t, sizeof host_t, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) return static_cast<int>(e);
-    }
+    e = cudaMemcpyToSymbol(c_xpow_tiles, xp, sizeof xp);
+    if (e != cudaSuccess) return e;
+    return cudaMemcpyToSymbol(c_xxh_secret, xxh3::kSecret, sizeof xxh3::kSecret);
+  });
+  if (e != cudaSuccess) return static_cast<int>(e);
+  if (l.algo == ALGO_CRC32C) {
+    e = g_crc_once.run(dev, [dev] {
+      static uint32_t host_t[kNumCrcTabs][4][256];  // under g_crc_once's lock
+      for (int t = 0; t < kNumCrcTabs; ++t) crc32c_shift_table(kCrcTabBytes[t], host_t[t]);
+      cudaError_t e = cudaSuccess;
+      if (!g_crc_tables[dev] && (e = cudaMalloc(reinterpret_cast<void**>(&g_crc_tables[dev]), sizeof host_t)) != cudaSuccess) return e;
+      return cudaMemcpy(g_crc_tables[dev], host_t, sizeof host_t, cudaMemcpyHostToDevice);
+    });
+    if (e != cudaSuccess) return static_cast<int>(e);
   }
   Params p;
   p.descs = l.descs;
@@ -719,20 +662,21 @@ int launch_xfer(const XferLaunch& l) {
   p.done_ws = l.done_ws;
   p.digest_out = l.digest_out;
   p.status_out = l.status_out;
-  p.crc_tables = ds.crc_tables;
+  p.crc_tables = g_crc_tables[dev];
   p.debug_d = l.debug_d;
   p.trace_d = reinterpret_cast<unsigned long long*>(l.trace_d);
   // At most 128 persistent CTAs (one per SM, 1 CTA/SM by shared memory) for the DRAM-bound digests; BB_XFER_CTAS overrides.
   static const int env_ctas = [] { const char* e = std::getenv("BB_XFER_CTAS"); return e ? std::atoi(e) : 0; }();
   // The fused CRC32C is bound by shared-memory lookups per SM, not by DRAM: it takes every SM.
-  int grid = l.max_ctas > 0 ? l.max_ctas : env_ctas > 0 ? env_ctas : l.algo == ALGO_CRC32C ? ds.sm_count : std::min(ds.sm_count, 128);
+  const int sms = current_sm_count();
+  int grid = l.max_ctas > 0 ? l.max_ctas : env_ctas > 0 ? env_ctas : l.algo == ALGO_CRC32C ? sms : std::min(sms, 128);
   grid = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), l.total_tiles));
   cudaStream_t st = static_cast<cudaStream_t>(l.stream);
   switch (l.algo) {
-    case ALGO_NONE: e = launch_t<ALGO_NONE>(ds, p, grid, st); break;
-    case ALGO_CRC32C: e = launch_t<ALGO_CRC32C>(ds, p, grid, st); break;
-    case ALGO_BBH64: e = launch_t<ALGO_BBH64>(ds, p, grid, st); break;
-    case ALGO_XXH3: e = launch_t<ALGO_XXH3>(ds, p, grid, st); break;
+    case ALGO_NONE: e = launch_t<ALGO_NONE>(dev, p, grid, st); break;
+    case ALGO_CRC32C: e = launch_t<ALGO_CRC32C>(dev, p, grid, st); break;
+    case ALGO_BBH64: e = launch_t<ALGO_BBH64>(dev, p, grid, st); break;
+    case ALGO_XXH3: e = launch_t<ALGO_XXH3>(dev, p, grid, st); break;
     default: return static_cast<int>(cudaErrorNotSupported);
   }
   return static_cast<int>(e);

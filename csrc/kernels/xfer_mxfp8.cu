@@ -1,8 +1,9 @@
 // bb_xfer_fp8: fused MXFP8 transfer kernels (sm_90a; SURVEY K12 "fp8 pack fused into put / unpack into get").
 //
 //   put  (PACK)   : TMA loads a 32 KiB bf16 tile -> 8 pack warps compute the E8M0 block scales and the E4M3
-//                   payload *in shared memory* -> the 16 KiB payload tile is hashed in place by wgmma
-//                   (BBH64, same tile hash as bb_xfer) -> TMA stores payload + 512 B of scales to the
+//                   payload *in shared memory* (the chunk codec of mxfp8.cuh, which the stand-alone kernels use
+//                   too) -> the 16 KiB payload tile is hashed in place by wgmma (BBH64, same tile hash as
+//                   bb_xfer) -> TMA stores payload + 512 B of scales to the
 //                   (peer) slab -- to up to 3 replicas of the object from the one converted tile.  The bf16 data
 //                   is read from HBM once and only the 0.52x packed bytes cross NVLink (once per replica).
 //   get  (UNPACK) : TMA loads payload tile + scales from the slab -> tensor-core hash of the payload tile ->
@@ -18,17 +19,16 @@
 //
 // Warp roles (24 warps): 0 producer, 1 idle, 2 store, 3 accumulator, 4-7 epilogue (the warpgroup issues the wgmma
 // tile product, bbh_tile.cuh, and turns its register accumulators into row hashes), 8-23 convert (pack / unpack).  Two shared-memory rings: 3 x 32 KiB bf16 tiles and 6 x (16 KiB payload + 512 B scales).
-#include <cuda_bf16.h>
-#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <mutex>
 
 #include "common/tchash_def.h"
 #include "kernels/bbh_tile.cuh"
+#include "kernels/mxfp8.cuh"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
+#include "kernels/xfer_common.cuh"
 
 namespace bb::gpu {
 namespace {
@@ -91,59 +91,6 @@ struct FpParams {
   unsigned long long* sum_ws;  // [ndesc] raw BBH64 sums of the payload tiles (zero on entry)
 };
 
-__device__ __forceinline__ __nv_bfloat162 as_bf162(uint32_t v) { return *reinterpret_cast<const __nv_bfloat162*>(&v); }
-
-// One 16-byte chunk (8 bf16) per lane, 4 lanes per 32-element block.  Same arithmetic as mxfp8_pack_kernel
-// (mxfp8.cu) and the CPU reference (common/mxfp8.cpp) -- the stored bytes are identical -- but on packed bf16x2
-// max / paired E4M3 conversions, which halves the instruction count of the straightforward form.
-__device__ __forceinline__ void pack_chunk(const uint4 v, uint2* payload_out, uint8_t* scale_out, bool write_scale) {
-  // |x| on bf16x2 = clear the sign bits; max on the magnitudes as *integers* (monotonic for non-negative bf16).
-  // NaN magnitudes (> 0x7F80) are skipped like the scalar code's `a > amax` does; an Inf (0x7F80) wins the max and
-  // then selects the neutral scale below, again like the scalar code
-  auto mag = [](uint32_t w) { return w & 0x7FFF7FFFu; };
-  auto finite_max = [](uint32_t m, uint32_t cur) {
-    const uint32_t lo = m & 0xFFFFu, hi = m >> 16;
-    uint32_t r = cur;
-    r = (lo <= 0x7F80u && lo > r) ? lo : r;
-    r = (hi <= 0x7F80u && hi > r) ? hi : r;
-    return r;
-  };
-  uint32_t am = 0;
-  am = finite_max(mag(v.x), am);
-  am = finite_max(mag(v.y), am);
-  am = finite_max(mag(v.z), am);
-  am = finite_max(mag(v.w), am);
-  am = max(am, __shfl_xor_sync(0xffffffffu, am, 1));
-  am = max(am, __shfl_xor_sync(0xffffffffu, am, 2));
-  // am = bf16 bits of the block's largest finite magnitude; exponent field = bits 14..7
-  int e = 127;
-  if (am != 0 && am < 0x7F80u) {
-    const int be = static_cast<int>(am >> 7);
-    e = (be == 0 ? -127 : be - 127) - 8 + 127;
-    e = max(0, min(254, e));
-  }
-  const float inv = __int_as_float((254 - e) << 23);
-  auto cvt2 = [&](uint32_t w) -> uint32_t {
-    const float2 f = __bfloat1622float2(as_bf162(w));
-    return static_cast<uint32_t>(__nv_cvt_float2_to_fp8x2(make_float2(f.x * inv, f.y * inv), __NV_SATFINITE, __NV_E4M3));
-  };
-  const uint32_t lo = cvt2(v.x) | (cvt2(v.y) << 16);
-  const uint32_t hi = cvt2(v.z) | (cvt2(v.w) << 16);
-  *payload_out = make_uint2(lo, hi);
-  if (write_scale) *scale_out = static_cast<uint8_t>(e);
-}
-
-__device__ __forceinline__ uint4 unpack_chunk(const uint2 p, uint8_t scale) {
-  const float s = __int_as_float(static_cast<int>(scale) << 23);  // 2^(e-127); e == 0 flushes to zero
-  auto cvt2 = [&](uint32_t two) -> uint32_t {  // two E4M3 bytes -> bf16x2
-    const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two & 0xFFFFu), __NV_E4M3);
-    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));
-    const __nv_bfloat162 h = __floats2bfloat162_rn(f.x * s, f.y * s);
-    return *reinterpret_cast<const uint32_t*>(&h);
-  };
-  return make_uint4(cvt2(p.x), cvt2(p.x >> 16), cvt2(p.y), cvt2(p.y >> 16));
-}
-
 template <bool UNPACK>
 __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid_constant__ FpParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -151,9 +98,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31u;
 
-  const uint32_t tpc = (p.total_tiles + gridDim.x - 1) / gridDim.x;
-  const uint32_t t0 = blockIdx.x * tpc;
-  const uint32_t my_tiles = t0 < p.total_tiles ? min(tpc, p.total_tiles - t0) : 0;
+  const auto [t0, my_tiles] = cta_tile_run(p.total_tiles);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kTileStages; ++i) {
@@ -167,8 +112,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     }
     fence_mbar_init();
   }
-  for (uint32_t o = threadIdx.x; o < 2048; o += kFpThreads)
-    s.w[o] = static_cast<uint8_t>(tchash::weight(tchash::off_to_k(o), tchash::off_to_row(o)));
+  bbh_load_weights(s.w, threadIdx.x, kFpThreads);
   fence_proxy_async_smem();
   __syncthreads();
 
@@ -179,20 +123,14 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
       const uint32_t idx = base + lane;
       if (idx < my_tiles) {
         const uint32_t t = t0 + idx;
-        uint32_t lo = 0, hi = p.ndesc;
-        while (hi - lo > 1) {
-          const uint32_t mid = (lo + hi) >> 1;
-          if (__ldg(&p.tile_start[mid]) <= t) lo = mid; else hi = mid;
-        }
-        const uint32_t first = __ldg(&p.tile_start[lo]);
-        const uint32_t next = __ldg(&p.tile_start[lo + 1]);
-        const uint4* q = reinterpret_cast<const uint4*>(&p.descs[lo]);
-        const uint4 q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2);
-        const uint64_t src = (static_cast<uint64_t>(q0.y) << 32) | q0.x;
-        const uint64_t d0 = (static_cast<uint64_t>(q0.w) << 32) | q0.z;
-        const uint64_t d1 = (static_cast<uint64_t>(q1.y) << 32) | q1.x;
-        const uint64_t d2 = (static_cast<uint64_t>(q1.w) << 32) | q1.z;
-        const uint64_t nbytes = (static_cast<uint64_t>(q2.y) << 32) | q2.x;  // payload bytes == elements
+        const DescTable<false> tab{p.descs, p.tile_start, p.ndesc};
+        const uint32_t lo = tab.desc_of_tile(t);
+        const uint32_t first = tab.start(lo);
+        const uint32_t next = tab.start(lo + 1);
+        const XferDesc d = tab[lo];
+        const uint64_t src = reinterpret_cast<uint64_t>(d.src), d0 = reinterpret_cast<uint64_t>(d.dst[0]),
+                       d1 = reinterpret_cast<uint64_t>(d.dst[1]), d2 = reinterpret_cast<uint64_t>(d.dst[2]);
+        const uint64_t nbytes = d.nbytes;  // payload bytes == elements
         const uint32_t ti = t - first;
         FpLookup& e = s.lk[lane];
         e.m.desc = lo;
@@ -215,7 +153,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kTileBytes;
           e.m.dst[1] = d1 + static_cast<uint64_t>(ti) * kTileBytes;
           e.m.dst[2] = d2 + static_cast<uint64_t>(ti) * kTileBytes;
-          e.m.ndst = min(max(q2.w, 1u), kMaxDst);
+          e.m.ndst = min(max(d.ndst, 1u), kMaxDst);
         }
       }
       __syncwarp();
@@ -380,13 +318,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
 
 }
 
-struct FpDeviceState {
-  bool consts = false;
-  bool attr[2] = {false, false};
-  int sm_count = 0;
-};
-FpDeviceState g_fp_dev[16];
-std::mutex g_fp_mu;
+PerDeviceOnce g_fp_consts;  // __constant__ uploads
 
 }  // namespace
 
@@ -395,36 +327,24 @@ int xfer_fp8_smem_bytes() { return static_cast<int>(sizeof(SmemFp)); }
 int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
   if (l.ndesc == 0 || l.total_tiles == 0) return 0;
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = current_device(&dev);
   if (e != cudaSuccess) return static_cast<int>(e);
-  if (dev < 0 || dev >= 16) return static_cast<int>(cudaErrorInvalidDevice);
-  FpDeviceState& ds = g_fp_dev[dev];
-  {
-    std::lock_guard<std::mutex> lk(g_fp_mu);
-    if (!ds.consts) {
-      uint64_t h[tchash::kN];
-      for (uint32_t n = 0; n < tchash::kN; ++n) h[n] = tchash::col_mul(n);
-      e = cudaMemcpyToSymbol(c_fp_col_mul, h, sizeof h);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      int n = 0;
-      if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-      ds.sm_count = n;
-      ds.consts = true;
-    }
-    if (!ds.attr[unpack ? 1 : 0]) {
-      e = unpack ? cudaFuncSetAttribute(bb_xfer_fp8_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(SmemFp)))
-                 : cudaFuncSetAttribute(bb_xfer_fp8_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(SmemFp)));
-      if (e != cudaSuccess) return static_cast<int>(e);
-      ds.attr[unpack ? 1 : 0] = true;
-    }
-  }
+  e = g_fp_consts.run(dev, [] {
+    uint64_t h[tchash::kN];
+    for (uint32_t n = 0; n < tchash::kN; ++n) h[n] = tchash::col_mul(n);
+    return cudaMemcpyToSymbol(c_fp_col_mul, h, sizeof h);
+  });
+  if (e != cudaSuccess) return static_cast<int>(e);
+  e = unpack ? set_max_dynamic_smem_once<bb_xfer_fp8_kernel<true>>(dev, static_cast<int>(sizeof(SmemFp)))
+             : set_max_dynamic_smem_once<bb_xfer_fp8_kernel<false>>(dev, static_cast<int>(sizeof(SmemFp)));
+  if (e != cudaSuccess) return static_cast<int>(e);
   FpParams p;
   p.descs = l.descs;
   p.tile_start = l.tile_start;
   p.ndesc = l.ndesc;
   p.total_tiles = l.total_tiles;
   p.sum_ws = reinterpret_cast<unsigned long long*>(l.sum_ws);
-  int grid = l.max_ctas > 0 ? l.max_ctas : std::min(ds.sm_count, 128);
+  int grid = l.max_ctas > 0 ? l.max_ctas : std::min(current_sm_count(), 128);
   grid = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), l.total_tiles));
   cudaStream_t st = static_cast<cudaStream_t>(l.stream);
   if (unpack) bb_xfer_fp8_kernel<true><<<grid, kFpThreads, sizeof(SmemFp), st>>>(p);

@@ -12,18 +12,19 @@
 //     BBH64  : the tile product D = A.W is evaluated with dp4a against the same weight matrix (packed in shared memory);
 //              lane l holds K-chunk (l & 7) of rows (l >> 3) * 8 + j, partial row hashes are combined by shuffles;
 //     CRC32C : each lane runs the word-at-a-time table CRC over its 128 bytes, lanes are combined with per-lane
-//              x^(8*distance) multipliers in GF(2)[x]/P (same "raw remainder, un-pad, init term" algebra as the big kernel).
+//              x^(8*distance) multipliers in GF(2)[x]/P (same "raw remainder, un-pad, init term" algebra and the same
+//              GF(2) multiply, xfer_common.cuh, as the big kernel).
 //   A put of 4096 objects is 512 CTAs x 8 warps in one launch; a single put/get is one warp.
 #include <cuda_runtime.h>
 
 #include <cstring>
-#include <mutex>
 
 #include "common/checksum.h"
 #include "common/tchash_def.h"
 #include "common/xxh3.h"
 #include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
+#include "kernels/xfer_common.cuh"
 
 namespace bb::gpu {
 namespace {
@@ -52,22 +53,6 @@ struct SmallParams {
   uint32_t flag_mode;
   XferDesc inl_descs[kInlineDescs];
 };
-
-__device__ __forceinline__ uint32_t gf2_mulmod_small(uint32_t a, uint32_t b) {
-  uint32_t p = 0;
-#pragma unroll 8
-  for (int i = 31; i >= 0; --i) {
-    p ^= ((a >> i) & 1u) ? b : 0u;
-    b = (b >> 1) ^ ((b & 1u) ? 0x82F63B78u : 0u);
-  }
-  return p;
-}
-
-__device__ __forceinline__ uint64_t shfl_xor64(uint64_t v, int m) {
-  const uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), m);
-  const uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), m);
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
 
 // The per-object work of one warp: load (<= 4 KiB, lane l owns bytes [128 l, 128 l + 128)), store to the destinations, digest on
 // the registers.  Shared by the batch kernel (one warp per descriptor) and the mailbox kernel (one resident warp).
@@ -165,15 +150,15 @@ __device__ __forceinline__ void small_object(uint64_t src, const uint64_t (&dst)
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       uint64_t t = rr[j];
-      t += shfl_xor64(t, 1);
-      t += shfl_xor64(t, 2);
-      t += shfl_xor64(t, 4);
+      t += shfl_xor_u64(t, 1);
+      t += shfl_xor_u64(t, 2);
+      t += shfl_xor_u64(t, 4);
       if (static_cast<uint32_t>(j) == kc) mine = t;
     }
     const uint32_t row = (lane >> 3) * 8u + kc;
     uint64_t c = tchash::row_contrib(mine, row);  // tile index 0
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) c += shfl_xor64(c, o);
+    for (int o = 16; o > 0; o >>= 1) c += shfl_xor_u64(c, o);
     digest = tchash::finalize(c + zero_rows, nbytes);
   } else if constexpr (ALGO == ALGO_XXH3) {
     // Standard XXH3-64 of the object zero padded to one 16 KiB tile.  Lane l holds stripes 2 (l & 7) and 2 (l & 7) + 1 of
@@ -199,33 +184,29 @@ __device__ __forceinline__ void small_object(uint64_t src, const uint64_t (&dst)
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const uint64_t keep = (lane & 4u) ? S[i + 4] : S[i], send = (lane & 4u) ? S[i] : S[i + 4];
-      m4[i] = keep + shfl_xor64(send, 4);
+      m4[i] = keep + shfl_xor_u64(send, 4);
     }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const uint64_t keep = (lane & 2u) ? m4[i + 2] : m4[i], send = (lane & 2u) ? m4[i] : m4[i + 2];
-      m2[i] = keep + shfl_xor64(send, 2);
+      m2[i] = keep + shfl_xor_u64(send, 2);
     }
-    const uint64_t tot = ((lane & 1u) ? m2[1] : m2[0]) + shfl_xor64((lane & 1u) ? m2[0] : m2[1], 1);  // [block lane >> 3][acc lane & 7]
+    const uint64_t tot = ((lane & 1u) ? m2[1] : m2[0]) + shfl_xor_u64((lane & 1u) ? m2[0] : m2[1], 1);  // [block lane >> 3][acc lane & 7]
     const uint32_t l8 = lane & 7u;
     uint64_t a = xxh3::init_acc(l8);
     const uint64_t skey = c_xxh[24 + l8], zero_blk = c_xxh[40 + l8];
 #pragma unroll
     for (int b = 0; b < 4; ++b) {
-      const uint32_t lo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(tot), static_cast<int>(l8 + 8u * b));
-      const uint32_t hi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(tot >> 32), static_cast<int>(l8 + 8u * b));
-      a = xxh3::scramble(a + ((static_cast<uint64_t>(hi) << 32) | lo), skey);
+      a = xxh3::scramble(a + shfl_u64(tot, static_cast<int>(l8 + 8u * b)), skey);
     }
 #pragma unroll
     for (int b = 4; b < 15; ++b) a = xxh3::scramble(a + zero_blk, skey);
     a += c_xxh[48 + l8];
     const uint64_t mkey = c_xxh[32 + l8];
-    const uint32_t nlo = __shfl_sync(0xffffffffu, static_cast<uint32_t>(a), static_cast<int>((lane + 1u) & 31u));
-    const uint32_t nhi = __shfl_sync(0xffffffffu, static_cast<uint32_t>(a >> 32), static_cast<int>((lane + 1u) & 31u));
-    const uint64_t nb = (static_cast<uint64_t>(nhi) << 32) | nlo;
+    const uint64_t nb = shfl_u64(a, static_cast<int>((lane + 1u) & 31u));
     uint64_t mg = (l8 & 1u) ? 0ull : xxh3::mul128_fold64(a ^ mkey, nb ^ c_xxh[32 + ((l8 + 1u) & 7u)]);
-    mg += shfl_xor64(mg, 2);
-    mg += shfl_xor64(mg, 4);
+    mg += shfl_xor_u64(mg, 2);
+    mg += shfl_xor_u64(mg, 4);
     const uint64_t h = xxh3::avalanche(mg + static_cast<uint64_t>(kTileBytes) * xxh3::P64_1);
     digest = tchash::finalize(tchash::mix64(h + tchash::kGold), nbytes);  // tile index 0
   } else {
@@ -241,10 +222,10 @@ __device__ __forceinline__ void small_object(uint64_t src, const uint64_t (&dst)
       }
     }
     // place the segment inside a zero-padded 16 KiB tile and add the lanes up (XOR)
-    uint32_t acc = gf2_mulmod_small(s, c_lane_mul[lane]);
+    uint32_t acc = gf2_mulmod_dev(s, c_lane_mul[lane]);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc ^= __shfl_xor_sync(0xffffffffu, acc, o);
-    digest = gf2_mulmod_small(acc, reserved) ^ static_cast<uint32_t>(expect >> 32) ^ 0xFFFFFFFFu;
+    digest = gf2_mulmod_dev(acc, reserved) ^ static_cast<uint32_t>(expect >> 32) ^ 0xFFFFFFFFu;
     expect &= 0xFFFFFFFFull;
   }
   *digest_out = digest;
@@ -276,30 +257,11 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32) bb_xfer_small_kernel(const 
   const uint32_t d = blockIdx.x * kWarpsPerCta + warp;
   if (d >= p.ndesc) return;
   // ---- descriptor (every lane reads the same words: broadcast)
-  uint64_t src, dst[kMaxDst], nbytes, expect;
-  uint32_t ndst, flags, reserved;
-  if (p.use_inline) {
-    const XferDesc& q = p.inl_descs[d];
-    src = reinterpret_cast<uint64_t>(q.src);
-#pragma unroll
-    for (uint32_t r = 0; r < kMaxDst; ++r) dst[r] = reinterpret_cast<uint64_t>(q.dst[r]);
-    nbytes = q.nbytes, expect = q.expect, ndst = q.ndst, flags = q.flags, reserved = q.reserved;
-  } else {
-    const uint4* q = reinterpret_cast<const uint4*>(&p.descs[d]);
-    const uint4 q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2), q3 = __ldg(q + 3);
-    src = (static_cast<uint64_t>(q0.y) << 32) | q0.x;
-    dst[0] = (static_cast<uint64_t>(q0.w) << 32) | q0.z;
-    dst[1] = (static_cast<uint64_t>(q1.y) << 32) | q1.x;
-    dst[2] = (static_cast<uint64_t>(q1.w) << 32) | q1.z;
-    nbytes = (static_cast<uint64_t>(q2.y) << 32) | q2.x;
-    ndst = q2.w;
-    expect = (static_cast<uint64_t>(q3.y) << 32) | q3.x;
-    flags = q3.z;
-    reserved = q3.w;
-  }
+  const XferDesc q = p.use_inline ? DescTable<true>{p.inl_descs, nullptr, p.ndesc}[d] : DescTable<false>{p.descs, nullptr, p.ndesc}[d];
+  const uint64_t dst[kMaxDst] = {reinterpret_cast<uint64_t>(q.dst[0]), reinterpret_cast<uint64_t>(q.dst[1]), reinterpret_cast<uint64_t>(q.dst[2])};
   uint64_t digest = 0;
   uint32_t status = 0;
-  small_object<ALGO, false>(src, dst, ndst, nbytes, expect, flags, reserved, lane, p.zero_rows, s_w, s_t4, s_xk, &digest, &status);
+  small_object<ALGO, false>(reinterpret_cast<uint64_t>(q.src), dst, q.ndst, q.nbytes, q.expect, q.flags, q.reserved, lane, p.zero_rows, s_w, s_t4, s_xk, &digest, &status);
   if (p.flag_mode) {
     __threadfence_system();  // every lane: its stores of the payload are performed system-wide ...
     __syncwarp();            // ... before lane 0 publishes the result
@@ -391,56 +353,51 @@ __global__ void __launch_bounds__(32) bb_mailbox_kernel(const MailSlot* slots, M
   }
 }
 
-struct SmallState {
-  bool consts = false;
+struct SmallTables {
   uint32_t* t4 = nullptr;
   uint64_t zero_rows = 0;
 };
-SmallState g_small[16];
-std::mutex g_small_mu;
+SmallTables g_small[kMaxDevices];
+PerDeviceOnce g_small_once;
 
-// Per-device constants and tables of the small-object kernels (idempotent).
-int ensure_small_state(SmallState** out) {
+// The current device's tables, made (and the __constant__ tables uploaded) on first use.
+int ensure_small_state(SmallTables** out) {
   int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = current_device(&dev);
   if (e != cudaSuccess) return static_cast<int>(e);
-  if (dev < 0 || dev >= 16) return static_cast<int>(cudaErrorInvalidDevice);
-  SmallState& st = g_small[dev];
-  std::lock_guard<std::mutex> lk(g_small_mu);
-    if (!st.consts) {
-      uint32_t mul[32];
-      for (uint32_t ln = 0; ln < 32; ++ln) mul[ln] = gf2_xpow_bytes(128ull * (31 - ln) + (kTileBytes - kSmallBytes));
-      e = cudaMemcpyToSymbol(c_lane_mul, mul, sizeof mul);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      uint32_t t4[4][256];
-      crc32c_shift_table(4, t4);
-      e = cudaMalloc(reinterpret_cast<void**>(&st.t4), sizeof t4);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      e = cudaMemcpy(st.t4, t4, sizeof t4, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      uint64_t z = 0;
-      for (uint32_t m = kSmallBytes / 128; m < tchash::kRows; ++m) z += tchash::row_contrib(0, m);
-      st.zero_rows = z;
-      uint64_t xk[56] = {};
-      for (uint32_t i = 0; i < 23; ++i) xk[i] = xxh3::secret64(8 * i);
-      for (uint32_t i = 0; i < 8; ++i) {
-        xk[24 + i] = xxh3::scramble_key(i);
-        xk[32 + i] = xxh3::merge_key(i);
-        uint64_t zsum = 0, zlast = 0;
-        for (uint32_t sidx = 0; sidx < 16; ++sidx) {
-          const uint64_t k = xxh3::stripe_key(sidx, i);
-          zsum += static_cast<uint64_t>(static_cast<uint32_t>(k)) * (k >> 32);
-          if (sidx < 15) zlast += static_cast<uint64_t>(static_cast<uint32_t>(k)) * (k >> 32);
-        }
-        const uint64_t lk = xxh3::last_key(i);
-        zlast += static_cast<uint64_t>(static_cast<uint32_t>(lk)) * (lk >> 32);
-        xk[40 + i] = zsum;
-        xk[48 + i] = zlast;
+  SmallTables& st = g_small[dev];
+  e = g_small_once.run(dev, [&st] {
+    uint32_t mul[32];
+    for (uint32_t ln = 0; ln < 32; ++ln) mul[ln] = gf2_xpow_bytes(128ull * (31 - ln) + (kTileBytes - kSmallBytes));
+    cudaError_t e = cudaMemcpyToSymbol(c_lane_mul, mul, sizeof mul);
+    if (e != cudaSuccess) return e;
+    uint32_t t4[4][256];
+    crc32c_shift_table(4, t4);
+    if (!st.t4 && (e = cudaMalloc(reinterpret_cast<void**>(&st.t4), sizeof t4)) != cudaSuccess) return e;
+    e = cudaMemcpy(st.t4, t4, sizeof t4, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) return e;
+    uint64_t z = 0;
+    for (uint32_t m = kSmallBytes / 128; m < tchash::kRows; ++m) z += tchash::row_contrib(0, m);
+    st.zero_rows = z;
+    uint64_t xk[56] = {};
+    for (uint32_t i = 0; i < 23; ++i) xk[i] = xxh3::secret64(8 * i);
+    for (uint32_t i = 0; i < 8; ++i) {
+      xk[24 + i] = xxh3::scramble_key(i);
+      xk[32 + i] = xxh3::merge_key(i);
+      uint64_t zsum = 0, zlast = 0;
+      for (uint32_t sidx = 0; sidx < 16; ++sidx) {
+        const uint64_t k = xxh3::stripe_key(sidx, i);
+        zsum += static_cast<uint64_t>(static_cast<uint32_t>(k)) * (k >> 32);
+        if (sidx < 15) zlast += static_cast<uint64_t>(static_cast<uint32_t>(k)) * (k >> 32);
       }
-      e = cudaMemcpyToSymbol(c_xxh, xk, sizeof xk);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      st.consts = true;
+      const uint64_t lk = xxh3::last_key(i);
+      zlast += static_cast<uint64_t>(static_cast<uint32_t>(lk)) * (lk >> 32);
+      xk[40 + i] = zsum;
+      xk[48 + i] = zlast;
     }
+    return cudaMemcpyToSymbol(c_xxh, xk, sizeof xk);
+  });
+  if (e != cudaSuccess) return static_cast<int>(e);
   *out = &st;
   return 0;
 }
@@ -448,7 +405,7 @@ int ensure_small_state(SmallState** out) {
 
 int launch_mailbox(const MailSlot* slots, MailResult* results, MailCtl* ctl, uint32_t first_seq, uint32_t epoch, uint64_t linger_ns,
                    uint64_t max_ns, void* stream) {
-  SmallState* st = nullptr;
+  SmallTables* st = nullptr;
   if (const int rc = ensure_small_state(&st)) return rc;
   bb_mailbox_kernel<<<1, 32, 0, static_cast<cudaStream_t>(stream)>>>(slots, results, ctl, first_seq, epoch, linger_ns, max_ns, st->t4, st->zero_rows);
   return static_cast<int>(cudaGetLastError());
@@ -456,10 +413,8 @@ int launch_mailbox(const MailSlot* slots, MailResult* results, MailCtl* ctl, uin
 
 int launch_xfer_small(const XferLaunch& l) {
   if (l.ndesc == 0) return 0;
-  SmallState* stp = nullptr;
-  if (const int rc = ensure_small_state(&stp)) return rc;
-  SmallState& st = *stp;
-  cudaError_t e = cudaSuccess;
+  SmallTables* st = nullptr;
+  if (const int rc = ensure_small_state(&st)) return rc;
   SmallParams p;
   p.descs = l.descs;
   p.ndesc = l.ndesc;
@@ -470,8 +425,8 @@ int launch_xfer_small(const XferLaunch& l) {
   }
   p.digest_out = l.digest_out;
   p.status_out = l.status_out;
-  p.crc_t4 = st.t4;
-  p.zero_rows = st.zero_rows;
+  p.crc_t4 = st->t4;
+  p.zero_rows = st->zero_rows;
   p.flag_mode = l.flag_completion ? 1u : 0u;
   const int grid = static_cast<int>((l.ndesc + kWarpsPerCta - 1) / kWarpsPerCta);
   const int threads = l.ndesc < static_cast<uint32_t>(kWarpsPerCta) ? static_cast<int>(l.ndesc) * 32 : kWarpsPerCta * 32;

@@ -54,6 +54,20 @@ def test_gpu_pack_unpack_match_cpu_reference(bb):
     n = 32 * 40000 + 32 * 3
     x = (torch.randn(n, device="cuda", generator=g) * 10 ** torch.empty(n, device="cuda").uniform_(-3, 2, generator=g)).to(torch.bfloat16)
     x[64:96] = 0
+    # blocks with special values (bf16 bit patterns): +-Inf, NaN of either sign, subnormals, negative zeros, and mixes
+    # of them with normal values; the block maximum skips NaN, an Inf selects the neutral scale
+    special = torch.from_numpy(np.array([
+        [0x7F80, 0x3F80, 0xC000] + [0x3E00] * 29,    # +Inf with normals
+        [0xFF80, 0x4100, 0x0001] + [0xBC00] * 29,    # -Inf with a normal and a subnormal
+        [0x7FC0, 0x4000, 0xC040] + [0x3C00] * 29,    # NaN with normals
+        [0xFFC1, 0x7FC0] + [0xFFC0] * 30,            # NaN only
+        [0x0001, 0x8003, 0x007F, 0x8040] * 8,        # subnormals only (the scale clamps at 0)
+        [0x0001, 0x807F, 0x3F80, 0x8000] * 8,        # subnormals and -0 next to 1.0
+        [0x8000] * 32,                               # negative zeros only
+        [0x8000, 0x0000, 0x0080, 0x8080] * 8,        # +-0 and +-the smallest normal (the scale clamps at 0)
+    ], dtype=np.uint16).view(np.int16)).view(torch.bfloat16).view(-1).cuda()
+    nx, x = n, torch.cat([x, special])
+    n = x.numel()
     packed = torch.zeros(bb.mxfp8_packed_bytes(n), dtype=torch.uint8, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
     bb.mxfp8_pack(x.data_ptr(), n, packed.data_ptr(), s)
@@ -67,10 +81,17 @@ def test_gpu_pack_unpack_match_cpu_reference(bb):
     bb.mxfp8_unpack(packed.data_ptr(), n, out.data_ptr(), s)
     torch.cuda.synchronize()
     back_ref = torch.frombuffer(bytearray(bb.mxfp8_unpack_ref(got, n)), dtype=torch.bfloat16)
-    assert torch.equal(out.cpu(), back_ref)
+    back = out.cpu()
+    nan = back_ref.isnan()
+    assert torch.equal(back.isnan(), nan)  # NaN stays NaN (the NaN bit patterns of the two sides differ)
+    # A block scale of 0 (2^-127) dequantises to zero on the GPU; the CPU reference multiplies by 2^-127.
+    flushed = torch.from_numpy(got[n:].copy() == 0).repeat_interleave(32)
+    assert bool((back[flushed] == 0).all())
+    keep = ~nan & ~flushed
+    assert torch.equal(back[keep], back_ref[keep])
     # fp32 reference of the op: dequantised values stay within the E4M3 error bound
-    err = (out.float() - x.float()).abs().view(-1, 32).amax(dim=1)
-    assert bool((err <= x.float().abs().view(-1, 32).amax(dim=1) * 2 ** -3 + 1e-30).all())
+    err = (out[:nx].float() - x[:nx].float()).abs().view(-1, 32).amax(dim=1)
+    assert bool((err <= x[:nx].float().abs().view(-1, 32).amax(dim=1) * 2 ** -3 + 1e-30).all())
 
 
 @pytest.mark.gpu
