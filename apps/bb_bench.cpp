@@ -180,21 +180,35 @@ int main(int argc, char** argv) {
     // reaches it over the same-host shared-memory channel), synthetic GPU pools, and a transport whose transfers are free.
     // What is left is exactly what bounds batches of small objects: Keystone round trips + the client's own per-object work.
     struct NullTransport : client::DeviceTransport {
-      ErrorCode put_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>&, ChecksumAlgo, void*,
-                           std::vector<uint64_t>* digests) override {
-        if (digests) digests->assign(ops.size(), 0x1234);
-        ++n;
+      // ticket = launch number; the batch's op count is all wait_* needs
+      Result<uint64_t> submit_put(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>&, ChecksumAlgo,
+                                  void*) override {
+        return submit(ops.size());
+      }
+      ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override {
+        if (digests) digests->assign(take(ticket), 0x1234);
         return ErrorCode::OK;
       }
-      ErrorCode get_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>&, ChecksumAlgo, void*,
-                           std::vector<uint32_t>* status) override {
-        if (status) status->assign(ops.size(), 0);
-        ++n;
+      Result<uint64_t> submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>&, void*) override {
+        return submit(ops.size());
+      }
+      ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override {
+        if (status) status->assign(take(ticket), 0);
         return ErrorCode::OK;
       }
       bool can_reach(const ShardPlacement&) const override { return true; }
       uint64_t launches() const override { return n; }
+      uint64_t submit(size_t nops) {
+        nops_of[++n] = nops;
+        return n;
+      }
+      size_t take(uint64_t ticket) {
+        const size_t nops = nops_of[ticket];
+        nops_of.erase(ticket);
+        return nops;
+      }
       uint64_t n = 0;
+      std::map<uint64_t, size_t> nops_of;
     };
     const int batch = std::max(1, static_cast<int>(args.num("batch", 4096)));
     const int iters = std::max(1, static_cast<int>(args.num("iterations", 20)));

@@ -1272,7 +1272,8 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
     if (ops.empty()) break;
     metrics_.inc("replica_failover_total");
     std::vector<uint32_t> status;
-    ErrorCode ec = device_->get_shards(ops, dev_ptrs, ChecksumAlgo::NONE, stream, &status);
+    auto t = device_->submit_get(ops, dev_ptrs, stream);
+    ErrorCode ec = t.ok() ? device_->wait_get(t.value(), &status) : t.error();
     if (ec != ErrorCode::OK) {
       for (size_t i = 0; i < keys.size(); ++i)
         if (pending[i]) {
@@ -1337,36 +1338,55 @@ bool HostLoopbackTransport::can_reach(const ShardPlacement& s) const {
   return reach_disk_ || !is_disk_class(s.storage_class);
 }
 
-ErrorCode HostLoopbackTransport::put_shards(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
-                                            void*, std::vector<uint64_t>* digests) {
+Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs,
+                                                   ChecksumAlgo algo, void*) {
   ++launches_;  // one "launch" per batch, like the fused kernel
-  if (digests) digests->assign(ops.size(), 0);
+  std::vector<uint64_t> digests(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     const auto* src = static_cast<const uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
-    uint64_t d = 0;
-    ErrorCode ec = io_->write_shard(*op.placement, src, &d, algo);
+    ErrorCode ec = io_->write_shard(*op.placement, src, &digests[k], algo);
     for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], src, nullptr, ChecksumAlgo::NONE);
     if (ec != ErrorCode::OK) return ec;
-    if (digests) (*digests)[k] = d;
   }
-  return ErrorCode::OK;
+  std::lock_guard<std::mutex> lk(done_mu_);
+  done_[next_ticket_].first = std::move(digests);
+  return next_ticket_++;
 }
 
-ErrorCode HostLoopbackTransport::get_shards(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo, void*,
-                                            std::vector<uint32_t>* status) {
+Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void*) {
   ++launches_;
-  if (status) status->assign(ops.size(), 0);
+  std::vector<uint32_t> status(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     auto* dst = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
     const ErrorCode ec = io_->read_shard(*op.placement, dst, op.placement->checksum_algo);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
-      if (status) (*status)[k] = 1;  // reported per shard, like the kernel's verify flag
+      status[k] = 1;  // reported per shard, like the kernel's verify flag
     } else if (ec != ErrorCode::OK) {
       return ec;
     }
   }
+  std::lock_guard<std::mutex> lk(done_mu_);
+  done_[next_ticket_].second = std::move(status);
+  return next_ticket_++;
+}
+
+ErrorCode HostLoopbackTransport::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
+  std::lock_guard<std::mutex> lk(done_mu_);
+  auto it = done_.find(ticket);
+  if (it == done_.end()) return ErrorCode::NOT_FOUND;
+  if (digests) *digests = std::move(it->second.first);
+  done_.erase(it);
+  return ErrorCode::OK;
+}
+
+ErrorCode HostLoopbackTransport::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
+  std::lock_guard<std::mutex> lk(done_mu_);
+  auto it = done_.find(ticket);
+  if (it == done_.end()) return ErrorCode::NOT_FOUND;
+  if (status) *status = std::move(it->second.second);
+  done_.erase(it);
   return ErrorCode::OK;
 }
 

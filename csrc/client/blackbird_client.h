@@ -70,44 +70,16 @@ struct DeviceFp8Op {
 class DeviceTransport {
  public:
   virtual ~DeviceTransport() = default;
-  // dev_ptrs[item] is the client's device buffer of object `item`.
-  virtual ErrorCode put_shards(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs,
-                               ChecksumAlgo algo, void* stream, std::vector<uint64_t>* digests) = 0;
-  virtual ErrorCode get_shards(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo algo,
-                               void* stream, std::vector<uint32_t>* status) = 0;
   virtual bool can_reach(const ShardPlacement& s) const = 0;
   virtual uint64_t launches() const = 0;
-  // Asynchronous variants: enqueue the fused launch and return a ticket, so the caller can overlap
-  // control-plane round trips of the next chunk with this chunk's transfer.  Default = synchronous.
+  // submit_* enqueues a batch and returns a ticket, so the caller can overlap control-plane round trips of the next chunk
+  // with this one's transfer; wait_* blocks until it is done.  dev_ptrs[item] is the device buffer of object `item`.  A
+  // put returns one digest per op; a get verifies each shard with its placement's algorithm (status per op, 0 = ok).
   virtual Result<uint64_t> submit_put(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
-                                      void* stream) {
-    std::vector<uint64_t> d;
-    ErrorCode ec = put_shards(ops, dev_ptrs, algo, stream, &d);
-    if (ec != ErrorCode::OK) return ec;
-    sync_results_[++sync_ticket_] = {std::move(d), {}};
-    return sync_ticket_;
-  }
-  virtual ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
-    auto it = sync_results_.find(ticket);
-    if (it == sync_results_.end()) return ErrorCode::NOT_FOUND;
-    if (digests) *digests = std::move(it->second.first);
-    sync_results_.erase(it);
-    return ErrorCode::OK;
-  }
-  virtual Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) {
-    std::vector<uint32_t> st;
-    ErrorCode ec = get_shards(ops, dev_ptrs, ChecksumAlgo::NONE, stream, &st);
-    if (ec != ErrorCode::OK) return ec;
-    sync_results_[++sync_ticket_] = {{}, std::move(st)};
-    return sync_ticket_;
-  }
-  virtual ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
-    auto it = sync_results_.find(ticket);
-    if (it == sync_results_.end()) return ErrorCode::NOT_FOUND;
-    if (status) *status = std::move(it->second.second);
-    sync_results_.erase(it);
-    return ErrorCode::OK;
-  }
+                                      void* stream) = 0;
+  virtual ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) = 0;
+  virtual Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) = 0;
+  virtual ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) = 0;
   // True when the shard lives in this client's own device memory (a get from it never leaves the GPU).
   virtual bool is_local(const ShardPlacement& s) const { return false; }
   virtual size_t max_in_flight() const { return 1; }
@@ -121,10 +93,6 @@ class DeviceTransport {
   // Staging copies for objects (or shards) that live on host tiers: device <-> host buffer, synchronous.
   virtual ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
   virtual ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
-
- private:
-  uint64_t sync_ticket_ = 0;
-  std::map<uint64_t, std::pair<std::vector<uint64_t>, std::vector<uint32_t>>> sync_results_;
 };
 
 class HostLoopbackTransport;
@@ -234,10 +202,12 @@ class HostLoopbackTransport : public DeviceTransport {
   // `io` moves the bytes (its own connections / shared-memory mappings); it must outlive the transport.
   explicit HostLoopbackTransport(std::shared_ptr<BlackbirdClient> io, bool reach_disk_tiers = false)
       : io_(std::move(io)), reach_disk_(reach_disk_tiers) {}
-  ErrorCode put_shards(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo, void* stream,
-                       std::vector<uint64_t>* digests) override;
-  ErrorCode get_shards(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo algo, void* stream,
-                       std::vector<uint32_t>* status) override;
+  // Synchronous: submit_* moves the shards and keeps the result under the ticket it returns.
+  Result<uint64_t> submit_put(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
+                              void* stream) override;
+  ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override;
+  Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) override;
+  ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
   bool can_reach(const ShardPlacement& s) const override;
   uint64_t launches() const override { return launches_; }
   ErrorCode copy_h2d(void* dev, const void* host, size_t n, void*) override {
@@ -259,6 +229,9 @@ class HostLoopbackTransport : public DeviceTransport {
   std::shared_ptr<BlackbirdClient> io_;
   bool reach_disk_;
   std::atomic<uint64_t> launches_{0};
+  std::mutex done_mu_;
+  uint64_t next_ticket_ = 1;
+  std::map<uint64_t, std::pair<std::vector<uint64_t>, std::vector<uint32_t>>> done_;  // ticket -> (put digests, get status)
 };
 
 }  // namespace bb::client

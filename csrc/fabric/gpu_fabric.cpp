@@ -4,6 +4,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstring>
 
 #include "common/log.h"
@@ -157,21 +158,27 @@ ErrorCode GpuSlabBackend::device_copy(worker::StorageBackend& peer, bool to_peer
   if ((reinterpret_cast<uintptr_t>(mine) | reinterpret_cast<uintptr_t>(theirs)) & 15) return ErrorCode::NOT_IMPLEMENTED;  // staged path handles it
   std::lock_guard<std::mutex> lk(move_mu_);
   if (!cuda_ok(cudaSetDevice(opts_.gpu_device_id), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
+  return to_peer ? move_shard(mine, theirs, len, algo, digest, bytes_read_) : move_shard(theirs, mine, len, algo, digest, bytes_written_);
+}
+
+// One shard through the fused kernel on the tier-move engine; `moved` is the byte counter of its direction.  The caller
+// holds move_mu_ and has made the slab's device current.
+ErrorCode GpuSlabBackend::move_shard(const void* src, void* dst, uint64_t len, ChecksumAlgo algo, uint64_t* digest,
+                                     std::atomic<uint64_t>& moved) {
   if (!move_engine_) {
     auto e = XferEngine::create(opts_.gpu_device_id, 64, 1);
     if (!e.ok()) return e.error();
     move_engine_ = std::move(e.value());
   }
   XferItem it;
-  it.src = to_peer ? mine : theirs;
-  it.dst[0] = to_peer ? theirs : mine;
+  it.src = src;
+  it.dst[0] = dst;
   it.ndst = 1;
   it.nbytes = len;
   XferResult res;
-  ErrorCode ec = move_engine_->run({it}, algo, stream_, &res);
-  if (ec != ErrorCode::OK) return ec;
+  BB_TRY(move_engine_->run({it}, algo, stream_, &res));
   if (digest) *digest = res.digest.empty() ? 0 : res.digest[0];
-  (to_peer ? bytes_read_ : bytes_written_) += len;
+  moved += len;
   ++device_copies_;
   return ErrorCode::OK;
 }
@@ -202,23 +209,7 @@ ErrorCode GpuSlabBackend::pull_from_peer(const std::vector<uint8_t>& peer_key, u
   uint8_t* theirs = static_cast<uint8_t*>(peer_base) + peer_off;
   uint8_t* mine = base_ + my_off;
   if ((reinterpret_cast<uintptr_t>(mine) | reinterpret_cast<uintptr_t>(theirs)) & 15) return ErrorCode::NOT_IMPLEMENTED;
-  if (!move_engine_) {
-    auto e = XferEngine::create(opts_.gpu_device_id, 64, 1);
-    if (!e.ok()) return e.error();
-    move_engine_ = std::move(e.value());
-  }
-  XferItem item;
-  item.src = theirs;
-  item.dst[0] = mine;
-  item.ndst = 1;
-  item.nbytes = len;
-  XferResult res;
-  ErrorCode ec = move_engine_->run({item}, algo, stream_, &res);
-  if (ec != ErrorCode::OK) return ec;
-  if (digest) *digest = res.digest.empty() ? 0 : res.digest[0];
-  bytes_written_ += len;
-  ++device_copies_;
-  return ErrorCode::OK;
+  return move_shard(theirs, mine, len, algo, digest, bytes_written_);
 }
 
 void install_gpu_backend_factory() {
@@ -606,21 +597,25 @@ Result<uint64_t> GpuFabric::submit_put(const std::vector<client::DeviceShardOp>&
   return t.value();
 }
 
-ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
-  BB_TRACE_SPAN("fabric.wait_put");
-  InFlight fl;
+// Takes the bookkeeping of an in-flight batch and waits for its engine ticket.
+ErrorCode GpuFabric::finish(uint64_t ticket, InFlight* fl, XferResult* res) {
   {
     std::lock_guard<std::mutex> lk(mu_);
     auto it = inflight_.find(ticket);
     if (it == inflight_.end()) return ErrorCode::NOT_FOUND;
-    fl = std::move(it->second);
+    *fl = std::move(it->second);
     inflight_.erase(it);
   }
+  BB_TRY(engine_->wait(ticket, res));
+  note_device_ms(res->device_ms);
+  return ErrorCode::OK;
+}
+
+ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
+  BB_TRACE_SPAN("fabric.wait_put");
+  InFlight fl;
   XferResult res;
-  ErrorCode ec = engine_->wait(ticket, &res);
-  if (ec != ErrorCode::OK) return ec;
-  last_ms_ = res.device_ms;
-  total_ms_ += res.device_ms;
+  BB_TRY(finish(ticket, &fl, &res));
   if (digests) {
     digests->assign(fl.nops, 0);
     for (size_t i = fl.op_of_item.size(); i-- > 0;) (*digests)[fl.op_of_item[i]] = res.digest[i];
@@ -628,8 +623,7 @@ ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) {
-  BB_TRACE_SPAN("fabric.put_fp8", ops.size());
+ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, XferResult* res) {
   std::vector<Fp8Item> items;
   items.reserve(ops.size());
   for (const auto& op : ops) {
@@ -639,146 +633,102 @@ ErrorCode GpuFabric::put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* 
     it.wide = op.wide;
     it.packed = d.value();
     it.n_elems = op.n_elems;
-    if (op.replicas.size() + 1 > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
-    for (const ShardPlacement* rp : op.replicas) {
-      auto dr = resolve(*rp);
-      if (!dr.ok()) return dr.error();
-      it.more_packed[it.nreplicas - 1] = dr.value();
-      ++it.nreplicas;
+    if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
+      it.expect = op.placement->checksum;
+      it.verify = true;
+    } else {  // put: the same tile pass writes every replica
+      if (op.replicas.size() + 1 > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
+      for (const ShardPlacement* rp : op.replicas) {
+        auto dr = resolve(*rp);
+        if (!dr.ok()) return dr.error();
+        it.more_packed[it.nreplicas - 1] = dr.value();
+        ++it.nreplicas;
+      }
     }
     items.push_back(it);
   }
+  BB_TRY(engine_->run_fp8(items, unpack, stream, res));
+  note_device_ms(res->device_ms);
+  return ErrorCode::OK;
+}
+
+ErrorCode GpuFabric::put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) {
+  BB_TRACE_SPAN("fabric.put_fp8", ops.size());
   XferResult res;
-  ErrorCode ec = engine_->run_fp8(items, false, stream, &res);
-  if (ec != ErrorCode::OK) return ec;
-  last_ms_ = res.device_ms;
-  total_ms_ += res.device_ms;
+  BB_TRY(transfer_fp8(ops, false, stream, &res));
   if (digests) *digests = std::move(res.digest);
   return ErrorCode::OK;
 }
 
 ErrorCode GpuFabric::get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) {
   BB_TRACE_SPAN("fabric.get_fp8", ops.size());
-  std::vector<Fp8Item> items;
-  items.reserve(ops.size());
-  for (const auto& op : ops) {
-    auto d = resolve(*op.placement);
-    if (!d.ok()) return d.error();
-    Fp8Item it;
-    it.wide = op.wide;
-    it.packed = d.value();
-    it.n_elems = op.n_elems;
-    it.expect = op.placement->checksum;
-    it.verify = true;
-    items.push_back(it);
-  }
   XferResult res;
-  ErrorCode ec = engine_->run_fp8(items, true, stream, &res);
-  if (ec != ErrorCode::OK) return ec;
-  last_ms_ = res.device_ms;
-  total_ms_ += res.device_ms;
+  BB_TRY(transfer_fp8(ops, true, stream, &res));
   if (status) *status = std::move(res.status);
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::put_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
-                                void* stream, std::vector<uint64_t>* digests) {
-  auto t = submit_put(ops, dev_ptrs, algo, stream);
-  if (!t.ok()) return t.error();
-  return wait_put(t.value(), digests);
-}
-
-Result<uint64_t> GpuFabric::submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) {
-  BB_TRACE_SPAN("fabric.submit_get");
-  bool uniform = true;
-  for (const auto& op : ops) uniform &= op.placement->checksum_algo == ops[0].placement->checksum_algo;
-  InFlight fl;
-  fl.nops = ops.size();
-  if (!uniform || ops.empty()) {  // rare: objects written with different checksum algorithms in one batch
-    fl.sync_done = true;
-    ErrorCode ec = get_shards(ops, dev_ptrs, ChecksumAlgo::NONE, stream, &fl.sync_status);
-    if (ec != ErrorCode::OK) return ec;
-    std::lock_guard<std::mutex> lk(mu_);
-    const uint64_t t = next_sync_ticket_++;
-    inflight_[t] = std::move(fl);
-    return t;
-  }
-  const ChecksumAlgo algo = ops[0].placement->checksum_algo;
-  std::vector<XferItem> items;
-  items.reserve(ops.size());
-  for (const auto& op : ops) {
-    XferItem it;
+// Get descriptors of the ops whose objects were written with `algo`, in op order.
+ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo algo,
+                                     std::vector<XferItem>* items, std::vector<size_t>* op_of_item) {
+  items->reserve(ops.size());
+  op_of_item->reserve(ops.size());
+  for (size_t k = 0; k < ops.size(); ++k) {
+    const auto& op = ops[k];
+    if (op.placement->checksum_algo != algo) continue;
     auto s = resolve(*op.placement);
     if (!s.ok()) return s.error();
+    XferItem it;
     it.src = s.value();
     it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
     it.ndst = 1;
     it.nbytes = op.placement->length;
     it.expect = op.placement->checksum;
     it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
-    items.push_back(it);
+    items->push_back(it);
+    op_of_item->push_back(k);
     count(false, classify(*op.placement), it.nbytes);
   }
-  auto t = engine_->submit(items, algo, stream);
-  if (!t.ok()) return t.error();
-  std::lock_guard<std::mutex> lk(mu_);
-  inflight_[t.value()] = std::move(fl);
-  return t.value();
+  return ErrorCode::OK;
+}
+
+Result<uint64_t> GpuFabric::submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) {
+  BB_TRACE_SPAN("fabric.submit_get");
+  std::vector<ChecksumAlgo> algos;  // in order of first appearance
+  for (const auto& op : ops)
+    if (std::find(algos.begin(), algos.end(), op.placement->checksum_algo) == algos.end()) algos.push_back(op.placement->checksum_algo);
+  if (algos.empty()) algos.push_back(ChecksumAlgo::NONE);
+  InFlight fl;
+  fl.nops = ops.size();
+  for (size_t g = 0;; ++g) {
+    std::vector<XferItem> items;
+    fl.op_of_item.clear();
+    BB_TRY(build_get_items(ops, dev_ptrs, algos[g], &items, &fl.op_of_item));
+    auto t = engine_->submit(items, algos[g], stream);
+    if (!t.ok()) return t.error();
+    if (g + 1 == algos.size()) {
+      std::lock_guard<std::mutex> lk(mu_);
+      inflight_[t.value()] = std::move(fl);
+      return t.value();
+    }
+    // rare: objects written with different checksum algorithms in one batch
+    XferResult res;
+    BB_TRY(engine_->wait(t.value(), &res));
+    note_device_ms(res.device_ms);
+    fl.status.resize(ops.size(), 0);
+    for (size_t i = 0; i < fl.op_of_item.size(); ++i) fl.status[fl.op_of_item[i]] = res.status[i];
+  }
 }
 
 ErrorCode GpuFabric::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
   BB_TRACE_SPAN("fabric.wait_get");
   InFlight fl;
-  {
-    std::lock_guard<std::mutex> lk(mu_);
-    auto it = inflight_.find(ticket);
-    if (it == inflight_.end()) return ErrorCode::NOT_FOUND;
-    fl = std::move(it->second);
-    inflight_.erase(it);
-  }
-  if (fl.sync_done) {
-    if (status) *status = std::move(fl.sync_status);
-    return ErrorCode::OK;
-  }
   XferResult res;
-  ErrorCode ec = engine_->wait(ticket, &res);
-  if (ec != ErrorCode::OK) return ec;
-  last_ms_ = res.device_ms;
-  total_ms_ += res.device_ms;
-  if (status) *status = std::move(res.status);
-  return ErrorCode::OK;
-}
-
-ErrorCode GpuFabric::get_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo,
-                                void* stream, std::vector<uint32_t>* status) {
-  if (status) status->assign(ops.size(), 0);
-  // one launch per checksum algorithm present in the batch (normally exactly one)
-  for (ChecksumAlgo algo : {ChecksumAlgo::XXH3, ChecksumAlgo::BBH64, ChecksumAlgo::CRC32C, ChecksumAlgo::NONE}) {
-    std::vector<XferItem> items;
-    std::vector<size_t> idx;
-    for (size_t k = 0; k < ops.size(); ++k) {
-      const auto& op = ops[k];
-      if (op.placement->checksum_algo != algo) continue;
-      XferItem it;
-      auto s = resolve(*op.placement);
-      if (!s.ok()) return s.error();
-      it.src = s.value();
-      it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
-      it.ndst = 1;
-      it.nbytes = op.placement->length;
-      it.expect = op.placement->checksum;
-      it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
-      items.push_back(it);
-      idx.push_back(k);
-    }
-    if (items.empty()) continue;
-    XferResult res;
-    ErrorCode ec = engine_->run(items, algo, stream, &res);
-    if (ec != ErrorCode::OK) return ec;
-    last_ms_ = res.device_ms;
-  total_ms_ += res.device_ms;
-    if (status)
-      for (size_t i = 0; i < idx.size(); ++i) (*status)[idx[i]] = res.status[i];
+  BB_TRY(finish(ticket, &fl, &res));
+  if (status) {
+    *status = std::move(fl.status);
+    status->resize(fl.nops, 0);
+    for (size_t i = 0; i < fl.op_of_item.size(); ++i) (*status)[fl.op_of_item[i]] = res.status[i];
   }
   return ErrorCode::OK;
 }

@@ -53,6 +53,7 @@ class GpuSlabBackend : public worker::StorageBackend {
   std::string registration_key_hex() const override { return handle_hex_; }
 
  private:
+  ErrorCode move_shard(const void* src, void* dst, uint64_t len, ChecksumAlgo algo, uint64_t* digest, std::atomic<uint64_t>& moved);
   uint8_t* base_ = nullptr;
   uint64_t rkey_ = 0;
   std::string handle_hex_;
@@ -70,16 +71,14 @@ class GpuFabric : public client::DeviceTransport {
   static Result<std::shared_ptr<GpuFabric>> create(int device, std::shared_ptr<rpc::KeystoneApi> keystone);
   ~GpuFabric() override;
 
-  ErrorCode put_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
-                       void* stream, std::vector<uint64_t>* digests) override;
-  ErrorCode get_shards(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo algo, void* stream,
-                       std::vector<uint32_t>* status) override;
   bool can_reach(const ShardPlacement& s) const override;
   bool is_local(const ShardPlacement& s) const override;
   uint64_t launches() const override { return engine_->launches(); }
   Result<uint64_t> submit_put(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
                               void* stream) override;
   ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override;
+  // One engine batch per checksum algorithm in `ops` (normally exactly one).  A batch that mixes algorithms runs all
+  // groups but the last to completion before returning, so it never holds more than one engine slot.
   Result<uint64_t> submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) override;
   ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
   size_t max_in_flight() const override { return 3; }
@@ -130,14 +129,20 @@ class GpuFabric : public client::DeviceTransport {
   Result<void*> resolve(const ShardPlacement& s);
   ErrorCode build_put_items(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs,
                             std::vector<XferItem>* items, std::vector<size_t>* op_of_item);
+  ErrorCode build_get_items(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, ChecksumAlgo algo,
+                            std::vector<XferItem>* items, std::vector<size_t>* op_of_item);
   struct InFlight {
     size_t nops = 0;
-    std::vector<size_t> op_of_item;       // put: item -> op
-    bool sync_done = false;               // mixed-algorithm get handled synchronously
-    std::vector<uint32_t> sync_status;
+    std::vector<size_t> op_of_item;  // item -> op
+    std::vector<uint32_t> status;    // get: per op, from the groups of a mixed batch that finished in submit_get
   };
+  ErrorCode finish(uint64_t ticket, InFlight* fl, XferResult* res);
+  ErrorCode transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, XferResult* res);
+  void note_device_ms(float ms) {
+    last_ms_ = ms;
+    total_ms_ += ms;
+  }
   std::map<uint64_t, InFlight> inflight_;  // engine ticket -> bookkeeping
-  uint64_t next_sync_ticket_ = 1ull << 62;
   int device_ = 0;
   std::shared_ptr<rpc::KeystoneApi> keystone_;
   std::unique_ptr<XferEngine> engine_;

@@ -13,17 +13,39 @@
 
 namespace bb::gpu {
 
-#define BB_CUDA(expr)                                                                      \
-  do {                                                                                     \
-    cudaError_t _e = (expr);                                                               \
-    if (_e != cudaSuccess) {                                                               \
-      BB_LOG(ERROR) << "CUDA error " << cudaGetErrorString(_e) << " (" << static_cast<int>(_e) << ") at " #expr; \
-      last_cuda_error_ = static_cast<int>(_e);                                             \
-      return ErrorCode::FABRIC_ERROR;                                                      \
-    }                                                                                      \
+// Logs a failed CUDA call and returns FABRIC_ERROR.  Inside XferEngine's members `cuda_failed` is the member, which also
+// keeps the code for last_cuda_error(); in the free helpers below it is the namespace-level function.
+#define BB_CUDA(expr)                                                        \
+  do {                                                                       \
+    const cudaError_t _e = (expr);                                           \
+    if (_e != cudaSuccess) return cuda_failed(static_cast<int>(_e), #expr);  \
   } while (0)
 
+static ErrorCode cuda_failed(int code, const char* what) {
+  BB_LOG(ERROR) << "CUDA error " << cudaGetErrorString(static_cast<cudaError_t>(code)) << " (" << code << ") at " << what;
+  return ErrorCode::FABRIC_ERROR;
+}
+
+ErrorCode XferEngine::cuda_failed(int code, const char* what) {
+  last_cuda_error_ = code;
+  return gpu::cuda_failed(code, what);
+}
+
+namespace {
+// Frees a slot when the call that holds it returns, whichever way it returns.
+struct SlotRelease {
+  uint64_t& ticket;
+  ~SlotRelease() { ticket = 0; }
+};
+}  // namespace
+
 struct XferEngine::Slot {
+  // How wait() learns that the batch has finished (chosen in submit()).
+  enum class Completion {
+    EVENTS,   // CUDA events: timing events around the launch, a completion event after the result copies
+    FLAG,     // the kernel's status words in pinned memory; no event on the stream (small-object latency path)
+    MAILBOX,  // served by the resident mailbox warp: results arrive in the mailbox's result ring
+  };
   // host (pinned): [descs | tile_start]
   uint8_t* h_tab = nullptr;
   // device
@@ -39,10 +61,9 @@ struct XferEngine::Slot {
   uint64_t* d_trace = nullptr;
   size_t d_trace_bytes = 0;
   bool traced = false;
-  bool mailed = false;     // served by the resident mailbox warp: results arrive in the mailbox's result ring
-  uint32_t mail_first = 0;  // first sequence number of this batch in the mailbox
-  bool flagged = false;    // completion by status flag in pinned memory (small-object latency path), no events recorded
-  void* stream = nullptr;  // stream of a flagged batch (fallback sync)
+  Completion completion = Completion::EVENTS;
+  uint32_t mail_first = 0;  // MAILBOX: first sequence number of this batch in the mailbox
+  void* stream = nullptr;   // FLAG: stream of the batch (fallback sync)
   cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_done = nullptr;
   uint64_t ticket = 0;  // 0 = free
   uint32_t nitems = 0;
@@ -143,11 +164,7 @@ ErrorCode XferEngine::mailbox_launch_locked(uint32_t first_seq) {
   Mailbox& m = *mb_;
   ++m.epoch;
   const int rc = launch_mailbox(m.slots, m.results, m.ctl, first_seq, m.epoch, m.linger_ns, m.max_ns, m.stream);
-  if (rc != 0) {
-    last_cuda_error_ = rc;
-    BB_LOG(ERROR) << "launch_mailbox failed: " << cuda_error_string(rc);
-    return ErrorCode::FABRIC_ERROR;
-  }
+  if (rc != 0) return cuda_failed(rc, "launch_mailbox");
   ++mailbox_launches_;
   ++launches_;
   return ErrorCode::OK;
@@ -242,135 +259,150 @@ bool XferEngine::small_path_enabled() {
   return on && small_path_;
 }
 
+XferEngine::Slot* XferEngine::free_slot() {
+  for (auto& c : slots_)
+    if (c->ticket == 0) return c.get();
+  return nullptr;
+}
+
+// Completes the slot's pinned table for the `nd` descriptors at its start, [descs | tile_start]: every descriptor's
+// first_tile and the nd + 1 tile_start prefix sums behind the descriptors.
+ErrorCode XferEngine::write_tile_table(Slot* s, uint32_t nd) {
+  auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
+  auto* tile_start = reinterpret_cast<uint32_t*>(s->h_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
+  uint64_t tiles = 0;
+  for (uint32_t i = 0; i < nd; ++i) {
+    descs[i].first_tile = tile_start[i] = static_cast<uint32_t>(tiles);
+    tiles += (descs[i].nbytes + kTileBytes - 1) / kTileBytes;
+    if (tiles > 0xFFFFFFF0ull) return ErrorCode::VALUE_OUT_OF_RANGE;
+  }
+  tile_start[nd] = static_cast<uint32_t>(tiles);
+  s->ndesc = nd;
+  s->total_tiles = static_cast<uint32_t>(tiles);
+  return ErrorCode::OK;
+}
+
 Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream,
                                     bool capture_debug) {
   if (items.size() > max_items_) return ErrorCode::RESOURCE_EXHAUSTED;
-  // pick a free slot (or recycle the oldest finished one)
-  Slot* s = nullptr;
-  for (auto& c : slots_)
-    if (c->ticket == 0) { s = c.get(); break; }
+  Slot* s = free_slot();
   if (!s) return ErrorCode::RESOURCE_EXHAUSTED;  // caller must wait() on outstanding tickets
-
-  auto run = [&]() -> ErrorCode {
-    BB_CUDA(cudaSetDevice(device_));
-    auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
-    s->item_to_desc.assign(items.size(), -1);
-    uint32_t nd = 0, tiles = 0;
-    bool all_small = small_path_enabled();
-    for (size_t i = 0; i < items.size(); ++i) {
-      const XferItem& it = items[i];
-      if (it.nbytes == 0) continue;
-      all_small = all_small && it.nbytes <= kSmallBytes && !(it.flags & XFER_RAW_SUM) && it.ndst >= 1;
-      if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
-      uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
-      for (uint32_t r = 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
-      if (al & 15) return ErrorCode::INVALID_ADDRESS;
-      if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
-      XferDesc& d = descs[nd];
-      d.src = it.src;
-      for (uint32_t r = 0; r < kMaxDst; ++r) d.dst[r] = r < it.ndst ? it.dst[r] : nullptr;
-      d.nbytes = it.nbytes;
-      d.first_tile = tiles;
-      d.ndst = it.ndst;
-      d.expect = it.expect;
-      d.flags = it.flags;
-      d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
-      if (algo == ChecksumAlgo::CRC32C) {
-        d.expect = (static_cast<uint64_t>(crc_init_term_for(it.nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
-        d.reserved = crc_unpad_for(it.nbytes);
-      }
-      s->item_to_desc[i] = static_cast<int32_t>(nd);
-      const uint64_t nt = (it.nbytes + kTileBytes - 1) / kTileBytes;
-      if (tiles + nt > 0xFFFFFFF0ull) return ErrorCode::VALUE_OUT_OF_RANGE;
-      tiles += static_cast<uint32_t>(nt);
-      ++nd;
+  BB_CUDA(cudaSetDevice(device_));
+  auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
+  s->item_to_desc.assign(items.size(), -1);
+  uint32_t nd = 0;
+  bool all_small = small_path_enabled();
+  for (size_t i = 0; i < items.size(); ++i) {
+    const XferItem& it = items[i];
+    if (it.nbytes == 0) continue;
+    all_small = all_small && it.nbytes <= kSmallBytes && !(it.flags & XFER_RAW_SUM) && it.ndst >= 1;
+    if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
+    uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
+    for (uint32_t r = 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
+    if (al & 15) return ErrorCode::INVALID_ADDRESS;
+    if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
+    XferDesc& d = descs[nd];
+    d.src = it.src;
+    for (uint32_t r = 0; r < kMaxDst; ++r) d.dst[r] = r < it.ndst ? it.dst[r] : nullptr;
+    d.nbytes = it.nbytes;
+    d.ndst = it.ndst;
+    d.expect = it.expect;
+    d.flags = it.flags;
+    d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
+    if (algo == ChecksumAlgo::CRC32C) {
+      d.expect = (static_cast<uint64_t>(crc_init_term_for(it.nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
+      d.reserved = crc_unpad_for(it.nbytes);
     }
-    auto* tile_start = reinterpret_cast<uint32_t*>(s->h_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
-    for (uint32_t i = 0; i < nd; ++i) tile_start[i] = descs[i].first_tile;
-    tile_start[nd] = tiles;
-    s->nitems = static_cast<uint32_t>(items.size());
-    s->ndesc = nd;
-    s->total_tiles = tiles;
-    s->debug = capture_debug;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (nd) {
-      const size_t tab = static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
-      const bool inline_tab = nd <= kInlineDescs;
-      if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
-      if (capture_debug) {
-        const size_t need = static_cast<size_t>(tiles) * tchash::kRows * tchash::kN * 4;
-        if (need > s->d_debug_bytes) {
-          if (s->d_debug) cudaFree(s->d_debug);
-          BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->d_debug), need));
-          s->d_debug_bytes = need;
-        }
-      }
-      XferLaunch l;
-      l.descs = reinterpret_cast<const XferDesc*>(s->d_tab);
-      l.tile_start = reinterpret_cast<const uint32_t*>(s->d_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
-      l.ndesc = nd;
-      l.total_tiles = tiles;
-      l.sum_ws = s->d_sum;
-      l.done_ws = s->d_done;
-      // Small batches: the finalizer warp writes digests / status straight into the pinned result
-      // block (UVA), so the launch is the only operation on the stream.
-      const bool direct = nd <= kDirectResults;
-      l.digest_out = direct ? reinterpret_cast<uint64_t*>(s->h_res) : s->d_digest;
-      l.status_out = direct ? reinterpret_cast<uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8) : s->d_status;
-      if (inline_tab) {
-        l.host_descs = descs;
-        l.host_tile_start = tile_start;
-      }
-      l.debug_d = capture_debug ? s->d_debug : nullptr;
-      s->traced = tile_trace_;
-      if (tile_trace_) {
-        const size_t need = static_cast<size_t>(tiles) * 4 * sizeof(uint64_t);
-        if (need > s->d_trace_bytes) {
-          if (s->d_trace) cudaFree(s->d_trace);
-          BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->d_trace), need));
-          s->d_trace_bytes = need;
-        }
-        BB_CUDA(cudaMemsetAsync(s->d_trace, 0, need, st));
-        l.trace_d = s->d_trace;
-      }
-      l.algo = algo == ChecksumAlgo::BBH64 ? ALGO_BBH64 : algo == ChecksumAlgo::CRC32C ? ALGO_CRC32C : algo == ChecksumAlgo::XXH3 ? ALGO_XXH3 : ALGO_NONE;
-      l.max_ctas = max_ctas_;
-      l.stream = stream;
-      l.small_path = all_small;
-      // Latency path: a small batch whose results land in pinned memory completes by flag -- the launch is the ONLY
-      // stream operation (no timing events, no completion event: each costs about as much GPU time as the kernel).
-      // (1) resident mailbox warp: no launch at all.  The request bypasses `stream`, so everything already queued there
-      // must have finished (the caller's source data is ready), and only one mailed batch is in flight at a time.
-      if (all_small && direct && nd <= kMailSlots / 2 && !capture_debug && !tile_trace_ && mailbox_enabled() &&
-          (!mb_ || mb_->outstanding == 0)) {
-        bool simple = true;
-        for (uint32_t i = 0; i < nd; ++i) simple = simple && descs[i].ndst == 1 && !(descs[i].flags & XFER_MULTIMEM);
-        if (simple && cudaStreamQuery(st) == cudaSuccess) {
-          const ErrorCode mec = mailbox_post(s, descs, nd, l.algo);
-          if (mec != ErrorCode::OK) return mec;
-          s->mailed = true;
-          return ErrorCode::OK;
-        }
+    s->item_to_desc[i] = static_cast<int32_t>(nd++);
+  }
+  BB_TRY(write_tile_table(s, nd));
+  s->nitems = static_cast<uint32_t>(items.size());
+  s->debug = capture_debug;
+  s->traced = tile_trace_;
+  s->hashed = algo != ChecksumAlgo::NONE;
+  s->empty_digest = is_tile_sum(algo) ? tchash::finalize(0, 0) : 0;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int xalgo = algo == ChecksumAlgo::BBH64 ? ALGO_BBH64 : algo == ChecksumAlgo::CRC32C ? ALGO_CRC32C : algo == ChecksumAlgo::XXH3 ? ALGO_XXH3 : ALGO_NONE;
+  // Small batches: the finalizer warp writes digests / status straight into the pinned result block (UVA).
+  const bool direct = nd <= kDirectResults;
+
+  // Completion mode.  A small batch without diagnostics whose results land in pinned memory needs no CUDA event (each
+  // costs about as much GPU time as the kernel): the resident mailbox warp serves it without any launch, or else it
+  // completes by flag and the launch is the ONLY stream operation.  The mailbox request bypasses `stream`, so
+  // everything already queued there must have finished (the caller's source data is ready), and only one mailed batch
+  // is in flight at a time.
+  using Completion = Slot::Completion;
+  s->completion = Completion::EVENTS;
+  if (nd && all_small && direct && !capture_debug && !tile_trace_) {
+    if (nd <= kMailSlots / 2 && mailbox_enabled() && (!mb_ || mb_->outstanding == 0)) {
+      bool simple = true;
+      for (uint32_t i = 0; i < nd; ++i) simple = simple && descs[i].ndst == 1 && !(descs[i].flags & XFER_MULTIMEM);
+      if (simple && cudaStreamQuery(st) == cudaSuccess)
+        s->completion = Completion::MAILBOX;
+      else
         cudaGetLastError();  // cudaErrorNotReady is not sticky, but keep the error state clean
+    }
+    if (s->completion == Completion::EVENTS && flag_completion_enabled()) s->completion = Completion::FLAG;
+  }
+
+  if (s->completion == Completion::MAILBOX) {
+    BB_TRY(mailbox_post(s, descs, nd, xalgo));
+    s->ticket = next_ticket_++;
+    return s->ticket;
+  }
+  if (nd) {
+    const size_t tab = static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
+    const bool inline_tab = nd <= kInlineDescs;
+    if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
+    if (capture_debug) {
+      const size_t need = static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN * 4;
+      if (need > s->d_debug_bytes) {
+        if (s->d_debug) cudaFree(s->d_debug);
+        BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->d_debug), need));
+        s->d_debug_bytes = need;
       }
-      s->flagged = all_small && direct && !capture_debug && !tile_trace_ && flag_completion_enabled();
-      if (s->flagged) {
-        auto* stt = reinterpret_cast<volatile uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8);
-        for (uint32_t i = 0; i < nd; ++i) stt[i] = kSmallPending;
-        l.flag_completion = true;
-        s->stream = stream;
-      } else {
-        BB_CUDA(cudaEventRecord(s->ev_start, st));
+    }
+    XferLaunch l;
+    l.descs = reinterpret_cast<const XferDesc*>(s->d_tab);
+    l.tile_start = reinterpret_cast<const uint32_t*>(s->d_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
+    l.ndesc = nd;
+    l.total_tiles = s->total_tiles;
+    l.sum_ws = s->d_sum;
+    l.done_ws = s->d_done;
+    l.digest_out = direct ? reinterpret_cast<uint64_t*>(s->h_res) : s->d_digest;
+    l.status_out = direct ? reinterpret_cast<uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8) : s->d_status;
+    if (inline_tab) {
+      l.host_descs = descs;
+      l.host_tile_start = reinterpret_cast<const uint32_t*>(s->h_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
+    }
+    l.debug_d = capture_debug ? s->d_debug : nullptr;
+    if (tile_trace_) {
+      const size_t need = static_cast<size_t>(s->total_tiles) * 4 * sizeof(uint64_t);
+      if (need > s->d_trace_bytes) {
+        if (s->d_trace) cudaFree(s->d_trace);
+        BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&s->d_trace), need));
+        s->d_trace_bytes = need;
       }
-      const int rc = launch_xfer(l);
-      if (rc != 0) {
-        last_cuda_error_ = rc;
-        BB_LOG(ERROR) << "launch_xfer failed: " << cuda_error_string(rc);
-        return ErrorCode::FABRIC_ERROR;
-      }
-      ++launches_;
-      if (all_small && !capture_debug && !tile_trace_) ++small_launches_;
-      if (s->flagged) return ErrorCode::OK;
+      BB_CUDA(cudaMemsetAsync(s->d_trace, 0, need, st));
+      l.trace_d = s->d_trace;
+    }
+    l.algo = xalgo;
+    l.max_ctas = max_ctas_;
+    l.stream = stream;
+    l.small_path = all_small;
+    if (s->completion == Completion::FLAG) {
+      auto* stt = reinterpret_cast<volatile uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8);
+      for (uint32_t i = 0; i < nd; ++i) stt[i] = kSmallPending;
+      l.flag_completion = true;
+      s->stream = stream;
+    } else {
+      BB_CUDA(cudaEventRecord(s->ev_start, st));
+    }
+    const int rc = launch_xfer(l);
+    if (rc != 0) return cuda_failed(rc, "launch_xfer");
+    ++launches_;
+    if (all_small && !capture_debug && !tile_trace_) ++small_launches_;
+    if (s->completion == Completion::EVENTS) {
       BB_CUDA(cudaEventRecord(s->ev_stop, st));
       if (algo != ChecksumAlgo::NONE && !direct) {
         BB_CUDA(cudaMemcpyAsync(s->h_res, s->d_digest, static_cast<size_t>(nd) * 8, cudaMemcpyDeviceToHost, st));
@@ -378,16 +410,9 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
                                 cudaMemcpyDeviceToHost, st));
       }
     }
-    BB_CUDA(cudaEventRecord(s->ev_done, st));
-    return ErrorCode::OK;
-  };
-  s->flagged = false;
-  s->mailed = false;
-  ErrorCode ec = run();
-  if (ec != ErrorCode::OK) return ec;
+  }
+  if (s->completion == Completion::EVENTS) BB_CUDA(cudaEventRecord(s->ev_done, st));
   s->ticket = next_ticket_++;
-  s->hashed = algo != ChecksumAlgo::NONE;
-  s->empty_digest = is_tile_sum(algo) ? tchash::finalize(0, 0) : 0;
   return s->ticket;
 }
 
@@ -396,37 +421,38 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
   for (auto& c : slots_)
     if (c->ticket == ticket) { s = c.get(); break; }
   if (!s) return ErrorCode::NOT_FOUND;
+  SlotRelease release{s->ticket};
   const uint32_t nd = s->ndesc;
-  if (s->mailed) {
-    const ErrorCode mec = mailbox_wait(s);
-    if (mec != ErrorCode::OK) {
-      s->ticket = 0;
-      return mec;
-    }
-  } else if (s->flagged) {
-    // spin on the status words the kernel writes last (pinned memory); fall back to a stream sync if they do not show
-    // up within a generous bound, so that a launch failure surfaces as an error instead of a hang
-    const auto* stt = reinterpret_cast<const volatile uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8);
-    const auto t0 = std::chrono::steady_clock::now();
-    uint32_t done = 0, spins = 0;
-    while (done < nd) {
-      if (stt[done] != kSmallPending) {
-        ++done;
-        continue;
-      }
-      if ((++spins & 0x3FFu) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(200)) {
-        BB_CUDA(cudaSetDevice(device_));
-        BB_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(s->stream)));
-        if (stt[done] == kSmallPending) {
-          BB_LOG(ERROR) << "XferEngine: small-object kernel finished without publishing its results";
-          s->ticket = 0;
-          return ErrorCode::FABRIC_ERROR;
+  switch (s->completion) {
+    case Slot::Completion::MAILBOX:
+      BB_TRY(mailbox_wait(s));
+      break;
+    case Slot::Completion::FLAG: {
+      // spin on the status words the kernel writes last (pinned memory); fall back to a stream sync if they do not show
+      // up within a generous bound, so that a launch failure surfaces as an error instead of a hang
+      const auto* stt = reinterpret_cast<const volatile uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 8);
+      const auto t0 = std::chrono::steady_clock::now();
+      uint32_t done = 0, spins = 0;
+      while (done < nd) {
+        if (stt[done] != kSmallPending) {
+          ++done;
+          continue;
+        }
+        if ((++spins & 0x3FFu) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::milliseconds(200)) {
+          BB_CUDA(cudaSetDevice(device_));
+          BB_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(s->stream)));
+          if (stt[done] == kSmallPending) {
+            BB_LOG(ERROR) << "XferEngine: small-object kernel finished without publishing its results";
+            return ErrorCode::FABRIC_ERROR;
+          }
         }
       }
+      std::atomic_thread_fence(std::memory_order_acquire);
+      break;
     }
-    std::atomic_thread_fence(std::memory_order_acquire);
-  } else {
-    BB_CUDA(cudaEventSynchronize(s->ev_done));
+    case Slot::Completion::EVENTS:
+      BB_CUDA(cudaEventSynchronize(s->ev_done));
+      break;
   }
   const bool no_hash = !s->hashed;
   if (out) {
@@ -444,7 +470,7 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
       }
     }
     out->device_ms = 0.f;
-    if (nd && !s->flagged && !s->mailed) cudaEventElapsedTime(&out->device_ms, s->ev_start, s->ev_stop);
+    if (nd && s->completion == Slot::Completion::EVENTS) cudaEventElapsedTime(&out->device_ms, s->ev_start, s->ev_stop);
   }
   if (s->debug && nd) {
     debug_host_.resize(static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN);
@@ -454,26 +480,8 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
     trace_host_.resize(static_cast<size_t>(s->total_tiles) * 4);
     BB_CUDA(cudaMemcpy(trace_host_.data(), s->d_trace, trace_host_.size() * 8, cudaMemcpyDeviceToHost));
   }
-  s->ticket = 0;
   return ErrorCode::OK;
 }
-
-struct XferEngine::Fp8State {
-  uint8_t* h_tab = nullptr;
-  uint8_t* d_tab = nullptr;
-  uint64_t* d_sum = nullptr;
-  uint64_t* h_sum = nullptr;
-  uint32_t cap = 0;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  ~Fp8State() {
-    if (h_tab) cudaFreeHost(h_tab);
-    if (h_sum) cudaFreeHost(h_sum);
-    if (d_tab) cudaFree(d_tab);
-    if (d_sum) cudaFree(d_sum);
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-  }
-};
 
 ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, void* stream, XferResult* out) {
   const uint32_t n = static_cast<uint32_t>(items.size());
@@ -481,25 +489,13 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   if (n > max_items_) return ErrorCode::RESOURCE_EXHAUSTED;
   BB_CUDA(cudaSetDevice(device_));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!fp8_) fp8_ = std::make_unique<Fp8State>();
-  Fp8State& f = *fp8_;
-  if (f.cap < n) {
-    Fp8State fresh;
-    const uint32_t cap = std::max<uint32_t>(n, 256);
-    const size_t tab = static_cast<size_t>(cap) * sizeof(XferDesc) + (static_cast<size_t>(cap) + 1) * 4;
-    BB_CUDA(cudaMallocHost(reinterpret_cast<void**>(&fresh.h_tab), tab));
-    BB_CUDA(cudaMallocHost(reinterpret_cast<void**>(&fresh.h_sum), static_cast<size_t>(cap) * 8));
-    BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&fresh.d_tab), tab));
-    BB_CUDA(cudaMalloc(reinterpret_cast<void**>(&fresh.d_sum), static_cast<size_t>(cap) * 8));
-    BB_CUDA(cudaEventCreate(&fresh.ev0));
-    BB_CUDA(cudaEventCreate(&fresh.ev1));
-    fresh.cap = cap;
-    std::swap(f.h_tab, fresh.h_tab), std::swap(f.h_sum, fresh.h_sum), std::swap(f.d_tab, fresh.d_tab), std::swap(f.d_sum, fresh.d_sum);
-    std::swap(f.ev0, fresh.ev0), std::swap(f.ev1, fresh.ev1), std::swap(f.cap, fresh.cap);
-  }
-  auto* descs = reinterpret_cast<XferDesc*>(f.h_tab);
-  auto* tile_start = reinterpret_cast<uint32_t*>(f.h_tab + static_cast<size_t>(n) * sizeof(XferDesc));
-  uint32_t tiles = 0;
+  // The fused kernel's batch holds this slot for the whole call; the scales batch below takes a second one.  The slot's
+  // d_digest collects the payload sums (d_sum must stay zero between batches for bb_xfer).
+  Slot* s = free_slot();
+  if (!s) return ErrorCode::RESOURCE_EXHAUSTED;
+  s->ticket = next_ticket_++;
+  SlotRelease release{s->ticket};
+  auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
@@ -515,18 +511,14 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     d.dst[0] = unpack ? it.wide : static_cast<void*>(payload);  // pack: base of the packed object in every replica
     d.dst[1] = nrep > 1 ? it.more_packed[0] : nullptr;
     d.dst[2] = nrep > 2 ? it.more_packed[1] : nullptr;
-    d.nbytes = it.n_elems;
-    d.first_tile = tiles;
+    d.nbytes = it.n_elems;  // payload tiles, the last one possibly partial
     d.ndst = nrep;
     d.expect = 0;
     d.flags = 0;
     d.reserved = 0;
-    tile_start[i] = tiles;
-    const uint64_t nt = (it.n_elems + kTileBytes - 1) / kTileBytes;  // payload tiles, the last one possibly partial
-    const uint64_t nt_full = it.n_elems / kTileBytes;                // hashed by the fused kernel
-    if (tiles + nt > 0xFFFFFFF0ull) return ErrorCode::VALUE_OUT_OF_RANGE;
-    tiles += static_cast<uint32_t>(nt);
-    // everything past the last whole payload tile (payload tail + scales) is hashed from the stored bytes as a slice
+    // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
+    // stored bytes as a slice
+    const uint64_t nt_full = it.n_elems / kTileBytes;
     XferItem& sc = scale_items[i];
     sc.src = payload + nt_full * kTileBytes;
     sc.ndst = 0;
@@ -534,43 +526,39 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     sc.flags = XFER_RAW_SUM;
     sc.tile_base = static_cast<uint32_t>(nt_full);
   }
-  tile_start[n] = tiles;
+  BB_TRY(write_tile_table(s, n));
   const size_t tab = static_cast<size_t>(n) * sizeof(XferDesc) + (static_cast<size_t>(n) + 1) * 4;
-  BB_CUDA(cudaMemcpyAsync(f.d_tab, f.h_tab, tab, cudaMemcpyHostToDevice, st));
-  BB_CUDA(cudaMemsetAsync(f.d_sum, 0, static_cast<size_t>(n) * 8, st));
+  BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
+  BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;
-  l.descs = reinterpret_cast<const XferDesc*>(f.d_tab);
-  l.tile_start = reinterpret_cast<const uint32_t*>(f.d_tab + static_cast<size_t>(n) * sizeof(XferDesc));
+  l.descs = reinterpret_cast<const XferDesc*>(s->d_tab);
+  l.tile_start = reinterpret_cast<const uint32_t*>(s->d_tab + static_cast<size_t>(n) * sizeof(XferDesc));
   l.ndesc = n;
-  l.total_tiles = tiles;
-  l.sum_ws = f.d_sum;
+  l.total_tiles = s->total_tiles;
+  l.sum_ws = s->d_digest;
   l.max_ctas = max_ctas_;
   l.stream = stream;
-  BB_CUDA(cudaEventRecord(f.ev0, st));
+  BB_CUDA(cudaEventRecord(s->ev_start, st));
   const int rc = launch_xfer_fp8(l, unpack);
-  if (rc != 0) {
-    last_cuda_error_ = rc;
-    BB_LOG(ERROR) << "launch_xfer_fp8 failed: " << cuda_error_string(rc);
-    return ErrorCode::FABRIC_ERROR;
-  }
+  if (rc != 0) return cuda_failed(rc, "launch_xfer_fp8");
   ++launches_;
-  BB_CUDA(cudaEventRecord(f.ev1, st));
-  BB_CUDA(cudaMemcpyAsync(f.h_sum, f.d_sum, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, st));
+  BB_CUDA(cudaEventRecord(s->ev_stop, st));
+  BB_CUDA(cudaMemcpyAsync(s->h_res, s->d_digest, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, st));
   // scales: for a put they were just written by the kernel above (same stream), for a get they are read twice
   XferResult sres;
-  ErrorCode ec = run(scale_items, ChecksumAlgo::BBH64, stream, &sres);  // waits for the stream up to here
-  if (ec != ErrorCode::OK) return ec;
+  BB_TRY(run(scale_items, ChecksumAlgo::BBH64, stream, &sres));  // waits for the stream up to here
   BB_CUDA(cudaStreamSynchronize(st));
   if (out) {
+    const auto* sums = reinterpret_cast<const uint64_t*>(s->h_res);
     out->digest.assign(n, 0);
     out->status.assign(n, 0);
     for (uint32_t i = 0; i < n; ++i) {
       const uint64_t total = items[i].n_elems + items[i].n_elems / 32;
-      out->digest[i] = tchash::finalize(f.h_sum[i] + sres.digest[i], total);
+      out->digest[i] = tchash::finalize(sums[i] + sres.digest[i], total);
       if (items[i].verify && out->digest[i] != items[i].expect) out->status[i] = 1;
     }
     float ms = 0.f;
-    cudaEventElapsedTime(&ms, f.ev0, f.ev1);
+    cudaEventElapsedTime(&ms, s->ev_start, s->ev_stop);
     out->device_ms = ms + sres.device_ms;
   }
   return ErrorCode::OK;
@@ -583,18 +571,6 @@ ErrorCode XferEngine::run(const std::vector<XferItem>& items, ChecksumAlgo algo,
 }
 
 // ---------------------------------------------------------------- helpers
-static int g_dummy_err = 0;
-#undef BB_CUDA
-#define BB_CUDA_S(expr)                                                                                      \
-  do {                                                                                                       \
-    cudaError_t _e = (expr);                                                                                 \
-    if (_e != cudaSuccess) {                                                                                 \
-      BB_LOG(ERROR) << "CUDA error " << cudaGetErrorString(_e) << " at " #expr;                              \
-      g_dummy_err = static_cast<int>(_e);                                                                    \
-      return ErrorCode::FABRIC_ERROR;                                                                        \
-    }                                                                                                        \
-  } while (0)
-
 ErrorCode device_count(int* n) {
   *n = 0;
   cudaError_t e = cudaGetDeviceCount(n);
@@ -605,7 +581,7 @@ ErrorCode device_count(int* n) {
   return ErrorCode::OK;
 }
 ErrorCode device_malloc(int device, uint64_t bytes, void** out) {
-  BB_CUDA_S(cudaSetDevice(device));
+  BB_CUDA(cudaSetDevice(device));
   cudaError_t e = cudaMalloc(out, bytes);
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -614,8 +590,8 @@ ErrorCode device_malloc(int device, uint64_t bytes, void** out) {
   return ErrorCode::OK;
 }
 ErrorCode device_free(int device, void* p) {
-  BB_CUDA_S(cudaSetDevice(device));
-  BB_CUDA_S(cudaFree(p));
+  BB_CUDA(cudaSetDevice(device));
+  BB_CUDA(cudaFree(p));
   return ErrorCode::OK;
 }
 ErrorCode host_alloc_pinned(uint64_t bytes, void** out) {
@@ -627,16 +603,16 @@ ErrorCode host_alloc_pinned(uint64_t bytes, void** out) {
   return ErrorCode::OK;
 }
 ErrorCode host_free_pinned(void* p) {
-  BB_CUDA_S(cudaFreeHost(p));
+  BB_CUDA(cudaFreeHost(p));
   return ErrorCode::OK;
 }
 ErrorCode stream_synchronize(void* stream) {
-  BB_CUDA_S(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
+  BB_CUDA(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
   return ErrorCode::OK;
 }
 ErrorCode device_synchronize(int device) {
-  BB_CUDA_S(cudaSetDevice(device));
-  BB_CUDA_S(cudaDeviceSynchronize());
+  BB_CUDA(cudaSetDevice(device));
+  BB_CUDA(cudaDeviceSynchronize());
   return ErrorCode::OK;
 }
 int device_memcpy_peer_async(void* dst, int dst_device, const void* src, int src_device, uint64_t nbytes, void* stream) {

@@ -63,7 +63,8 @@ class XferEngine {
   ErrorCode run(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream, XferResult* out);
   // Fused MXFP8 put (pack = bf16 -> slab) or get (unpack = slab -> bf16): the bf16 side is read / written once, the
   // E4M3 payload is hashed on the tensor cores while it sits in shared memory, and the digest returned is the
-  // BBH64 of the stored packed object (identical to hashing the output of mxfp8_pack).  Synchronous.
+  // BBH64 of the stored packed object (identical to hashing the output of mxfp8_pack).  Synchronous; needs two free
+  // slots (the fused kernel's batch and the batch that hashes the scales).
   ErrorCode run_fp8(const std::vector<Fp8Item>& items, bool unpack, void* stream, XferResult* out);
   static bool fp8_eligible(uint64_t n_elems) { return n_elems != 0 && n_elems % 32 == 0; }  // whole MX blocks
 
@@ -94,6 +95,9 @@ class XferEngine {
  private:
   struct Slot;
   XferEngine() = default;
+  Slot* free_slot();
+  ErrorCode write_tile_table(Slot* s, uint32_t nd);
+  ErrorCode cuda_failed(int code, const char* what);
   int device_ = 0;
   uint32_t max_items_ = 0;
   std::vector<std::unique_ptr<Slot>> slots_;
@@ -117,8 +121,6 @@ class XferEngine {
   std::vector<uint32_t> debug_host_;
   bool tile_trace_ = false;
   std::vector<uint64_t> trace_host_;
-  struct Fp8State;
-  std::unique_ptr<Fp8State> fp8_;
 };
 
 // Device helpers used by bindings, the worker and benchmarks (all return ErrorCode).

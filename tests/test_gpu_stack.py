@@ -490,6 +490,85 @@ def test_fused_fp8_put_fans_out_to_replicas_and_get_fails_over(bb, torch_cuda):
         cl.stop()
 
 
+def _flip_byte(be, offset):
+    be.write(offset, bytes([be.read(offset, 1)[0] ^ 0xFF]))
+
+
+def test_device_get_fails_over_to_the_next_replica(bb, torch_cuda):
+    """A plain device get whose replica is corrupt: the fused kernel reports the mismatch and the client re-reads the
+    object from the next replica, until one verifies; with every copy corrupt the get reports CHECKSUM_MISMATCH."""
+    torch = torch_cuda
+    from blackbird_b200.parallel import GpuRankCluster
+
+    cl = GpuRankCluster(slab_bytes=64 << 20, cluster_id="t-failover")
+    try:
+        s = _stream(torch)
+        n, size = 4, 100000
+        stride = ((size + 255) // 256) * 256
+        src = torch.randint(0, 256, (n * stride,), dtype=torch.uint8, device="cuda")
+        keys = [f"fo/{i}" for i in range(n)]
+        cfg = bb.WorkerConfig(replication_factor=3, max_workers_per_copy=1, ttl_ms=0, preferred_classes=[bb.StorageClass.RAM_GPU])
+        ecs = cl.client.batch_put_device(keys, [src.data_ptr() + i * stride for i in range(n)], [size] * n, cfg, s)
+        assert ecs == [bb.ErrorCode.OK] * n, ecs
+        be = cl.worker.backend("hbm0")
+        copies = cl.client.get_workers(keys[1])
+        assert len(copies) == 3 and len({c.shards[0].offset for c in copies}) == 3
+        # corrupt two of the three copies of object 1: the get must end on the intact one
+        for c in copies[:2]:
+            _flip_byte(be, c.shards[0].offset + 777)
+        out = torch.zeros_like(src)
+        ecs, sizes = cl.client.batch_get_device(keys, [out.data_ptr() + i * stride for i in range(n)], [stride] * n, s)
+        torch.cuda.synchronize()
+        assert ecs == [bb.ErrorCode.OK] * n and sizes == [size] * n, ecs
+        for i in range(n):
+            assert torch.equal(src[i * stride:i * stride + size], out[i * stride:i * stride + size])
+        assert "bb_client_replica_failover_total" in cl.client.metrics_text()
+        # all three corrupt -> CHECKSUM_MISMATCH
+        _flip_byte(be, copies[2].shards[0].offset + 5)
+        ecs, _ = cl.client.batch_get_device([keys[1]], [out.data_ptr() + stride], [stride], s)
+        assert ecs == [bb.ErrorCode.CHECKSUM_MISMATCH]
+    finally:
+        cl.stop()
+
+
+def test_device_get_of_a_batch_that_mixes_checksum_algorithms(bb, torch_cuda):
+    """Objects written with XXH3 and with CRC32C, read back in one batch_get_device: each is verified against its own
+    algorithm's digest, and a corrupt object in each group is reported for that object only."""
+    torch = torch_cuda
+    from blackbird_b200.parallel import GpuRankCluster
+
+    cl = GpuRankCluster(slab_bytes=64 << 20, cluster_id="t-mixalgo")
+    try:
+        s = _stream(torch)
+        sizes = [5000, 70000, 16384, 300, 100000, 4096]
+        algos = [bb.ChecksumAlgo.XXH3] * 3 + [bb.ChecksumAlgo.CRC32C] * 3
+        n, stride = len(sizes), 100096
+        src = torch.randint(0, 256, (n * stride,), dtype=torch.uint8, device="cuda")
+        keys = [f"mix/{i}" for i in range(n)]
+        for i in range(n):
+            cfg = bb.WorkerConfig(replication_factor=1, max_workers_per_copy=1, ttl_ms=0, preferred_classes=[bb.StorageClass.RAM_GPU],
+                                  checksum=algos[i])
+            assert cl.client.batch_put_device([keys[i]], [src.data_ptr() + i * stride], [sizes[i]], cfg, s) == [bb.ErrorCode.OK]
+        shards = [cl.client.get_workers(k)[0].shards[0] for k in keys]
+        assert [sh.checksum_algo for sh in shards] == algos
+        out = torch.zeros_like(src)
+        ptrs = [out.data_ptr() + i * stride for i in range(n)]
+        ecs, got = cl.client.batch_get_device(keys, ptrs, [stride] * n, s)
+        torch.cuda.synchronize()
+        assert ecs == [bb.ErrorCode.OK] * n and got == sizes, ecs
+        for i in range(n):
+            assert torch.equal(src[i * stride:i * stride + sizes[i]], out[i * stride:i * stride + sizes[i]])
+        # one corrupt object per algorithm
+        be = cl.worker.backend("hbm0")
+        for i in (1, 4):
+            _flip_byte(be, shards[i].offset + sizes[i] // 2)
+        ecs, _ = cl.client.batch_get_device(keys, ptrs, [stride] * n, s)
+        want = [bb.ErrorCode.CHECKSUM_MISMATCH if i in (1, 4) else bb.ErrorCode.OK for i in range(n)]
+        assert ecs == want, ecs
+    finally:
+        cl.stop()
+
+
 @pytest.mark.parametrize("n", [32, 96, 16384 + 32, 3 * 16384 + 7 * 32, 2 * 16384 + 16352, 5 * 16384])
 def test_fused_fp8_handles_any_whole_number_of_mx_blocks(bb, torch_cuda, n):
     """The fused pack-put / unpack-get kernels take any multiple of 32 elements: the tail tile is converted and stored
