@@ -71,8 +71,16 @@ struct XferEngine::Slot {
   uint32_t total_tiles = 0;
   bool debug = false;
   bool hashed = true;
+  bool crc = false;
   uint64_t empty_digest = 0;
   std::vector<int32_t> item_to_desc;  // -1 for zero-size items
+  // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
+  struct Empty {
+    uint32_t item;
+    uint32_t flags;
+    uint64_t expect;
+  };
+  std::vector<Empty> empties;
 };
 
 Result<std::unique_ptr<XferEngine>> XferEngine::create(int device, uint32_t max_items, int slots) {
@@ -290,11 +298,15 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   BB_CUDA(cudaSetDevice(device_));
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   s->item_to_desc.assign(items.size(), -1);
+  s->empties.clear();
   uint32_t nd = 0;
   bool all_small = small_path_enabled();
   for (size_t i = 0; i < items.size(); ++i) {
     const XferItem& it = items[i];
-    if (it.nbytes == 0) continue;
+    if (it.nbytes == 0) {
+      s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
+      continue;
+    }
     all_small = all_small && it.nbytes <= kSmallBytes && !(it.flags & XFER_RAW_SUM) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
@@ -320,6 +332,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   s->debug = capture_debug;
   s->traced = tile_trace_;
   s->hashed = algo != ChecksumAlgo::NONE;
+  s->crc = algo == ChecksumAlgo::CRC32C;
   s->empty_digest = is_tile_sum(algo) ? tchash::finalize(0, 0) : 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int xalgo = algo == ChecksumAlgo::BBH64 ? ALGO_BBH64 : algo == ChecksumAlgo::CRC32C ? ALGO_CRC32C : algo == ChecksumAlgo::XXH3 ? ALGO_XXH3 : ALGO_NONE;
@@ -467,6 +480,14 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
           out->digest[i] = dg[d];
           out->status[i] = stt[d];
         }
+      }
+      // The digest of an empty object (a RAW_SUM slice of no tiles sums to 0); verified as the kernels verify: CRC32C
+      // compares the low 32 bits of `expect`.
+      for (const Slot::Empty& e : s->empties) {
+        const uint64_t digest = (e.flags & XFER_RAW_SUM) ? 0 : s->empty_digest;
+        const uint64_t want = s->crc ? (e.expect & 0xFFFFFFFFull) : e.expect;
+        out->digest[e.item] = digest;
+        out->status[e.item] = ((e.flags & XFER_VERIFY) && digest != want) ? 1u : 0u;
       }
     }
     out->device_ms = 0.f;

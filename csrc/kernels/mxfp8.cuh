@@ -53,7 +53,9 @@ __device__ __forceinline__ void pack_chunk(const uint4 v, uint2* payload_out, ui
 
 // Unpacks one 8-byte payload chunk with its block's scale into 8 bf16.
 __device__ __forceinline__ uint4 unpack_chunk(const uint2 p, uint8_t scale) {
-  const float s = __int_as_float(static_cast<int>(scale) << 23);  // 2^(e-127); e == 0 flushes to zero
+  // 2^(e-127).  e == 0 is 2^-127, the fp32 subnormal 0x00400000: the build keeps subnormals (no -ftz, no fast math), so
+  // the products below are exact and only the bf16 conversion rounds, as in the CPU reference.
+  const float s = __int_as_float(scale ? static_cast<int>(scale) << 23 : 0x00400000);
   auto cvt2 = [&](uint32_t two) -> uint32_t {  // two E4M3 bytes -> bf16x2
     const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two & 0xFFFFu), __NV_E4M3);
     const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hr));

@@ -20,24 +20,29 @@ void check(ErrorCode ec, const char* what) {
 void check_cuda(int rc, const char* what) {
   if (rc != 0) throw std::runtime_error(std::string(what) + ": CUDA error " + std::to_string(rc) + " " + cuda_error_string(rc));
 }
-// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0)
+// Pointers given as one integer or a list of up to kMaxDst integers; returns how many.
+uint32_t to_ptrs(const py::handle& h, void* (&out)[kMaxDst]) {
+  if (py::isinstance<py::int_>(h)) {
+    out[0] = reinterpret_cast<void*>(h.cast<uintptr_t>());
+    return 1;
+  }
+  auto v = h.cast<std::vector<uintptr_t>>();
+  if (v.size() > kMaxDst) throw py::value_error("at most 3 destinations");
+  for (size_t i = 0; i < v.size(); ++i) out[i] = reinterpret_cast<void*>(v[i]);
+  return static_cast<uint32_t>(v.size());
+}
+// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0).  An empty destination list makes a
+// hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3) throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags]])");
+  if (t.size() < 3 || t.size() > 6) throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base]]])");
   XferItem it;
   it.src = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
-  if (py::isinstance<py::int_>(t[1])) {
-    it.dst[0] = reinterpret_cast<void*>(t[1].cast<uintptr_t>());
-    it.ndst = 1;
-  } else {
-    auto v = t[1].cast<std::vector<uintptr_t>>();
-    if (v.empty() || v.size() > kMaxDst) throw py::value_error("1..3 destinations");
-    it.ndst = static_cast<uint32_t>(v.size());
-    for (size_t i = 0; i < v.size(); ++i) it.dst[i] = reinterpret_cast<void*>(v[i]);
-  }
+  it.ndst = to_ptrs(t[1], it.dst);
   it.nbytes = t[2].cast<uint64_t>();
   if (t.size() > 3) it.expect = t[3].cast<uint64_t>();
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
+  if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   return it;
 }
 }  // namespace
@@ -46,6 +51,7 @@ void bind_gpu(py::module_& m) {
   m.attr("TILE_BYTES") = kTileBytes;
   m.attr("XFER_VERIFY") = static_cast<uint32_t>(XFER_VERIFY);
   m.attr("XFER_MULTIMEM") = static_cast<uint32_t>(XFER_MULTIMEM);
+  m.attr("XFER_RAW_SUM") = static_cast<uint32_t>(XFER_RAW_SUM);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -74,7 +80,9 @@ void bind_gpu(py::module_& m) {
              return py::make_tuple(res.digest, res.status, res.device_ms);
            },
            py::arg("items"), py::arg("algo") = ChecksumAlgo::BBH64, py::arg("stream") = 0, py::arg("debug") = false,
-           "Runs one fused batch; returns (digests, status, device_ms).")
+           "Runs one fused batch; items = (src, dst | [dst, ...], nbytes[, expect[, flags[, tile_base]]]), where [] "
+           "destinations with XFER_RAW_SUM hash a slice whose first tile is tile `tile_base` of its object (digest = the "
+           "unfinalised tile sum); returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
              std::vector<gpu::Fp8Item> v;
@@ -82,7 +90,12 @@ void bind_gpu(py::module_& m) {
                auto t = h.cast<py::tuple>();
                gpu::Fp8Item it;
                it.wide = reinterpret_cast<void*>(t[0].cast<uintptr_t>());
-               it.packed = reinterpret_cast<void*>(t[1].cast<uintptr_t>());
+               void* packed[kMaxDst] = {nullptr, nullptr, nullptr};
+               it.nreplicas = to_ptrs(t[1], packed);
+               if (it.nreplicas == 0) throw py::value_error("1..3 packed objects");
+               it.packed = packed[0];
+               it.more_packed[0] = packed[1];
+               it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
                if (t.size() > 3) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                v.push_back(it);
@@ -95,8 +108,9 @@ void bind_gpu(py::module_& m) {
              return py::make_tuple(res.digest, res.status, res.device_ms);
            },
            py::arg("items"), py::arg("unpack"), py::arg("stream") = 0,
-           "Fused MXFP8 put (unpack=False: bf16 -> packed slab object) or get (unpack=True); items = (bf16_ptr, packed_ptr, "
-           "n_elems[, expected_digest]); returns (digests of the packed objects, status, device_ms).")
+           "Fused MXFP8 put (unpack=False: bf16 -> packed slab object) or get (unpack=True); items = (bf16_ptr, packed_ptr "
+           "| [packed_ptr, ...], n_elems[, expected_digest]), where a put writes every packed replica in the list (1..3) and "
+           "a get reads the first; returns (digests of the packed objects, status, device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {

@@ -47,26 +47,54 @@ def test_pack_reference_matches_torch_model(bb):
     assert bool((err <= bound).all())
 
 
+# Blocks with special values (bf16 bit patterns): +-Inf, NaN of either sign, subnormals, negative zeros, and mixes of them
+# with normal values; the block maximum skips NaN, an Inf selects the neutral scale.
+SPECIAL_BLOCKS = np.array([
+    [0x7F80, 0x3F80, 0xC000] + [0x3E00] * 29,    # +Inf with normals
+    [0xFF80, 0x4100, 0x0001] + [0xBC00] * 29,    # -Inf with a normal and a subnormal
+    [0x7FC0, 0x4000, 0xC040] + [0x3C00] * 29,    # NaN with normals
+    [0xFFC1, 0x7FC0] + [0xFFC0] * 30,            # NaN only
+    [0x0001, 0x8003, 0x007F, 0x8040] * 8,        # subnormals only (the scale clamps at 0)
+    [0x0001, 0x807F, 0x3F80, 0x8000] * 8,        # subnormals and -0 next to 1.0
+    [0x8000] * 32,                               # negative zeros only
+    [0x8000, 0x0000, 0x0080, 0x8080] * 8,        # +-0 and +-the smallest normal (the scale clamps at 0)
+], dtype=np.uint16)
+
+
+def special_blocks(rows=slice(None)):
+    """SPECIAL_BLOCKS[rows] as one flat bf16 tensor on the GPU."""
+    return torch.from_numpy(SPECIAL_BLOCKS[rows].reshape(-1).view(np.int16).copy()).view(torch.bfloat16).cuda()
+
+
+def check_packed(got, ref, n, what=""):
+    """Stored MXFP8 object (numpy uint8) vs mxfp8_pack_ref: block scales identical, payload identical up to the sign of a
+    zero."""
+    assert np.array_equal(got[n:], ref[n:]), f"{what}: block scales differ at {np.nonzero(got[n:] != ref[n:])[0][:10]}"
+    diff = (got[:n] != ref[:n]) & ~(((got[:n] & 0x7F) == 0) & ((ref[:n] & 0x7F) == 0))
+    assert not diff.any(), f"{what}: payload differs at {np.nonzero(diff)[0][:10]}"
+
+
+def check_unpacked(bb, back, packed, n, what=""):
+    """Dequantised bf16 (CPU tensor) vs mxfp8_unpack_ref of the same packed bytes: bit for bit, every block scale included;
+    NaN is compared only as NaN (the NaN bit patterns of the two sides differ)."""
+    ref = torch.frombuffer(bytearray(bb.mxfp8_unpack_ref(packed, n)), dtype=torch.bfloat16)
+    nan = ref.isnan()
+    assert torch.equal(back.isnan(), nan), f"{what}: NaN positions differ"
+    bad = back.view(torch.int16) != ref.view(torch.int16)
+    bad &= ~nan
+    assert not bool(bad.any()), f"{what}: elements {bad.nonzero().flatten()[:10].tolist()} differ"
+
+
 @pytest.mark.gpu
-def test_gpu_pack_unpack_match_cpu_reference(bb):
+def test_gpu_pack_unpack_match_cpu_reference_at_every_block_scale(bb):
+    """mxfp8_pack / mxfp8_unpack against the CPU reference: stored bytes, and dequantised values bit for bit at every block
+    scale, 0 (2^-127, an fp32 subnormal) included."""
     assert torch.cuda.is_available()
     g = torch.Generator(device="cuda").manual_seed(1)
     n = 32 * 40000 + 32 * 3
     x = (torch.randn(n, device="cuda", generator=g) * 10 ** torch.empty(n, device="cuda").uniform_(-3, 2, generator=g)).to(torch.bfloat16)
     x[64:96] = 0
-    # blocks with special values (bf16 bit patterns): +-Inf, NaN of either sign, subnormals, negative zeros, and mixes
-    # of them with normal values; the block maximum skips NaN, an Inf selects the neutral scale
-    special = torch.from_numpy(np.array([
-        [0x7F80, 0x3F80, 0xC000] + [0x3E00] * 29,    # +Inf with normals
-        [0xFF80, 0x4100, 0x0001] + [0xBC00] * 29,    # -Inf with a normal and a subnormal
-        [0x7FC0, 0x4000, 0xC040] + [0x3C00] * 29,    # NaN with normals
-        [0xFFC1, 0x7FC0] + [0xFFC0] * 30,            # NaN only
-        [0x0001, 0x8003, 0x007F, 0x8040] * 8,        # subnormals only (the scale clamps at 0)
-        [0x0001, 0x807F, 0x3F80, 0x8000] * 8,        # subnormals and -0 next to 1.0
-        [0x8000] * 32,                               # negative zeros only
-        [0x8000, 0x0000, 0x0080, 0x8080] * 8,        # +-0 and +-the smallest normal (the scale clamps at 0)
-    ], dtype=np.uint16).view(np.int16)).view(torch.bfloat16).view(-1).cuda()
-    nx, x = n, torch.cat([x, special])
+    nx, x = n, torch.cat([x, special_blocks()])
     n = x.numel()
     packed = torch.zeros(bb.mxfp8_packed_bytes(n), dtype=torch.uint8, device="cuda")
     s = torch.cuda.current_stream().cuda_stream
@@ -74,21 +102,12 @@ def test_gpu_pack_unpack_match_cpu_reference(bb):
     torch.cuda.synchronize()
     ref = np.frombuffer(bb.mxfp8_pack_ref(x.cpu().view(torch.int16).numpy()), dtype=np.uint8)
     got = packed.cpu().numpy()
-    assert np.array_equal(got[n:], ref[n:])  # block scales identical
-    diff = (got[:n] != ref[:n]) & ~(((got[:n] & 0x7F) == 0) & ((ref[:n] & 0x7F) == 0))
-    assert not diff.any(), np.nonzero(diff)[0][:10]
+    check_packed(got, ref, n)
     out = torch.zeros(n, dtype=torch.bfloat16, device="cuda")
     bb.mxfp8_unpack(packed.data_ptr(), n, out.data_ptr(), s)
     torch.cuda.synchronize()
-    back_ref = torch.frombuffer(bytearray(bb.mxfp8_unpack_ref(got, n)), dtype=torch.bfloat16)
-    back = out.cpu()
-    nan = back_ref.isnan()
-    assert torch.equal(back.isnan(), nan)  # NaN stays NaN (the NaN bit patterns of the two sides differ)
-    # A block scale of 0 (2^-127) dequantises to zero on the GPU; the CPU reference multiplies by 2^-127.
-    flushed = torch.from_numpy(got[n:].copy() == 0).repeat_interleave(32)
-    assert bool((back[flushed] == 0).all())
-    keep = ~nan & ~flushed
-    assert torch.equal(back[keep], back_ref[keep])
+    assert bool((got[n:] == 0).any())  # blocks whose scale is 0 (2^-127) are among those compared
+    check_unpacked(bb, out.cpu(), got, n)
     # fp32 reference of the op: dequantised values stay within the E4M3 error bound
     err = (out[:nx].float() - x[:nx].float()).abs().view(-1, 32).amax(dim=1)
     assert bool((err <= x[:nx].float().abs().view(-1, 32).amax(dim=1) * 2 ** -3 + 1e-30).all())
@@ -132,3 +151,31 @@ def test_fused_fp8_put_get_matches_unfused_pack_and_cpu_digest(bb):
     slabs[2][sizes[2] + 17] ^= 0x01
     _, st3, _ = eng.run_fp8([(o.data_ptr(), sl.data_ptr(), n, d) for o, sl, n, d in zip(outs, slabs, sizes, dg)], True, s)
     assert st3 == [0, 1, 1]
+
+
+@pytest.mark.gpu
+def test_standalone_kernels_at_their_grid_stride_edges(bb):
+    """mxfp8_pack / mxfp8_unpack are grid-stride loops over 16-byte chunks (4 per block) on at most 8 CTAs of 256 threads
+    per SM, and the pack pads its trip count to whole warps.  Objects of one to four blocks (a partial warp), and chunk
+    counts one block below, at and one block above what one pass of the largest grid covers, each ending in special-value
+    blocks: stored bytes, dequantised values and the bytes past both outputs against the CPU reference."""
+    assert torch.cuda.is_available()
+    s = torch.cuda.current_stream().cuda_stream
+    one_pass = torch.cuda.get_device_properties(0).multi_processor_count * 8 * 256  # chunks covered by the largest grid
+    g = torch.Generator(device="cuda").manual_seed(11)
+    for i, n in enumerate([32, 64, 96, 128] + [8 * (one_pass + d) for d in (-4, 0, 4)]):
+        x = (torch.randn(n, device="cuda", generator=g) * 10 ** torch.empty(n, device="cuda").uniform_(-4, 3, generator=g)).to(torch.bfloat16)
+        sp = special_blocks([(k + 3 * i) % 8 for k in range(min(n // 32, 8))])
+        x[n - sp.numel():] = sp
+        m = bb.mxfp8_packed_bytes(n)
+        packed = torch.full((m + 64,), 0xA5, dtype=torch.uint8, device="cuda")
+        out = torch.full((n + 32,), 0x5A5A, dtype=torch.int16, device="cuda")
+        bb.mxfp8_pack(x.data_ptr(), n, packed.data_ptr(), s)
+        bb.mxfp8_unpack(packed.data_ptr(), n, out.data_ptr(), s)
+        torch.cuda.synchronize()
+        got = packed.cpu().numpy()
+        check_packed(got[:m], np.frombuffer(bb.mxfp8_pack_ref(x.cpu().view(torch.int16).numpy()), dtype=np.uint8), n, f"n={n}")
+        assert bool((got[m:] == 0xA5).all()), f"n={n}: the pack wrote past the packed object"
+        back = out.cpu()
+        check_unpacked(bb, back[:n].view(torch.bfloat16), got[:m], n, f"n={n}")
+        assert bool((back[n:] == 0x5A5A).all()), f"n={n}: the unpack wrote past the output"
