@@ -891,6 +891,21 @@ static void ewma_update(std::atomic<double>& v, double sample) {
   v.store(old == 0 ? sample : 0.75 * old + 0.25 * sample, std::memory_order_relaxed);
 }
 
+// The fused kernels move 16-byte aligned buffers only (XferEngine::submit refuses a whole batch otherwise).  An object
+// whose caller buffer is not 16-byte aligned where one of its shards starts is staged through host memory instead, so
+// that it does not fail its neighbours.
+static bool fabric_aligned(const void* ptr, const std::vector<CopyPlacement>& copies) {
+  const auto base = reinterpret_cast<uintptr_t>(ptr);
+  for (const auto& c : copies) {
+    uint64_t off = 0;
+    for (const auto& sh : c.shards) {
+      if ((base + off) & 15) return false;
+      off += sh.length;
+    }
+  }
+  return true;
+}
+
 std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                                          const std::vector<size_t>& sizes, const WorkerConfig& cfg, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
@@ -936,8 +951,9 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
       out[i] = ErrorCode::OK;
       const auto& copies = pr.value();
       if (copies.empty()) continue;
-      // placements on host tiers (DRAM / CXL / NVMe): stage through host memory and use the data servers
-      bool on_fabric = true;
+      // placements on host tiers (DRAM / CXL / NVMe) and unaligned caller buffers: stage through host memory and use the
+      // data servers
+      bool on_fabric = fabric_aligned(dev_ptrs[i], copies);
       for (const auto& c : copies)
         for (const auto& sh : c.shards) {
           // a batch lands on a handful of pools: ask the transport once per run of shards on the same pool
@@ -1185,8 +1201,10 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
       const auto& copies = placed[i].value();
       // (the spread over replicas only matters when there is more than one; thousands of single-copy objects skip the hash)
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
+      // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
+      const bool aligned = fabric_aligned(dev_ptrs[i], copies);
       bool found = false;
-      for (size_t k = 0; k < copies.size() && !found; ++k) {
+      for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
         bool local = !copies[k].shards.empty();
         for (const auto& sh : copies[k].shards) local &= pool_is_local(sh);
         if (local) {
@@ -1196,7 +1214,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
         }
       }
       // HBM replicas first (NVLink), then replicas in mapped DRAM pools (PCIe)
-      for (int pass = 0; pass < 2 && !found; ++pass) {
+      for (int pass = 0; aligned && pass < 2 && !found; ++pass) {
         for (size_t k = 0; k < copies.size() && !found; ++k) {
           const auto& c = copies[(start + k) % copies.size()];
           bool ok = !c.shards.empty();

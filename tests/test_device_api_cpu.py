@@ -102,6 +102,55 @@ def test_device_api_stages_through_the_host_for_unreachable_tiers_and_pipelines_
         assert ecs == [bb.ErrorCode.OK] * n and np.array_equal(src, out)
 
 
+def _counter(client, name):
+    for line in client.metrics_text().splitlines():
+        if line.startswith(f"bb_client_{name} "):
+            return int(float(line.split()[1]))
+    return 0
+
+
+def test_device_api_stages_only_the_objects_whose_pointer_is_unaligned(bb):
+    """The fused kernels take 16-byte aligned pointers only. An object whose caller pointer is not aligned is staged through
+    the host, with the same bytes and digest, and its aligned neighbours in the batch are unaffected. The GPU fabric gives
+    the same answer (tests/test_device_path.py)."""
+    with LocalCluster(cluster_id="devalign", n_workers=2, pool_bytes=32 * MiB) as c:
+        cl = make_client(bb, c)
+        pools = {p.id: p for p in cl.keystone().get_memory_pools()}
+        sizes = [5000, 70001, 4096, 1 << 20, 17]
+        stride = (1 << 20) + 4096
+        n = len(sizes)
+        src = np.frombuffer(os.urandom(n * stride), dtype=np.uint8).copy()
+        base = (src.ctypes.data + 15) // 16 * 16 - src.ctypes.data  # first 16-byte aligned offset into src
+        offs = [base + i * stride + (8 if i == 2 else 0) for i in range(n)]
+        keys = [f"al/{i}" for i in range(n)]
+        for algo, ref in ((bb.ChecksumAlgo.CRC32C, bb.crc32c), (bb.ChecksumAlgo.BBH64, bb.bbh64_reference)):
+            cfg = bb.WorkerConfig(replication_factor=2, max_workers_per_copy=1, ttl_ms=0, checksum=algo, preferred_classes=[bb.StorageClass.RAM_CPU])
+            staged = _counter(cl, "device_put_host_staged_total")
+            ecs = cl.batch_put_device(keys, [src.ctypes.data + o for o in offs], sizes, cfg, 0)
+            assert ecs == [bb.ErrorCode.OK] * n, ecs
+            assert _counter(cl, "device_put_host_staged_total") == staged + 1
+            for i in range(n):
+                blob = src[offs[i]:offs[i] + sizes[i]]
+                for cp in cl.get_workers(keys[i]):
+                    sh = cp.shards[0]
+                    w = [w for w in c.workers if w.backend(sh.pool_id) is not None][0]
+                    stored = w.backend(sh.pool_id).read(sh.location["remote_addr"] - pools[sh.pool_id].ucx_remote_addr, sh.length)
+                    assert stored == bytes(blob) and sh.checksum == ref(blob), (i, algo)
+            # the get: object 3 lands 8 bytes past an aligned address, the others on aligned ones; nothing else is written
+            out = np.full(n * stride + 64, 0xA5, dtype=np.uint8)
+            obase = (out.ctypes.data + 15) // 16 * 16 - out.ctypes.data
+            dst = [obase + i * stride + (8 if i == 3 else 0) for i in range(n)]
+            staged = _counter(cl, "device_get_host_staged_total")
+            ecs, got = cl.batch_get_device(keys, [out.ctypes.data + d for d in dst], [stride - 8] * n, 0)
+            assert ecs == [bb.ErrorCode.OK] * n and got == sizes, ecs
+            assert _counter(cl, "device_get_host_staged_total") == staged + 1
+            want = np.full_like(out, 0xA5)
+            for i in range(n):
+                want[dst[i]:dst[i] + sizes[i]] = src[offs[i]:offs[i] + sizes[i]]
+            assert np.array_equal(out, want)
+            assert cl.batch_remove(keys) == [bb.ErrorCode.OK] * n
+
+
 def test_device_gets_survive_concurrent_compaction_and_migration(bb):
     """batch_get_device re-reads the placements of objects whose digest did not verify: readers racing with compaction
     and tier moves never see CHECKSUM_MISMATCH for an intact object."""
