@@ -103,13 +103,17 @@ class TensorStore:
         self.batch_put([key], [tensor], pack_fp8, config)
 
     # ------------------------------------------------------------------ get
-    def batch_get(self, keys: Sequence[str], device: Optional[torch.device] = None) -> list:
-        device = device or torch.device("cuda", torch.cuda.current_device())
+    def _metas(self, keys: Sequence[str]) -> list:
         metas = []
         for ec, blob in self.client.batch_get([k + "#meta" for k in keys]):
             if ec != _bb.ErrorCode.OK:
                 raise KeyError(f"object metadata missing: {ec}")
             metas.append(json.loads(blob))
+        return metas
+
+    def batch_get(self, keys: Sequence[str], device: Optional[torch.device] = None) -> list:
+        device = device or torch.device("cuda", torch.cuda.current_device())
+        metas = self._metas(keys)
         keys = list(keys)
         result = [None] * len(keys)
         # MXFP8 objects made of whole tiles: unpack fused into the get kernel (falls through when the object is not a
@@ -155,6 +159,50 @@ class TensorStore:
 
     def get(self, key: str, device: Optional[torch.device] = None) -> torch.Tensor:
         return self.batch_get([key], device)[0]
+
+    def batch_get_rows(self, keys: Sequence[str], starts: Sequence[int], stops: Sequence[int],
+                       device: Optional[torch.device] = None) -> list:
+        """Rows [start, stop) along dim 0 of each stored tensor, as new tensors (`t[start:stop]`): a tensor-parallel rank
+        loads its shard of a weight, a reader a few KV blocks of a layer.  Only the byte range of those rows is stored
+        into the result; every shard of the object that overlaps it is still read whole and verified against its
+        digest.  IndexError unless 0 <= start <= stop <= shape[0]; 0-d tensors have no rows.  MXFP8-packed tensors are
+        read whole, unpacked and sliced (correct, but not a ranged read)."""
+        device = device or torch.device("cuda", torch.cuda.current_device())
+        keys, starts, stops = list(keys), list(starts), list(stops)
+        if not len(keys) == len(starts) == len(stops):
+            raise ValueError("keys, starts and stops differ in length")
+        metas = self._metas(keys)
+        for k, m, a, b in zip(keys, metas, starts, stops):
+            if not m["shape"]:
+                raise IndexError(f"{k}: a 0-d tensor has no rows")
+            if not 0 <= a <= b <= m["shape"][0]:
+                raise IndexError(f"{k}: rows [{a}, {b}) outside [0, {m['shape'][0]}]")
+        result = [None] * len(keys)
+        packed = [i for i, m in enumerate(metas) if m["packed"]]
+        if packed:
+            whole = self.batch_get([keys[i] for i in packed], device)
+            for i, t in zip(packed, whole):
+                result[i] = t[starts[i]:stops[i]].clone()
+        ranged = [i for i, m in enumerate(metas) if not m["packed"]]
+        if ranged:
+            offsets, lengths = [], []
+            for i in ranged:
+                m = metas[i]
+                dtype = _DTYPES[m["dtype"]]
+                row = torch.Size(m["shape"][1:]).numel() * torch.empty((), dtype=dtype).element_size()
+                result[i] = torch.empty([stops[i] - starts[i]] + m["shape"][1:], dtype=dtype, device=device)
+                offsets.append(starts[i] * row)
+                lengths.append((stops[i] - starts[i]) * row)
+            ecs = self.client.batch_get_device_range([keys[i] for i in ranged], [result[i].data_ptr() for i in ranged], offsets,
+                                                     lengths, self._stream())
+            bad = [(keys[i], e) for i, e in zip(ranged, ecs) if e != _bb.ErrorCode.OK]
+            if bad:
+                raise RuntimeError(f"range get failed: {bad[:3]}")
+        return result
+
+    def get_rows(self, key: str, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
+        """`t[start:stop]` of the tensor stored under `key` (see batch_get_rows)."""
+        return self.batch_get_rows([key], [start], [stop], device)[0]
 
     def remove(self, keys: Sequence[str]) -> None:
         self.client.batch_remove(list(keys) + [k + "#meta" for k in keys])

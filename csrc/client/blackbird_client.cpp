@@ -467,7 +467,8 @@ ErrorCode BlackbirdClient::transfer_put(const std::vector<CopyPlacement>& copies
   });
 }
 
-ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size) {
+ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo, uint64_t hi) {
+  const bool whole = lo == 0 && hi == UINT64_MAX;
   ErrorCode last = ErrorCode::NO_COMPLETE_WORKER;
   for (const auto& copy : copies) {  // replica fail-over (reference reads copy 0 only, :283-287)
     uint64_t total = 0;
@@ -483,6 +484,7 @@ ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies
       off += copy.shards[s].length;
     }
     last = parallel_for(copy.shards.size(), opts_.io_parallelism, [&](size_t s) {
+      if (!whole && !(offs[s] < hi && offs[s] + copy.shards[s].length > lo)) return ErrorCode::OK;  // outside the range
       return read_shard(copy.shards[s], dst + offs[s], copy.shards[s].checksum_algo);
     });
     if (last == ErrorCode::OK) return ErrorCode::OK;
@@ -1087,32 +1089,86 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
 std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                          const std::vector<size_t>& capacity, void* stream,
                                                          std::vector<size_t>* out_sizes) {
+  return get_device(keys, dev_ptrs, capacity, nullptr, stream, out_sizes);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                               const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths,
+                                                               void* stream) {
+  if (offsets.size() != keys.size() || lengths.size() != keys.size())
+    return std::vector<ErrorCode>(keys.size(), keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  std::vector<ByteRange> ranges(keys.size());
+  std::vector<size_t> lens(keys.size());
+  for (size_t i = 0; i < keys.size(); ++i) {
+    ranges[i] = {offsets[i], lengths[i]};
+    lens[i] = static_cast<size_t>(lengths[i]);
+  }
+  auto out = get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr);
+  uint64_t n = 0, bytes = 0;
+  for (size_t i = 0; i < out.size(); ++i)
+    if (out[i] == ErrorCode::OK) ++n, bytes += lengths[i];
+  metrics_.inc("device_get_range_total", n);
+  metrics_.inc("device_get_range_bytes_total", bytes);
+  return out;
+}
+
+// Shard [off, off + len) of an object takes part in a get of object bytes [lo, hi): every shard of a whole-object get
+// (`all`, zero-length objects included), else the shards that overlap the range.
+namespace {
+struct GetSpan {
+  uint64_t lo = 0, hi = 0;
+  bool all = true;
+  bool overlaps(uint64_t off, uint64_t len) const { return all || (off < hi && off + len > lo); }
+};
+}  // namespace
+
+std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                   const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges, void* stream,
+                                                   std::vector<size_t>* out_sizes) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size()) return out;
+  if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size())) return out;
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_get_device", keys.size());
   if (out_sizes) out_sizes->assign(keys.size(), 0);
   std::vector<Result<std::vector<CopyPlacement>>> placed(keys.size(), Result<std::vector<CopyPlacement>>(ErrorCode::INTERNAL_ERROR));
   std::vector<size_t> copy_choice(keys.size(), 0);
   std::vector<bool> pending(keys.size(), false);
+  std::vector<GetSpan> span(keys.size());
+  // Where object byte 0 would land: the caller's pointer, or for a range get the virtual base `ptr - offset` (the fabric
+  // stores object byte x at base + x and never touches an address outside the range).
+  std::vector<void*> range_bases;
+  if (ranges) {
+    range_bases.resize(keys.size());
+    for (size_t i = 0; i < keys.size(); ++i)
+      range_bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - (*ranges)[i].offset);
+  }
+  const std::vector<void*>& bases = ranges ? range_bases : dev_ptrs;
 
   auto build_ops = [&](size_t begin, size_t end, std::vector<DeviceShardOp>& ops) {
     for (size_t i = begin; i < end; ++i) {
       if (!pending[i]) continue;
       const auto& copies = placed[i].value();
       const auto& copy = copies[copy_choice[i] % copies.size()];
+      const GetSpan& sp = span[i];
       uint64_t off = 0;
       for (size_t s = 0; s < copy.shards.size(); ++s) {
-        DeviceShardOp op;
-        op.item = i;
-        op.copy = copy_choice[i] % copies.size();
-        op.shard = s;
-        op.placement = &copy.shards[s];
-        op.obj_offset = off;
-        ops.push_back(std::move(op));
-        off += copy.shards[s].length;
+        const uint64_t len = copy.shards[s].length;
+        if (sp.overlaps(off, len)) {
+          DeviceShardOp op;
+          op.item = i;
+          op.copy = copy_choice[i] % copies.size();
+          op.shard = s;
+          op.placement = &copy.shards[s];
+          op.obj_offset = off;
+          if (!sp.all) {
+            op.win_lo = std::max(sp.lo, off) - off;
+            op.win_hi = std::min(sp.hi, off + len) - off;
+          }
+          ops.push_back(std::move(op));
+        }
+        off += len;
       }
     }
   };
@@ -1192,21 +1248,46 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
       size_t size = 0;
       for (const auto& s : placed[i].value()[0].shards) size += s.length;
       if (out_sizes) (*out_sizes)[i] = size;
-      if (size > capacity[i]) {
-        out[i] = ErrorCode::BUFFER_OVERFLOW;
-        continue;
+      GetSpan& sp = span[i];
+      if (ranges) {
+        const ByteRange& r = (*ranges)[i];
+        if (r.offset + r.length < r.offset || r.offset + r.length > size) {
+          out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
+          continue;
+        }
+        if (r.length == 0) {  // nothing to read or store
+          out[i] = ErrorCode::OK;
+          continue;
+        }
+        sp = {r.offset, r.offset + r.length, false};
+      } else {
+        if (size > capacity[i]) {
+          out[i] = ErrorCode::BUFFER_OVERFLOW;
+          continue;
+        }
+        sp.hi = size;
       }
       // replica choice: one that lives on this client's own GPU (HBM speed, no NVLink), else a replica that is
-      // fully reachable over the GPU fabric (readers spread over the replicas), else stage through the host
+      // fully reachable over the GPU fabric (readers spread over the replicas), else stage through the host.  Only the
+      // shards a get reads count: a range get ignores the shards outside its range.
       const auto& copies = placed[i].value();
+      auto for_read_shards = [&](const CopyPlacement& c, auto&& f) {  // returns how many shards the get reads
+        size_t n = 0;
+        uint64_t off = 0;
+        for (const auto& sh : c.shards) {
+          if (sp.overlaps(off, sh.length)) f(sh), ++n;
+          off += sh.length;
+        }
+        return n;
+      };
       // (the spread over replicas only matters when there is more than one; thousands of single-copy objects skip the hash)
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
       // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
-      const bool aligned = fabric_aligned(dev_ptrs[i], copies);
+      const bool aligned = fabric_aligned(bases[i], copies);
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
-        bool local = !copies[k].shards.empty();
-        for (const auto& sh : copies[k].shards) local &= pool_is_local(sh);
+        bool local = true;
+        local = for_read_shards(copies[k], [&](const ShardPlacement& sh) { local &= pool_is_local(sh); }) > 0 && local;
         if (local) {
           copy_choice[i] = k;
           found = true;
@@ -1216,9 +1297,10 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
       // HBM replicas first (NVLink), then replicas in mapped DRAM pools (PCIe)
       for (int pass = 0; aligned && pass < 2 && !found; ++pass) {
         for (size_t k = 0; k < copies.size() && !found; ++k) {
-          const auto& c = copies[(start + k) % copies.size()];
-          bool ok = !c.shards.empty();
-          for (const auto& sh : c.shards) ok = ok && (pass == 1 || sh.storage_class == StorageClass::RAM_GPU) && pool_reachable(sh);
+          bool ok = true;
+          ok = for_read_shards(copies[(start + k) % copies.size()], [&](const ShardPlacement& sh) {
+                 ok = ok && (pass == 1 || sh.storage_class == StorageClass::RAM_GPU) && pool_reachable(sh);
+               }) > 0 && ok;
           if (ok) {
             copy_choice[i] = (start + k) % copies.size();
             found = true;
@@ -1228,8 +1310,9 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
       }
       if (!found) {
         std::vector<uint8_t> stage(size);
-        ErrorCode ec = transfer_get(copies, stage.data(), size);  // data servers + CPU checksum + replica fail-over
-        if (ec == ErrorCode::OK) ec = device_->copy_h2d(dev_ptrs[i], stage.data(), size, stream);
+        // data servers + CPU checksum + replica fail-over, over the shards the get reads
+        ErrorCode ec = sp.all ? transfer_get(copies, stage.data(), size) : transfer_get(copies, stage.data(), size, sp.lo, sp.hi);
+        if (ec == ErrorCode::OK) ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, sp.hi - sp.lo, stream);
         out[i] = ec;
         metrics_.inc("device_get_host_staged_total");
         continue;
@@ -1239,7 +1322,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
     build_ops(ch.begin, ch.end, ch.ops);
     if (ch.ops.empty()) return;
     const TimePoint t1 = Clock::now();
-    auto t = device_->submit_get(ch.ops, dev_ptrs, stream);
+    auto t = device_->submit_get(ch.ops, bases, stream);
     metrics_.observe("phase_get_submit_us", us_since(t1));
     if (t.ok()) {
       ch.ticket = t.value();
@@ -1290,7 +1373,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
     if (ops.empty()) break;
     metrics_.inc("replica_failover_total");
     std::vector<uint32_t> status;
-    auto t = device_->submit_get(ops, dev_ptrs, stream);
+    auto t = device_->submit_get(ops, bases, stream);
     ErrorCode ec = t.ok() ? device_->wait_get(t.value(), &status) : t.error();
     if (ec != ErrorCode::OK) {
       for (size_t i = 0; i < keys.size(); ++i)
@@ -1321,6 +1404,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
       std::vector<ObjectKey> rkeys;
       std::vector<void*> rptrs;
       std::vector<size_t> rcaps, ridx;
+      std::vector<ByteRange> rranges;
       for (size_t k = 0; k < bad.size(); ++k) {
         const size_t i = bad[k];
         if (!again[k].ok()) {
@@ -1329,13 +1413,14 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
           // changed placements, or (once) the same ones: a remove + re-put can land on the very same extent (first fit)
           // and be read half-written
           rkeys.push_back(keys[i]), rptrs.push_back(dev_ptrs[i]), rcaps.push_back(capacity[i]), ridx.push_back(i);
+          if (ranges) rranges.push_back((*ranges)[i]);
         }
       }
       if (!rkeys.empty()) {
         metrics_.inc("get_placement_refresh_total", rkeys.size());
         std::vector<size_t> rsizes;
         ++refresh_depth;
-        auto recs = batch_get_device(rkeys, rptrs, rcaps, stream, &rsizes);
+        auto recs = get_device(rkeys, rptrs, rcaps, ranges ? &rranges : nullptr, stream, &rsizes);
         --refresh_depth;
         for (size_t k = 0; k < ridx.size(); ++k) {
           out[ridx[k]] = recs[k];
@@ -1377,8 +1462,18 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
   std::vector<uint32_t> status(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
-    auto* dst = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
-    const ErrorCode ec = io_->read_shard(*op.placement, dst, op.placement->checksum_algo);
+    // dev_ptrs[item] is where object byte 0 would land; for a range get only the window is real memory
+    const uintptr_t dst = reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + op.obj_offset;
+    ErrorCode ec;
+    if (op.windowed()) {  // as the kernel does: read and verify the whole shard, store only the window
+      std::vector<uint8_t> whole(op.placement->length);
+      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
+      const uint64_t hi = std::min<uint64_t>(op.win_hi, whole.size());
+      if (ec == ErrorCode::OK && hi > op.win_lo)
+        std::memcpy(reinterpret_cast<uint8_t*>(dst + op.win_lo), whole.data() + op.win_lo, hi - op.win_lo);
+    } else {
+      ec = io_->read_shard(*op.placement, reinterpret_cast<uint8_t*>(dst), op.placement->checksum_algo);
+    }
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
       status[k] = 1;  // reported per shard, like the kernel's verify flag
     } else if (ec != ErrorCode::OK) {

@@ -55,6 +55,10 @@ struct DeviceShardOp {
   const ShardPlacement* placement = nullptr;
   std::vector<const ShardPlacement*> replicas;  // same shard on the other copies (put fan-out)
   uint64_t obj_offset = 0;    // byte offset of this shard inside the object
+  // Get of a byte range: only shard bytes [win_lo, win_hi) are stored (the whole shard is still read and verified).  Any
+  // op whose window is not narrower than the shard, the default included, is a whole-shard op.
+  uint64_t win_lo = 0, win_hi = UINT64_MAX;
+  bool windowed() const { return placement && (win_lo > 0 || win_hi < placement->length); }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
@@ -144,6 +148,13 @@ class BlackbirdClient {
   // out_sizes[i] receives the object size; buffers must be large enough (capacity[i]).
   std::vector<ErrorCode> batch_get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                           const std::vector<size_t>& capacity, void* stream, std::vector<size_t>* out_sizes);
+  // Byte-range gets: bytes [offsets[i], offsets[i] + lengths[i]) of object i land at dev_ptrs[i].  Every shard that overlaps
+  // a range is read whole and verified against its digest (a corrupt byte outside the range still fails that copy over to
+  // the next replica); shards outside the range are not touched.  A range whose virtual base dev_ptrs[i] - offsets[i] is
+  // not 16-byte aligned at a shard start is staged through the host, like a misaligned batch_get_device.  Per-object
+  // VALUE_OUT_OF_RANGE when the range passes the end of the object.
+  std::vector<ErrorCode> batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths, void* stream);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }
@@ -162,7 +173,16 @@ class BlackbirdClient {
   ErrorCode put_once(const ObjectKey& key, const uint8_t* data, size_t size, const WorkerConfig& cfg);
   ErrorCode transfer_put(const std::vector<CopyPlacement>& copies, const uint8_t* data, ChecksumAlgo algo,
                          keystone::ShardChecksums* sums);
-  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size);
+  // Reads the object into dst[0, size) from the first copy that verifies.  With a byte range [lo, hi) only the shards that
+  // overlap it are read (whole, and verified); the other bytes of dst are left as they are.
+  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo = 0, uint64_t hi = UINT64_MAX);
+  // batch_get_device and batch_get_device_range: `ranges` null = whole objects into buffers of `capacity`, else object i's
+  // range into dev_ptrs[i] (capacity[i] = its length, for the chunk plan).
+  struct ByteRange {
+    uint64_t offset = 0, length = 0;
+  };
+  std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
+                                    const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
   ErrorCode get_with_refresh(const ObjectKey& key, uint8_t* (*alloc)(void*, size_t), void* ctx, size_t capacity, size_t* out_size);
   static uint64_t shard_offset(const ShardPlacement& s);
   static ChecksumAlgo algo_of(const std::vector<CopyPlacement>& copies, ChecksumAlgo hint);

@@ -456,7 +456,9 @@ GpuFabric::Path GpuFabric::classify(const ShardPlacement& s) const {
 
 std::string GpuFabric::metrics_text() const {
   static const char* kPath[kNumPaths] = {"hbm", "nvlink", "pcie", "nvlink_multicast"};
-  std::string out = "# HELP bb_fabric_bytes_total payload bytes moved by the fused transfer kernels\n# TYPE bb_fabric_bytes_total counter\n";
+  std::string out =
+      "# HELP bb_fabric_bytes_total payload bytes moved by the fused transfer kernels (get: bytes read, i.e. whole shards for "
+      "a verified range get)\n# TYPE bb_fabric_bytes_total counter\n";
   const std::string g = std::to_string(device_);
   for (int d = 0; d < 2; ++d)
     for (int p = 0; p < kNumPaths; ++p) {
@@ -685,9 +687,14 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
     it.nbytes = op.placement->length;
     it.expect = op.placement->checksum;
     it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
+    if (op.windowed()) {  // whole-shard ops keep exactly the descriptors they always had
+      it.flags |= XFER_WINDOW;
+      it.win_lo = op.win_lo;
+      it.win_hi = std::min(op.win_hi, it.nbytes);
+    }
     items->push_back(it);
     op_of_item->push_back(k);
-    count(false, classify(*op.placement), it.nbytes);
+    count(false, classify(*op.placement), window_read_bytes(it, algo));
   }
   return ErrorCode::OK;
 }

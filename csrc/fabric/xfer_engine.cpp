@@ -303,27 +303,40 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   bool all_small = small_path_enabled();
   for (size_t i = 0; i < items.size(); ++i) {
     const XferItem& it = items[i];
-    if (it.nbytes == 0) {
+    const bool win = it.flags & XFER_WINDOW;
+    if (win && (it.win_lo > it.win_hi || it.win_hi > it.nbytes || it.ndst != 1 || (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM))))
+      return ErrorCode::INVALID_ARGUMENT;
+    // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
+    // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
+    const uint64_t nbytes = window_read_bytes(it, algo);
+    const uint64_t trim = win && algo == ChecksumAlgo::NONE ? it.win_lo & ~uint64_t{15} : 0;
+    if (nbytes == 0) {
       s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
       continue;
     }
-    all_small = all_small && it.nbytes <= kSmallBytes && !(it.flags & XFER_RAW_SUM) && it.ndst >= 1;
+    // windowed items always take bb_xfer: neither the warp-per-object kernel nor the mailbox has a store window
+    all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW)) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
     for (uint32_t r = 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
     if (al & 15) return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
-    d.src = it.src;
+    d.src = static_cast<const uint8_t*>(it.src) + trim;
     for (uint32_t r = 0; r < kMaxDst; ++r) d.dst[r] = r < it.ndst ? it.dst[r] : nullptr;
-    d.nbytes = it.nbytes;
+    if (win) {
+      d.win.base = static_cast<uint8_t*>(it.dst[0]) + trim;
+      d.win.lo = it.win_lo - trim;
+      d.win.hi = it.win_hi - trim;
+    }
+    d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;
     d.flags = it.flags;
     d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
     if (algo == ChecksumAlgo::CRC32C) {
-      d.expect = (static_cast<uint64_t>(crc_init_term_for(it.nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
-      d.reserved = crc_unpad_for(it.nbytes);
+      d.expect = (static_cast<uint64_t>(crc_init_term_for(nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
+      d.reserved = crc_unpad_for(nbytes);
     }
     s->item_to_desc[i] = static_cast<int32_t>(nd++);
   }
@@ -349,7 +362,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   if (nd && all_small && direct && !capture_debug && !tile_trace_) {
     if (nd <= kMailSlots / 2 && mailbox_enabled() && (!mb_ || mb_->outstanding == 0)) {
       bool simple = true;
-      for (uint32_t i = 0; i < nd; ++i) simple = simple && descs[i].ndst == 1 && !(descs[i].flags & XFER_MULTIMEM);
+      for (uint32_t i = 0; i < nd; ++i) simple = simple && descs[i].ndst == 1 && !(descs[i].flags & (XFER_MULTIMEM | XFER_WINDOW));
       if (simple && cudaStreamQuery(st) == cudaSuccess)
         s->completion = Completion::MAILBOX;
       else

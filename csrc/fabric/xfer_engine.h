@@ -25,7 +25,18 @@ struct XferItem {
   uint64_t expect = 0;   // expected digest when flags & XFER_VERIFY
   uint32_t flags = 0;
   uint32_t tile_base = 0;  // XFER_RAW_SUM: index of this slice's first tile inside the hashed object
+  // XFER_WINDOW: only object bytes [win_lo, win_hi) are stored, byte x at dst[0] + x (dst[0] = caller buffer - win_lo).
+  // The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine reads only the 16-byte
+  // aligned span of the window (see window_read_bytes).
+  uint64_t win_lo = 0, win_hi = 0;
 };
+
+// Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span
+// [win_lo & ~15, win_hi) (nothing for an empty window).
+inline uint64_t window_read_bytes(const XferItem& it, ChecksumAlgo algo) {
+  if (!(it.flags & XFER_WINDOW) || algo != ChecksumAlgo::NONE) return it.nbytes;
+  return it.win_hi > it.win_lo ? it.win_hi - (it.win_lo & ~uint64_t{15}) : 0;
+}
 
 // One object of a fused MXFP8 transfer: `wide` is the caller's bf16 tensor, `packed` the slab location of the
 // stored object ([E4M3 payload n_elems][E8M0 scales n_elems / 32]).

@@ -20,12 +20,25 @@ enum XferFlags : uint32_t {
   // index, so a byte range can be hashed as a slice of a larger object (its sums add up with the slices
   // hashed elsewhere; the host finalises).  With ndst == 0 the descriptor is hash-only (nothing is stored).
   XFER_RAW_SUM = 1u << 2,
+  // Store window (range reads): every tile is still loaded and hashed, but only object bytes [win.lo, win.hi) are
+  // stored.  Only with ndst == 1, never with XFER_MULTIMEM or XFER_RAW_SUM.
+  XFER_WINDOW = 1u << 3,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
+//
+// dst[0] is where object byte 0 lands, so byte x is stored at dst[0] + x.  With XFER_WINDOW the caller's buffer holds only
+// the window: dst[0] is then the virtual base `buffer - lo`, an address that is never dereferenced outside [lo, hi).  A
+// windowed descriptor has one destination, so the words of dst[1] / dst[2] carry the window bounds (`win`).
 struct XferDesc {
   const void* src;          // 16-byte aligned; local or peer-mapped
-  void* dst[kMaxDst];       // 16-byte aligned; local, peer-mapped or multicast
+  union {
+    void* dst[kMaxDst];     // 16-byte aligned; local, peer-mapped or multicast
+    struct {
+      void* base;           // = dst[0]
+      uint64_t lo, hi;      // XFER_WINDOW: byte range of the object that is stored, lo <= hi <= nbytes
+    } win;
+  };
   uint64_t nbytes;
   uint32_t first_tile;      // exclusive prefix sum of ceil(nbytes / kTileBytes)
   uint32_t ndst;
@@ -34,6 +47,8 @@ struct XferDesc {
   uint32_t reserved;        // CRC32C: x^(-8*pad) mod P (crc_unpad_for); BBH64 + XFER_RAW_SUM: tile index base
 };
 static_assert(sizeof(XferDesc) == 64, "XferDesc must be 64 bytes");
+static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offsetof(XferDesc, win.hi) == offsetof(XferDesc, dst) + 16,
+              "the window bounds are the words of dst[1] / dst[2]");
 
 constexpr uint32_t kSmallBytes = 4096;     // objects up to this size may take the warp-per-object path (xfer_small.cu)
 constexpr uint32_t kSmallPending = 0xFFFFFFFFu;  // value of a status slot whose object has not completed yet (flag completion)

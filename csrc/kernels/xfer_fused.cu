@@ -292,23 +292,33 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
       if (p.trace_d && lane == 0) p.trace_d[static_cast<uint64_t>(t0 + it) * 4 + 1] = globaltimer_ns();
       const StageMeta& m = s.meta[stage];
       const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kTileBytes;
-      const uint32_t b16 = m.bytes & ~15u;
-      const uint32_t tail = m.bytes & 15u;
       const uint32_t ndst = m.ndst_flags & 0xFFu;
       const uint32_t flags = m.ndst_flags >> 8;
+      // Tile-relative span [x0, x1) to store: the whole tile, or its part inside the window [dst[1], dst[2]) (object
+      // offsets).  Its 16-byte aligned middle [a0, a1) goes out by TMA; the head [x0, h1) and the tail [t0, x1) are
+      // under 16 bytes each and are stored by lanes 0-15 and 16-31.  Without a window x0 = 0, so there is no head.
+      uint32_t x0 = 0, x1 = m.bytes;
+      if (flags & XFER_WINDOW) {
+        x0 = static_cast<uint32_t>(min(max(m.dst[1], off) - off, static_cast<uint64_t>(m.bytes)));
+        x1 = static_cast<uint32_t>(max(min(m.dst[2], off + m.bytes), off) - off);
+        x1 = max(x1, x0);
+      }
+      const uint32_t a0 = (x0 + 15u) & ~15u, a1 = max(x1 & ~15u, a0);
+      const uint32_t h1 = min(a0, x1), tb = max(a1, h1);
       if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);
-        for (uint32_t o = lane * 16; o < b16; o += 512)
+        for (uint32_t o = a0 + lane * 16; o < a1; o += 512)
           multimem_st_v4(mc + o, *reinterpret_cast<const uint4*>(&s.tile[stage][o]));
       } else if (lane == 0) {
         for (uint32_t r = 0; r < ndst; ++r)
-          if (b16) bulk_s2g(reinterpret_cast<void*>(m.dst[r] + off), s.tile[stage], b16);
+          if (a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[r] + off + a0), &s.tile[stage][a0], a1 - a0);
       }
       if (lane == 0) bulk_commit();
       if (p.trace_d && lane == 0) p.trace_d[static_cast<uint64_t>(t0 + it) * 4 + 2] = globaltimer_ns();
-      if (lane < tail) {
-        const uint8_t b = s.tile[stage][b16 + lane];
-        for (uint32_t r = 0; r < ndst; ++r) *reinterpret_cast<uint8_t*>(m.dst[r] + off + b16 + lane) = b;
+      const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);
+      if (o < (lane < 16 ? h1 : x1)) {
+        const uint8_t b = s.tile[stage][o];
+        for (uint32_t r = 0; r < ndst; ++r) *reinterpret_cast<uint8_t*>(m.dst[r] + off + o) = b;
       }
       __syncwarp();
       if (it >= kStoreLag && lane == 0) {

@@ -1196,6 +1196,14 @@ void bind_control(py::module_& m) {
         }
         return py::make_tuple(ecs_to_py(ecs), sizes);
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("capacity"), py::arg("stream") = 0)
+      .def("batch_get_device_range", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+                                        const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths, uintptr_t stream) {
+        std::vector<void*> p;
+        for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
+        return ecs_to_py(nogil([&] { return c.batch_get_device_range(keys, p, offsets, lengths, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("lengths"), py::arg("stream") = 0,
+         "Bytes [offsets[i], offsets[i] + lengths[i]) of object i into dev_ptrs[i]; every overlapping shard is read whole and "
+         "verified; returns one ErrorCode per object.")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

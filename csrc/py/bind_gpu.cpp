@@ -31,11 +31,13 @@ uint32_t to_ptrs(const py::handle& h, void* (&out)[kMaxDst]) {
   for (size_t i = 0; i < v.size(); ++i) out[i] = reinterpret_cast<void*>(v[i]);
   return static_cast<uint32_t>(v.size());
 }
-// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0).  An empty destination list makes a
-// hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).
+// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None).  An empty destination list makes
+// a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window (lo, hi) sets XFER_WINDOW: only
+// object bytes [lo, hi) are stored, byte x at dst + x.
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 6) throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base]]])");
+  if (t.size() < 3 || t.size() > 7)
+    throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)]]]])");
   XferItem it;
   it.src = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
   it.ndst = to_ptrs(t[1], it.dst);
@@ -43,6 +45,12 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 3) it.expect = t[3].cast<uint64_t>();
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
+  if (t.size() > 6 && !t[6].is_none()) {
+    auto w = t[6].cast<std::pair<uint64_t, uint64_t>>();
+    it.win_lo = w.first;
+    it.win_hi = w.second;
+    it.flags |= XFER_WINDOW;
+  }
   return it;
 }
 }  // namespace
@@ -52,6 +60,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_VERIFY") = static_cast<uint32_t>(XFER_VERIFY);
   m.attr("XFER_MULTIMEM") = static_cast<uint32_t>(XFER_MULTIMEM);
   m.attr("XFER_RAW_SUM") = static_cast<uint32_t>(XFER_RAW_SUM);
+  m.attr("XFER_WINDOW") = static_cast<uint32_t>(XFER_WINDOW);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -80,9 +89,11 @@ void bind_gpu(py::module_& m) {
              return py::make_tuple(res.digest, res.status, res.device_ms);
            },
            py::arg("items"), py::arg("algo") = ChecksumAlgo::BBH64, py::arg("stream") = 0, py::arg("debug") = false,
-           "Runs one fused batch; items = (src, dst | [dst, ...], nbytes[, expect[, flags[, tile_base]]]), where [] "
+           "Runs one fused batch; items = (src, dst | [dst, ...], nbytes[, expect[, flags[, tile_base[, (lo, hi)]]]]), where [] "
            "destinations with XFER_RAW_SUM hash a slice whose first tile is tile `tile_base` of its object (digest = the "
-           "unfinalised tile sum); returns (digests, status, device_ms).")
+           "unfinalised tile sum), and a window (lo, hi) sets XFER_WINDOW: the whole object is read and verified but only "
+           "bytes [lo, hi) are stored, object byte x at dst + x (pass dst = buffer - lo; one destination; with "
+           "ChecksumAlgo.NONE only the window's 16-byte aligned span is read); returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
              std::vector<gpu::Fp8Item> v;
