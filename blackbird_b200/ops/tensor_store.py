@@ -165,8 +165,10 @@ class TensorStore:
         """Rows [start, stop) along dim 0 of each stored tensor, as new tensors (`t[start:stop]`): a tensor-parallel rank
         loads its shard of a weight, a reader a few KV blocks of a layer.  Only the byte range of those rows is stored
         into the result; every shard of the object that overlaps it is still read whole and verified against its
-        digest.  IndexError unless 0 <= start <= stop <= shape[0]; 0-d tensors have no rows.  MXFP8-packed tensors are
-        read whole, unpacked and sliced (correct, but not a ranged read)."""
+        digest.  IndexError unless 0 <= start <= stop <= shape[0]; 0-d tensors have no rows.  MXFP8-packed tensors take
+        the fused element-range get: the whole packed object is read and verified, only the rows' elements are unpacked
+        and stored.  Packed tensors the fused kernel cannot read (striped, demoted to a host tier) are read whole,
+        unpacked and sliced."""
         device = device or torch.device("cuda", torch.cuda.current_device())
         keys, starts, stops = list(keys), list(starts), list(stops)
         if not len(keys) == len(starts) == len(stops):
@@ -180,9 +182,27 @@ class TensorStore:
         result = [None] * len(keys)
         packed = [i for i, m in enumerate(metas) if m["packed"]]
         if packed:
-            whole = self.batch_get([keys[i] for i in packed], device)
-            for i, t in zip(packed, whole):
-                result[i] = t[starts[i]:stops[i]].clone()
+            # Elements [lo, hi) of the (padded) packed object; their window ends before any pad.  Each result sits at
+            # element lo % 8 of its own allocation, so that the virtual base ptr - 2 * lo is 16-byte aligned and every
+            # row size takes the fused path.
+            los, counts, ptrs = [], [], []
+            for i in packed:
+                m = metas[i]
+                row = torch.Size(m["shape"][1:]).numel()
+                lo, count = starts[i] * row, (stops[i] - starts[i]) * row
+                buf = torch.empty(count + lo % 8, dtype=torch.bfloat16, device=device)
+                result[i] = buf[lo % 8:].view([stops[i] - starts[i]] + m["shape"][1:])
+                los.append(lo), counts.append(count), ptrs.append(result[i].data_ptr())
+            ecs = self.client.batch_get_device_fp8_range([keys[i] for i in packed], ptrs, [metas[i]["padded_numel"] for i in packed], los,
+                                                         counts, self._stream())
+            bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+            if bad:
+                raise RuntimeError(f"fused fp8 range get failed: {bad[:3]}")
+            unfused = [i for i, e in zip(packed, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
+            if unfused:
+                whole = self.batch_get([keys[i] for i in unfused], device)
+                for i, t in zip(unfused, whole):
+                    result[i] = t[starts[i]:stops[i]].clone()
         ranged = [i for i, m in enumerate(metas) if not m["packed"]]
         if ranged:
             offsets, lengths = [], []

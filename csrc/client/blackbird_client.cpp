@@ -666,18 +666,55 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8(const std::vector<O
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                              const std::vector<uint64_t>& n_elems, void* stream) {
+  return get_device_fp8(keys, bf16_ptrs, n_elems, nullptr, stream);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                                   const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
+                                                                   const std::vector<uint64_t>& elem_counts, void* stream) {
+  if (elem_offsets.size() != keys.size() || elem_counts.size() != keys.size())
+    return std::vector<ErrorCode>(keys.size(), keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  std::vector<ByteRange> ranges(keys.size());
+  for (size_t i = 0; i < keys.size(); ++i) ranges[i] = {elem_offsets[i], elem_counts[i]};
+  auto out = get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream);
+  uint64_t n = 0, bytes = 0;
+  for (size_t i = 0; i < out.size(); ++i)
+    if (out[i] == ErrorCode::OK) ++n, bytes += 2 * elem_counts[i];
+  metrics_.inc("device_get_fp8_range_total", n);
+  metrics_.inc("device_get_fp8_range_bytes_total", bytes);
+  return out;
+}
+
+std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                       const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size()) return out;
+  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size())) return out;
   BB_TRACE_SPAN("batch_get_device_fp8", keys.size());
   auto placed = keystone_->batch_get_workers(keys);
   std::vector<std::vector<size_t>> candidates(keys.size());
   std::vector<size_t> idx;
+  // Where element 0 would land: the caller's pointer, or for a range get the virtual base `ptr - 2 * offset` (the kernel
+  // stores element x at base + 2x and never touches an address outside the range).
+  std::vector<void*> bases = bf16_ptrs;
+  for (size_t i = 0; ranges && i < keys.size(); ++i)
+    bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * (*ranges)[i].offset);
   for (size_t i = 0; i < keys.size(); ++i) {
     if (!placed[i].ok()) {
       out[i] = placed[i].error();
       continue;
+    }
+    if (ranges) {
+      const ByteRange& r = (*ranges)[i];
+      if (r.offset + r.length < r.offset || r.offset + r.length > n_elems[i]) {
+        out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
+        continue;
+      }
+      if (r.length == 0) {  // nothing to read or store
+        out[i] = ErrorCode::OK;
+        continue;
+      }
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
@@ -697,6 +734,12 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<O
       out[i] = ErrorCode::NOT_IMPLEMENTED;  // demoted to a host tier, striped, other digest: caller gets + unpacks instead
       continue;
     }
+    // a range whose virtual base the kernel cannot store from (TMA needs 16 bytes) fails alone, so that the rest of the
+    // batch still takes the fused launch; the caller reads it whole and slices instead
+    if (ranges && (reinterpret_cast<uintptr_t>(bases[i]) & 15)) {
+      out[i] = ErrorCode::NOT_IMPLEMENTED;
+      continue;
+    }
     candidates[i] = std::move(order);
     idx.push_back(i);
   }
@@ -710,7 +753,9 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<O
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      ops.push_back(DeviceFp8Op{&placed[i].value()[candidates[i][attempt]].shards[0], bf16_ptrs[i], n_elems[i], {}});
+      DeviceFp8Op op{&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}};
+      if (ranges) op.win_lo = (*ranges)[i].offset, op.win_hi = (*ranges)[i].offset + (*ranges)[i].length;
+      ops.push_back(std::move(op));
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -740,16 +785,21 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<O
       std::vector<void*> rptrs;
       std::vector<uint64_t> rn;
       std::vector<size_t> ridx;
+      std::vector<ByteRange> rranges;
       for (size_t k = 0; k < bad.size(); ++k) {
         const size_t i = bad[k];
-        if (!again[k].ok()) out[i] = again[k].error();
-        // changed placements, or (once) the same ones: a remove + re-put can land on the very same extent and be read half-written
-        else if (!(again[k].value() == placed[i].value()) || fp8_refresh_depth == 0) rkeys.push_back(keys[i]), rptrs.push_back(bf16_ptrs[i]), rn.push_back(n_elems[i]), ridx.push_back(i);
+        if (!again[k].ok()) {
+          out[i] = again[k].error();
+        } else if (!(again[k].value() == placed[i].value()) || fp8_refresh_depth == 0) {
+          // changed placements, or (once) the same ones: a remove + re-put can land on the very same extent and be read half-written
+          rkeys.push_back(keys[i]), rptrs.push_back(bf16_ptrs[i]), rn.push_back(n_elems[i]), ridx.push_back(i);
+          if (ranges) rranges.push_back((*ranges)[i]);
+        }
       }
       if (!rkeys.empty()) {
         metrics_.inc("get_placement_refresh_total", rkeys.size());
         ++fp8_refresh_depth;
-        auto recs = batch_get_device_fp8(rkeys, rptrs, rn, stream);
+        auto recs = get_device_fp8(rkeys, rptrs, rn, ranges ? &rranges : nullptr, stream);  // the same ranges again
         --fp8_refresh_depth;
         for (size_t k = 0; k < ridx.size(); ++k) out[ridx[k]] = recs[k];
       }
@@ -1524,6 +1574,8 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
   if (status) status->assign(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
+    const bool whole = op.win_lo == 0 && op.win_hi == UINT64_MAX;
+    if (!whole && (op.win_lo > op.win_hi || op.win_hi > op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
@@ -1531,7 +1583,13 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       continue;
     }
     if (ec != ErrorCode::OK) return ec;
-    mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
+    if (whole) {
+      mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
+    } else if (op.win_hi > op.win_lo) {  // as the kernel does: the whole object is read and verified, only the window stored
+      std::vector<uint16_t> wide(op.n_elems);
+      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
+      std::memcpy(static_cast<uint16_t*>(op.wide) + op.win_lo, wide.data() + op.win_lo, 2 * (op.win_hi - op.win_lo));
+    }
   }
   return ErrorCode::OK;
 }

@@ -64,9 +64,12 @@ struct DeviceShardOp {
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
 struct DeviceFp8Op {
   const ShardPlacement* placement = nullptr;
-  void* wide = nullptr;     // client's bf16 tensor (source of a put, destination of a get)
+  void* wide = nullptr;     // client's bf16 tensor (source of a put, destination of a get: where element 0 lands)
   uint64_t n_elems = 0;
   std::vector<const ShardPlacement*> replicas;  // put: the other copies (<= 2), written by the same tile pass
+  // Get of an element range: only elements [win_lo, win_hi) are stored, element x at wide + 2x (wide is then the virtual
+  // base `buffer - 2 * win_lo`); the whole packed object is still read and verified.  The default is the whole object.
+  uint64_t win_lo = 0, win_hi = UINT64_MAX;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -130,6 +133,16 @@ class BlackbirdClient {
                                               const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                               const std::vector<uint64_t>& n_elems, void* stream);
+  // Element-range gets of packed tensors: elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of the n_elems[i]-element
+  // object i, unpacked to bf16, land at bf16_ptrs[i].  The whole packed object is read and verified against its digest (a
+  // corrupt byte outside the range still fails that copy over to the next replica); only the range is unpacked and stored,
+  // and no byte outside it is ever written.  Per object: VALUE_OUT_OF_RANGE when the range passes n_elems or overflows; a
+  // zero count is OK and moves nothing; NOT_IMPLEMENTED when the object is not fusable (as batch_get_device_fp8) or when
+  // the virtual base bf16_ptrs[i] - 2 * elem_offsets[i] is not 16-byte aligned -- the rest of the batch still takes the
+  // fused launch.  On CHECKSUM_MISMATCH the range's contents are unspecified.
+  std::vector<ErrorCode> batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                    const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
+                                                    const std::vector<uint64_t>& elem_counts, void* stream);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -183,6 +196,10 @@ class BlackbirdClient {
   };
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
+  // batch_get_device_fp8 and batch_get_device_fp8_range: `ranges` null = whole tensors, else object i's element range
+  // (offset and length in elements) into bf16_ptrs[i].
+  std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream);
   ErrorCode get_with_refresh(const ObjectKey& key, uint8_t* (*alloc)(void*, size_t), void* ctx, size_t capacity, size_t* out_size);
   static uint64_t shard_offset(const ShardPlacement& s);
   static ChecksumAlgo algo_of(const std::vector<CopyPlacement>& copies, ChecksumAlgo hint);

@@ -537,6 +537,8 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     if ((reinterpret_cast<uintptr_t>(it.wide) | reinterpret_cast<uintptr_t>(it.packed)) & 15) return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
+    if ((it.win_lo != 0 || it.win_hi != UINT64_MAX) && (!unpack || it.win_lo > it.win_hi || it.win_hi > it.n_elems))
+      return ErrorCode::INVALID_ARGUMENT;
     for (uint32_t r = 1; r < nrep; ++r)
       if (!it.more_packed[r - 1] || (reinterpret_cast<uintptr_t>(it.more_packed[r - 1]) & 15)) return ErrorCode::INVALID_ADDRESS;
     auto* payload = static_cast<uint8_t*>(it.packed);
@@ -550,6 +552,11 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     d.expect = 0;
     d.flags = 0;
     d.reserved = 0;
+    if (unpack && (it.win_lo > 0 || it.win_hi < it.n_elems)) {  // whole-object gets keep exactly the descriptors they had
+      d.flags = XFER_WINDOW;
+      d.win.lo = 2 * it.win_lo;
+      d.win.hi = 2 * it.win_hi;
+    }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
     const uint64_t nt_full = it.n_elems / kTileBytes;

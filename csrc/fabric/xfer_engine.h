@@ -48,6 +48,9 @@ struct Fp8Item {
   uint64_t n_elems = 0;   // multiple of 32 (whole MX blocks)
   uint64_t expect = 0;    // unpack + verify: digest recorded at put time
   bool verify = false;
+  // Unpack only: store elements [win_lo, win_hi) of the object, element x at wide + 2x (wide = caller buffer - 2 * win_lo,
+  // the virtual base).  The whole packed object is still read and verified.  The default is the whole object.
+  uint64_t win_lo = 0, win_hi = UINT64_MAX;
 };
 
 struct XferResult {

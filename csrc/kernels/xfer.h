@@ -21,7 +21,8 @@ enum XferFlags : uint32_t {
   // hashed elsewhere; the host finalises).  With ndst == 0 the descriptor is hash-only (nothing is stored).
   XFER_RAW_SUM = 1u << 2,
   // Store window (range reads): every tile is still loaded and hashed, but only object bytes [win.lo, win.hi) are
-  // stored.  Only with ndst == 1, never with XFER_MULTIMEM or XFER_RAW_SUM.
+  // stored.  Only with ndst == 1, never with XFER_MULTIMEM or XFER_RAW_SUM.  The fused MXFP8 get honours it too, with the
+  // window in bf16 bytes of the unpacked object; an MXFP8 put never carries it.
   XFER_WINDOW = 1u << 3,
 };
 
@@ -120,7 +121,8 @@ int xfer_smem_bytes(int algo);
 // Fused MXFP8 transfer (xfer_mxfp8.cu).  The packed object is one contiguous [payload n][scales n/32] extent.
 // Descriptors: pack (put): src = bf16 source, dst[0..ndst-1] = base of the packed object in every replica (the scales
 // follow the payload), nbytes = payload bytes (= elements, a multiple of kTileBytes); unpack (get): src = base of the
-// packed object, dst[0] = bf16 destination.  `sum_ws` receives the unfinalised
+// packed object, dst[0] = bf16 destination (where element 0 lands); an unpack descriptor may carry XFER_WINDOW, whose
+// `win` is then in bf16 bytes of the object ([2 * first element, 2 * end element)).  `sum_ws` receives the unfinalised
 // BBH64 sum of the payload tiles per descriptor (must be zero on entry); descs / tile_start are device tables.
 int launch_xfer_fp8(const XferLaunch& l, bool unpack);
 int xfer_fp8_smem_bytes();

@@ -83,6 +83,26 @@ __device__ __forceinline__ uint2 cta_tile_run(uint32_t total_tiles) {
   return make_uint2(t0, t0 < total_tiles ? min(tpc, total_tiles - t0) : 0);
 }
 
+// ---------------------------------------------------------------- store window
+// The part of one tile a store warp writes: object bytes [off, off + bytes) of the tile, cut to the store window [lo, hi)
+// (object offsets) when `windowed`.  [x0, x1) is that span, tile-relative (x0 == x1: nothing to store); its 16-byte
+// aligned middle [a0, a1) goes out by TMA; the head [x0, h1) and the tail [tb, x1) are under 16 bytes each and are
+// stored byte-wise by lanes 0-15 and 16-31.  Without a window x0 = 0, so there is no head.
+struct TileSpan {
+  uint32_t x0, x1, a0, a1, h1, tb;
+};
+__device__ __forceinline__ TileSpan tile_span(uint64_t off, uint32_t bytes, bool windowed, uint64_t lo, uint64_t hi) {
+  uint32_t x0 = 0, x1 = bytes;
+  if (windowed) {
+    x0 = static_cast<uint32_t>(min(max(lo, off) - off, static_cast<uint64_t>(bytes)));
+    x1 = static_cast<uint32_t>(max(min(hi, off + bytes), off) - off);
+    x1 = max(x1, x0);
+  }
+  const uint32_t a0 = (x0 + 15u) & ~15u, a1 = max(x1 & ~15u, a0);
+  const uint32_t h1 = min(a0, x1), tb = max(a1, h1);
+  return {x0, x1, a0, a1, h1, tb};
+}
+
 // ---------------------------------------------------------------- warp helpers
 __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
   const uint32_t lo = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v), m);

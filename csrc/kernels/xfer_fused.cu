@@ -294,17 +294,8 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
       const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kTileBytes;
       const uint32_t ndst = m.ndst_flags & 0xFFu;
       const uint32_t flags = m.ndst_flags >> 8;
-      // Tile-relative span [x0, x1) to store: the whole tile, or its part inside the window [dst[1], dst[2]) (object
-      // offsets).  Its 16-byte aligned middle [a0, a1) goes out by TMA; the head [x0, h1) and the tail [t0, x1) are
-      // under 16 bytes each and are stored by lanes 0-15 and 16-31.  Without a window x0 = 0, so there is no head.
-      uint32_t x0 = 0, x1 = m.bytes;
-      if (flags & XFER_WINDOW) {
-        x0 = static_cast<uint32_t>(min(max(m.dst[1], off) - off, static_cast<uint64_t>(m.bytes)));
-        x1 = static_cast<uint32_t>(max(min(m.dst[2], off + m.bytes), off) - off);
-        x1 = max(x1, x0);
-      }
-      const uint32_t a0 = (x0 + 15u) & ~15u, a1 = max(x1 & ~15u, a0);
-      const uint32_t h1 = min(a0, x1), tb = max(a1, h1);
+      // the whole tile, or its part inside the window [dst[1], dst[2]) (object offsets)
+      const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, m.bytes, flags & XFER_WINDOW, m.dst[1], m.dst[2]);
       if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);
         for (uint32_t o = a0 + lane * 16; o < a1; o += 512)

@@ -8,6 +8,9 @@
 //                   is read from HBM once and only the 0.52x packed bytes cross NVLink (once per replica).
 //   get  (UNPACK) : TMA loads payload tile + scales from the slab -> tensor-core hash of the payload tile ->
 //                   8 unpack warps expand to bf16 in shared memory -> TMA stores the 32 KiB tile to the caller.
+//                   With XFER_WINDOW (element-range gets) only the bf16 bytes [win.lo, win.hi) of the object are
+//                   stored, object byte x at dst[0] + x; every tile is still loaded and hashed, so the digest is the
+//                   whole object's, and tiles outside the window are not unpacked.
 //
 // The stored object keeps the layout of the unfused path ([E4M3 payload n][E8M0 scales n/32], common/mxfp8.h), and so
 // does its digest: BBH64 is a sum of per-tile terms, this kernel accumulates the payload tiles (tile index 0..T-1)
@@ -46,7 +49,8 @@ constexpr int kFpStoreLag = 1;
 __constant__ uint64_t c_fp_col_mul[tchash::kN];
 
 struct FpMeta {            // 64 bytes
-  uint64_t dst[kMaxDst];   // pack: this tile's payload address in every replica; unpack: dst[0] = bf16 destination
+  uint64_t dst[kMaxDst];   // pack: this tile's payload address in every replica; unpack: dst[0] = the tile's bf16
+                           // destination, dst[1..2] = the object's store window [lo, hi) in bf16 bytes
   int64_t scales_delta;    // pack: (tile's scales address) - (tile's payload address), the same in every replica
   uint32_t desc;
   uint32_t tile_in_obj;
@@ -145,7 +149,10 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           e.src = src + static_cast<uint64_t>(ti) * kTileBytes;  // payload tile in the slab
           e.src_scales = e.src + e.m.scales_delta;               // its scales
           e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kWideBytes;  // bf16 destination
-          e.m.dst[1] = e.m.dst[2] = 0;
+          // store window in bf16 bytes of the object (XferDesc::win); a whole-object get stores [0, 2^64), i.e. every tile whole
+          const bool win = d.flags & XFER_WINDOW;
+          e.m.dst[1] = win ? d1 : 0;
+          e.m.dst[2] = win ? d2 : ~0ull;
           e.m.ndst = 1;
         } else {
           e.src = src + static_cast<uint64_t>(ti) * kWideBytes;  // bf16 source tile
@@ -197,10 +204,15 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
       const uint32_t st = it % kRing, par = (it / kRing) & 1u;
       if constexpr (UNPACK) {
         mbar_wait(&s.w_full[st], par);
+        const FpMeta& m = s.w_meta[st];
+        // the tile's bf16 bytes inside the store window: the middle by TMA, head and tail byte-wise (as bb_xfer does)
+        const auto [x0, x1, a0, a1, h1, tb] = tile_span(static_cast<uint64_t>(m.tile_in_obj) * kWideBytes, 2u * m.valid, true, m.dst[1], m.dst[2]);
         if (lane == 0) {
-          bulk_s2g(reinterpret_cast<void*>(s.w_meta[st].dst[0]), s.wide[st], 2u * s.w_meta[st].valid);
+          if (a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[0] + a0), &s.wide[st][a0], a1 - a0);
           bulk_commit();
         }
+        const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);
+        if (o < (lane < 16 ? h1 : x1)) *reinterpret_cast<uint8_t*>(m.dst[0] + o) = s.wide[st][o];
       } else {
         mbar_wait(&s.t_full[st], par);
         const FpMeta& m = s.t_meta[st];
@@ -281,12 +293,18 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
       if constexpr (UNPACK) {
         mbar_wait(&s.t_full[ts], tp);         // payload + scales landed
         mbar_wait(&s.w_empty[ws], wp ^ 1u);   // wide slot drained by the store warp
+        const FpMeta& m = s.t_meta[ts];
+        // a tile outside the store window is hashed (epilogue) but neither unpacked nor stored; one that overlaps it is
+        // unpacked whole.  The barrier arrivals below are the same for every tile.
+        const TileSpan sp = tile_span(static_cast<uint64_t>(m.tile_in_obj) * kWideBytes, 2u * m.valid, true, m.dst[1], m.dst[2]);
         const uint2* pay = reinterpret_cast<const uint2*>(s.tile[ts]);
         uint4* out = reinterpret_cast<uint4*>(s.wide[ws]);
+        if (sp.x1 > sp.x0) {
 #pragma unroll 4
-        for (uint32_t k = 0; k < kPer / 32; ++k) {
-          const uint32_t c = cw * kPer + k * 32 + lane;
-          out[c] = unpack_chunk(pay[c], s.scales[ts][c >> 2]);
+          for (uint32_t k = 0; k < kPer / 32; ++k) {
+            const uint32_t c = cw * kPer + k * 32 + lane;
+            out[c] = unpack_chunk(pay[c], s.scales[ts][c >> 2]);
+          }
         }
         if (cw == 0 && lane < 4) reinterpret_cast<uint4*>(&s.w_meta[ws])[lane] = reinterpret_cast<const uint4*>(&s.t_meta[ts])[lane];
         fence_proxy_async_smem();  // generic-proxy writes -> TMA store

@@ -109,6 +109,11 @@ void bind_gpu(py::module_& m) {
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
                if (t.size() > 3) it.expect = t[3].cast<uint64_t>(), it.verify = true;
+               if (t.size() > 4 && !t[4].is_none()) {
+                 auto w = t[4].cast<std::pair<uint64_t, uint64_t>>();
+                 it.win_lo = w.first;
+                 it.win_hi = w.second;
+               }
                v.push_back(it);
              }
              XferResult res;
@@ -120,8 +125,11 @@ void bind_gpu(py::module_& m) {
            },
            py::arg("items"), py::arg("unpack"), py::arg("stream") = 0,
            "Fused MXFP8 put (unpack=False: bf16 -> packed slab object) or get (unpack=True); items = (bf16_ptr, packed_ptr "
-           "| [packed_ptr, ...], n_elems[, expected_digest]), where a put writes every packed replica in the list (1..3) and "
-           "a get reads the first; returns (digests of the packed objects, status, device_ms).")
+           "| [packed_ptr, ...], n_elems[, expected_digest[, (lo, hi)]]), where a put writes every packed replica in the list "
+           "(1..3) and a get reads the first.  A get with a window (lo, hi) reads and verifies the whole packed object but "
+           "stores only elements [lo, hi), element x at bf16_ptr + 2x (pass bf16_ptr = buffer - 2 * lo, 16-byte aligned); a "
+           "window on a put, lo > hi or hi > n_elems is INVALID_ARGUMENT.  Returns (digests of the packed objects, status, "
+           "device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
