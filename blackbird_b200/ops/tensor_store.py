@@ -179,6 +179,9 @@ class TensorStore:
                 raise IndexError(f"{k}: a 0-d tensor has no rows")
             if not 0 <= a <= b <= m["shape"][0]:
                 raise IndexError(f"{k}: rows [{a}, {b}) outside [0, {m['shape'][0]}]")
+        return self._get_rows(keys, metas, starts, stops, device)
+
+    def _get_rows(self, keys: list, metas: list, starts: list, stops: list, device: torch.device) -> list:
         result = [None] * len(keys)
         packed = [i for i, m in enumerate(metas) if m["packed"]]
         if packed:
@@ -223,6 +226,66 @@ class TensorStore:
     def get_rows(self, key: str, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
         """`t[start:stop]` of the tensor stored under `key` (see batch_get_rows)."""
         return self.batch_get_rows([key], [start], [stop], device)[0]
+
+    def batch_get_slices(self, keys: Sequence[str], dims: Sequence[int], starts: Sequence[int], stops: Sequence[int],
+                         device: Optional[torch.device] = None) -> list:
+        """`t.narrow(dim, start, stop - start).contiguous()` of each stored tensor, along any dimension: a row-parallel rank
+        loads its columns `W[:, k0:k1]` of a weight stored whole, a decode rank its heads `kv[:, :, h0:h1, :]` of a KV
+        layer.  Negative dims count from the end.  IndexError for 0-d tensors, a dim out of range, or bounds outside
+        0 <= start <= stop <= shape[dim].
+
+        dim 0 is batch_get_rows.  Along any other dim the slice is prod(shape[:dim]) rows of the same width, one per
+        index of the outer dims, and the strided device get stores just those rows, densely: every shard of the object
+        that holds a byte of them is read whole and verified against its digest, shards wholly between two rows are not
+        read.  Each result starts at byte `offset % 16` of its own allocation, so that single-shard tensors take the fused
+        kernel for every slice whose row gap is a multiple of 16 bytes; other slices are staged through the host.
+        MXFP8-packed tensors are read whole through the fused get (the unpack kernel has no strided store) and narrowed."""
+        device = device or torch.device("cuda", torch.cuda.current_device())
+        keys, dims, starts, stops = list(keys), list(dims), list(starts), list(stops)
+        if not len(keys) == len(dims) == len(starts) == len(stops):
+            raise ValueError("keys, dims, starts and stops differ in length")
+        metas = self._metas(keys)
+        for j, (k, m, a, b) in enumerate(zip(keys, metas, starts, stops)):
+            shape = m["shape"]
+            if not shape:
+                raise IndexError(f"{k}: a 0-d tensor has no dimension to slice")
+            if not -len(shape) <= dims[j] < len(shape):
+                raise IndexError(f"{k}: dim {dims[j]} out of range for {len(shape)} dimensions")
+            dims[j] %= len(shape)
+            if not 0 <= a <= b <= shape[dims[j]]:
+                raise IndexError(f"{k}: [{a}, {b}) outside [0, {shape[dims[j]]}] along dim {dims[j]}")
+        result = [None] * len(keys)
+        first = [i for i, d in enumerate(dims) if d == 0]
+        if first:
+            rows = self._get_rows([keys[i] for i in first], [metas[i] for i in first], [starts[i] for i in first],
+                                  [stops[i] for i in first], device)
+            for i, t in zip(first, rows):
+                result[i] = t
+        packed = [i for i, m in enumerate(metas) if dims[i] != 0 and m["packed"]]
+        if packed:
+            for i, t in zip(packed, self.batch_get([keys[i] for i in packed], device)):
+                result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).contiguous()
+        strided = [i for i, m in enumerate(metas) if dims[i] != 0 and not m["packed"]]
+        if strided:
+            offsets, widths, pitches, nrows = [], [], [], []
+            for i in strided:
+                shape, d, dtype = metas[i]["shape"], dims[i], _DTYPES[metas[i]["dtype"]]
+                inner = torch.Size(shape[d + 1:]).numel() * torch.empty((), dtype=dtype).element_size()
+                offset, width = starts[i] * inner, (stops[i] - starts[i]) * inner
+                rows = torch.Size(shape[:d]).numel()
+                buf = torch.empty(rows * width + offset % 16, dtype=torch.uint8, device=device)
+                result[i] = buf[offset % 16:].view(dtype).view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
+                offsets.append(offset), widths.append(width), pitches.append(shape[d] * inner), nrows.append(rows)
+            ecs = self.client.batch_get_device_strided([keys[i] for i in strided], [result[i].data_ptr() for i in strided], offsets,
+                                                       widths, pitches, nrows, self._stream())
+            bad = [(keys[i], e) for i, e in zip(strided, ecs) if e != _bb.ErrorCode.OK]
+            if bad:
+                raise RuntimeError(f"strided get failed: {bad[:3]}")
+        return result
+
+    def get_slice(self, key: str, dim: int, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
+        """`t.narrow(dim, start, stop - start).contiguous()` of the tensor stored under `key` (see batch_get_slices)."""
+        return self.batch_get_slices([key], [dim], [start], [stop], device)[0]
 
     def remove(self, keys: Sequence[str]) -> None:
         self.client.batch_remove(list(keys) + [k + "#meta" for k in keys])

@@ -467,7 +467,18 @@ ErrorCode BlackbirdClient::transfer_put(const std::vector<CopyPlacement>& copies
   });
 }
 
-ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo, uint64_t hi) {
+// Whether a get of object bytes [lo, hi) reads shard [off, off + len): the shard overlaps the range and, for rows of
+// `width` bytes every `pitch` bytes from lo (pitch 0: one range), holds at least one byte of a row.  A shard that lies
+// wholly in the gap between two rows holds none.
+static bool reads_shard(uint64_t off, uint64_t len, uint64_t lo, uint64_t hi, uint64_t pitch, uint64_t width) {
+  if (!(off < hi && off + len > lo)) return false;
+  if (pitch == 0) return true;
+  const uint64_t y = std::max(off, lo) - lo, end = std::min(off + len, hi) - lo;  // the overlap, relative to the first row
+  return y % pitch < width || (y / pitch + 1) * pitch < end;
+}
+
+ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo, uint64_t hi,
+                                        uint64_t pitch, uint64_t width) {
   const bool whole = lo == 0 && hi == UINT64_MAX;
   ErrorCode last = ErrorCode::NO_COMPLETE_WORKER;
   for (const auto& copy : copies) {  // replica fail-over (reference reads copy 0 only, :283-287)
@@ -484,7 +495,7 @@ ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies
       off += copy.shards[s].length;
     }
     last = parallel_for(copy.shards.size(), opts_.io_parallelism, [&](size_t s) {
-      if (!whole && !(offs[s] < hi && offs[s] + copy.shards[s].length > lo)) return ErrorCode::OK;  // outside the range
+      if (!whole && !reads_shard(offs[s], copy.shards[s].length, lo, hi, pitch, width)) return ErrorCode::OK;  // nothing to store
       return read_shard(copy.shards[s], dst + offs[s], copy.shards[s].checksum_algo);
     });
     if (last == ErrorCode::OK) return ErrorCode::OK;
@@ -1162,14 +1173,42 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector
   return out;
 }
 
-// Shard [off, off + len) of an object takes part in a get of object bytes [lo, hi): every shard of a whole-object get
-// (`all`, zero-length objects included), else the shards that overlap the range.
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                                 const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                                                 const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows,
+                                                                 void* stream) {
+  const size_t n = keys.size();
+  if (offsets.size() != n || widths.size() != n || pitches.size() != n || rows.size() != n)
+    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  std::vector<ByteRange> ranges(n);
+  std::vector<size_t> lens(n);
+  for (size_t i = 0; i < n; ++i) {
+    ranges[i] = {offsets[i], widths[i], pitches[i], rows[i]};
+    uint64_t total = 0;
+    lens[i] = __builtin_mul_overflow(rows[i], widths[i], &total) ? SIZE_MAX : static_cast<size_t>(total);
+  }
+  auto out = get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr);
+  uint64_t k = 0, bytes = 0;
+  for (size_t i = 0; i < n; ++i)
+    if (out[i] == ErrorCode::OK) ++k, bytes += lens[i];
+  metrics_.inc("device_get_strided_total", k);
+  metrics_.inc("device_get_strided_bytes_total", bytes);
+  return out;
+}
+
+// Shard [off, off + len) of an object takes part in a get: every shard of a whole-object get (`all`, zero-length objects
+// included), else the shards that hold a byte the get stores (reads_shard): of the object bytes [lo, hi), and for a
+// strided get (pitch != 0) only those of its rows, byte lo + y with y % pitch < width.
 namespace {
 struct GetSpan {
   uint64_t lo = 0, hi = 0;
+  uint64_t pitch = 0, width = 0;
   bool all = true;
-  bool overlaps(uint64_t off, uint64_t len) const { return all || (off < hi && off + len > lo); }
+  bool reads(uint64_t off, uint64_t len) const { return all || reads_shard(off, len, lo, hi, pitch, width); }
 };
+
+// Rows with gaps between them; anything else (one row, or rows that touch) is one byte range.
+bool has_gaps(uint64_t rows, uint64_t width, uint64_t pitch) { return rows > 1 && width < pitch; }
 }  // namespace
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1187,12 +1226,16 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   std::vector<bool> pending(keys.size(), false);
   std::vector<GetSpan> span(keys.size());
   // Where object byte 0 would land: the caller's pointer, or for a range get the virtual base `ptr - offset` (the fabric
-  // stores object byte x at base + x and never touches an address outside the range).
+  // stores object byte x at base + x and never touches an address outside the range).  A strided get passes the caller's
+  // pointer, where its row 0 lands (DeviceShardOp::win_row).
   std::vector<void*> range_bases;
   if (ranges) {
     range_bases.resize(keys.size());
-    for (size_t i = 0; i < keys.size(); ++i)
-      range_bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - (*ranges)[i].offset);
+    for (size_t i = 0; i < keys.size(); ++i) {
+      const ByteRange& r = (*ranges)[i];
+      range_bases[i] = has_gaps(r.rows, r.length, r.pitch) ? dev_ptrs[i]
+                                                           : reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - r.offset);
+    }
   }
   const std::vector<void*>& bases = ranges ? range_bases : dev_ptrs;
 
@@ -1205,7 +1248,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       uint64_t off = 0;
       for (size_t s = 0; s < copy.shards.size(); ++s) {
         const uint64_t len = copy.shards[s].length;
-        if (sp.overlaps(off, len)) {
+        if (sp.reads(off, len)) {
           DeviceShardOp op;
           op.item = i;
           op.copy = copy_choice[i] % copies.size();
@@ -1215,6 +1258,14 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           if (!sp.all) {
             op.win_lo = std::max(sp.lo, off) - off;
             op.win_hi = std::min(sp.hi, off + len) - off;
+          }
+          if (sp.pitch) {  // shard byte x is byte x + d of the rows: row floor((x + d) / pitch), d = off - lo
+            const int64_t d = static_cast<int64_t>(off) - static_cast<int64_t>(sp.lo), p = static_cast<int64_t>(sp.pitch);
+            const int64_t row = d / p - (d % p < 0 ? 1 : 0);
+            op.win_pitch = sp.pitch;
+            op.win_width = sp.width;
+            op.win_phase = static_cast<uint64_t>(d - row * p);
+            op.win_row = row;
           }
           ops.push_back(std::move(op));
         }
@@ -1301,15 +1352,32 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       GetSpan& sp = span[i];
       if (ranges) {
         const ByteRange& r = (*ranges)[i];
-        if (r.offset + r.length < r.offset || r.offset + r.length > size) {
+        // the rows span object bytes [offset, offset + (rows - 1) * pitch + length); rows that touch are one range
+        uint64_t extent = r.length;
+        if (r.rows != 1) {
+          if (r.rows > 1 && r.length > r.pitch) {
+            out[i] = ErrorCode::INVALID_ARGUMENT;
+            continue;
+          }
+          if (r.rows == 0 || r.length == 0) {  // nothing to read or store
+            out[i] = ErrorCode::OK;
+            continue;
+          }
+          if (__builtin_mul_overflow(r.rows - 1, r.pitch, &extent) || __builtin_add_overflow(extent, r.length, &extent)) {
+            out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
+            continue;
+          }
+        }
+        if (r.offset + extent < r.offset || r.offset + extent > size) {
           out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
           continue;
         }
-        if (r.length == 0) {  // nothing to read or store
+        if (extent == 0) {  // nothing to read or store
           out[i] = ErrorCode::OK;
           continue;
         }
-        sp = {r.offset, r.offset + r.length, false};
+        sp = {r.offset, r.offset + extent, 0, 0, false};
+        if (has_gaps(r.rows, r.length, r.pitch)) sp.pitch = r.pitch, sp.width = r.length;
       } else {
         if (size > capacity[i]) {
           out[i] = ErrorCode::BUFFER_OVERFLOW;
@@ -1325,15 +1393,30 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         size_t n = 0;
         uint64_t off = 0;
         for (const auto& sh : c.shards) {
-          if (sp.overlaps(off, sh.length)) f(sh), ++n;
+          if (sp.reads(off, sh.length)) f(sh), ++n;
           off += sh.length;
         }
         return n;
       };
       // (the spread over replicas only matters when there is more than one; thousands of single-copy objects skip the hash)
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
-      // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
-      const bool aligned = fabric_aligned(bases[i], copies);
+      // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned).  A strided get
+      // needs every row co-aligned with the tiles of each shard it reads (XferItem::win_pitch): the virtual base aligned at
+      // those shards' starts, and the gap between rows a multiple of 16 bytes.
+      bool aligned;
+      if (sp.pitch) {
+        const uintptr_t vbase = reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.lo;
+        aligned = (sp.pitch - sp.width) % 16 == 0;
+        for (const auto& c : copies) {
+          uint64_t off = 0;
+          for (const auto& sh : c.shards) {
+            if (sp.reads(off, sh.length) && (vbase + off) % 16) aligned = false;
+            off += sh.length;
+          }
+        }
+      } else {
+        aligned = fabric_aligned(bases[i], copies);
+      }
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
         bool local = true;
@@ -1361,8 +1444,16 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       if (!found) {
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
-        ErrorCode ec = sp.all ? transfer_get(copies, stage.data(), size) : transfer_get(copies, stage.data(), size, sp.lo, sp.hi);
-        if (ec == ErrorCode::OK) ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, sp.hi - sp.lo, stream);
+        ErrorCode ec = sp.all ? transfer_get(copies, stage.data(), size)
+                              : transfer_get(copies, stage.data(), size, sp.lo, sp.hi, sp.pitch, sp.width);
+        if (ec == ErrorCode::OK && sp.pitch) {  // compact the rows on the host: one H2D copy of rows * width bytes
+          const uint64_t nrows = (sp.hi - sp.lo - sp.width) / sp.pitch + 1;
+          std::vector<uint8_t> dense(nrows * sp.width);
+          for (uint64_t r = 0; r < nrows; ++r) std::memcpy(dense.data() + r * sp.width, stage.data() + sp.lo + r * sp.pitch, sp.width);
+          ec = device_->copy_h2d(dev_ptrs[i], dense.data(), dense.size(), stream);
+        } else if (ec == ErrorCode::OK) {
+          ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, sp.hi - sp.lo, stream);
+        }
         out[i] = ec;
         metrics_.inc("device_get_host_staged_total");
         continue;
@@ -1515,7 +1606,22 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
     // dev_ptrs[item] is where object byte 0 would land; for a range get only the window is real memory
     const uintptr_t dst = reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + op.obj_offset;
     ErrorCode ec;
-    if (op.windowed()) {  // as the kernel does: read and verify the whole shard, store only the window
+    if (op.strided()) {  // as the kernel does: read and verify the whole shard, store the window's row segments densely
+      std::vector<uint8_t> whole(op.placement->length);
+      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
+      const uint64_t hi = std::min<uint64_t>(op.win_hi, whole.size());
+      const uintptr_t row0 = reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + static_cast<uintptr_t>(op.win_row) * op.win_width;
+      for (uint64_t x = op.win_lo; ec == ErrorCode::OK && x < hi;) {
+        const uint64_t y = x + op.win_phase, c = y % op.win_pitch;
+        if (c >= op.win_width) {  // in the gap: on to the next row
+          x += op.win_pitch - c;
+          continue;
+        }
+        const uint64_t n = std::min(op.win_width - c, hi - x);
+        std::memcpy(reinterpret_cast<uint8_t*>(row0 + y / op.win_pitch * op.win_width + c), whole.data() + x, n);
+        x += n;
+      }
+    } else if (op.windowed()) {  // as the kernel does: read and verify the whole shard, store only the window
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
       const uint64_t hi = std::min<uint64_t>(op.win_hi, whole.size());

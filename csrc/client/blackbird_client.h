@@ -59,6 +59,13 @@ struct DeviceShardOp {
   // op whose window is not narrower than the shard, the default included, is a whole-shard op.
   uint64_t win_lo = 0, win_hi = UINT64_MAX;
   bool windowed() const { return placement && (win_lo > 0 || win_hi < placement->length); }
+  // Strided get (win_pitch != 0, always with a window): of the shard bytes in [win_lo, win_hi), byte x is stored iff
+  // c = (x + win_phase) % win_pitch < win_width, as row win_row + (x + win_phase) / win_pitch of the caller's dense result:
+  // at dev_ptrs[item] + (win_row + (x + win_phase) / win_pitch) * win_width + c.  dev_ptrs[item] is then where the caller's
+  // row 0 lands, and win_row is negative when the shard starts before the first row.
+  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
+  int64_t win_row = 0;
+  bool strided() const { return win_pitch != 0; }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
@@ -168,6 +175,18 @@ class BlackbirdClient {
   // VALUE_OUT_OF_RANGE when the range passes the end of the object.
   std::vector<ErrorCode> batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                 const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths, void* stream);
+  // Strided gets (a slice along an inner dimension): rows[i] rows of widths[i] bytes, row r being object bytes
+  // [offsets[i] + r * pitches[i], + widths[i]), land densely at dev_ptrs[i] + r * widths[i].  Every shard that holds a stored
+  // byte is read whole and verified; shards that hold none (outside the rows, or wholly inside a gap between them) are not
+  // touched.  The fused path needs the virtual base dev_ptrs[i] - offsets[i] 16-byte aligned at the start of every shard
+  // it reads and, for rows[i] > 1, (pitches[i] - widths[i]) % 16 == 0; any other item is staged through the host (its rows
+  // compacted there, one H2D copy) while the rest of the batch keeps the fused launch.  Per object: INVALID_ARGUMENT for
+  // widths[i] > pitches[i] with rows[i] > 1; VALUE_OUT_OF_RANGE when the last row passes the end of the object or the
+  // arithmetic overflows; OK with nothing read for rows[i] == 0 or widths[i] == 0; Keystone errors as for
+  // batch_get_device_range.  rows[i] == 1 is batch_get_device_range of (offsets[i], widths[i]).
+  std::vector<ErrorCode> batch_get_device_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                  const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                                  const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, void* stream);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }
@@ -187,12 +206,16 @@ class BlackbirdClient {
   ErrorCode transfer_put(const std::vector<CopyPlacement>& copies, const uint8_t* data, ChecksumAlgo algo,
                          keystone::ShardChecksums* sums);
   // Reads the object into dst[0, size) from the first copy that verifies.  With a byte range [lo, hi) only the shards that
-  // overlap it are read (whole, and verified); the other bytes of dst are left as they are.
-  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo = 0, uint64_t hi = UINT64_MAX);
-  // batch_get_device and batch_get_device_range: `ranges` null = whole objects into buffers of `capacity`, else object i's
-  // range into dev_ptrs[i] (capacity[i] = its length, for the chunk plan).
+  // overlap it are read (whole, and verified); with a pitch as well, only those that hold a byte y of it with
+  // (y - lo) % pitch < width.  The other bytes of dst are left as they are.
+  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo = 0, uint64_t hi = UINT64_MAX,
+                         uint64_t pitch = 0, uint64_t width = 0);
+  // batch_get_device, batch_get_device_range and batch_get_device_strided: `ranges` null = whole objects into buffers of
+  // `capacity`, else object i's rows into dev_ptrs[i] (capacity[i] = rows * length, for the chunk plan).  A range is the
+  // single row `rows == 1`.
   struct ByteRange {
     uint64_t offset = 0, length = 0;
+    uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)
   };
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);

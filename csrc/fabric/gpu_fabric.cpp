@@ -689,10 +689,17 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
     it.nbytes = op.placement->length;
     it.expect = op.placement->checksum;
     it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
-    if (op.windowed()) {  // whole-shard ops keep exactly the descriptors they always had
+    if (op.windowed() || op.strided()) {  // whole-shard ops keep exactly the descriptors they always had
       it.flags |= XFER_WINDOW;
       it.win_lo = op.win_lo;
       it.win_hi = std::min(op.win_hi, it.nbytes);
+    }
+    if (op.strided()) {  // row 0 of the shard's pattern is the caller's row win_row (dev_ptrs[item] = the caller's row 0)
+      it.flags |= XFER_STRIDED;
+      it.dst[0] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + static_cast<uintptr_t>(op.win_row) * op.win_width);
+      it.win_pitch = op.win_pitch;
+      it.win_width = op.win_width;
+      it.win_phase = op.win_phase;
     }
     items->push_back(it);
     op_of_item->push_back(k);

@@ -37,6 +37,20 @@ struct SlotRelease {
   uint64_t& ticket;
   ~SlotRelease() { ticket = 0; }
 };
+
+// A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items].
+size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
+
+// Whether every row a strided item's window touches is co-aligned with the tiles: object byte x of row r lands at
+// dst[0] + phase - r * (pitch - width) + x, so that base must be 16-byte aligned for the first row, and the same for every
+// later row.
+bool stride_coaligned(const XferItem& it) {
+  const uint64_t gap = it.win_pitch - it.win_width;
+  const uint64_t r_lo = (it.win_lo + it.win_phase) / it.win_pitch;
+  const uint64_t r_hi = it.win_hi > it.win_lo ? (it.win_hi - 1 + it.win_phase) / it.win_pitch : r_lo;
+  if (r_hi > r_lo && gap % 16) return false;
+  return (reinterpret_cast<uintptr_t>(it.dst[0]) + it.win_phase - r_lo * gap) % 16 == 0;
+}
 }  // namespace
 
 struct XferEngine::Slot {
@@ -74,6 +88,7 @@ struct XferEngine::Slot {
   bool crc = false;
   uint64_t empty_digest = 0;
   std::vector<int32_t> item_to_desc;  // -1 for zero-size items
+  std::vector<XferStride> strides;     // per descriptor up to the last XFER_STRIDED one; empty when the batch has none
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
     uint32_t item;
@@ -90,7 +105,7 @@ Result<std::unique_ptr<XferEngine>> XferEngine::create(int device, uint32_t max_
   int prev = 0;
   if (cudaGetDevice(&prev) != cudaSuccess) return ErrorCode::FABRIC_ERROR;
   if (cudaSetDevice(device) != cudaSuccess) return ErrorCode::FABRIC_ERROR;
-  const size_t tab_bytes = static_cast<size_t>(max_items) * sizeof(XferDesc) + (static_cast<size_t>(max_items) + 1) * 4;
+  const size_t tab_bytes = stride_table_offset(max_items) + static_cast<size_t>(max_items) * sizeof(XferStride);
   const size_t res_bytes = static_cast<size_t>(max_items) * 12;
   bool ok = true;
   for (int i = 0; i < slots && ok; ++i) {
@@ -299,12 +314,16 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   s->item_to_desc.assign(items.size(), -1);
   s->empties.clear();
+  s->strides.clear();
   uint32_t nd = 0;
   bool all_small = small_path_enabled();
   for (size_t i = 0; i < items.size(); ++i) {
     const XferItem& it = items[i];
     const bool win = it.flags & XFER_WINDOW;
+    const bool strided = it.flags & XFER_STRIDED;
     if (win && (it.win_lo > it.win_hi || it.win_hi > it.nbytes || it.ndst != 1 || (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM))))
+      return ErrorCode::INVALID_ARGUMENT;
+    if (strided && (!win || it.win_width == 0 || it.win_width > it.win_pitch || it.win_phase >= it.win_pitch))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
@@ -314,12 +333,13 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
       continue;
     }
-    // windowed items always take bb_xfer: neither the warp-per-object kernel nor the mailbox has a store window
+    // windowed items (strided ones included) always take bb_xfer: neither the warp-per-object kernel nor the mailbox has a
+    // store window
     all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW)) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
-    for (uint32_t r = 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
-    if (al & 15) return ErrorCode::INVALID_ADDRESS;
+    for (uint32_t r = strided ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);  // strided: rows instead
+    if ((al & 15) || (strided && !stride_coaligned(it))) return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
     d.src = static_cast<const uint8_t*>(it.src) + trim;
@@ -328,6 +348,14 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       d.win.base = static_cast<uint8_t*>(it.dst[0]) + trim;
       d.win.lo = it.win_lo - trim;
       d.win.hi = it.win_hi - trim;
+    }
+    if (strided) {
+      // the trim shifts the pattern's origin: trimmed byte x' is object byte x' + trim, so the phase grows by `trim` and
+      // whole rows that carries over move the base by as many widths
+      const uint64_t shifted = it.win_phase + trim;
+      d.win.base = static_cast<uint8_t*>(it.dst[0]) + shifted / it.win_pitch * it.win_width;
+      if (s->strides.size() <= nd) s->strides.resize(nd + 1, XferStride{1, 1, 0});
+      s->strides[nd] = {it.win_pitch, it.win_width, shifted % it.win_pitch};
     }
     d.nbytes = nbytes;
     d.ndst = it.ndst;
@@ -341,6 +369,11 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     s->item_to_desc[i] = static_cast<int32_t>(nd++);
   }
   BB_TRY(write_tile_table(s, nd));
+  const bool any_strided = !s->strides.empty();
+  if (any_strided) {
+    s->strides.resize(nd, XferStride{1, 1, 0});
+    std::memcpy(s->h_tab + stride_table_offset(nd), s->strides.data(), static_cast<size_t>(nd) * sizeof(XferStride));
+  }
   s->nitems = static_cast<uint32_t>(items.size());
   s->debug = capture_debug;
   s->traced = tile_trace_;
@@ -377,7 +410,8 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     return s->ticket;
   }
   if (nd) {
-    const size_t tab = static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
+    const size_t tab = any_strided ? stride_table_offset(nd) + static_cast<size_t>(nd) * sizeof(XferStride)
+                                   : static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
     const bool inline_tab = nd <= kInlineDescs;
     if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
     if (capture_debug) {
@@ -400,6 +434,10 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     if (inline_tab) {
       l.host_descs = descs;
       l.host_tile_start = reinterpret_cast<const uint32_t*>(s->h_tab + static_cast<size_t>(nd) * sizeof(XferDesc));
+    }
+    if (any_strided) {
+      l.strides = reinterpret_cast<const XferStride*>(s->d_tab + stride_table_offset(nd));
+      if (inline_tab) l.host_strides = reinterpret_cast<const XferStride*>(s->h_tab + stride_table_offset(nd));
     }
     l.debug_d = capture_debug ? s->d_debug : nullptr;
     if (tile_trace_) {

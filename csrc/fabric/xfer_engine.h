@@ -29,6 +29,12 @@ struct XferItem {
   // The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine reads only the 16-byte
   // aligned span of the window (see window_read_bytes).
   uint64_t win_lo = 0, win_hi = 0;
+  // XFER_STRIDED (with XFER_WINDOW): of the window, byte x is stored iff c = (x + win_phase) % win_pitch < win_width, at
+  // dst[0] + ((x + win_phase) / win_pitch) * win_width + c.  0 < win_width <= win_pitch and win_phase < win_pitch, else
+  // INVALID_ARGUMENT.  Every row the window touches must be co-aligned, else INVALID_ADDRESS: dst[0] + win_phase -
+  // r * (win_pitch - win_width) is 16-byte aligned for the window's first row r, and (win_pitch - win_width) % 16 == 0
+  // when the window touches more than one row.
+  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span

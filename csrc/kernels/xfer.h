@@ -24,6 +24,10 @@ enum XferFlags : uint32_t {
   // stored.  Only with ndst == 1, never with XFER_MULTIMEM or XFER_RAW_SUM.  The fused MXFP8 get honours it too, with the
   // window in bf16 bytes of the unpacked object; an MXFP8 put never carries it.
   XFER_WINDOW = 1u << 3,
+  // Strided store window (slices along an inner dimension), only together with XFER_WINDOW and only in bb_xfer: of the
+  // window [win.lo, win.hi), byte x is stored iff c = (x + phase) % pitch < width, at dst[0] + ((x + phase) / pitch) *
+  // width + c, so the rows land densely.  The pattern is the descriptor's entry of the launch's XferStride table.
+  XFER_STRIDED = 1u << 4,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -51,6 +55,13 @@ static_assert(sizeof(XferDesc) == 64, "XferDesc must be 64 bytes");
 static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offsetof(XferDesc, win.hi) == offsetof(XferDesc, dst) + 16,
               "the window bounds are the words of dst[1] / dst[2]");
 
+// Row pattern of an XFER_STRIDED descriptor (see XferFlags): 0 < width <= pitch, phase < pitch.  With pitch == width and
+// phase == 0 it stores exactly the plain window.  Every stored row must be co-aligned with the tile (the destination of
+// object byte x congruent to x mod 16), so that the kernel only bulk-stores 16-byte congruent spans.
+struct XferStride {
+  uint64_t pitch, width, phase;
+};
+
 constexpr uint32_t kSmallBytes = 4096;     // objects up to this size may take the warp-per-object path (xfer_small.cu)
 constexpr uint32_t kSmallPending = 0xFFFFFFFFu;  // value of a status slot whose object has not completed yet (flag completion)
 constexpr uint32_t kInlineDescs = 8;       // descriptors that fit in the kernel parameter block
@@ -74,6 +85,10 @@ struct XferLaunch {
   // kernel parameters instead (descs / tile_start may then be null).
   const XferDesc* host_descs = nullptr;
   const uint32_t* host_tile_start = nullptr;
+  // Row patterns of the XFER_STRIDED descriptors, one entry per descriptor (the entries of unflagged descriptors are never
+  // read); null when the batch has none.  host_strides is their copy for the kernel parameters of an inline batch.
+  const XferStride* strides = nullptr;
+  const XferStride* host_strides = nullptr;
   int algo = ALGO_BBH64;
   bool small_path = false;               // every descriptor is <= kSmallBytes, none is a RAW_SUM slice: warp-per-object kernel
   bool flag_completion = false;          // small path only: status_out (pinned, preset to kSmallPending) is the completion flag

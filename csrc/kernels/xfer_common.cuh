@@ -91,6 +91,12 @@ __device__ __forceinline__ uint2 cta_tile_run(uint32_t total_tiles) {
 struct TileSpan {
   uint32_t x0, x1, a0, a1, h1, tb;
 };
+// The parts of the tile-relative span [x0, x1): aligned middle, head and tail as above.
+__device__ __forceinline__ TileSpan span_parts(uint32_t x0, uint32_t x1) {
+  const uint32_t a0 = (x0 + 15u) & ~15u, a1 = max(x1 & ~15u, a0);
+  const uint32_t h1 = min(a0, x1), tb = max(a1, h1);
+  return {x0, x1, a0, a1, h1, tb};
+}
 __device__ __forceinline__ TileSpan tile_span(uint64_t off, uint32_t bytes, bool windowed, uint64_t lo, uint64_t hi) {
   uint32_t x0 = 0, x1 = bytes;
   if (windowed) {
@@ -98,9 +104,28 @@ __device__ __forceinline__ TileSpan tile_span(uint64_t off, uint32_t bytes, bool
     x1 = static_cast<uint32_t>(max(min(hi, off + bytes), off) - off);
     x1 = max(x1, x0);
   }
-  const uint32_t a0 = (x0 + 15u) & ~15u, a1 = max(x1 & ~15u, a0);
-  const uint32_t h1 = min(a0, x1), tb = max(a1, h1);
-  return {x0, x1, a0, a1, h1, tb};
+  return span_parts(x0, x1);
+}
+
+// Strided window (XFER_STRIDED, pattern `st`): the span [x0, x1) of a tile at object offset `off` (from tile_span) holds
+// rows first_row(...) .. + row_count(...) - 1 of the pattern, in part or whole.  Row r's segment is the tile-relative span
+// segment_span(...) of it, stored at row_dst(...) + o for tile byte o; with co-aligned rows that address is congruent to o
+// mod 16, so the segment splits into TMA middle, head and tail exactly like a window span.
+__device__ __forceinline__ uint64_t first_row(uint64_t off, uint32_t x0, const XferStride& st) {
+  return (off + x0 + st.phase) / st.pitch;
+}
+__device__ __forceinline__ uint32_t row_count(uint64_t off, uint32_t x0, uint32_t x1, const XferStride& st) {
+  return x1 > x0 ? static_cast<uint32_t>((off + x1 - 1u + st.phase) / st.pitch - first_row(off, x0, st) + 1u) : 0u;
+}
+__device__ __forceinline__ TileSpan segment_span(uint64_t off, uint32_t x0, uint32_t x1, uint64_t r, const XferStride& st) {
+  const int64_t s = static_cast<int64_t>(r * st.pitch) - static_cast<int64_t>(off + st.phase);  // row start, tile-relative
+  const uint32_t s0 = static_cast<uint32_t>(min(max(s, static_cast<int64_t>(x0)), static_cast<int64_t>(x1)));
+  const uint32_t s1 = static_cast<uint32_t>(min(max(s + static_cast<int64_t>(st.width), static_cast<int64_t>(s0)), static_cast<int64_t>(x1)));
+  return span_parts(s0, s1);
+}
+// dst[0] + r * width + (off + o + phase - r * pitch): where tile byte o of row r lands, less o.
+__device__ __forceinline__ uint64_t row_dst(uint64_t dst0, uint64_t off, uint64_t r, const XferStride& st) {
+  return dst0 + off + st.phase - r * (st.pitch - st.width);
 }
 
 // ---------------------------------------------------------------- warp helpers

@@ -9,7 +9,8 @@
 //                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
-//                      to an NVLS multicast address (one store, N replicas).
+//                      to an NVLS multicast address (one store, N replicas).  A store window (XFER_WINDOW) cuts
+//                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.
 //   warp 3  finalizer: folds the per-tile partials into per-object digests in registers; an
 //                      object that lives entirely inside this CTA's run is finalised with no
 //                      global atomics; only the <=2 objects straddling a CTA boundary use them.
@@ -125,6 +126,9 @@ struct Params {
   uint32_t use_inline;
   uint32_t inl_tile_start[kInlineDescs + 1];
   XferDesc inl_descs[kInlineDescs];
+  // Row patterns of XFER_STRIDED descriptors (XferLaunch::strides), and their copy for inline batches.
+  const XferStride* strides;
+  XferStride inl_strides[kInlineDescs];
 };
 
 // s * x^(8k) mod P through the 4x256 table of distance k.
@@ -285,6 +289,10 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
     // idle: the BBH64 tensor-core product is issued by the epilogue warpgroup that consumes it
   } else if (warp == 2) {
     // ================================================================ store warp
+    // Bulk async-groups belong to the thread that commits them: every lane commits one group per tile (empty unless the
+    // lane stored a strided segment) and waits on its own groups before lane 0 releases the stage.
+    uint32_t st_desc = 0xFFFFFFFFu;  // descriptor whose row pattern is in `st`
+    XferStride st{1, 1, 0};
     for (uint32_t it = 0; it < my_tiles; ++it) {
       const uint32_t stage = it % kStages;
       const uint32_t par = (it / kStages) & 1u;
@@ -294,9 +302,31 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
       const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kTileBytes;
       const uint32_t ndst = m.ndst_flags & 0xFFu;
       const uint32_t flags = m.ndst_flags >> 8;
+      const bool strided = flags & XFER_STRIDED;
       // the whole tile, or its part inside the window [dst[1], dst[2]) (object offsets)
       const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, m.bytes, flags & XFER_WINDOW, m.dst[1], m.dst[2]);
-      if (flags & XFER_MULTIMEM) {
+      if (strided) {
+        // one row segment per lane (a tile can hold thousands of short rows): TMA middle, head and tail byte-wise
+        if (m.desc != st_desc) {
+          st_desc = m.desc;
+          if (p.use_inline) {
+            st = p.inl_strides[st_desc];
+          } else {
+            const uint64_t* e = reinterpret_cast<const uint64_t*>(&p.strides[st_desc]);
+            st = {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
+          }
+        }
+        const uint64_t r0 = first_row(off, x0, st);
+        const uint32_t nrow = row_count(off, x0, x1, st);
+        for (uint32_t k = lane; k < nrow; k += 32) {
+          const uint64_t r = r0 + k;
+          const TileSpan g = segment_span(off, x0, x1, r, st);
+          uint8_t* d = reinterpret_cast<uint8_t*>(row_dst(m.dst[0], off, r, st));
+          if (g.a1 > g.a0) bulk_s2g(d + g.a0, &s.tile[stage][g.a0], g.a1 - g.a0);
+          for (uint32_t o = g.x0; o < g.h1; ++o) d[o] = s.tile[stage][o];
+          for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = s.tile[stage][o];
+        }
+      } else if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);
         for (uint32_t o = a0 + lane * 16; o < a1; o += 512)
           multimem_st_v4(mc + o, *reinterpret_cast<const uint4*>(&s.tile[stage][o]));
@@ -304,29 +334,30 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
         for (uint32_t r = 0; r < ndst; ++r)
           if (a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[r] + off + a0), &s.tile[stage][a0], a1 - a0);
       }
-      if (lane == 0) bulk_commit();
+      bulk_commit();
       if (p.trace_d && lane == 0) p.trace_d[static_cast<uint64_t>(t0 + it) * 4 + 2] = globaltimer_ns();
       const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);
-      if (o < (lane < 16 ? h1 : x1)) {
+      if (!strided && o < (lane < 16 ? h1 : x1)) {
         const uint8_t b = s.tile[stage][o];
         for (uint32_t r = 0; r < ndst; ++r) *reinterpret_cast<uint8_t*>(m.dst[r] + off + o) = b;
       }
+      if (it >= kStoreLag) bulk_wait_read<kStoreLag>();
       __syncwarp();
       if (it >= kStoreLag && lane == 0) {
-        bulk_wait_read<kStoreLag>();
         mbar_arrive(&s.empty[(it - kStoreLag) % kStages]);
         if (p.trace_d) p.trace_d[static_cast<uint64_t>(t0 + it - kStoreLag) * 4 + 3] = globaltimer_ns();
       }
     }
+    bulk_wait_read<0>();
+    __syncwarp();
     if (lane == 0) {
-      bulk_wait_read<0>();
       const uint32_t first = my_tiles > kStoreLag ? my_tiles - kStoreLag : 0;
       for (uint32_t it = first; it < my_tiles; ++it) {
         mbar_arrive(&s.empty[it % kStages]);
         if (p.trace_d) p.trace_d[static_cast<uint64_t>(t0 + it) * 4 + 3] = globaltimer_ns();
       }
-      bulk_wait<0>();  // writes performed before the kernel retires
     }
+    bulk_wait<0>();  // writes performed before the kernel retires
   } else if (warp == 3) {
     // ================================================================ finalizer
     if constexpr (kHash) {
@@ -656,7 +687,9 @@ int launch_xfer(const XferLaunch& l) {
     p.use_inline = 1;
     std::memcpy(p.inl_descs, l.host_descs, l.ndesc * sizeof(XferDesc));
     std::memcpy(p.inl_tile_start, l.host_tile_start, (l.ndesc + 1) * sizeof(uint32_t));
+    if (l.host_strides) std::memcpy(p.inl_strides, l.host_strides, l.ndesc * sizeof(XferStride));
   }
+  p.strides = l.strides;
   p.ndesc = l.ndesc;
   p.total_tiles = l.total_tiles;
   p.sum_ws = reinterpret_cast<unsigned long long*>(l.sum_ws);

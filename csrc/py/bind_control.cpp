@@ -1216,6 +1216,16 @@ void bind_control(py::module_& m) {
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("lengths"), py::arg("stream") = 0,
          "Bytes [offsets[i], offsets[i] + lengths[i]) of object i into dev_ptrs[i]; every overlapping shard is read whole and "
          "verified; returns one ErrorCode per object.")
+      .def("batch_get_device_strided", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+                                          const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                          const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, uintptr_t stream) {
+        std::vector<void*> p;
+        for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
+        return ecs_to_py(nogil([&] { return c.batch_get_device_strided(keys, p, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("widths"), py::arg("pitches"), py::arg("rows"), py::arg("stream") = 0,
+         "rows[i] rows of widths[i] bytes of object i, row r = bytes [offsets[i] + r * pitches[i], + widths[i]), densely into "
+         "dev_ptrs[i] (row r at dev_ptrs[i] + r * widths[i]); every shard holding a stored byte is read whole and verified; "
+         "returns one ErrorCode per object.")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

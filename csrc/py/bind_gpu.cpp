@@ -33,7 +33,8 @@ uint32_t to_ptrs(const py::handle& h, void* (&out)[kMaxDst]) {
 }
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None).  An empty destination list makes
 // a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window (lo, hi) sets XFER_WINDOW: only
-// object bytes [lo, hi) are stored, byte x at dst + x.
+// object bytes [lo, hi) are stored, byte x at dst + x.  A window (lo, hi, pitch, width, phase) also sets XFER_STRIDED: of
+// [lo, hi), byte x is stored iff c = (x + phase) % pitch < width, at dst + ((x + phase) / pitch) * width + c.
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
   if (t.size() < 3 || t.size() > 7)
@@ -46,10 +47,17 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) {
-    auto w = t[6].cast<std::pair<uint64_t, uint64_t>>();
-    it.win_lo = w.first;
-    it.win_hi = w.second;
+    auto w = t[6].cast<std::vector<uint64_t>>();
+    if (w.size() != 2 && w.size() != 5) throw py::value_error("window = (lo, hi) or (lo, hi, pitch, width, phase)");
+    it.win_lo = w[0];
+    it.win_hi = w[1];
     it.flags |= XFER_WINDOW;
+    if (w.size() == 5) {
+      it.win_pitch = w[2];
+      it.win_width = w[3];
+      it.win_phase = w[4];
+      it.flags |= XFER_STRIDED;
+    }
   }
   return it;
 }
@@ -61,6 +69,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_MULTIMEM") = static_cast<uint32_t>(XFER_MULTIMEM);
   m.attr("XFER_RAW_SUM") = static_cast<uint32_t>(XFER_RAW_SUM);
   m.attr("XFER_WINDOW") = static_cast<uint32_t>(XFER_WINDOW);
+  m.attr("XFER_STRIDED") = static_cast<uint32_t>(XFER_STRIDED);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -93,7 +102,9 @@ void bind_gpu(py::module_& m) {
            "destinations with XFER_RAW_SUM hash a slice whose first tile is tile `tile_base` of its object (digest = the "
            "unfinalised tile sum), and a window (lo, hi) sets XFER_WINDOW: the whole object is read and verified but only "
            "bytes [lo, hi) are stored, object byte x at dst + x (pass dst = buffer - lo; one destination; with "
-           "ChecksumAlgo.NONE only the window's 16-byte aligned span is read); returns (digests, status, device_ms).")
+           "ChecksumAlgo.NONE only the window's 16-byte aligned span is read).  A window (lo, hi, pitch, width, phase) also "
+           "sets XFER_STRIDED: of [lo, hi), byte x is stored iff c = (x + phase) % pitch < width, at dst + ((x + phase) // "
+           "pitch) * width + c; returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
              std::vector<gpu::Fp8Item> v;
