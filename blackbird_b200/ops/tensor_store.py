@@ -239,7 +239,12 @@ class TensorStore:
         that holds a byte of them is read whole and verified against its digest, shards wholly between two rows are not
         read.  Each result starts at byte `offset % 16` of its own allocation, so that single-shard tensors take the fused
         kernel for every slice whose row gap is a multiple of 16 bytes; other slices are staged through the host.
-        MXFP8-packed tensors are read whole through the fused get (the unpack kernel has no strided store) and narrowed."""
+
+        MXFP8-packed tensors, padded ones included (their pad lies past the last row), take the fused strided get of
+        packed tensors: the whole packed object is read and verified against its digest, only the rows' elements are
+        unpacked and stored.  Each result starts at element `offset % 8` of its own allocation, so only a slice whose row
+        gap is not a multiple of 8 elements misses the fused kernel; such slices, and packed tensors the fused kernel
+        cannot read (striped, demoted to a host tier), are read whole, unpacked and narrowed."""
         device = device or torch.device("cuda", torch.cuda.current_device())
         keys, dims, starts, stops = list(keys), list(dims), list(starts), list(stops)
         if not len(keys) == len(dims) == len(starts) == len(stops):
@@ -263,8 +268,26 @@ class TensorStore:
                 result[i] = t
         packed = [i for i, m in enumerate(metas) if dims[i] != 0 and m["packed"]]
         if packed:
-            for i, t in zip(packed, self.batch_get([keys[i] for i in packed], device)):
-                result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).contiguous()
+            # prod(shape[:dim]) rows of (stop - start) * inner elements every shape[dim] * inner elements
+            offsets, widths, pitches, nrows = [], [], [], []
+            for i in packed:
+                shape, d = metas[i]["shape"], dims[i]
+                inner = torch.Size(shape[d + 1:]).numel()
+                offset, width = starts[i] * inner, (stops[i] - starts[i]) * inner
+                rows = torch.Size(shape[:d]).numel()
+                buf = torch.empty(rows * width + offset % 8, dtype=torch.bfloat16, device=device)
+                result[i] = buf[offset % 8:].view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
+                offsets.append(offset), widths.append(width), pitches.append(shape[d] * inner), nrows.append(rows)
+            ecs = self.client.batch_get_device_fp8_strided([keys[i] for i in packed], [result[i].data_ptr() for i in packed],
+                                                           [metas[i]["padded_numel"] for i in packed], offsets, widths, pitches,
+                                                           nrows, self._stream())
+            bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+            if bad:
+                raise RuntimeError(f"fused fp8 strided get failed: {bad[:3]}")
+            unfused = [i for i, e in zip(packed, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
+            if unfused:
+                for i, t in zip(unfused, self.batch_get([keys[i] for i in unfused], device)):
+                    result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).contiguous()
         strided = [i for i, m in enumerate(metas) if dims[i] != 0 and not m["packed"]]
         if strided:
             offsets, widths, pitches, nrows = [], [], [], []

@@ -477,6 +477,27 @@ static bool reads_shard(uint64_t off, uint64_t len, uint64_t lo, uint64_t hi, ui
   return y % pitch < width || (y / pitch + 1) * pitch < end;
 }
 
+// Rows with gaps between them; anything else (one row, or rows that touch) is one range.
+static bool has_gaps(uint64_t rows, uint64_t width, uint64_t pitch) { return rows > 1 && width < pitch; }
+
+// The span [offset, offset + *extent) of an object of `size` units that `rows` rows of `width` units every `pitch` units
+// from `offset` cover.  OK with *extent == 0 when there is nothing to read (no rows, or rows of zero width);
+// INVALID_ARGUMENT for several rows wider than the pitch; VALUE_OUT_OF_RANGE when the last row passes `size` or the
+// arithmetic overflows.
+static ErrorCode rows_extent(uint64_t offset, uint64_t width, uint64_t pitch, uint64_t rows, uint64_t size, uint64_t* extent) {
+  *extent = width;
+  if (rows != 1) {
+    if (rows > 1 && width > pitch) return ErrorCode::INVALID_ARGUMENT;
+    if (rows == 0 || width == 0) {
+      *extent = 0;
+      return ErrorCode::OK;
+    }
+    if (__builtin_mul_overflow(rows - 1, pitch, extent) || __builtin_add_overflow(*extent, width, extent)) return ErrorCode::VALUE_OUT_OF_RANGE;
+  }
+  if (offset + *extent < offset || offset + *extent > size) return ErrorCode::VALUE_OUT_OF_RANGE;
+  return ErrorCode::OK;
+}
+
 ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo, uint64_t hi,
                                         uint64_t pitch, uint64_t width) {
   const bool whole = lo == 0 && hi == UINT64_MAX;
@@ -696,6 +717,24 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::ve
   return out;
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                                     const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
+                                                                     const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
+                                                                     const std::vector<uint64_t>& rows, void* stream) {
+  const size_t n = keys.size();
+  if (elem_offsets.size() != n || elem_widths.size() != n || elem_pitches.size() != n || rows.size() != n)
+    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  std::vector<ByteRange> ranges(n);
+  for (size_t i = 0; i < n; ++i) ranges[i] = {elem_offsets[i], elem_widths[i], elem_pitches[i], rows[i]};
+  auto out = get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream);
+  uint64_t k = 0, bytes = 0;
+  for (size_t i = 0; i < n; ++i)
+    if (out[i] == ErrorCode::OK) ++k, bytes += 2 * rows[i] * elem_widths[i];  // an OK item's rows lie inside the object
+  metrics_.inc("device_get_fp8_strided_total", k);
+  metrics_.inc("device_get_fp8_strided_bytes_total", bytes);
+  return out;
+}
+
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
@@ -707,10 +746,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   std::vector<std::vector<size_t>> candidates(keys.size());
   std::vector<size_t> idx;
   // Where element 0 would land: the caller's pointer, or for a range get the virtual base `ptr - 2 * offset` (the kernel
-  // stores element x at base + 2x and never touches an address outside the range).
+  // stores element x at base + 2x and never touches an address outside the range).  Rows with gaps land densely instead
+  // (DeviceFp8Op::win_pitch), but the virtual base is still the address their alignment is judged by.
   std::vector<void*> bases = bf16_ptrs;
   for (size_t i = 0; ranges && i < keys.size(); ++i)
     bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * (*ranges)[i].offset);
+  std::vector<uint64_t> extents(keys.size(), 0);  // elements [offset, offset + extent) hold the rows of a range get
   for (size_t i = 0; i < keys.size(); ++i) {
     if (!placed[i].ok()) {
       out[i] = placed[i].error();
@@ -718,12 +759,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     }
     if (ranges) {
       const ByteRange& r = (*ranges)[i];
-      if (r.offset + r.length < r.offset || r.offset + r.length > n_elems[i]) {
-        out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
-        continue;
-      }
-      if (r.length == 0) {  // nothing to read or store
-        out[i] = ErrorCode::OK;
+      const ErrorCode ec = rows_extent(r.offset, r.length, r.pitch, r.rows, n_elems[i], &extents[i]);
+      if (ec != ErrorCode::OK || extents[i] == 0) {  // an error, or nothing to read or store
+        out[i] = ec;
         continue;
       }
     }
@@ -746,8 +784,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       continue;
     }
     // a range whose virtual base the kernel cannot store from (TMA needs 16 bytes) fails alone, so that the rest of the
-    // batch still takes the fused launch; the caller reads it whole and slices instead
-    if (ranges && (reinterpret_cast<uintptr_t>(bases[i]) & 15)) {
+    // batch still takes the fused launch; the caller reads it whole and slices instead.  Rows with gaps are co-aligned
+    // only when the gap is a whole number of 16-byte units (XferItem::win_pitch).
+    if (ranges && ((reinterpret_cast<uintptr_t>(bases[i]) & 15) ||
+                   (has_gaps((*ranges)[i].rows, (*ranges)[i].length, (*ranges)[i].pitch) && ((*ranges)[i].pitch - (*ranges)[i].length) % 8))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
@@ -765,7 +805,17 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         continue;
       }
       DeviceFp8Op op{&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}};
-      if (ranges) op.win_lo = (*ranges)[i].offset, op.win_hi = (*ranges)[i].offset + (*ranges)[i].length;
+      if (ranges) {
+        const ByteRange& r = (*ranges)[i];
+        op.win_lo = r.offset, op.win_hi = r.offset + extents[i];
+        if (has_gaps(r.rows, r.length, r.pitch)) {
+          // the pattern's rows start at multiples of the pitch, so the caller's row 0 is the pattern's row
+          // (offset + phase) / pitch and `wide` lies that many rows before the caller's pointer
+          op.win_pitch = r.pitch, op.win_width = r.length, op.win_phase = (r.pitch - r.offset % r.pitch) % r.pitch;
+          op.wide = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) -
+                                            2 * ((r.offset + op.win_phase) / r.pitch) * r.length);
+        }
+      }
       ops.push_back(std::move(op));
       cur.push_back(i);
     }
@@ -1206,9 +1256,6 @@ struct GetSpan {
   bool all = true;
   bool reads(uint64_t off, uint64_t len) const { return all || reads_shard(off, len, lo, hi, pitch, width); }
 };
-
-// Rows with gaps between them; anything else (one row, or rows that touch) is one byte range.
-bool has_gaps(uint64_t rows, uint64_t width, uint64_t pitch) { return rows > 1 && width < pitch; }
 }  // namespace
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1353,27 +1400,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       if (ranges) {
         const ByteRange& r = (*ranges)[i];
         // the rows span object bytes [offset, offset + (rows - 1) * pitch + length); rows that touch are one range
-        uint64_t extent = r.length;
-        if (r.rows != 1) {
-          if (r.rows > 1 && r.length > r.pitch) {
-            out[i] = ErrorCode::INVALID_ARGUMENT;
-            continue;
-          }
-          if (r.rows == 0 || r.length == 0) {  // nothing to read or store
-            out[i] = ErrorCode::OK;
-            continue;
-          }
-          if (__builtin_mul_overflow(r.rows - 1, r.pitch, &extent) || __builtin_add_overflow(extent, r.length, &extent)) {
-            out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
-            continue;
-          }
-        }
-        if (r.offset + extent < r.offset || r.offset + extent > size) {
-          out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
-          continue;
-        }
-        if (extent == 0) {  // nothing to read or store
-          out[i] = ErrorCode::OK;
+        uint64_t extent = 0;
+        const ErrorCode ec = rows_extent(r.offset, r.length, r.pitch, r.rows, size, &extent);
+        if (ec != ErrorCode::OK || extent == 0) {  // an error, or nothing to read or store
+          out[i] = ec;
           continue;
         }
         sp = {r.offset, r.offset + extent, 0, 0, false};
@@ -1682,6 +1712,7 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
     const DeviceFp8Op& op = ops[k];
     const bool whole = op.win_lo == 0 && op.win_hi == UINT64_MAX;
     if (!whole && (op.win_lo > op.win_hi || op.win_hi > op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
+    if (op.strided() && (op.win_width == 0 || op.win_width > op.win_pitch || op.win_phase >= op.win_pitch)) return ErrorCode::INVALID_ARGUMENT;
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
@@ -1689,8 +1720,22 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       continue;
     }
     if (ec != ErrorCode::OK) return ec;
-    if (whole) {
+    if (whole && !op.strided()) {
       mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
+    } else if (op.strided()) {  // as the kernel does: read and verify the whole object, store the window's row segments densely
+      std::vector<uint16_t> wide(op.n_elems);
+      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
+      const uint64_t hi = std::min(op.win_hi, op.n_elems);
+      for (uint64_t x = op.win_lo; x < hi;) {
+        const uint64_t y = x + op.win_phase, c = y % op.win_pitch;
+        if (c >= op.win_width) {  // in the gap: on to the next row
+          x += op.win_pitch - c;
+          continue;
+        }
+        const uint64_t n = std::min(op.win_width - c, hi - x);
+        std::memcpy(reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(op.wide) + 2 * (y / op.win_pitch * op.win_width + c)), wide.data() + x, 2 * n);
+        x += n;
+      }
     } else if (op.win_hi > op.win_lo) {  // as the kernel does: the whole object is read and verified, only the window stored
       std::vector<uint16_t> wide(op.n_elems);
       mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());

@@ -77,6 +77,11 @@ struct DeviceFp8Op {
   // Get of an element range: only elements [win_lo, win_hi) are stored, element x at wide + 2x (wide is then the virtual
   // base `buffer - 2 * win_lo`); the whole packed object is still read and verified.  The default is the whole object.
   uint64_t win_lo = 0, win_hi = UINT64_MAX;
+  // Strided get (win_pitch != 0, always with a window), in elements, with the meaning DeviceShardOp's pattern has: of the
+  // window, element x is stored iff c = (x + win_phase) % win_pitch < win_width, at wide + 2 * (((x + win_phase) /
+  // win_pitch) * win_width + c).  `wide` is then where the pattern's row 0 lands.
+  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
+  bool strided() const { return win_pitch != 0; }
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -150,6 +155,20 @@ class BlackbirdClient {
   std::vector<ErrorCode> batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                     const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
                                                     const std::vector<uint64_t>& elem_counts, void* stream);
+  // Strided gets of packed tensors (a slice along an inner dimension): rows[i] rows of elem_widths[i] elements, row r being
+  // elements [elem_offsets[i] + r * elem_pitches[i], + elem_widths[i]) of the n_elems[i]-element object i, unpacked to bf16,
+  // land densely at bf16_ptrs[i] + 2 * r * elem_widths[i].  The whole packed object is read and verified (a corrupt byte
+  // in a gap between rows still fails that copy over to the next replica); only the rows are unpacked and stored, and no
+  // byte outside them is ever written.  Per object: INVALID_ARGUMENT for elem_widths[i] > elem_pitches[i] with rows[i] > 1;
+  // VALUE_OUT_OF_RANGE when the last row passes n_elems or the arithmetic overflows; OK with nothing read for rows[i] == 0
+  // or elem_widths[i] == 0; Keystone errors as before; NOT_IMPLEMENTED when the object is not fusable (as
+  // batch_get_device_fp8), or when the virtual base bf16_ptrs[i] - 2 * elem_offsets[i] is not 16-byte aligned or, for
+  // rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 != 0 -- the rest of the batch still takes the fused launch.
+  // rows[i] == 1, and rows that touch, are batch_get_device_fp8_range.
+  std::vector<ErrorCode> batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                      const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
+                                                      const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
+                                                      const std::vector<uint64_t>& rows, void* stream);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -219,8 +238,8 @@ class BlackbirdClient {
   };
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
-  // batch_get_device_fp8 and batch_get_device_fp8_range: `ranges` null = whole tensors, else object i's element range
-  // (offset and length in elements) into bf16_ptrs[i].
+  // batch_get_device_fp8, batch_get_device_fp8_range and batch_get_device_fp8_strided: `ranges` null = whole tensors, else
+  // object i's rows (offset, length and pitch in elements) into bf16_ptrs[i].
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream);
   ErrorCode get_with_refresh(const ObjectKey& key, uint8_t* (*alloc)(void*, size_t), void* ctx, size_t capacity, size_t* out_size);

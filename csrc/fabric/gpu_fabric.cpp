@@ -637,6 +637,9 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.n_elems = op.n_elems;
     it.win_lo = op.win_lo;  // a window on a put is refused by the engine
     it.win_hi = op.win_hi;
+    it.win_pitch = op.win_pitch;  // as is a stride
+    it.win_width = op.win_width;
+    it.win_phase = op.win_phase;
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;

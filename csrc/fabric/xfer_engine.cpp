@@ -569,13 +569,20 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   SlotRelease release{s->ticket};
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
+  std::vector<XferStride> strides;       // per descriptor up to the last strided one; empty when the batch has none
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
+    const bool strided = it.win_pitch != 0 || it.win_width != 0 || it.win_phase != 0;
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
-    if ((reinterpret_cast<uintptr_t>(it.wide) | reinterpret_cast<uintptr_t>(it.packed)) & 15) return ErrorCode::INVALID_ADDRESS;
+    // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window): the rows are
+    // checked below instead
+    if (((strided ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15) return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
     if ((it.win_lo != 0 || it.win_hi != UINT64_MAX) && (!unpack || it.win_lo > it.win_hi || it.win_hi > it.n_elems))
+      return ErrorCode::INVALID_ARGUMENT;
+    // (a pitch beyond 2^62 elements would overflow its byte count)
+    if (strided && (!unpack || it.win_width == 0 || it.win_width > it.win_pitch || it.win_phase >= it.win_pitch || it.win_pitch > (UINT64_MAX >> 2)))
       return ErrorCode::INVALID_ARGUMENT;
     for (uint32_t r = 1; r < nrep; ++r)
       if (!it.more_packed[r - 1] || (reinterpret_cast<uintptr_t>(it.more_packed[r - 1]) & 15)) return ErrorCode::INVALID_ADDRESS;
@@ -590,10 +597,24 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     d.expect = 0;
     d.flags = 0;
     d.reserved = 0;
-    if (unpack && (it.win_lo > 0 || it.win_hi < it.n_elems)) {  // whole-object gets keep exactly the descriptors they had
+    // whole-object gets keep exactly the descriptors they had; a strided item always carries its window
+    if (unpack && (strided || it.win_lo > 0 || it.win_hi < it.n_elems)) {
       d.flags = XFER_WINDOW;
       d.win.lo = 2 * it.win_lo;
-      d.win.hi = 2 * it.win_hi;
+      d.win.hi = 2 * std::min(it.win_hi, it.n_elems);
+    }
+    if (strided) {  // the pattern in bf16 bytes, held to the rule submit() applies to a strided XferItem
+      XferItem b;
+      b.dst[0] = it.wide;
+      b.win_lo = d.win.lo;
+      b.win_hi = d.win.hi;
+      b.win_pitch = 2 * it.win_pitch;
+      b.win_width = 2 * it.win_width;
+      b.win_phase = 2 * it.win_phase;
+      if (!stride_coaligned(b)) return ErrorCode::INVALID_ADDRESS;
+      d.flags |= XFER_STRIDED;
+      strides.resize(i + 1, XferStride{1, 1, 0});
+      strides[i] = {b.win_pitch, b.win_width, b.win_phase};
     }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
@@ -606,7 +627,13 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     sc.tile_base = static_cast<uint32_t>(nt_full);
   }
   BB_TRY(write_tile_table(s, n));
-  const size_t tab = static_cast<size_t>(n) * sizeof(XferDesc) + (static_cast<size_t>(n) + 1) * 4;
+  const bool any_strided = !strides.empty();
+  if (any_strided) {  // the same layout submit() uses: [descs | tile_start | strides]
+    strides.resize(n, XferStride{1, 1, 0});
+    std::memcpy(s->h_tab + stride_table_offset(n), strides.data(), static_cast<size_t>(n) * sizeof(XferStride));
+  }
+  const size_t tab = any_strided ? stride_table_offset(n) + static_cast<size_t>(n) * sizeof(XferStride)
+                                 : static_cast<size_t>(n) * sizeof(XferDesc) + (static_cast<size_t>(n) + 1) * 4;
   BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
   BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;
@@ -614,6 +641,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   l.tile_start = reinterpret_cast<const uint32_t*>(s->d_tab + static_cast<size_t>(n) * sizeof(XferDesc));
   l.ndesc = n;
   l.total_tiles = s->total_tiles;
+  if (any_strided) l.strides = reinterpret_cast<const XferStride*>(s->d_tab + stride_table_offset(n));
   l.sum_ws = s->d_digest;
   l.max_ctas = max_ctas_;
   l.stream = stream;

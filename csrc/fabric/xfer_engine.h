@@ -57,6 +57,11 @@ struct Fp8Item {
   // Unpack only: store elements [win_lo, win_hi) of the object, element x at wide + 2x (wide = caller buffer - 2 * win_lo,
   // the virtual base).  The whole packed object is still read and verified.  The default is the whole object.
   uint64_t win_lo = 0, win_hi = UINT64_MAX;
+  // Unpack only, strided (any of the three non-zero): of the window, element x is stored iff c = (x + win_phase) % win_pitch
+  // < win_width, at wide + 2 * (((x + win_phase) / win_pitch) * win_width + c), so the rows land densely (wide is where
+  // the pattern's row 0 lands).  0 < win_width <= win_pitch and win_phase < win_pitch, else INVALID_ARGUMENT; every row
+  // the window touches must be co-aligned in bf16 bytes, as XferItem's, else INVALID_ADDRESS.
+  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
 };
 
 struct XferResult {

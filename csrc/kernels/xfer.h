@@ -24,9 +24,10 @@ enum XferFlags : uint32_t {
   // stored.  Only with ndst == 1, never with XFER_MULTIMEM or XFER_RAW_SUM.  The fused MXFP8 get honours it too, with the
   // window in bf16 bytes of the unpacked object; an MXFP8 put never carries it.
   XFER_WINDOW = 1u << 3,
-  // Strided store window (slices along an inner dimension), only together with XFER_WINDOW and only in bb_xfer: of the
-  // window [win.lo, win.hi), byte x is stored iff c = (x + phase) % pitch < width, at dst[0] + ((x + phase) / pitch) *
-  // width + c, so the rows land densely.  The pattern is the descriptor's entry of the launch's XferStride table.
+  // Strided store window (slices along an inner dimension), only together with XFER_WINDOW, in bb_xfer and the fused
+  // MXFP8 get: of the window [win.lo, win.hi), byte x is stored iff c = (x + phase) % pitch < width, at dst[0] + ((x +
+  // phase) / pitch) * width + c, so the rows land densely.  The pattern is the descriptor's entry of the launch's
+  // XferStride table; the MXFP8 get counts all of it in bf16 bytes of the unpacked object.
   XFER_STRIDED = 1u << 4,
 };
 
@@ -137,8 +138,9 @@ int xfer_smem_bytes(int algo);
 // Descriptors: pack (put): src = bf16 source, dst[0..ndst-1] = base of the packed object in every replica (the scales
 // follow the payload), nbytes = payload bytes (= elements, a multiple of kTileBytes); unpack (get): src = base of the
 // packed object, dst[0] = bf16 destination (where element 0 lands); an unpack descriptor may carry XFER_WINDOW, whose
-// `win` is then in bf16 bytes of the object ([2 * first element, 2 * end element)).  `sum_ws` receives the unfinalised
-// BBH64 sum of the payload tiles per descriptor (must be zero on entry); descs / tile_start are device tables.
+// `win` is then in bf16 bytes of the object ([2 * first element, 2 * end element)), and XFER_STRIDED, whose pattern in
+// `strides` (a device table; no inline copy) is in bf16 bytes too.  `sum_ws` receives the unfinalised BBH64 sum of the
+// payload tiles per descriptor (must be zero on entry); descs / tile_start are device tables.
 int launch_xfer_fp8(const XferLaunch& l, bool unpack);
 int xfer_fp8_smem_bytes();
 

@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <mutex>
 
+#include "kernels/ptx.cuh"
 #include "kernels/xfer.h"
 
 namespace bb::gpu {
@@ -126,6 +127,27 @@ __device__ __forceinline__ TileSpan segment_span(uint64_t off, uint32_t x0, uint
 // dst[0] + r * width + (off + o + phase - r * pitch): where tile byte o of row r lands, less o.
 __device__ __forceinline__ uint64_t row_dst(uint64_t dst0, uint64_t off, uint64_t r, const XferStride& st) {
   return dst0 + off + st.phase - r * (st.pitch - st.width);
+}
+// The store warp's part of a strided tile: the row segments of the span [x0, x1) of `tile` (shared memory, object bytes
+// [off, off + ...)), one per lane (a tile can hold thousands of short rows), each as a TMA middle plus a byte-wise head and
+// tail.  dst0 is the descriptor's dst[0].  The calling lane still has to commit its bulk group and wait on it.
+__device__ __forceinline__ void store_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t x0, uint32_t x1,
+                                                   const XferStride& st, uint32_t lane) {
+  const uint64_t r0 = first_row(off, x0, st);
+  const uint32_t nrow = row_count(off, x0, x1, st);
+  for (uint32_t k = lane; k < nrow; k += 32) {
+    const uint64_t r = r0 + k;
+    const TileSpan g = segment_span(off, x0, x1, r, st);
+    uint8_t* d = reinterpret_cast<uint8_t*>(row_dst(dst0, off, r, st));
+    if (g.a1 > g.a0) ptx::bulk_s2g(d + g.a0, tile + g.a0, g.a1 - g.a0);
+    for (uint32_t o = g.x0; o < g.h1; ++o) d[o] = tile[o];
+    for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = tile[o];
+  }
+}
+// The row pattern of descriptor `i` from a device table (read-only path).
+__device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i) {
+  const uint64_t* e = reinterpret_cast<const uint64_t*>(&table[i]);
+  return {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
 }
 
 // ---------------------------------------------------------------- warp helpers

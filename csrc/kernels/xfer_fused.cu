@@ -309,23 +309,10 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
         // one row segment per lane (a tile can hold thousands of short rows): TMA middle, head and tail byte-wise
         if (m.desc != st_desc) {
           st_desc = m.desc;
-          if (p.use_inline) {
-            st = p.inl_strides[st_desc];
-          } else {
-            const uint64_t* e = reinterpret_cast<const uint64_t*>(&p.strides[st_desc]);
-            st = {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
-          }
+          if (p.use_inline) st = p.inl_strides[st_desc];
+          else st = load_stride(p.strides, st_desc);
         }
-        const uint64_t r0 = first_row(off, x0, st);
-        const uint32_t nrow = row_count(off, x0, x1, st);
-        for (uint32_t k = lane; k < nrow; k += 32) {
-          const uint64_t r = r0 + k;
-          const TileSpan g = segment_span(off, x0, x1, r, st);
-          uint8_t* d = reinterpret_cast<uint8_t*>(row_dst(m.dst[0], off, r, st));
-          if (g.a1 > g.a0) bulk_s2g(d + g.a0, &s.tile[stage][g.a0], g.a1 - g.a0);
-          for (uint32_t o = g.x0; o < g.h1; ++o) d[o] = s.tile[stage][o];
-          for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = s.tile[stage][o];
-        }
+        store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);
       } else if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);
         for (uint32_t o = a0 + lane * 16; o < a1; o += 512)

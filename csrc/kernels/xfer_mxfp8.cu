@@ -10,7 +10,9 @@
 //                   8 unpack warps expand to bf16 in shared memory -> TMA stores the 32 KiB tile to the caller.
 //                   With XFER_WINDOW (element-range gets) only the bf16 bytes [win.lo, win.hi) of the object are
 //                   stored, object byte x at dst[0] + x; every tile is still loaded and hashed, so the digest is the
-//                   whole object's, and tiles outside the window are not unpacked.
+//                   whole object's, and tiles outside the window are not unpacked.  With XFER_STRIDED as well
+//                   (slices along an inner dimension) the store warp stores only the window's row segments, densely,
+//                   one per lane, by the same rule as bb_xfer; a tile wholly inside a gap between rows is still unpacked.
 //
 // The stored object keeps the layout of the unfused path ([E4M3 payload n][E8M0 scales n/32], common/mxfp8.h), and so
 // does its digest: BBH64 is a sum of per-tile terms, this kernel accumulates the payload tiles (tile index 0..T-1)
@@ -57,7 +59,7 @@ struct FpMeta {            // 64 bytes
   uint32_t obj_ntiles;
   uint32_t ndst;           // pack: replicas written by this pass (1..kMaxDst)
   uint32_t valid;          // payload bytes (= elements) of this tile: 16384, or the multiple-of-32 tail of the object
-  uint32_t pad32;
+  uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided (FpParams::strides); pack: 0
   uint64_t pad;
 };
 static_assert(sizeof(FpMeta) == 64);
@@ -93,6 +95,7 @@ struct FpParams {
   uint32_t ndesc;
   uint32_t total_tiles;
   unsigned long long* sum_ws;  // [ndesc] raw BBH64 sums of the payload tiles (zero on entry)
+  const XferStride* strides;   // unpack: row patterns of the XFER_STRIDED descriptors (XferLaunch::strides), else null
 };
 
 template <bool UNPACK>
@@ -140,7 +143,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.pad32 = 0;
+        e.m.strided = UNPACK ? d.flags & XFER_STRIDED : 0u;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
         // the packed object is [payload nbytes][scales nbytes/32]: a tile's scales sit (nbytes - ti*(16384-512)) past its payload
@@ -199,20 +202,31 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     // idle: the tensor-core hash of the payload tile is issued by the epilogue warpgroup that consumes it
   } else if (warp == 2) {
     // ================================================================ store warp
+    // Bulk async-groups belong to the thread that commits them: every lane commits one group per tile (empty unless the
+    // lane stored something by TMA) and waits on its own groups before lane 0 releases the slot.
     constexpr int kRing = UNPACK ? kWideStages : kTileStages;
+    uint32_t pat_desc = 0xFFFFFFFFu;  // unpack: descriptor whose row pattern is in `pat`
+    XferStride pat{1, 1, 0};
     for (uint32_t it = 0; it < my_tiles; ++it) {
       const uint32_t st = it % kRing, par = (it / kRing) & 1u;
       if constexpr (UNPACK) {
         mbar_wait(&s.w_full[st], par);
         const FpMeta& m = s.w_meta[st];
-        // the tile's bf16 bytes inside the store window: the middle by TMA, head and tail byte-wise (as bb_xfer does)
-        const auto [x0, x1, a0, a1, h1, tb] = tile_span(static_cast<uint64_t>(m.tile_in_obj) * kWideBytes, 2u * m.valid, true, m.dst[1], m.dst[2]);
-        if (lane == 0) {
-          if (a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[0] + a0), &s.wide[st][a0], a1 - a0);
-          bulk_commit();
+        // the tile's bf16 bytes inside the store window: the middle by TMA, head and tail byte-wise (as bb_xfer does); a
+        // strided window (XFER_STRIDED) cuts them further to its row segments, one per lane
+        const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kWideBytes;
+        const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, 2u * m.valid, true, m.dst[1], m.dst[2]);
+        if (m.strided) {
+          if (m.desc != pat_desc) {
+            pat_desc = m.desc;
+            pat = load_stride(p.strides, pat_desc);
+          }
+          store_row_segments(s.wide[st], m.dst[0] - off, off, x0, x1, pat, lane);  // m.dst[0] = dst[0] + off
+        } else {
+          if (lane == 0 && a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[0] + a0), &s.wide[st][a0], a1 - a0);
+          const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);
+          if (o < (lane < 16 ? h1 : x1)) *reinterpret_cast<uint8_t*>(m.dst[0] + o) = s.wide[st][o];
         }
-        const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);
-        if (o < (lane < 16 ? h1 : x1)) *reinterpret_cast<uint8_t*>(m.dst[0] + o) = s.wide[st][o];
       } else {
         mbar_wait(&s.t_full[st], par);
         const FpMeta& m = s.t_meta[st];
@@ -222,29 +236,30 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             bulk_s2g(reinterpret_cast<void*>(m.dst[r]), s.tile[st], m.valid);
             if (sb16) bulk_s2g(reinterpret_cast<void*>(m.dst[r] + m.scales_delta), s.scales[st], sb16);
           }
-          bulk_commit();
         }
         if (lane < (sb & 15u)) {  // tail tile: the scale bytes past the last 16-byte multiple
           const uint8_t v = s.scales[st][sb16 + lane];
           for (uint32_t r = 0; r < m.ndst; ++r) *reinterpret_cast<uint8_t*>(m.dst[r] + m.scales_delta + sb16 + lane) = v;
         }
       }
+      bulk_commit();
+      if (it >= kFpStoreLag) bulk_wait_read<kFpStoreLag>();
       __syncwarp();
       if (it >= kFpStoreLag && lane == 0) {
-        bulk_wait_read<kFpStoreLag>();
         if constexpr (UNPACK) mbar_arrive(&s.w_empty[(it - kFpStoreLag) % kRing]);
         else mbar_arrive(&s.t_empty[(it - kFpStoreLag) % kRing]);
       }
     }
+    bulk_wait_read<0>();
+    __syncwarp();
     if (lane == 0) {
-      bulk_wait_read<0>();
       const uint32_t first = my_tiles > kFpStoreLag ? my_tiles - kFpStoreLag : 0;
       for (uint32_t it = first; it < my_tiles; ++it) {
         if constexpr (UNPACK) mbar_arrive(&s.w_empty[it % kRing]);
         else mbar_arrive(&s.t_empty[it % kRing]);
       }
-      bulk_wait<0>();
     }
+    bulk_wait<0>();  // writes performed before the kernel retires
   } else if (warp == 3) {
     // ================================================================ accumulator: per-object raw sums
     uint32_t cur_d = 0xFFFFFFFFu;
@@ -362,6 +377,7 @@ int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
   p.ndesc = l.ndesc;
   p.total_tiles = l.total_tiles;
   p.sum_ws = reinterpret_cast<unsigned long long*>(l.sum_ws);
+  p.strides = l.strides;
   int grid = l.max_ctas > 0 ? l.max_ctas : std::min(current_sm_count(), 128);
   grid = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), l.total_tiles));
   cudaStream_t st = static_cast<cudaStream_t>(l.stream);

@@ -1160,6 +1160,21 @@ void bind_control(py::module_& m) {
            "Elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of packed tensor i (n_elems[i] elements), unpacked to "
            "bf16 at bf16_ptrs[i]; the whole packed object is read and verified; returns one ErrorCode per object "
            "(NOT_IMPLEMENTED: read it whole and slice).")
+      .def("batch_get_device_fp8_strided",
+           [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
+              const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+              const std::vector<uint64_t>& rows, uintptr_t stream) {
+             std::vector<void*> p;
+             for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
+             py::gil_scoped_release rel;
+             return c.batch_get_device_fp8_strided(keys, p, n_elems, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream));
+           },
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_widths"),
+           py::arg("elem_pitches"), py::arg("rows"), py::arg("stream") = 0,
+           "rows[i] rows of elem_widths[i] elements of packed tensor i (n_elems[i] elements), row r = elements "
+           "[elem_offsets[i] + r * elem_pitches[i], + elem_widths[i]), unpacked to bf16 densely at bf16_ptrs[i] (row r at "
+           "bf16_ptrs[i] + 2 * r * elem_widths[i]); the whole packed object is read and verified; returns one ErrorCode per "
+           "object (NOT_IMPLEMENTED: read it whole and narrow).")
       .def("device_fp8_eligible", &BlackbirdClient::device_fp8_eligible)
       .def("batch_put", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<py::buffer>& data, const WorkerConfig& cfg) {
         std::vector<const uint8_t*> ptrs;

@@ -121,9 +121,15 @@ void bind_gpu(py::module_& m) {
                it.n_elems = t[2].cast<uint64_t>();
                if (t.size() > 3) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) {
-                 auto w = t[4].cast<std::pair<uint64_t, uint64_t>>();
-                 it.win_lo = w.first;
-                 it.win_hi = w.second;
+                 auto w = t[4].cast<std::vector<uint64_t>>();
+                 if (w.size() != 2 && w.size() != 5) throw py::value_error("window = (lo, hi) or (lo, hi, pitch, width, phase)");
+                 it.win_lo = w[0];
+                 it.win_hi = w[1];
+                 if (w.size() == 5) {
+                   it.win_pitch = w[2];
+                   it.win_width = w[3];
+                   it.win_phase = w[4];
+                 }
                }
                v.push_back(it);
              }
@@ -139,7 +145,11 @@ void bind_gpu(py::module_& m) {
            "| [packed_ptr, ...], n_elems[, expected_digest[, (lo, hi)]]), where a put writes every packed replica in the list "
            "(1..3) and a get reads the first.  A get with a window (lo, hi) reads and verifies the whole packed object but "
            "stores only elements [lo, hi), element x at bf16_ptr + 2x (pass bf16_ptr = buffer - 2 * lo, 16-byte aligned); a "
-           "window on a put, lo > hi or hi > n_elems is INVALID_ARGUMENT.  Returns (digests of the packed objects, status, "
+           "window on a put, lo > hi or hi > n_elems is INVALID_ARGUMENT.  A window (lo, hi, pitch, width, phase), in "
+           "elements, is strided: of [lo, hi), element x is stored iff c = (x + phase) % pitch < width, at bf16_ptr + 2 * "
+           "((x + phase) // pitch * width + c); INVALID_ARGUMENT for width == 0, width > pitch or phase >= pitch, "
+           "INVALID_ADDRESS unless every row the window touches is co-aligned in bf16 bytes (the address of its first "
+           "element congruent to twice that element's index mod 16).  Returns (digests of the packed objects, status, "
            "device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
