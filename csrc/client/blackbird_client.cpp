@@ -467,40 +467,7 @@ ErrorCode BlackbirdClient::transfer_put(const std::vector<CopyPlacement>& copies
   });
 }
 
-// Whether a get of object bytes [lo, hi) reads shard [off, off + len): the shard overlaps the range and, for rows of
-// `width` bytes every `pitch` bytes from lo (pitch 0: one range), holds at least one byte of a row.  A shard that lies
-// wholly in the gap between two rows holds none.
-static bool reads_shard(uint64_t off, uint64_t len, uint64_t lo, uint64_t hi, uint64_t pitch, uint64_t width) {
-  if (!(off < hi && off + len > lo)) return false;
-  if (pitch == 0) return true;
-  const uint64_t y = std::max(off, lo) - lo, end = std::min(off + len, hi) - lo;  // the overlap, relative to the first row
-  return y % pitch < width || (y / pitch + 1) * pitch < end;
-}
-
-// Rows with gaps between them; anything else (one row, or rows that touch) is one range.
-static bool has_gaps(uint64_t rows, uint64_t width, uint64_t pitch) { return rows > 1 && width < pitch; }
-
-// The span [offset, offset + *extent) of an object of `size` units that `rows` rows of `width` units every `pitch` units
-// from `offset` cover.  OK with *extent == 0 when there is nothing to read (no rows, or rows of zero width);
-// INVALID_ARGUMENT for several rows wider than the pitch; VALUE_OUT_OF_RANGE when the last row passes `size` or the
-// arithmetic overflows.
-static ErrorCode rows_extent(uint64_t offset, uint64_t width, uint64_t pitch, uint64_t rows, uint64_t size, uint64_t* extent) {
-  *extent = width;
-  if (rows != 1) {
-    if (rows > 1 && width > pitch) return ErrorCode::INVALID_ARGUMENT;
-    if (rows == 0 || width == 0) {
-      *extent = 0;
-      return ErrorCode::OK;
-    }
-    if (__builtin_mul_overflow(rows - 1, pitch, extent) || __builtin_add_overflow(*extent, width, extent)) return ErrorCode::VALUE_OUT_OF_RANGE;
-  }
-  if (offset + *extent < offset || offset + *extent > size) return ErrorCode::VALUE_OUT_OF_RANGE;
-  return ErrorCode::OK;
-}
-
-ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo, uint64_t hi,
-                                        uint64_t pitch, uint64_t width) {
-  const bool whole = lo == 0 && hi == UINT64_MAX;
+ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, const StoreWindow& win) {
   ErrorCode last = ErrorCode::NO_COMPLETE_WORKER;
   for (const auto& copy : copies) {  // replica fail-over (reference reads copy 0 only, :283-287)
     uint64_t total = 0;
@@ -516,7 +483,7 @@ ErrorCode BlackbirdClient::transfer_get(const std::vector<CopyPlacement>& copies
       off += copy.shards[s].length;
     }
     last = parallel_for(copy.shards.size(), opts_.io_parallelism, [&](size_t s) {
-      if (!whole && !reads_shard(offs[s], copy.shards[s].length, lo, hi, pitch, width)) return ErrorCode::OK;  // nothing to store
+      if (!win.touches(offs[s], copy.shards[s].length)) return ErrorCode::OK;  // nothing to store
       return read_shard(copy.shards[s], dst + offs[s], copy.shards[s].checksum_algo);
     });
     if (last == ErrorCode::OK) return ErrorCode::OK;
@@ -745,25 +712,24 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   auto placed = keystone_->batch_get_workers(keys);
   std::vector<std::vector<size_t>> candidates(keys.size());
   std::vector<size_t> idx;
-  // Where element 0 would land: the caller's pointer, or for a range get the virtual base `ptr - 2 * offset` (the kernel
-  // stores element x at base + 2x and never touches an address outside the range).  Rows with gaps land densely instead
-  // (DeviceFp8Op::win_pitch), but the virtual base is still the address their alignment is judged by.
+  // The elements each get stores, and the base they land relative to: the caller's pointer, less the window's offset for
+  // a range get (the virtual base; the kernel never touches an address outside the range).
+  std::vector<StoreWindow> wins(keys.size());
   std::vector<void*> bases = bf16_ptrs;
-  for (size_t i = 0; ranges && i < keys.size(); ++i)
-    bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * (*ranges)[i].offset);
-  std::vector<uint64_t> extents(keys.size(), 0);  // elements [offset, offset + extent) hold the rows of a range get
   for (size_t i = 0; i < keys.size(); ++i) {
     if (!placed[i].ok()) {
       out[i] = placed[i].error();
       continue;
     }
+    StoreWindow& w = wins[i];
     if (ranges) {
       const ByteRange& r = (*ranges)[i];
-      const ErrorCode ec = rows_extent(r.offset, r.length, r.pitch, r.rows, n_elems[i], &extents[i]);
-      if (ec != ErrorCode::OK || extents[i] == 0) {  // an error, or nothing to read or store
+      const ErrorCode ec = StoreWindow::from_rows(r.offset, r.length, r.pitch, r.rows, n_elems[i], &w);
+      if (ec != ErrorCode::OK || w.empty()) {  // an error, or nothing to read or store
         out[i] = ec;
         continue;
       }
+      bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * w.base_shift(w.lo));
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
@@ -783,11 +749,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       out[i] = ErrorCode::NOT_IMPLEMENTED;  // demoted to a host tier, striped, other digest: caller gets + unpacks instead
       continue;
     }
-    // a range whose virtual base the kernel cannot store from (TMA needs 16 bytes) fails alone, so that the rest of the
-    // batch still takes the fused launch; the caller reads it whole and slices instead.  Rows with gaps are co-aligned
-    // only when the gap is a whole number of 16-byte units (XferItem::win_pitch).
-    if (ranges && ((reinterpret_cast<uintptr_t>(bases[i]) & 15) ||
-                   (has_gaps((*ranges)[i].rows, (*ranges)[i].length, (*ranges)[i].pitch) && ((*ranges)[i].pitch - (*ranges)[i].length) % 8))) {
+    // a range whose virtual base `ptr - 2 * lo` the kernel cannot store from (TMA needs 16 bytes) fails alone, so that the
+    // rest of the batch still takes the fused launch; the caller reads it whole and slices instead.  Rows with gaps are
+    // co-aligned only when the gap is a whole number of 16-byte units (StoreWindow::coaligned).
+    if (ranges && (((reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * w.lo) & 15) || (w.strided() && (w.pitch - w.width) % 8))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
@@ -804,19 +769,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      DeviceFp8Op op{&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}};
-      if (ranges) {
-        const ByteRange& r = (*ranges)[i];
-        op.win_lo = r.offset, op.win_hi = r.offset + extents[i];
-        if (has_gaps(r.rows, r.length, r.pitch)) {
-          // the pattern's rows start at multiples of the pitch, so the caller's row 0 is the pattern's row
-          // (offset + phase) / pitch and `wide` lies that many rows before the caller's pointer
-          op.win_pitch = r.pitch, op.win_width = r.length, op.win_phase = (r.pitch - r.offset % r.pitch) % r.pitch;
-          op.wide = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) -
-                                            2 * ((r.offset + op.win_phase) / r.pitch) * r.length);
-        }
-      }
-      ops.push_back(std::move(op));
+      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i]});
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -1246,18 +1199,6 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
   return out;
 }
 
-// Shard [off, off + len) of an object takes part in a get: every shard of a whole-object get (`all`, zero-length objects
-// included), else the shards that hold a byte the get stores (reads_shard): of the object bytes [lo, hi), and for a
-// strided get (pitch != 0) only those of its rows, byte lo + y with y % pitch < width.
-namespace {
-struct GetSpan {
-  uint64_t lo = 0, hi = 0;
-  uint64_t pitch = 0, width = 0;
-  bool all = true;
-  bool reads(uint64_t off, uint64_t len) const { return all || reads_shard(off, len, lo, hi, pitch, width); }
-};
-}  // namespace
-
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                    const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges, void* stream,
                                                    std::vector<size_t>* out_sizes) {
@@ -1271,19 +1212,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   std::vector<Result<std::vector<CopyPlacement>>> placed(keys.size(), Result<std::vector<CopyPlacement>>(ErrorCode::INTERNAL_ERROR));
   std::vector<size_t> copy_choice(keys.size(), 0);
   std::vector<bool> pending(keys.size(), false);
-  std::vector<GetSpan> span(keys.size());
-  // Where object byte 0 would land: the caller's pointer, or for a range get the virtual base `ptr - offset` (the fabric
-  // stores object byte x at base + x and never touches an address outside the range).  A strided get passes the caller's
-  // pointer, where its row 0 lands (DeviceShardOp::win_row).
+  // The object bytes each get stores (every shard of a whole-object get is read, zero-length ones included), and the base
+  // they land relative to: the caller's pointer, less the window's offset for a range get (the virtual base; the fabric
+  // never touches an address outside the range).
+  std::vector<StoreWindow> span(keys.size());
   std::vector<void*> range_bases;
-  if (ranges) {
-    range_bases.resize(keys.size());
-    for (size_t i = 0; i < keys.size(); ++i) {
-      const ByteRange& r = (*ranges)[i];
-      range_bases[i] = has_gaps(r.rows, r.length, r.pitch) ? dev_ptrs[i]
-                                                           : reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - r.offset);
-    }
-  }
+  if (ranges) range_bases.resize(keys.size());
   const std::vector<void*>& bases = ranges ? range_bases : dev_ptrs;
 
   auto build_ops = [&](size_t begin, size_t end, std::vector<DeviceShardOp>& ops) {
@@ -1291,29 +1225,19 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       if (!pending[i]) continue;
       const auto& copies = placed[i].value();
       const auto& copy = copies[copy_choice[i] % copies.size()];
-      const GetSpan& sp = span[i];
+      const StoreWindow& sp = span[i];
+      const bool whole = sp.whole();
       uint64_t off = 0;
       for (size_t s = 0; s < copy.shards.size(); ++s) {
         const uint64_t len = copy.shards[s].length;
-        if (sp.reads(off, len)) {
+        if (whole || sp.touches(off, len)) {
           DeviceShardOp op;
           op.item = i;
           op.copy = copy_choice[i] % copies.size();
           op.shard = s;
           op.placement = &copy.shards[s];
           op.obj_offset = off;
-          if (!sp.all) {
-            op.win_lo = std::max(sp.lo, off) - off;
-            op.win_hi = std::min(sp.hi, off + len) - off;
-          }
-          if (sp.pitch) {  // shard byte x is byte x + d of the rows: row floor((x + d) / pitch), d = off - lo
-            const int64_t d = static_cast<int64_t>(off) - static_cast<int64_t>(sp.lo), p = static_cast<int64_t>(sp.pitch);
-            const int64_t row = d / p - (d % p < 0 ? 1 : 0);
-            op.win_pitch = sp.pitch;
-            op.win_width = sp.width;
-            op.win_phase = static_cast<uint64_t>(d - row * p);
-            op.win_row = row;
-          }
+          if (!whole) op.win = sp.rebase(off, len);
           ops.push_back(std::move(op));
         }
         off += len;
@@ -1396,24 +1320,18 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       size_t size = 0;
       for (const auto& s : placed[i].value()[0].shards) size += s.length;
       if (out_sizes) (*out_sizes)[i] = size;
-      GetSpan& sp = span[i];
+      StoreWindow& sp = span[i];
       if (ranges) {
         const ByteRange& r = (*ranges)[i];
-        // the rows span object bytes [offset, offset + (rows - 1) * pitch + length); rows that touch are one range
-        uint64_t extent = 0;
-        const ErrorCode ec = rows_extent(r.offset, r.length, r.pitch, r.rows, size, &extent);
-        if (ec != ErrorCode::OK || extent == 0) {  // an error, or nothing to read or store
+        const ErrorCode ec = StoreWindow::from_rows(r.offset, r.length, r.pitch, r.rows, size, &sp);
+        if (ec != ErrorCode::OK || sp.empty()) {  // an error, or nothing to read or store
           out[i] = ec;
           continue;
         }
-        sp = {r.offset, r.offset + extent, 0, 0, false};
-        if (has_gaps(r.rows, r.length, r.pitch)) sp.pitch = r.pitch, sp.width = r.length;
-      } else {
-        if (size > capacity[i]) {
-          out[i] = ErrorCode::BUFFER_OVERFLOW;
-          continue;
-        }
-        sp.hi = size;
+        range_bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.base_shift(sp.lo));
+      } else if (size > capacity[i]) {
+        out[i] = ErrorCode::BUFFER_OVERFLOW;
+        continue;
       }
       // replica choice: one that lives on this client's own GPU (HBM speed, no NVLink), else a replica that is
       // fully reachable over the GPU fabric (readers spread over the replicas), else stage through the host.  Only the
@@ -1423,7 +1341,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         size_t n = 0;
         uint64_t off = 0;
         for (const auto& sh : c.shards) {
-          if (sp.reads(off, sh.length)) f(sh), ++n;
+          if (sp.touches(off, sh.length)) f(sh), ++n;
           off += sh.length;
         }
         return n;
@@ -1431,16 +1349,16 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       // (the spread over replicas only matters when there is more than one; thousands of single-copy objects skip the hash)
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
       // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned).  A strided get
-      // needs every row co-aligned with the tiles of each shard it reads (XferItem::win_pitch): the virtual base aligned at
-      // those shards' starts, and the gap between rows a multiple of 16 bytes.
+      // needs every row co-aligned with the tiles of each shard it reads (StoreWindow::coaligned): the virtual base aligned
+      // at those shards' starts, and the gap between rows a multiple of 16 bytes.
       bool aligned;
-      if (sp.pitch) {
+      if (sp.strided()) {
         const uintptr_t vbase = reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.lo;
         aligned = (sp.pitch - sp.width) % 16 == 0;
         for (const auto& c : copies) {
           uint64_t off = 0;
           for (const auto& sh : c.shards) {
-            if (sp.reads(off, sh.length) && (vbase + off) % 16) aligned = false;
+            if (sp.touches(off, sh.length) && (vbase + off) % 16) aligned = false;
             off += sh.length;
           }
         }
@@ -1474,15 +1392,13 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       if (!found) {
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
-        ErrorCode ec = sp.all ? transfer_get(copies, stage.data(), size)
-                              : transfer_get(copies, stage.data(), size, sp.lo, sp.hi, sp.pitch, sp.width);
-        if (ec == ErrorCode::OK && sp.pitch) {  // compact the rows on the host: one H2D copy of rows * width bytes
-          const uint64_t nrows = (sp.hi - sp.lo - sp.width) / sp.pitch + 1;
-          std::vector<uint8_t> dense(nrows * sp.width);
-          for (uint64_t r = 0; r < nrows; ++r) std::memcpy(dense.data() + r * sp.width, stage.data() + sp.lo + r * sp.pitch, sp.width);
+        ErrorCode ec = transfer_get(copies, stage.data(), size, sp);
+        if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
+          std::vector<uint8_t> dense(capacity[i]);
+          sp.for_each_run(size, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + at, stage.data() + x, n); });
           ec = device_->copy_h2d(dev_ptrs[i], dense.data(), dense.size(), stream);
         } else if (ec == ErrorCode::OK) {
-          ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, sp.hi - sp.lo, stream);
+          ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
         }
         out[i] = ec;
         metrics_.inc("device_get_host_staged_total");
@@ -1633,32 +1549,15 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
   std::vector<uint32_t> status(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
-    // dev_ptrs[item] is where object byte 0 would land; for a range get only the window is real memory
-    const uintptr_t dst = reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + op.obj_offset;
     ErrorCode ec;
-    if (op.strided()) {  // as the kernel does: read and verify the whole shard, store the window's row segments densely
+    if (op.win.covers(op.placement->length)) {
+      ec = io_->read_shard(*op.placement, static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset, op.placement->checksum_algo);
+    } else {  // as the kernel does: read and verify the whole shard, store only the window (only it is real memory)
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      const uint64_t hi = std::min<uint64_t>(op.win_hi, whole.size());
-      const uintptr_t row0 = reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + static_cast<uintptr_t>(op.win_row) * op.win_width;
-      for (uint64_t x = op.win_lo; ec == ErrorCode::OK && x < hi;) {
-        const uint64_t y = x + op.win_phase, c = y % op.win_pitch;
-        if (c >= op.win_width) {  // in the gap: on to the next row
-          x += op.win_pitch - c;
-          continue;
-        }
-        const uint64_t n = std::min(op.win_width - c, hi - x);
-        std::memcpy(reinterpret_cast<uint8_t*>(row0 + y / op.win_pitch * op.win_width + c), whole.data() + x, n);
-        x += n;
-      }
-    } else if (op.windowed()) {  // as the kernel does: read and verify the whole shard, store only the window
-      std::vector<uint8_t> whole(op.placement->length);
-      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      const uint64_t hi = std::min<uint64_t>(op.win_hi, whole.size());
-      if (ec == ErrorCode::OK && hi > op.win_lo)
-        std::memcpy(reinterpret_cast<uint8_t*>(dst + op.win_lo), whole.data() + op.win_lo, hi - op.win_lo);
-    } else {
-      ec = io_->read_shard(*op.placement, reinterpret_cast<uint8_t*>(dst), op.placement->checksum_algo);
+      auto* dst = static_cast<uint8_t*>(op.dst(dev_ptrs[op.item]));
+      if (ec == ErrorCode::OK)
+        op.win.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + at, whole.data() + x, n); });
     }
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
       status[k] = 1;  // reported per shard, like the kernel's verify flag
@@ -1710,9 +1609,7 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
   if (status) status->assign(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
-    const bool whole = op.win_lo == 0 && op.win_hi == UINT64_MAX;
-    if (!whole && (op.win_lo > op.win_hi || op.win_hi > op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
-    if (op.strided() && (op.win_width == 0 || op.win_width > op.win_pitch || op.win_phase >= op.win_pitch)) return ErrorCode::INVALID_ARGUMENT;
+    if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
@@ -1720,26 +1617,14 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       continue;
     }
     if (ec != ErrorCode::OK) return ec;
-    if (whole && !op.strided()) {
+    if (op.win.whole()) {
       mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
-    } else if (op.strided()) {  // as the kernel does: read and verify the whole object, store the window's row segments densely
+    } else {  // as the kernel does: the whole object is read and verified, only the window stored
       std::vector<uint16_t> wide(op.n_elems);
       mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
-      const uint64_t hi = std::min(op.win_hi, op.n_elems);
-      for (uint64_t x = op.win_lo; x < hi;) {
-        const uint64_t y = x + op.win_phase, c = y % op.win_pitch;
-        if (c >= op.win_width) {  // in the gap: on to the next row
-          x += op.win_pitch - c;
-          continue;
-        }
-        const uint64_t n = std::min(op.win_width - c, hi - x);
-        std::memcpy(reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(op.wide) + 2 * (y / op.win_pitch * op.win_width + c)), wide.data() + x, 2 * n);
-        x += n;
-      }
-    } else if (op.win_hi > op.win_lo) {  // as the kernel does: the whole object is read and verified, only the window stored
-      std::vector<uint16_t> wide(op.n_elems);
-      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
-      std::memcpy(static_cast<uint16_t*>(op.wide) + op.win_lo, wide.data() + op.win_lo, 2 * (op.win_hi - op.win_lo));
+      op.win.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) {
+        std::memcpy(static_cast<uint16_t*>(op.wide) + at, wide.data() + x, 2 * n);
+      });
     }
   }
   return ErrorCode::OK;

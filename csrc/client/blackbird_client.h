@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "common/metrics.h"
+#include "common/store_window.h"
 #include "net/tcp.h"
 #include "rpc/rpc_service.h"
 
@@ -55,33 +56,23 @@ struct DeviceShardOp {
   const ShardPlacement* placement = nullptr;
   std::vector<const ShardPlacement*> replicas;  // same shard on the other copies (put fan-out)
   uint64_t obj_offset = 0;    // byte offset of this shard inside the object
-  // Get of a byte range: only shard bytes [win_lo, win_hi) are stored (the whole shard is still read and verified).  Any
-  // op whose window is not narrower than the shard, the default included, is a whole-shard op.
-  uint64_t win_lo = 0, win_hi = UINT64_MAX;
-  bool windowed() const { return placement && (win_lo > 0 || win_hi < placement->length); }
-  // Strided get (win_pitch != 0, always with a window): of the shard bytes in [win_lo, win_hi), byte x is stored iff
-  // c = (x + win_phase) % win_pitch < win_width, as row win_row + (x + win_phase) / win_pitch of the caller's dense result:
-  // at dev_ptrs[item] + (win_row + (x + win_phase) / win_pitch) * win_width + c.  dev_ptrs[item] is then where the caller's
-  // row 0 lands, and win_row is negative when the shard starts before the first row.
-  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
-  int64_t win_row = 0;
-  bool strided() const { return win_pitch != 0; }
+  // Get: the shard bytes that are stored (common/store_window.h); the whole shard is still read and verified.  An op whose
+  // window covers the shard, the default included, is a whole-shard op.
+  StoreWindow win;
+  // The base `win` goes with, given the object's: dev_ptrs[item] is where object byte 0 lands, or for a strided get where
+  // the result's row 0 lands.
+  void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(obj_offset); }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
 struct DeviceFp8Op {
   const ShardPlacement* placement = nullptr;
-  void* wide = nullptr;     // client's bf16 tensor (source of a put, destination of a get: where element 0 lands)
+  void* wide = nullptr;     // client's bf16 tensor (source of a put, destination of a get: the base of `win`)
   uint64_t n_elems = 0;
   std::vector<const ShardPlacement*> replicas;  // put: the other copies (<= 2), written by the same tile pass
-  // Get of an element range: only elements [win_lo, win_hi) are stored, element x at wide + 2x (wide is then the virtual
-  // base `buffer - 2 * win_lo`); the whole packed object is still read and verified.  The default is the whole object.
-  uint64_t win_lo = 0, win_hi = UINT64_MAX;
-  // Strided get (win_pitch != 0, always with a window), in elements, with the meaning DeviceShardOp's pattern has: of the
-  // window, element x is stored iff c = (x + win_phase) % win_pitch < win_width, at wide + 2 * (((x + win_phase) /
-  // win_pitch) * win_width + c).  `wide` is then where the pattern's row 0 lands.
-  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
-  bool strided() const { return win_pitch != 0; }
+  // Get: the elements that are stored (common/store_window.h); the whole packed object is still read and verified.  The
+  // default is the whole object.
+  StoreWindow win;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -224,11 +215,9 @@ class BlackbirdClient {
   ErrorCode put_once(const ObjectKey& key, const uint8_t* data, size_t size, const WorkerConfig& cfg);
   ErrorCode transfer_put(const std::vector<CopyPlacement>& copies, const uint8_t* data, ChecksumAlgo algo,
                          keystone::ShardChecksums* sums);
-  // Reads the object into dst[0, size) from the first copy that verifies.  With a byte range [lo, hi) only the shards that
-  // overlap it are read (whole, and verified); with a pitch as well, only those that hold a byte y of it with
-  // (y - lo) % pitch < width.  The other bytes of dst are left as they are.
-  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, uint64_t lo = 0, uint64_t hi = UINT64_MAX,
-                         uint64_t pitch = 0, uint64_t width = 0);
+  // Reads the object into dst[0, size) from the first copy that verifies: every shard, or with a window only those that
+  // hold a byte it stores (whole, and verified).  The other bytes of dst are left as they are.
+  ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, const StoreWindow& win = {});
   // batch_get_device, batch_get_device_range and batch_get_device_strided: `ranges` null = whole objects into buffers of
   // `capacity`, else object i's rows into dev_ptrs[i] (capacity[i] = rows * length, for the chunk plan).  A range is the
   // single row `rows == 1`.

@@ -635,11 +635,7 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.wide = op.wide;
     it.packed = d.value();
     it.n_elems = op.n_elems;
-    it.win_lo = op.win_lo;  // a window on a put is refused by the engine
-    it.win_hi = op.win_hi;
-    it.win_pitch = op.win_pitch;  // as is a stride
-    it.win_width = op.win_width;
-    it.win_phase = op.win_phase;
+    it.win = op.win;  // a window on a put is refused by the engine
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;
@@ -692,17 +688,11 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
     it.nbytes = op.placement->length;
     it.expect = op.placement->checksum;
     it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
-    if (op.windowed() || op.strided()) {  // whole-shard ops keep exactly the descriptors they always had
-      it.flags |= XFER_WINDOW;
-      it.win_lo = op.win_lo;
-      it.win_hi = std::min(op.win_hi, it.nbytes);
-    }
-    if (op.strided()) {  // row 0 of the shard's pattern is the caller's row win_row (dev_ptrs[item] = the caller's row 0)
-      it.flags |= XFER_STRIDED;
-      it.dst[0] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[op.item]) + static_cast<uintptr_t>(op.win_row) * op.win_width);
-      it.win_pitch = op.win_pitch;
-      it.win_width = op.win_width;
-      it.win_phase = op.win_phase;
+    if (!op.win.covers(it.nbytes)) {  // whole-shard ops keep exactly the descriptors they always had
+      it.flags |= op.win.strided() ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
+      it.dst[0] = op.dst(dev_ptrs[op.item]);
+      it.win = op.win;
+      it.win.hi = std::min(op.win.hi, it.nbytes);
     }
     items->push_back(it);
     op_of_item->push_back(k);

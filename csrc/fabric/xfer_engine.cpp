@@ -40,17 +40,6 @@ struct SlotRelease {
 
 // A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items].
 size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
-
-// Whether every row a strided item's window touches is co-aligned with the tiles: object byte x of row r lands at
-// dst[0] + phase - r * (pitch - width) + x, so that base must be 16-byte aligned for the first row, and the same for every
-// later row.
-bool stride_coaligned(const XferItem& it) {
-  const uint64_t gap = it.win_pitch - it.win_width;
-  const uint64_t r_lo = (it.win_lo + it.win_phase) / it.win_pitch;
-  const uint64_t r_hi = it.win_hi > it.win_lo ? (it.win_hi - 1 + it.win_phase) / it.win_pitch : r_lo;
-  if (r_hi > r_lo && gap % 16) return false;
-  return (reinterpret_cast<uintptr_t>(it.dst[0]) + it.win_phase - r_lo * gap) % 16 == 0;
-}
 }  // namespace
 
 struct XferEngine::Slot {
@@ -89,6 +78,18 @@ struct XferEngine::Slot {
   uint64_t empty_digest = 0;
   std::vector<int32_t> item_to_desc;  // -1 for zero-size items
   std::vector<XferStride> strides;     // per descriptor up to the last XFER_STRIDED one; empty when the batch has none
+  void set_stride(uint32_t k, const StoreWindow& w) {
+    if (strides.size() <= k) strides.resize(k + 1, XferStride{1, 1, 0});
+    strides[k] = {w.pitch, w.width, w.phase};
+  }
+  // Writes the stride table behind tile_start when the batch has a strided descriptor, and returns the bytes of the
+  // table to copy to the device: [descs | tile_start | strides], or without the strides.
+  size_t write_strides(uint32_t nd) {
+    if (strides.empty()) return static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
+    strides.resize(nd, XferStride{1, 1, 0});
+    std::memcpy(h_tab + stride_table_offset(nd), strides.data(), static_cast<size_t>(nd) * sizeof(XferStride));
+    return stride_table_offset(nd) + static_cast<size_t>(nd) * sizeof(XferStride);
+  }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
     uint32_t item;
@@ -321,14 +322,13 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const XferItem& it = items[i];
     const bool win = it.flags & XFER_WINDOW;
     const bool strided = it.flags & XFER_STRIDED;
-    if (win && (it.win_lo > it.win_hi || it.win_hi > it.nbytes || it.ndst != 1 || (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM))))
-      return ErrorCode::INVALID_ARGUMENT;
-    if (strided && (!win || it.win_width == 0 || it.win_width > it.win_pitch || it.win_phase >= it.win_pitch))
+    if ((strided && !win) || (win && (strided != it.win.strided() || !it.win.valid(it.nbytes) || it.ndst != 1 ||
+                                      (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
     const uint64_t nbytes = window_read_bytes(it, algo);
-    const uint64_t trim = win && algo == ChecksumAlgo::NONE ? it.win_lo & ~uint64_t{15} : 0;
+    const uint64_t trim = win && algo == ChecksumAlgo::NONE ? it.win.lo & ~uint64_t{15} : 0;
     if (nbytes == 0) {
       s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
       continue;
@@ -339,23 +339,17 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
     for (uint32_t r = strided ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);  // strided: rows instead
-    if ((al & 15) || (strided && !stride_coaligned(it))) return ErrorCode::INVALID_ADDRESS;
+    if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0])))) return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
     d.src = static_cast<const uint8_t*>(it.src) + trim;
     for (uint32_t r = 0; r < kMaxDst; ++r) d.dst[r] = r < it.ndst ? it.dst[r] : nullptr;
-    if (win) {
-      d.win.base = static_cast<uint8_t*>(it.dst[0]) + trim;
-      d.win.lo = it.win_lo - trim;
-      d.win.hi = it.win_hi - trim;
-    }
-    if (strided) {
-      // the trim shifts the pattern's origin: trimmed byte x' is object byte x' + trim, so the phase grows by `trim` and
-      // whole rows that carries over move the base by as many widths
-      const uint64_t shifted = it.win_phase + trim;
-      d.win.base = static_cast<uint8_t*>(it.dst[0]) + shifted / it.win_pitch * it.win_width;
-      if (s->strides.size() <= nd) s->strides.resize(nd + 1, XferStride{1, 1, 0});
-      s->strides[nd] = {it.win_pitch, it.win_width, shifted % it.win_pitch};
+    if (win) {  // the descriptor's byte 0 is object byte `trim`
+      const StoreWindow w = it.win.rebase(trim);
+      d.win.base = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(it.dst[0]) + w.base_shift(trim) + w.origin());
+      d.win.lo = w.lo;
+      d.win.hi = w.hi;
+      if (strided) s->set_stride(nd, w);
     }
     d.nbytes = nbytes;
     d.ndst = it.ndst;
@@ -370,10 +364,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   }
   BB_TRY(write_tile_table(s, nd));
   const bool any_strided = !s->strides.empty();
-  if (any_strided) {
-    s->strides.resize(nd, XferStride{1, 1, 0});
-    std::memcpy(s->h_tab + stride_table_offset(nd), s->strides.data(), static_cast<size_t>(nd) * sizeof(XferStride));
-  }
+  const size_t tab = s->write_strides(nd);
   s->nitems = static_cast<uint32_t>(items.size());
   s->debug = capture_debug;
   s->traced = tile_trace_;
@@ -410,8 +401,6 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     return s->ticket;
   }
   if (nd) {
-    const size_t tab = any_strided ? stride_table_offset(nd) + static_cast<size_t>(nd) * sizeof(XferStride)
-                                   : static_cast<size_t>(nd) * sizeof(XferDesc) + (static_cast<size_t>(nd) + 1) * 4;
     const bool inline_tab = nd <= kInlineDescs;
     if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
     if (capture_debug) {
@@ -569,21 +558,19 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   SlotRelease release{s->ticket};
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
-  std::vector<XferStride> strides;       // per descriptor up to the last strided one; empty when the batch has none
+  s->strides.clear();
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
-    const bool strided = it.win_pitch != 0 || it.win_width != 0 || it.win_phase != 0;
+    const bool strided = it.win.strided();
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
     // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window): the rows are
     // checked below instead
     if (((strided ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15) return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
-    if ((it.win_lo != 0 || it.win_hi != UINT64_MAX) && (!unpack || it.win_lo > it.win_hi || it.win_hi > it.n_elems))
-      return ErrorCode::INVALID_ARGUMENT;
-    // (a pitch beyond 2^62 elements would overflow its byte count)
-    if (strided && (!unpack || it.win_width == 0 || it.win_width > it.win_pitch || it.win_phase >= it.win_pitch || it.win_pitch > (UINT64_MAX >> 2)))
-      return ErrorCode::INVALID_ARGUMENT;
+    // a put stores the whole object; from here on the window is in bf16 bytes
+    StoreWindow w = it.win.over(it.n_elems);
+    if ((!unpack && !it.win.whole()) || !w.valid(it.n_elems) || !w.to_bf16_bytes(&w)) return ErrorCode::INVALID_ARGUMENT;
     for (uint32_t r = 1; r < nrep; ++r)
       if (!it.more_packed[r - 1] || (reinterpret_cast<uintptr_t>(it.more_packed[r - 1]) & 15)) return ErrorCode::INVALID_ADDRESS;
     auto* payload = static_cast<uint8_t*>(it.packed);
@@ -598,23 +585,16 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     d.flags = 0;
     d.reserved = 0;
     // whole-object gets keep exactly the descriptors they had; a strided item always carries its window
-    if (unpack && (strided || it.win_lo > 0 || it.win_hi < it.n_elems)) {
+    if (unpack && !it.win.covers(it.n_elems)) {
       d.flags = XFER_WINDOW;
-      d.win.lo = 2 * it.win_lo;
-      d.win.hi = 2 * std::min(it.win_hi, it.n_elems);
+      d.win.lo = w.lo;
+      d.win.hi = w.hi;
     }
-    if (strided) {  // the pattern in bf16 bytes, held to the rule submit() applies to a strided XferItem
-      XferItem b;
-      b.dst[0] = it.wide;
-      b.win_lo = d.win.lo;
-      b.win_hi = d.win.hi;
-      b.win_pitch = 2 * it.win_pitch;
-      b.win_width = 2 * it.win_width;
-      b.win_phase = 2 * it.win_phase;
-      if (!stride_coaligned(b)) return ErrorCode::INVALID_ADDRESS;
+    if (strided) {  // held to the rule submit() applies to a strided XferItem
+      if (!w.coaligned(reinterpret_cast<uintptr_t>(it.wide))) return ErrorCode::INVALID_ADDRESS;
+      d.win.base = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(it.wide) + w.origin());
       d.flags |= XFER_STRIDED;
-      strides.resize(i + 1, XferStride{1, 1, 0});
-      strides[i] = {b.win_pitch, b.win_width, b.win_phase};
+      s->set_stride(i, w);
     }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
@@ -627,13 +607,8 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     sc.tile_base = static_cast<uint32_t>(nt_full);
   }
   BB_TRY(write_tile_table(s, n));
-  const bool any_strided = !strides.empty();
-  if (any_strided) {  // the same layout submit() uses: [descs | tile_start | strides]
-    strides.resize(n, XferStride{1, 1, 0});
-    std::memcpy(s->h_tab + stride_table_offset(n), strides.data(), static_cast<size_t>(n) * sizeof(XferStride));
-  }
-  const size_t tab = any_strided ? stride_table_offset(n) + static_cast<size_t>(n) * sizeof(XferStride)
-                                 : static_cast<size_t>(n) * sizeof(XferDesc) + (static_cast<size_t>(n) + 1) * 4;
+  const bool any_strided = !s->strides.empty();
+  const size_t tab = s->write_strides(n);
   BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
   BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;

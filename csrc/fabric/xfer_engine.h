@@ -13,6 +13,7 @@
 #include "common/checksum.h"
 #include "common/error.h"
 #include "common/result.h"
+#include "common/store_window.h"
 #include "kernels/xfer.h"
 
 namespace bb::gpu {
@@ -25,23 +26,18 @@ struct XferItem {
   uint64_t expect = 0;   // expected digest when flags & XFER_VERIFY
   uint32_t flags = 0;
   uint32_t tile_base = 0;  // XFER_RAW_SUM: index of this slice's first tile inside the hashed object
-  // XFER_WINDOW: only object bytes [win_lo, win_hi) are stored, byte x at dst[0] + x (dst[0] = caller buffer - win_lo).
-  // The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine reads only the 16-byte
-  // aligned span of the window (see window_read_bytes).
-  uint64_t win_lo = 0, win_hi = 0;
-  // XFER_STRIDED (with XFER_WINDOW): of the window, byte x is stored iff c = (x + win_phase) % win_pitch < win_width, at
-  // dst[0] + ((x + win_phase) / win_pitch) * win_width + c.  0 < win_width <= win_pitch and win_phase < win_pitch, else
-  // INVALID_ARGUMENT.  Every row the window touches must be co-aligned, else INVALID_ADDRESS: dst[0] + win_phase -
-  // r * (win_pitch - win_width) is 16-byte aligned for the window's first row r, and (win_pitch - win_width) % 16 == 0
-  // when the window touches more than one row.
-  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
+  // XFER_WINDOW: only the object bytes `win` selects are stored (common/store_window.h), relative to dst[0]; XFER_STRIDED
+  // exactly when it has a pattern.  INVALID_ARGUMENT unless win.valid(nbytes); INVALID_ADDRESS unless a strided window is
+  // win.coaligned(dst[0]).  The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine
+  // reads only the 16-byte aligned span of the window (see window_read_bytes).
+  StoreWindow win;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span
-// [win_lo & ~15, win_hi) (nothing for an empty window).
+// [win.lo & ~15, win.hi) (nothing for an empty window).
 inline uint64_t window_read_bytes(const XferItem& it, ChecksumAlgo algo) {
   if (!(it.flags & XFER_WINDOW) || algo != ChecksumAlgo::NONE) return it.nbytes;
-  return it.win_hi > it.win_lo ? it.win_hi - (it.win_lo & ~uint64_t{15}) : 0;
+  return it.win.hi > it.win.lo ? it.win.hi - (it.win.lo & ~uint64_t{15}) : 0;
 }
 
 // One object of a fused MXFP8 transfer: `wide` is the caller's bf16 tensor, `packed` the slab location of the
@@ -54,14 +50,10 @@ struct Fp8Item {
   uint64_t n_elems = 0;   // multiple of 32 (whole MX blocks)
   uint64_t expect = 0;    // unpack + verify: digest recorded at put time
   bool verify = false;
-  // Unpack only: store elements [win_lo, win_hi) of the object, element x at wide + 2x (wide = caller buffer - 2 * win_lo,
-  // the virtual base).  The whole packed object is still read and verified.  The default is the whole object.
-  uint64_t win_lo = 0, win_hi = UINT64_MAX;
-  // Unpack only, strided (any of the three non-zero): of the window, element x is stored iff c = (x + win_phase) % win_pitch
-  // < win_width, at wide + 2 * (((x + win_phase) / win_pitch) * win_width + c), so the rows land densely (wide is where
-  // the pattern's row 0 lands).  0 < win_width <= win_pitch and win_phase < win_pitch, else INVALID_ARGUMENT; every row
-  // the window touches must be co-aligned in bf16 bytes, as XferItem's, else INVALID_ADDRESS.
-  uint64_t win_pitch = 0, win_width = 0, win_phase = 0;
+  // Unpack only: the elements of the object that are stored (common/store_window.h), relative to `wide`; the default is
+  // the whole object.  The whole packed object is still read and verified.  INVALID_ARGUMENT unless valid against
+  // n_elems; INVALID_ADDRESS unless a strided window is co-aligned in bf16 bytes, as XferItem's.
+  StoreWindow win;
 };
 
 struct XferResult {

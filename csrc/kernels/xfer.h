@@ -25,9 +25,9 @@ enum XferFlags : uint32_t {
   // window in bf16 bytes of the unpacked object; an MXFP8 put never carries it.
   XFER_WINDOW = 1u << 3,
   // Strided store window (slices along an inner dimension), only together with XFER_WINDOW, in bb_xfer and the fused
-  // MXFP8 get: of the window [win.lo, win.hi), byte x is stored iff c = (x + phase) % pitch < width, at dst[0] + ((x +
-  // phase) / pitch) * width + c, so the rows land densely.  The pattern is the descriptor's entry of the launch's
-  // XferStride table; the MXFP8 get counts all of it in bf16 bytes of the unpacked object.
+  // MXFP8 get: the rule of common/store_window.h with row == 0, so dst[0] is where the pattern's row 0 lands and the rows
+  // land densely from there.  The pattern is the descriptor's entry of the launch's XferStride table; the MXFP8 get
+  // counts all of it in bf16 bytes of the unpacked object.
   XFER_STRIDED = 1u << 4,
 };
 

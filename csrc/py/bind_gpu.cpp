@@ -31,10 +31,22 @@ uint32_t to_ptrs(const py::handle& h, void* (&out)[kMaxDst]) {
   for (size_t i = 0; i < v.size(); ++i) out[i] = reinterpret_cast<void*>(v[i]);
   return static_cast<uint32_t>(v.size());
 }
+// A store window (common/store_window.h) given as (lo, hi) or (lo, hi, pitch, width, phase); returns whether it has the
+// pattern's three numbers.
+bool to_window(const py::handle& h, StoreWindow* win) {
+  auto w = h.cast<std::vector<uint64_t>>();
+  if (w.size() != 2 && w.size() != 5) throw py::value_error("window = (lo, hi) or (lo, hi, pitch, width, phase)");
+  win->lo = w[0];
+  win->hi = w[1];
+  if (w.size() == 2) return false;
+  win->pitch = w[2];
+  win->width = w[3];
+  win->phase = w[4];
+  return true;
+}
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None).  An empty destination list makes
-// a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window (lo, hi) sets XFER_WINDOW: only
-// object bytes [lo, hi) are stored, byte x at dst + x.  A window (lo, hi, pitch, width, phase) also sets XFER_STRIDED: of
-// [lo, hi), byte x is stored iff c = (x + phase) % pitch < width, at dst + ((x + phase) / pitch) * width + c.
+// a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets XFER_WINDOW, and one with
+// a pattern XFER_STRIDED as well.
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
   if (t.size() < 3 || t.size() > 7)
@@ -46,19 +58,7 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 3) it.expect = t[3].cast<uint64_t>();
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
-  if (t.size() > 6 && !t[6].is_none()) {
-    auto w = t[6].cast<std::vector<uint64_t>>();
-    if (w.size() != 2 && w.size() != 5) throw py::value_error("window = (lo, hi) or (lo, hi, pitch, width, phase)");
-    it.win_lo = w[0];
-    it.win_hi = w[1];
-    it.flags |= XFER_WINDOW;
-    if (w.size() == 5) {
-      it.win_pitch = w[2];
-      it.win_width = w[3];
-      it.win_phase = w[4];
-      it.flags |= XFER_STRIDED;
-    }
-  }
+  if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
   return it;
 }
 }  // namespace
@@ -120,17 +120,7 @@ void bind_gpu(py::module_& m) {
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
                if (t.size() > 3) it.expect = t[3].cast<uint64_t>(), it.verify = true;
-               if (t.size() > 4 && !t[4].is_none()) {
-                 auto w = t[4].cast<std::vector<uint64_t>>();
-                 if (w.size() != 2 && w.size() != 5) throw py::value_error("window = (lo, hi) or (lo, hi, pitch, width, phase)");
-                 it.win_lo = w[0];
-                 it.win_hi = w[1];
-                 if (w.size() == 5) {
-                   it.win_pitch = w[2];
-                   it.win_width = w[3];
-                   it.win_phase = w[4];
-                 }
-               }
+               if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                v.push_back(it);
              }
              XferResult res;
