@@ -41,10 +41,44 @@ class TensorStore:
         return (t.dtype == torch.bfloat16 and self.client.device_fp8_eligible(t.numel()) and 1 <= cfg.replication_factor <= 3
                 and cfg.max_workers_per_copy == 1 and t.data_ptr() % 16 == 0)
 
+    @staticmethod
+    def _source_rows(t: torch.Tensor):
+        """(width, pitch, rows) in bytes when `t`'s elements are rows of `width` bytes every `pitch` bytes from
+        t.data_ptr() in row-major order, else None: a contiguous block of trailing dims gives the width and the leading dims
+        must collapse to one stride, the pitch.  This covers `narrow` along any dim of a contiguous tensor and `t[::k]`;
+        transposed, overlapping or otherwise permuted layouts give None."""
+        dims = [(n, s) for n, s in zip(t.shape, t.stride()) if n != 1]
+        width = t.element_size()
+        while dims and dims[-1][1] * t.element_size() == width:  # the trailing contiguous block
+            width *= dims.pop()[0]
+        if not dims:
+            return width, width, 1
+        pitch, rows = dims[-1][1] * t.element_size(), 1
+        for k, (n, s) in enumerate(dims):
+            if k + 1 < len(dims) and s != dims[k + 1][1] * dims[k + 1][0]:
+                return None
+            rows *= n
+        return (width, pitch, rows) if pitch >= width else None
+
+    def _gatherable(self, t: torch.Tensor):
+        """The (width, pitch, rows) of a non-contiguous CUDA tensor that the fused put can read in place: rows (see
+        _source_rows), a 16-byte aligned start and a row gap that is a multiple of 16 bytes.  None for any other tensor;
+        those are made contiguous on the device first, which beats staging them through the host."""
+        if not t.is_cuda or t.is_contiguous() or t.numel() == 0 or t.data_ptr() % 16:
+            return None
+        r = self._source_rows(t)
+        return r if r is not None and (r[2] == 1 or (r[1] - r[0]) % 16 == 0) else None
+
     def batch_put(self, keys: Sequence[str], tensors: Sequence[torch.Tensor], pack_fp8: bool = False, config=None) -> None:
+        """Stores each tensor under its key.  A slice of a larger CUDA tensor whose elements are rows -- `W[:, a:b]`, `kv[:,
+        :, h0:h1, :]`, `t[::k]` -- is read in place by the fused put kernel (batch_put_device_strided) when its start is
+        16-byte aligned and its row gap a multiple of 16 bytes; no contiguous copy is made.  Other layouts, and every tensor
+        with pack_fp8, are made contiguous first.  The stored object is that of `t.contiguous()` either way."""
         cfg = config or self.config
         keys = list(keys)
-        tensors = [t.contiguous() for t in tensors]
+        tensors = list(tensors)
+        rows = [None if pack_fp8 else self._gatherable(t) for t in tensors]
+        tensors = [t if r is not None else t.contiguous() for t, r in zip(tensors, rows)]
         if pack_fp8:
             # objects the fused kernel can take go through batch_put_device_fp8 (bf16 read once, packed bytes on the
             # wire, digest of the packed object from the tensor cores); the rest are packed first (unfused path below)
@@ -90,8 +124,14 @@ class TensorStore:
             assert t.data_ptr() % 16 == 0, "tensor storage must be 16-byte aligned"
             payloads.append(t)
             metas.append(json.dumps(meta).encode())
-        ecs = self.client.batch_put_device(list(keys), [p.data_ptr() for p in payloads], [p.numel() * p.element_size() for p in payloads],
-                                           cfg, self._stream())
+        ptrs, sizes = [p.data_ptr() for p in payloads], [p.numel() * p.element_size() for p in payloads]
+        if any(r is not None for r in rows):
+            # one call and one launch for the whole batch: the other tensors go as one row each (pack_fp8 has no rows)
+            shapes = [r if r is not None else (n, n, 1) for r, n in zip(rows, sizes)]
+            ecs = self.client.batch_put_device_strided(list(keys), ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
+                                                       [s[2] for s in shapes], cfg, self._stream())
+        else:
+            ecs = self.client.batch_put_device(list(keys), ptrs, sizes, cfg, self._stream())
         bad = [(k, e) for k, e in zip(keys, ecs) if e != _bb.ErrorCode.OK]
         if bad:
             raise RuntimeError(f"put failed: {bad[:3]}")

@@ -958,14 +958,15 @@ static void ewma_update(std::atomic<double>& v, double sample) {
 }
 
 // The fused kernels move 16-byte aligned buffers only (XferEngine::submit refuses a whole batch otherwise).  An object
-// whose caller buffer is not 16-byte aligned where one of its shards starts is staged through host memory instead, so
-// that it does not fail its neighbours.
-static bool fabric_aligned(const void* ptr, const std::vector<CopyPlacement>& copies) {
+// whose caller buffer is not 16-byte aligned where one of its shards starts -- for a strided source, whose shards are not
+// co-aligned -- is staged through host memory instead, so that it does not fail its neighbours.
+static bool fabric_aligned(const void* ptr, const SourceRows& rows, const std::vector<CopyPlacement>& copies) {
   const auto base = reinterpret_cast<uintptr_t>(ptr);
   for (const auto& c : copies) {
     uint64_t off = 0;
     for (const auto& sh : c.shards) {
-      if ((base + off) & 15) return false;
+      uint64_t at = 0;
+      if (!rows.rebase(off, &at).coaligned(base + at, sh.length)) return false;
       off += sh.length;
     }
   }
@@ -974,10 +975,52 @@ static bool fabric_aligned(const void* ptr, const std::vector<CopyPlacement>& co
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                                          const std::vector<size_t>& sizes, const WorkerConfig& cfg, void* stream) {
+  return put_device(keys, dev_ptrs, sizes, nullptr, cfg, stream);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
+                                                                 const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                                                 const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
+  const size_t n = keys.size();
+  if (dev_ptrs.size() != n || widths.size() != n || pitches.size() != n || rows.size() != n)
+    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  // invalid items fail here, before the Keystone allocates anything for them; the others are one batch
+  std::vector<ErrorCode> out(n, ErrorCode::OK);
+  std::vector<size_t> idx, sizes;
+  std::vector<ObjectKey> k;
+  std::vector<const void*> p;
+  std::vector<SourceRows> pats;
+  for (size_t i = 0; i < n; ++i) {
+    SourceRows pat;
+    uint64_t size = 0, extent = 0;
+    out[i] = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pat, &size, &extent);
+    if (out[i] != ErrorCode::OK) continue;
+    if (size > SIZE_MAX) {
+      out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
+      continue;
+    }
+    idx.push_back(i), k.push_back(keys[i]), p.push_back(dev_ptrs[i]), sizes.push_back(static_cast<size_t>(size)), pats.push_back(pat);
+  }
+  if (idx.empty()) return out;
+  const auto ecs = put_device(k, p, sizes, &pats, cfg, stream);
+  uint64_t done = 0, bytes = 0;
+  for (size_t j = 0; j < idx.size(); ++j) {
+    out[idx[j]] = ecs[j];
+    if (ecs[j] == ErrorCode::OK) ++done, bytes += sizes[j];
+  }
+  metrics_.inc("device_put_strided_total", done);
+  metrics_.inc("device_put_strided_bytes_total", bytes);
+  return out;
+}
+
+std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
+                                                   const std::vector<size_t>& sizes, const std::vector<SourceRows>* rows,
+                                                   const WorkerConfig& cfg, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size()) return out;
+  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size() || (rows && rows->size() != keys.size())) return out;
+  auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_put_device", keys.size());
 
@@ -1019,7 +1062,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
       if (copies.empty()) continue;
       // placements on host tiers (DRAM / CXL / NVMe) and unaligned caller buffers: stage through host memory and use the
       // data servers
-      bool on_fabric = fabric_aligned(dev_ptrs[i], copies);
+      bool on_fabric = fabric_aligned(dev_ptrs[i], rows_of(i), copies);
       for (const auto& c : copies)
         for (const auto& sh : c.shards) {
           // a batch lands on a handful of pools: ask the transport once per run of shards on the same pool
@@ -1036,6 +1079,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
       }
       bool same_layout = true;
       for (const auto& c : copies) same_layout &= c.shards.size() == copies[0].shards.size();
+      const SourceRows pat = rows_of(i);
       if (same_layout) {
         uint64_t off = 0;
         for (size_t s = 0; s < copies[0].shards.size(); ++s) {
@@ -1045,6 +1089,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
           op.shard = s;
           op.placement = &copies[0].shards[s];
           op.obj_offset = off;
+          op.rows = pat.rebase(off, &op.rows_at);
           for (size_t c = 1; c < copies.size(); ++c) op.replicas.push_back(&copies[c].shards[s]);
           ch.ops.push_back(std::move(op));
           off += copies[0].shards[s].length;
@@ -1059,6 +1104,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
             op.shard = s;
             op.placement = &copies[c].shards[s];
             op.obj_offset = o2;
+            op.rows = pat.rebase(o2, &op.rows_at);
             ch.ops.push_back(std::move(op));
             o2 += copies[c].shards[s].length;
           }
@@ -1133,10 +1179,19 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device(const std::vector<Objec
     start_chunk(chunks[c]);
   }
   while (finished < chunks.size()) finish_chunk(chunks[finished++]);
-  // host-tier placements: D2H into a staging buffer, then the TCP data path (checksums on the CPU)
+  // host-tier placements: D2H into a staging buffer, then the TCP data path (checksums on the CPU).  A strided source is
+  // copied as its whole extent in one D2H, and its rows compacted here.
   for (size_t i : host_put) {
     std::vector<uint8_t> stage(sizes[i]);
-    ErrorCode ec = device_->copy_d2h(stage.data(), dev_ptrs[i], sizes[i], stream);
+    const SourceRows pat = rows_of(i);
+    ErrorCode ec;
+    if (pat.strided()) {
+      std::vector<uint8_t> extent(pat.extent(sizes[i]));
+      ec = device_->copy_d2h(extent.data(), dev_ptrs[i], extent.size(), stream);
+      pat.for_each_run(sizes[i], [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(stage.data() + x, extent.data() + at, n); });
+    } else {
+      ec = device_->copy_d2h(stage.data(), dev_ptrs[i], sizes[i], stream);
+    }
     ShardChecksums sums;
     if (ec == ErrorCode::OK) ec = transfer_put(host_placed[i], stage.data(), cfg.checksum, &sums);
     if (ec == ErrorCode::OK) ec = keystone_->put_complete(keys[i], sums);
@@ -1363,7 +1418,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           }
         }
       } else {
-        aligned = fabric_aligned(bases[i], copies);
+        aligned = fabric_aligned(bases[i], SourceRows{}, copies);
       }
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
@@ -1534,7 +1589,14 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
   std::vector<uint64_t> digests(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
-    const auto* src = static_cast<const uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
+    const auto* src = static_cast<const uint8_t*>(op.src(dev_ptrs[op.item]));
+    std::vector<uint8_t> dense;
+    if (op.rows.strided()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows
+      if (!op.rows.valid()) return ErrorCode::INVALID_ARGUMENT;
+      dense.resize(op.placement->length);
+      op.rows.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, src + at, n); });
+      src = dense.data();
+    }
     ErrorCode ec = io_->write_shard(*op.placement, src, &digests[k], algo);
     for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], src, nullptr, ChecksumAlgo::NONE);
     if (ec != ErrorCode::OK) return ec;

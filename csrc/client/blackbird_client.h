@@ -62,6 +62,13 @@ struct DeviceShardOp {
   // The base `win` goes with, given the object's: dev_ptrs[item] is where object byte 0 lands, or for a strided get where
   // the result's row 0 lands.
   void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(obj_offset); }
+  // Put: where the shard's bytes are read from (common/store_window.h), the object's source rows rebased to obj_offset, and
+  // rows_at, where the shard's pattern row 0 starts relative to dev_ptrs[item].  The default is a contiguous source.
+  SourceRows rows;
+  uint64_t rows_at = 0;
+  const void* src(const void* obj_base) const {
+    return static_cast<const uint8_t*>(obj_base) + (rows.strided() ? rows_at : obj_offset);
+  }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
@@ -175,6 +182,19 @@ class BlackbirdClient {
   void set_device_transport(std::shared_ptr<DeviceTransport> t) { device_ = std::move(t); }
   std::vector<ErrorCode> batch_put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                           const std::vector<size_t>& sizes, const WorkerConfig& cfg, void* stream);
+  // Puts of strided sources (a slice of a larger tensor along an inner dimension): object i is the rows[i] * widths[i]
+  // bytes of rows[i] rows of widths[i] bytes, row r read from dev_ptrs[i] + r * pitches[i] (SourceRows in
+  // common/store_window.h).  The stored object and its digests are those of batch_put_device of the compacted rows, so
+  // every get reads it.  The fused path gathers the rows in the put kernel; it needs dev_ptrs[i] 16-byte aligned, for
+  // rows[i] > 1 (pitches[i] - widths[i]) % 16 == 0, and every shard start 16-byte aligned.  Any other item, and every
+  // placement the fabric cannot reach, is staged through the host (one copy of the source extent, rows compacted there)
+  // while the rest of the batch keeps the fused launch.  Per object, before anything is allocated: INVALID_ARGUMENT for
+  // widths[i] > pitches[i] with rows[i] > 1; VALUE_OUT_OF_RANGE when the size or the extent overflows.  rows[i] == 1 or
+  // widths[i] == pitches[i] is exactly batch_put_device of one contiguous block, rows[i] == 0 or widths[i] == 0 that of a
+  // zero-byte object.
+  std::vector<ErrorCode> batch_put_device_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
+                                                  const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                                  const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream);
   // out_sizes[i] receives the object size; buffers must be large enough (capacity[i]).
   std::vector<ErrorCode> batch_get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                           const std::vector<size_t>& capacity, void* stream, std::vector<size_t>* out_sizes);
@@ -225,6 +245,9 @@ class BlackbirdClient {
     uint64_t offset = 0, length = 0;
     uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)
   };
+  // batch_put_device and batch_put_device_strided: `rows` null = contiguous sources, else object i is read by (*rows)[i].
+  std::vector<ErrorCode> put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs, const std::vector<size_t>& sizes,
+                                    const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
   // batch_get_device_fp8, batch_get_device_fp8_range and batch_get_device_fp8_strided: `ranges` null = whole tensors, else

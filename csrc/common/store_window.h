@@ -9,6 +9,8 @@
 //   (row + (x + phase) / pitch) * width + c    strided: the base is where the result's row 0 lands, so the rows land densely
 //                                              and pattern row 0 is result row `row` (negative when the window starts later).
 // The default window, [0, UINT64_MAX) without a pattern, is the whole object.
+//
+// SourceRows, below, is the put side's counterpart: where each byte of an object is read from a strided source.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -122,6 +124,84 @@ struct StoreWindow {
       }
       const uint64_t n = std::min(width - c, end - x);
       f(x, (static_cast<uint64_t>(row) + y / pitch) * width + c, n);
+      x += n;
+    }
+  }
+};
+
+// SourceRows: where a device put reads each byte of an object from, when the source is rows of `width` bytes every `pitch`
+// bytes (a slice of a larger tensor).  It is the inverse of a strided StoreWindow, which maps a strided object onto a dense
+// destination: here the object is dense and the source strided.  This is the one statement of the rule; the transfer
+// engine (XferItem), the fabric's DeviceShardOp, the client, the host loopback transport and the kernel's XFER_GATHER
+// descriptors (kernels/xfer.h) all follow it.
+//
+// With `src` where the pattern's row 0 starts, object byte x is read from
+//   src + ((x + phase) / width) * pitch + (x + phase) % width
+// so the rows are read back to back and the object holds no gaps.  pitch == 0 (the default) is a contiguous source: byte x
+// at src + x.
+struct SourceRows {
+  uint64_t pitch = 0, width = 0, phase = 0;
+
+  bool strided() const { return pitch != 0; }
+  // 0 < width <= pitch and phase < width for a pattern.
+  bool valid() const { return !strided() || (width != 0 && width <= pitch && phase < width); }
+
+  // The source of `rows` rows of `width` bytes every `pitch` bytes: an object of *size = rows * width bytes spread over
+  // *extent = (rows - 1) * pitch + width source bytes.  INVALID_ARGUMENT for several rows wider than the pitch;
+  // VALUE_OUT_OF_RANGE when either product overflows.  One row, rows that touch, no rows and rows of zero width are a
+  // contiguous source (no pattern).
+  static ErrorCode from_rows(uint64_t width, uint64_t pitch, uint64_t rows, SourceRows* out, uint64_t* size, uint64_t* extent) {
+    *out = {};
+    if (rows > 1 && width > pitch) return ErrorCode::INVALID_ARGUMENT;
+    if (rows == 0 || width == 0) {
+      *size = *extent = 0;
+      return ErrorCode::OK;
+    }
+    if (__builtin_mul_overflow(rows, width, size) || __builtin_mul_overflow(rows - 1, pitch, extent) ||
+        __builtin_add_overflow(*extent, width, extent))
+      return ErrorCode::VALUE_OUT_OF_RANGE;
+    if (rows > 1 && width < pitch) out->pitch = pitch, out->width = width;
+    return ErrorCode::OK;
+  }
+
+  // The pattern seen from object byte `off`: byte x of the result is byte off + x here, read relative to a source that
+  // has moved by *shift bytes (where the new pattern's row 0 starts).
+  SourceRows rebase(uint64_t off, uint64_t* shift) const {
+    if (!strided()) {
+      *shift = off;
+      return *this;
+    }
+    *shift = (phase + off) / width * pitch;
+    return {pitch, width, (phase + off) % width};
+  }
+
+  // Source bytes from where the pattern's row 0 starts to the last byte object bytes [0, n) are read from.
+  uint64_t extent(uint64_t n) const {
+    if (!strided() || n == 0) return n;
+    const uint64_t last = n - 1 + phase;
+    return last / width * pitch + last % width + 1;
+  }
+
+  // Whether object bytes [0, len) read from `src` are co-aligned with the tiles, so that the kernel only bulk-loads 16-byte
+  // congruent spans: byte x of row r is read from src + phase + r * (pitch - width) + x, so src + phase must be 16-byte
+  // aligned, and the gap a multiple of 16 when the span covers more than one row.
+  bool coaligned(uintptr_t src, uint64_t len) const {
+    if (!strided()) return src % 16 == 0;
+    if (len > 0 && (len - 1 + phase) / width > 0 && (pitch - width) % 16) return false;
+    return (src + phase) % 16 == 0;
+  }
+
+  // Calls f(x, at, n) for every run of n contiguous source bytes of object bytes [0, len): object bytes [x, x + n) are read
+  // from src + at, in order.
+  template <class F>
+  void for_each_run(uint64_t len, F&& f) const {
+    if (!strided()) {
+      if (len) f(0, 0, len);
+      return;
+    }
+    for (uint64_t x = 0; x < len;) {
+      const uint64_t y = x + phase, c = y % width, n = std::min(width - c, len - x);
+      f(x, y / width * pitch + c, n);
       x += n;
     }
   }

@@ -528,8 +528,12 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
   for (size_t k = 0; k < ops.size(); ++k) {
     const auto& op = ops[k];
     XferItem it;
-    it.src = static_cast<const uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
+    it.src = op.src(dev_ptrs[op.item]);
     it.nbytes = op.placement->length;
+    if (op.rows.strided()) {  // a gathered put: every pass and the multicast item read the same rows
+      it.rows = op.rows;
+      it.flags |= XFER_GATHER;
+    }
     // NVLS: the replica set is one whole multicast group at one offset -> a single multimem.st stream
     if (arena_ && !op.replicas.empty() && (it.nbytes & 15) == 0) {
       size_t grp = 0, g2 = 0;
@@ -571,6 +575,8 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
       XferItem more;
       more.src = it.src;
       more.nbytes = it.nbytes;
+      more.rows = it.rows;
+      more.flags = it.flags & XFER_GATHER;
       more.ndst = 0;
       for (; r < op.replicas.size() && more.ndst < kMaxDst; ++r) {
         auto d = resolve(*op.replicas[r]);

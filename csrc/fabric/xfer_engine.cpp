@@ -77,11 +77,13 @@ struct XferEngine::Slot {
   bool crc = false;
   uint64_t empty_digest = 0;
   std::vector<int32_t> item_to_desc;  // -1 for zero-size items
-  std::vector<XferStride> strides;     // per descriptor up to the last XFER_STRIDED one; empty when the batch has none
-  void set_stride(uint32_t k, const StoreWindow& w) {
+  // per descriptor up to the last XFER_STRIDED or XFER_GATHER one; empty when the batch has none
+  std::vector<XferStride> strides;
+  void set_stride(uint32_t k, const XferStride& e) {
     if (strides.size() <= k) strides.resize(k + 1, XferStride{1, 1, 0});
-    strides[k] = {w.pitch, w.width, w.phase};
+    strides[k] = e;
   }
+  void set_stride(uint32_t k, const StoreWindow& w) { set_stride(k, XferStride{w.pitch, w.width, w.phase}); }
   // Writes the stride table behind tile_start when the batch has a strided descriptor, and returns the bytes of the
   // table to copy to the device: [descs | tile_start | strides], or without the strides.
   size_t write_strides(uint32_t nd) {
@@ -322,8 +324,11 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const XferItem& it = items[i];
     const bool win = it.flags & XFER_WINDOW;
     const bool strided = it.flags & XFER_STRIDED;
+    const bool gather = it.flags & XFER_GATHER;
     if ((strided && !win) || (win && (strided != it.win.strided() || !it.win.valid(it.nbytes) || it.ndst != 1 ||
                                       (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
+      return ErrorCode::INVALID_ARGUMENT;
+    if (gather != it.rows.strided() || (gather && (!it.rows.valid() || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
@@ -333,13 +338,15 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
       continue;
     }
-    // windowed items (strided ones included) always take bb_xfer: neither the warp-per-object kernel nor the mailbox has a
-    // store window
-    all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW)) && it.ndst >= 1;
+    // windowed items (strided ones included) and gathered ones always take bb_xfer: neither the warp-per-object kernel nor
+    // the mailbox has a store window or a gathering load
+    all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW | XFER_GATHER)) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
-    uintptr_t al = reinterpret_cast<uintptr_t>(it.src);
+    uintptr_t al = gather ? 0 : reinterpret_cast<uintptr_t>(it.src);  // gathered: source rows instead
     for (uint32_t r = strided ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);  // strided: rows instead
-    if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0])))) return ErrorCode::INVALID_ADDRESS;
+    if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]))) ||
+        (gather && !it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes)))
+      return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
     d.src = static_cast<const uint8_t*>(it.src) + trim;
@@ -351,6 +358,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       d.win.hi = w.hi;
       if (strided) s->set_stride(nd, w);
     }
+    if (gather) s->set_stride(nd, XferStride{it.rows.pitch, it.rows.width, it.rows.phase});
     d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;

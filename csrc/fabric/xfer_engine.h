@@ -31,6 +31,10 @@ struct XferItem {
   // win.coaligned(dst[0]).  The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine
   // reads only the 16-byte aligned span of the window (see window_read_bytes).
   StoreWindow win;
+  // Put of a strided source (common/store_window.h): src is where the pattern's row 0 starts; XFER_GATHER exactly when it
+  // has a pattern.  INVALID_ARGUMENT for an invalid pattern, or one with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM;
+  // INVALID_ADDRESS unless rows.coaligned(src, nbytes), which replaces the 16-byte alignment check of src.
+  SourceRows rows;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span

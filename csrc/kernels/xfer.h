@@ -29,6 +29,12 @@ enum XferFlags : uint32_t {
   // land densely from there.  The pattern is the descriptor's entry of the launch's XferStride table; the MXFP8 get
   // counts all of it in bf16 bytes of the unpacked object.
   XFER_STRIDED = 1u << 4,
+  // Gathering load (puts of a strided source), in bb_xfer only: the rule of SourceRows (common/store_window.h), so `src` is
+  // where the pattern's row 0 starts and object byte x is read from src + ((x + phase) / width) * pitch + (x + phase) % width.
+  // The pattern is the descriptor's entry of the launch's XferStride table.  Never with XFER_WINDOW, XFER_STRIDED or
+  // XFER_RAW_SUM; with 1-3 destinations or XFER_MULTIMEM.  The tile in shared memory is byte for byte the tile of the
+  // dense object, so the digest and the stored bytes are those of a put of the compacted rows.
+  XFER_GATHER = 1u << 5,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -58,7 +64,9 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 
 // Row pattern of an XFER_STRIDED descriptor (see XferFlags): 0 < width <= pitch, phase < pitch.  With pitch == width and
 // phase == 0 it stores exactly the plain window.  Every stored row must be co-aligned with the tile (the destination of
-// object byte x congruent to x mod 16), so that the kernel only bulk-stores 16-byte congruent spans.
+// object byte x congruent to x mod 16), so that the kernel only bulk-stores 16-byte congruent spans.  An XFER_GATHER
+// descriptor's entry is its source rows instead: 0 < width <= pitch, phase < width, and the source of object byte x
+// congruent to x mod 16 (SourceRows::coaligned).
 struct XferStride {
   uint64_t pitch, width, phase;
 };
@@ -86,8 +94,9 @@ struct XferLaunch {
   // kernel parameters instead (descs / tile_start may then be null).
   const XferDesc* host_descs = nullptr;
   const uint32_t* host_tile_start = nullptr;
-  // Row patterns of the XFER_STRIDED descriptors, one entry per descriptor (the entries of unflagged descriptors are never
-  // read); null when the batch has none.  host_strides is their copy for the kernel parameters of an inline batch.
+  // Row patterns of the XFER_STRIDED and XFER_GATHER descriptors, one entry per descriptor (the entries of unflagged
+  // descriptors are never read); null when the batch has none.  host_strides is their copy for the kernel parameters of an
+  // inline batch.
   const XferStride* strides = nullptr;
   const XferStride* host_strides = nullptr;
   int algo = ALGO_BBH64;

@@ -144,6 +144,36 @@ __device__ __forceinline__ void store_row_segments(const uint8_t* tile, uint64_t
     for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = tile[o];
   }
 }
+// Gathering load (XFER_GATHER, source rows `st`), the mirror of the strided store: a tile at object offset `off` of `bytes`
+// bytes holds rows first_row(...) .. + row_count(...) - 1 of the object's own dense layout {width, width, phase}, and tile
+// byte o of row r is read from row_src(...) + o.  With co-aligned rows that address is congruent to o mod 16, so each row
+// segment splits into TMA middle, head and tail exactly like a store segment.
+__device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t r, const XferStride& st) {
+  return src + off + st.phase + r * (st.pitch - st.width);
+}
+// The producer's part of a gathered tile: the row segments of the tile, one per lane, the middle bulk-loaded into `tile`
+// with completion on `bar`, head and tail by plain loads and shared stores.  Returns the bytes this lane's bulk loads
+// deliver; the caller sums them over the warp for the stage's expect_tx, and the calling lane still has to fence its
+// shared stores for the async proxy.
+__device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t* bar, uint64_t src, uint64_t off, uint32_t bytes,
+                                                        const XferStride& st, uint32_t lane) {
+  const XferStride dense{st.width, st.width, st.phase};
+  const uint64_t r0 = first_row(off, 0, dense);
+  const uint32_t nrow = row_count(off, 0, bytes, dense);
+  uint32_t tx = 0;
+  for (uint32_t k = lane; k < nrow; k += 32) {
+    const uint64_t r = r0 + k;
+    const TileSpan g = segment_span(off, 0, bytes, r, dense);
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_src(src, off, r, st));
+    if (g.a1 > g.a0) {
+      ptx::bulk_g2s(tile + g.a0, s + g.a0, g.a1 - g.a0, bar);
+      tx += g.a1 - g.a0;
+    }
+    for (uint32_t o = g.x0; o < g.h1; ++o) tile[o] = s[o];
+    for (uint32_t o = g.tb; o < g.x1; ++o) tile[o] = s[o];
+  }
+  return tx;
+}
 // The row pattern of descriptor `i` from a device table (read-only path).
 __device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i) {
   const uint64_t* e = reinterpret_cast<const uint64_t*>(&table[i]);

@@ -6,7 +6,9 @@
 //
 //   warp 0  producer : descriptor lookup (32 tiles looked up in parallel, xfer_common.cuh), zero-pads short
 //                      tiles, `cp.async.bulk` global -> shared (TMA, mbarrier complete_tx).
-//                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).
+//                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).  A gathering load
+//                      (XFER_GATHER: a put of a strided source) fills the tile from its source row segments, one per
+//                      lane, so the tile is byte for byte the tile of the dense object.
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
 //                      to an NVLS multicast address (one store, N replicas).  A store window (XFER_WINDOW) cuts
@@ -217,6 +219,8 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
   if (warp == 0) {
     // ================================================================ TMA producer
     uint32_t it = 0;
+    uint32_t g_desc = 0xFFFFFFFFu;  // descriptor whose source rows are in `gst`
+    XferStride gst{1, 1, 0};
     for (uint32_t base = 0; base < my_tiles; base += 32) {
       const uint32_t idx = base + lane;
       if (idx < my_tiles) {
@@ -255,6 +259,7 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
         const uint32_t bytes = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), e.m.nbytes - off));
         const uint32_t b16 = bytes & ~15u;
         const uint32_t tail = bytes & 15u;
+        const bool gather = (e.m.ndst_flags >> 8) & XFER_GATHER;
         mbar_wait(&s.empty[stage], par ^ 1u);
         bool wrote = false;
         if constexpr (kHash) {
@@ -264,7 +269,19 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
             wrote = true;
           }
         }
-        if (lane < tail) {
+        uint32_t tx = b16;  // bytes the stage's bulk loads deliver
+        if (gather) {
+          // one row segment per lane; the pad above may have zeroed the 16-byte chunk that holds a gathered tail, so the
+          // gathered bytes are written after it
+          __syncwarp();
+          if (e.m.desc != g_desc) {
+            g_desc = e.m.desc;
+            if (p.use_inline) gst = p.inl_strides[g_desc];
+            else gst = load_stride(p.strides, g_desc);
+          }
+          tx = __reduce_add_sync(0xffffffffu, gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane));
+          wrote = true;
+        } else if (lane < tail) {
           s.tile[stage][b16 + lane] = *reinterpret_cast<const uint8_t*>(src_i + off + b16 + lane);
           wrote = true;
         }
@@ -277,8 +294,8 @@ __global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_const
         __syncwarp();
         if (lane == 0) {
           s.dirty[stage] = (bytes + 15u) & ~15u;
-          mbar_arrive_expect_tx(&s.full[stage], b16);
-          if (b16) bulk_g2s(s.tile[stage], reinterpret_cast<const void*>(src_i + off), b16, &s.full[stage]);
+          mbar_arrive_expect_tx(&s.full[stage], tx);
+          if (b16 && !gather) bulk_g2s(s.tile[stage], reinterpret_cast<const void*>(src_i + off), b16, &s.full[stage]);
           if (p.trace_d) p.trace_d[static_cast<uint64_t>(t0 + base + i) * 4 + 0] = globaltimer_ns();
         }
         __syncwarp();

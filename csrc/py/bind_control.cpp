@@ -347,6 +347,39 @@ void bind_control(py::module_& m) {
   // ---------------------------------------------------------------- allocator
   using alloc::AllocationRequest;
   using alloc::AllocationResult;
+  py::class_<SourceRows>(m, "SourceRows", "Where a device put reads each object byte from a strided source (common/store_window.h).")
+      .def(py::init([](uint64_t pitch, uint64_t width, uint64_t phase) { return SourceRows{pitch, width, phase}; }), py::arg("pitch") = 0,
+           py::arg("width") = 0, py::arg("phase") = 0)
+      .def_readonly("pitch", &SourceRows::pitch)
+      .def_readonly("width", &SourceRows::width)
+      .def_readonly("phase", &SourceRows::phase)
+      .def("strided", &SourceRows::strided)
+      .def("valid", &SourceRows::valid)
+      .def_static("from_rows",
+                  [](uint64_t width, uint64_t pitch, uint64_t rows) {
+                    SourceRows r;
+                    uint64_t size = 0, extent = 0;
+                    const ErrorCode ec = SourceRows::from_rows(width, pitch, rows, &r, &size, &extent);
+                    return py::make_tuple(ec, r, size, extent);
+                  },
+                  py::arg("width"), py::arg("pitch"), py::arg("rows"), "(ErrorCode, SourceRows, object bytes, source extent)")
+      .def("rebase",
+           [](const SourceRows& r, uint64_t off) {
+             uint64_t shift = 0;
+             const SourceRows s = r.rebase(off, &shift);
+             return py::make_tuple(s, shift);
+           },
+           py::arg("off"), "(the pattern seen from object byte off, how far the source moves)")
+      .def("extent", &SourceRows::extent, py::arg("n"))
+      .def("coaligned", &SourceRows::coaligned, py::arg("src"), py::arg("len"))
+      .def("runs",
+           [](const SourceRows& r, uint64_t len) {
+             std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> out;
+             r.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { out.emplace_back(x, at, n); });
+             return out;
+           },
+           py::arg("len"), "[(x, at, n)]: object bytes [x, x + n) are read from source bytes [at, at + n)");
+
   using alloc::PoolAllocator;
   using alloc::Range;
   using alloc::RangeAllocator;
@@ -1211,7 +1244,17 @@ void bind_control(py::module_& m) {
         for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
         return ecs_to_py(nogil([&] { return c.batch_put_device(keys, p, sizes, cfg, reinterpret_cast<void*>(stream)); }));
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("sizes"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0)
-      .def("batch_get_device", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+      .def("batch_put_device_strided", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+                                          const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                          const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream) {
+        std::vector<const void*> p;
+        for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
+        return ecs_to_py(nogil([&] { return c.batch_put_device_strided(keys, p, widths, pitches, rows, cfg, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("widths"), py::arg("pitches"), py::arg("rows"), py::arg("config") = WorkerConfig{},
+         py::arg("stream") = 0,
+         "Object i = rows[i] rows of widths[i] bytes, row r read from dev_ptrs[i] + r * pitches[i]; stored as a put of the "
+         "compacted rows would store it; returns one ErrorCode per object.")
+      .def("batch_get_device",[](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                   const std::vector<size_t>& caps, uintptr_t stream) {
         std::vector<void*> p;
         for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));

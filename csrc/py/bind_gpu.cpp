@@ -44,13 +44,13 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
-// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None).  An empty destination list makes
-// a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets XFER_WINDOW, and one with
-// a pattern XFER_STRIDED as well.
+// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None).  An empty destination
+// list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets XFER_WINDOW, and
+// one with a pattern XFER_STRIDED as well.  A gather pattern (pitch, width, phase) sets XFER_GATHER, with src = row 0.
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 7)
-    throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)]]]])");
+  if (t.size() < 3 || t.size() > 8)
+    throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, (pitch, width, phase)]]]]])");
   XferItem it;
   it.src = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
   it.ndst = to_ptrs(t[1], it.dst);
@@ -59,6 +59,12 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
+  if (t.size() > 7 && !t[7].is_none()) {
+    auto g = t[7].cast<std::vector<uint64_t>>();
+    if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
+    it.rows = {g[0], g[1], g[2]};
+    it.flags |= XFER_GATHER;
+  }
   return it;
 }
 }  // namespace
@@ -70,6 +76,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_RAW_SUM") = static_cast<uint32_t>(XFER_RAW_SUM);
   m.attr("XFER_WINDOW") = static_cast<uint32_t>(XFER_WINDOW);
   m.attr("XFER_STRIDED") = static_cast<uint32_t>(XFER_STRIDED);
+  m.attr("XFER_GATHER") = static_cast<uint32_t>(XFER_GATHER);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -104,7 +111,8 @@ void bind_gpu(py::module_& m) {
            "bytes [lo, hi) are stored, object byte x at dst + x (pass dst = buffer - lo; one destination; with "
            "ChecksumAlgo.NONE only the window's 16-byte aligned span is read).  A window (lo, hi, pitch, width, phase) also "
            "sets XFER_STRIDED: of [lo, hi), byte x is stored iff c = (x + phase) % pitch < width, at dst + ((x + phase) // "
-           "pitch) * width + c; returns (digests, status, device_ms).")
+           "pitch) * width + c.  A gather pattern (pitch, width, phase) as the eighth element sets XFER_GATHER: object byte x "
+           "is read from src + ((x + phase) // width) * pitch + (x + phase) % width; returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
              std::vector<gpu::Fp8Item> v;
