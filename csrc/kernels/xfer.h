@@ -102,12 +102,24 @@ struct XferLaunch {
   int algo = ALGO_BBH64;
   bool small_path = false;               // every descriptor is <= kSmallBytes, none is a RAW_SUM slice: warp-per-object kernel
   bool flag_completion = false;          // small path only: status_out (pinned, preset to kSmallPending) is the completion flag
-  int max_ctas = 0;                      // 0 = one CTA per SM
+  int max_ctas = 0;                      // 0 = the default geometry (xfer_geometry)
   void* stream = nullptr;                // cudaStream_t
 };
 
 // Returns 0 on success, else a cudaError_t value.
 int launch_xfer(const XferLaunch& l);
+// What launch_xfer's fused kernel launches for a batch of `total_tiles` tiles on the current device.  CRC32C: one
+// persistent CTA per SM.  The other digests: CTAs of at most 8 tiles, at least two per SM, which the block scheduler
+// hands to whichever SM frees a slot first.  max_ctas > 0 (or else BB_XFER_CTAS) sets the grid instead.  Every CTA gets
+// ceil(total_tiles / grid) consecutive tiles and CTAs that would get none are not launched.
+struct XferGeometry {
+  int grid = 0;        // CTAs
+  int stages = 0;      // 16 KiB shared-memory pipeline stages per CTA
+  int smem_bytes = 0;  // dynamic shared memory per CTA
+};
+XferGeometry xfer_geometry(int algo, uint32_t total_tiles, int max_ctas);
+// CTAs of the fused kernel for `algo` the current device keeps resident per SM (occupancy query); -1 on a CUDA error.
+int xfer_resident_ctas(int algo);
 // ---- mailbox (xfer_small.cu): a resident warp fed through pinned host memory, so that a single small put / get costs no
 // kernel launch.  All three structures live in pinned host memory (the device reads / writes them over PCIe).
 constexpr uint32_t kMailSlots = 16;

@@ -1,8 +1,9 @@
 // bb_xfer: the fused batched put/get kernel (sm_90a).
 //
 // Replaces the reference's per-shard UCX RMA calls (blackbird_client.cpp:231-237 put,
-// :315-327 get; SURVEY K1/K4/K6/K11/K13) with ONE persistent launch per batch.  Every CTA owns
-// a contiguous run of 16 KiB tiles of the batch and pipelines them through 8 smem stages:
+// :315-327 get; SURVEY K1/K4/K6/K11/K13) with ONE launch per batch.  Every CTA owns a contiguous
+// run of 16 KiB tiles of the batch (at most 8 tiles, two CTAs per SM, for NONE / XXH3 / BBH64; one
+// persistent CTA per SM for CRC32C: see kStagesFor) and pipelines them through 6 (8) smem stages:
 //
 //   warp 0  producer : descriptor lookup (32 tiles looked up in parallel, xfer_common.cuh), zero-pads short
 //                      tiles, `cp.async.bulk` global -> shared (TMA, mbarrier complete_tx).
@@ -50,10 +51,25 @@ namespace {
 
 using namespace bb::ptx;
 
-constexpr int kStages = 8;
 constexpr int kThreads = 256;
 constexpr int kStoreLag = 2;         // stores may trail this many tiles before their stage is released
 static_assert(kTileBytes == tchash::kTileBytes);
+
+// Launch geometry.  The DRAM-bound digests (NONE, XXH3, BBH64) run short CTAs of at most kRunTiles tiles, two resident
+// per SM with 6 stages each (12 tiles in flight per SM), and leave the balancing to the hardware block scheduler: a CTA
+// that finishes frees its slot for the next run, so a launch no longer ends with the slowest SM's fixed share of the
+// batch.  CRC32C is bound by shared-memory lookups, not by DRAM, and each CTA builds ~14 KB of shift tables before its
+// first tile: it keeps one persistent CTA per SM with 8 stages.
+template <int ALGO>
+constexpr int kStagesFor = ALGO == ALGO_CRC32C ? 8 : 6;
+// CTAs per SM that shared memory admits at STAGES stages of 16 KiB (checked against SmemT below).
+constexpr int resident_ctas(int stages) { return stages <= 6 ? 2 : 1; }
+// Tiles per CTA run of the short-CTA geometry (128 KiB).  bench/cta_balance.py at 64 x 64 MiB, XXH3, H100 SXM 80 GB at
+// 700 W, kernel-only put ms for runs of 64 / 32 / 24 / 16 / 12 / 8 / 4 tiles: 3.00 / 2.98 / 2.97 / 2.94 / 2.93 / 2.88 /
+// 2.86 (one persistent CTA per SM: 3.01).  Shorter runs raise the steady rate and cut the end-of-launch tail to ~10 µs
+// at 8 tiles.  4-tile runs were another 1% faster on that local-HBM shape, but a run
+// shorter than the 6-stage ring cannot fill it, and peer reads over NVLink need every tile in flight to hide latency.
+constexpr uint32_t kRunTiles = 8;
 
 __constant__ uint64_t c_col_mul[tchash::kN];
 __constant__ uint32_t c_xpow_tiles[32];  // x^(8 * 16384 * 2^j) mod P  (CRC32C cross-CTA combine)
@@ -85,7 +101,7 @@ struct LookupEntry {  // producer-private staging of 32 parallel lookups
   uint64_t pad;
 };
 
-template <int ALGO>
+template <int ALGO, int kStages>
 struct __align__(1024) SmemT {
   uint8_t tile[kStages][kTileBytes];
   uint8_t w[2048];
@@ -165,9 +181,9 @@ __device__ __forceinline__ uint32_t warp_xpow_tiles(uint32_t k, uint32_t lane) {
   return v;
 }
 
-template <int ALGO>
-__global__ void __launch_bounds__(kThreads, 1) bb_xfer_kernel(const __grid_constant__ Params p) {
-  using Smem = SmemT<ALGO>;
+template <int ALGO, int kStages>
+__global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kernel(const __grid_constant__ Params p) {
+  using Smem = SmemT<ALGO, kStages>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
   const uint32_t warp = threadIdx.x >> 5;
@@ -591,21 +607,70 @@ PerDeviceOnce g_crc_once;    // CRC32C shift tables, on the first CRC32C launch
 uint32_t* g_crc_tables[kMaxDevices] = {};
 
 template <int ALGO>
+using SmemOf = SmemT<ALGO, kStagesFor<ALGO>>;
+template <int ALGO>
+constexpr auto kKernelOf = bb_xfer_kernel<ALGO, kStagesFor<ALGO>>;
+
+// Two CTAs per SM: 227 KiB of shared memory per SM for blocks, each block also reserving 1 KiB for the system.
+template <int ALGO>
+constexpr bool fits_resident = resident_ctas(kStagesFor<ALGO>) * (sizeof(SmemOf<ALGO>) + 1024) <= 228 * 1024;
+static_assert(fits_resident<ALGO_NONE> && fits_resident<ALGO_CRC32C> && fits_resident<ALGO_XXH3> && fits_resident<ALGO_BBH64>);
+
+template <int ALGO>
 cudaError_t launch_t(int dev, const Params& p, int grid, cudaStream_t st) {
-  const cudaError_t e = set_max_dynamic_smem_once<bb_xfer_kernel<ALGO>>(dev, static_cast<int>(sizeof(SmemT<ALGO>)));
+  const cudaError_t e = set_max_dynamic_smem_once<kKernelOf<ALGO>>(dev, static_cast<int>(sizeof(SmemOf<ALGO>)));
   if (e != cudaSuccess) return e;
-  bb_xfer_kernel<ALGO><<<grid, kThreads, sizeof(SmemT<ALGO>), st>>>(p);
+  kKernelOf<ALGO><<<grid, kThreads, sizeof(SmemOf<ALGO>), st>>>(p);
   return cudaGetLastError();
+}
+
+template <int ALGO>
+int resident_t(int dev) {
+  int n = 0;
+  if (set_max_dynamic_smem_once<kKernelOf<ALGO>>(dev, static_cast<int>(sizeof(SmemOf<ALGO>))) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kKernelOf<ALGO>, kThreads, sizeof(SmemOf<ALGO>)) != cudaSuccess)
+    return -1;
+  return n;
 }
 
 }  // namespace
 
 int xfer_smem_bytes(int algo) {
   switch (algo) {
-    case ALGO_NONE: return static_cast<int>(sizeof(SmemT<ALGO_NONE>));
-    case ALGO_CRC32C: return static_cast<int>(sizeof(SmemT<ALGO_CRC32C>));
-    case ALGO_XXH3: return static_cast<int>(sizeof(SmemT<ALGO_XXH3>));
-    default: return static_cast<int>(sizeof(SmemT<ALGO_BBH64>));
+    case ALGO_NONE: return static_cast<int>(sizeof(SmemOf<ALGO_NONE>));
+    case ALGO_CRC32C: return static_cast<int>(sizeof(SmemOf<ALGO_CRC32C>));
+    case ALGO_XXH3: return static_cast<int>(sizeof(SmemOf<ALGO_XXH3>));
+    default: return static_cast<int>(sizeof(SmemOf<ALGO_BBH64>));
+  }
+}
+
+XferGeometry xfer_geometry(int algo, uint32_t total_tiles, int max_ctas) {
+  static const int env_ctas = [] { const char* e = std::getenv("BB_XFER_CTAS"); return e ? std::atoi(e) : 0; }();
+  const bool crc = algo == ALGO_CRC32C;
+  XferGeometry g;
+  g.stages = crc ? kStagesFor<ALGO_CRC32C> : kStagesFor<ALGO_XXH3>;
+  g.smem_bytes = xfer_smem_bytes(algo);
+  if (total_tiles == 0) return g;
+  const uint64_t sms = static_cast<uint64_t>(current_sm_count());
+  uint64_t grid;
+  if (max_ctas > 0 || env_ctas > 0) grid = static_cast<uint64_t>(max_ctas > 0 ? max_ctas : env_ctas);
+  else if (crc) grid = sms;  // one persistent CTA per SM
+  else grid = std::max(std::min(sms * resident_ctas(g.stages), uint64_t{total_tiles}), (uint64_t{total_tiles} + kRunTiles - 1) / kRunTiles);
+  grid = std::min<uint64_t>(grid, total_tiles);
+  // cta_tile_run gives every CTA ceil(total / grid) tiles: launch only the CTAs that get any
+  const uint64_t tpc = (total_tiles + grid - 1) / grid;
+  g.grid = static_cast<int>((total_tiles + tpc - 1) / tpc);
+  return g;
+}
+
+int xfer_resident_ctas(int algo) {
+  int dev = 0;
+  if (current_device(&dev) != cudaSuccess) return -1;
+  switch (algo) {
+    case ALGO_NONE: return resident_t<ALGO_NONE>(dev);
+    case ALGO_CRC32C: return resident_t<ALGO_CRC32C>(dev);
+    case ALGO_XXH3: return resident_t<ALGO_XXH3>(dev);
+    default: return resident_t<ALGO_BBH64>(dev);
   }
 }
 
@@ -703,12 +768,7 @@ int launch_xfer(const XferLaunch& l) {
   p.crc_tables = g_crc_tables[dev];
   p.debug_d = l.debug_d;
   p.trace_d = reinterpret_cast<unsigned long long*>(l.trace_d);
-  // At most 128 persistent CTAs (one per SM, 1 CTA/SM by shared memory) for the DRAM-bound digests; BB_XFER_CTAS overrides.
-  static const int env_ctas = [] { const char* e = std::getenv("BB_XFER_CTAS"); return e ? std::atoi(e) : 0; }();
-  // The fused CRC32C is bound by shared-memory lookups per SM, not by DRAM: it takes every SM.
-  const int sms = current_sm_count();
-  int grid = l.max_ctas > 0 ? l.max_ctas : env_ctas > 0 ? env_ctas : l.algo == ALGO_CRC32C ? sms : std::min(sms, 128);
-  grid = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), l.total_tiles));
+  const int grid = xfer_geometry(l.algo, l.total_tiles, l.max_ctas).grid;
   cudaStream_t st = static_cast<cudaStream_t>(l.stream);
   switch (l.algo) {
     case ALGO_NONE: e = launch_t<ALGO_NONE>(dev, p, grid, st); break;

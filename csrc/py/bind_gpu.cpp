@@ -204,6 +204,23 @@ void bind_gpu(py::module_& m) {
      "cudaMemcpyPeerAsync (copy engines): the naive P2P comparator of BASELINE.md section 4.");
   m.def("enable_peer_access", [](int device, int peer) { check_cuda(device_enable_peer_access(device, peer), "enable_peer_access"); });
   m.def("xfer_smem_bytes", [] { return xfer_smem_bytes(ALGO_BBH64); });
+  m.def(
+      "xfer_geometry",
+      [](ChecksumAlgo algo, uint32_t total_tiles, int max_ctas) {
+        const int a = algo == ChecksumAlgo::BBH64 ? ALGO_BBH64 : algo == ChecksumAlgo::CRC32C ? ALGO_CRC32C : algo == ChecksumAlgo::XXH3 ? ALGO_XXH3 : ALGO_NONE;
+        const XferGeometry g = xfer_geometry(a, total_tiles, max_ctas);
+        const int resident = xfer_resident_ctas(a);
+        if (resident < 0) throw std::runtime_error("xfer_geometry: the occupancy query failed");
+        py::dict d;
+        d["grid"] = g.grid;
+        d["stages"] = g.stages;
+        d["smem_bytes"] = g.smem_bytes;
+        d["resident_ctas_per_sm"] = resident;
+        return d;
+      },
+      py::arg("algo"), py::arg("total_tiles"), py::arg("max_ctas") = 0,
+      "Launch geometry of the fused kernel on the current device for a batch of total_tiles 16 KiB tiles: grid, stages, "
+      "smem_bytes per CTA and resident_ctas_per_sm (occupancy query); max_ctas as XferEngine.set_max_ctas.");
   m.def("mxfp8_pack", [](uintptr_t src, uint64_t n, uintptr_t dst, uintptr_t stream) {
     check_cuda(launch_mxfp8_pack(reinterpret_cast<const void*>(src), n, reinterpret_cast<void*>(dst), reinterpret_cast<void*>(stream)), "mxfp8_pack");
   }, py::arg("src_bf16"), py::arg("n_elems"), py::arg("dst_packed"), py::arg("stream") = 0);
