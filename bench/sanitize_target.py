@@ -69,4 +69,15 @@ back = torch.empty_like(x)
 _bb.mxfp8_unpack(packed.data_ptr(), x.numel(), back.data_ptr(), s)
 torch.cuda.synchronize()
 assert (back.float() - x.float()).abs().max().item() <= x.float().abs().max().item() * 2 ** -3
-print(f"sanitize target OK: {checked} kernel configurations + mxfp8")
+# fused MXFP8 put gathering its elements from rows of 128 every 544 elements, starting 4 elements into row 0 (so every
+# row segment has a head and a tail), into 2 replicas; compared with an unpatterned put of the compacted elements
+flat = (torch.randn(64 * 544, device="cuda") * 4).to(torch.bfloat16)
+n, row0 = 63 * 128, 132  # 2 * (row0 + 4) is 16-byte aligned
+x = torch.arange(n, device="cuda") + 4
+dense = flat[row0 + x // 128 * 544 + x % 128].contiguous()
+reps = [torch.zeros(_bb.mxfp8_packed_bytes(n), dtype=torch.uint8, device="cuda") for _ in range(3)]
+dg, st, _ = eng.run_fp8([(flat.data_ptr() + 2 * row0, [r.data_ptr() for r in reps[:2]], n, None, None, (544, 128, 4))], False, s)
+dg2, _, _ = eng.run_fp8([(dense.data_ptr(), reps[2].data_ptr(), n)], False, s)
+torch.cuda.synchronize()
+assert dg == dg2 and torch.equal(reps[0], reps[2]) and torch.equal(reps[1], reps[2])
+print(f"sanitize target OK: {checked} kernel configurations + mxfp8 + gathered mxfp8 put")

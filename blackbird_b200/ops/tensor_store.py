@@ -72,12 +72,16 @@ class TensorStore:
     def batch_put(self, keys: Sequence[str], tensors: Sequence[torch.Tensor], pack_fp8: bool = False, config=None) -> None:
         """Stores each tensor under its key.  A slice of a larger CUDA tensor whose elements are rows -- `W[:, a:b]`, `kv[:,
         :, h0:h1, :]`, `t[::k]` -- is read in place by the fused put kernel (batch_put_device_strided) when its start is
-        16-byte aligned and its row gap a multiple of 16 bytes; no contiguous copy is made.  Other layouts, and every tensor
-        with pack_fp8, are made contiguous first.  The stored object is that of `t.contiguous()` either way."""
+        16-byte aligned and its row gap a multiple of 16 bytes; no contiguous copy is made.  With pack_fp8 such a bf16
+        slice whose element count is a whole number of 32-element MX blocks is gathered the same way by the fused pack
+        kernel (batch_put_device_fp8_strided) when the config is fusable.  Other layouts are made contiguous first.  The
+        stored object is that of `t.contiguous()` either way."""
         cfg = config or self.config
         keys = list(keys)
         tensors = list(tensors)
-        rows = [None if pack_fp8 else self._gatherable(t) for t in tensors]
+        rows = [self._gatherable(t) for t in tensors]
+        if pack_fp8:  # only slices the fused pack kernel can take are gathered
+            rows = [r if r is not None and self._fused_fp8_ok(t, cfg) else None for t, r in zip(tensors, rows)]
         tensors = [t if r is not None else t.contiguous() for t, r in zip(tensors, rows)]
         if pack_fp8:
             # objects the fused kernel can take go through batch_put_device_fp8 (bf16 read once, packed bytes on the
@@ -85,8 +89,15 @@ class TensorStore:
             fused = [i for i, t in enumerate(tensors) if t.is_cuda and self._fused_fp8_ok(t, cfg)]
             if fused:
                 fk = [keys[i] for i in fused]
-                ecs = self.client.batch_put_device_fp8(fk, [tensors[i].data_ptr() for i in fused], [tensors[i].numel() for i in fused],
-                                                       cfg, self._stream())
+                ptrs = [tensors[i].data_ptr() for i in fused]
+                if any(rows[i] is not None for i in fused):
+                    # one call and one launch: contiguous tensors go as one row each; widths and pitches in elements
+                    shapes = [(rows[i][0] // 2, rows[i][1] // 2, rows[i][2]) if rows[i] is not None else (tensors[i].numel(),) * 2 + (1,)
+                              for i in fused]
+                    ecs = self.client.batch_put_device_fp8_strided(fk, ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
+                                                                   [s[2] for s in shapes], cfg, self._stream())
+                else:
+                    ecs = self.client.batch_put_device_fp8(fk, ptrs, [tensors[i].numel() for i in fused], cfg, self._stream())
                 done = [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.OK]
                 bad = [(keys[i], e) for i, e in zip(fused, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
                 if bad:
@@ -101,7 +112,10 @@ class TensorStore:
                     if any(e != _bb.ErrorCode.OK for e in ecs):
                         raise RuntimeError("meta put failed")
                 rest = [i for i in range(len(keys)) if i not in set(done)]
-                keys, tensors = [keys[i] for i in rest], [tensors[i] for i in rest]
+                # a gathered slice the fused put refused (its placement is not one GPU-fabric shard per copy) is made
+                # contiguous and packed first, like any other
+                keys, tensors = [keys[i] for i in rest], [tensors[i].contiguous() for i in rest]
+                rows = [None] * len(keys)
                 if not keys:
                     return
         payloads, metas, keep = [], [], []

@@ -603,10 +603,58 @@ ErrorCode BlackbirdClient::remove(const ObjectKey& key) {
 // ================================================================ fused MXFP8 device API
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                              const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream) {
+  return put_device_fp8(keys, bf16_ptrs, n_elems, nullptr, cfg, stream);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
+                                                                     const std::vector<uint64_t>& elem_widths,
+                                                                     const std::vector<uint64_t>& elem_pitches,
+                                                                     const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
+  const size_t n = keys.size();
+  if (bf16_ptrs.size() != n || elem_widths.size() != n || elem_pitches.size() != n || rows.size() != n)
+    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  // invalid and unfusable items fail here, before the Keystone allocates anything for them; the others are one batch
+  std::vector<ErrorCode> out(n, ErrorCode::OK);
+  std::vector<size_t> idx;
+  std::vector<ObjectKey> k;
+  std::vector<const void*> p;
+  std::vector<uint64_t> elems;
+  std::vector<SourceRows> pats;
+  for (size_t i = 0; i < n; ++i) {
+    SourceRows pat, bytes;
+    uint64_t size = 0, extent = 0;
+    out[i] = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pat, &size, &extent);
+    if (out[i] != ErrorCode::OK) continue;
+    if (extent > UINT64_MAX / 2 || !pat.to_bf16_bytes(&bytes)) {
+      out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
+      continue;
+    }
+    // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
+    if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 2 * size)) {
+      out[i] = ErrorCode::NOT_IMPLEMENTED;
+      continue;
+    }
+    idx.push_back(i), k.push_back(keys[i]), p.push_back(bf16_ptrs[i]), elems.push_back(size), pats.push_back(pat);
+  }
+  if (idx.empty()) return out;
+  const auto ecs = put_device_fp8(k, p, elems, &pats, cfg, stream);
+  uint64_t done = 0, bf16_bytes = 0;
+  for (size_t j = 0; j < idx.size(); ++j) {
+    out[idx[j]] = ecs[j];
+    if (ecs[j] == ErrorCode::OK) ++done, bf16_bytes += 2 * elems[j];
+  }
+  metrics_.inc("device_put_fp8_strided_total", done);
+  metrics_.inc("device_put_fp8_strided_bytes_total", bf16_bytes);
+  return out;
+}
+
+std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
+                                                       const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows,
+                                                       const WorkerConfig& cfg, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size()) return out;
+  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (rows && rows->size() != keys.size())) return out;
   BB_TRACE_SPAN("batch_put_device_fp8", keys.size());
   WorkerConfig c = cfg;
   c.replication_factor = std::max<size_t>(1, std::min<size_t>(cfg.replication_factor, 3));  // one tile pass fans out to <= 3 copies
@@ -636,6 +684,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8(const std::vector<O
       continue;
     }
     DeviceFp8Op op{&copies[0].shards[0], const_cast<void*>(bf16_ptrs[i]), n_elems[i], {}};
+    if (rows) op.rows = (*rows)[i];
     for (size_t cidx = 1; cidx < copies.size(); ++cidx) op.replicas.push_back(&copies[cidx].shards[0]);
     ops.push_back(std::move(op));
     idx.push_back(i);
@@ -1655,8 +1704,18 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
   if (digests) digests->assign(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
+    const auto* src = static_cast<const uint16_t*>(op.wide);
+    std::vector<uint16_t> dense;
+    if (op.rows.strided()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows
+      SourceRows b;
+      if (!op.rows.valid() || !op.rows.to_bf16_bytes(&b)) return ErrorCode::INVALID_ARGUMENT;
+      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), 2 * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      dense.resize(op.n_elems);
+      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, src + at, 2 * n); });
+      src = dense.data();
+    }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
-    mxfp8::pack_bf16(static_cast<const uint16_t*>(op.wide), op.n_elems, packed.data());
+    mxfp8::pack_bf16(src, op.n_elems, packed.data());
     uint64_t d = 0;
     ErrorCode ec = io_->write_shard(*op.placement, packed.data(), &d, ChecksumAlgo::BBH64);
     for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], packed.data(), nullptr, ChecksumAlgo::NONE);

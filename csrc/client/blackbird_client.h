@@ -80,6 +80,9 @@ struct DeviceFp8Op {
   // Get: the elements that are stored (common/store_window.h); the whole packed object is still read and verified.  The
   // default is the whole object.
   StoreWindow win;
+  // Put: the source rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts.  The packed
+  // object is one shard, so the pattern is the object's own.  The default is a contiguous source.
+  SourceRows rows;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -141,6 +144,19 @@ class BlackbirdClient {
   // shard per object.  The stored object is identical to packing first and putting the packed bytes.
   std::vector<ErrorCode> batch_put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                               const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream);
+  // Packed puts of sliced bf16 tensors (`kv[:, h0:h1, :]`, `W[:, k0:k1]`, `t[::k]`): object i holds the rows[i] *
+  // elem_widths[i] elements of rows[i] rows of elem_widths[i] elements, row r read from bf16_ptrs[i] + 2 * r *
+  // elem_pitches[i] (SourceRows in common/store_window.h, in elements).  The put kernel gathers the rows while it packs, so
+  // no contiguous copy is made; the stored packed object and its digest are byte for byte those of batch_put_device_fp8
+  // of the compacted rows, so every fp8 get reads it.  Placement, replica fan-out and errors are batch_put_device_fp8's.
+  // Per object, before anything is allocated: INVALID_ARGUMENT for elem_widths[i] > elem_pitches[i] with rows[i] > 1;
+  // VALUE_OUT_OF_RANGE when the element count or the source extent overflows; NOT_IMPLEMENTED unless bf16_ptrs[i] is
+  // 16-byte aligned and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is no host-staged path;
+  // the rest of the batch keeps its single launch.  rows[i] == 1 or elem_widths[i] == elem_pitches[i] is exactly
+  // batch_put_device_fp8 of one contiguous tensor.
+  std::vector<ErrorCode> batch_put_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
+                                                      const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
+                                                      const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                               const std::vector<uint64_t>& n_elems, void* stream);
   // Element-range gets of packed tensors: elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of the n_elems[i]-element
@@ -250,6 +266,11 @@ class BlackbirdClient {
                                     const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
+  // batch_put_device_fp8 and batch_put_device_fp8_strided: `rows` null = contiguous tensors, else object i is read by
+  // (*rows)[i], in elements.
+  std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
+                                        const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows, const WorkerConfig& cfg,
+                                        void* stream);
   // batch_get_device_fp8, batch_get_device_fp8_range and batch_get_device_fp8_strided: `ranges` null = whole tensors, else
   // object i's rows (offset, length and pitch in elements) into bf16_ptrs[i].
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,

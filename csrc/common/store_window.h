@@ -132,8 +132,9 @@ struct StoreWindow {
 // SourceRows: where a device put reads each byte of an object from, when the source is rows of `width` bytes every `pitch`
 // bytes (a slice of a larger tensor).  It is the inverse of a strided StoreWindow, which maps a strided object onto a dense
 // destination: here the object is dense and the source strided.  This is the one statement of the rule; the transfer
-// engine (XferItem), the fabric's DeviceShardOp, the client, the host loopback transport and the kernel's XFER_GATHER
-// descriptors (kernels/xfer.h) all follow it.
+// engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and
+// the kernels' XFER_GATHER descriptors (kernels/xfer.h) all follow it.  The unit is a byte, or for an MXFP8 put an element
+// of the bf16 source (to_bf16_bytes() turns elements into bf16 bytes).
 //
 // With `src` where the pattern's row 0 starts, object byte x is read from
 //   src + ((x + phase) / width) * pitch + (x + phase) % width
@@ -145,6 +146,14 @@ struct SourceRows {
   bool strided() const { return pitch != 0; }
   // 0 < width <= pitch and phase < width for a pattern.
   bool valid() const { return !strided() || (width != 0 && width <= pitch && phase < width); }
+
+  // The source rows of an MXFP8 put, given in elements, in bf16 bytes of the source.  False for a pitch of 2^62 elements or
+  // more, whose byte arithmetic could overflow (as StoreWindow::to_bf16_bytes).
+  bool to_bf16_bytes(SourceRows* out) const {
+    if (pitch > (UINT64_MAX >> 2)) return false;
+    *out = {2 * pitch, 2 * width, 2 * phase};
+    return true;
+  }
 
   // The source of `rows` rows of `width` bytes every `pitch` bytes: an object of *size = rows * width bytes spread over
   // *extent = (rows - 1) * pitch + width source bytes.  INVALID_ARGUMENT for several rows wider than the pitch;

@@ -641,7 +641,8 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.wide = op.wide;
     it.packed = d.value();
     it.n_elems = op.n_elems;
-    it.win = op.win;  // a window on a put is refused by the engine
+    it.win = op.win;    // a window on a put is refused by the engine
+    it.rows = op.rows;  // and source rows on a get
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;

@@ -570,10 +570,15 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
+    const bool gather = it.rows.strided();
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
-    // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window): the rows are
-    // checked below instead
-    if (((strided ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15) return ErrorCode::INVALID_ADDRESS;
+    SourceRows rows;  // a gathered put's source rows in bf16 bytes
+    if (gather && (unpack || !it.rows.valid() || !it.rows.to_bf16_bytes(&rows))) return ErrorCode::INVALID_ARGUMENT;
+    // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
+    // first element after row 0's start): the rows are checked instead
+    if (((strided || gather ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
+        (gather && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), 2 * it.n_elems)))
+      return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
     // a put stores the whole object; from here on the window is in bf16 bytes
@@ -603,6 +608,10 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       d.win.base = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(it.wide) + w.origin());
       d.flags |= XFER_STRIDED;
       s->set_stride(i, w);
+    }
+    if (gather) {  // d.src is the pattern's row 0
+      d.flags |= XFER_GATHER;
+      s->set_stride(i, XferStride{rows.pitch, rows.width, rows.phase});
     }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice

@@ -58,6 +58,11 @@ struct Fp8Item {
   // the whole object.  The whole packed object is still read and verified.  INVALID_ARGUMENT unless valid against
   // n_elems; INVALID_ADDRESS unless a strided window is co-aligned in bf16 bytes, as XferItem's.
   StoreWindow win;
+  // Put only: the source rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts; the
+  // default is a contiguous source.  run_fp8 sets XFER_GATHER exactly when it has a pattern.  INVALID_ARGUMENT for a
+  // pattern on an unpack, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned
+  // in bf16 bytes, which replaces the 16-byte alignment check of `wide`.
+  SourceRows rows;
 };
 
 struct XferResult {

@@ -29,9 +29,10 @@ enum XferFlags : uint32_t {
   // land densely from there.  The pattern is the descriptor's entry of the launch's XferStride table; the MXFP8 get
   // counts all of it in bf16 bytes of the unpacked object.
   XFER_STRIDED = 1u << 4,
-  // Gathering load (puts of a strided source), in bb_xfer only: the rule of SourceRows (common/store_window.h), so `src` is
-  // where the pattern's row 0 starts and object byte x is read from src + ((x + phase) / width) * pitch + (x + phase) % width.
-  // The pattern is the descriptor's entry of the launch's XferStride table.  Never with XFER_WINDOW, XFER_STRIDED or
+  // Gathering load (puts of a strided source), in bb_xfer and the fused MXFP8 put: the rule of SourceRows
+  // (common/store_window.h), so `src` is where the pattern's row 0 starts and object byte x is read from
+  // src + ((x + phase) / width) * pitch + (x + phase) % width.  The pattern is the descriptor's entry of the launch's
+  // XferStride table; the MXFP8 put counts all of it in bf16 bytes of the source.  Never with XFER_WINDOW, XFER_STRIDED or
   // XFER_RAW_SUM; with 1-3 destinations or XFER_MULTIMEM.  The tile in shared memory is byte for byte the tile of the
   // dense object, so the digest and the stored bytes are those of a put of the compacted rows.
   XFER_GATHER = 1u << 5,

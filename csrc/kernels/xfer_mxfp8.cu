@@ -6,6 +6,9 @@
 //                   bb_xfer) -> TMA stores payload + 512 B of scales to the
 //                   (peer) slab -- to up to 3 replicas of the object from the one converted tile.  The bf16 data
 //                   is read from HBM once and only the 0.52x packed bytes cross NVLink (once per replica).
+//                   With XFER_GATHER (puts of a sliced tensor) the producer fills the bf16 tile from the source rows,
+//                   one row segment per lane, by the rule of SourceRows (common/store_window.h) in bf16 bytes, so the
+//                   tile, the packed object and its digest are those of a put of the compacted rows.
 //   get  (UNPACK) : TMA loads payload tile + scales from the slab -> tensor-core hash of the payload tile ->
 //                   8 unpack warps expand to bf16 in shared memory -> TMA stores the 32 KiB tile to the caller.
 //                   With XFER_WINDOW (element-range gets) only the bf16 bytes [win.lo, win.hi) of the object are
@@ -59,7 +62,8 @@ struct FpMeta {            // 64 bytes
   uint32_t obj_ntiles;
   uint32_t ndst;           // pack: replicas written by this pass (1..kMaxDst)
   uint32_t valid;          // payload bytes (= elements) of this tile: 16384, or the multiple-of-32 tail of the object
-  uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided (FpParams::strides); pack: 0
+  uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided; pack: XFER_GATHER when its
+                           // source is rows (the pattern in FpParams::strides either way)
   uint64_t pad;
 };
 static_assert(sizeof(FpMeta) == 64);
@@ -95,7 +99,8 @@ struct FpParams {
   uint32_t ndesc;
   uint32_t total_tiles;
   unsigned long long* sum_ws;  // [ndesc] raw BBH64 sums of the payload tiles (zero on entry)
-  const XferStride* strides;   // unpack: row patterns of the XFER_STRIDED descriptors (XferLaunch::strides), else null
+  const XferStride* strides;   // row patterns of the XFER_STRIDED (unpack) or XFER_GATHER (pack) descriptors
+                               // (XferLaunch::strides), else null
 };
 
 template <bool UNPACK>
@@ -126,6 +131,8 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
   if (warp == 0) {
     // ================================================================ TMA producer
     uint32_t it = 0;
+    uint32_t g_desc = 0xFFFFFFFFu;  // pack: descriptor whose source rows are in `gst`
+    XferStride gst{1, 1, 0};
     for (uint32_t base = 0; base < my_tiles; base += 32) {
       const uint32_t idx = base + lane;
       if (idx < my_tiles) {
@@ -143,7 +150,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = UNPACK ? d.flags & XFER_STRIDED : 0u;
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED : XFER_GATHER);
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
         // the packed object is [payload nbytes][scales nbytes/32]: a tile's scales sit (nbytes - ti*(16384-512)) past its payload
@@ -158,7 +165,8 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           e.m.dst[2] = win ? d2 : ~0ull;
           e.m.ndst = 1;
         } else {
-          e.src = src + static_cast<uint64_t>(ti) * kWideBytes;  // bf16 source tile
+          // bf16 source tile; for a gathering load the pattern's row 0 (the tile's rows are found from its object offset)
+          e.src = e.m.strided ? src : src + static_cast<uint64_t>(ti) * kWideBytes;
           e.src_scales = 0;
           e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kTileBytes;
           e.m.dst[1] = d1 + static_cast<uint64_t>(ti) * kTileBytes;
@@ -188,10 +196,26 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           const uint32_t ws = it % kWideStages, wp = (it / kWideStages) & 1u;
           mbar_wait(&s.w_empty[ws], wp ^ 1u);
           if (lane < 4) reinterpret_cast<uint4*>(&s.w_meta[ws])[lane] = reinterpret_cast<const uint4*>(&e.m)[lane];
+          uint32_t tx = 2u * e.m.valid;  // bytes the stage's bulk loads deliver
+          if (e.m.strided) {
+            // Gathering load (XFER_GATHER): one source row segment per lane, so the wide tile is byte for byte the tile of
+            // the compacted rows.  A short last tile needs no zero pad: only its `valid` elements are stored, and it is
+            // not hashed here.  The lanes' head and tail bytes are generic shared stores read only by the convert warps'
+            // generic loads (no TMA store or wgmma reads the wide tile), so no async-proxy fence: the __syncwarp below
+            // orders them before lane 0's arrive (release), and the convert warps' wait on w_full (acquire) orders that
+            // before their loads.
+            if (e.m.desc != g_desc) {
+              g_desc = e.m.desc;
+              gst = load_stride(p.strides, g_desc);
+            }
+            tx = __reduce_add_sync(0xffffffffu, gather_row_segments(s.wide[ws], &s.w_full[ws], e.src,
+                                                                     static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes,
+                                                                     2u * e.m.valid, gst, lane));
+          }
           __syncwarp();
           if (lane == 0) {
-            mbar_arrive_expect_tx(&s.w_full[ws], 2u * e.m.valid);
-            bulk_g2s(s.wide[ws], reinterpret_cast<const void*>(e.src), 2u * e.m.valid, &s.w_full[ws]);
+            mbar_arrive_expect_tx(&s.w_full[ws], tx);
+            if (!e.m.strided) bulk_g2s(s.wide[ws], reinterpret_cast<const void*>(e.src), 2u * e.m.valid, &s.w_full[ws]);
           }
         }
         __syncwarp();

@@ -1172,6 +1172,19 @@ void bind_control(py::module_& m) {
              return c.batch_put_device_fp8(keys, p, n_elems, cfg, reinterpret_cast<void*>(stream));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("config"), py::arg("stream") = 0)
+      .def("batch_put_device_fp8_strided",
+           [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& widths,
+              const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream) {
+             std::vector<const void*> p;
+             for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
+             py::gil_scoped_release rel;
+             return c.batch_put_device_fp8_strided(keys, p, widths, pitches, rows, cfg, reinterpret_cast<void*>(stream));
+           },
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("elem_widths"), py::arg("elem_pitches"), py::arg("rows"), py::arg("config"),
+           py::arg("stream") = 0,
+           "Packed tensor i = rows[i] rows of elem_widths[i] bf16 elements, row r read from bf16_ptrs[i] + 2 * r * "
+           "elem_pitches[i]; packed in the put kernel and stored as batch_put_device_fp8 of the compacted rows would store it; "
+           "returns one ErrorCode per object (NOT_IMPLEMENTED: make it contiguous and put that).")
       .def("batch_get_device_fp8",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               uintptr_t stream) {

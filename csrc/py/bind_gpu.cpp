@@ -127,8 +127,15 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() > 3) it.expect = t[3].cast<uint64_t>(), it.verify = true;
+               if (t.size() < 3 || t.size() > 6)
+                 throw py::value_error("fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, (pitch, width, phase)]]])");
+               if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
+               if (t.size() > 5 && !t[5].is_none()) {
+                 auto g = t[5].cast<std::vector<uint64_t>>();
+                 if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
+                 it.rows = {g[0], g[1], g[2]};
+               }
                v.push_back(it);
              }
              XferResult res;
@@ -147,8 +154,13 @@ void bind_gpu(py::module_& m) {
            "elements, is strided: of [lo, hi), element x is stored iff c = (x + phase) % pitch < width, at bf16_ptr + 2 * "
            "((x + phase) // pitch * width + c); INVALID_ARGUMENT for width == 0, width > pitch or phase >= pitch, "
            "INVALID_ADDRESS unless every row the window touches is co-aligned in bf16 bytes (the address of its first "
-           "element congruent to twice that element's index mod 16).  Returns (digests of the packed objects, status, "
-           "device_ms).")
+           "element congruent to twice that element's index mod 16).  A put's gather pattern (pitch, width, phase), in "
+           "elements, as the sixth element (expected_digest and window may be None) reads the bf16 source in rows: element x "
+           "is read from bf16_ptr + 2 * ((x + phase) // width * pitch + (x + phase) % width), bf16_ptr being where the "
+           "pattern's row 0 starts, and the packed object and its digest are those of the compacted rows; INVALID_ARGUMENT "
+           "for a pattern on a get, width == 0, width > pitch, phase >= width or pitch >= 2^62, INVALID_ADDRESS unless "
+           "bf16_ptr + 2 * phase is 16-byte aligned and, when the object spans more than one row, (pitch - width) % 8 == 0.  "
+           "Returns (digests of the packed objects, status, device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
