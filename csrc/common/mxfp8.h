@@ -6,6 +6,9 @@
 //   shared_exp(block) = floor(log2(amax(block))) - 8        (8 = emax of E4M3: 448 = 1.75 * 2^8)
 //   E8M0 byte         = clamp(shared_exp + 127, 0, 254);  all-zero block -> 127 (scale 1)
 //   element           = sat_e4m3( x * 2^-shared_exp ), round-to-nearest-even
+// The pack never emits E8M0 0xFF (a finite bf16 block gives at most 246).  Given one, the unpacks (this one and the
+// device codec, kernels/mxfp8.cuh) read it as 2^128, which overflows fp32: +-Inf, and NaN for a zero payload, not the
+// OCP NaN scale.  tests/test_mxfp8_exhaustive.py checks every (payload, scale) pair against an exact model of this rule.
 #pragma once
 #include <cstddef>
 #include <cstdint>

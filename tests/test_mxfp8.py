@@ -67,10 +67,10 @@ def special_blocks(rows=slice(None)):
 
 
 def check_packed(got, ref, n, what=""):
-    """Stored MXFP8 object (numpy uint8) vs mxfp8_pack_ref: block scales identical, payload identical up to the sign of a
-    zero."""
+    """Stored MXFP8 object (numpy uint8) vs mxfp8_pack_ref: block scales and payload identical, the sign of a zero
+    included (a negative element that rounds to zero is stored as -0, 0x80)."""
     assert np.array_equal(got[n:], ref[n:]), f"{what}: block scales differ at {np.nonzero(got[n:] != ref[n:])[0][:10]}"
-    diff = (got[:n] != ref[:n]) & ~(((got[:n] & 0x7F) == 0) & ((ref[:n] & 0x7F) == 0))
+    diff = got[:n] != ref[:n]
     assert not diff.any(), f"{what}: payload differs at {np.nonzero(diff)[0][:10]}"
 
 
