@@ -600,6 +600,73 @@ ErrorCode BlackbirdClient::remove(const ObjectKey& key) {
   return keystone_->remove_object(key);
 }
 
+// ================================================================ shared by the device calls
+template <class T>
+static std::vector<T> pick(const std::vector<T>& v, const std::vector<size_t>& idx) {
+  std::vector<T> out;
+  out.reserve(idx.size());
+  for (size_t i : idx) out.push_back(v[i]);
+  return out;
+}
+
+// The shaped calls (strided puts; range and strided gets; bytes and MXFP8) over put_device, put_device_fp8, get_device and
+// get_device_fp8.  Unless `arity_ok`, every item is INVALID_PARAMETERS (CLIENT_DISCONNECTED without a Keystone).  Then
+// shape(i, &bytes) records item i's shape and returns its error.  For a put (`admit`) an item with an error fails here,
+// before the Keystone allocates anything for it, and run(idx) puts the others as one batch, or nothing runs when there
+// are none.  A get refuses no item here (the Keystone's answer comes first), and run(idx) gets them all, an empty batch
+// included.  <name>_total and <name>_bytes_total count the OK items and their `bytes`.
+template <class Shape, class Run>
+std::vector<ErrorCode> BlackbirdClient::shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run) {
+  if (!arity_ok) return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
+  std::vector<ErrorCode> out(n, ErrorCode::OK);
+  std::vector<uint64_t> bytes(n, 0);
+  std::vector<size_t> idx;
+  idx.reserve(n);
+  for (size_t i = 0; i < n; ++i) {
+    out[i] = shape(i, &bytes[i]);
+    if (out[i] == ErrorCode::OK) idx.push_back(i);
+  }
+  if (admit && idx.empty()) return out;
+  const std::vector<ErrorCode> ecs = run(idx);
+  uint64_t done = 0, total = 0;
+  for (size_t j = 0; j < idx.size(); ++j) {
+    out[idx[j]] = ecs[j];
+    if (ecs[j] == ErrorCode::OK) ++done, total += bytes[idx[j]];
+  }
+  metrics_.inc(std::string(name) + "_total", done);
+  metrics_.inc(std::string(name) + "_bytes_total", total);
+  return out;
+}
+
+// A digest mismatch on every replica can also mean that the Keystone moved the object under us (tier move, compaction,
+// repair): the extents we read were freed and re-used.  Items whose placements changed since we fetched them get one
+// more pass, reissue(idx) being the same get of items idx; so do unchanged ones once, at the outermost call, because a
+// remove + re-put can land on the very same extent (first fit) and be read half-written.  Passes nest at most twice.
+static thread_local int refresh_depth = 0;
+
+template <class Reissue>
+void BlackbirdClient::refresh_placements(const std::vector<ObjectKey>& keys, const std::vector<Result<std::vector<CopyPlacement>>>& placed,
+                                         std::vector<ErrorCode>& out, Reissue&& reissue) {
+  if (refresh_depth >= 2) return;
+  std::vector<size_t> bad;
+  for (size_t i = 0; i < keys.size(); ++i)
+    if (out[i] == ErrorCode::CHECKSUM_MISMATCH && placed[i].ok()) bad.push_back(i);
+  if (bad.empty()) return;
+  const auto again = keystone_->batch_get_workers(pick(keys, bad));
+  std::vector<size_t> redo;
+  for (size_t k = 0; k < bad.size(); ++k) {
+    const size_t i = bad[k];
+    if (!again[k].ok()) out[i] = again[k].error();  // removed (or being re-written) meanwhile: that is the answer
+    else if (!(again[k].value() == placed[i].value()) || refresh_depth == 0) redo.push_back(i);
+  }
+  if (redo.empty()) return;
+  metrics_.inc("get_placement_refresh_total", redo.size());
+  ++refresh_depth;
+  const std::vector<ErrorCode> recs = reissue(redo);
+  --refresh_depth;
+  for (size_t k = 0; k < redo.size(); ++k) out[redo[k]] = recs[k];
+}
+
 // ================================================================ fused MXFP8 device API
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                              const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream) {
@@ -611,41 +678,25 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::
                                                                      const std::vector<uint64_t>& elem_pitches,
                                                                      const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
-  if (bf16_ptrs.size() != n || elem_widths.size() != n || elem_pitches.size() != n || rows.size() != n)
-    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
-  // invalid and unfusable items fail here, before the Keystone allocates anything for them; the others are one batch
-  std::vector<ErrorCode> out(n, ErrorCode::OK);
-  std::vector<size_t> idx;
-  std::vector<ObjectKey> k;
-  std::vector<const void*> p;
-  std::vector<uint64_t> elems;
-  std::vector<SourceRows> pats;
-  for (size_t i = 0; i < n; ++i) {
-    SourceRows pat, bytes;
-    uint64_t size = 0, extent = 0;
-    out[i] = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pat, &size, &extent);
-    if (out[i] != ErrorCode::OK) continue;
-    if (extent > UINT64_MAX / 2 || !pat.to_bf16_bytes(&bytes)) {
-      out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
-      continue;
-    }
-    // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
-    if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 2 * size)) {
-      out[i] = ErrorCode::NOT_IMPLEMENTED;
-      continue;
-    }
-    idx.push_back(i), k.push_back(keys[i]), p.push_back(bf16_ptrs[i]), elems.push_back(size), pats.push_back(pat);
-  }
-  if (idx.empty()) return out;
-  const auto ecs = put_device_fp8(k, p, elems, &pats, cfg, stream);
-  uint64_t done = 0, bf16_bytes = 0;
-  for (size_t j = 0; j < idx.size(); ++j) {
-    out[idx[j]] = ecs[j];
-    if (ecs[j] == ErrorCode::OK) ++done, bf16_bytes += 2 * elems[j];
-  }
-  metrics_.inc("device_put_fp8_strided_total", done);
-  metrics_.inc("device_put_fp8_strided_bytes_total", bf16_bytes);
-  return out;
+  std::vector<uint64_t> elems(n);
+  std::vector<SourceRows> pats(n);
+  return shaped_batch(
+      "device_put_fp8_strided", true, n, bf16_ptrs.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* bf16_bytes) {
+        SourceRows bytes;
+        uint64_t extent = 0;
+        const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems[i], &extent);
+        *bf16_bytes = 2 * elems[i];
+        if (ec != ErrorCode::OK) return ec;
+        if (extent > UINT64_MAX / 2 || !pats[i].to_bf16_bytes(&bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
+        if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 2 * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &p, cfg, stream);
+      });
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
@@ -720,17 +771,16 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<O
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                                    const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
                                                                    const std::vector<uint64_t>& elem_counts, void* stream) {
-  if (elem_offsets.size() != keys.size() || elem_counts.size() != keys.size())
-    return std::vector<ErrorCode>(keys.size(), keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
-  std::vector<ByteRange> ranges(keys.size());
-  for (size_t i = 0; i < keys.size(); ++i) ranges[i] = {elem_offsets[i], elem_counts[i]};
-  auto out = get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream);
-  uint64_t n = 0, bytes = 0;
-  for (size_t i = 0; i < out.size(); ++i)
-    if (out[i] == ErrorCode::OK) ++n, bytes += 2 * elem_counts[i];
-  metrics_.inc("device_get_fp8_range_total", n);
-  metrics_.inc("device_get_fp8_range_bytes_total", bytes);
-  return out;
+  const size_t n = keys.size();
+  std::vector<ByteRange> ranges(n);
+  return shaped_batch(
+      "device_get_fp8_range", false, n, elem_offsets.size() == n && elem_counts.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {elem_offsets[i], elem_counts[i]};
+        *bytes = 2 * elem_counts[i];
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -738,17 +788,15 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
                                                                      const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
                                                                      const std::vector<uint64_t>& rows, void* stream) {
   const size_t n = keys.size();
-  if (elem_offsets.size() != n || elem_widths.size() != n || elem_pitches.size() != n || rows.size() != n)
-    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
   std::vector<ByteRange> ranges(n);
-  for (size_t i = 0; i < n; ++i) ranges[i] = {elem_offsets[i], elem_widths[i], elem_pitches[i], rows[i]};
-  auto out = get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream);
-  uint64_t k = 0, bytes = 0;
-  for (size_t i = 0; i < n; ++i)
-    if (out[i] == ErrorCode::OK) ++k, bytes += 2 * rows[i] * elem_widths[i];  // an OK item's rows lie inside the object
-  metrics_.inc("device_get_fp8_strided_total", k);
-  metrics_.inc("device_get_fp8_strided_bytes_total", bytes);
-  return out;
+  return shaped_batch(
+      "device_get_fp8_strided", false, n, elem_offsets.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {elem_offsets[i], elem_widths[i], elem_pitches[i], rows[i]};
+        *bytes = 2 * rows[i] * elem_widths[i];  // counted for OK items only, whose rows lie inside the object
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -798,10 +846,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       out[i] = ErrorCode::NOT_IMPLEMENTED;  // demoted to a host tier, striped, other digest: caller gets + unpacks instead
       continue;
     }
-    // a range whose virtual base `ptr - 2 * lo` the kernel cannot store from (TMA needs 16 bytes) fails alone, so that the
-    // rest of the batch still takes the fused launch; the caller reads it whole and slices instead.  Rows with gaps are
-    // co-aligned only when the gap is a whole number of 16-byte units (StoreWindow::coaligned).
-    if (ranges && (((reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * w.lo) & 15) || (w.strided() && (w.pitch - w.width) % 8))) {
+    // a range the kernel cannot store (StoreWindow::fused_get_aligned) fails alone, so that the rest of the batch still
+    // takes the fused launch; the caller reads it whole and slices instead.  A whole tensor is left to the engine.
+    StoreWindow bytes;
+    if (ranges && (!w.to_bf16_bytes(&bytes) || !bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, 2 * n_elems[i]))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
@@ -832,42 +880,11 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       else out[cur[k]] = ErrorCode::OK;
     }
   }
-  // Same rule as batch_get_device: a digest mismatch on every replica can mean the object was moved under us (tier
-  // move, compaction, repair).  Keys whose placements changed since we read them get one more pass; a key that moved
-  // to a non-fusable placement comes back NOT_IMPLEMENTED from that pass, i.e. "get + unpack instead".
-  static thread_local int fp8_refresh_depth = 0;
-  if (fp8_refresh_depth < 2) {
-    std::vector<size_t> bad;
-    for (size_t i = 0; i < keys.size(); ++i)
-      if (out[i] == ErrorCode::CHECKSUM_MISMATCH && placed[i].ok()) bad.push_back(i);
-    if (!bad.empty()) {
-      std::vector<ObjectKey> bkeys;
-      for (size_t i : bad) bkeys.push_back(keys[i]);
-      auto again = keystone_->batch_get_workers(bkeys);
-      std::vector<ObjectKey> rkeys;
-      std::vector<void*> rptrs;
-      std::vector<uint64_t> rn;
-      std::vector<size_t> ridx;
-      std::vector<ByteRange> rranges;
-      for (size_t k = 0; k < bad.size(); ++k) {
-        const size_t i = bad[k];
-        if (!again[k].ok()) {
-          out[i] = again[k].error();
-        } else if (!(again[k].value() == placed[i].value()) || fp8_refresh_depth == 0) {
-          // changed placements, or (once) the same ones: a remove + re-put can land on the very same extent and be read half-written
-          rkeys.push_back(keys[i]), rptrs.push_back(bf16_ptrs[i]), rn.push_back(n_elems[i]), ridx.push_back(i);
-          if (ranges) rranges.push_back((*ranges)[i]);
-        }
-      }
-      if (!rkeys.empty()) {
-        metrics_.inc("get_placement_refresh_total", rkeys.size());
-        ++fp8_refresh_depth;
-        auto recs = get_device_fp8(rkeys, rptrs, rn, ranges ? &rranges : nullptr, stream);  // the same ranges again
-        --fp8_refresh_depth;
-        for (size_t k = 0; k < ridx.size(); ++k) out[ridx[k]] = recs[k];
-      }
-    }
-  }
+  // a key that moved to a non-fusable placement comes back NOT_IMPLEMENTED from the refresh, i.e. "get + unpack instead"
+  refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
+    const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
+    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, stream);
+  });
   metrics_.inc("device_get_fp8_batches_total");
   return out;
 }
@@ -1007,15 +1024,15 @@ static void ewma_update(std::atomic<double>& v, double sample) {
 }
 
 // The fused kernels move 16-byte aligned buffers only (XferEngine::submit refuses a whole batch otherwise).  An object
-// whose caller buffer is not 16-byte aligned where one of its shards starts -- for a strided source, whose shards are not
-// co-aligned -- is staged through host memory instead, so that it does not fail its neighbours.
-static bool fabric_aligned(const void* ptr, const SourceRows& rows, const std::vector<CopyPlacement>& copies) {
-  const auto base = reinterpret_cast<uintptr_t>(ptr);
+// whose caller buffer is not aligned with one of its shards is staged through host memory instead, so that it does not
+// fail its neighbours: a put's source where every shard starts (for a strided source, every shard co-aligned), a get's
+// destination by StoreWindow::fused_get_aligned.  Whether ok(off, len) holds for the shard [off, off + len) of every copy.
+template <class F>
+static bool fabric_aligned(const std::vector<CopyPlacement>& copies, F&& ok) {
   for (const auto& c : copies) {
     uint64_t off = 0;
     for (const auto& sh : c.shards) {
-      uint64_t at = 0;
-      if (!rows.rebase(off, &at).coaligned(base + at, sh.length)) return false;
+      if (!ok(off, sh.length)) return false;
       off += sh.length;
     }
   }
@@ -1031,35 +1048,22 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vect
                                                                  const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                                  const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
-  if (dev_ptrs.size() != n || widths.size() != n || pitches.size() != n || rows.size() != n)
-    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
-  // invalid items fail here, before the Keystone allocates anything for them; the others are one batch
-  std::vector<ErrorCode> out(n, ErrorCode::OK);
-  std::vector<size_t> idx, sizes;
-  std::vector<ObjectKey> k;
-  std::vector<const void*> p;
-  std::vector<SourceRows> pats;
-  for (size_t i = 0; i < n; ++i) {
-    SourceRows pat;
-    uint64_t size = 0, extent = 0;
-    out[i] = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pat, &size, &extent);
-    if (out[i] != ErrorCode::OK) continue;
-    if (size > SIZE_MAX) {
-      out[i] = ErrorCode::VALUE_OUT_OF_RANGE;
-      continue;
-    }
-    idx.push_back(i), k.push_back(keys[i]), p.push_back(dev_ptrs[i]), sizes.push_back(static_cast<size_t>(size)), pats.push_back(pat);
-  }
-  if (idx.empty()) return out;
-  const auto ecs = put_device(k, p, sizes, &pats, cfg, stream);
-  uint64_t done = 0, bytes = 0;
-  for (size_t j = 0; j < idx.size(); ++j) {
-    out[idx[j]] = ecs[j];
-    if (ecs[j] == ErrorCode::OK) ++done, bytes += sizes[j];
-  }
-  metrics_.inc("device_put_strided_total", done);
-  metrics_.inc("device_put_strided_bytes_total", bytes);
-  return out;
+  std::vector<size_t> sizes(n);
+  std::vector<SourceRows> pats(n);
+  return shaped_batch(
+      "device_put_strided", true, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* size) {
+        uint64_t extent = 0;
+        const ErrorCode ec = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pats[i], size, &extent);
+        if (ec != ErrorCode::OK) return ec;
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        sizes[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return put_device(pick(keys, idx), pick(dev_ptrs, idx), pick(sizes, idx), &p, cfg, stream);
+      });
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
@@ -1111,7 +1115,12 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
       if (copies.empty()) continue;
       // placements on host tiers (DRAM / CXL / NVMe) and unaligned caller buffers: stage through host memory and use the
       // data servers
-      bool on_fabric = fabric_aligned(dev_ptrs[i], rows_of(i), copies);
+      const SourceRows pat = rows_of(i);
+      const auto src = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
+      bool on_fabric = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
+        uint64_t at = 0;
+        return pat.rebase(off, &at).coaligned(src + at, len);
+      });
       for (const auto& c : copies)
         for (const auto& sh : c.shards) {
           // a batch lands on a handful of pools: ask the transport once per run of shards on the same pool
@@ -1126,37 +1135,22 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
         host_placed[i] = copies;
         continue;
       }
+      // copies striped differently cannot share a descriptor: then every shard of every copy is an op of its own
       bool same_layout = true;
       for (const auto& c : copies) same_layout &= c.shards.size() == copies[0].shards.size();
-      const SourceRows pat = rows_of(i);
-      if (same_layout) {
+      for (size_t c = 0; c < (same_layout ? 1 : copies.size()); ++c) {
         uint64_t off = 0;
-        for (size_t s = 0; s < copies[0].shards.size(); ++s) {
+        for (size_t s = 0; s < copies[c].shards.size(); ++s) {
           DeviceShardOp op;
           op.item = i;
-          op.copy = 0;
+          op.copy = c;
           op.shard = s;
-          op.placement = &copies[0].shards[s];
+          op.placement = &copies[c].shards[s];
           op.obj_offset = off;
           op.rows = pat.rebase(off, &op.rows_at);
-          for (size_t c = 1; c < copies.size(); ++c) op.replicas.push_back(&copies[c].shards[s]);
+          for (size_t r = 1; same_layout && r < copies.size(); ++r) op.replicas.push_back(&copies[r].shards[s]);
           ch.ops.push_back(std::move(op));
-          off += copies[0].shards[s].length;
-        }
-      } else {
-        for (size_t c = 0; c < copies.size(); ++c) {
-          uint64_t o2 = 0;
-          for (size_t s = 0; s < copies[c].shards.size(); ++s) {
-            DeviceShardOp op;
-            op.item = i;
-            op.copy = c;
-            op.shard = s;
-            op.placement = &copies[c].shards[s];
-            op.obj_offset = o2;
-            op.rows = pat.rebase(o2, &op.rows_at);
-            ch.ops.push_back(std::move(op));
-            o2 += copies[c].shards[s].length;
-          }
+          off += copies[c].shards[s].length;
         }
       }
     }
@@ -1263,21 +1257,18 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<Objec
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                                const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths,
                                                                void* stream) {
-  if (offsets.size() != keys.size() || lengths.size() != keys.size())
-    return std::vector<ErrorCode>(keys.size(), keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
-  std::vector<ByteRange> ranges(keys.size());
-  std::vector<size_t> lens(keys.size());
-  for (size_t i = 0; i < keys.size(); ++i) {
-    ranges[i] = {offsets[i], lengths[i]};
-    lens[i] = static_cast<size_t>(lengths[i]);
-  }
-  auto out = get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr);
-  uint64_t n = 0, bytes = 0;
-  for (size_t i = 0; i < out.size(); ++i)
-    if (out[i] == ErrorCode::OK) ++n, bytes += lengths[i];
-  metrics_.inc("device_get_range_total", n);
-  metrics_.inc("device_get_range_bytes_total", bytes);
-  return out;
+  const size_t n = keys.size();
+  std::vector<ByteRange> ranges(n);
+  std::vector<size_t> lens(n);
+  return shaped_batch(
+      "device_get_range", false, n, offsets.size() == n && lengths.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {offsets[i], lengths[i]};
+        lens[i] = static_cast<size_t>(lengths[i]);
+        *bytes = lengths[i];
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1285,22 +1276,18 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
                                                                  const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows,
                                                                  void* stream) {
   const size_t n = keys.size();
-  if (offsets.size() != n || widths.size() != n || pitches.size() != n || rows.size() != n)
-    return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
   std::vector<ByteRange> ranges(n);
   std::vector<size_t> lens(n);
-  for (size_t i = 0; i < n; ++i) {
-    ranges[i] = {offsets[i], widths[i], pitches[i], rows[i]};
-    uint64_t total = 0;
-    lens[i] = __builtin_mul_overflow(rows[i], widths[i], &total) ? SIZE_MAX : static_cast<size_t>(total);
-  }
-  auto out = get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr);
-  uint64_t k = 0, bytes = 0;
-  for (size_t i = 0; i < n; ++i)
-    if (out[i] == ErrorCode::OK) ++k, bytes += lens[i];
-  metrics_.inc("device_get_strided_total", k);
-  metrics_.inc("device_get_strided_bytes_total", bytes);
-  return out;
+  return shaped_batch(
+      "device_get_strided", false, n, offsets.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {offsets[i], widths[i], pitches[i], rows[i]};
+        uint64_t total = 0;
+        lens[i] = __builtin_mul_overflow(rows[i], widths[i], &total) ? SIZE_MAX : static_cast<size_t>(total);
+        *bytes = lens[i];
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1452,23 +1439,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       };
       // (the spread over replicas only matters when there is more than one; thousands of single-copy objects skip the hash)
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
-      // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned).  A strided get
-      // needs every row co-aligned with the tiles of each shard it reads (StoreWindow::coaligned): the virtual base aligned
-      // at those shards' starts, and the gap between rows a multiple of 16 bytes.
-      bool aligned;
-      if (sp.strided()) {
-        const uintptr_t vbase = reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.lo;
-        aligned = (sp.pitch - sp.width) % 16 == 0;
-        for (const auto& c : copies) {
-          uint64_t off = 0;
-          for (const auto& sh : c.shards) {
-            if (sp.touches(off, sh.length) && (vbase + off) % 16) aligned = false;
-            off += sh.length;
-          }
-        }
-      } else {
-        aligned = fabric_aligned(bases[i], SourceRows{}, copies);
-      }
+      // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
+      const auto dst = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
+      const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) { return sp.fused_get_aligned(dst, off, len); });
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
         bool local = true;
@@ -1581,45 +1554,13 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
     if (pending[i]) out[i] = ErrorCode::CHECKSUM_MISMATCH;
   if (n_local) metrics_.inc("device_get_local_replica_total", n_local);
   if (n_dram_direct) metrics_.inc("device_get_dram_direct_total", n_dram_direct);
-  // ---- a mismatch can also mean that the Keystone moved the object under us (tier move, compaction, repair): the
-  // extents we read were freed and re-used.  Objects whose placements changed since we fetched them get one more pass.
-  static thread_local int refresh_depth = 0;
-  if (refresh_depth < 2) {
-    std::vector<size_t> bad;
-    for (size_t i = 0; i < keys.size(); ++i)
-      if (out[i] == ErrorCode::CHECKSUM_MISMATCH && placed[i].ok()) bad.push_back(i);
-    if (!bad.empty()) {
-      std::vector<ObjectKey> bkeys;
-      for (size_t i : bad) bkeys.push_back(keys[i]);
-      auto again = keystone_->batch_get_workers(bkeys);
-      std::vector<ObjectKey> rkeys;
-      std::vector<void*> rptrs;
-      std::vector<size_t> rcaps, ridx;
-      std::vector<ByteRange> rranges;
-      for (size_t k = 0; k < bad.size(); ++k) {
-        const size_t i = bad[k];
-        if (!again[k].ok()) {
-          out[i] = again[k].error();  // removed (or being re-written) meanwhile: that is the answer
-        } else if (!(again[k].value() == placed[i].value()) || refresh_depth == 0) {
-          // changed placements, or (once) the same ones: a remove + re-put can land on the very same extent (first fit)
-          // and be read half-written
-          rkeys.push_back(keys[i]), rptrs.push_back(dev_ptrs[i]), rcaps.push_back(capacity[i]), ridx.push_back(i);
-          if (ranges) rranges.push_back((*ranges)[i]);
-        }
-      }
-      if (!rkeys.empty()) {
-        metrics_.inc("get_placement_refresh_total", rkeys.size());
-        std::vector<size_t> rsizes;
-        ++refresh_depth;
-        auto recs = get_device(rkeys, rptrs, rcaps, ranges ? &rranges : nullptr, stream, &rsizes);
-        --refresh_depth;
-        for (size_t k = 0; k < ridx.size(); ++k) {
-          out[ridx[k]] = recs[k];
-          if (out_sizes && k < rsizes.size()) (*out_sizes)[ridx[k]] = rsizes[k];
-        }
-      }
-    }
-  }
+  refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
+    const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
+    std::vector<size_t> rsizes;
+    auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, stream, &rsizes);
+    for (size_t k = 0; out_sizes && k < r.size() && k < rsizes.size(); ++k) (*out_sizes)[r[k]] = rsizes[k];
+    return recs;
+  });
   if (!keys.empty()) ewma_update(get_rpc_us_per_obj_, rpc_us_total / static_cast<double>(keys.size()));
   metrics_.inc("device_get_batches_total");
   metrics_.observe("device_get_batch_latency_us", us_since(t_all));

@@ -103,11 +103,11 @@ class DeviceTransport {
   // True when the shard lives in this client's own device memory (a get from it never leaves the GPU).
   virtual bool is_local(const ShardPlacement& s) const { return false; }
   virtual size_t max_in_flight() const { return 1; }
-  // Fused MXFP8 put / get (pack / unpack inside the transfer kernel).  digests[i] = BBH64 of the stored packed
-  // object; status[i] != 0 = digest mismatch on get.  Objects must satisfy fp8_eligible().
   // Prometheus lines of the transport's own counters (bytes per path, launches, ...); appended to the client's metrics.
   virtual std::string metrics_text() const { return {}; }
   virtual bool fp8_eligible(uint64_t n_elems) const { return false; }
+  // Fused MXFP8 put / get (pack / unpack inside the transfer kernel).  digests[i] = BBH64 of the stored packed
+  // object; status[i] != 0 = digest mismatch on get.  Objects must satisfy fp8_eligible().
   virtual ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) { return ErrorCode::NOT_IMPLEMENTED; }
   virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
   // Staging copies for objects (or shards) that live on host tiers: device <-> host buffer, synchronous.
@@ -217,8 +217,9 @@ class BlackbirdClient {
   // Byte-range gets: bytes [offsets[i], offsets[i] + lengths[i]) of object i land at dev_ptrs[i].  Every shard that overlaps
   // a range is read whole and verified against its digest (a corrupt byte outside the range still fails that copy over to
   // the next replica); shards outside the range are not touched.  A range whose virtual base dev_ptrs[i] - offsets[i] is
-  // not 16-byte aligned at a shard start is staged through the host, like a misaligned batch_get_device.  Per-object
-  // VALUE_OUT_OF_RANGE when the range passes the end of the object.
+  // not 16-byte aligned at the start of every shard of every copy is staged through the host, like a misaligned
+  // batch_get_device (StoreWindow::fused_get_aligned).  Per-object VALUE_OUT_OF_RANGE when the range passes the end of the
+  // object.
   std::vector<ErrorCode> batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                 const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths, void* stream);
   // Strided gets (a slice along an inner dimension): rows[i] rows of widths[i] bytes, row r being object bytes
@@ -275,6 +276,12 @@ class BlackbirdClient {
   // object i's rows (offset, length and pitch in elements) into bf16_ptrs[i].
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream);
+  // The six shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
+  template <class Shape, class Run>
+  std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);
+  template <class Reissue>
+  void refresh_placements(const std::vector<ObjectKey>& keys, const std::vector<Result<std::vector<CopyPlacement>>>& placed,
+                          std::vector<ErrorCode>& out, Reissue&& reissue);
   ErrorCode get_with_refresh(const ObjectKey& key, uint8_t* (*alloc)(void*, size_t), void* ctx, size_t capacity, size_t* out_size);
   static uint64_t shard_offset(const ShardPlacement& s);
   static ChecksumAlgo algo_of(const std::vector<CopyPlacement>& copies, ChecksumAlgo hint);

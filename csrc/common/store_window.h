@@ -107,6 +107,22 @@ struct StoreWindow {
     return (base + origin() + phase - r_lo * gap) % 16 == 0;
   }
 
+  // The client's rule for whether a device get of this window (in bytes; an MXFP8 get's after to_bf16_bytes()) into `ptr`,
+  // where its first stored unit lands, may take the fused path as far as the shard [off, off + len) of a copy goes; the
+  // get is fused only if every shard of every copy passes (an MXFP8 object is one shard, [0, 2 * n_elems)).  The kernels
+  // store 16-byte aligned spans only, so the virtual base ptr - lo must be 16-byte aligned at the shard's start: at every
+  // shard for a contiguous window, at the shards it touches for a strided one.  A strided window also needs a gap that is
+  // a multiple of 16 bytes, even where each shard it touches holds a single row and coaligned() would pass it: so whether
+  // a strided get is fused depends on its own shape and pointer, as the API documents it, not on where the placement
+  // happened to cut the object.
+  bool fused_get_aligned(uintptr_t ptr, uint64_t off, uint64_t len) const {
+    if (strided()) {
+      if ((pitch - width) % 16) return false;
+      if (!touches(off, len)) return true;
+    }
+    return (ptr - lo + off) % 16 == 0;
+  }
+
   // Calls f(x, at, n) for every run of n stored units from unit x of an object of n_units, landing at `at` relative to
   // the base, in order.
   template <class F>

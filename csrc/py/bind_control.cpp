@@ -42,6 +42,15 @@ auto nogil(F&& f) {
   return f();
 }
 
+// Device pointers cross the boundary as integers (tensor.data_ptr()).
+template <typename P>
+std::vector<P> to_ptrs(const std::vector<uintptr_t>& v) {
+  std::vector<P> out;
+  out.reserve(v.size());
+  for (auto p : v) out.push_back(reinterpret_cast<P>(p));
+  return out;
+}
+
 // list[ErrorCode] for batch results.  pybind builds a fresh enum instance per element (~0.3 us); a batch of thousands of
 // objects gets the cached instance of each code instead (enum members are immutable).  GIL held.
 py::list ecs_to_py(const std::vector<ErrorCode>& v) {
@@ -1166,19 +1175,15 @@ void bind_control(py::module_& m) {
       .def("batch_put_device_fp8",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               const WorkerConfig& cfg, uintptr_t stream) {
-             std::vector<const void*> p;
-             for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
-             py::gil_scoped_release rel;
-             return c.batch_put_device_fp8(keys, p, n_elems, cfg, reinterpret_cast<void*>(stream));
+             return ecs_to_py(nogil([&] { return c.batch_put_device_fp8(keys, to_ptrs<const void*>(ptrs), n_elems, cfg, reinterpret_cast<void*>(stream)); }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("config"), py::arg("stream") = 0)
       .def("batch_put_device_fp8_strided",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& widths,
               const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream) {
-             std::vector<const void*> p;
-             for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
-             py::gil_scoped_release rel;
-             return c.batch_put_device_fp8_strided(keys, p, widths, pitches, rows, cfg, reinterpret_cast<void*>(stream));
+             return ecs_to_py(nogil([&] {
+               return c.batch_put_device_fp8_strided(keys, to_ptrs<const void*>(ptrs), widths, pitches, rows, cfg, reinterpret_cast<void*>(stream));
+             }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("elem_widths"), py::arg("elem_pitches"), py::arg("rows"), py::arg("config"),
            py::arg("stream") = 0,
@@ -1188,19 +1193,15 @@ void bind_control(py::module_& m) {
       .def("batch_get_device_fp8",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               uintptr_t stream) {
-             std::vector<void*> p;
-             for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
-             py::gil_scoped_release rel;
-             return c.batch_get_device_fp8(keys, p, n_elems, reinterpret_cast<void*>(stream));
+             return ecs_to_py(nogil([&] { return c.batch_get_device_fp8(keys, to_ptrs<void*>(ptrs), n_elems, reinterpret_cast<void*>(stream)); }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("stream") = 0)
       .def("batch_get_device_fp8_range",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& counts, uintptr_t stream) {
-             std::vector<void*> p;
-             for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
-             py::gil_scoped_release rel;
-             return c.batch_get_device_fp8_range(keys, p, n_elems, offsets, counts, reinterpret_cast<void*>(stream));
+             return ecs_to_py(nogil([&] {
+               return c.batch_get_device_fp8_range(keys, to_ptrs<void*>(ptrs), n_elems, offsets, counts, reinterpret_cast<void*>(stream));
+             }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_counts"), py::arg("stream") = 0,
            "Elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of packed tensor i (n_elems[i] elements), unpacked to "
@@ -1210,10 +1211,9 @@ void bind_control(py::module_& m) {
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
               const std::vector<uint64_t>& rows, uintptr_t stream) {
-             std::vector<void*> p;
-             for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
-             py::gil_scoped_release rel;
-             return c.batch_get_device_fp8_strided(keys, p, n_elems, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream));
+             return ecs_to_py(nogil([&] {
+               return c.batch_get_device_fp8_strided(keys, to_ptrs<void*>(ptrs), n_elems, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream));
+             }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_widths"),
            py::arg("elem_pitches"), py::arg("rows"), py::arg("stream") = 0,
@@ -1252,47 +1252,36 @@ void bind_control(py::module_& m) {
       })
       .def("batch_put_device", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                   const std::vector<size_t>& sizes, const WorkerConfig& cfg, uintptr_t stream) {
-        std::vector<const void*> p;
-        p.reserve(ptrs.size());
-        for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
-        return ecs_to_py(nogil([&] { return c.batch_put_device(keys, p, sizes, cfg, reinterpret_cast<void*>(stream)); }));
+        return ecs_to_py(nogil([&] { return c.batch_put_device(keys, to_ptrs<const void*>(ptrs), sizes, cfg, reinterpret_cast<void*>(stream)); }));
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("sizes"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0)
       .def("batch_put_device_strided", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                           const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                           const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream) {
-        std::vector<const void*> p;
-        for (auto v : ptrs) p.push_back(reinterpret_cast<const void*>(v));
-        return ecs_to_py(nogil([&] { return c.batch_put_device_strided(keys, p, widths, pitches, rows, cfg, reinterpret_cast<void*>(stream)); }));
+        return ecs_to_py(nogil([&] {
+          return c.batch_put_device_strided(keys, to_ptrs<const void*>(ptrs), widths, pitches, rows, cfg, reinterpret_cast<void*>(stream));
+        }));
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("widths"), py::arg("pitches"), py::arg("rows"), py::arg("config") = WorkerConfig{},
          py::arg("stream") = 0,
          "Object i = rows[i] rows of widths[i] bytes, row r read from dev_ptrs[i] + r * pitches[i]; stored as a put of the "
          "compacted rows would store it; returns one ErrorCode per object.")
       .def("batch_get_device",[](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                   const std::vector<size_t>& caps, uintptr_t stream) {
-        std::vector<void*> p;
-        for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
         std::vector<size_t> sizes;
-        std::vector<ErrorCode> ecs;
-        {
-          py::gil_scoped_release rel;
-          ecs = c.batch_get_device(keys, p, caps, reinterpret_cast<void*>(stream), &sizes);
-        }
+        const auto ecs = nogil([&] { return c.batch_get_device(keys, to_ptrs<void*>(ptrs), caps, reinterpret_cast<void*>(stream), &sizes); });
         return py::make_tuple(ecs_to_py(ecs), sizes);
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("capacity"), py::arg("stream") = 0)
       .def("batch_get_device_range", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                         const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths, uintptr_t stream) {
-        std::vector<void*> p;
-        for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
-        return ecs_to_py(nogil([&] { return c.batch_get_device_range(keys, p, offsets, lengths, reinterpret_cast<void*>(stream)); }));
+        return ecs_to_py(nogil([&] { return c.batch_get_device_range(keys, to_ptrs<void*>(ptrs), offsets, lengths, reinterpret_cast<void*>(stream)); }));
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("lengths"), py::arg("stream") = 0,
          "Bytes [offsets[i], offsets[i] + lengths[i]) of object i into dev_ptrs[i]; every overlapping shard is read whole and "
          "verified; returns one ErrorCode per object.")
       .def("batch_get_device_strided", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                           const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
                                           const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, uintptr_t stream) {
-        std::vector<void*> p;
-        for (auto v : ptrs) p.push_back(reinterpret_cast<void*>(v));
-        return ecs_to_py(nogil([&] { return c.batch_get_device_strided(keys, p, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream)); }));
+        return ecs_to_py(nogil([&] {
+          return c.batch_get_device_strided(keys, to_ptrs<void*>(ptrs), offsets, widths, pitches, rows, reinterpret_cast<void*>(stream));
+        }));
       }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("widths"), py::arg("pitches"), py::arg("rows"), py::arg("stream") = 0,
          "rows[i] rows of widths[i] bytes of object i, row r = bytes [offsets[i] + r * pitches[i], + widths[i]), densely into "
          "dev_ptrs[i] (row r at dev_ptrs[i] + r * widths[i]); every shard holding a stored byte is read whole and verified; "

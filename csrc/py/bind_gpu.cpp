@@ -44,6 +44,12 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
+// A put's gather pattern (common/store_window.h) given as (pitch, width, phase).
+SourceRows to_rows(const py::handle& h) {
+  auto g = h.cast<std::vector<uint64_t>>();
+  if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
+  return {g[0], g[1], g[2]};
+}
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None).  An empty destination
 // list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets XFER_WINDOW, and
 // one with a pattern XFER_STRIDED as well.  A gather pattern (pitch, width, phase) sets XFER_GATHER, with src = row 0.
@@ -60,9 +66,7 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
   if (t.size() > 7 && !t[7].is_none()) {
-    auto g = t[7].cast<std::vector<uint64_t>>();
-    if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
-    it.rows = {g[0], g[1], g[2]};
+    it.rows = to_rows(t[7]);
     it.flags |= XFER_GATHER;
   }
   return it;
@@ -131,11 +135,7 @@ void bind_gpu(py::module_& m) {
                  throw py::value_error("fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, (pitch, width, phase)]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
-               if (t.size() > 5 && !t[5].is_none()) {
-                 auto g = t[5].cast<std::vector<uint64_t>>();
-                 if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
-                 it.rows = {g[0], g[1], g[2]};
-               }
+               if (t.size() > 5 && !t[5].is_none()) it.rows = to_rows(t[5]);
                v.push_back(it);
              }
              XferResult res;

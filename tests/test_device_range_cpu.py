@@ -184,14 +184,21 @@ def test_unaligned_virtual_bases_are_staged_and_their_neighbours_are_not(bb):
         size = 300000
         blob = np.frombuffer(os.urandom(size), dtype=np.uint8).copy()
         assert cl.batch_put_device(["a"], [blob.ctypes.data], [size], _cfg(bb, 1, 1), 0) == [bb.ErrorCode.OK]
-        # (ptr - offset) % 16: 0, 0, 3, 0 -- only the third is staged
-        ranges = [(16, 5000), (7, 100), (20, 4000), (1, 33)]
-        skew = {0: 0, 1: 7, 2: 7, 3: 1}
+        # a striped object whose second stripe starts at an address that is not a multiple of 16
+        striped = np.frombuffer(os.urandom(size + 3), dtype=np.uint8).copy()
+        assert cl.batch_put_device(["b"], [striped.ctypes.data], [striped.size], _cfg(bb, 1, 2), 0) == [bb.ErrorCode.OK]
+        (lay,) = Shards(c, cl).layout("b")
+        e1 = lay[1][0]
+        assert len(lay) == 2 and e1 % 16, [o for o, _ in lay]
+        # (ptr - offset) % 16: 0, 0, 3, 0 -- only the third is staged.  The fifth, inside the second stripe, is aligned at
+        # that stripe's start but not at the first stripe's: a range checks every shard of every copy, so it is staged too.
+        ranges = [(16, 5000), (7, 100), (20, 4000), (1, 33), (e1 + 17, 1000)]
+        skew = {0: 0, 1: 7, 2: 7, 3: 1, 4: 1}
         staged = _counter(cl, "device_get_host_staged_total")
-        ecs, raw, dsts = _get_ranges(cl, ["a"] * 4, ranges, skew)
-        assert ecs == [bb.ErrorCode.OK] * 4
-        _check(raw, dsts, [blob] * 4, ranges, [True] * 4)
-        assert _counter(cl, "device_get_host_staged_total") == staged + 1
+        ecs, raw, dsts = _get_ranges(cl, ["a"] * 4 + ["b"], ranges, skew)
+        assert ecs == [bb.ErrorCode.OK] * 5
+        _check(raw, dsts, [blob] * 4 + [striped], ranges, [True] * 5)
+        assert _counter(cl, "device_get_host_staged_total") == staged + 2
 
 
 def test_range_gets_survive_concurrent_migration(bb):

@@ -191,20 +191,25 @@ def test_a_corrupt_byte_in_a_gap_of_a_read_shard_fails_over(bb):
 
 
 def test_misaligned_items_are_staged_and_their_neighbours_are_not(bb):
-    """(ptr - offset) % 16 != 0 or a row gap that is not a multiple of 16: staged through the host (rows compacted there);
-    the other items of the batch take the transport."""
+    """(ptr - offset) % 16 != 0 or a row gap that is not a multiple of 16, even where every shard read holds one row:
+    staged through the host (rows compacted there); the other items of the batch take the transport."""
     with LocalCluster(cluster_id="stral", n_workers=2, pool_bytes=32 * MiB) as c:
         cl = make_client(bb, c)
         size = 300000
         blob = np.frombuffer(os.urandom(size), dtype=np.uint8).copy()
         assert cl.batch_put_device(["a"], [blob.ctypes.data], [size], _cfg(bb, 1, 1), 0) == [bb.ErrorCode.OK]
-        pats = [(16, 100, 132, 50), (7, 33, 49, 80), (20, 40, 72, 30), (3, 40, 75, 30)]
-        skew = {2: 5}  # item 2: misaligned base; item 3: gap 35
+        big = np.frombuffer(os.urandom(2 * MiB), dtype=np.uint8).copy()
+        assert cl.batch_put_device(["b"], [big.ctypes.data], [big.size], _cfg(bb, 1, 2), 0) == [bb.ErrorCode.OK]
+        (lay,) = Shards(c, cl).layout("b")
+        assert [o for o, _ in lay] == [0, MiB]
+        # item 2: misaligned base; item 3: gap 35; item 4: gap MiB - 24 with one row in each stripe it reads
+        pats = [(16, 100, 132, 50), (7, 33, 49, 80), (20, 40, 72, 30), (3, 40, 75, 30), (16, 32, MiB + 8, 2)]
+        skew = {2: 5}
         staged = _counter(cl, "device_get_host_staged_total")
-        ecs, raw, dsts = _get_strided(cl, ["a"] * 4, pats, skew)
-        assert ecs == [bb.ErrorCode.OK] * 4
-        _check(raw, dsts, [blob] * 4, pats, [True] * 4)
-        assert _counter(cl, "device_get_host_staged_total") == staged + 2
+        ecs, raw, dsts = _get_strided(cl, ["a"] * 4 + ["b"], pats, skew)
+        assert ecs == [bb.ErrorCode.OK] * 5
+        _check(raw, dsts, [blob] * 4 + [big], pats, [True] * 5)
+        assert _counter(cl, "device_get_host_staged_total") == staged + 3
 
 
 def test_one_row_counts_as_a_range(bb):
