@@ -80,4 +80,29 @@ dg, st, _ = eng.run_fp8([(flat.data_ptr() + 2 * row0, [r.data_ptr() for r in rep
 dg2, _, _ = eng.run_fp8([(dense.data_ptr(), reps[2].data_ptr(), n)], False, s)
 torch.cuda.synchronize()
 assert dg == dg2 and torch.equal(reps[0], reps[2]) and torch.equal(reps[1], reps[2])
-print(f"sanitize target OK: {checked} kernel configurations + mxfp8 + gathered mxfp8 put")
+# scattering store of bb_xfer: an object stored into rows of 100 every 132 bytes, starting 4 bytes into row 0 (so every row
+# segment has a head and a tail), verified; the gaps keep their guard
+n = 3 * 16384 + 77
+src = torch.randint(0, 256, (n,), dtype=torch.uint8, device="cuda")
+gdst = torch.full(((n + 4) // 100 * 132 + 256,), 0xA5, dtype=torch.uint8, device="cuda")
+x = torch.arange(n, device="cuda") + 4
+at = 12 + x // 100 * 132 + x % 100  # row 0 at byte 12 of gdst, so that row 0 + phase is 16-byte aligned
+dg, st, _ = eng.run([(src.data_ptr(), gdst.data_ptr() + 12, n, _bb.xxh3t64(src.cpu().numpy()), _bb.XFER_VERIFY, 0, None, None,
+                      (132, 100, 4))], _bb.ChecksumAlgo.XXH3, s)
+torch.cuda.synchronize()
+mask = torch.ones_like(gdst, dtype=torch.bool)
+mask[at] = False
+assert st == [0] and torch.equal(gdst[at], src) and bool((gdst[mask] == 0xA5).all())
+# scattering store of the fused MXFP8 unpack: the packed object above unpacked into rows of 128 every 544 elements from
+# element 4 of row 0, compared with a plain unpack scattered by torch
+out = torch.full((64 * 544,), -7.0, dtype=torch.bfloat16, device="cuda")
+plain = torch.empty(63 * 128, dtype=torch.bfloat16, device="cuda")
+eng.run_fp8([(plain.data_ptr(), reps[2].data_ptr(), 63 * 128)], True, s)
+dg3, st3, _ = eng.run_fp8([(out.data_ptr() + 2 * row0, reps[2].data_ptr(), 63 * 128, dg2[0], None, None, (544, 128, 4))], True, s)
+torch.cuda.synchronize()
+x = torch.arange(63 * 128, device="cuda") + 4
+at = row0 + x // 128 * 544 + x % 128
+mask = torch.ones_like(out, dtype=torch.bool)
+mask[at] = False
+assert st3 == [0] and torch.equal(out[at].view(torch.int16), plain.view(torch.int16)) and bool((out[mask] == -7.0).all())
+print(f"sanitize target OK: {checked} kernel configurations + mxfp8 + gathered mxfp8 put + scattered get + scattered mxfp8 get")

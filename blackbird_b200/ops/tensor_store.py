@@ -214,6 +214,84 @@ class TensorStore:
     def get(self, key: str, device: Optional[torch.device] = None) -> torch.Tensor:
         return self.batch_get([key], device)[0]
 
+    def batch_get_into(self, keys: Sequence[str], outs: Sequence[torch.Tensor]) -> list:
+        """Loads each stored tensor into an existing CUDA tensor on the current device and returns `outs`: restoring a KV
+        block into its slot of a preallocated cache (`cache[layer, :, slot]`), a tensor-parallel shard into its columns of
+        a full weight (`W[:, k0:k1]`), or a tensor into a parameter's storage.  No element of an out's storage outside the
+        view is written.  The outs must not overlap one another (not checked).
+
+        Every check comes before any transfer: KeyError for a missing key, TypeError unless out.dtype is the stored
+        dtype (bfloat16 for packed tensors), ValueError unless out.shape is the stored shape and out is a CUDA tensor on
+        the current device.  Then each route is one call for all the tensors that take it:
+          1. unpacked, contiguous out: batch_get_device into its storage;
+          2. unpacked, out whose elements are rows (see _source_rows: `narrow` along any dim, `t[::k]`):
+             batch_get_device_scatter, whose kernel stores each tile straight into the rows (misaligned rows are staged
+             through the host by the client);
+          3. MXFP8-packed whole-block tensors, contiguous or rows: batch_get_device_fp8, or batch_get_device_fp8_scatter
+             when any out is rows (contiguous ones go as one row);
+          4. everything else -- transposed or overlapping layouts, padded packed tensors, packed tensors the fused
+             kernels refuse (NOT_IMPLEMENTED: misaligned rows, unfusable placements) -- batch_get into a temporary, then
+             out.copy_()."""
+        keys, outs = list(keys), list(outs)
+        if len(keys) != len(outs):
+            raise ValueError("keys and outs differ in length")
+        metas = self._metas(keys)
+        dev = torch.cuda.current_device()
+        for k, m, o in zip(keys, metas, outs):
+            want = torch.bfloat16 if m["packed"] else _DTYPES[m["dtype"]]
+            if o.dtype != want:
+                raise TypeError(f"{k}: out is {o.dtype}, the stored tensor {want}")
+            if list(o.shape) != m["shape"]:
+                raise ValueError(f"{k}: out has shape {list(o.shape)}, the stored tensor {m['shape']}")
+            if not o.is_cuda or o.device.index != dev:
+                raise ValueError(f"{k}: out must be a CUDA tensor on cuda:{dev}, not {o.device}")
+        rows = [None if o.is_contiguous() else self._source_rows(o) for o in outs]
+        rest = []  # route 4
+
+        def check(name, idx, ecs):
+            bad = [(keys[i], e) for i, e in zip(idx, ecs) if e != _bb.ErrorCode.OK]
+            if bad:
+                raise RuntimeError(f"{name} failed: {bad[:3]}")
+
+        plain = [i for i, m in enumerate(metas) if not m["packed"]]
+        dense = [i for i in plain if outs[i].is_contiguous()]
+        if dense:
+            ecs, _ = self.client.batch_get_device([keys[i] for i in dense], [outs[i].data_ptr() for i in dense],
+                                                  [outs[i].numel() * outs[i].element_size() for i in dense], self._stream())
+            check("get", dense, ecs)
+        scattered = [i for i in plain if not outs[i].is_contiguous() and rows[i] is not None]
+        if scattered:
+            ecs, _ = self.client.batch_get_device_scatter([keys[i] for i in scattered], [outs[i].data_ptr() for i in scattered],
+                                                          [rows[i][0] for i in scattered], [rows[i][1] for i in scattered],
+                                                          [rows[i][2] for i in scattered], self._stream())
+            check("scattered get", scattered, ecs)
+        rest += [i for i in plain if not outs[i].is_contiguous() and rows[i] is None]
+        packed = [i for i, m in enumerate(metas) if m["packed"]]
+        fused = [i for i in packed if metas[i]["padded_numel"] == metas[i]["numel"] and self.client.device_fp8_eligible(metas[i]["numel"])
+                 and (outs[i].is_contiguous() or rows[i] is not None)]
+        rest += [i for i in packed if i not in set(fused)]
+        if fused:
+            fk, ptrs = [keys[i] for i in fused], [outs[i].data_ptr() for i in fused]
+            if any(rows[i] is not None for i in fused):
+                # widths and pitches in elements; contiguous outs go as one row each
+                shapes = [(rows[i][0] // 2, rows[i][1] // 2, rows[i][2]) if rows[i] is not None else (outs[i].numel(),) * 2 + (1,)
+                          for i in fused]
+                ecs = self.client.batch_get_device_fp8_scatter(fk, ptrs, [outs[i].numel() for i in fused], [s[0] for s in shapes],
+                                                               [s[1] for s in shapes], [s[2] for s in shapes], self._stream())
+            else:
+                ecs = self.client.batch_get_device_fp8(fk, ptrs, [outs[i].numel() for i in fused], self._stream())
+            check("fused fp8 get", [i for i, e in zip(fused, ecs) if e != _bb.ErrorCode.NOT_IMPLEMENTED],
+                  [e for e in ecs if e != _bb.ErrorCode.NOT_IMPLEMENTED])
+            rest += [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
+        if rest:
+            for i, t in zip(rest, self.batch_get([keys[i] for i in rest], outs[rest[0]].device)):
+                outs[i].copy_(t)
+        return outs
+
+    def get_into(self, key: str, out: torch.Tensor) -> torch.Tensor:
+        """Loads the tensor stored under `key` into `out` and returns it (see batch_get_into)."""
+        return self.batch_get_into([key], [out])[0]
+
     def batch_get_rows(self, keys: Sequence[str], starts: Sequence[int], stops: Sequence[int],
                        device: Optional[torch.device] = None) -> list:
         """Rows [start, stop) along dim 0 of each stored tensor, as new tensors (`t[start:stop]`): a tensor-parallel rank
@@ -417,6 +495,24 @@ class AsyncTensorStore(TensorStore):
                 out = self.batch_get(keys)
             self._side.synchronize()
             return out
+
+        return self._pool.submit(run)
+
+    def get_into_async(self, keys: Sequence[str], outs: Sequence[torch.Tensor]):
+        """batch_get_into on the side stream; the future yields `outs`, already synchronised with it.  The side stream
+        first waits for the work already queued on the caller's stream, so the get does not overtake the caller's earlier
+        reads or writes of the outs."""
+        ready = torch.cuda.Event()
+        ready.record(torch.cuda.current_stream())
+        keys, outs = list(keys), list(outs)
+
+        def run():
+            torch.cuda.set_device(self._device)
+            self._side.wait_event(ready)
+            with torch.cuda.stream(self._side):
+                self.batch_get_into(keys, outs)
+            self._side.synchronize()
+            return outs
 
         return self._pool.submit(run)
 

@@ -765,7 +765,32 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                              const std::vector<uint64_t>& n_elems, void* stream) {
-  return get_device_fp8(keys, bf16_ptrs, n_elems, nullptr, stream);
+  return get_device_fp8(keys, bf16_ptrs, n_elems, nullptr, nullptr, stream);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                                     const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
+                                                                     const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
+                                                                     void* stream) {
+  const size_t n = keys.size();
+  std::vector<SourceRows> pats(n);
+  return shaped_batch(
+      "device_get_fp8_scatter", false, n,
+      bf16_ptrs.size() == n && n_elems.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* bf16_bytes) {
+        SourceRows bytes;
+        uint64_t elems = 0, extent = 0;
+        const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems, &extent);
+        if (ec != ErrorCode::OK) return ec;
+        if (elems != n_elems[i]) return ErrorCode::INVALID_ARGUMENT;
+        if (extent > UINT64_MAX / 2 || !pats[i].to_bf16_bytes(&bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *bf16_bytes = 2 * elems;
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &p, stream);
+      });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -780,7 +805,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::ve
         *bytes = 2 * elem_counts[i];
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream); });
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -796,15 +821,18 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
         *bytes = 2 * rows[i] * elem_widths[i];  // counted for OK items only, whose rows lie inside the object
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, stream); });
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
-                                                       const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream) {
+                                                       const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
+                                                       const std::vector<SourceRows>* rows, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size())) return out;
+  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
+      (rows && (ranges || rows->size() != keys.size())))
+    return out;
   BB_TRACE_SPAN("batch_get_device_fp8", keys.size());
   auto placed = keystone_->batch_get_workers(keys);
   std::vector<std::vector<size_t>> candidates(keys.size());
@@ -853,6 +881,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
+    SourceRows dst_bytes;  // so do destination rows the kernel cannot store into
+    if (rows && (!(*rows)[i].to_bf16_bytes(&dst_bytes) ||
+                 !dst_bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, 2 * n_elems[i]))) {
+      out[i] = ErrorCode::NOT_IMPLEMENTED;
+      continue;
+    }
     candidates[i] = std::move(order);
     idx.push_back(i);
   }
@@ -866,7 +900,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i]});
+      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}});
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -883,7 +917,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   // a key that moved to a non-fusable placement comes back NOT_IMPLEMENTED from the refresh, i.e. "get + unpack instead"
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
-    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, stream);
+    const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
+    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr, stream);
   });
   metrics_.inc("device_get_fp8_batches_total");
   return out;
@@ -1251,7 +1286,33 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
 std::vector<ErrorCode> BlackbirdClient::batch_get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                          const std::vector<size_t>& capacity, void* stream,
                                                          std::vector<size_t>* out_sizes) {
-  return get_device(keys, dev_ptrs, capacity, nullptr, stream, out_sizes);
+  return get_device(keys, dev_ptrs, capacity, nullptr, nullptr, stream, out_sizes);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                                 const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                                                 const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes) {
+  const size_t n = keys.size();
+  std::vector<size_t> caps(n);
+  std::vector<SourceRows> pats(n);
+  if (out_sizes) out_sizes->assign(n, 0);
+  return shaped_batch(
+      "device_get_scatter", false, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
+      [&](size_t i, uint64_t* size) {
+        uint64_t extent = 0;
+        const ErrorCode ec = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pats[i], size, &extent);
+        if (ec != ErrorCode::OK) return ec;
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        caps[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        std::vector<size_t> sizes;
+        auto ecs = get_device(pick(keys, idx), pick(dev_ptrs, idx), pick(caps, idx), nullptr, &p, stream, &sizes);
+        for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
+        return ecs;
+      });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1268,7 +1329,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector
         *bytes = lengths[i];
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr); });
+      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, nullptr, stream, nullptr); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1287,16 +1348,19 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
         *bytes = lens[i];
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, stream, nullptr); });
+      [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, nullptr, stream, nullptr); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
-                                                   const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges, void* stream,
-                                                   std::vector<size_t>* out_sizes) {
+                                                   const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges,
+                                                   const std::vector<SourceRows>* rows, void* stream, std::vector<size_t>* out_sizes) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size())) return out;
+  if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
+      (rows && (ranges || rows->size() != keys.size())))
+    return out;
+  auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_get_device", keys.size());
   if (out_sizes) out_sizes->assign(keys.size(), 0);
@@ -1329,6 +1393,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           op.placement = &copy.shards[s];
           op.obj_offset = off;
           if (!whole) op.win = sp.rebase(off, len);
+          if (rows) op.rows = (*rows)[i].rebase(off, &op.rows_at);  // a scattered get: the shard's destination rows
           ops.push_back(std::move(op));
         }
         off += len;
@@ -1441,7 +1506,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
       // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
       const auto dst = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
-      const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) { return sp.fused_get_aligned(dst, off, len); });
+      const SourceRows pat = rows_of(i);
+      const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
+        return rows ? pat.fused_get_aligned(dst, off, len) : sp.fused_get_aligned(dst, off, len);
+      });
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
         bool local = true;
@@ -1474,6 +1542,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           std::vector<uint8_t> dense(capacity[i]);
           sp.for_each_run(size, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + at, stage.data() + x, n); });
           ec = device_->copy_h2d(dev_ptrs[i], dense.data(), dense.size(), stream);
+        } else if (ec == ErrorCode::OK && pat.strided()) {
+          // into the destination rows: one 2-D H2D copy of the whole rows, then the object's part of the next row
+          const uint64_t full = size / pat.width, part = size % pat.width;
+          ec = device_->copy_h2d_rows(dev_ptrs[i], pat.pitch, stage.data(), pat.width, full, stream);
+          if (ec == ErrorCode::OK && part)
+            ec = device_->copy_h2d(static_cast<uint8_t*>(dev_ptrs[i]) + full * pat.pitch, stage.data() + full * pat.width, part, stream);
         } else if (ec == ErrorCode::OK) {
           ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
         }
@@ -1556,8 +1630,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   if (n_dram_direct) metrics_.inc("device_get_dram_direct_total", n_dram_direct);
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
+    const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
     std::vector<size_t> rsizes;
-    auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, stream, &rsizes);
+    auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr,
+                           stream, &rsizes);
     for (size_t k = 0; out_sizes && k < r.size() && k < rsizes.size(); ++k) (*out_sizes)[r[k]] = rsizes[k];
     return recs;
   });
@@ -1602,7 +1678,14 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     ErrorCode ec;
-    if (op.win.covers(op.placement->length)) {
+    if (op.rows.strided()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows
+      if (!op.rows.valid() || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
+      std::vector<uint8_t> whole(op.placement->length);
+      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
+      auto* dst = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.rows_at;
+      if (ec == ErrorCode::OK)
+        op.rows.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + at, whole.data() + x, n); });
+    } else if (op.win.covers(op.placement->length)) {
       ec = io_->read_shard(*op.placement, static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset, op.placement->checksum_algo);
     } else {  // as the kernel does: read and verify the whole shard, store only the window (only it is real memory)
       std::vector<uint8_t> whole(op.placement->length);
@@ -1672,6 +1755,11 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
     if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
+    SourceRows b;
+    if (op.rows.strided()) {  // as the engine: destination rows, never with a window, co-aligned in bf16 bytes
+      if (!op.win.whole() || !op.rows.valid() || !op.rows.to_bf16_bytes(&b)) return ErrorCode::INVALID_ARGUMENT;
+      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), 2 * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+    }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
@@ -1679,7 +1767,13 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       continue;
     }
     if (ec != ErrorCode::OK) return ec;
-    if (op.win.whole()) {
+    if (op.rows.strided()) {  // as the kernel's scattering store: the unpacked elements, stored into their rows
+      std::vector<uint16_t> wide(op.n_elems);
+      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
+      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) {
+        std::memcpy(static_cast<uint16_t*>(op.wide) + at, wide.data() + x, 2 * n);
+      });
+    } else if (op.win.whole()) {
       mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
     } else {  // as the kernel does: the whole object is read and verified, only the window stored
       std::vector<uint16_t> wide(op.n_elems);

@@ -62,8 +62,10 @@ struct DeviceShardOp {
   // The base `win` goes with, given the object's: dev_ptrs[item] is where object byte 0 lands, or for a strided get where
   // the result's row 0 lands.
   void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(obj_offset); }
-  // Put: where the shard's bytes are read from (common/store_window.h), the object's source rows rebased to obj_offset, and
-  // rows_at, where the shard's pattern row 0 starts relative to dev_ptrs[item].  The default is a contiguous source.
+  // Where the shard's bytes sit in the caller's strided memory (common/store_window.h): a put's source rows, or a get's
+  // destination rows (a get into a sliced tensor), the object's rows rebased to obj_offset; rows_at is where the shard's
+  // pattern row 0 starts relative to dev_ptrs[item].  The default is contiguous memory.  A get op never has both a
+  // pattern and a window.
   SourceRows rows;
   uint64_t rows_at = 0;
   const void* src(const void* obj_base) const {
@@ -80,8 +82,9 @@ struct DeviceFp8Op {
   // Get: the elements that are stored (common/store_window.h); the whole packed object is still read and verified.  The
   // default is the whole object.
   StoreWindow win;
-  // Put: the source rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts.  The packed
-  // object is one shard, so the pattern is the object's own.  The default is a contiguous source.
+  // The bf16 side's rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts: a put's source
+  // rows, or a get's destination rows (never together with a window).  The packed object is one shard, so the pattern is
+  // the object's own.  The default is contiguous memory.
   SourceRows rows;
 };
 
@@ -112,6 +115,10 @@ class DeviceTransport {
   virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
   // Staging copies for objects (or shards) that live on host tiers: device <-> host buffer, synchronous.
   virtual ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
+  // `rows` rows of `width` bytes, packed back to back at `host`, into row r = dev + r * pitch: one copy however many rows.
+  virtual ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) {
+    return ErrorCode::NOT_IMPLEMENTED;
+  }
   virtual ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
 };
 
@@ -183,6 +190,18 @@ class BlackbirdClient {
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
                                                       const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
                                                       const std::vector<uint64_t>& rows, void* stream);
+  // Gets of packed tensors into sliced bf16 tensors the caller owns: object i (n_elems[i] elements) is unpacked into rows[i]
+  // rows of elem_widths[i] elements, row r at bf16_ptrs[i] + 2 * r * elem_pitches[i] (SourceRows in common/store_window.h,
+  // in elements), by the scattering store of the fused unpack.  No element outside the rows is ever written.  Fail-over
+  // and the placement refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT unless rows[i] * elem_widths[i] ==
+  // n_elems[i], or for elem_widths[i] > elem_pitches[i] with rows[i] > 1; VALUE_OUT_OF_RANGE when a product overflows;
+  // NOT_IMPLEMENTED when the object is not fusable (as batch_get_device_fp8), or unless bf16_ptrs[i] is 16-byte aligned
+  // and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is no host-staged path; the rest of the
+  // batch keeps the fused launch.  rows[i] == 1 or elem_widths[i] == elem_pitches[i] is batch_get_device_fp8.
+  std::vector<ErrorCode> batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                      const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
+                                                      const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
+                                                      void* stream);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -234,6 +253,20 @@ class BlackbirdClient {
   std::vector<ErrorCode> batch_get_device_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                   const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
                                                   const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, void* stream);
+  // Gets into strided destinations (a slice of a tensor the caller owns, `cache[layer, :, slot]`, `W[:, k0:k1]`): object i
+  // lands in rows[i] rows of widths[i] bytes, row r at dev_ptrs[i] + r * pitches[i] (SourceRows in common/store_window.h),
+  // object byte x at row x / widths[i], column x % widths[i].  The capacity is rows[i] * widths[i]: a larger object is
+  // BUFFER_OVERFLOW, a shorter one fills its bytes in row order; out_sizes[i] receives the size.  No byte outside the
+  // object's bytes of the rows is ever written.  Every shard is read whole and verified, with fail-over and the placement
+  // refresh of batch_get_device.  The fused path scatters the rows in the get kernel; it needs dev_ptrs[i] 16-byte aligned,
+  // for rows[i] > 1 (pitches[i] - widths[i]) % 16 == 0, and every shard start 16-byte aligned.  Any other item, and every
+  // placement the fabric cannot reach, is staged through the host (one 2-D H2D copy of the rows) while the rest of the
+  // batch keeps the fused launch.  Per object, before anything is read: INVALID_ARGUMENT for widths[i] > pitches[i] with
+  // rows[i] > 1; VALUE_OUT_OF_RANGE when the size or the extent overflows.  rows[i] == 1 or widths[i] == pitches[i] is
+  // exactly batch_get_device with capacity rows[i] * widths[i].
+  std::vector<ErrorCode> batch_get_device_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                  const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                                  const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }
@@ -255,9 +288,10 @@ class BlackbirdClient {
   // Reads the object into dst[0, size) from the first copy that verifies: every shard, or with a window only those that
   // hold a byte it stores (whole, and verified).  The other bytes of dst are left as they are.
   ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, const StoreWindow& win = {});
-  // batch_get_device, batch_get_device_range and batch_get_device_strided: `ranges` null = whole objects into buffers of
-  // `capacity`, else object i's rows into dev_ptrs[i] (capacity[i] = rows * length, for the chunk plan).  A range is the
-  // single row `rows == 1`.
+  // batch_get_device, batch_get_device_range, batch_get_device_strided and batch_get_device_scatter: `ranges` null = whole
+  // objects into buffers of `capacity`, else object i's rows into dev_ptrs[i] (capacity[i] = rows * length, for the chunk
+  // plan).  A range is the single row `rows == 1`.  `rows` (whole objects only) null = contiguous buffers, else object i
+  // lands in (*rows)[i], row 0 at dev_ptrs[i].
   struct ByteRange {
     uint64_t offset = 0, length = 0;
     uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)
@@ -266,17 +300,20 @@ class BlackbirdClient {
   std::vector<ErrorCode> put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs, const std::vector<size_t>& sizes,
                                     const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
-                                    const std::vector<ByteRange>* ranges, void* stream, std::vector<size_t>* out_sizes);
+                                    const std::vector<ByteRange>* ranges, const std::vector<SourceRows>* rows, void* stream,
+                                    std::vector<size_t>* out_sizes);
   // batch_put_device_fp8 and batch_put_device_fp8_strided: `rows` null = contiguous tensors, else object i is read by
   // (*rows)[i], in elements.
   std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows, const WorkerConfig& cfg,
                                         void* stream);
-  // batch_get_device_fp8, batch_get_device_fp8_range and batch_get_device_fp8_strided: `ranges` null = whole tensors, else
-  // object i's rows (offset, length and pitch in elements) into bf16_ptrs[i].
+  // batch_get_device_fp8, batch_get_device_fp8_range, batch_get_device_fp8_strided and batch_get_device_fp8_scatter:
+  // `ranges` null = whole tensors, else object i's rows (offset, length and pitch in elements) into bf16_ptrs[i]; `rows`
+  // (whole tensors only) null = contiguous destinations, else object i lands in (*rows)[i], in elements.
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
-                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges, void* stream);
-  // The six shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
+                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
+                                        const std::vector<SourceRows>* rows, void* stream);
+  // The eight shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
   template <class Shape, class Run>
   std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);
   template <class Reissue>
@@ -331,6 +368,10 @@ class HostLoopbackTransport : public DeviceTransport {
   uint64_t launches() const override { return launches_; }
   ErrorCode copy_h2d(void* dev, const void* host, size_t n, void*) override {
     std::memcpy(dev, host, n);
+    return ErrorCode::OK;
+  }
+  ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void*) override {
+    for (size_t r = 0; r < rows; ++r) std::memcpy(static_cast<uint8_t*>(dev) + r * pitch, static_cast<const uint8_t*>(host) + r * width, width);
     return ErrorCode::OK;
   }
   ErrorCode copy_d2h(void* host, const void* dev, size_t n, void*) override {

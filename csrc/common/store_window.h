@@ -10,7 +10,8 @@
 //                                              and pattern row 0 is result row `row` (negative when the window starts later).
 // The default window, [0, UINT64_MAX) without a pattern, is the whole object.
 //
-// SourceRows, below, is the put side's counterpart: where each byte of an object is read from a strided source.
+// SourceRows, below, maps a dense object onto strided memory instead: where a put reads each byte from, or where a get into
+// a sliced destination stores it.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -145,17 +146,18 @@ struct StoreWindow {
   }
 };
 
-// SourceRows: where a device put reads each byte of an object from, when the source is rows of `width` bytes every `pitch`
-// bytes (a slice of a larger tensor).  It is the inverse of a strided StoreWindow, which maps a strided object onto a dense
-// destination: here the object is dense and the source strided.  This is the one statement of the rule; the transfer
-// engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and
-// the kernels' XFER_GATHER descriptors (kernels/xfer.h) all follow it.  The unit is a byte, or for an MXFP8 put an element
-// of the bf16 source (to_bf16_bytes() turns elements into bf16 bytes).
+// SourceRows: where each byte of a dense object sits in strided memory, rows of `width` bytes every `pitch` bytes (a slice
+// of a larger tensor), on either side of a transfer: the source a device put reads from, or the destination a device get
+// stores into.  It is the inverse of a strided StoreWindow, which maps a strided object onto a dense destination: here the
+// object is dense and the memory strided.  This is the one statement of the rule; the transfer engine (XferItem, Fp8Item),
+// the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and the kernels' XFER_GATHER and
+// XFER_SCATTER descriptors (kernels/xfer.h) all follow it.  The unit is a byte, or for an MXFP8 transfer an element of the
+// bf16 side (to_bf16_bytes() turns elements into bf16 bytes).
 //
-// With `src` where the pattern's row 0 starts, object byte x is read from
+// With `src` where the pattern's row 0 starts, object byte x is read from (put) or stored at (get)
 //   src + ((x + phase) / width) * pitch + (x + phase) % width
-// so the rows are read back to back and the object holds no gaps.  pitch == 0 (the default) is a contiguous source: byte x
-// at src + x.
+// so the rows are read or written back to back and the object holds no gaps.  pitch == 0 (the default) is contiguous
+// memory: byte x at src + x.
 struct SourceRows {
   uint64_t pitch = 0, width = 0, phase = 0;
 
@@ -214,6 +216,18 @@ struct SourceRows {
     if (!strided()) return src % 16 == 0;
     if (len > 0 && (len - 1 + phase) / width > 0 && (pitch - width) % 16) return false;
     return (src + phase) % 16 == 0;
+  }
+
+  // The client's rule for whether a device get into these rows (in bytes; an MXFP8 get's after to_bf16_bytes()), row 0 at
+  // `dst`, may take the fused path as far as the shard [off, off + len) of a copy goes; the get is fused only if every shard
+  // of every copy passes.  The shard's rows must be co-aligned from where it starts, and the gap a multiple of 16 bytes
+  // even where the shard holds a single row, so that whether a get is fused depends on its own shape and pointer, not on
+  // where the placement happened to cut the object (as StoreWindow::fused_get_aligned).
+  bool fused_get_aligned(uintptr_t dst, uint64_t off, uint64_t len) const {
+    if (strided() && (pitch - width) % 16) return false;
+    uint64_t at = 0;
+    const SourceRows r = rebase(off, &at);
+    return r.coaligned(dst + at, len);
   }
 
   // Calls f(x, at, n) for every run of n contiguous source bytes of object bytes [0, len): object bytes [x, x + n) are read

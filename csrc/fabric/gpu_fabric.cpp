@@ -514,6 +514,16 @@ ErrorCode GpuFabric::copy_h2d(void* dev, const void* host, size_t n, void* strea
   return ErrorCode::OK;
 }
 
+ErrorCode GpuFabric::copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) {
+  if (rows == 0 || width == 0) return ErrorCode::OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice") ||
+      !cuda_ok(cudaMemcpy2DAsync(dev, pitch, host, width, width, rows, cudaMemcpyHostToDevice, st), "H2D rows") ||
+      !cuda_ok(cudaStreamSynchronize(st), "sync"))
+    return ErrorCode::FABRIC_ERROR;
+  return ErrorCode::OK;
+}
+
 ErrorCode GpuFabric::copy_d2h(void* host, const void* dev, size_t n, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice") || !cuda_ok(cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, st), "D2H") ||
@@ -641,8 +651,9 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.wide = op.wide;
     it.packed = d.value();
     it.n_elems = op.n_elems;
-    it.win = op.win;    // a window on a put is refused by the engine
-    it.rows = op.rows;  // and source rows on a get
+    it.win = op.win;  // a window on a put is refused by the engine
+    if (unpack) it.dst_rows = op.rows;  // the rows are the destination's on a get, the source's on a put
+    else it.rows = op.rows;
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;
@@ -700,6 +711,11 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
       it.dst[0] = op.dst(dev_ptrs[op.item]);
       it.win = op.win;
       it.win.hi = std::min(op.win.hi, it.nbytes);
+    }
+    if (op.rows.strided()) {  // a get into a strided destination: the shard's rows start at rows_at
+      it.flags |= XFER_SCATTER;
+      it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.rows_at;
+      it.dst_rows = op.rows;
     }
     items->push_back(it);
     op_of_item->push_back(k);

@@ -86,6 +86,7 @@ class GpuFabric : public client::DeviceTransport {
   ErrorCode put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override;
   ErrorCode get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override;
   ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) override;
+  ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) override;
   ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) override;
 
   // Re-reads the pool registry from the keystone and maps any new GPU slab.

@@ -77,13 +77,14 @@ struct XferEngine::Slot {
   bool crc = false;
   uint64_t empty_digest = 0;
   std::vector<int32_t> item_to_desc;  // -1 for zero-size items
-  // per descriptor up to the last XFER_STRIDED or XFER_GATHER one; empty when the batch has none
+  // per descriptor up to the last XFER_STRIDED, XFER_GATHER or XFER_SCATTER one; empty when the batch has none
   std::vector<XferStride> strides;
   void set_stride(uint32_t k, const XferStride& e) {
     if (strides.size() <= k) strides.resize(k + 1, XferStride{1, 1, 0});
     strides[k] = e;
   }
   void set_stride(uint32_t k, const StoreWindow& w) { set_stride(k, XferStride{w.pitch, w.width, w.phase}); }
+  void set_stride(uint32_t k, const SourceRows& r) { set_stride(k, XferStride{r.pitch, r.width, r.phase}); }
   // Writes the stride table behind tile_start when the batch has a strided descriptor, and returns the bytes of the
   // table to copy to the device: [descs | tile_start | strides], or without the strides.
   size_t write_strides(uint32_t nd) {
@@ -325,10 +326,15 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const bool win = it.flags & XFER_WINDOW;
     const bool strided = it.flags & XFER_STRIDED;
     const bool gather = it.flags & XFER_GATHER;
+    const bool scatter = it.flags & XFER_SCATTER;
     if ((strided && !win) || (win && (strided != it.win.strided() || !it.win.valid(it.nbytes) || it.ndst != 1 ||
                                       (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     if (gather != it.rows.strided() || (gather && (!it.rows.valid() || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM)))))
+      return ErrorCode::INVALID_ARGUMENT;
+    if (scatter != it.dst_rows.strided() ||
+        (scatter && (!it.dst_rows.valid() || it.ndst != 1 ||
+                     (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
@@ -338,14 +344,16 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       s->empties.push_back({static_cast<uint32_t>(i), it.flags, it.expect});
       continue;
     }
-    // windowed items (strided ones included) and gathered ones always take bb_xfer: neither the warp-per-object kernel nor
-    // the mailbox has a store window or a gathering load
-    all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW | XFER_GATHER)) && it.ndst >= 1;
+    // windowed items (strided ones included), gathered and scattered ones always take bb_xfer: neither the warp-per-object
+    // kernel nor the mailbox has a store window, a gathering load or a scattering store
+    all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW | XFER_GATHER | XFER_SCATTER)) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
     uintptr_t al = gather ? 0 : reinterpret_cast<uintptr_t>(it.src);  // gathered: source rows instead
-    for (uint32_t r = strided ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);  // strided: rows instead
+    // strided and scattered: rows instead
+    for (uint32_t r = strided || scatter ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
     if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]))) ||
-        (gather && !it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes)))
+        (gather && !it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes)) ||
+        (scatter && !it.dst_rows.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]), it.nbytes)))
       return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
@@ -358,7 +366,8 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       d.win.hi = w.hi;
       if (strided) s->set_stride(nd, w);
     }
-    if (gather) s->set_stride(nd, XferStride{it.rows.pitch, it.rows.width, it.rows.phase});
+    if (gather) s->set_stride(nd, it.rows);
+    if (scatter) s->set_stride(nd, it.dst_rows);
     d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;
@@ -571,13 +580,16 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
     const bool gather = it.rows.strided();
+    const bool scatter = it.dst_rows.strided();
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
-    SourceRows rows;  // a gathered put's source rows in bf16 bytes
+    SourceRows rows;  // a gathered put's source rows, or a scattered get's destination rows, in bf16 bytes
     if (gather && (unpack || !it.rows.valid() || !it.rows.to_bf16_bytes(&rows))) return ErrorCode::INVALID_ARGUMENT;
+    if (scatter && (!unpack || gather || !it.win.whole() || !it.dst_rows.valid() || !it.dst_rows.to_bf16_bytes(&rows)))
+      return ErrorCode::INVALID_ARGUMENT;
     // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
     // first element after row 0's start): the rows are checked instead
-    if (((strided || gather ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
-        (gather && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), 2 * it.n_elems)))
+    if (((strided || gather || scatter ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
+        ((gather || scatter) && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), 2 * it.n_elems)))
       return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
@@ -609,9 +621,9 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       d.flags |= XFER_STRIDED;
       s->set_stride(i, w);
     }
-    if (gather) {  // d.src is the pattern's row 0
-      d.flags |= XFER_GATHER;
-      s->set_stride(i, XferStride{rows.pitch, rows.width, rows.phase});
+    if (gather || scatter) {  // d.src (gather) or d.dst[0] (scatter) is the pattern's row 0
+      d.flags |= gather ? XFER_GATHER : XFER_SCATTER;
+      s->set_stride(i, rows);
     }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice

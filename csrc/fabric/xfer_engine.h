@@ -35,6 +35,11 @@ struct XferItem {
   // has a pattern.  INVALID_ARGUMENT for an invalid pattern, or one with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM;
   // INVALID_ADDRESS unless rows.coaligned(src, nbytes), which replaces the 16-byte alignment check of src.
   SourceRows rows;
+  // Get into a strided destination, the same rule on the other side: dst[0] is where the pattern's row 0 starts;
+  // XFER_SCATTER exactly when it has a pattern.  INVALID_ARGUMENT for an invalid pattern, or one with XFER_WINDOW,
+  // XFER_STRIDED, XFER_GATHER, XFER_MULTIMEM, XFER_RAW_SUM or ndst != 1; INVALID_ADDRESS unless
+  // dst_rows.coaligned(dst[0], nbytes), which replaces the 16-byte alignment check of dst[0].
+  SourceRows dst_rows;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span
@@ -63,6 +68,11 @@ struct Fp8Item {
   // pattern on an unpack, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned
   // in bf16 bytes, which replaces the 16-byte alignment check of `wide`.
   SourceRows rows;
+  // Unpack only: the destination rows in elements, `wide` being where the pattern's row 0 starts; the default is a
+  // contiguous destination.  run_fp8 sets XFER_SCATTER exactly when it has a pattern.  INVALID_ARGUMENT for a pattern on a
+  // pack, with a window, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned in
+  // bf16 bytes, which replaces the 16-byte alignment check of `wide`.
+  SourceRows dst_rows;
 };
 
 struct XferResult {

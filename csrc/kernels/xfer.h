@@ -36,6 +36,13 @@ enum XferFlags : uint32_t {
   // XFER_RAW_SUM; with 1-3 destinations or XFER_MULTIMEM.  The tile in shared memory is byte for byte the tile of the
   // dense object, so the digest and the stored bytes are those of a put of the compacted rows.
   XFER_GATHER = 1u << 5,
+  // Scattering store (gets into a strided destination), the mirror of XFER_GATHER, in bb_xfer and the fused MXFP8 get: the
+  // same SourceRows rule applied to the destination, so dst[0] is where the pattern's row 0 starts and object byte x is
+  // stored at dst[0] + ((x + phase) / width) * pitch + (x + phase) % width.  The pattern is the descriptor's entry of the
+  // launch's XferStride table; the MXFP8 get counts all of it in bf16 bytes of the destination.  Only with ndst == 1; never
+  // with XFER_WINDOW, XFER_STRIDED, XFER_GATHER, XFER_MULTIMEM or XFER_RAW_SUM.  The tile in shared memory is the object's
+  // tile, so the digest and the verify are those of a plain get.
+  XFER_SCATTER = 1u << 6,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -67,7 +74,8 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 // phase == 0 it stores exactly the plain window.  Every stored row must be co-aligned with the tile (the destination of
 // object byte x congruent to x mod 16), so that the kernel only bulk-stores 16-byte congruent spans.  An XFER_GATHER
 // descriptor's entry is its source rows instead: 0 < width <= pitch, phase < width, and the source of object byte x
-// congruent to x mod 16 (SourceRows::coaligned).
+// congruent to x mod 16 (SourceRows::coaligned).  An XFER_SCATTER descriptor's entry is its destination rows, under the
+// same rules.
 struct XferStride {
   uint64_t pitch, width, phase;
 };
@@ -95,7 +103,7 @@ struct XferLaunch {
   // kernel parameters instead (descs / tile_start may then be null).
   const XferDesc* host_descs = nullptr;
   const uint32_t* host_tile_start = nullptr;
-  // Row patterns of the XFER_STRIDED and XFER_GATHER descriptors, one entry per descriptor (the entries of unflagged
+  // Row patterns of the XFER_STRIDED, XFER_GATHER and XFER_SCATTER descriptors, one entry per descriptor (the entries of unflagged
   // descriptors are never read); null when the batch has none.  host_strides is their copy for the kernel parameters of an
   // inline batch.
   const XferStride* strides = nullptr;
@@ -161,7 +169,8 @@ int xfer_smem_bytes(int algo);
 // follow the payload), nbytes = payload bytes (= elements, a multiple of kTileBytes); unpack (get): src = base of the
 // packed object, dst[0] = bf16 destination (where element 0 lands); an unpack descriptor may carry XFER_WINDOW, whose
 // `win` is then in bf16 bytes of the object ([2 * first element, 2 * end element)), and XFER_STRIDED, whose pattern in
-// `strides` (a device table; no inline copy) is in bf16 bytes too.  `sum_ws` receives the unfinalised BBH64 sum of the
+// `strides` (a device table; no inline copy) is in bf16 bytes too; or instead XFER_SCATTER, with dst[0] where the
+// destination pattern's row 0 starts and the pattern in bf16 bytes in `strides`.  `sum_ws` receives the unfinalised BBH64 sum of the
 // payload tiles per descriptor (must be zero on entry); descs / tile_start are device tables.
 int launch_xfer_fp8(const XferLaunch& l, bool unpack);
 int xfer_fp8_smem_bytes();

@@ -128,26 +128,37 @@ __device__ __forceinline__ TileSpan segment_span(uint64_t off, uint32_t x0, uint
 __device__ __forceinline__ uint64_t row_dst(uint64_t dst0, uint64_t off, uint64_t r, const XferStride& st) {
   return dst0 + off + st.phase - r * (st.pitch - st.width);
 }
-// The store warp's part of a strided tile: the row segments of the span [x0, x1) of `tile` (shared memory, object bytes
-// [off, off + ...)), one per lane (a tile can hold thousands of short rows), each as a TMA middle plus a byte-wise head and
-// tail.  dst0 is the descriptor's dst[0].  The calling lane still has to commit its bulk group and wait on it.
-__device__ __forceinline__ void store_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t x0, uint32_t x1,
-                                                   const XferStride& st, uint32_t lane) {
+// Calls f(r, g) for every row r of pattern `st` that the span [x0, x1) of a tile at object offset `off` holds, in part or
+// whole, g being that row's segment (segment_span); one row per lane (a tile can hold thousands of short rows).
+template <class F>
+__device__ __forceinline__ void for_row_segments(uint64_t off, uint32_t x0, uint32_t x1, const XferStride& st, uint32_t lane, F&& f) {
   const uint64_t r0 = first_row(off, x0, st);
   const uint32_t nrow = row_count(off, x0, x1, st);
   for (uint32_t k = lane; k < nrow; k += 32) {
     const uint64_t r = r0 + k;
-    const TileSpan g = segment_span(off, x0, x1, r, st);
-    uint8_t* d = reinterpret_cast<uint8_t*>(row_dst(dst0, off, r, st));
-    if (g.a1 > g.a0) ptx::bulk_s2g(d + g.a0, tile + g.a0, g.a1 - g.a0);
-    for (uint32_t o = g.x0; o < g.h1; ++o) d[o] = tile[o];
-    for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = tile[o];
+    f(r, segment_span(off, x0, x1, r, st));
   }
+}
+// Stores the tile bytes of segment g at d + o for tile byte o (d + o congruent to o mod 16): the TMA middle, then the head
+// and tail byte-wise.  The calling lane still has to commit its bulk group and wait on it.
+__device__ __forceinline__ void store_segment(uint8_t* d, const uint8_t* tile, const TileSpan& g) {
+  if (g.a1 > g.a0) ptx::bulk_s2g(d + g.a0, tile + g.a0, g.a1 - g.a0);
+  for (uint32_t o = g.x0; o < g.h1; ++o) d[o] = tile[o];
+  for (uint32_t o = g.tb; o < g.x1; ++o) d[o] = tile[o];
+}
+// The store warp's part of a strided tile: the row segments of the span [x0, x1) of `tile` (shared memory, object bytes
+// [off, off + ...)), one per lane, each as a TMA middle plus a byte-wise head and tail.  dst0 is the descriptor's dst[0].
+__device__ __forceinline__ void store_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t x0, uint32_t x1,
+                                                   const XferStride& st, uint32_t lane) {
+  for_row_segments(off, x0, x1, st, lane, [&](uint64_t r, const TileSpan& g) {
+    store_segment(reinterpret_cast<uint8_t*>(row_dst(dst0, off, r, st)), tile, g);
+  });
 }
 // Gathering load (XFER_GATHER, source rows `st`), the mirror of the strided store: a tile at object offset `off` of `bytes`
 // bytes holds rows first_row(...) .. + row_count(...) - 1 of the object's own dense layout {width, width, phase}, and tile
 // byte o of row r is read from row_src(...) + o.  With co-aligned rows that address is congruent to o mod 16, so each row
-// segment splits into TMA middle, head and tail exactly like a store segment.
+// segment splits into TMA middle, head and tail exactly like a store segment.  The scattering store (XFER_SCATTER) is the
+// same map with the rows on the destination side: tile byte o of row r is stored at row_src(dst0, ...) + o.
 __device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t r, const XferStride& st) {
   return src + off + st.phase + r * (st.pitch - st.width);
 }
@@ -157,13 +168,8 @@ __device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t
 // shared stores for the async proxy.
 __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t* bar, uint64_t src, uint64_t off, uint32_t bytes,
                                                         const XferStride& st, uint32_t lane) {
-  const XferStride dense{st.width, st.width, st.phase};
-  const uint64_t r0 = first_row(off, 0, dense);
-  const uint32_t nrow = row_count(off, 0, bytes, dense);
   uint32_t tx = 0;
-  for (uint32_t k = lane; k < nrow; k += 32) {
-    const uint64_t r = r0 + k;
-    const TileSpan g = segment_span(off, 0, bytes, r, dense);
+  for_row_segments(off, 0, bytes, XferStride{st.width, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
     const uint8_t* s = reinterpret_cast<const uint8_t*>(row_src(src, off, r, st));
     if (g.a1 > g.a0) {
       ptx::bulk_g2s(tile + g.a0, s + g.a0, g.a1 - g.a0, bar);
@@ -171,8 +177,18 @@ __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t*
     }
     for (uint32_t o = g.x0; o < g.h1; ++o) tile[o] = s[o];
     for (uint32_t o = g.tb; o < g.x1; ++o) tile[o] = s[o];
-  }
+  });
   return tx;
+}
+// The store warp's part of a scattered tile (XFER_SCATTER, destination rows `st`), the mirror of gather_row_segments: the
+// tile's `bytes` object bytes from `off`, in the object's dense layout {width, width, phase}, one row segment per lane,
+// each stored at row_src(dst0, ...) as a TMA middle plus a byte-wise head and tail.  dst0 is the descriptor's dst[0], where
+// the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.
+__device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t bytes,
+                                                     const XferStride& st, uint32_t lane) {
+  for_row_segments(off, 0, bytes, XferStride{st.width, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    store_segment(reinterpret_cast<uint8_t*>(row_src(dst0, off, r, st)), tile, g);
+  });
 }
 // The row pattern of descriptor `i` from a device table (read-only path).
 __device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i) {

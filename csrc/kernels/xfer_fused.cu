@@ -13,7 +13,9 @@
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
 //                      to an NVLS multicast address (one store, N replicas).  A store window (XFER_WINDOW) cuts
-//                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.
+//                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.  A
+//                      scattering store (XFER_SCATTER: a get into a strided destination) stores the whole tile as
+//                      the row segments of the destination rows, one per lane.
 //   warp 3  finalizer: folds the per-tile partials into per-object digests in registers; an
 //                      object that lives entirely inside this CTA's run is finalised with no
 //                      global atomics; only the <=2 objects straddling a CTA boundary use them.
@@ -144,7 +146,8 @@ struct Params {
   uint32_t use_inline;
   uint32_t inl_tile_start[kInlineDescs + 1];
   XferDesc inl_descs[kInlineDescs];
-  // Row patterns of XFER_STRIDED descriptors (XferLaunch::strides), and their copy for inline batches.
+  // Row patterns of XFER_STRIDED, XFER_GATHER and XFER_SCATTER descriptors (XferLaunch::strides), and their copy for
+  // inline batches.
   const XferStride* strides;
   XferStride inl_strides[kInlineDescs];
 };
@@ -335,17 +338,19 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
       const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kTileBytes;
       const uint32_t ndst = m.ndst_flags & 0xFFu;
       const uint32_t flags = m.ndst_flags >> 8;
-      const bool strided = flags & XFER_STRIDED;
+      const bool strided = flags & (XFER_STRIDED | XFER_SCATTER);
       // the whole tile, or its part inside the window [dst[1], dst[2]) (object offsets)
       const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, m.bytes, flags & XFER_WINDOW, m.dst[1], m.dst[2]);
       if (strided) {
-        // one row segment per lane (a tile can hold thousands of short rows): TMA middle, head and tail byte-wise
+        // one row segment per lane (a tile can hold thousands of short rows): TMA middle, head and tail byte-wise; a
+        // strided window's rows, or the destination rows of a scattering store
         if (m.desc != st_desc) {
           st_desc = m.desc;
           if (p.use_inline) st = p.inl_strides[st_desc];
           else st = load_stride(p.strides, st_desc);
         }
-        store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);
+        if (flags & XFER_SCATTER) scatter_row_segments(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
+        else store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);
       } else if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);
         for (uint32_t o = a0 + lane * 16; o < a1; o += 512)

@@ -16,6 +16,8 @@
 //                   whole object's, and tiles outside the window are not unpacked.  With XFER_STRIDED as well
 //                   (slices along an inner dimension) the store warp stores only the window's row segments, densely,
 //                   one per lane, by the same rule as bb_xfer; a tile wholly inside a gap between rows is still unpacked.
+//                   With XFER_SCATTER instead (gets into a sliced tensor) the store warp stores every 32 KiB bf16 tile
+//                   as the row segments of the destination rows, by the SourceRows rule in bf16 bytes, as bb_xfer does.
 //
 // The stored object keeps the layout of the unfused path ([E4M3 payload n][E8M0 scales n/32], common/mxfp8.h), and so
 // does its digest: BBH64 is a sum of per-tile terms, this kernel accumulates the payload tiles (tile index 0..T-1)
@@ -62,8 +64,9 @@ struct FpMeta {            // 64 bytes
   uint32_t obj_ntiles;
   uint32_t ndst;           // pack: replicas written by this pass (1..kMaxDst)
   uint32_t valid;          // payload bytes (= elements) of this tile: 16384, or the multiple-of-32 tail of the object
-  uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided; pack: XFER_GATHER when its
-                           // source is rows (the pattern in FpParams::strides either way)
+  uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
+                           // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
+                           // FpParams::strides either way)
   uint64_t pad;
 };
 static_assert(sizeof(FpMeta) == 64);
@@ -99,7 +102,7 @@ struct FpParams {
   uint32_t ndesc;
   uint32_t total_tiles;
   unsigned long long* sum_ws;  // [ndesc] raw BBH64 sums of the payload tiles (zero on entry)
-  const XferStride* strides;   // row patterns of the XFER_STRIDED (unpack) or XFER_GATHER (pack) descriptors
+  const XferStride* strides;   // row patterns of the XFER_STRIDED / XFER_SCATTER (unpack) or XFER_GATHER (pack) descriptors
                                // (XferLaunch::strides), else null
 };
 
@@ -150,7 +153,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED : XFER_GATHER);
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER : XFER_GATHER);
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
         // the packed object is [payload nbytes][scales nbytes/32]: a tile's scales sit (nbytes - ti*(16384-512)) past its payload
@@ -245,7 +248,9 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             pat_desc = m.desc;
             pat = load_stride(p.strides, pat_desc);
           }
-          store_row_segments(s.wide[st], m.dst[0] - off, off, x0, x1, pat, lane);  // m.dst[0] = dst[0] + off
+          // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile
+          if (m.strided & XFER_SCATTER) scatter_row_segments(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
+          else store_row_segments(s.wide[st], m.dst[0] - off, off, x0, x1, pat, lane);
         } else {
           if (lane == 0 && a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[0] + a0), &s.wide[st][a0], a1 - a0);
           const uint32_t o = lane < 16 ? x0 + lane : tb + (lane - 16u);

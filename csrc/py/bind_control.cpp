@@ -356,7 +356,7 @@ void bind_control(py::module_& m) {
   // ---------------------------------------------------------------- allocator
   using alloc::AllocationRequest;
   using alloc::AllocationResult;
-  py::class_<SourceRows>(m, "SourceRows", "Where a device put reads each object byte from a strided source (common/store_window.h).")
+  py::class_<SourceRows>(m, "SourceRows", "Where each byte of a dense object sits in strided memory: a device put's source, or a scattered get's destination (common/store_window.h).")
       .def(py::init([](uint64_t pitch, uint64_t width, uint64_t phase) { return SourceRows{pitch, width, phase}; }), py::arg("pitch") = 0,
            py::arg("width") = 0, py::arg("phase") = 0)
       .def_readonly("pitch", &SourceRows::pitch)
@@ -1221,6 +1221,19 @@ void bind_control(py::module_& m) {
            "[elem_offsets[i] + r * elem_pitches[i], + elem_widths[i]), unpacked to bf16 densely at bf16_ptrs[i] (row r at "
            "bf16_ptrs[i] + 2 * r * elem_widths[i]); the whole packed object is read and verified; returns one ErrorCode per "
            "object (NOT_IMPLEMENTED: read it whole and narrow).")
+      .def("batch_get_device_fp8_scatter",
+           [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
+              const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, uintptr_t stream) {
+             return ecs_to_py(nogil([&] {
+               return c.batch_get_device_fp8_scatter(keys, to_ptrs<void*>(ptrs), n_elems, widths, pitches, rows, reinterpret_cast<void*>(stream));
+             }));
+           },
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_widths"), py::arg("elem_pitches"), py::arg("rows"),
+           py::arg("stream") = 0,
+           "Packed tensor i (n_elems[i] == rows[i] * elem_widths[i] elements), unpacked to bf16 into rows[i] rows of "
+           "elem_widths[i] elements, row r at bf16_ptrs[i] + 2 * r * elem_pitches[i]; the whole packed object is read and "
+           "verified, no element outside the rows is written; returns one ErrorCode per object (NOT_IMPLEMENTED: get it "
+           "whole and copy).")
       .def("device_fp8_eligible", &BlackbirdClient::device_fp8_eligible)
       .def("batch_put", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<py::buffer>& data, const WorkerConfig& cfg) {
         std::vector<const uint8_t*> ptrs;
@@ -1286,6 +1299,18 @@ void bind_control(py::module_& m) {
          "rows[i] rows of widths[i] bytes of object i, row r = bytes [offsets[i] + r * pitches[i], + widths[i]), densely into "
          "dev_ptrs[i] (row r at dev_ptrs[i] + r * widths[i]); every shard holding a stored byte is read whole and verified; "
          "returns one ErrorCode per object.")
+      .def("batch_get_device_scatter", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+                                          const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+                                          const std::vector<uint64_t>& rows, uintptr_t stream) {
+        std::vector<size_t> sizes;
+        const auto ecs = nogil([&] {
+          return c.batch_get_device_scatter(keys, to_ptrs<void*>(ptrs), widths, pitches, rows, reinterpret_cast<void*>(stream), &sizes);
+        });
+        return py::make_tuple(ecs_to_py(ecs), sizes);
+      }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("widths"), py::arg("pitches"), py::arg("rows"), py::arg("stream") = 0,
+         "Object i into rows[i] rows of widths[i] bytes, row r at dev_ptrs[i] + r * pitches[i] (capacity rows[i] * "
+         "widths[i]); every shard is read whole and verified, no byte outside the rows is written; returns (one ErrorCode "
+         "per object, object sizes).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

@@ -44,19 +44,22 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
-// A put's gather pattern (common/store_window.h) given as (pitch, width, phase).
+// A gather or scatter pattern (common/store_window.h) given as (pitch, width, phase).
 SourceRows to_rows(const py::handle& h) {
   auto g = h.cast<std::vector<uint64_t>>();
-  if (g.size() != 3) throw py::value_error("gather = (pitch, width, phase)");
+  if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
   return {g[0], g[1], g[2]};
 }
-// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None).  An empty destination
-// list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets XFER_WINDOW, and
-// one with a pattern XFER_STRIDED as well.  A gather pattern (pitch, width, phase) sets XFER_GATHER, with src = row 0.
+// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None).  An
+// empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets
+// XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern (pitch, width, phase) sets XFER_GATHER, with
+// src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.
 XferItem to_item(const py::handle& h) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 8)
-    throw py::value_error("xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, (pitch, width, phase)]]]]])");
+  if (t.size() < 3 || t.size() > 9)
+    throw py::value_error(
+        "xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, gather (pitch, width, phase)[, scatter "
+        "(pitch, width, phase)]]]]]])");
   XferItem it;
   it.src = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
   it.ndst = to_ptrs(t[1], it.dst);
@@ -68,6 +71,10 @@ XferItem to_item(const py::handle& h) {
   if (t.size() > 7 && !t[7].is_none()) {
     it.rows = to_rows(t[7]);
     it.flags |= XFER_GATHER;
+  }
+  if (t.size() > 8 && !t[8].is_none()) {
+    it.dst_rows = to_rows(t[8]);
+    it.flags |= XFER_SCATTER;
   }
   return it;
 }
@@ -81,6 +88,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_WINDOW") = static_cast<uint32_t>(XFER_WINDOW);
   m.attr("XFER_STRIDED") = static_cast<uint32_t>(XFER_STRIDED);
   m.attr("XFER_GATHER") = static_cast<uint32_t>(XFER_GATHER);
+  m.attr("XFER_SCATTER") = static_cast<uint32_t>(XFER_SCATTER);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -116,7 +124,9 @@ void bind_gpu(py::module_& m) {
            "ChecksumAlgo.NONE only the window's 16-byte aligned span is read).  A window (lo, hi, pitch, width, phase) also "
            "sets XFER_STRIDED: of [lo, hi), byte x is stored iff c = (x + phase) % pitch < width, at dst + ((x + phase) // "
            "pitch) * width + c.  A gather pattern (pitch, width, phase) as the eighth element sets XFER_GATHER: object byte x "
-           "is read from src + ((x + phase) // width) * pitch + (x + phase) % width; returns (digests, status, device_ms).")
+           "is read from src + ((x + phase) // width) * pitch + (x + phase) % width.  A scatter pattern (pitch, width, phase) "
+           "as the ninth element (the slots before it may be None) sets XFER_SCATTER: object byte x is stored at dst + ((x + "
+           "phase) // width) * pitch + (x + phase) % width; returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
              std::vector<gpu::Fp8Item> v;
@@ -131,11 +141,14 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 6)
-                 throw py::value_error("fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, (pitch, width, phase)]]])");
+               if (t.size() < 3 || t.size() > 7)
+                 throw py::value_error(
+                     "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
+                     "scatter (pitch, width, phase)]]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 5 && !t[5].is_none()) it.rows = to_rows(t[5]);
+               if (t.size() > 6 && !t[6].is_none()) it.dst_rows = to_rows(t[6]);
                v.push_back(it);
              }
              XferResult res;
@@ -160,7 +173,9 @@ void bind_gpu(py::module_& m) {
            "pattern's row 0 starts, and the packed object and its digest are those of the compacted rows; INVALID_ARGUMENT "
            "for a pattern on a get, width == 0, width > pitch, phase >= width or pitch >= 2^62, INVALID_ADDRESS unless "
            "bf16_ptr + 2 * phase is 16-byte aligned and, when the object spans more than one row, (pitch - width) % 8 == 0.  "
-           "Returns (digests of the packed objects, status, device_ms).")
+           "A get's scatter pattern (pitch, width, phase), in elements, as the seventh element stores into rows by the same "
+           "rule, element x at bf16_ptr + 2 * ((x + phase) // width * pitch + (x + phase) % width), under the same rules; "
+           "INVALID_ARGUMENT on a put or with a window.  Returns (digests of the packed objects, status, device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
