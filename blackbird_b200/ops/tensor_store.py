@@ -2,8 +2,8 @@
 
     store = TensorStore(cluster.client)
     store.batch_put(["act/0", "act/1"], [t0, t1])                  # BBH64 digest fused into the copy
-    store.put("kv/layer3", kv_bf16, pack_fp8=True)                  # block-scaled MXFP8 on the wire / in the slab
-    t = store.get("kv/layer3")                                      # verified + unpacked bf16 tensor
+    store.put("kv/layer3", kv_fp16, pack_fp8=True)                  # block-scaled MXFP8 on the wire / in the slab
+    t = store.get("kv/layer3")                                      # verified + unpacked fp16 tensor
 
 Tensor metadata (dtype, shape, packing) travels in a small side object `<key>#meta`.
 """
@@ -18,6 +18,21 @@ from .. import _bb
 
 _DTYPES = {str(d).replace("torch.", ""): d for d in (torch.uint8, torch.int8, torch.int16, torch.int32, torch.int64, torch.float16,
                                                      torch.bfloat16, torch.float32, torch.float64, torch.bool)}
+# dtypes MXFP8 packing takes, and the wide type the kernels read / write them as
+_MX_WIDE = {torch.bfloat16: _bb.MxWide.BF16, torch.float16: _bb.MxWide.F16, torch.float32: _bb.MxWide.F32}
+
+
+def _stored_dtype(m) -> torch.dtype:
+    """The dtype a stored tensor is returned as: its own, packed or not (packed metas always record it)."""
+    return _DTYPES[m["dtype"]]
+
+
+def _by_dtype(idx, dtype_of) -> dict:
+    """idx grouped by dtype_of(i), in order: one native call per wide type."""
+    groups = {}
+    for i in idx:
+        groups.setdefault(dtype_of(i), []).append(i)
+    return groups
 
 
 class TensorStore:
@@ -36,9 +51,9 @@ class TensorStore:
 
     # ------------------------------------------------------------------ put
     def _fused_fp8_ok(self, t: torch.Tensor, cfg) -> bool:
-        """Pack fused into the put kernel: bf16, a whole number of 32-element MX blocks, up to 3 copies (one tile pass
-        fans out to every replica), each copy in one shard."""
-        return (t.dtype == torch.bfloat16 and self.client.device_fp8_eligible(t.numel()) and 1 <= cfg.replication_factor <= 3
+        """Pack fused into the put kernel: bf16, fp16 or fp32, a whole number of 32-element MX blocks, up to 3 copies (one
+        tile pass fans out to every replica), each copy in one shard."""
+        return (t.dtype in _MX_WIDE and self.client.device_fp8_eligible(t.numel()) and 1 <= cfg.replication_factor <= 3
                 and cfg.max_workers_per_copy == 1 and t.data_ptr() % 16 == 0)
 
     @staticmethod
@@ -72,13 +87,21 @@ class TensorStore:
     def batch_put(self, keys: Sequence[str], tensors: Sequence[torch.Tensor], pack_fp8: bool = False, config=None) -> None:
         """Stores each tensor under its key.  A slice of a larger CUDA tensor whose elements are rows -- `W[:, a:b]`, `kv[:,
         :, h0:h1, :]`, `t[::k]` -- is read in place by the fused put kernel (batch_put_device_strided) when its start is
-        16-byte aligned and its row gap a multiple of 16 bytes; no contiguous copy is made.  With pack_fp8 such a bf16
-        slice whose element count is a whole number of 32-element MX blocks is gathered the same way by the fused pack
-        kernel (batch_put_device_fp8_strided) when the config is fusable.  Other layouts are made contiguous first.  The
-        stored object is that of `t.contiguous()` either way."""
+        16-byte aligned and its row gap a multiple of 16 bytes; no contiguous copy is made.  With pack_fp8 such a slice
+        whose element count is a whole number of 32-element MX blocks is gathered the same way by the fused pack kernel
+        (batch_put_device_fp8_strided) when the config is fusable.  Other layouts are made contiguous first.  The stored
+        object is that of `t.contiguous()` either way.
+
+        pack_fp8 takes bf16, fp16 and fp32 tensors (TypeError for any other dtype, before anything is stored): each is
+        packed from its own values, with no bf16 copy, and gets return it in its own dtype.  A batch that mixes dtypes
+        makes one native call per dtype."""
         cfg = config or self.config
         keys = list(keys)
         tensors = list(tensors)
+        if pack_fp8:
+            bad = [(k, t.dtype) for k, t in zip(keys, tensors) if t.dtype not in _MX_WIDE]
+            if bad:
+                raise TypeError(f"MXFP8 packing takes bfloat16, float16 and float32 tensors, not {bad[:3]}")
         rows = [self._gatherable(t) for t in tensors]
         if pack_fp8:  # only slices the fused pack kernel can take are gathered
             rows = [r if r is not None and self._fused_fp8_ok(t, cfg) else None for t, r in zip(tensors, rows)]
@@ -86,27 +109,30 @@ class TensorStore:
         if pack_fp8:
             # objects the fused kernel can take go through batch_put_device_fp8 (bf16 read once, packed bytes on the
             # wire, digest of the packed object from the tensor cores); the rest are packed first (unfused path below)
-            fused = [i for i, t in enumerate(tensors) if t.is_cuda and self._fused_fp8_ok(t, cfg)]
-            if fused:
+            fused_all = [i for i, t in enumerate(tensors) if t.is_cuda and self._fused_fp8_ok(t, cfg)]
+            done = []
+            for dt, fused in _by_dtype(fused_all, lambda i: tensors[i].dtype).items():
                 fk = [keys[i] for i in fused]
                 ptrs = [tensors[i].data_ptr() for i in fused]
+                es, wide = tensors[fused[0]].element_size(), _MX_WIDE[dt]
                 if any(rows[i] is not None for i in fused):
                     # one call and one launch: contiguous tensors go as one row each; widths and pitches in elements
-                    shapes = [(rows[i][0] // 2, rows[i][1] // 2, rows[i][2]) if rows[i] is not None else (tensors[i].numel(),) * 2 + (1,)
+                    shapes = [(rows[i][0] // es, rows[i][1] // es, rows[i][2]) if rows[i] is not None else (tensors[i].numel(),) * 2 + (1,)
                               for i in fused]
                     ecs = self.client.batch_put_device_fp8_strided(fk, ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
-                                                                   [s[2] for s in shapes], cfg, self._stream())
+                                                                   [s[2] for s in shapes], cfg, self._stream(), wide=wide)
                 else:
-                    ecs = self.client.batch_put_device_fp8(fk, ptrs, [tensors[i].numel() for i in fused], cfg, self._stream())
-                done = [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.OK]
+                    ecs = self.client.batch_put_device_fp8(fk, ptrs, [tensors[i].numel() for i in fused], cfg, self._stream(), wide=wide)
+                done += [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.OK]
                 bad = [(keys[i], e) for i, e in zip(fused, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
                 if bad:
                     raise RuntimeError(f"fused fp8 put failed: {bad[:3]}")
+            if fused_all:
                 metas = []
                 for i in done:
                     t = tensors[i]
-                    metas.append(json.dumps({"dtype": "bfloat16", "shape": list(t.shape), "packed": "mxfp8", "numel": t.numel(),
-                                             "padded_numel": t.numel()}).encode())
+                    metas.append(json.dumps({"dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape), "packed": "mxfp8",
+                                             "numel": t.numel(), "padded_numel": t.numel()}).encode())
                 if done:
                     ecs = self.client.batch_put([keys[i] + "#meta" for i in done], metas, self._meta_cfg())
                     if any(e != _bb.ErrorCode.OK for e in ecs):
@@ -123,14 +149,13 @@ class TensorStore:
             assert t.is_cuda, "TensorStore moves CUDA tensors (host data: use client.put)"
             meta = {"dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape), "packed": None, "numel": t.numel()}
             if pack_fp8:
-                assert t.dtype == torch.bfloat16, "MXFP8 packing takes bf16 tensors"
                 n = t.numel()
                 npad = (n + 31) // 32 * 32
                 src = t.view(-1)
                 if npad != n:
                     src = torch.cat([src, torch.zeros(npad - n, dtype=t.dtype, device=t.device)])
                 packed = torch.empty(_bb.mxfp8_packed_bytes(npad), dtype=torch.uint8, device=t.device)
-                _bb.mxfp8_pack(src.data_ptr(), npad, packed.data_ptr(), self._stream())
+                _bb.mxfp8_pack(src.data_ptr(), npad, packed.data_ptr(), self._stream(), wide=_MX_WIDE[t.dtype])
                 keep.append(src)
                 meta["packed"] = "mxfp8"
                 meta["padded_numel"] = npad
@@ -172,12 +197,12 @@ class TensorStore:
         result = [None] * len(keys)
         # MXFP8 objects made of whole tiles: unpack fused into the get kernel (falls through when the object is not a
         # single GPU-fabric shard any more, e.g. after demotion to a host tier)
-        fused = [i for i, m in enumerate(metas) if m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"]
-                 and self.client.device_fp8_eligible(m["numel"])]
-        if fused:
-            outs = [torch.empty(metas[i]["numel"], dtype=torch.bfloat16, device=device) for i in fused]
+        fused_all = [i for i, m in enumerate(metas) if m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"]
+                     and self.client.device_fp8_eligible(m["numel"])]
+        for dt, fused in _by_dtype(fused_all, lambda i: _stored_dtype(metas[i])).items():
+            outs = [torch.empty(metas[i]["numel"], dtype=dt, device=device) for i in fused]
             ecs = self.client.batch_get_device_fp8([keys[i] for i in fused], [o.data_ptr() for o in outs], [metas[i]["numel"] for i in fused],
-                                                   self._stream())
+                                                   self._stream(), wide=_MX_WIDE[dt])
             for i, o, e in zip(fused, outs, ecs):
                 if e == _bb.ErrorCode.OK:
                     result[i] = o.view(metas[i]["shape"])
@@ -202,8 +227,9 @@ class TensorStore:
         out = []
         for m, b in zip(metas, bufs):
             if m["packed"] == "mxfp8":
-                t = torch.empty(m["padded_numel"], dtype=torch.bfloat16, device=device)
-                _bb.mxfp8_unpack(b.data_ptr(), m["padded_numel"], t.data_ptr(), self._stream())
+                dt = _stored_dtype(m)  # unpacked straight to the stored dtype
+                t = torch.empty(m["padded_numel"], dtype=dt, device=device)
+                _bb.mxfp8_unpack(b.data_ptr(), m["padded_numel"], t.data_ptr(), self._stream(), wide=_MX_WIDE[dt])
                 out.append(t[: m["numel"]].view(m["shape"]))
             else:
                 out.append(b)
@@ -221,7 +247,7 @@ class TensorStore:
         view is written.  The outs must not overlap one another (not checked).
 
         Every check comes before any transfer: KeyError for a missing key, TypeError unless out.dtype is the stored
-        dtype (bfloat16 for packed tensors), ValueError unless out.shape is the stored shape and out is a CUDA tensor on
+        dtype (packed tensors included), ValueError unless out.shape is the stored shape and out is a CUDA tensor on
         the current device.  Then each route is one call for all the tensors that take it:
           1. unpacked, contiguous out: batch_get_device into its storage;
           2. unpacked, out whose elements are rows (see _source_rows: `narrow` along any dim, `t[::k]`):
@@ -238,7 +264,7 @@ class TensorStore:
         metas = self._metas(keys)
         dev = torch.cuda.current_device()
         for k, m, o in zip(keys, metas, outs):
-            want = torch.bfloat16 if m["packed"] else _DTYPES[m["dtype"]]
+            want = _stored_dtype(m)
             if o.dtype != want:
                 raise TypeError(f"{k}: out is {o.dtype}, the stored tensor {want}")
             if list(o.shape) != m["shape"]:
@@ -270,16 +296,17 @@ class TensorStore:
         fused = [i for i in packed if metas[i]["padded_numel"] == metas[i]["numel"] and self.client.device_fp8_eligible(metas[i]["numel"])
                  and (outs[i].is_contiguous() or rows[i] is not None)]
         rest += [i for i in packed if i not in set(fused)]
-        if fused:
+        for dt, fused in _by_dtype(fused, lambda i: outs[i].dtype).items():
             fk, ptrs = [keys[i] for i in fused], [outs[i].data_ptr() for i in fused]
+            es, wide = outs[fused[0]].element_size(), _MX_WIDE[dt]
             if any(rows[i] is not None for i in fused):
                 # widths and pitches in elements; contiguous outs go as one row each
-                shapes = [(rows[i][0] // 2, rows[i][1] // 2, rows[i][2]) if rows[i] is not None else (outs[i].numel(),) * 2 + (1,)
+                shapes = [(rows[i][0] // es, rows[i][1] // es, rows[i][2]) if rows[i] is not None else (outs[i].numel(),) * 2 + (1,)
                           for i in fused]
                 ecs = self.client.batch_get_device_fp8_scatter(fk, ptrs, [outs[i].numel() for i in fused], [s[0] for s in shapes],
-                                                               [s[1] for s in shapes], [s[2] for s in shapes], self._stream())
+                                                               [s[1] for s in shapes], [s[2] for s in shapes], self._stream(), wide=wide)
             else:
-                ecs = self.client.batch_get_device_fp8(fk, ptrs, [outs[i].numel() for i in fused], self._stream())
+                ecs = self.client.batch_get_device_fp8(fk, ptrs, [outs[i].numel() for i in fused], self._stream(), wide=wide)
             check("fused fp8 get", [i for i, e in zip(fused, ecs) if e != _bb.ErrorCode.NOT_IMPLEMENTED],
                   [e for e in ecs if e != _bb.ErrorCode.NOT_IMPLEMENTED])
             rest += [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
@@ -315,21 +342,22 @@ class TensorStore:
 
     def _get_rows(self, keys: list, metas: list, starts: list, stops: list, device: torch.device) -> list:
         result = [None] * len(keys)
-        packed = [i for i, m in enumerate(metas) if m["packed"]]
-        if packed:
+        packed_all = [i for i, m in enumerate(metas) if m["packed"]]
+        for dt, packed in _by_dtype(packed_all, lambda i: _stored_dtype(metas[i])).items():
             # Elements [lo, hi) of the (padded) packed object; their window ends before any pad.  Each result sits at
-            # element lo % 8 of its own allocation, so that the virtual base ptr - 2 * lo is 16-byte aligned and every
-            # row size takes the fused path.
+            # element lo % (16 / element size) of its own allocation, so that the virtual base ptr - size * lo is 16-byte
+            # aligned and every row size takes the fused path.
+            per = 16 // torch.empty((), dtype=dt).element_size()
             los, counts, ptrs = [], [], []
             for i in packed:
                 m = metas[i]
                 row = torch.Size(m["shape"][1:]).numel()
                 lo, count = starts[i] * row, (stops[i] - starts[i]) * row
-                buf = torch.empty(count + lo % 8, dtype=torch.bfloat16, device=device)
-                result[i] = buf[lo % 8:].view([stops[i] - starts[i]] + m["shape"][1:])
+                buf = torch.empty(count + lo % per, dtype=dt, device=device)
+                result[i] = buf[lo % per:].view([stops[i] - starts[i]] + m["shape"][1:])
                 los.append(lo), counts.append(count), ptrs.append(result[i].data_ptr())
             ecs = self.client.batch_get_device_fp8_range([keys[i] for i in packed], ptrs, [metas[i]["padded_numel"] for i in packed], los,
-                                                         counts, self._stream())
+                                                         counts, self._stream(), wide=_MX_WIDE[dt])
             bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
             if bad:
                 raise RuntimeError(f"fused fp8 range get failed: {bad[:3]}")
@@ -374,8 +402,8 @@ class TensorStore:
 
         MXFP8-packed tensors, padded ones included (their pad lies past the last row), take the fused strided get of
         packed tensors: the whole packed object is read and verified against its digest, only the rows' elements are
-        unpacked and stored.  Each result starts at element `offset % 8` of its own allocation, so only a slice whose row
-        gap is not a multiple of 8 elements misses the fused kernel; such slices, and packed tensors the fused kernel
+        unpacked and stored.  Each result starts at element `offset % (16 / element size)` of its own allocation, so only a
+        slice whose row gap is not a multiple of that many elements (8 for bf16 and fp16, 4 for fp32) misses the fused kernel; such slices, and packed tensors the fused kernel
         cannot read (striped, demoted to a host tier), are read whole, unpacked and narrowed."""
         device = device or torch.device("cuda", torch.cuda.current_device())
         keys, dims, starts, stops = list(keys), list(dims), list(starts), list(stops)
@@ -398,21 +426,22 @@ class TensorStore:
                                   [stops[i] for i in first], device)
             for i, t in zip(first, rows):
                 result[i] = t
-        packed = [i for i, m in enumerate(metas) if dims[i] != 0 and m["packed"]]
-        if packed:
+        packed_all = [i for i, m in enumerate(metas) if dims[i] != 0 and m["packed"]]
+        for dt, packed in _by_dtype(packed_all, lambda i: _stored_dtype(metas[i])).items():
             # prod(shape[:dim]) rows of (stop - start) * inner elements every shape[dim] * inner elements
+            per = 16 // torch.empty((), dtype=dt).element_size()
             offsets, widths, pitches, nrows = [], [], [], []
             for i in packed:
                 shape, d = metas[i]["shape"], dims[i]
                 inner = torch.Size(shape[d + 1:]).numel()
                 offset, width = starts[i] * inner, (stops[i] - starts[i]) * inner
                 rows = torch.Size(shape[:d]).numel()
-                buf = torch.empty(rows * width + offset % 8, dtype=torch.bfloat16, device=device)
-                result[i] = buf[offset % 8:].view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
+                buf = torch.empty(rows * width + offset % per, dtype=dt, device=device)
+                result[i] = buf[offset % per:].view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
                 offsets.append(offset), widths.append(width), pitches.append(shape[d] * inner), nrows.append(rows)
             ecs = self.client.batch_get_device_fp8_strided([keys[i] for i in packed], [result[i].data_ptr() for i in packed],
                                                            [metas[i]["padded_numel"] for i in packed], offsets, widths, pitches,
-                                                           nrows, self._stream())
+                                                           nrows, self._stream(), wide=_MX_WIDE[dt])
             bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
             if bad:
                 raise RuntimeError(f"fused fp8 strided get failed: {bad[:3]}")

@@ -669,39 +669,42 @@ void BlackbirdClient::refresh_placements(const std::vector<ObjectKey>& keys, con
 
 // ================================================================ fused MXFP8 device API
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
-                                                             const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream) {
-  return put_device_fp8(keys, bf16_ptrs, n_elems, nullptr, cfg, stream);
+                                                             const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream,
+                                                             mxfp8::Wide wide) {
+  return put_device_fp8(keys, bf16_ptrs, n_elems, nullptr, cfg, stream, wide);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                                      const std::vector<uint64_t>& elem_widths,
                                                                      const std::vector<uint64_t>& elem_pitches,
-                                                                     const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
+                                                                     const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream,
+                                                                     mxfp8::Wide wide) {
   const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<uint64_t> elems(n);
   std::vector<SourceRows> pats(n);
   return shaped_batch(
       "device_put_fp8_strided", true, n, bf16_ptrs.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* bf16_bytes) {
+      [&](size_t i, uint64_t* wide_bytes) {
         SourceRows bytes;
         uint64_t extent = 0;
         const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems[i], &extent);
-        *bf16_bytes = 2 * elems[i];
+        *wide_bytes = b * elems[i];
         if (ec != ErrorCode::OK) return ec;
-        if (extent > UINT64_MAX / 2 || !pats[i].to_bf16_bytes(&bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        if (extent > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
         // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
-        if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 2 * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
+        if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
         const auto p = pick(pats, idx);
-        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &p, cfg, stream);
+        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &p, cfg, stream, wide);
       });
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows,
-                                                       const WorkerConfig& cfg, void* stream) {
+                                                       const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
@@ -736,6 +739,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
     }
     DeviceFp8Op op{&copies[0].shards[0], const_cast<void*>(bf16_ptrs[i]), n_elems[i], {}};
     if (rows) op.rows = (*rows)[i];
+    op.wide_type = wide;
     for (size_t cidx = 1; cidx < copies.size(); ++cidx) op.replicas.push_back(&copies[cidx].shards[0]);
     ops.push_back(std::move(op));
     idx.push_back(i);
@@ -764,70 +768,74 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
-                                                             const std::vector<uint64_t>& n_elems, void* stream) {
-  return get_device_fp8(keys, bf16_ptrs, n_elems, nullptr, nullptr, stream);
+                                                             const std::vector<uint64_t>& n_elems, void* stream, mxfp8::Wide wide) {
+  return get_device_fp8(keys, bf16_ptrs, n_elems, nullptr, nullptr, stream, wide);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                                      const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
                                                                      const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
-                                                                     void* stream) {
+                                                                     void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<SourceRows> pats(n);
   return shaped_batch(
       "device_get_fp8_scatter", false, n,
       bf16_ptrs.size() == n && n_elems.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* bf16_bytes) {
+      [&](size_t i, uint64_t* wide_bytes) {
         SourceRows bytes;
         uint64_t elems = 0, extent = 0;
         const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems, &extent);
         if (ec != ErrorCode::OK) return ec;
         if (elems != n_elems[i]) return ErrorCode::INVALID_ARGUMENT;
-        if (extent > UINT64_MAX / 2 || !pats[i].to_bf16_bytes(&bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
-        *bf16_bytes = 2 * elems;
+        if (extent > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *wide_bytes = b * elems;
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
         const auto p = pick(pats, idx);
-        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &p, stream);
+        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &p, stream, wide);
       });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                                    const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
-                                                                   const std::vector<uint64_t>& elem_counts, void* stream) {
+                                                                   const std::vector<uint64_t>& elem_counts, void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<ByteRange> ranges(n);
   return shaped_batch(
       "device_get_fp8_range", false, n, elem_offsets.size() == n && elem_counts.size() == n,
       [&](size_t i, uint64_t* bytes) {
         ranges[i] = {elem_offsets[i], elem_counts[i]};
-        *bytes = 2 * elem_counts[i];
+        *bytes = b * elem_counts[i];
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream); });
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream, wide); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                                      const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
                                                                      const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
-                                                                     const std::vector<uint64_t>& rows, void* stream) {
+                                                                     const std::vector<uint64_t>& rows, void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<ByteRange> ranges(n);
   return shaped_batch(
       "device_get_fp8_strided", false, n, elem_offsets.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
       [&](size_t i, uint64_t* bytes) {
         ranges[i] = {elem_offsets[i], elem_widths[i], elem_pitches[i], rows[i]};
-        *bytes = 2 * rows[i] * elem_widths[i];  // counted for OK items only, whose rows lie inside the object
+        *bytes = b * rows[i] * elem_widths[i];  // counted for OK items only, whose rows lie inside the object
         return ErrorCode::OK;
       },
-      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream); });
+      [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream, wide); });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                                       const std::vector<SourceRows>* rows, void* stream) {
+                                                       const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
+  const uint64_t b = mxfp8::wide_bytes(wide);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
@@ -854,7 +862,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ec;
         continue;
       }
-      bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - 2 * w.base_shift(w.lo));
+      bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - b * w.base_shift(w.lo));
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
@@ -877,13 +885,13 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     // a range the kernel cannot store (StoreWindow::fused_get_aligned) fails alone, so that the rest of the batch still
     // takes the fused launch; the caller reads it whole and slices instead.  A whole tensor is left to the engine.
     StoreWindow bytes;
-    if (ranges && (!w.to_bf16_bytes(&bytes) || !bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, 2 * n_elems[i]))) {
+    if (ranges && (!w.to_wide_bytes(b, &bytes) || !bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, b * n_elems[i]))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
     SourceRows dst_bytes;  // so do destination rows the kernel cannot store into
-    if (rows && (!(*rows)[i].to_bf16_bytes(&dst_bytes) ||
-                 !dst_bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, 2 * n_elems[i]))) {
+    if (rows && (!(*rows)[i].to_wide_bytes(b, &dst_bytes) ||
+                 !dst_bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, b * n_elems[i]))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
@@ -900,7 +908,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}});
+      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}, wide});
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -918,7 +926,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
     const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
-    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr, stream);
+    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr, stream,
+                          wide);
   });
   metrics_.inc("device_get_fp8_batches_total");
   return out;
@@ -1728,18 +1737,20 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
   if (digests) digests->assign(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
-    const auto* src = static_cast<const uint16_t*>(op.wide);
-    std::vector<uint16_t> dense;
+    const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
+    if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
+    const auto* src = static_cast<const uint8_t*>(op.wide);
+    std::vector<uint8_t> dense;
     if (op.rows.strided()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows
       SourceRows b;
-      if (!op.rows.valid() || !op.rows.to_bf16_bytes(&b)) return ErrorCode::INVALID_ARGUMENT;
-      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), 2 * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
-      dense.resize(op.n_elems);
-      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, src + at, 2 * n); });
+      if (!op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      dense.resize(eb * op.n_elems);
+      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + eb * x, src + eb * at, eb * n); });
       src = dense.data();
     }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
-    mxfp8::pack_bf16(src, op.n_elems, packed.data());
+    mxfp8::pack(src, op.wide_type, op.n_elems, packed.data());
     uint64_t d = 0;
     ErrorCode ec = io_->write_shard(*op.placement, packed.data(), &d, ChecksumAlgo::BBH64);
     for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], packed.data(), nullptr, ChecksumAlgo::NONE);
@@ -1754,11 +1765,13 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
   if (status) status->assign(ops.size(), 0);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
+    const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
+    if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
     if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
     SourceRows b;
-    if (op.rows.strided()) {  // as the engine: destination rows, never with a window, co-aligned in bf16 bytes
-      if (!op.win.whole() || !op.rows.valid() || !op.rows.to_bf16_bytes(&b)) return ErrorCode::INVALID_ARGUMENT;
-      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), 2 * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+    if (op.rows.strided()) {  // as the engine: destination rows, never with a window, co-aligned in wide bytes
+      if (!op.win.whole() || !op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
     }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
@@ -1767,21 +1780,16 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       continue;
     }
     if (ec != ErrorCode::OK) return ec;
-    if (op.rows.strided()) {  // as the kernel's scattering store: the unpacked elements, stored into their rows
-      std::vector<uint16_t> wide(op.n_elems);
-      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
-      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) {
-        std::memcpy(static_cast<uint16_t*>(op.wide) + at, wide.data() + x, 2 * n);
-      });
-    } else if (op.win.whole()) {
-      mxfp8::unpack_bf16(packed.data(), op.n_elems, static_cast<uint16_t*>(op.wide));
-    } else {  // as the kernel does: the whole object is read and verified, only the window stored
-      std::vector<uint16_t> wide(op.n_elems);
-      mxfp8::unpack_bf16(packed.data(), op.n_elems, wide.data());
-      op.win.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) {
-        std::memcpy(static_cast<uint16_t*>(op.wide) + at, wide.data() + x, 2 * n);
-      });
+    auto* dst = static_cast<uint8_t*>(op.wide);
+    if (op.win.whole() && !op.rows.strided()) {
+      mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, dst);
+      continue;
     }
+    std::vector<uint8_t> wide(eb * op.n_elems);
+    mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, wide.data());
+    auto store = [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + eb * at, wide.data() + eb * x, eb * n); };
+    if (op.rows.strided()) op.rows.for_each_run(op.n_elems, store);  // as the kernel's scattering store: into the rows
+    else op.win.for_each_run(op.n_elems, store);  // as the kernel does: the whole object read and verified, only the window stored
   }
   return ErrorCode::OK;
 }

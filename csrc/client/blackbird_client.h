@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "common/metrics.h"
+#include "common/mxfp8.h"
 #include "common/store_window.h"
 #include "net/tcp.h"
 #include "rpc/rpc_service.h"
@@ -76,16 +77,18 @@ struct DeviceShardOp {
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
 struct DeviceFp8Op {
   const ShardPlacement* placement = nullptr;
-  void* wide = nullptr;     // client's bf16 tensor (source of a put, destination of a get: the base of `win`)
+  void* wide = nullptr;     // client's tensor (source of a put, destination of a get: the base of `win`)
   uint64_t n_elems = 0;
   std::vector<const ShardPlacement*> replicas;  // put: the other copies (<= 2), written by the same tile pass
   // Get: the elements that are stored (common/store_window.h); the whole packed object is still read and verified.  The
   // default is the whole object.
   StoreWindow win;
-  // The bf16 side's rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts: a put's source
+  // The wide side's rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts: a put's source
   // rows, or a get's destination rows (never together with a window).  The packed object is one shard, so the pattern is
   // the object's own.  The default is contiguous memory.
   SourceRows rows;
+  // The element type of `wide`: bf16, fp16 or fp32 (common/mxfp8.h).  Ops of one call share its size (2 or 4 bytes).
+  mxfp8::Wide wide_type = mxfp8::Wide::BF16;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -149,8 +152,15 @@ class BlackbirdClient {
   // into the get kernel.  n_elems[i] must be a multiple of 32 (whole MX blocks; pad + mxfp8_pack otherwise); up to 3 copies
   // (written by one tile pass: converted once, stored to every replica; gets fail over between them), one
   // shard per object.  The stored object is identical to packing first and putting the packed bytes.
+  //
+  // Every fp8 call takes a trailing `wide`: the element type of the tensors on the device side, bf16 (the default), fp16
+  // or fp32, the same for the whole call.  The packed format does not depend on it (common/mxfp8.h): a bf16-representable
+  // tensor packs to the same bytes from any type, and any packed object can be read into any type.  Below, "2 * x"
+  // bytes and "% 8" elements are stated for 2-byte types: with b = wide_bytes(wide) they are b * x bytes and
+  // % (16 / b) elements (4 for fp32).  The *_bytes_total metrics count wide bytes.
   std::vector<ErrorCode> batch_put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
-                                              const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream);
+                                              const std::vector<uint64_t>& n_elems, const WorkerConfig& cfg, void* stream,
+                                              mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Packed puts of sliced bf16 tensors (`kv[:, h0:h1, :]`, `W[:, k0:k1]`, `t[::k]`): object i holds the rows[i] *
   // elem_widths[i] elements of rows[i] rows of elem_widths[i] elements, row r read from bf16_ptrs[i] + 2 * r *
   // elem_pitches[i] (SourceRows in common/store_window.h, in elements).  The put kernel gathers the rows while it packs, so
@@ -163,9 +173,10 @@ class BlackbirdClient {
   // batch_put_device_fp8 of one contiguous tensor.
   std::vector<ErrorCode> batch_put_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
-                                                      const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream);
+                                                      const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream,
+                                                      mxfp8::Wide wide = mxfp8::Wide::BF16);
   std::vector<ErrorCode> batch_get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
-                                              const std::vector<uint64_t>& n_elems, void* stream);
+                                              const std::vector<uint64_t>& n_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Element-range gets of packed tensors: elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of the n_elems[i]-element
   // object i, unpacked to bf16, land at bf16_ptrs[i].  The whole packed object is read and verified against its digest (a
   // corrupt byte outside the range still fails that copy over to the next replica); only the range is unpacked and stored,
@@ -175,7 +186,7 @@ class BlackbirdClient {
   // fused launch.  On CHECKSUM_MISMATCH the range's contents are unspecified.
   std::vector<ErrorCode> batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                     const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
-                                                    const std::vector<uint64_t>& elem_counts, void* stream);
+                                                    const std::vector<uint64_t>& elem_counts, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Strided gets of packed tensors (a slice along an inner dimension): rows[i] rows of elem_widths[i] elements, row r being
   // elements [elem_offsets[i] + r * elem_pitches[i], + elem_widths[i]) of the n_elems[i]-element object i, unpacked to bf16,
   // land densely at bf16_ptrs[i] + 2 * r * elem_widths[i].  The whole packed object is read and verified (a corrupt byte
@@ -189,7 +200,7 @@ class BlackbirdClient {
   std::vector<ErrorCode> batch_get_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
                                                       const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
-                                                      const std::vector<uint64_t>& rows, void* stream);
+                                                      const std::vector<uint64_t>& rows, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Gets of packed tensors into sliced bf16 tensors the caller owns: object i (n_elems[i] elements) is unpacked into rows[i]
   // rows of elem_widths[i] elements, row r at bf16_ptrs[i] + 2 * r * elem_pitches[i] (SourceRows in common/store_window.h,
   // in elements), by the scattering store of the fused unpack.  No element outside the rows is ever written.  Fail-over
@@ -201,7 +212,7 @@ class BlackbirdClient {
   std::vector<ErrorCode> batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
                                                       const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
-                                                      void* stream);
+                                                      void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -306,13 +317,13 @@ class BlackbirdClient {
   // (*rows)[i], in elements.
   std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows, const WorkerConfig& cfg,
-                                        void* stream);
+                                        void* stream, mxfp8::Wide wide);
   // batch_get_device_fp8, batch_get_device_fp8_range, batch_get_device_fp8_strided and batch_get_device_fp8_scatter:
   // `ranges` null = whole tensors, else object i's rows (offset, length and pitch in elements) into bf16_ptrs[i]; `rows`
   // (whole tensors only) null = contiguous destinations, else object i lands in (*rows)[i], in elements.
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                        const std::vector<SourceRows>* rows, void* stream);
+                                        const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide);
   // The eight shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
   template <class Shape, class Run>
   std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);

@@ -1,7 +1,8 @@
 // StoreWindow: which units of an object a device get stores, and where each one lands.  This is the one statement of the
 // rule; the transfer engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host
 // loopback transport and the kernels' XFER_WINDOW / XFER_STRIDED descriptors (kernels/xfer.h) all follow it.  A unit is a
-// byte of an object or shard, or an element of an MXFP8-packed tensor (to_bf16_bytes() turns elements into bf16 bytes).
+// byte of an object or shard, or an element of an MXFP8-packed tensor (to_wide_bytes() turns elements into bytes of its
+// wide side: bf16, fp16 or fp32).
 //
 // Unit x in [lo, hi) is stored iff pitch == 0 or c = (x + phase) % pitch < width.  Relative to the base the window goes
 // with, it lands at
@@ -64,11 +65,12 @@ struct StoreWindow {
   // phase < pitch.
   bool valid(uint64_t n) const { return lo <= hi && hi <= n && (!strided() || (width != 0 && width <= pitch && phase < pitch)); }
 
-  // The window of an MXFP8 get in bf16 bytes of the unpacked object.  False for a pitch of 2^62 elements or more, whose
-  // byte arithmetic could overflow.
-  bool to_bf16_bytes(StoreWindow* out) const {
-    if (pitch > (UINT64_MAX >> 2)) return false;
-    *out = {2 * lo, 2 * hi, 2 * pitch, 2 * width, 2 * phase, row};
+  // The window of an MXFP8 get in bytes of the unpacked object, whose elements are `b` bytes (2 or 4).  False for a pitch
+  // of 2^63 / b elements or more, whose byte arithmetic could overflow.  The default bounds [0, UINT64_MAX) stay the whole
+  // object only through over() first.
+  bool to_wide_bytes(uint64_t b, StoreWindow* out) const {
+    if (pitch > (UINT64_MAX >> 1) / b) return false;
+    *out = {b * lo, b * hi, b * pitch, b * width, b * phase, row};
     return true;
   }
 
@@ -108,7 +110,7 @@ struct StoreWindow {
     return (base + origin() + phase - r_lo * gap) % 16 == 0;
   }
 
-  // The client's rule for whether a device get of this window (in bytes; an MXFP8 get's after to_bf16_bytes()) into `ptr`,
+  // The client's rule for whether a device get of this window (in bytes; an MXFP8 get's after to_wide_bytes()) into `ptr`,
   // where its first stored unit lands, may take the fused path as far as the shard [off, off + len) of a copy goes; the
   // get is fused only if every shard of every copy passes (an MXFP8 object is one shard, [0, 2 * n_elems)).  The kernels
   // store 16-byte aligned spans only, so the virtual base ptr - lo must be 16-byte aligned at the shard's start: at every
@@ -152,7 +154,7 @@ struct StoreWindow {
 // object is dense and the memory strided.  This is the one statement of the rule; the transfer engine (XferItem, Fp8Item),
 // the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and the kernels' XFER_GATHER and
 // XFER_SCATTER descriptors (kernels/xfer.h) all follow it.  The unit is a byte, or for an MXFP8 transfer an element of the
-// bf16 side (to_bf16_bytes() turns elements into bf16 bytes).
+// wide side (to_wide_bytes() turns elements into bytes of the wide type).
 //
 // With `src` where the pattern's row 0 starts, object byte x is read from (put) or stored at (get)
 //   src + ((x + phase) / width) * pitch + (x + phase) % width
@@ -165,11 +167,11 @@ struct SourceRows {
   // 0 < width <= pitch and phase < width for a pattern.
   bool valid() const { return !strided() || (width != 0 && width <= pitch && phase < width); }
 
-  // The source rows of an MXFP8 put, given in elements, in bf16 bytes of the source.  False for a pitch of 2^62 elements or
-  // more, whose byte arithmetic could overflow (as StoreWindow::to_bf16_bytes).
-  bool to_bf16_bytes(SourceRows* out) const {
-    if (pitch > (UINT64_MAX >> 2)) return false;
-    *out = {2 * pitch, 2 * width, 2 * phase};
+  // The rows of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False for a
+  // pitch of 2^63 / b elements or more, whose byte arithmetic could overflow (as StoreWindow::to_wide_bytes).
+  bool to_wide_bytes(uint64_t b, SourceRows* out) const {
+    if (pitch > (UINT64_MAX >> 1) / b) return false;
+    *out = {b * pitch, b * width, b * phase};
     return true;
   }
 
@@ -218,7 +220,7 @@ struct SourceRows {
     return (src + phase) % 16 == 0;
   }
 
-  // The client's rule for whether a device get into these rows (in bytes; an MXFP8 get's after to_bf16_bytes()), row 0 at
+  // The client's rule for whether a device get into these rows (in bytes; an MXFP8 get's after to_wide_bytes()), row 0 at
   // `dst`, may take the fused path as far as the shard [off, off + len) of a copy goes; the get is fused only if every shard
   // of every copy passes.  The shard's rows must be co-aligned from where it starts, and the gap a multiple of 16 bytes
   // even where the shard holds a single row, so that whether a get is fused depends on its own shape and pointer, not on

@@ -651,6 +651,7 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.wide = op.wide;
     it.packed = d.value();
     it.n_elems = op.n_elems;
+    it.wide_type = op.wide_type;
     it.win = op.win;  // a window on a put is refused by the engine
     if (unpack) it.dst_rows = op.rows;  // the rows are the destination's on a get, the source's on a put
     else it.rows = op.rows;

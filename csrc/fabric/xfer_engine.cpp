@@ -576,26 +576,31 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
   s->strides.clear();
+  // one kernel instantiation per launch: bf16 and fp16 items share the 2-byte one, fp32 items take the 4-byte one
+  const uint32_t eb = mxfp8::wide_bytes(items[0].wide_type);
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
     const bool gather = it.rows.strided();
     const bool scatter = it.dst_rows.strided();
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
-    SourceRows rows;  // a gathered put's source rows, or a scattered get's destination rows, in bf16 bytes
-    if (gather && (unpack || !it.rows.valid() || !it.rows.to_bf16_bytes(&rows))) return ErrorCode::INVALID_ARGUMENT;
-    if (scatter && (!unpack || gather || !it.win.whole() || !it.dst_rows.valid() || !it.dst_rows.to_bf16_bytes(&rows)))
+    if (it.wide_type != mxfp8::Wide::BF16 && it.wide_type != mxfp8::Wide::F16 && it.wide_type != mxfp8::Wide::F32)
+      return ErrorCode::INVALID_ARGUMENT;
+    if (mxfp8::wide_bytes(it.wide_type) != eb) return ErrorCode::INVALID_ARGUMENT;  // mixes 2- and 4-byte wide types
+    SourceRows rows;  // a gathered put's source rows, or a scattered get's destination rows, in wide bytes
+    if (gather && (unpack || !it.rows.valid() || !it.rows.to_wide_bytes(eb, &rows))) return ErrorCode::INVALID_ARGUMENT;
+    if (scatter && (!unpack || gather || !it.win.whole() || !it.dst_rows.valid() || !it.dst_rows.to_wide_bytes(eb, &rows)))
       return ErrorCode::INVALID_ARGUMENT;
     // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
     // first element after row 0's start): the rows are checked instead
     if (((strided || gather || scatter ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
-        ((gather || scatter) && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), 2 * it.n_elems)))
+        ((gather || scatter) && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
       return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
-    // a put stores the whole object; from here on the window is in bf16 bytes
+    // a put stores the whole object; from here on the window is in wide bytes
     StoreWindow w = it.win.over(it.n_elems);
-    if ((!unpack && !it.win.whole()) || !w.valid(it.n_elems) || !w.to_bf16_bytes(&w)) return ErrorCode::INVALID_ARGUMENT;
+    if ((!unpack && !it.win.whole()) || !w.valid(it.n_elems) || !w.to_wide_bytes(eb, &w)) return ErrorCode::INVALID_ARGUMENT;
     for (uint32_t r = 1; r < nrep; ++r)
       if (!it.more_packed[r - 1] || (reinterpret_cast<uintptr_t>(it.more_packed[r - 1]) & 15)) return ErrorCode::INVALID_ADDRESS;
     auto* payload = static_cast<uint8_t*>(it.packed);
@@ -607,11 +612,11 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     d.nbytes = it.n_elems;  // payload tiles, the last one possibly partial
     d.ndst = nrep;
     d.expect = 0;
-    d.flags = 0;
+    d.flags = it.wide_type == mxfp8::Wide::F16 ? XFER_WIDE_F16 : 0u;
     d.reserved = 0;
     // whole-object gets keep exactly the descriptors they had; a strided item always carries its window
     if (unpack && !it.win.covers(it.n_elems)) {
-      d.flags = XFER_WINDOW;
+      d.flags |= XFER_WINDOW;
       d.win.lo = w.lo;
       d.win.hi = w.hi;
     }
@@ -650,7 +655,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   l.max_ctas = max_ctas_;
   l.stream = stream;
   BB_CUDA(cudaEventRecord(s->ev_start, st));
-  const int rc = launch_xfer_fp8(l, unpack);
+  const int rc = launch_xfer_fp8(l, unpack, eb);
   if (rc != 0) return cuda_failed(rc, "launch_xfer_fp8");
   ++launches_;
   BB_CUDA(cudaEventRecord(s->ev_stop, st));

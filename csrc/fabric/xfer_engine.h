@@ -49,10 +49,14 @@ inline uint64_t window_read_bytes(const XferItem& it, ChecksumAlgo algo) {
   return it.win.hi > it.win.lo ? it.win.hi - (it.win.lo & ~uint64_t{15}) : 0;
 }
 
-// One object of a fused MXFP8 transfer: `wide` is the caller's bf16 tensor, `packed` the slab location of the
-// stored object ([E4M3 payload n_elems][E8M0 scales n_elems / 32]).
+// One object of a fused MXFP8 transfer: `wide` is the caller's tensor, of element type `wide_type` (bf16, fp16 or fp32),
+// `packed` the slab location of the stored object ([E4M3 payload n_elems][E8M0 scales n_elems / 32]).  Below, "bf16
+// bytes" are bytes of the wide type.
 struct Fp8Item {
   void* wide = nullptr;
+  // run_fp8 returns INVALID_ARGUMENT for a batch that mixes 2-byte (bf16, fp16) and 4-byte (fp32) types: each is one
+  // launch of its own kernel instantiation.
+  mxfp8::Wide wide_type = mxfp8::Wide::BF16;
   void* packed = nullptr;            // replica 0 (the copy a get reads)
   void* more_packed[kMaxDst - 1] = {nullptr, nullptr};  // put: further replicas written by the same tile pass
   uint32_t nreplicas = 1;            // put: 1..kMaxDst
@@ -97,7 +101,7 @@ class XferEngine {
   ErrorCode wait(uint64_t ticket, XferResult* out);
   // Convenience: submit + wait.
   ErrorCode run(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream, XferResult* out);
-  // Fused MXFP8 put (pack = bf16 -> slab) or get (unpack = slab -> bf16): the bf16 side is read / written once, the
+  // Fused MXFP8 put (pack = wide -> slab) or get (unpack = slab -> wide): the wide side is read / written once, the
   // E4M3 payload is hashed on the tensor cores while it sits in shared memory, and the digest returned is the
   // BBH64 of the stored packed object (identical to hashing the output of mxfp8_pack).  Synchronous; needs two free
   // slots (the fused kernel's batch and the batch that hashes the scales).

@@ -8,6 +8,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "common/mxfp8.h"
+
 namespace bb::gpu {
 
 constexpr uint32_t kTileBytes = 16384;   // one TMA tile == one BBH64 tile (tchash_def.h)
@@ -43,6 +45,10 @@ enum XferFlags : uint32_t {
   // with XFER_WINDOW, XFER_STRIDED, XFER_GATHER, XFER_MULTIMEM or XFER_RAW_SUM.  The tile in shared memory is the object's
   // tile, so the digest and the verify are those of a plain get.
   XFER_SCATTER = 1u << 6,
+  // Fused MXFP8 only: the descriptor's wide side is fp16, not bf16 (mxfp8::Wide::F16), in the 2-byte instantiation of
+  // the kernel.  A batch of bf16 and fp16 items is one launch; fp32 items take the 4-byte instantiation, a launch of their
+  // own.
+  XFER_WIDE_F16 = 1u << 7,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -164,7 +170,9 @@ int launch_mailbox(const MailSlot* slots, MailResult* results, MailCtl* ctl, uin
 // Small-object latency tier: one warp per descriptor, digest bit-identical to launch_xfer's (needs descs; not tile_start).
 int launch_xfer_small(const XferLaunch& l);
 int xfer_smem_bytes(int algo);
-// Fused MXFP8 transfer (xfer_mxfp8.cu).  The packed object is one contiguous [payload n][scales n/32] extent.
+// Fused MXFP8 transfer (xfer_mxfp8.cu).  The packed object is one contiguous [payload n][scales n/32] extent.  The wide
+// side holds `wide_bytes` (2 or 4) bytes per element: bf16, or fp16 for descriptors with XFER_WIDE_F16, when it is 2;
+// fp32 when it is 4.  Below, "bf16 bytes" means bytes of that wide side.
 // Descriptors: pack (put): src = bf16 source, dst[0..ndst-1] = base of the packed object in every replica (the scales
 // follow the payload), nbytes = payload bytes (= elements, a multiple of kTileBytes); unpack (get): src = base of the
 // packed object, dst[0] = bf16 destination (where element 0 lands); an unpack descriptor may carry XFER_WINDOW, whose
@@ -172,8 +180,9 @@ int xfer_smem_bytes(int algo);
 // `strides` (a device table; no inline copy) is in bf16 bytes too; or instead XFER_SCATTER, with dst[0] where the
 // destination pattern's row 0 starts and the pattern in bf16 bytes in `strides`.  `sum_ws` receives the unfinalised BBH64 sum of the
 // payload tiles per descriptor (must be zero on entry); descs / tile_start are device tables.
-int launch_xfer_fp8(const XferLaunch& l, bool unpack);
-int xfer_fp8_smem_bytes();
+int launch_xfer_fp8(const XferLaunch& l, bool unpack, uint32_t wide_bytes = 2);
+// Dynamic shared memory of the instantiation for `wide_bytes`-byte elements (its ring stage counts differ).
+int xfer_fp8_smem_bytes(uint32_t wide_bytes = 2);
 
 // CRC32C per-object constants (host): un-padding multiplier and the init-register term.
 uint32_t crc_unpad_for(uint64_t nbytes);
@@ -193,9 +202,9 @@ int launch_fill(void* dst, uint64_t nbytes, uint32_t value, void* stream);
 // Fills a buffer with deterministic pseudo-random bytes (synthetic objects).
 int launch_random_fill(void* dst, uint64_t nbytes, uint64_t seed, void* stream);
 
-// MXFP8 pack / unpack (mxfp8.cu): bf16 <-> [E4M3 payload | E8M0 scale per 32 elements].
-// n_elems % 32 == 0; packed size = n_elems + n_elems / 32 bytes (common/mxfp8.h).
-int launch_mxfp8_pack(const void* src_bf16, uint64_t n_elems, void* dst_packed, void* stream);
-int launch_mxfp8_unpack(const void* src_packed, uint64_t n_elems, void* dst_bf16, void* stream);
+// MXFP8 pack / unpack (mxfp8.cu): bf16 / fp16 / fp32 <-> [E4M3 payload | E8M0 scale per 32 elements].
+// n_elems % 32 == 0; packed size = n_elems + n_elems / 32 bytes (common/mxfp8.h); the wide side 16-byte aligned.
+int launch_mxfp8_pack(const void* src_wide, uint64_t n_elems, void* dst_packed, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+int launch_mxfp8_unpack(const void* src_packed, uint64_t n_elems, void* dst_wide, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
 
 }  // namespace bb::gpu

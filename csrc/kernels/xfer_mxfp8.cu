@@ -45,12 +45,18 @@ namespace {
 
 using namespace bb::ptx;
 
-constexpr int kWideStages = 3;              // ring of 32 KiB bf16 tiles
-constexpr int kTileStages = 6;              // ring of 16 KiB payload tiles (+ 512 B scales)
 constexpr int kConvertWarps = 16;           // warps 8..23 (the pack side is ALU bound: ncu issue-active 51 % with 8)
 constexpr int kFpThreads = (8 + kConvertWarps) * 32;
-constexpr uint32_t kWideBytes = 2 * kTileBytes;  // bf16 side of one payload tile
 constexpr uint32_t kScaleBytes = kTileBytes / 32;
+
+// One instantiation per wide element size WB: 2 (bf16, and fp16 by XFER_WIDE_F16) or 4 (fp32).  A wide tile is the
+// WB * 16 KiB of one 16 KiB payload tile, so the fp32 rings are shorter: 3 wide + 6 payload stages would not fit.
+template <uint32_t WB>
+struct FpCfg {
+  static constexpr int kWideStages = WB == 2 ? 3 : 2;  // ring of WB * 16 KiB wide tiles
+  static constexpr int kTileStages = WB == 2 ? 6 : 4;  // ring of 16 KiB payload tiles (+ 512 B scales)
+  static constexpr uint32_t kWideBytes = WB * kTileBytes;  // wide side of one payload tile
+};
 constexpr int kFpStoreLag = 1;
 
 __constant__ uint64_t c_fp_col_mul[tchash::kN];
@@ -67,7 +73,8 @@ struct FpMeta {            // 64 bytes
   uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
                            // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
                            // FpParams::strides either way)
-  uint64_t pad;
+  uint32_t f16;            // XFER_WIDE_F16: the wide side is fp16 (2-byte instantiation only)
+  uint32_t pad;
 };
 static_assert(sizeof(FpMeta) == 64);
 
@@ -77,10 +84,12 @@ struct FpLookup {
   uint64_t src_scales;  // unpack: scales source
 };
 
-// Two rings: the wide (bf16) ring only spans load -> convert (pack) or convert -> store (unpack), the payload
+// Two rings: the wide ring only spans load -> convert (pack) or convert -> store (unpack), the payload
 // ring spans convert/load -> tensor-core hash -> store/accumulate.  Decoupling them lets 3 + 6 slots cover a
-// pipeline that would need 6 x 48.5 KiB as one ring.
+// pipeline that would need 6 x 48.5 KiB as one ring (bf16 / fp16; fp32: 2 + 4).
+template <uint32_t WB, int kWideStages = FpCfg<WB>::kWideStages, int kTileStages = FpCfg<WB>::kTileStages>
 struct __align__(1024) SmemFp {
+  static constexpr uint32_t kWideBytes = FpCfg<WB>::kWideBytes;
   uint8_t tile[kTileStages][kTileBytes];
   uint8_t wide[kWideStages][kWideBytes];
   uint8_t scales[kTileStages][kScaleBytes];
@@ -95,6 +104,8 @@ struct __align__(1024) SmemFp {
   uint64_t part[kTileStages][4];
   FpLookup lk[32];
 };
+// 227 KiB: the opt-in dynamic shared memory of one sm_90 CTA
+static_assert(sizeof(SmemFp<2>) <= 227 * 1024 && sizeof(SmemFp<4>) <= 227 * 1024, "SmemFp exceeds the shared memory of one CTA");
 
 struct FpParams {
   const XferDesc* descs;
@@ -106,10 +117,13 @@ struct FpParams {
                                // (XferLaunch::strides), else null
 };
 
-template <bool UNPACK>
+template <bool UNPACK, uint32_t WB>
 __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid_constant__ FpParams p) {
+  constexpr int kWideStages = FpCfg<WB>::kWideStages;
+  constexpr int kTileStages = FpCfg<WB>::kTileStages;
+  constexpr uint32_t kWideBytes = FpCfg<WB>::kWideBytes;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  SmemFp& s = *reinterpret_cast<SmemFp*>(smem_raw);
+  SmemFp<WB>& s = *reinterpret_cast<SmemFp<WB>*>(smem_raw);
   const uint32_t warp = threadIdx.x >> 5;
   const uint32_t lane = threadIdx.x & 31u;
 
@@ -154,6 +168,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
         e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER : XFER_GATHER);
+        e.m.f16 = d.flags & XFER_WIDE_F16;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
         // the packed object is [payload nbytes][scales nbytes/32]: a tile's scales sit (nbytes - ti*(16384-512)) past its payload
@@ -161,14 +176,14 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         if constexpr (UNPACK) {
           e.src = src + static_cast<uint64_t>(ti) * kTileBytes;  // payload tile in the slab
           e.src_scales = e.src + e.m.scales_delta;               // its scales
-          e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kWideBytes;  // bf16 destination
-          // store window in bf16 bytes of the object (XferDesc::win); a whole-object get stores [0, 2^64), i.e. every tile whole
+          e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kWideBytes;  // wide destination
+          // store window in wide bytes of the object (XferDesc::win); a whole-object get stores [0, 2^64), i.e. every tile whole
           const bool win = d.flags & XFER_WINDOW;
           e.m.dst[1] = win ? d1 : 0;
           e.m.dst[2] = win ? d2 : ~0ull;
           e.m.ndst = 1;
         } else {
-          // bf16 source tile; for a gathering load the pattern's row 0 (the tile's rows are found from its object offset)
+          // wide source tile; for a gathering load the pattern's row 0 (the tile's rows are found from its object offset)
           e.src = e.m.strided ? src : src + static_cast<uint64_t>(ti) * kWideBytes;
           e.src_scales = 0;
           e.m.dst[0] = d0 + static_cast<uint64_t>(ti) * kTileBytes;
@@ -199,7 +214,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           const uint32_t ws = it % kWideStages, wp = (it / kWideStages) & 1u;
           mbar_wait(&s.w_empty[ws], wp ^ 1u);
           if (lane < 4) reinterpret_cast<uint4*>(&s.w_meta[ws])[lane] = reinterpret_cast<const uint4*>(&e.m)[lane];
-          uint32_t tx = 2u * e.m.valid;  // bytes the stage's bulk loads deliver
+          uint32_t tx = WB * e.m.valid;  // bytes the stage's bulk loads deliver
           if (e.m.strided) {
             // Gathering load (XFER_GATHER): one source row segment per lane, so the wide tile is byte for byte the tile of
             // the compacted rows.  A short last tile needs no zero pad: only its `valid` elements are stored, and it is
@@ -213,12 +228,12 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             }
             tx = __reduce_add_sync(0xffffffffu, gather_row_segments(s.wide[ws], &s.w_full[ws], e.src,
                                                                      static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes,
-                                                                     2u * e.m.valid, gst, lane));
+                                                                     WB * e.m.valid, gst, lane));
           }
           __syncwarp();
           if (lane == 0) {
             mbar_arrive_expect_tx(&s.w_full[ws], tx);
-            if (!e.m.strided) bulk_g2s(s.wide[ws], reinterpret_cast<const void*>(e.src), 2u * e.m.valid, &s.w_full[ws]);
+            if (!e.m.strided) bulk_g2s(s.wide[ws], reinterpret_cast<const void*>(e.src), WB * e.m.valid, &s.w_full[ws]);
           }
         }
         __syncwarp();
@@ -239,10 +254,10 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
       if constexpr (UNPACK) {
         mbar_wait(&s.w_full[st], par);
         const FpMeta& m = s.w_meta[st];
-        // the tile's bf16 bytes inside the store window: the middle by TMA, head and tail byte-wise (as bb_xfer does); a
+        // the tile's wide bytes inside the store window: the middle by TMA, head and tail byte-wise (as bb_xfer does); a
         // strided window (XFER_STRIDED) cuts them further to its row segments, one per lane
         const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kWideBytes;
-        const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, 2u * m.valid, true, m.dst[1], m.dst[2]);
+        const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, WB * m.valid, true, m.dst[1], m.dst[2]);
         if (m.strided) {
           if (m.desc != pat_desc) {
             pat_desc = m.desc;
@@ -329,7 +344,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
     }
   } else {
     // ================================================================ convert warps 8..15
-    const uint32_t cw = warp - 8;  // convert warp: chunks [cw*kPer, (cw+1)*kPer) of the tile's 2048 16-byte bf16 chunks
+    const uint32_t cw = warp - 8;  // convert warp: chunks [cw*kPer, (cw+1)*kPer) of the tile's 2048 chunks of 8 elements
     constexpr uint32_t kPer = 2048 / kConvertWarps;
     for (uint32_t it = 0; it < my_tiles; ++it) {
       const uint32_t ts = it % kTileStages, tp = (it / kTileStages) & 1u;
@@ -340,14 +355,15 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         const FpMeta& m = s.t_meta[ts];
         // a tile outside the store window is hashed (epilogue) but neither unpacked nor stored; one that overlaps it is
         // unpacked whole.  The barrier arrivals below are the same for every tile.
-        const TileSpan sp = tile_span(static_cast<uint64_t>(m.tile_in_obj) * kWideBytes, 2u * m.valid, true, m.dst[1], m.dst[2]);
+        const TileSpan sp = tile_span(static_cast<uint64_t>(m.tile_in_obj) * kWideBytes, WB * m.valid, true, m.dst[1], m.dst[2]);
         const uint2* pay = reinterpret_cast<const uint2*>(s.tile[ts]);
         uint4* out = reinterpret_cast<uint4*>(s.wide[ws]);
+        const bool f16 = m.f16;
         if (sp.x1 > sp.x0) {
 #pragma unroll 4
           for (uint32_t k = 0; k < kPer / 32; ++k) {
             const uint32_t c = cw * kPer + k * 32 + lane;
-            out[c] = unpack_chunk(pay[c], s.scales[ts][c >> 2]);
+            unpack_wide_chunk<WB>(pay[c], s.scales[ts][c >> 2], f16, out, c);
           }
         }
         if (cw == 0 && lane < 4) reinterpret_cast<uint4*>(&s.w_meta[ws])[lane] = reinterpret_cast<const uint4*>(&s.t_meta[ts])[lane];
@@ -358,14 +374,15 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           mbar_arrive(&s.t_empty[ts]);
         }
       } else {
-        mbar_wait(&s.w_full[ws], wp);         // bf16 tile landed
+        mbar_wait(&s.w_full[ws], wp);         // wide tile landed
         mbar_wait(&s.t_empty[ts], tp ^ 1u);   // payload slot released by store + accumulator
         const uint4* in = reinterpret_cast<const uint4*>(s.wide[ws]);
         uint2* pay = reinterpret_cast<uint2*>(s.tile[ts]);
+        const bool f16 = s.w_meta[ws].f16;
 #pragma unroll 4
         for (uint32_t k = 0; k < kPer / 32; ++k) {
           const uint32_t c = cw * kPer + k * 32 + lane;
-          pack_chunk(in[c], &pay[c], &s.scales[ts][c >> 2], (c & 3u) == 0);
+          pack_wide_chunk<WB>(in, c, f16, &pay[c], &s.scales[ts][c >> 2], (c & 3u) == 0);
         }
         if (cw == 0 && lane < 4) reinterpret_cast<uint4*>(&s.t_meta[ts])[lane] = reinterpret_cast<const uint4*>(&s.w_meta[ws])[lane];
         fence_proxy_async_smem();  // generic-proxy writes -> tensor core / TMA store readers
@@ -384,9 +401,20 @@ PerDeviceOnce g_fp_consts;  // __constant__ uploads
 
 }  // namespace
 
-int xfer_fp8_smem_bytes() { return static_cast<int>(sizeof(SmemFp)); }
+int xfer_fp8_smem_bytes(uint32_t wide_bytes) {
+  return static_cast<int>(wide_bytes == 4 ? sizeof(SmemFp<4>) : sizeof(SmemFp<2>));
+}
 
-int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
+template <bool UNPACK, uint32_t WB>
+static cudaError_t launch_fp8_kernel(int dev, int grid, const FpParams& p, cudaStream_t st) {
+  const cudaError_t e = set_max_dynamic_smem_once<bb_xfer_fp8_kernel<UNPACK, WB>>(dev, static_cast<int>(sizeof(SmemFp<WB>)));
+  if (e != cudaSuccess) return e;
+  bb_xfer_fp8_kernel<UNPACK, WB><<<grid, kFpThreads, sizeof(SmemFp<WB>), st>>>(p);
+  return cudaGetLastError();
+}
+
+int launch_xfer_fp8(const XferLaunch& l, bool unpack, uint32_t wide_bytes) {
+  if (wide_bytes != 2 && wide_bytes != 4) return static_cast<int>(cudaErrorInvalidValue);
   if (l.ndesc == 0 || l.total_tiles == 0) return 0;
   int dev = 0;
   cudaError_t e = current_device(&dev);
@@ -396,9 +424,6 @@ int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
     for (uint32_t n = 0; n < tchash::kN; ++n) h[n] = tchash::col_mul(n);
     return cudaMemcpyToSymbol(c_fp_col_mul, h, sizeof h);
   });
-  if (e != cudaSuccess) return static_cast<int>(e);
-  e = unpack ? set_max_dynamic_smem_once<bb_xfer_fp8_kernel<true>>(dev, static_cast<int>(sizeof(SmemFp)))
-             : set_max_dynamic_smem_once<bb_xfer_fp8_kernel<false>>(dev, static_cast<int>(sizeof(SmemFp)));
   if (e != cudaSuccess) return static_cast<int>(e);
   FpParams p;
   p.descs = l.descs;
@@ -410,9 +435,9 @@ int launch_xfer_fp8(const XferLaunch& l, bool unpack) {
   int grid = l.max_ctas > 0 ? l.max_ctas : std::min(current_sm_count(), 128);
   grid = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), l.total_tiles));
   cudaStream_t st = static_cast<cudaStream_t>(l.stream);
-  if (unpack) bb_xfer_fp8_kernel<true><<<grid, kFpThreads, sizeof(SmemFp), st>>>(p);
-  else bb_xfer_fp8_kernel<false><<<grid, kFpThreads, sizeof(SmemFp), st>>>(p);
-  return static_cast<int>(cudaGetLastError());
+  if (wide_bytes == 4) e = unpack ? launch_fp8_kernel<true, 4>(dev, grid, p, st) : launch_fp8_kernel<false, 4>(dev, grid, p, st);
+  else e = unpack ? launch_fp8_kernel<true, 2>(dev, grid, p, st) : launch_fp8_kernel<false, 2>(dev, grid, p, st);
+  return static_cast<int>(e);
 }
 
 }  // namespace bb::gpu

@@ -207,21 +207,28 @@ void bind_common(py::module_& m) {
     if (!v) return py::none();
     return py::int_(*v);
   });
-  m.def("mxfp8_pack_ref", [](py::buffer bf16_bits) {
-    py::buffer_info i = bf16_bits.request();
-    const size_t n = static_cast<size_t>(i.size * i.itemsize) / 2;
+  py::enum_<mxfp8::Wide>(m, "MxWide", "Element type of the wide (unpacked) side of an MXFP8 transfer")
+      .value("BF16", mxfp8::Wide::BF16)
+      .value("F16", mxfp8::Wide::F16)
+      .value("F32", mxfp8::Wide::F32);
+  m.def("mxfp8_wide_bytes", [](mxfp8::Wide w) { return mxfp8::wide_bytes(w); });
+  m.def("mxfp8_pack_ref", [](py::buffer wide_bits, mxfp8::Wide wide) {
+    py::buffer_info i = wide_bits.request();
+    const size_t n = static_cast<size_t>(i.size * i.itemsize) / mxfp8::wide_bytes(wide);
     if (n % 32) throw py::value_error("element count must be a multiple of 32");
     std::string out(mxfp8::packed_bytes(n), '\0');
-    mxfp8::pack_bf16(static_cast<const uint16_t*>(i.ptr), n, reinterpret_cast<uint8_t*>(out.data()));
+    mxfp8::pack(i.ptr, wide, n, reinterpret_cast<uint8_t*>(out.data()));
     return py::bytes(out);
-  }, "CPU reference: bf16 bits -> [E4M3 payload | E8M0 scales]");
-  m.def("mxfp8_unpack_ref", [](py::buffer packed, size_t n) {
+  }, py::arg("wide_bits"), py::arg("wide") = mxfp8::Wide::BF16,
+     "CPU reference: raw bits of n elements of type `wide` (bf16 / fp16 / fp32) -> [E4M3 payload | E8M0 scales]");
+  m.def("mxfp8_unpack_ref", [](py::buffer packed, size_t n, mxfp8::Wide wide) {
     py::buffer_info i = packed.request();
     if (static_cast<size_t>(i.size * i.itemsize) < mxfp8::packed_bytes(n)) throw py::value_error("packed buffer too small");
-    std::string out(n * 2, '\0');
-    mxfp8::unpack_bf16(static_cast<const uint8_t*>(i.ptr), n, reinterpret_cast<uint16_t*>(out.data()));
+    std::string out(n * mxfp8::wide_bytes(wide), '\0');
+    mxfp8::unpack(static_cast<const uint8_t*>(i.ptr), n, wide, out.data());
     return py::bytes(out);
-  });
+  }, py::arg("packed"), py::arg("n"), py::arg("wide") = mxfp8::Wide::BF16,
+     "CPU reference: packed object of n elements -> raw bits of n elements of type `wide`");
   m.def("e4m3_from_float", [](float f) { return mxfp8::float_to_e4m3_sat(f); });
   m.def("e4m3_to_float", [](uint8_t v) { return mxfp8::e4m3_to_float(v); });
   m.def("mxfp8_packed_bytes", [](size_t n) { return mxfp8::packed_bytes(n); });

@@ -1174,62 +1174,68 @@ void bind_control(py::module_& m) {
       .def("migrate", &BlackbirdClient::migrate, py::call_guard<py::gil_scoped_release>())
       .def("batch_put_device_fp8",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
-              const WorkerConfig& cfg, uintptr_t stream) {
-             return ecs_to_py(nogil([&] { return c.batch_put_device_fp8(keys, to_ptrs<const void*>(ptrs), n_elems, cfg, reinterpret_cast<void*>(stream)); }));
+              const WorkerConfig& cfg, uintptr_t stream, mxfp8::Wide wide) {
+             return ecs_to_py(nogil([&] { return c.batch_put_device_fp8(keys, to_ptrs<const void*>(ptrs), n_elems, cfg, reinterpret_cast<void*>(stream), wide); }));
            },
-           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("config"), py::arg("stream") = 0)
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("config"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+           "Tensors of type `wide` (MxWide: bf16, fp16 or fp32; one type per call) packed to MXFP8 in the put kernel.  Every "
+           "fp8 call takes `wide`: its '2 *' bytes and '% 8' elements below are b * and % (16 / b) for b-byte elements.")
       .def("batch_put_device_fp8_strided",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& widths,
-              const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream) {
+              const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, const WorkerConfig& cfg, uintptr_t stream,
+              mxfp8::Wide wide) {
              return ecs_to_py(nogil([&] {
-               return c.batch_put_device_fp8_strided(keys, to_ptrs<const void*>(ptrs), widths, pitches, rows, cfg, reinterpret_cast<void*>(stream));
+               return c.batch_put_device_fp8_strided(keys, to_ptrs<const void*>(ptrs), widths, pitches, rows, cfg, reinterpret_cast<void*>(stream), wide);
              }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("elem_widths"), py::arg("elem_pitches"), py::arg("rows"), py::arg("config"),
-           py::arg("stream") = 0,
+           py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
            "Packed tensor i = rows[i] rows of elem_widths[i] bf16 elements, row r read from bf16_ptrs[i] + 2 * r * "
            "elem_pitches[i]; packed in the put kernel and stored as batch_put_device_fp8 of the compacted rows would store it; "
            "returns one ErrorCode per object (NOT_IMPLEMENTED: make it contiguous and put that).")
       .def("batch_get_device_fp8",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
-              uintptr_t stream) {
-             return ecs_to_py(nogil([&] { return c.batch_get_device_fp8(keys, to_ptrs<void*>(ptrs), n_elems, reinterpret_cast<void*>(stream)); }));
+              uintptr_t stream, mxfp8::Wide wide) {
+             return ecs_to_py(nogil([&] { return c.batch_get_device_fp8(keys, to_ptrs<void*>(ptrs), n_elems, reinterpret_cast<void*>(stream), wide); }));
            },
-           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("stream") = 0)
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16)
       .def("batch_get_device_fp8_range",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
-              const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& counts, uintptr_t stream) {
+              const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& counts, uintptr_t stream, mxfp8::Wide wide) {
              return ecs_to_py(nogil([&] {
-               return c.batch_get_device_fp8_range(keys, to_ptrs<void*>(ptrs), n_elems, offsets, counts, reinterpret_cast<void*>(stream));
+               return c.batch_get_device_fp8_range(keys, to_ptrs<void*>(ptrs), n_elems, offsets, counts, reinterpret_cast<void*>(stream), wide);
              }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_counts"), py::arg("stream") = 0,
+           py::arg("wide") = mxfp8::Wide::BF16,
            "Elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of packed tensor i (n_elems[i] elements), unpacked to "
            "bf16 at bf16_ptrs[i]; the whole packed object is read and verified; returns one ErrorCode per object "
            "(NOT_IMPLEMENTED: read it whole and slice).")
       .def("batch_get_device_fp8_strided",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
-              const std::vector<uint64_t>& rows, uintptr_t stream) {
+              const std::vector<uint64_t>& rows, uintptr_t stream, mxfp8::Wide wide) {
              return ecs_to_py(nogil([&] {
-               return c.batch_get_device_fp8_strided(keys, to_ptrs<void*>(ptrs), n_elems, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream));
+               return c.batch_get_device_fp8_strided(keys, to_ptrs<void*>(ptrs), n_elems, offsets, widths, pitches, rows, reinterpret_cast<void*>(stream),
+                                                     wide);
              }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_widths"),
-           py::arg("elem_pitches"), py::arg("rows"), py::arg("stream") = 0,
+           py::arg("elem_pitches"), py::arg("rows"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
            "rows[i] rows of elem_widths[i] elements of packed tensor i (n_elems[i] elements), row r = elements "
            "[elem_offsets[i] + r * elem_pitches[i], + elem_widths[i]), unpacked to bf16 densely at bf16_ptrs[i] (row r at "
            "bf16_ptrs[i] + 2 * r * elem_widths[i]); the whole packed object is read and verified; returns one ErrorCode per "
            "object (NOT_IMPLEMENTED: read it whole and narrow).")
       .def("batch_get_device_fp8_scatter",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
-              const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, uintptr_t stream) {
+              const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows, uintptr_t stream,
+              mxfp8::Wide wide) {
              return ecs_to_py(nogil([&] {
-               return c.batch_get_device_fp8_scatter(keys, to_ptrs<void*>(ptrs), n_elems, widths, pitches, rows, reinterpret_cast<void*>(stream));
+               return c.batch_get_device_fp8_scatter(keys, to_ptrs<void*>(ptrs), n_elems, widths, pitches, rows, reinterpret_cast<void*>(stream), wide);
              }));
            },
            py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_widths"), py::arg("elem_pitches"), py::arg("rows"),
-           py::arg("stream") = 0,
+           py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
            "Packed tensor i (n_elems[i] == rows[i] * elem_widths[i] elements), unpacked to bf16 into rows[i] rows of "
            "elem_widths[i] elements, row r at bf16_ptrs[i] + 2 * r * elem_pitches[i]; the whole packed object is read and "
            "verified, no element outside the rows is written; returns one ErrorCode per object (NOT_IMPLEMENTED: get it "

@@ -128,12 +128,13 @@ void bind_gpu(py::module_& m) {
            "as the ninth element (the slots before it may be None) sets XFER_SCATTER: object byte x is stored at dst + ((x + "
            "phase) // width) * pitch + (x + phase) % width; returns (digests, status, device_ms).")
       .def("run_fp8",
-           [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream) {
+           [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream, mxfp8::Wide wide) {
              std::vector<gpu::Fp8Item> v;
              for (auto h : items) {
                auto t = h.cast<py::tuple>();
                gpu::Fp8Item it;
                it.wide = reinterpret_cast<void*>(t[0].cast<uintptr_t>());
+               it.wide_type = wide;
                void* packed[kMaxDst] = {nullptr, nullptr, nullptr};
                it.nreplicas = to_ptrs(t[1], packed);
                if (it.nreplicas == 0) throw py::value_error("1..3 packed objects");
@@ -141,14 +142,15 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 7)
+               if (t.size() < 3 || t.size() > 8)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
-                     "scatter (pitch, width, phase)]]]])");
+                     "scatter (pitch, width, phase)[, wide]]]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 5 && !t[5].is_none()) it.rows = to_rows(t[5]);
                if (t.size() > 6 && !t[6].is_none()) it.dst_rows = to_rows(t[6]);
+               if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
                v.push_back(it);
              }
              XferResult res;
@@ -158,8 +160,10 @@ void bind_gpu(py::module_& m) {
              }
              return py::make_tuple(res.digest, res.status, res.device_ms);
            },
-           py::arg("items"), py::arg("unpack"), py::arg("stream") = 0,
-           "Fused MXFP8 put (unpack=False: bf16 -> packed slab object) or get (unpack=True); items = (bf16_ptr, packed_ptr "
+           py::arg("items"), py::arg("unpack"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+           "`wide` (MxWide) is the element type of every item's wide side: bf16, fp16 or fp32, unless an item gives its own as "
+           "the eighth element (a batch mixing 2- and 4-byte types is INVALID_ARGUMENT); below, '2' bytes per element "
+           "and '% 8' elements are those of bf16 and fp16, 4 and % 4 for fp32.  Fused MXFP8 put (unpack=False: bf16 -> packed slab object) or get (unpack=True); items = (bf16_ptr, packed_ptr "
            "| [packed_ptr, ...], n_elems[, expected_digest[, (lo, hi)]]), where a put writes every packed replica in the list "
            "(1..3) and a get reads the first.  A get with a window (lo, hi) reads and verifies the whole packed object but "
            "stores only elements [lo, hi), element x at bf16_ptr + 2x (pass bf16_ptr = buffer - 2 * lo, 16-byte aligned); a "
@@ -248,12 +252,16 @@ void bind_gpu(py::module_& m) {
       py::arg("algo"), py::arg("total_tiles"), py::arg("max_ctas") = 0,
       "Launch geometry of the fused kernel on the current device for a batch of total_tiles 16 KiB tiles: grid, stages, "
       "smem_bytes per CTA and resident_ctas_per_sm (occupancy query); max_ctas as XferEngine.set_max_ctas.");
-  m.def("mxfp8_pack", [](uintptr_t src, uint64_t n, uintptr_t dst, uintptr_t stream) {
-    check_cuda(launch_mxfp8_pack(reinterpret_cast<const void*>(src), n, reinterpret_cast<void*>(dst), reinterpret_cast<void*>(stream)), "mxfp8_pack");
-  }, py::arg("src_bf16"), py::arg("n_elems"), py::arg("dst_packed"), py::arg("stream") = 0);
-  m.def("mxfp8_unpack", [](uintptr_t src, uint64_t n, uintptr_t dst, uintptr_t stream) {
-    check_cuda(launch_mxfp8_unpack(reinterpret_cast<const void*>(src), n, reinterpret_cast<void*>(dst), reinterpret_cast<void*>(stream)), "mxfp8_unpack");
-  }, py::arg("src_packed"), py::arg("n_elems"), py::arg("dst_bf16"), py::arg("stream") = 0);
+  m.def("mxfp8_pack", [](uintptr_t src, uint64_t n, uintptr_t dst, uintptr_t stream, mxfp8::Wide wide) {
+    check_cuda(launch_mxfp8_pack(reinterpret_cast<const void*>(src), n, reinterpret_cast<void*>(dst), reinterpret_cast<void*>(stream), wide), "mxfp8_pack");
+  }, py::arg("src_bf16"), py::arg("n_elems"), py::arg("dst_packed"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+     "n_elems elements of type `wide` (bf16 / fp16 / fp32, 16-byte aligned) -> [E4M3 payload | E8M0 scales]");
+  m.def("mxfp8_unpack", [](uintptr_t src, uint64_t n, uintptr_t dst, uintptr_t stream, mxfp8::Wide wide) {
+    check_cuda(launch_mxfp8_unpack(reinterpret_cast<const void*>(src), n, reinterpret_cast<void*>(dst), reinterpret_cast<void*>(stream), wide), "mxfp8_unpack");
+  }, py::arg("src_packed"), py::arg("n_elems"), py::arg("dst_bf16"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+     "packed object of n_elems elements -> n_elems elements of type `wide` (16-byte aligned)");
+  m.def("xfer_fp8_smem_bytes", [](mxfp8::Wide wide) { return xfer_fp8_smem_bytes(mxfp8::wide_bytes(wide)); }, py::arg("wide") = mxfp8::Wide::BF16,
+        "Dynamic shared memory per CTA of the fused MXFP8 kernel instantiation for `wide`");
 
   // ---- fabric: GPU tier + device transport of the client SDK
   m.def("install_gpu_backend_factory", &install_gpu_backend_factory,
