@@ -1069,8 +1069,8 @@ static void ewma_update(std::atomic<double>& v, double sample) {
 
 // The fused kernels move 16-byte aligned buffers only (XferEngine::submit refuses a whole batch otherwise).  An object
 // whose caller buffer is not aligned with one of its shards is staged through host memory instead, so that it does not
-// fail its neighbours: a put's source where every shard starts (for a strided source, every shard co-aligned), a get's
-// destination by StoreWindow::fused_get_aligned.  Whether ok(off, len) holds for the shard [off, off + len) of every copy.
+// fail its neighbours: a put's source where every shard starts (for a strided or paged source, every shard co-aligned), a
+// get's destination by StoreWindow::fused_get_aligned (SourceRows's or SourcePages's for a get into rows or pages).  Whether ok(off, len) holds for the shard [off, off + len) of every copy.
 template <class F>
 static bool fabric_aligned(const std::vector<CopyPlacement>& copies, F&& ok) {
   for (const auto& c : copies) {
@@ -1110,14 +1110,37 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vect
       });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                               const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream) {
+  const size_t n = keys.size();
+  std::vector<size_t> sizes(n);
+  std::vector<SourcePages> pats(n);
+  return shaped_batch(
+      "device_put_paged", true, n, pages.size() == n && page_bytes.size() == n,
+      [&](size_t i, uint64_t* size) {
+        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &pats[i], size);
+        if (ec != ErrorCode::OK) return ec;
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        sizes[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), nullptr, cfg, stream, &p);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                                    const std::vector<size_t>& sizes, const std::vector<SourceRows>* rows,
-                                                   const WorkerConfig& cfg, void* stream) {
+                                                   const WorkerConfig& cfg, void* stream, const std::vector<SourcePages>* pages) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size() || (rows && rows->size() != keys.size())) return out;
+  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size() || (rows && rows->size() != keys.size()) ||
+      (pages && pages->size() != keys.size()))
+    return out;
   auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
+  auto pages_of = [&](size_t i) { return pages ? (*pages)[i] : SourcePages{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_put_device", keys.size());
 
@@ -1160,8 +1183,10 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
       // placements on host tiers (DRAM / CXL / NVMe) and unaligned caller buffers: stage through host memory and use the
       // data servers
       const SourceRows pat = rows_of(i);
+      const SourcePages pg = pages_of(i);
       const auto src = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
       bool on_fabric = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
+        if (pg.paged()) return pg.rebase(off).coaligned(len);
         uint64_t at = 0;
         return pat.rebase(off, &at).coaligned(src + at, len);
       });
@@ -1192,6 +1217,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
           op.placement = &copies[c].shards[s];
           op.obj_offset = off;
           op.rows = pat.rebase(off, &op.rows_at);
+          op.pages = pg.rebase(off);
           for (size_t r = 1; same_layout && r < copies.size(); ++r) op.replicas.push_back(&copies[r].shards[s]);
           ch.ops.push_back(std::move(op));
           off += copies[c].shards[s].length;
@@ -1267,12 +1293,15 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
   }
   while (finished < chunks.size()) finish_chunk(chunks[finished++]);
   // host-tier placements: D2H into a staging buffer, then the TCP data path (checksums on the CPU).  A strided source is
-  // copied as its whole extent in one D2H, and its rows compacted here.
+  // copied as its whole extent in one D2H, and its rows compacted here; a paged one with one D2H per run of pages.
   for (size_t i : host_put) {
     std::vector<uint8_t> stage(sizes[i]);
     const SourceRows pat = rows_of(i);
+    const SourcePages pg = pages_of(i);
     ErrorCode ec;
-    if (pat.strided()) {
+    if (pg.paged()) {
+      ec = device_->copy_d2h_pages(stage.data(), pg, sizes[i], stream);
+    } else if (pat.strided()) {
       std::vector<uint8_t> extent(pat.extent(sizes[i]));
       ec = device_->copy_d2h(extent.data(), dev_ptrs[i], extent.size(), stream);
       pat.for_each_run(sizes[i], [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(stage.data() + x, extent.data() + at, n); });
@@ -1324,6 +1353,30 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_scatter(const std::vect
       });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                               const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes) {
+  const size_t n = keys.size();
+  std::vector<size_t> caps(n);
+  std::vector<SourcePages> pats(n);
+  if (out_sizes) out_sizes->assign(n, 0);
+  return shaped_batch(
+      "device_get_paged", false, n, pages.size() == n && page_bytes.size() == n,
+      [&](size_t i, uint64_t* size) {
+        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &pats[i], size);
+        if (ec != ErrorCode::OK) return ec;
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        caps[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        std::vector<size_t> sizes;
+        auto ecs = get_device(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(caps, idx), nullptr, nullptr, stream, &sizes, &p);
+        for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
+        return ecs;
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                                const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths,
                                                                void* stream) {
@@ -1362,14 +1415,16 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                    const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges,
-                                                   const std::vector<SourceRows>* rows, void* stream, std::vector<size_t>* out_sizes) {
+                                                   const std::vector<SourceRows>* rows, void* stream, std::vector<size_t>* out_sizes,
+                                                   const std::vector<SourcePages>* pages) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (rows && (ranges || rows->size() != keys.size())))
+      (rows && (ranges || rows->size() != keys.size())) || (pages && (ranges || rows || pages->size() != keys.size())))
     return out;
   auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
+  auto pages_of = [&](size_t i) { return pages ? (*pages)[i] : SourcePages{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_get_device", keys.size());
   if (out_sizes) out_sizes->assign(keys.size(), 0);
@@ -1403,6 +1458,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           op.obj_offset = off;
           if (!whole) op.win = sp.rebase(off, len);
           if (rows) op.rows = (*rows)[i].rebase(off, &op.rows_at);  // a scattered get: the shard's destination rows
+          if (pages) op.pages = (*pages)[i].rebase(off);            // a paged get: the shard's destination pages
           ops.push_back(std::move(op));
         }
         off += len;
@@ -1516,7 +1572,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
       const auto dst = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
       const SourceRows pat = rows_of(i);
+      const SourcePages pg = pages_of(i);
       const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
+        if (pages) return pg.fused_get_aligned(off, len);
         return rows ? pat.fused_get_aligned(dst, off, len) : sp.fused_get_aligned(dst, off, len);
       });
       bool found = false;
@@ -1547,7 +1605,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
         ErrorCode ec = transfer_get(copies, stage.data(), size, sp);
-        if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
+        if (ec == ErrorCode::OK && pages) {  // into the pages: one H2D copy per run of pages
+          ec = device_->copy_h2d_pages(pg, stage.data(), size, stream);
+        } else if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
           std::vector<uint8_t> dense(capacity[i]);
           sp.for_each_run(size, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + at, stage.data() + x, n); });
           ec = device_->copy_h2d(dev_ptrs[i], dense.data(), dense.size(), stream);
@@ -1640,9 +1700,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
     const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
+    const auto rpages = pages ? pick(*pages, r) : std::vector<SourcePages>();
     std::vector<size_t> rsizes;
     auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr,
-                           stream, &rsizes);
+                           stream, &rsizes, pages ? &rpages : nullptr);
     for (size_t k = 0; out_sizes && k < r.size() && k < rsizes.size(); ++k) (*out_sizes)[r[k]] = rsizes[k];
     return recs;
   });
@@ -1666,7 +1727,14 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
     const DeviceShardOp& op = ops[k];
     const auto* src = static_cast<const uint8_t*>(op.src(dev_ptrs[op.item]));
     std::vector<uint8_t> dense;
-    if (op.rows.strided()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows
+    if (op.pages.paged()) {  // as the kernel's paged gathering load: the shard's bytes, compacted from its pages
+      if (!op.pages.valid(op.placement->length) || op.rows.strided()) return ErrorCode::INVALID_ARGUMENT;
+      dense.resize(op.placement->length);
+      op.pages.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) {
+        std::memcpy(dense.data() + x, reinterpret_cast<const void*>(at), n);
+      });
+      src = dense.data();
+    } else if (op.rows.strided()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows
       if (!op.rows.valid()) return ErrorCode::INVALID_ARGUMENT;
       dense.resize(op.placement->length);
       op.rows.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, src + at, n); });
@@ -1687,7 +1755,15 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     ErrorCode ec;
-    if (op.rows.strided()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows
+    if (op.pages.paged()) {  // as the kernel's paged scattering store: the whole shard, read and verified, stored into its pages
+      if (!op.pages.valid(op.placement->length) || op.rows.strided() || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
+      std::vector<uint8_t> whole(op.placement->length);
+      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
+      if (ec == ErrorCode::OK)
+        op.pages.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) {
+          std::memcpy(reinterpret_cast<void*>(at), whole.data() + x, n);
+        });
+    } else if (op.rows.strided()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows
       if (!op.rows.valid() || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);

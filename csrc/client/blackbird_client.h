@@ -69,6 +69,9 @@ struct DeviceShardOp {
   // pattern and a window.
   SourceRows rows;
   uint64_t rows_at = 0;
+  // A put's source pages or a get's destination pages (common/store_window.h), the object's table rebased to obj_offset;
+  // dev_ptrs[item] is not used then.  Never together with rows or a window.
+  SourcePages pages;
   const void* src(const void* obj_base) const {
     return static_cast<const uint8_t*>(obj_base) + (rows.strided() ? rows_at : obj_offset);
   }
@@ -123,6 +126,10 @@ class DeviceTransport {
     return ErrorCode::NOT_IMPLEMENTED;
   }
   virtual ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
+  // Object bytes [0, n) of `pages` (common/store_window.h) from / to n bytes packed back to back at `host`: one copy per
+  // run of pages (SourcePages::for_each_run), synchronous.
+  virtual ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
+  virtual ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
 };
 
 class HostLoopbackTransport;
@@ -278,6 +285,27 @@ class BlackbirdClient {
   std::vector<ErrorCode> batch_get_device_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                   const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                   const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes);
+  // Paged puts (the blocks of a paged KV cache, one object for a whole request): object i is the concatenation of the
+  // pages[i].size() pages of page_bytes[i] bytes at the device addresses pages[i], in list order (SourcePages in
+  // common/store_window.h); one object, one metadata record.  A page may repeat.  The stored object and its digests are
+  // those of batch_put_device of the concatenation, so every get reads it.  The fused path reads each page in place in
+  // the put kernel; it needs every shard of every copy co-aligned (SourcePages::coaligned: 16-byte aligned pages and shard starts and, for
+  // several pages, page_bytes[i] % 16 == 0).  Any other item, and every placement the fabric cannot reach, is staged
+  // through the host (one D2H copy per run of pages) while the rest of the batch keeps the fused launch.  Per object,
+  // before anything is allocated: INVALID_ARGUMENT for page_bytes[i] == 0 with pages; VALUE_OUT_OF_RANGE when the size
+  // overflows.  No pages is a zero-byte object.
+  std::vector<ErrorCode> batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream);
+  // Paged gets, the mirror: object i lands in the pages pages[i] of page_bytes[i] bytes, object byte x in page
+  // x / page_bytes[i] at offset x % page_bytes[i].  The capacity is pages[i].size() * page_bytes[i]: a larger object is
+  // BUFFER_OVERFLOW, a shorter one fills its bytes in page order; out_sizes[i] receives the size.  Only the object's bytes
+  // are written.  Pages of one get must not overlap (not checked).  Every shard is read whole and verified, with the
+  // fail-over and placement refresh of batch_get_device.  The fused path scatters the pages in the get kernel; it needs
+  // SourcePages::fused_get_aligned for every shard of every copy.  Any other item, and every placement the fabric cannot
+  // reach, is staged through the host (one H2D copy per run of pages).  Per object: INVALID_ARGUMENT for
+  // page_bytes[i] == 0 with pages; VALUE_OUT_OF_RANGE when the capacity overflows.
+  std::vector<ErrorCode> batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }
@@ -307,12 +335,17 @@ class BlackbirdClient {
     uint64_t offset = 0, length = 0;
     uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)
   };
-  // batch_put_device and batch_put_device_strided: `rows` null = contiguous sources, else object i is read by (*rows)[i].
+  // batch_put_device, batch_put_device_strided and batch_put_device_paged: `rows` null = contiguous sources, else object i
+  // is read by (*rows)[i]; `pages` non-null = object i is read from the pages (*pages)[i] wherever they are paged (dev_ptrs
+  // are then not read).
   std::vector<ErrorCode> put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs, const std::vector<size_t>& sizes,
-                                    const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream);
+                                    const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream,
+                                    const std::vector<SourcePages>* pages = nullptr);
+  // `pages` (whole objects only, never with `rows`) non-null = object i lands in the pages (*pages)[i] wherever they are
+  // paged.
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, const std::vector<SourceRows>* rows, void* stream,
-                                    std::vector<size_t>* out_sizes);
+                                    std::vector<size_t>* out_sizes, const std::vector<SourcePages>* pages = nullptr);
   // batch_put_device_fp8 and batch_put_device_fp8_strided: `rows` null = contiguous tensors, else object i is read by
   // (*rows)[i], in elements.
   std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
@@ -387,6 +420,18 @@ class HostLoopbackTransport : public DeviceTransport {
   }
   ErrorCode copy_d2h(void* host, const void* dev, size_t n, void*) override {
     std::memcpy(host, dev, n);
+    return ErrorCode::OK;
+  }
+  ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void*) override {
+    pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
+      std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(at), len);
+    });
+    return ErrorCode::OK;
+  }
+  ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void*) override {
+    pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
+      std::memcpy(reinterpret_cast<void*>(at), static_cast<const uint8_t*>(host) + x, len);
+    });
     return ErrorCode::OK;
   }
   size_t max_in_flight() const override { return 2; }

@@ -12,7 +12,7 @@
 // The default window, [0, UINT64_MAX) without a pattern, is the whole object.
 //
 // SourceRows, below, maps a dense object onto strided memory instead: where a put reads each byte from, or where a get into
-// a sliced destination stores it.
+// a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -245,6 +245,85 @@ struct SourceRows {
       f(x, y / width * pitch + c, n);
       x += n;
     }
+  }
+};
+
+// SourcePages: a dense object cut into equal pages of `page` bytes that sit at arbitrary addresses (the blocks of a paged
+// KV cache), on either side of a transfer: the source a device put reads from, or the destination a device get stores
+// into.  Object byte x lives at
+//   addrs[(x + phase) / page] + (x + phase) % page
+// `addrs` is a host array of npages page addresses owned by the caller.  SourceRows is the special case
+// addrs[k] = src + k * pitch (with page = width).  This is the one statement of the rule; the transfer engine (XferItem),
+// the fabric's ops (DeviceShardOp), the client, the host loopback transport and the kernel's XFER_PAGED descriptors
+// (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.
+struct SourcePages {
+  const uint64_t* addrs = nullptr;
+  uint64_t npages = 0, page = 0, phase = 0;
+
+  bool paged() const { return page != 0; }
+  // Pages that object bytes [0, len) touch.
+  uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
+  // Whether the table holds every page of an object of `len` bytes, with phase < page.
+  bool valid(uint64_t len) const { return paged() && phase < page && pages_for(len) <= npages; }
+
+  // The table of `npages` pages of `page` bytes at addrs: an object of *size = npages * page bytes.  INVALID_ARGUMENT for
+  // page == 0 with pages; VALUE_OUT_OF_RANGE when the product overflows.  No pages is a zero-byte object (no table).
+  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, SourcePages* out, uint64_t* size) {
+    *out = {};
+    *size = 0;
+    if (npages == 0) return ErrorCode::OK;
+    if (page == 0) return ErrorCode::INVALID_ARGUMENT;
+    if (__builtin_mul_overflow(npages, page, size)) return ErrorCode::VALUE_OUT_OF_RANGE;
+    *out = {addrs, npages, page, 0};
+    return ErrorCode::OK;
+  }
+
+  // The table seen from object byte `off`: byte x of the result is byte off + x here.  Shards of a striped object may
+  // start mid-page, which the new phase records.
+  SourcePages rebase(uint64_t off) const {
+    if (!paged()) return *this;
+    const uint64_t k = (phase + off) / page;
+    return {addrs + std::min(k, npages), npages - std::min(k, npages), page, (phase + off) % page};
+  }
+
+  // Whether object bytes [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by
+  // TMA: byte x of page k lives at addrs[k] + phase - k * page + x, so addrs[k] + phase must be 16-byte aligned for every
+  // page touched, and the page a multiple of 16 bytes when more than one page is touched.  (With phase % 16 == 0, as for
+  // a table cut at 16-byte shard starts, that is every page 16-byte aligned.)
+  bool coaligned(uint64_t len) const {
+    const uint64_t n = pages_for(len);
+    if (n > 1 && page % 16) return false;
+    for (uint64_t k = 0; k < n; ++k)
+      if ((addrs[k] + phase) % 16) return false;
+    return true;
+  }
+
+  // The client's rule for whether a device get into these pages may take the fused path as far as the shard
+  // [off, off + len) of a copy goes; the get is fused only if every shard of every copy passes.  The page must be a
+  // multiple of 16 bytes whenever the table has more than one page, even where a shard touches a single page, so that
+  // whether a get is fused depends on the call, not on where the placement cut the object (as
+  // SourceRows::fused_get_aligned).
+  bool fused_get_aligned(uint64_t off, uint64_t len) const {
+    if (npages > 1 && page % 16) return false;
+    return rebase(off).coaligned(len);
+  }
+
+  // Calls f(x, addr, n) for every run of n contiguous bytes of object bytes [0, len): object bytes [x, x + n) live at
+  // [addr, addr + n), in order.  Pages that follow one another in memory make one run.
+  template <class F>
+  void for_each_run(uint64_t len, F&& f) const {
+    uint64_t x = 0, run_x = 0, run_at = 0, run_n = 0;
+    for (uint64_t k = 0; x < len; ++k) {
+      const uint64_t c = k == 0 ? phase : 0, n = std::min(page - c, len - x), at = addrs[k] + c;
+      if (run_n && run_at + run_n == at) {
+        run_n += n;
+      } else {
+        if (run_n) f(run_x, run_at, run_n);
+        run_x = x, run_at = at, run_n = n;
+      }
+      x += n;
+    }
+    if (run_n) f(run_x, run_at, run_n);
   }
 };
 

@@ -532,6 +532,31 @@ ErrorCode GpuFabric::copy_d2h(void* host, const void* dev, size_t n, void* strea
   return ErrorCode::OK;
 }
 
+// One async copy per run of pages, then one synchronise.
+ErrorCode GpuFabric::copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
+  bool ok = true;
+  pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
+    ok = ok && cuda_ok(cudaMemcpyAsync(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(at), len, cudaMemcpyDeviceToHost, st),
+                       "D2H pages");
+  });
+  if (!cuda_ok(cudaStreamSynchronize(st), "sync") || !ok) return ErrorCode::FABRIC_ERROR;
+  return ErrorCode::OK;
+}
+
+ErrorCode GpuFabric::copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
+  bool ok = true;
+  pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
+    ok = ok && cuda_ok(cudaMemcpyAsync(reinterpret_cast<void*>(at), static_cast<const uint8_t*>(host) + x, len, cudaMemcpyHostToDevice, st),
+                       "H2D pages");
+  });
+  if (!cuda_ok(cudaStreamSynchronize(st), "sync") || !ok) return ErrorCode::FABRIC_ERROR;
+  return ErrorCode::OK;
+}
+
 ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs,
                                      std::vector<XferItem>* items, std::vector<size_t>* op_of_item) {
   items->reserve(ops.size());
@@ -543,6 +568,11 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
     if (op.rows.strided()) {  // a gathered put: every pass and the multicast item read the same rows
       it.rows = op.rows;
       it.flags |= XFER_GATHER;
+    }
+    if (op.pages.paged()) {  // a paged put: the same, from the shard's pages
+      it.src = nullptr;
+      it.pages = op.pages;
+      it.flags |= XFER_GATHER | XFER_PAGED;
     }
     // NVLS: the replica set is one whole multicast group at one offset -> a single multimem.st stream
     if (arena_ && !op.replicas.empty() && (it.nbytes & 15) == 0) {
@@ -586,7 +616,8 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
       more.src = it.src;
       more.nbytes = it.nbytes;
       more.rows = it.rows;
-      more.flags = it.flags & XFER_GATHER;
+      more.pages = it.pages;
+      more.flags = it.flags & (XFER_GATHER | XFER_PAGED);
       more.ndst = 0;
       for (; r < op.replicas.size() && more.ndst < kMaxDst; ++r) {
         auto d = resolve(*op.replicas[r]);
@@ -717,6 +748,11 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
       it.flags |= XFER_SCATTER;
       it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.rows_at;
       it.dst_rows = op.rows;
+    }
+    if (op.pages.paged()) {  // a get into pages: the shard's table, rebased to its first byte
+      it.flags |= XFER_SCATTER | XFER_PAGED;
+      it.dst[0] = nullptr;
+      it.dst_pages = op.pages;
     }
     items->push_back(it);
     op_of_item->push_back(k);

@@ -88,6 +88,8 @@ class GpuFabric : public client::DeviceTransport {
   ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) override;
   ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) override;
   ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) override;
+  ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) override;
+  ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) override;
 
   // Re-reads the pool registry from the keystone and maps any new GPU slab.
   ErrorCode refresh_pools();

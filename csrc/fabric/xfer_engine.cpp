@@ -38,8 +38,10 @@ struct SlotRelease {
   ~SlotRelease() { ticket = 0; }
 };
 
-// A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items].
+// A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items |
+// page entries, only for batches with paged items].
 size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
+size_t page_table_offset(size_t nd) { return stride_table_offset(nd) + nd * sizeof(XferStride); }
 }  // namespace
 
 struct XferEngine::Slot {
@@ -49,10 +51,11 @@ struct XferEngine::Slot {
     FLAG,     // the kernel's status words in pinned memory; no event on the stream (small-object latency path)
     MAILBOX,  // served by the resident mailbox warp: results arrive in the mailbox's result ring
   };
-  // host (pinned): [descs | tile_start]
+  // host (pinned): [descs | tile_start | strides | pages], tab_bytes each way
   uint8_t* h_tab = nullptr;
   // device
   uint8_t* d_tab = nullptr;
+  size_t tab_bytes = 0;
   uint64_t* d_sum = nullptr;
   uint32_t* d_done = nullptr;
   uint64_t* d_digest = nullptr;
@@ -93,6 +96,15 @@ struct XferEngine::Slot {
     std::memcpy(h_tab + stride_table_offset(nd), strides.data(), static_cast<size_t>(nd) * sizeof(XferStride));
     return stride_table_offset(nd) + static_cast<size_t>(nd) * sizeof(XferStride);
   }
+  // The page entries of the batch's XFER_PAGED descriptors, back to back; each one's stride entry holds the index of its
+  // first entry here until write_pages() turns it into a device address.
+  std::vector<uint64_t> pages;
+  std::vector<uint32_t> paged_descs;
+  void add_pages(uint32_t k, const SourcePages& p, uint64_t nbytes) {
+    set_stride(k, XferStride{{pages.size()}, p.page, p.phase});
+    paged_descs.push_back(k);
+    pages.insert(pages.end(), p.addrs, p.addrs + p.pages_for(nbytes));
+  }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
     uint32_t item;
@@ -117,6 +129,7 @@ Result<std::unique_ptr<XferEngine>> XferEngine::create(int device, uint32_t max_
     ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_tab), tab_bytes) == cudaSuccess;
     ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_res), res_bytes) == cudaSuccess;
     ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_tab), tab_bytes) == cudaSuccess;
+    s->tab_bytes = tab_bytes;
     ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_sum), static_cast<size_t>(max_items) * 8) == cudaSuccess;
     ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_done), static_cast<size_t>(max_items) * 4) == cudaSuccess;
     ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_digest), static_cast<size_t>(max_items) * 8) == cudaSuccess;
@@ -309,6 +322,37 @@ ErrorCode XferEngine::write_tile_table(Slot* s, uint32_t nd) {
   return ErrorCode::OK;
 }
 
+// Appends the batch's page entries to the slot's table of `nd` descriptors (written up to tile_start), growing both
+// copies of the table first when they are too small (the slot is idle: nothing reads them), and points every paged
+// descriptor's stride entry at its first entry in the device copy.  *tab: the bytes of the table to copy to the device.
+ErrorCode XferEngine::write_pages(Slot* s, uint32_t nd, size_t* tab) {
+  const size_t off = page_table_offset(nd), need = off + s->pages.size() * sizeof(uint64_t);
+  if (need > s->tab_bytes) {
+    // both new buffers first: on a failure the slot keeps its old, still valid pair
+    uint8_t *h = nullptr, *d = nullptr;
+    const cudaError_t eh = cudaMallocHost(reinterpret_cast<void**>(&h), need);
+    const cudaError_t ed = eh == cudaSuccess ? cudaMalloc(reinterpret_cast<void**>(&d), need) : eh;
+    if (ed != cudaSuccess) {
+      if (h) cudaFreeHost(h);
+      cudaGetLastError();
+      BB_LOG(ERROR) << "XferEngine: growing a descriptor table to " << need << " bytes failed: " << cudaGetErrorString(ed);
+      return ErrorCode::OUT_OF_MEMORY;
+    }
+    std::memcpy(h, s->h_tab, stride_table_offset(nd));
+    cudaFreeHost(s->h_tab);
+    cudaFree(s->d_tab);
+    s->h_tab = h;
+    s->d_tab = d;
+    s->tab_bytes = need;
+  }
+  const auto d_pages = reinterpret_cast<uint64_t>(s->d_tab + off);
+  for (uint32_t k : s->paged_descs) s->strides[k].pages = d_pages + s->strides[k].pages * sizeof(uint64_t);
+  s->write_strides(nd);
+  std::memcpy(s->h_tab + off, s->pages.data(), s->pages.size() * sizeof(uint64_t));
+  *tab = need;
+  return ErrorCode::OK;
+}
+
 Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream,
                                     bool capture_debug) {
   if (items.size() > max_items_) return ErrorCode::RESOURCE_EXHAUSTED;
@@ -319,6 +363,8 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   s->item_to_desc.assign(items.size(), -1);
   s->empties.clear();
   s->strides.clear();
+  s->pages.clear();
+  s->paged_descs.clear();
   uint32_t nd = 0;
   bool all_small = small_path_enabled();
   for (size_t i = 0; i < items.size(); ++i) {
@@ -327,13 +373,20 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const bool strided = it.flags & XFER_STRIDED;
     const bool gather = it.flags & XFER_GATHER;
     const bool scatter = it.flags & XFER_SCATTER;
+    const bool src_paged = it.pages.paged(), dst_paged = it.dst_pages.paged();
     if ((strided && !win) || (win && (strided != it.win.strided() || !it.win.valid(it.nbytes) || it.ndst != 1 ||
                                       (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
-    if (gather != it.rows.strided() || (gather && (!it.rows.valid() || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM)))))
+    // pages are the gathering load's source or the scattering store's destination, instead of rows on the same side
+    if (static_cast<bool>(it.flags & XFER_PAGED) != (src_paged || dst_paged) || (src_paged && (dst_paged || it.rows.strided())) ||
+        (dst_paged && it.dst_rows.strided()) || (src_paged && !it.pages.valid(it.nbytes)) ||
+        (dst_paged && !it.dst_pages.valid(it.nbytes)))
       return ErrorCode::INVALID_ARGUMENT;
-    if (scatter != it.dst_rows.strided() ||
-        (scatter && (!it.dst_rows.valid() || it.ndst != 1 ||
+    if (gather != (it.rows.strided() || src_paged) ||
+        (gather && ((!src_paged && !it.rows.valid()) || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM)))))
+      return ErrorCode::INVALID_ARGUMENT;
+    if (scatter != (it.dst_rows.strided() || dst_paged) ||
+        (scatter && ((!dst_paged && !it.dst_rows.valid()) || it.ndst != 1 ||
                      (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
@@ -352,8 +405,8 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     // strided and scattered: rows instead
     for (uint32_t r = strided || scatter ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
     if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]))) ||
-        (gather && !it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes)) ||
-        (scatter && !it.dst_rows.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]), it.nbytes)))
+        (gather && !(src_paged ? it.pages.coaligned(it.nbytes) : it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes))) ||
+        (scatter && !(dst_paged ? it.dst_pages.coaligned(it.nbytes) : it.dst_rows.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]), it.nbytes))))
       return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
@@ -366,8 +419,10 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       d.win.hi = w.hi;
       if (strided) s->set_stride(nd, w);
     }
-    if (gather) s->set_stride(nd, it.rows);
-    if (scatter) s->set_stride(nd, it.dst_rows);
+    if (src_paged) s->add_pages(nd, it.pages, nbytes);
+    else if (dst_paged) s->add_pages(nd, it.dst_pages, nbytes);
+    else if (gather) s->set_stride(nd, it.rows);
+    else if (scatter) s->set_stride(nd, it.dst_rows);
     d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;
@@ -381,7 +436,10 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   }
   BB_TRY(write_tile_table(s, nd));
   const bool any_strided = !s->strides.empty();
-  const size_t tab = s->write_strides(nd);
+  size_t tab = 0;
+  if (s->pages.empty()) tab = s->write_strides(nd);
+  else BB_TRY(write_pages(s, nd, &tab));
+  descs = reinterpret_cast<XferDesc*>(s->h_tab);  // write_pages may have moved the table
   s->nitems = static_cast<uint32_t>(items.size());
   s->debug = capture_debug;
   s->traced = tile_trace_;
@@ -418,7 +476,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     return s->ticket;
   }
   if (nd) {
-    const bool inline_tab = nd <= kInlineDescs;
+    const bool inline_tab = nd <= kInlineDescs && s->pages.empty();  // page entries live in the device table only
     if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
     if (capture_debug) {
       const size_t need = static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN * 4;

@@ -40,6 +40,15 @@ struct XferItem {
   // XFER_STRIDED, XFER_GATHER, XFER_MULTIMEM, XFER_RAW_SUM or ndst != 1; INVALID_ADDRESS unless
   // dst_rows.coaligned(dst[0], nbytes), which replaces the 16-byte alignment check of dst[0].
   SourceRows dst_rows;
+  // Paged put source (with XFER_GATHER) or paged get destination (with XFER_SCATTER), XFER_PAGED exactly when one of them
+  // is set (common/store_window.h): object byte x at addrs[(x + phase) / page] + (x + phase) % page; src, or dst[0], is
+  // not read.  The page entries are copied into the batch's device table by submit(), so the host array need only live
+  // until submit() returns.  INVALID_ARGUMENT for both at once, a table too short for nbytes or phase >= page, pages
+  // together with a SourceRows pattern on the same side, or XFER_PAGED without its XFER_GATHER / XFER_SCATTER, with
+  // XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM; the destination rules are those of rows / dst_rows.  INVALID_ADDRESS
+  // unless the pages are coaligned(nbytes).
+  SourcePages pages;
+  SourcePages dst_pages;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span
@@ -137,6 +146,7 @@ class XferEngine {
   XferEngine() = default;
   Slot* free_slot();
   ErrorCode write_tile_table(Slot* s, uint32_t nd);
+  ErrorCode write_pages(Slot* s, uint32_t nd, size_t* tab);
   ErrorCode cuda_failed(int code, const char* what);
   int device_ = 0;
   uint32_t max_items_ = 0;

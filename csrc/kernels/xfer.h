@@ -49,6 +49,13 @@ enum XferFlags : uint32_t {
   // the kernel.  A batch of bf16 and fp16 items is one launch; fp32 items take the 4-byte instantiation, a launch of their
   // own.
   XFER_WIDE_F16 = 1u << 7,
+  // Paged source or destination, in bb_xfer only, together with XFER_GATHER (a put reads its pages) or XFER_SCATTER (a get
+  // stores into them): the rule of SourcePages (common/store_window.h), object byte x at
+  // pages[(x + phase) / page] + (x + phase) % page.  The descriptor's XferStride entry is {device address of its first
+  // page entry, page, phase}; `src` (put) or dst[0] (get) is not read.  The destination forms are those of XFER_GATHER
+  // or XFER_SCATTER; never with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM.  The tile in shared memory is the dense
+  // object's tile, so the digest, the verify and the stored bytes are those of a contiguous put or get.
+  XFER_PAGED = 1u << 8,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -81,9 +88,15 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 // object byte x congruent to x mod 16), so that the kernel only bulk-stores 16-byte congruent spans.  An XFER_GATHER
 // descriptor's entry is its source rows instead: 0 < width <= pitch, phase < width, and the source of object byte x
 // congruent to x mod 16 (SourceRows::coaligned).  An XFER_SCATTER descriptor's entry is its destination rows, under the
-// same rules.
+// same rules.  An XFER_PAGED descriptor's entry is {pages, page, phase}: `pages` the device address of the first of its
+// page entries (uint64_t addresses, one per page the descriptor touches), `page` in `width`, phase < page, every page
+// co-aligned: pages[k] + phase 16-byte aligned (SourcePages::coaligned).
 struct XferStride {
-  uint64_t pitch, width, phase;
+  union {
+    uint64_t pitch;
+    uint64_t pages;  // XFER_PAGED
+  };
+  uint64_t width, phase;
 };
 
 constexpr uint32_t kSmallBytes = 4096;     // objects up to this size may take the warp-per-object path (xfer_small.cu)
@@ -111,7 +124,7 @@ struct XferLaunch {
   const uint32_t* host_tile_start = nullptr;
   // Row patterns of the XFER_STRIDED, XFER_GATHER and XFER_SCATTER descriptors, one entry per descriptor (the entries of unflagged
   // descriptors are never read); null when the batch has none.  host_strides is their copy for the kernel parameters of an
-  // inline batch.
+  // inline batch; a batch with XFER_PAGED descriptors has no inline copy (their entries point into device memory).
   const XferStride* strides = nullptr;
   const XferStride* host_strides = nullptr;
   int algo = ALGO_BBH64;

@@ -162,15 +162,23 @@ __device__ __forceinline__ void store_row_segments(const uint8_t* tile, uint64_t
 __device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t r, const XferStride& st) {
   return src + off + st.phase + r * (st.pitch - st.width);
 }
+// The same for a paged descriptor (XFER_PAGED, entry {pages, page, phase}): row r of the dense layout is page r, which
+// starts at pages[r], so tile byte o of it sits at pages[r] + off + phase - r * page + o.  `base` is ignored.
+template <bool PAGED>
+__device__ __forceinline__ uint64_t row_addr(uint64_t base, uint64_t off, uint64_t r, const XferStride& st) {
+  if constexpr (PAGED) return __ldg(reinterpret_cast<const unsigned long long*>(st.pages) + r) + off + st.phase - r * st.width;
+  else return row_src(base, off, r, st);
+}
 // The producer's part of a gathered tile: the row segments of the tile, one per lane, the middle bulk-loaded into `tile`
 // with completion on `bar`, head and tail by plain loads and shared stores.  Returns the bytes this lane's bulk loads
 // deliver; the caller sums them over the warp for the stage's expect_tx, and the calling lane still has to fence its
-// shared stores for the async proxy.
+// shared stores for the async proxy.  PAGED: the rows are the pages of an XFER_PAGED descriptor (row_addr).
+template <bool PAGED = false>
 __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t* bar, uint64_t src, uint64_t off, uint32_t bytes,
                                                         const XferStride& st, uint32_t lane) {
   uint32_t tx = 0;
-  for_row_segments(off, 0, bytes, XferStride{st.width, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
-    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_src(src, off, r, st));
+  for_row_segments(off, 0, bytes, XferStride{{st.width}, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_addr<PAGED>(src, off, r, st));
     if (g.a1 > g.a0) {
       ptx::bulk_g2s(tile + g.a0, s + g.a0, g.a1 - g.a0, bar);
       tx += g.a1 - g.a0;
@@ -183,11 +191,13 @@ __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t*
 // The store warp's part of a scattered tile (XFER_SCATTER, destination rows `st`), the mirror of gather_row_segments: the
 // tile's `bytes` object bytes from `off`, in the object's dense layout {width, width, phase}, one row segment per lane,
 // each stored at row_src(dst0, ...) as a TMA middle plus a byte-wise head and tail.  dst0 is the descriptor's dst[0], where
-// the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.
+// the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.  PAGED: the rows are
+// the pages of an XFER_PAGED descriptor (row_addr), dst0 is not read.
+template <bool PAGED = false>
 __device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t bytes,
                                                      const XferStride& st, uint32_t lane) {
-  for_row_segments(off, 0, bytes, XferStride{st.width, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
-    store_segment(reinterpret_cast<uint8_t*>(row_src(dst0, off, r, st)), tile, g);
+  for_row_segments(off, 0, bytes, XferStride{{st.width}, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    store_segment(reinterpret_cast<uint8_t*>(row_addr<PAGED>(dst0, off, r, st)), tile, g);
   });
 }
 // The row pattern of descriptor `i` from a device table (read-only path).

@@ -9,13 +9,15 @@
 //                      tiles, `cp.async.bulk` global -> shared (TMA, mbarrier complete_tx).
 //                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).  A gathering load
 //                      (XFER_GATHER: a put of a strided source) fills the tile from its source row segments, one per
-//                      lane, so the tile is byte for byte the tile of the dense object.
+//                      lane, so the tile is byte for byte the tile of the dense object.  A paged one (XFER_PAGED)
+//                      reads each row segment from its page, whose address it loads from the page table.
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
 //                      to an NVLS multicast address (one store, N replicas).  A store window (XFER_WINDOW) cuts
 //                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.  A
 //                      scattering store (XFER_SCATTER: a get into a strided destination) stores the whole tile as
-//                      the row segments of the destination rows, one per lane.
+//                      the row segments of the destination rows, one per lane; a paged one (XFER_PAGED) as the
+//                      segments of its pages.
 //   warp 3  finalizer: folds the per-tile partials into per-object digests in registers; an
 //                      object that lives entirely inside this CTA's run is finalised with no
 //                      global atomics; only the <=2 objects straddling a CTA boundary use them.
@@ -298,7 +300,10 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
             if (p.use_inline) gst = p.inl_strides[g_desc];
             else gst = load_stride(p.strides, g_desc);
           }
-          tx = __reduce_add_sync(0xffffffffu, gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane));
+          const uint32_t seg_tx = (e.m.ndst_flags >> 8) & XFER_PAGED
+                                      ? gather_row_segments<true>(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane)
+                                      : gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane);
+          tx = __reduce_add_sync(0xffffffffu, seg_tx);
           wrote = true;
         } else if (lane < tail) {
           s.tile[stage][b16 + lane] = *reinterpret_cast<const uint8_t*>(src_i + off + b16 + lane);
@@ -349,7 +354,8 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
           if (p.use_inline) st = p.inl_strides[st_desc];
           else st = load_stride(p.strides, st_desc);
         }
-        if (flags & XFER_SCATTER) scatter_row_segments(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
+        if (flags & XFER_PAGED) scatter_row_segments<true>(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
+        else if (flags & XFER_SCATTER) scatter_row_segments(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
         else store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);
       } else if (flags & XFER_MULTIMEM) {
         uint8_t* mc = reinterpret_cast<uint8_t*>(m.dst[0] + off);

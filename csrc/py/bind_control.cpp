@@ -1,6 +1,7 @@
 // Python bindings of the control plane: types, allocator, coordination store, keystone, RPC,
 // worker + storage backends, client SDK.  Result<T> maps to "value or raise BlackbirdError".
 #include <pybind11/functional.h>
+#include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
@@ -50,6 +51,26 @@ std::vector<P> to_ptrs(const std::vector<uintptr_t>& v) {
   for (auto p : v) out.push_back(reinterpret_cast<P>(p));
   return out;
 }
+
+// A page-address list given as a 1-D integer array-like: a numpy array or CPU tensor is copied as a block, a list element
+// by element.
+std::vector<uint64_t> to_page_addrs(const py::handle& h) {
+  auto a = py::array_t<uint64_t, py::array::c_style | py::array::forcecast>::ensure(h);
+  if (!a) throw py::type_error("a page list is a 1-D integer array-like (list, numpy array or CPU tensor)");
+  if (a.ndim() != 1) throw py::value_error("a page list is one-dimensional");
+  return std::vector<uint64_t>(a.data(), a.data() + a.size());
+}
+std::vector<std::vector<uint64_t>> to_page_lists(const py::sequence& s) {
+  std::vector<std::vector<uint64_t>> out;
+  out.reserve(s.size());
+  for (auto h : s) out.push_back(to_page_addrs(h));
+  return out;
+}
+// SourcePages for Python: the table owns its page addresses (a rebased table shares them).
+struct PyPages {
+  std::shared_ptr<const std::vector<uint64_t>> addrs;
+  SourcePages p;
+};
 
 // list[ErrorCode] for batch results.  pybind builds a fresh enum instance per element (~0.3 us); a batch of thousands of
 // objects gets the cached instance of each code instead (enum members are immutable).  GIL held.
@@ -388,6 +409,37 @@ void bind_control(py::module_& m) {
              return out;
            },
            py::arg("len"), "[(x, at, n)]: object bytes [x, x + n) are read from source bytes [at, at + n)");
+  py::class_<PyPages>(m, "SourcePages",
+                      "A dense object cut into equal pages at arbitrary addresses: a paged device put's source, or a paged get's "
+                      "destination (common/store_window.h).  Object byte x lives at addrs[(x + phase) // page] + (x + phase) % page.")
+      .def_property_readonly("npages", [](const PyPages& t) { return t.p.npages; })
+      .def_property_readonly("page", [](const PyPages& t) { return t.p.page; })
+      .def_property_readonly("phase", [](const PyPages& t) { return t.p.phase; })
+      .def_property_readonly("addrs", [](const PyPages& t) { return std::vector<uint64_t>(t.p.addrs, t.p.addrs + t.p.npages); })
+      .def("paged", [](const PyPages& t) { return t.p.paged(); })
+      .def("valid", [](const PyPages& t, uint64_t len) { return t.p.valid(len); }, py::arg("len"))
+      .def_static("from_pages",
+                  [](const py::handle& addrs, uint64_t page) {
+                    auto v = std::make_shared<const std::vector<uint64_t>>(to_page_addrs(addrs));
+                    PyPages t{v, {}};
+                    uint64_t size = 0;
+                    const ErrorCode ec = SourcePages::from_pages(v->size(), page, v->data(), &t.p, &size);
+                    return py::make_tuple(ec, t, size);
+                  },
+                  py::arg("addrs"), py::arg("page"), "(ErrorCode, SourcePages, object bytes)")
+      .def("rebase", [](const PyPages& t, uint64_t off) { return PyPages{t.addrs, t.p.rebase(off)}; }, py::arg("off"),
+           "the table seen from object byte off")
+      .def("coaligned", [](const PyPages& t, uint64_t len) { return t.p.coaligned(len); }, py::arg("len"))
+      .def("fused_get_aligned", [](const PyPages& t, uint64_t off, uint64_t len) { return t.p.fused_get_aligned(off, len); },
+           py::arg("off"), py::arg("len"))
+      .def("runs",
+           [](const PyPages& t, uint64_t len) {
+             if (len > 0 && !t.p.valid(len)) throw py::value_error("the table does not hold len bytes");
+             std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> out;
+             t.p.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { out.emplace_back(x, at, n); });
+             return out;
+           },
+           py::arg("len"), "[(x, addr, n)]: object bytes [x, x + n) live at [addr, addr + n); adjacent pages make one run");
 
   using alloc::PoolAllocator;
   using alloc::Range;
@@ -1317,6 +1369,24 @@ void bind_control(py::module_& m) {
          "Object i into rows[i] rows of widths[i] bytes, row r at dev_ptrs[i] + r * pitches[i] (capacity rows[i] * "
          "widths[i]); every shard is read whole and verified, no byte outside the rows is written; returns (one ErrorCode "
          "per object, object sizes).")
+      .def("batch_put_device_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
+                                        const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, uintptr_t stream) {
+        const auto lists = to_page_lists(pages);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_paged(keys, lists, page_bytes, cfg, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
+         "Object i = the len(pages[i]) pages of page_bytes[i] bytes at the device addresses pages[i] (each a 1-D integer "
+         "array-like: list, numpy array or CPU tensor), concatenated in order; stored as a put of the concatenation would "
+         "store it; returns one ErrorCode per object.")
+      .def("batch_get_device_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
+                                        const std::vector<uint64_t>& page_bytes, uintptr_t stream) {
+        const auto lists = to_page_lists(pages);
+        std::vector<size_t> sizes;
+        const auto ecs = nogil([&] { return c.batch_get_device_paged(keys, lists, page_bytes, reinterpret_cast<void*>(stream), &sizes); });
+        return py::make_tuple(ecs_to_py(ecs), sizes);
+      }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("stream") = 0,
+         "Object i into the pages pages[i] of page_bytes[i] bytes, byte x in page x // page_bytes[i] (capacity len(pages[i]) "
+         "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; pages of one get "
+         "must not overlap (not checked); returns (one ErrorCode per object, object sizes).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

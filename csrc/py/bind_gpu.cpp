@@ -4,6 +4,8 @@
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
 
+#include <deque>
+
 #include "client/blackbird_client.h"
 #include "fabric/gpu_fabric.h"
 #include "fabric/xfer_engine.h"
@@ -50,16 +52,25 @@ SourceRows to_rows(const py::handle& h) {
   if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
   return {g[0], g[1], g[2]};
 }
-// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None).  An
-// empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects it without that flag).  A window sets
-// XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern (pitch, width, phase) sets XFER_GATHER, with
-// src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.
-XferItem to_item(const py::handle& h) {
+// A page table (common/store_window.h) given as (addrs, page, phase); the addresses are kept in `keep` until the batch
+// has been submitted.
+SourcePages to_pages(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
+  auto t = py::cast<py::tuple>(h);
+  if (t.size() != 3) throw py::value_error("pages = (addrs, page, phase)");
+  keep.push_back(t[0].cast<std::vector<uint64_t>>());
+  return {keep.back().data(), keep.back().size(), t[1].cast<uint64_t>(), t[2].cast<uint64_t>()};
+}
+// item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None,
+// src_pages=None, dst_pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
+// it without that flag).  A window sets XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern
+// (pitch, width, phase) sets XFER_GATHER, with src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.  Source
+// pages (addrs, page, phase) set XFER_GATHER | XFER_PAGED, destination pages XFER_SCATTER | XFER_PAGED.
+XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 9)
+  if (t.size() < 3 || t.size() > 11)
     throw py::value_error(
         "xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, gather (pitch, width, phase)[, scatter "
-        "(pitch, width, phase)]]]]]])");
+        "(pitch, width, phase)[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]]])");
   XferItem it;
   it.src = reinterpret_cast<const void*>(t[0].cast<uintptr_t>());
   it.ndst = to_ptrs(t[1], it.dst);
@@ -76,6 +87,14 @@ XferItem to_item(const py::handle& h) {
     it.dst_rows = to_rows(t[8]);
     it.flags |= XFER_SCATTER;
   }
+  if (t.size() > 9 && !t[9].is_none()) {
+    it.pages = to_pages(t[9], keep);
+    it.flags |= XFER_GATHER | XFER_PAGED;
+  }
+  if (t.size() > 10 && !t[10].is_none()) {
+    it.dst_pages = to_pages(t[10], keep);
+    it.flags |= XFER_SCATTER | XFER_PAGED;
+  }
   return it;
 }
 }  // namespace
@@ -89,6 +108,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_STRIDED") = static_cast<uint32_t>(XFER_STRIDED);
   m.attr("XFER_GATHER") = static_cast<uint32_t>(XFER_GATHER);
   m.attr("XFER_SCATTER") = static_cast<uint32_t>(XFER_SCATTER);
+  m.attr("XFER_PAGED") = static_cast<uint32_t>(XFER_PAGED);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -105,8 +125,9 @@ void bind_gpu(py::module_& m) {
       .def("run",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream, bool debug) {
              std::vector<XferItem> v;
+             std::deque<std::vector<uint64_t>> keep;
              v.reserve(items.size());
-             for (auto h : items) v.push_back(to_item(h));
+             for (auto h : items) v.push_back(to_item(h, keep));
              XferResult res;
              {
                py::gil_scoped_release rel;
@@ -126,7 +147,10 @@ void bind_gpu(py::module_& m) {
            "pitch) * width + c.  A gather pattern (pitch, width, phase) as the eighth element sets XFER_GATHER: object byte x "
            "is read from src + ((x + phase) // width) * pitch + (x + phase) % width.  A scatter pattern (pitch, width, phase) "
            "as the ninth element (the slots before it may be None) sets XFER_SCATTER: object byte x is stored at dst + ((x + "
-           "phase) // width) * pitch + (x + phase) % width; returns (digests, status, device_ms).")
+           "phase) // width) * pitch + (x + phase) % width.  Source pages (addrs, page, phase) as the tenth element set "
+           "XFER_GATHER | XFER_PAGED: object byte x is read from addrs[(x + phase) // page] + (x + phase) % page (src is "
+           "not read); destination pages as the eleventh set XFER_SCATTER | XFER_PAGED and store by the same rule (dst is "
+           "not read); returns (digests, status, device_ms).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream, mxfp8::Wide wide) {
              std::vector<gpu::Fp8Item> v;
@@ -184,8 +208,9 @@ void bind_gpu(py::module_& m) {
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
              std::vector<XferItem> v;
+             std::deque<std::vector<uint64_t>> keep;
              v.reserve(items.size());
-             for (auto h : items) v.push_back(to_item(h));
+             for (auto h : items) v.push_back(to_item(h, keep));
              auto t = e.submit(v, algo, reinterpret_cast<void*>(stream));
              if (!t.ok()) check(t.error(), "XferEngine.submit");
              return t.value();
