@@ -27,6 +27,11 @@ _MX_WIDE = {torch.bfloat16: _bb.MxWide.BF16, torch.float16: _bb.MxWide.F16, torc
 # they win from 32 KiB pages (XXH3 put 1.65 vs 2.10 ms, get 1.35 vs 2.32 ms at 512 MiB, and no temporary) and lose at
 # 16 KiB and below (8 KiB: 1.1 vs 0.8 ms).
 PAGED_MIN_PAGE_BYTES = 32 << 10
+# The same for packed (MXFP8) objects, whose alternative route (index_select + packed put, get + index_copy_) runs the
+# pack or unpack kernel as well.  bench/fp8_paged_bench.py, 256 blocks of a bf16 cache on one H100 80GB HBM3 at 700 W,
+# median ms: the paged calls win at 32 KiB pages (put 1.19 vs 1.81, get 1.30 vs 1.76, and no 512 MiB temporary) and at
+# 16 KiB (put 0.96 vs 1.02, get 0.99 vs 1.10), and lose from 8 KiB down (put 0.98 vs 0.80, get 0.92 vs 0.84).
+FP8_PAGED_MIN_PAGE_BYTES = 16 << 10
 
 
 def _stored_dtype(m) -> torch.dtype:
@@ -57,11 +62,14 @@ class TensorStore:
                                 enable_soft_pin=self.config.enable_soft_pin, checksum=_bb.ChecksumAlgo.CRC32C)
 
     # ------------------------------------------------------------------ put
+    @staticmethod
+    def _fusable_fp8_cfg(cfg) -> bool:
+        """Up to 3 copies (one tile pass of the fused pack fans out to every replica), each copy in one shard."""
+        return 1 <= cfg.replication_factor <= 3 and cfg.max_workers_per_copy == 1
+
     def _fused_fp8_ok(self, t: torch.Tensor, cfg) -> bool:
-        """Pack fused into the put kernel: bf16, fp16 or fp32, a whole number of 32-element MX blocks, up to 3 copies (one
-        tile pass fans out to every replica), each copy in one shard."""
-        return (t.dtype in _MX_WIDE and self.client.device_fp8_eligible(t.numel()) and 1 <= cfg.replication_factor <= 3
-                and cfg.max_workers_per_copy == 1 and t.data_ptr() % 16 == 0)
+        """Pack fused into the put kernel: bf16, fp16 or fp32, a whole number of 32-element MX blocks, a fusable config."""
+        return t.dtype in _MX_WIDE and self.client.device_fp8_eligible(t.numel()) and self._fusable_fp8_cfg(cfg) and t.data_ptr() % 16 == 0
 
     @staticmethod
     def _source_rows(t: torch.Tensor):
@@ -218,13 +226,14 @@ class TensorStore:
         return a
 
     @staticmethod
-    def _block_pages(cache: torch.Tensor, dim: int, ids: np.ndarray):
+    def _block_pages(cache: torch.Tensor, dim: int, ids: np.ndarray, min_page: Optional[int] = None):
         """(page addresses, page bytes) of cache.index_select(dim, ids) for the paged device calls, or None when they should
         not move it.  Page (o, k) is cache[o..., ids[k]] over the dims after `dim`, in index_select order (outer index
         major): those dims must form one contiguous block of a multiple of 16 bytes, the outer dims must collapse to one
         positive stride, the blocks must not overlap one another (no zero or negative strides: an expanded cache takes
-        the fallback), every page must be 16-byte aligned, and the page at least PAGED_MIN_PAGE_BYTES.  The addresses are a
-        numpy int64 array, built without a loop per page."""
+        the fallback), every page must be 16-byte aligned, and the page at least `min_page` bytes (by default
+        PAGED_MIN_PAGE_BYTES; FP8_PAGED_MIN_PAGE_BYTES for packed objects).  The addresses are a numpy int64 array, built without a loop per
+        page."""
         if not cache.is_cuda or cache.numel() == 0 or ids.size == 0:
             return None
         es, shape, stride = cache.element_size(), cache.shape, cache.stride()
@@ -233,7 +242,7 @@ class TensorStore:
             if s * es != page:
                 return None
             page *= n
-        if page % 16 or page < PAGED_MIN_PAGE_BYTES:
+        if page % 16 or page < (PAGED_MIN_PAGE_BYTES if min_page is None else min_page):
             return None
         outer = [(n, s) for n, s in zip(shape[:dim], stride[:dim]) if n != 1]
         if any(s != s2 * n2 for (_, s), (n2, s2) in zip(outer, outer[1:])):
@@ -261,31 +270,65 @@ class TensorStore:
         When the cache is a CUDA tensor whose dims after `dim` form one contiguous block of a multiple of 16 bytes and at
         least PAGED_MIN_PAGE_BYTES (32 KiB, where the paged calls start to beat index_select), whose outer dims collapse
         to one stride, whose blocks do not overlap and whose pages are 16-byte aligned, the blocks are read in place by
-        the paged put (batch_put_device_paged): no index_select temporary, no extra device pass.  Any other layout, and
-        pack_fp8, takes index_select and batch_put.  IndexError for a dim out of range.  A CUDA `ids` tensor is copied to the host once, which synchronises."""
+        the paged put (batch_put_device_paged): no index_select temporary, no extra device pass.  Any other layout takes
+        index_select and batch_put.
+
+        With pack_fp8 (bf16, fp16 and fp32 caches; TypeError for any other dtype, before anything is stored), a cache of
+        that layout with pages of at least FP8_PAGED_MIN_PAGE_BYTES, whose selected element count is a whole number of
+        32-element MX blocks, under a fusable config (up to 3 copies, one shard each), is packed in place by the paged
+        pack kernel (batch_put_device_fp8_paged): no wide temporary.  The stored object is that of
+        put(index_select(...), pack_fp8=True).  Items the fused kernel refuses (NOT_IMPLEMENTED: an unfusable placement)
+        and other layouts take index_select and batch_put.  IndexError for a dim out of range.  A CUDA `ids` tensor is
+        copied to the host once, which synchronises."""
         keys, caches, ids = list(keys), list(caches), list(ids)
         if not len(keys) == len(caches) == len(ids):
             raise ValueError("keys, caches and ids differ in length")
+        cfg = config or self.config
+        if pack_fp8:
+            bad = [(k, c.dtype) for k, c in zip(keys, caches) if c.dtype not in _MX_WIDE]
+            if bad:
+                raise TypeError(f"MXFP8 packing takes bfloat16, float16 and float32 tensors, not {bad[:3]}")
         dims = [self._block_dim(k, c, dim) for k, c in zip(keys, caches)]
         idx = [self._block_ids(k, b, c.shape[d]) for k, c, b, d in zip(keys, caches, ids, dims)]
-        pages = [None if pack_fp8 else self._block_pages(c, d, b) for c, d, b in zip(caches, dims, idx)]
+        shapes = []
+        for c, d, b in zip(caches, dims, idx):
+            shapes.append(list(c.shape))
+            shapes[-1][d] = b.size
+        min_page = FP8_PAGED_MIN_PAGE_BYTES if pack_fp8 else PAGED_MIN_PAGE_BYTES
+        pages = [self._block_pages(c, d, b, min_page) for c, d, b in zip(caches, dims, idx)]
+        if pack_fp8:  # the fused pack takes whole MX blocks under a fusable config
+            pages = [p if p is not None and self._fusable_fp8_cfg(cfg) and self.client.device_fp8_eligible(torch.Size(s).numel()) else None
+                     for p, s in zip(pages, shapes)]
         paged = [i for i, p in enumerate(pages) if p is not None]
-        if paged:
+        if paged and pack_fp8:
+            done = []
+            for dt, grp in _by_dtype(paged, lambda i: caches[i].dtype).items():
+                es = caches[grp[0]].element_size()
+                ecs = self.client.batch_put_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
+                                                             cfg, self._stream(), wide=_MX_WIDE[dt])
+                bad = [(keys[i], e) for i, e in zip(grp, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+                if bad:
+                    raise RuntimeError(f"paged fp8 put failed: {bad[:3]}")
+                done += [i for i, e in zip(grp, ecs) if e == _bb.ErrorCode.OK]
+            paged = done
+        elif paged:
             ecs = self.client.batch_put_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged], [pages[i][1] for i in paged],
-                                                     config or self.config, self._stream())
+                                                     cfg, self._stream())
             bad = [(keys[i], e) for i, e in zip(paged, ecs) if e != _bb.ErrorCode.OK]
             if bad:
                 raise RuntimeError(f"paged put failed: {bad[:3]}")
+        if paged:
             metas = []
             for i in paged:
-                shape = list(caches[i].shape)
-                shape[dims[i]] = idx[i].size
-                metas.append(json.dumps({"dtype": str(caches[i].dtype).replace("torch.", ""), "shape": shape, "packed": None,
-                                         "numel": torch.Size(shape).numel()}).encode())
+                n = torch.Size(shapes[i]).numel()
+                meta = {"dtype": str(caches[i].dtype).replace("torch.", ""), "shape": shapes[i], "packed": None, "numel": n}
+                if pack_fp8:
+                    meta.update(packed="mxfp8", padded_numel=n)
+                metas.append(json.dumps(meta).encode())
             ecs = self.client.batch_put([keys[i] + "#meta" for i in paged], metas, self._meta_cfg())
             if any(e != _bb.ErrorCode.OK for e in ecs):
                 raise RuntimeError("meta put failed")
-        rest = [i for i, p in enumerate(pages) if p is None]
+        rest = [i for i in range(len(keys)) if i not in set(paged)]
         if rest:
             self.batch_put([keys[i] for i in rest], [caches[i].index_select(dims[i], torch.from_numpy(idx[i]).to(caches[i].device)) for i in rest],
                            pack_fp8, config)
@@ -303,9 +346,11 @@ class TensorStore:
         dtype, ValueError unless the stored shape is the index_select shape, for a cache that is not a CUDA tensor on the
         current device and for duplicate ids, IndexError for an id or a dim out of range.  Caches of the layout
         batch_put_blocks reads in place take the paged get (batch_get_device_paged), which stores each tile straight into
-        its pages (RuntimeError unless the stored object fills every selected block);
-        other layouts, and packed tensors, take a get followed by index_copy_.  A CUDA `ids` tensor is copied to the host
-        once, which synchronises."""
+        its pages (RuntimeError unless the stored object fills every selected block); packed whole-block tensors with
+        pages of at least FP8_PAGED_MIN_PAGE_BYTES take the paged unpack (batch_get_device_fp8_paged), which unpacks each
+        tile straight into its pages.  Other layouts, padded packed tensors, and packed objects the fused kernel refuses
+        (NOT_IMPLEMENTED: an unfusable placement) take a get followed by index_copy_.  A CUDA `ids` tensor is copied to
+        the host once, which synchronises."""
         keys, caches, ids = list(keys), list(caches), list(ids)
         if not len(keys) == len(caches) == len(ids):
             raise ValueError("keys, caches and ids differ in length")
@@ -326,8 +371,22 @@ class TensorStore:
             if np.unique(t).size != t.size:
                 raise ValueError(f"{k}: duplicate block ids")
             idx.append(t)
-        pages = [None if m["packed"] else self._block_pages(c, d, b) for m, c, d, b in zip(metas, caches, dims, idx)]
-        paged = [i for i, p in enumerate(pages) if p is not None]
+        # packed whole-block objects take the paged unpack; padded ones cannot fill whole pages
+        fp8 = [m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"] and self.client.device_fp8_eligible(m["numel"]) for m in metas]
+        pages = [self._block_pages(c, d, b, FP8_PAGED_MIN_PAGE_BYTES if f else PAGED_MIN_PAGE_BYTES) if f or not m["packed"] else None
+                 for m, f, c, d, b in zip(metas, fp8, caches, dims, idx)]
+        unpacked = [i for i, p in enumerate(pages) if p is not None and not fp8[i]]
+        for dt, grp in _by_dtype([i for i, p in enumerate(pages) if p is not None and fp8[i]], lambda i: caches[i].dtype).items():
+            es = caches[grp[0]].element_size()
+            ecs = self.client.batch_get_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
+                                                         self._stream(), wide=_MX_WIDE[dt])
+            bad = [(keys[i], e) for i, e in zip(grp, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+            if bad:
+                raise RuntimeError(f"paged fp8 get failed: {bad[:3]}")
+            for i, e in zip(grp, ecs):
+                if e == _bb.ErrorCode.NOT_IMPLEMENTED:
+                    pages[i] = None  # get + index_copy_ below
+        paged = unpacked
         if paged:
             ecs, sizes = self.client.batch_get_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged],
                                                             [pages[i][1] for i in paged], self._stream())

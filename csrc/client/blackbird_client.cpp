@@ -702,13 +702,42 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::
       });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                                   const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
+                                                                   mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
+  std::vector<uint64_t> elems(n);
+  std::vector<SourcePages> pats(n);
+  return shaped_batch(
+      "device_put_fp8_paged", true, n, pages.size() == n && page_elems.size() == n,
+      [&](size_t i, uint64_t* wide_bytes) {
+        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &pats[i], &elems[i]);
+        if (ec != ErrorCode::OK) return ec;
+        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks
+        SourcePages bytes;
+        if (elems[i] > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *wide_bytes = b * elems[i];
+        // the engine's rule for a paged pack, checked once: there is no host-staged path for packed puts
+        if (!bytes.coaligned(b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), nullptr, cfg, stream, wide, &p);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows,
-                                                       const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
+                                                       const WorkerConfig& cfg, void* stream, mxfp8::Wide wide,
+                                                       const std::vector<SourcePages>* pages) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (rows && rows->size() != keys.size())) return out;
+  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (rows && rows->size() != keys.size()) ||
+      (pages && (rows || pages->size() != keys.size())))
+    return out;
   BB_TRACE_SPAN("batch_put_device_fp8", keys.size());
   WorkerConfig c = cfg;
   c.replication_factor = std::max<size_t>(1, std::min<size_t>(cfg.replication_factor, 3));  // one tile pass fans out to <= 3 copies
@@ -739,6 +768,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
     }
     DeviceFp8Op op{&copies[0].shards[0], const_cast<void*>(bf16_ptrs[i]), n_elems[i], {}};
     if (rows) op.rows = (*rows)[i];
+    if (pages) op.pages = (*pages)[i];
     op.wide_type = wide;
     for (size_t cidx = 1; cidx < copies.size(); ++cidx) op.replicas.push_back(&copies[cidx].shards[0]);
     ops.push_back(std::move(op));
@@ -831,15 +861,38 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
       [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream, wide); });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                                   const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
+  std::vector<uint64_t> elems(n);
+  std::vector<SourcePages> pats(n);
+  return shaped_batch(
+      "device_get_fp8_paged", false, n, pages.size() == n && page_elems.size() == n,
+      [&](size_t i, uint64_t* wide_bytes) {
+        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &pats[i], &elems[i]);
+        if (ec != ErrorCode::OK) return ec;
+        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
+        if (elems[i] > UINT64_MAX / b) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *wide_bytes = b * elems[i];
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto p = pick(pats, idx);
+        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, nullptr, stream, wide, &p);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                                       const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide) {
+                                                       const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide,
+                                                       const std::vector<SourcePages>* pages) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   const uint64_t b = mxfp8::wide_bytes(wide);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (rows && (ranges || rows->size() != keys.size())))
+      (rows && (ranges || rows->size() != keys.size())) || (pages && (ranges || rows || pages->size() != keys.size())))
     return out;
   BB_TRACE_SPAN("batch_get_device_fp8", keys.size());
   auto placed = keystone_->batch_get_workers(keys);
@@ -866,6 +919,14 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
+    if (pages && !copies.empty()) {  // the pages must hold exactly the stored object's elements
+      uint64_t stored = 0;
+      for (const auto& sh : copies[0].shards) stored += sh.length;
+      if (stored != packed) {
+        out[i] = ErrorCode::INVALID_ARGUMENT;
+        continue;
+      }
+    }
     // usable copies: single GPU-fabric shard holding the whole packed object with a BBH64 digest; a copy in this
     // client's own HBM first, the others in hashed order (readers spread over the replicas)
     std::vector<size_t> order;
@@ -895,6 +956,11 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
+    SourcePages dst_pages;  // and destination pages
+    if (pages && (!(*pages)[i].to_wide_bytes(b, &dst_pages) || !dst_pages.fused_get_aligned(0, b * n_elems[i]))) {
+      out[i] = ErrorCode::NOT_IMPLEMENTED;
+      continue;
+    }
     candidates[i] = std::move(order);
     idx.push_back(i);
   }
@@ -908,7 +974,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}, wide});
+      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}, wide,
+                     pages ? (*pages)[i] : SourcePages{}});
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -926,8 +993,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
     const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
+    const auto rpages = pages ? pick(*pages, r) : std::vector<SourcePages>();
     return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr, stream,
-                          wide);
+                          wide, pages ? &rpages : nullptr);
   });
   metrics_.inc("device_get_fp8_batches_total");
   return out;
@@ -1817,7 +1885,15 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
     if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
     const auto* src = static_cast<const uint8_t*>(op.wide);
     std::vector<uint8_t> dense;
-    if (op.rows.strided()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows
+    if (op.pages.paged()) {  // as the engine and the kernel's paged gathering load: the elements, from their pages
+      SourcePages b;
+      if (op.rows.strided() || !op.win.whole() || !op.pages.valid(op.n_elems) || !op.pages.to_wide_bytes(eb, &b))
+        return ErrorCode::INVALID_ARGUMENT;
+      if (!b.coaligned(eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      dense.resize(eb * op.n_elems);
+      b.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, reinterpret_cast<const void*>(at), n); });
+      src = dense.data();
+    } else if (op.rows.strided()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows
       SourceRows b;
       if (!op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
@@ -1849,6 +1925,12 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
       if (!op.win.whole() || !op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
     }
+    SourcePages pb;
+    if (op.pages.paged()) {  // as the engine: destination pages, never with rows or a window, co-aligned in wide bytes
+      if (op.rows.strided() || !op.win.whole() || !op.pages.valid(op.n_elems) || !op.pages.to_wide_bytes(eb, &pb))
+        return ErrorCode::INVALID_ARGUMENT;
+      if (!pb.coaligned(eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+    }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
@@ -1857,12 +1939,16 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
     }
     if (ec != ErrorCode::OK) return ec;
     auto* dst = static_cast<uint8_t*>(op.wide);
-    if (op.win.whole() && !op.rows.strided()) {
+    if (op.win.whole() && !op.rows.strided() && !op.pages.paged()) {
       mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, dst);
       continue;
     }
     std::vector<uint8_t> wide(eb * op.n_elems);
     mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, wide.data());
+    if (op.pages.paged()) {  // as the kernel's paged scattering store: the unpacked object into its pages
+      pb.for_each_run(wide.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(reinterpret_cast<void*>(at), wide.data() + x, n); });
+      continue;
+    }
     auto store = [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + eb * at, wide.data() + eb * x, eb * n); };
     if (op.rows.strided()) op.rows.for_each_run(op.n_elems, store);  // as the kernel's scattering store: into the rows
     else op.win.for_each_run(op.n_elems, store);  // as the kernel does: the whole object read and verified, only the window stored

@@ -92,6 +92,9 @@ struct DeviceFp8Op {
   SourceRows rows;
   // The element type of `wide`: bf16, fp16 or fp32 (common/mxfp8.h).  Ops of one call share its size (2 or 4 bytes).
   mxfp8::Wide wide_type = mxfp8::Wide::BF16;
+  // The wide side's pages, page and phase in elements (SourcePages in common/store_window.h): a put's source pages or a
+  // get's destination pages; `wide` is not used then.  Never together with rows or a window.
+  SourcePages pages;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -220,6 +223,28 @@ class BlackbirdClient {
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
                                                       const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
                                                       void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+  // Packed puts of paged tensors (the blocks of a paged KV cache, one object for a whole request): object i is the
+  // concatenation of the pages[i].size() pages of page_elems[i] elements at the device addresses pages[i], in list order
+  // (SourcePages in common/store_window.h, page size in elements, addresses in bytes).  The pack kernel reads each page in
+  // place; an MX block may straddle two pages.  The stored packed object and its digest are byte for byte those of
+  // batch_put_device_fp8 of the concatenation, so every fp8 get reads it.  Placement, replica fan-out and errors are
+  // batch_put_device_fp8's.  Per object, before anything is allocated: INVALID_ARGUMENT for page_elems[i] == 0 with pages,
+  // or an element count that is not a positive whole number of MX blocks; VALUE_OUT_OF_RANGE when the count or its wide
+  // bytes overflow; NOT_IMPLEMENTED unless the table is co-aligned in wide bytes (every page 16-byte aligned and, for
+  // several pages, page_elems[i] % 8 == 0) -- there is no host-staged path; the rest of the batch keeps its launch.
+  std::vector<ErrorCode> batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                    const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
+                                                    mxfp8::Wide wide = mxfp8::Wide::BF16);
+  // Gets of packed tensors into pages, the mirror: object i is unpacked into the pages pages[i] of page_elems[i] elements,
+  // element x in page x / page_elems[i] at element x % page_elems[i], by the paged scattering store of the fused unpack.
+  // Only the object's elements are written; pages of one get must not overlap (not checked).  Fail-over and the placement
+  // refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT for page_elems[i] == 0 with pages, or unless the
+  // stored object holds exactly pages[i].size() * page_elems[i] elements (a positive whole number of MX blocks);
+  // VALUE_OUT_OF_RANGE when that count or its wide bytes overflow; NOT_IMPLEMENTED when the object is not fusable (as
+  // batch_get_device_fp8) or the pages fail SourcePages::fused_get_aligned in wide bytes -- there is no host-staged path;
+  // the rest of the batch keeps the fused launch.
+  std::vector<ErrorCode> batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
+                                                    const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -346,18 +371,22 @@ class BlackbirdClient {
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
                                     const std::vector<ByteRange>* ranges, const std::vector<SourceRows>* rows, void* stream,
                                     std::vector<size_t>* out_sizes, const std::vector<SourcePages>* pages = nullptr);
-  // batch_put_device_fp8 and batch_put_device_fp8_strided: `rows` null = contiguous tensors, else object i is read by
-  // (*rows)[i], in elements.
+  // batch_put_device_fp8, batch_put_device_fp8_strided and batch_put_device_fp8_paged: `rows` null = contiguous tensors,
+  // else object i is read by (*rows)[i], in elements; `pages` (never with `rows`) non-null = object i is read from the
+  // pages (*pages)[i], in elements (bf16_ptrs are then not read).
   std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows, const WorkerConfig& cfg,
-                                        void* stream, mxfp8::Wide wide);
-  // batch_get_device_fp8, batch_get_device_fp8_range, batch_get_device_fp8_strided and batch_get_device_fp8_scatter:
-  // `ranges` null = whole tensors, else object i's rows (offset, length and pitch in elements) into bf16_ptrs[i]; `rows`
-  // (whole tensors only) null = contiguous destinations, else object i lands in (*rows)[i], in elements.
+                                        void* stream, mxfp8::Wide wide, const std::vector<SourcePages>* pages = nullptr);
+  // batch_get_device_fp8, batch_get_device_fp8_range, batch_get_device_fp8_strided, batch_get_device_fp8_scatter and
+  // batch_get_device_fp8_paged: `ranges` null = whole tensors, else object i's rows (offset, length and pitch in elements)
+  // into bf16_ptrs[i]; `rows` (whole tensors only) null = contiguous destinations, else object i lands in (*rows)[i], in
+  // elements; `pages` (whole tensors only, never with `rows`) non-null = object i, which must hold exactly n_elems[i]
+  // elements, lands in the pages (*pages)[i], in elements.
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                        const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide);
-  // The eight shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
+                                        const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide,
+                                        const std::vector<SourcePages>* pages = nullptr);
+  // The shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
   template <class Shape, class Run>
   std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);
   template <class Reissue>

@@ -253,14 +253,24 @@ struct SourceRows {
 // into.  Object byte x lives at
 //   addrs[(x + phase) / page] + (x + phase) % page
 // `addrs` is a host array of npages page addresses owned by the caller.  SourceRows is the special case
-// addrs[k] = src + k * pitch (with page = width).  This is the one statement of the rule; the transfer engine (XferItem),
-// the fabric's ops (DeviceShardOp), the client, the host loopback transport and the kernel's XFER_PAGED descriptors
-// (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.
+// addrs[k] = src + k * pitch (with page = width).  This is the one statement of the rule; the transfer engine (XferItem,
+// Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and the kernels'
+// XFER_PAGED descriptors (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.  The unit of `page` and
+// `phase` is a byte, or for an MXFP8 transfer an element of the wide side (to_wide_bytes() turns elements into bytes);
+// the addresses are byte addresses either way.
 struct SourcePages {
   const uint64_t* addrs = nullptr;
   uint64_t npages = 0, page = 0, phase = 0;
 
   bool paged() const { return page != 0; }
+  // The table of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4): page and
+  // phase times b, the same addresses.  False when either product overflows.
+  bool to_wide_bytes(uint64_t b, SourcePages* out) const {
+    uint64_t pb = 0, fb = 0;
+    if (__builtin_mul_overflow(page, b, &pb) || __builtin_mul_overflow(phase, b, &fb)) return false;
+    *out = {addrs, npages, pb, fb};
+    return true;
+  }
   // Pages that object bytes [0, len) touch.
   uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
   // Whether the table holds every page of an object of `len` bytes, with phase < page.

@@ -684,8 +684,8 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.n_elems = op.n_elems;
     it.wide_type = op.wide_type;
     it.win = op.win;  // a window on a put is refused by the engine
-    if (unpack) it.dst_rows = op.rows;  // the rows are the destination's on a get, the source's on a put
-    else it.rows = op.rows;
+    if (unpack) it.dst_rows = op.rows, it.dst_pages = op.pages;  // rows and pages are the destination's on a get,
+    else it.rows = op.rows, it.pages = op.pages;                 // the source's on a put
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;

@@ -633,14 +633,18 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   SlotRelease release{s->ticket};
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
+  // as submit() does: nothing of the slot's last batch (a paged bb_xfer batch's page entries included) carries over
   s->strides.clear();
+  s->pages.clear();
+  s->paged_descs.clear();
   // one kernel instantiation per launch: bf16 and fp16 items share the 2-byte one, fp32 items take the 4-byte one
   const uint32_t eb = mxfp8::wide_bytes(items[0].wide_type);
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
-    const bool gather = it.rows.strided();
-    const bool scatter = it.dst_rows.strided();
+    const bool src_paged = it.pages.paged(), dst_paged = it.dst_pages.paged();
+    const bool gather = it.rows.strided() || src_paged;
+    const bool scatter = it.dst_rows.strided() || dst_paged;
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
     if (it.wide_type != mxfp8::Wide::BF16 && it.wide_type != mxfp8::Wide::F16 && it.wide_type != mxfp8::Wide::F32)
       return ErrorCode::INVALID_ARGUMENT;
@@ -649,10 +653,18 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     if (gather && (unpack || !it.rows.valid() || !it.rows.to_wide_bytes(eb, &rows))) return ErrorCode::INVALID_ARGUMENT;
     if (scatter && (!unpack || gather || !it.win.whole() || !it.dst_rows.valid() || !it.dst_rows.to_wide_bytes(eb, &rows)))
       return ErrorCode::INVALID_ARGUMENT;
+    // pages replace the rows on their side: the source of a pack or the destination of an unpack, never with a window
+    const bool paged = src_paged || dst_paged;
+    const SourcePages& pg = src_paged ? it.pages : it.dst_pages;
+    SourcePages pages;  // the table in wide bytes
+    if (paged && ((src_paged && it.rows.strided()) || (dst_paged && it.dst_rows.strided()) || !it.win.whole() ||
+                  !pg.valid(it.n_elems) || !pg.to_wide_bytes(eb, &pages)))
+      return ErrorCode::INVALID_ARGUMENT;
     // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
-    // first element after row 0's start): the rows are checked instead
+    // first element after row 0's start): the rows are checked instead, and a paged item's pages
     if (((strided || gather || scatter ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
-        ((gather || scatter) && !rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
+        ((gather || scatter) &&
+         !(paged ? pages.coaligned(eb * it.n_elems) : rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems))))
       return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
@@ -684,9 +696,14 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       d.flags |= XFER_STRIDED;
       s->set_stride(i, w);
     }
-    if (gather || scatter) {  // d.src (gather) or d.dst[0] (scatter) is the pattern's row 0
+    if (gather || scatter) {  // d.src (gather) or d.dst[0] (scatter) is the pattern's row 0, or not read when paged
       d.flags |= gather ? XFER_GATHER : XFER_SCATTER;
-      s->set_stride(i, rows);
+      if (paged) {
+        d.flags |= XFER_PAGED;
+        s->add_pages(i, pages, eb * it.n_elems);
+      } else {
+        s->set_stride(i, rows);
+      }
     }
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
@@ -700,7 +717,9 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   }
   BB_TRY(write_tile_table(s, n));
   const bool any_strided = !s->strides.empty();
-  const size_t tab = s->write_strides(n);
+  size_t tab = 0;
+  if (s->pages.empty()) tab = s->write_strides(n);
+  else BB_TRY(write_pages(s, n, &tab));  // may move the table: the launch's pointers are taken below
   BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
   BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;

@@ -86,6 +86,17 @@ struct Fp8Item {
   // pack, with a window, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned in
   // bf16 bytes, which replaces the 16-byte alignment check of `wide`.
   SourceRows dst_rows;
+  // Paged source (pack only, `pages`) or paged destination (unpack only, `dst_pages`), page and phase in elements, the
+  // addresses in bytes (SourcePages in common/store_window.h): element x at addrs[(x + phase) / page] + b * ((x + phase)
+  // % page) for b-byte elements; `wide` is not read.  run_fp8 sets XFER_GATHER | XFER_PAGED or XFER_SCATTER | XFER_PAGED
+  // exactly when one is set, and copies the page entries into the batch's device table, so the host array need only live
+  // until run_fp8 returns.  An MX block may straddle two pages.  INVALID_ARGUMENT for source pages on an unpack,
+  // destination pages on a pack, pages together with rows or a window, a table too short for n_elems, phase >= page, or a
+  // page whose wide-byte size overflows; INVALID_ADDRESS unless the table is co-aligned in wide bytes
+  // (SourcePages::coaligned of b * n_elems: addrs[k] + b * phase 16-byte aligned, and b * page % 16 == 0 for more than
+  // one page), which replaces the 16-byte alignment check of `wide`.
+  SourcePages pages;
+  SourcePages dst_pages;
 };
 
 struct XferResult {

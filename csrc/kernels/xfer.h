@@ -49,12 +49,13 @@ enum XferFlags : uint32_t {
   // the kernel.  A batch of bf16 and fp16 items is one launch; fp32 items take the 4-byte instantiation, a launch of their
   // own.
   XFER_WIDE_F16 = 1u << 7,
-  // Paged source or destination, in bb_xfer only, together with XFER_GATHER (a put reads its pages) or XFER_SCATTER (a get
-  // stores into them): the rule of SourcePages (common/store_window.h), object byte x at
+  // Paged source or destination, in bb_xfer and the fused MXFP8 put and get, together with XFER_GATHER (a put reads its
+  // pages) or XFER_SCATTER (a get stores into them): the rule of SourcePages (common/store_window.h), object byte x at
   // pages[(x + phase) / page] + (x + phase) % page.  The descriptor's XferStride entry is {device address of its first
-  // page entry, page, phase}; `src` (put) or dst[0] (get) is not read.  The destination forms are those of XFER_GATHER
-  // or XFER_SCATTER; never with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM.  The tile in shared memory is the dense
-  // object's tile, so the digest, the verify and the stored bytes are those of a contiguous put or get.
+  // page entry, page, phase}; `src` (put) or dst[0] (get) is not read.  The MXFP8 kernels count page and phase in bytes
+  // of the wide side.  The destination forms are those of XFER_GATHER or XFER_SCATTER; never with XFER_WINDOW,
+  // XFER_STRIDED or XFER_RAW_SUM.  The tile in shared memory is the dense object's tile, so the digest, the verify and
+  // the stored bytes are those of a contiguous put or get.
   XFER_PAGED = 1u << 8,
 };
 

@@ -8,7 +8,10 @@
 //                   is read from HBM once and only the 0.52x packed bytes cross NVLink (once per replica).
 //                   With XFER_GATHER (puts of a sliced tensor) the producer fills the bf16 tile from the source rows,
 //                   one row segment per lane, by the rule of SourceRows (common/store_window.h) in bf16 bytes, so the
-//                   tile, the packed object and its digest are those of a put of the compacted rows.
+//                   tile, the packed object and its digest are those of a put of the compacted rows.  With
+//                   XFER_GATHER | XFER_PAGED (puts of the blocks of a paged cache) the row segments are the pages of
+//                   SourcePages in wide bytes, each read from the address in the page table, so the tile is that
+//                   of the concatenated pages; an MX block may straddle two pages, the codec never sees it.
 //   get  (UNPACK) : TMA loads payload tile + scales from the slab -> tensor-core hash of the payload tile ->
 //                   8 unpack warps expand to bf16 in shared memory -> TMA stores the 32 KiB tile to the caller.
 //                   With XFER_WINDOW (element-range gets) only the bf16 bytes [win.lo, win.hi) of the object are
@@ -17,7 +20,9 @@
 //                   (slices along an inner dimension) the store warp stores only the window's row segments, densely,
 //                   one per lane, by the same rule as bb_xfer; a tile wholly inside a gap between rows is still unpacked.
 //                   With XFER_SCATTER instead (gets into a sliced tensor) the store warp stores every 32 KiB bf16 tile
-//                   as the row segments of the destination rows, by the SourceRows rule in bf16 bytes, as bb_xfer does.
+//                   as the row segments of the destination rows, by the SourceRows rule in bf16 bytes, as bb_xfer does;
+//                   with XFER_SCATTER | XFER_PAGED (gets into the blocks of a paged cache) as the segments of the
+//                   destination pages, by the SourcePages rule in wide bytes.
 //
 // The stored object keeps the layout of the unfused path ([E4M3 payload n][E8M0 scales n/32], common/mxfp8.h), and so
 // does its digest: BBH64 is a sum of per-tile terms, this kernel accumulates the payload tiles (tile index 0..T-1)
@@ -72,7 +77,7 @@ struct FpMeta {            // 64 bytes
   uint32_t valid;          // payload bytes (= elements) of this tile: 16384, or the multiple-of-32 tail of the object
   uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
                            // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
-                           // FpParams::strides either way)
+                           // FpParams::strides either way); XFER_PAGED as well when those rows are pages
   uint32_t f16;            // XFER_WIDE_F16: the wide side is fp16 (2-byte instantiation only)
   uint32_t pad;
 };
@@ -167,7 +172,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER : XFER_GATHER);
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED : XFER_GATHER | XFER_PAGED);
         e.m.f16 = d.flags & XFER_WIDE_F16;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
@@ -226,9 +231,12 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
               g_desc = e.m.desc;
               gst = load_stride(p.strides, g_desc);
             }
-            tx = __reduce_add_sync(0xffffffffu, gather_row_segments(s.wide[ws], &s.w_full[ws], e.src,
-                                                                     static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes,
-                                                                     WB * e.m.valid, gst, lane));
+            // XFER_PAGED: the rows are the pages of the table in gst, e.src is not read
+            const uint64_t off = static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes;
+            const uint32_t seg_tx = e.m.strided & XFER_PAGED
+                                        ? gather_row_segments<true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane)
+                                        : gather_row_segments(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane);
+            tx = __reduce_add_sync(0xffffffffu, seg_tx);
           }
           __syncwarp();
           if (lane == 0) {
@@ -263,8 +271,10 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             pat_desc = m.desc;
             pat = load_stride(p.strides, pat_desc);
           }
-          // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile
-          if (m.strided & XFER_SCATTER) scatter_row_segments(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
+          // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile.  A paged one stores
+          // into the pages of the table in `pat` and does not read dst[0].
+          if (m.strided & XFER_PAGED) scatter_row_segments<true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
+          else if (m.strided & XFER_SCATTER) scatter_row_segments(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
           else store_row_segments(s.wide[st], m.dst[0] - off, off, x0, x1, pat, lane);
         } else {
           if (lane == 0 && a1 > a0) bulk_s2g(reinterpret_cast<void*>(m.dst[0] + a0), &s.wide[st][a0], a1 - a0);

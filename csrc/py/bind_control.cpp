@@ -429,6 +429,13 @@ void bind_control(py::module_& m) {
                   py::arg("addrs"), py::arg("page"), "(ErrorCode, SourcePages, object bytes)")
       .def("rebase", [](const PyPages& t, uint64_t off) { return PyPages{t.addrs, t.p.rebase(off)}; }, py::arg("off"),
            "the table seen from object byte off")
+      .def("to_wide_bytes",
+           [](const PyPages& t, uint64_t b) {
+             PyPages w{t.addrs, {}};
+             const bool ok = t.p.to_wide_bytes(b, &w.p);
+             return py::make_tuple(ok, w);
+           },
+           py::arg("b"), "(ok, table): a table in elements of b bytes as the same table in bytes; ok is False on overflow")
       .def("coaligned", [](const PyPages& t, uint64_t len) { return t.p.coaligned(len); }, py::arg("len"))
       .def("fused_get_aligned", [](const PyPages& t, uint64_t off, uint64_t len) { return t.p.fused_get_aligned(off, len); },
            py::arg("off"), py::arg("len"))
@@ -1387,6 +1394,26 @@ void bind_control(py::module_& m) {
          "Object i into the pages pages[i] of page_bytes[i] bytes, byte x in page x // page_bytes[i] (capacity len(pages[i]) "
          "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; pages of one get "
          "must not overlap (not checked); returns (one ErrorCode per object, object sizes).")
+      .def("batch_put_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
+                                            const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, uintptr_t stream,
+                                            mxfp8::Wide wide) {
+        const auto lists = to_page_lists(pages);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_fp8_paged(keys, lists, page_elems, cfg, reinterpret_cast<void*>(stream), wide); }));
+      }, py::arg("keys"), py::arg("pages"), py::arg("page_elems"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
+         py::arg("wide") = mxfp8::Wide::BF16,
+         "Packed tensor i = the len(pages[i]) pages of page_elems[i] elements of type `wide` at the device addresses pages[i] "
+         "(each a 1-D integer array-like), concatenated in order; packed in the put kernel and stored as "
+         "batch_put_device_fp8 of the concatenation would store it; returns one ErrorCode per object (NOT_IMPLEMENTED: "
+         "gather the pages and put that).")
+      .def("batch_get_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
+                                            const std::vector<uint64_t>& page_elems, uintptr_t stream, mxfp8::Wide wide) {
+        const auto lists = to_page_lists(pages);
+        return ecs_to_py(nogil([&] { return c.batch_get_device_fp8_paged(keys, lists, page_elems, reinterpret_cast<void*>(stream), wide); }));
+      }, py::arg("keys"), py::arg("pages"), py::arg("page_elems"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         "Packed tensor i, which must hold len(pages[i]) * page_elems[i] elements, unpacked to type `wide` into the pages "
+         "pages[i] of page_elems[i] elements, element x in page x // page_elems[i]; the whole packed object is read and "
+         "verified, only its elements are written; returns one ErrorCode per object (NOT_IMPLEMENTED: get it whole and "
+         "copy).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

@@ -154,6 +154,7 @@ void bind_gpu(py::module_& m) {
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream, mxfp8::Wide wide) {
              std::vector<gpu::Fp8Item> v;
+             std::deque<std::vector<uint64_t>> keep;
              for (auto h : items) {
                auto t = h.cast<py::tuple>();
                gpu::Fp8Item it;
@@ -166,15 +167,17 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 8)
+               if (t.size() < 3 || t.size() > 10)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
-                     "scatter (pitch, width, phase)[, wide]]]]])");
+                     "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 5 && !t[5].is_none()) it.rows = to_rows(t[5]);
                if (t.size() > 6 && !t[6].is_none()) it.dst_rows = to_rows(t[6]);
                if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
+               if (t.size() > 8 && !t[8].is_none()) it.pages = to_pages(t[8], keep);
+               if (t.size() > 9 && !t[9].is_none()) it.dst_pages = to_pages(t[9], keep);
                v.push_back(it);
              }
              XferResult res;
@@ -203,7 +206,12 @@ void bind_gpu(py::module_& m) {
            "bf16_ptr + 2 * phase is 16-byte aligned and, when the object spans more than one row, (pitch - width) % 8 == 0.  "
            "A get's scatter pattern (pitch, width, phase), in elements, as the seventh element stores into rows by the same "
            "rule, element x at bf16_ptr + 2 * ((x + phase) // width * pitch + (x + phase) % width), under the same rules; "
-           "INVALID_ARGUMENT on a put or with a window.  Returns (digests of the packed objects, status, device_ms).")
+           "INVALID_ARGUMENT on a put or with a window.  A put's source pages (addrs, page, phase), page and phase in "
+           "elements, as the ninth element read element x from addrs[(x + phase) // page] + 2 * ((x + phase) % page) "
+           "(bf16_ptr is not read); a get's destination pages as the tenth store by the same rule.  INVALID_ARGUMENT for "
+           "pages on the wrong side, with rows or a window, phase >= page or a table too short; INVALID_ADDRESS unless "
+           "every page touched is co-aligned in wide bytes and, for several pages, page % 8 == 0.  Returns (digests of the "
+           "packed objects, status, device_ms).")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
