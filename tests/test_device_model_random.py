@@ -3,21 +3,32 @@ host model of the store.
 
 The cluster has an HBM slab, a pinned shared-memory DRAM pool (which the fused kernels reach over PCIe) and an NVMe pool
 (which device gets reach only through the host-staged path); ttl 0 and watermark 1.0, so nothing moves on its own.  Each
-step draws a byte put (plain or strided source, 1-3 replicas, 1-2 workers per copy, any algorithm), an fp8 put (plain or
-strided source), a byte get (whole, range or strided), an fp8 get (whole, range or strided), a tier move, a compaction
-of the HBM pool, a corruption of one copy or of every copy of an object followed by gets of it, or a remove.  Batches
-mix keys of different steps, tiers and algorithms; caller pointers are sometimes misaligned and some strided gaps are no
-multiple of 16 bytes (8 elements).
+step draws a byte put (plain, strided or paged source, 1-3 replicas, 1-2 workers per copy so that shard edges fall
+mid-page, any algorithm), an fp8 put (plain, strided or paged source, of bf16, fp16 or fp32 drawn per call), a byte get
+(whole, range, strided, into pages or into rows), an fp8 get (whole, range, strided, into pages or into rows, in a type
+drawn per call, so that objects packed from one type are read as another), a tier move, a compaction of the HBM pool, a
+corruption of one copy or of every copy of an object followed by gets of it through any of those calls, or a remove.
+Batches mix keys of different steps, tiers and algorithms; caller pointers and pages are sometimes misaligned, some
+strided gaps and pages are no multiple of 16 bytes, some page tables repeat a page, and some destinations are too small
+or larger than the object.
 
-The model predicts every item's error code from the documented rules, written out here: byte gets are staged, never
-refused; an fp8 get is NOT_IMPLEMENTED when its virtual base is misaligned, when a multi-row slice has a gap that is no
-multiple of 8 elements, or when the object sits on NVMe; CHECKSUM_MISMATCH only when every copy read is corrupt;
-OBJECT_NOT_FOUND after a remove.  After every step it checks the result bytes and the guard bytes around them, every
-copy's stored bytes and recorded digest (Store in test_device_path.py) and the client counters the step moves.
+The model predicts every item's error code from the documented rules of blackbird_client.h, written out here: byte gets
+are staged, never refused, and a paged or scattered one is BUFFER_OVERFLOW when the object is larger than its pages or
+rows (a shorter object fills them in order) and INVALID_ARGUMENT for page size 0; whether a byte item is fused or staged
+follows SourcePages::coaligned / fused_get_aligned and SourceRows::fused_get_aligned on every shard of every copy, and
+reachability; an fp8 get is NOT_IMPLEMENTED when its virtual base, row 0 or a page is misaligned, when a multi-row slice
+or scatter has a gap that is no multiple of 16 bytes, or when the object is not one shard in HBM or DRAM, and
+INVALID_ARGUMENT when the element count is not that of the rows or pages; CHECKSUM_MISMATCH only when every copy read is
+corrupt; OBJECT_NOT_FOUND after a remove.  After every step it checks the result bytes and the guard bytes around and
+between them, every copy's stored bytes and recorded digest (Store in test_device_path.py) and the client counters the
+step moves (staged items, placement refreshes).
 
-Models trusted: numpy slicing; bb.crc32c / bb.bbh64 / bb.xxh3t64 (checked in test_common.py against golden values,
-_bbh64_numpy and python-xxhash); the exact MXFP8 model of test_mxfp8_exhaustive.py (checked there against torch)."""
+Models trusted: numpy slicing, with the SourcePages and SourceRows rules of test_xfer_random.py; bb.crc32c / bb.bbh64 /
+bb.xxh3t64 (checked in test_common.py against golden values, _bbh64_numpy and python-xxhash); the exact MXFP8 models of
+test_mxfp8_exhaustive.py (model_pack, model_unpack) and test_mxfp8_wide.py (model_pack_w, model_unpack_w), checked
+there against torch."""
 import collections
+import math
 import os
 
 import numpy as np
@@ -26,6 +37,7 @@ import torch
 
 from test_device_path import Store, _counter, _ref
 from test_mxfp8_exhaustive import model_pack, model_unpack, same_bits
+from test_xfer_random import WB, WGUARD, WIDES, _pack_model, _same, _unpack_model, pages_at, rows_at
 
 pytestmark = pytest.mark.gpu
 
@@ -36,7 +48,8 @@ T = 16384
 ALGOS = ["NONE", "CRC32C", "BBH64", "XXH3"]
 SEEDS = [3, 17]
 STEPS = 150 + int(os.environ.get("BB_RANDOM_ROUNDS", "0")) * 10
-OPS = ["put", "put_fp8", "get", "get_fp8", "migrate", "compact", "corrupt", "remove"]
+OPS = ["put", "put_fp8", "get", "get_fp8", "migrate", "compact", "corrupt", "remove", "put_paged", "get_paged", "get_scatter",
+       "put_fp8_paged", "get_fp8_paged", "get_fp8_scatter"]
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -71,13 +84,62 @@ def _bf16(rng, n):
     return ((e << 7) | rng.integers(0, 128, (n // 32, 32)) | (rng.integers(0, 2, (n // 32, 32)) << 15)).reshape(-1).astype(np.uint16)
 
 
-class Obj:
-    """The model of one object: its bytes (a packed object's packed bytes), algorithm, copies and tier."""
+def _wide(rng, n, w):
+    """n patterns of type w across many binades, block by block (no NaN or Inf); fp16 reaches its subnormals."""
+    if w == "bf16":
+        return _bf16(rng, n)
+    field, lo, hi, mant = (10, 2, 31, 10) if w == "f16" else (23, 60, 200, 23)
+    top = rng.integers(lo, hi, n // 32)[:, None]
+    e = np.clip(top - rng.integers(0, 10, (n // 32, 32)), 0, hi - 1)
+    bits = (e << field) | rng.integers(0, 1 << mant, (n // 32, 32)) | (rng.integers(0, 2, (n // 32, 32)) << (field + (5 if w == "f16" else 8)))
+    return bits.reshape(-1).astype(np.uint16 if w == "f16" else np.uint32)
 
-    def __init__(self, data, algo, copies, tier, x=None):
-        self.data, self.algo, self.copies, self.tier, self.x = data, algo, copies, tier, x
+
+def _mx(bb, w):
+    return {"bf16": bb.MxWide.BF16, "f16": bb.MxWide.F16, "f32": bb.MxWide.F32}[w]
+
+
+def _starts(shs):
+    return np.cumsum([0] + [sh.length for sh in shs])[:-1].tolist()
+
+
+def pages_coaligned(addrs, page, off, length):
+    """SourcePages{addrs, page}.rebase(off).coaligned(length), written out: every page that object bytes [off, off +
+    length) touch has addr + (off % page) 16-byte aligned, and the page is a multiple of 16 when they touch several."""
+    ph, k0 = off % page, off // page
+    n = (length - 1 + ph) // page + 1 if length else 0
+    if n > 1 and page % 16:
+        return False
+    return all((addrs[k0 + j] + ph) % 16 == 0 for j in range(n))
+
+
+def pages_fused(addrs, page, off, length):
+    """SourcePages::fused_get_aligned: as pages_coaligned, and no table of several pages with page % 16 != 0."""
+    return not (len(addrs) > 1 and page % 16) and pages_coaligned(addrs, page, off, length)
+
+
+def rows_fused(dst, width, pitch, rows, off):
+    """SourceRows::fused_get_aligned for the rows of a scattered get, from object byte off: a gap that is a multiple of 16
+    and the rows co-aligned from where the shard starts."""
+    if rows > 1 and width < pitch:
+        return (pitch - width) % 16 == 0 and (dst + off // width * pitch + off % width) % 16 == 0
+    return (dst + off) % 16 == 0
+
+
+class Obj:
+    """The model of one object: its bytes (a packed object's packed bytes), algorithm, copies and tier; a packed object's
+    source patterns x and their type w."""
+
+    def __init__(self, data, algo, copies, tier, x=None, w="bf16"):
+        self.data, self.algo, self.copies, self.tier, self.x, self.w = data, algo, copies, tier, x, w
         self.flips = set()  # (copy, shard) corrupt right now
-        self.back = None if x is None else model_unpack(data, x.size)  # what an fp8 get returns
+        self._back = {}
+
+    def back(self, w):
+        """What an fp8 get of type w returns: the unpack of the packed bytes in that type."""
+        if w not in self._back:
+            self._back[w] = _unpack_model(self.data, self.x.size, w)
+        return self._back[w]
 
     @property
     def fp8(self):
@@ -187,9 +249,9 @@ class Model:
         bb, rng = self.bb, self.rng
         count = int(rng.integers(1, 5))
         # one copy, on the tier asked for: further replicas may be placed on NVMe, which an fp8 put cannot write
-        reps, tier = 1, str(rng.choice(["RAM_GPU", "RAM_CPU"]))
+        reps, tier, w = 1, str(rng.choice(["RAM_GPU", "RAM_CPU"])), str(rng.choice(WIDES))
         strided = rng.random() < 0.5
-        self.what = f"fp8 put{' strided' if strided else ''} of {count}, {tier}"
+        self.what = f"fp8 put{' strided' if strided else ''} of {count}, {w}, {tier}"
         keys = [self.new_key() for _ in range(count)]
         shapes, xs, srcs = [], [], []
         for _ in keys:
@@ -200,24 +262,24 @@ class Model:
                 rows = max(1, n // width)
             else:
                 width, pitch, rows = n, n, 1
-            x = _bf16(rng, width * rows)
-            buf = np.full((rows - 1) * pitch + width + 8, 0x7FC0, dtype=np.uint16)  # NaN in the gaps
+            x = _wide(rng, width * rows, w)
+            buf = np.full((rows - 1) * pitch + width + 8, {"bf16": 0x7FC0, "f16": 0x7E00, "f32": 0x7FC00000}[w], dtype=x.dtype)  # NaN in the gaps
             for i in range(rows):
                 buf[i * pitch:i * pitch + width] = x[i * width:(i + 1) * width]
-            srcs.append(torch.from_numpy(buf.view(np.int16)).cuda())
+            srcs.append(torch.from_numpy(buf.view(np.uint8)).cuda())
             shapes.append((width, pitch, rows))
             xs.append(x)
         cfg = _cfg(bb, "BBH64", reps, tier)
         ptrs = [s.data_ptr() for s in srcs]
         if strided:
             ecs = self.cl.client.batch_put_device_fp8_strided(keys, ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
-                                                              [s[2] for s in shapes], cfg, _stream())
+                                                              [s[2] for s in shapes], cfg, _stream(), wide=_mx(bb, w))
         else:
-            ecs = self.cl.client.batch_put_device_fp8(keys, ptrs, [x.size for x in xs], cfg, _stream())
+            ecs = self.cl.client.batch_put_device_fp8(keys, ptrs, [x.size for x in xs], cfg, _stream(), wide=_mx(bb, w))
         assert ecs == [bb.ErrorCode.OK] * count, f"{self.where()}: {ecs}"
         torch.cuda.synchronize()
         for k, x in zip(keys, xs):
-            self.objs[k] = Obj(model_pack(x), "BBH64", reps, tier, x)
+            self.objs[k] = Obj(_pack_model(x, w), "BBH64", reps, tier, x, w)
 
     def _byte_shape(self, o):
         """(kind, offset, width, pitch, rows) of a byte get of object o: whole, range or strided."""
@@ -359,18 +421,20 @@ class Model:
         keys = keys or self.pick(True, int(rng.integers(1, 7)), gone=0.3)
         if not keys:
             return
+        gw = str(rng.choice(WIDES))  # the type of the call: objects packed from any type are read into it
+        gb, per = WB[gw], 16 // WB[gw]
         items, o_ = [], 64
         for k in keys:
             o = self.objs.get(k)
             shape = ("range", 0, 64, 0, 1) if o is None else self._fp8_shape(o)
             # misaligned ranges and slices fail alone (NOT_IMPLEMENTED); a whole tensor's pointer is the engine's to check
-            skew = int(rng.choice([1, 4])) if rng.random() < 0.2 and shape[0] != "whole" else 0
-            region = (o_ + 7) // 8 * 8 + (shape[1] + skew) % 8  # element offset: virtual base aligned unless skewed
+            skew = int(rng.choice([1, per // 2])) if rng.random() < 0.2 and shape[0] != "whole" else 0
+            region = (o_ + per - 1) // per * per + (shape[1] + skew) % per  # element offset: virtual base aligned unless skewed
             items.append((k, o, shape, region, skew))
             o_ = region + shape[2] * shape[4] + 32
-        out = torch.full((o_ + 64,), GUARD16, dtype=torch.int16, device="cuda")
+        out = torch.full((o_ + 64,), WGUARD[gb], dtype=torch.int16 if gb == 2 else torch.int32, device="cuda")
         p = out.data_ptr()
-        self.what = f"fp8 get of {len(keys)}"
+        self.what = f"fp8 get of {len(keys)} as {gw}"
         ecs = {}
         ref0, fo0 = self.counter("get_placement_refresh_total"), self.counter("replica_failover_total")
         for kind in ("whole", "range", "strided"):
@@ -378,19 +442,20 @@ class Model:
             if not idx:
                 continue
             ks = [items[i][0] for i in idx]
-            ptrs = [p + 2 * items[i][3] for i in idx]
+            ptrs = [p + gb * items[i][3] for i in idx]
             ns = [items[i][1].x.size if items[i][1] is not None else 64 for i in idx]
             if kind == "whole":
-                got = self.cl.client.batch_get_device_fp8(ks, ptrs, ns, _stream())
+                got = self.cl.client.batch_get_device_fp8(ks, ptrs, ns, _stream(), wide=_mx(bb, gw))
             elif kind == "range":
-                got = self.cl.client.batch_get_device_fp8_range(ks, ptrs, ns, [items[i][2][1] for i in idx], [items[i][2][2] for i in idx], _stream())
+                got = self.cl.client.batch_get_device_fp8_range(ks, ptrs, ns, [items[i][2][1] for i in idx], [items[i][2][2] for i in idx], _stream(),
+                                                               wide=_mx(bb, gw))
             else:
                 got = self.cl.client.batch_get_device_fp8_strided(ks, ptrs, ns, [items[i][2][1] for i in idx], [items[i][2][2] for i in idx],
-                                                                  [items[i][2][3] for i in idx], [items[i][2][4] for i in idx], _stream())
+                                                                  [items[i][2][3] for i in idx], [items[i][2][4] for i in idx], _stream(),
+                                                                  wide=_mx(bb, gw))
             for i, ec in zip(idx, got):
                 ecs[i] = ec
         torch.cuda.synchronize()
-        want = np.full(out.numel(), GUARD16, dtype=np.uint16)
         written = np.zeros(out.numel(), dtype=bool)
         E = bb.ErrorCode
         mismatches = 0
@@ -399,8 +464,8 @@ class Model:
             if o is None:
                 exp = E.OBJECT_NOT_FOUND
             else:
-                desc += f" n={o.x.size} {o.tier} x{o.copies}"
-                gap_bad = rows > 1 and w < pitch and (pitch - w) % 8 != 0
+                desc += f" n={o.x.size} packed as {o.w} {o.tier} x{o.copies}"
+                gap_bad = rows > 1 and w < pitch and (pitch - w) % per != 0
                 usable = any(len(shs) == 1 and self.fabric(shs[0]) for shs in self.shards(k))
                 # the whole-object call leaves alignment to the engine: its buffers here are always aligned
                 if not usable or (kind != "whole" and (skew or gap_bad)):
@@ -415,16 +480,333 @@ class Model:
                 written[region:region + w * rows] = True
             if exp == E.OK:
                 el = np.concatenate([np.arange(off + r * pitch, off + r * pitch + w) for r in range(rows)])
-                want[region:region + el.size] = o.back[el]
                 written[region:region + el.size] = True
-                same_bits(out[region:region + el.size].cpu().numpy(), o.back[el], "bf16", self.where(i, desc))
+                _same(out[region:region + el.size].cpu().numpy(), o.back(gw)[el], gw, self.where(i, desc))
+                self.outcomes["cross-type read"] += gw != o.w
             self.outcomes[str(exp).split(".")[-1]] += 1
             self.outcomes["fused"] += exp == E.OK
-        got = out.cpu().numpy().view(np.uint16)
-        bad = np.nonzero(~written & (got != GUARD16))[0]
+        got = out.cpu().numpy().view(np.uint16 if gb == 2 else np.uint32)
+        bad = np.nonzero(~written & (got != WGUARD[gb]))[0]
         assert bad.size == 0, f"{self.where()}: {bad.size} elements written outside the results, first at {bad[:4].tolist()}"
         assert self.counter("get_placement_refresh_total") - ref0 == mismatches, f"{self.where()}: placement refreshes"
         self.outcomes["fail-over"] += self.counter("replica_failover_total") - fo0
+
+    # ------------------------------------------------------------------------------------------------ pages and rows
+
+    def put_staged(self, key, addrs, page):
+        """The client's documented rule for a paged put: fused only if every shard of every copy is co-aligned with the
+        pages (SourcePages::coaligned from the shard's start) and every shard is reachable by the fabric."""
+        placed = self.shards(key)
+        ok = all(pages_coaligned(addrs, page, off, sh.length) for shs in placed for off, sh in zip(_starts(shs), shs))
+        return not ok or not all(self.fabric(sh) for shs in placed for sh in shs)
+
+    def get_staged(self, key, aligned):
+        """The rule of a whole-object get into pages or rows: fused only if aligned(off, length) holds for every shard of
+        every copy and some copy has every shard in HBM or DRAM."""
+        placed = self.shards(key)
+        if not all(aligned(off, sh.length) for shs in placed for off, sh in zip(_starts(shs), shs)):
+            return True
+        return not any(all(self.fabric(sh) for sh in shs) for shs in placed)
+
+    def put_paged(self):
+        bb, rng = self.bb, self.rng
+        count = int(rng.integers(1, 5))
+        algo, reps, workers = ALGOS[int(rng.integers(0, 4))], int(rng.integers(1, 4)), int(rng.integers(1, 3))
+        tier = str(rng.choice(["RAM_GPU", "RAM_CPU"]))
+        self.what = f"paged put of {count}, {algo}, {reps} replicas, {workers} workers per copy, {tier}"
+        keys = [self.new_key() for _ in range(count)]
+        specs = []  # (page, pages, skew, repeats)
+        for _ in keys:
+            page = int(rng.choice([16, 48, 4096, T + 16, 32768 + 48, 16 * int(rng.integers(1, 300)), int(rng.integers(1, 5000)) | 1]))
+            npg = 1 if page % 16 else int(rng.integers(1, max(2, min(200, 300000 // page)) + 1))
+            specs.append((0 if rng.random() < 0.05 else page, npg, 8 if rng.random() < 0.15 else 0, npg > 1 and rng.random() < 0.2))
+        slot = (max(max(s[0], 16) for s in specs) + 15) // 16 * 16 + 64
+        src = torch.empty(sum(s[1] for s in specs) * slot + 64, dtype=torch.uint8, device="cuda")
+        bb.random_fill(src.data_ptr(), src.numel(), int(rng.integers(1, 1 << 40)), _stream())
+        host = src.cpu().numpy()
+        free = list(rng.permutation(sum(s[1] for s in specs)))
+        lists, datas = [], []
+        for page, npg, skew, rep in specs:
+            offs = [int(free.pop()) * slot + skew for _ in range(npg)]
+            if rep:  # a page may repeat
+                for j in rng.integers(0, npg, max(1, npg // 4)):
+                    offs[int(j)] = offs[int(rng.integers(0, npg))]
+            lists.append([src.data_ptr() + o for o in offs])
+            datas.append(np.concatenate([host[o:o + page] for o in offs]) if page else None)
+        st0 = self.counter("device_put_host_staged_total")
+        ecs = self.cl.client.batch_put_device_paged(keys, lists, [s[0] for s in specs], _cfg(bb, algo, reps, tier, workers), _stream())
+        staged = 0
+        for i, (k, (page, npg, skew, rep), addrs, data) in enumerate(zip(keys, specs, lists, datas)):
+            desc = f"{k} page={page} pages={npg} skew={skew} repeats={rep}"
+            exp = bb.ErrorCode.INVALID_ARGUMENT if page == 0 else bb.ErrorCode.OK
+            assert ecs[i] == exp, f"{self.where(i, desc)}: {ecs[i]}, want {exp}"
+            self.outcomes[str(exp).split(".")[-1]] += 1
+            if page:
+                self.objs[k] = Obj(data, algo, reps, None)
+                staged += self.put_staged(k, addrs, page)
+        assert self.counter("device_put_host_staged_total") - st0 == staged, f"{self.where()}: staged items"
+        self.outcomes["put staged"] += staged
+
+    def _results(self, out, want, items):
+        """Every result byte and every guard byte: `items` = (description, result offsets) per item."""
+        got = out.cpu().numpy().view(want.dtype)
+        bad = np.nonzero(got != want)[0]
+        if bad.size:
+            first = int(bad[0])
+            near = [(i, d) for i, (d, ds) in enumerate(items) if ds.size and ds.min() - 64 <= first <= ds.max() + 64]
+            pytest.fail(f"{self.where()}: {bad.size} wrong result or guard units, first at {first} (got {got[first]:#x}, "
+                        f"want {want[first]:#x}), near items {near}")
+
+    def get_paged(self, keys=None):
+        bb, rng = self.bb, self.rng
+        E = bb.ErrorCode
+        keys = keys or self.pick(False, int(rng.integers(1, 6)), gone=0.3)
+        if not keys:
+            return
+        specs, cur = [], 64
+        for k in keys:
+            o = self.objs.get(k)
+            n = o.data.size if o else 100
+            page = int(rng.choice([16, 48, 4096, T + 16, 32768 + 48, 16 * int(rng.integers(1, 100)) + 8]))
+            npg = -(-n // page)
+            r = rng.random()
+            npg = npg - 1 if r < 0.1 else npg + int(rng.integers(1, 3)) if r < 0.3 else npg  # too few pages, or more than needed
+            skew = 8 if rng.random() < 0.15 else 0
+            stride = (page + 15) // 16 * 16 + 48
+            offs = [cur + int(j) * stride + skew for j in rng.permutation(npg)]
+            cur += npg * stride + 64
+            specs.append((k, o, 0 if o is not None and offs and rng.random() < 0.05 else page, offs))  # page 0 with pages
+        out = torch.full((cur + 64,), GUARD, dtype=torch.uint8, device="cuda")
+        p = out.data_ptr()
+        self.what = f"paged get of {len(keys)}"
+        st0, ref0, fo0 = self.counter("device_get_host_staged_total"), self.counter("get_placement_refresh_total"), self.counter("replica_failover_total")
+        ecs, sizes = self.cl.client.batch_get_device_paged(keys, [[p + a for a in s[3]] for s in specs], [s[2] for s in specs], _stream())
+        torch.cuda.synchronize()
+        want = np.full(out.numel(), GUARD, dtype=np.uint8)
+        staged = mismatches = 0
+        items = []
+        for i, (k, o, page, offs) in enumerate(specs):
+            desc = f"{k} page={page} pages={len(offs)} skew={offs[0] % 16 if offs else 0}"
+            ds = np.zeros(0, dtype=np.int64)
+            if o is None:
+                exp = E.OBJECT_NOT_FOUND
+            elif page == 0:
+                exp = E.INVALID_ARGUMENT
+            elif o.data.size > page * len(offs):
+                exp = E.BUFFER_OVERFLOW
+            else:
+                desc += f" n={o.data.size} {o.algo} tier={o.tier} x{o.copies}"
+                bad_ = self.mismatch(k, o, 0, o.data.size, o.data.size, 1)
+                exp = E.CHECKSUM_MISMATCH if bad_ else E.OK
+                addrs = [p + a for a in offs]
+                staged += self.get_staged(k, lambda off, ln: pages_fused(addrs, page, off, ln)) * (1 + bad_)
+                ds = pages_at(o.data.size, offs, page, 0)
+                if exp == E.OK:
+                    want[ds] = o.data
+                    assert sizes[i] == o.data.size, f"{self.where(i, desc)}: size {sizes[i]}"
+                    self.outcomes["paged fused"] += not self.get_staged(k, lambda off, ln: pages_fused(addrs, page, off, ln))
+                else:
+                    want[ds] = out[torch.from_numpy(ds).cuda()].cpu().numpy()  # unspecified, nothing around them
+            assert ecs[i] == exp, f"{self.where(i, desc)}: {ecs[i]}, want {exp}"
+            mismatches += exp == E.CHECKSUM_MISMATCH
+            self.outcomes[str(exp).split(".")[-1]] += 1
+            items.append((desc, ds))
+        self._results(out, want, items)
+        assert self.counter("device_get_host_staged_total") - st0 == staged, f"{self.where()}: staged items"
+        assert self.counter("get_placement_refresh_total") - ref0 == mismatches, f"{self.where()}: placement refreshes"
+        self.outcomes["fail-over"] += self.counter("replica_failover_total") - fo0
+
+    def get_scatter(self, keys=None):
+        bb, rng = self.bb, self.rng
+        E = bb.ErrorCode
+        keys = keys or self.pick(False, int(rng.integers(1, 6)), gone=0.3)
+        if not keys:
+            return
+        specs, cur = [], 64
+        for k in keys:
+            o = self.objs.get(k)
+            n = o.data.size if o else 100
+            width = int(rng.integers(1, min(n, 4000) + 1))
+            pitch = width + int(rng.choice([0, 16, 16 * int(rng.integers(1, 40)), int(rng.integers(1, 200))]))
+            rows = -(-n // width)
+            r = rng.random()
+            rows = rows - 1 if r < 0.1 else rows + int(rng.integers(1, 3)) if r < 0.25 else rows
+            skew = 8 if rng.random() < 0.15 else int(rng.choice([0, 1, 3])) if rng.random() < 0.1 else 0
+            at = (cur + 15) // 16 * 16 + skew
+            cur = at + max(rows - 1, 0) * pitch + width + 64
+            specs.append((k, o, width, pitch, rows, at))
+        out = torch.full((cur + 64,), GUARD, dtype=torch.uint8, device="cuda")
+        p = out.data_ptr()
+        self.what = f"scattered get of {len(keys)}"
+        st0, ref0, fo0 = self.counter("device_get_host_staged_total"), self.counter("get_placement_refresh_total"), self.counter("replica_failover_total")
+        ecs, sizes = self.cl.client.batch_get_device_scatter(keys, [p + s[5] for s in specs], [s[2] for s in specs], [s[3] for s in specs],
+                                                             [s[4] for s in specs], _stream())
+        torch.cuda.synchronize()
+        want = np.full(out.numel(), GUARD, dtype=np.uint8)
+        staged = mismatches = 0
+        items = []
+        for i, (k, o, width, pitch, rows, at) in enumerate(specs):
+            desc = f"{k} width={width} pitch={pitch} rows={rows} at%16={at % 16}"
+            ds = np.zeros(0, dtype=np.int64)
+            if o is None:
+                exp = E.OBJECT_NOT_FOUND
+            elif o.data.size > rows * width:
+                exp = E.BUFFER_OVERFLOW
+            else:
+                desc += f" n={o.data.size} {o.algo} tier={o.tier} x{o.copies}"
+                bad_ = self.mismatch(k, o, 0, o.data.size, o.data.size, 1)
+                exp = E.CHECKSUM_MISMATCH if bad_ else E.OK
+                staged += self.get_staged(k, lambda off, ln: rows_fused(p + at, width, pitch, rows, off)) * (1 + bad_)
+                ds = at + rows_at(o.data.size, pitch if rows > 1 else width, width, 0)
+                if exp == E.OK:
+                    want[ds] = o.data
+                    assert sizes[i] == o.data.size, f"{self.where(i, desc)}: size {sizes[i]}"
+                else:
+                    want[ds] = out[torch.from_numpy(ds).cuda()].cpu().numpy()  # unspecified, nothing around them
+            assert ecs[i] == exp, f"{self.where(i, desc)}: {ecs[i]}, want {exp}"
+            mismatches += exp == E.CHECKSUM_MISMATCH
+            self.outcomes[str(exp).split(".")[-1]] += 1
+            items.append((desc, ds))
+        self._results(out, want, items)
+        assert self.counter("device_get_host_staged_total") - st0 == staged, f"{self.where()}: staged items"
+        assert self.counter("get_placement_refresh_total") - ref0 == mismatches, f"{self.where()}: placement refreshes"
+        self.outcomes["fail-over"] += self.counter("replica_failover_total") - fo0
+
+    def put_fp8_paged(self):
+        bb, rng = self.bb, self.rng
+        E = bb.ErrorCode
+        count = int(rng.integers(1, 4))
+        tier, w = str(rng.choice(["RAM_GPU", "RAM_CPU"])), str(rng.choice(WIDES))
+        b, per = WB[w], 16 // WB[w]
+        self.what = f"fp8 paged put of {count}, {w}, {tier}"
+        keys = [self.new_key() for _ in range(count)]
+        specs, cur = [], 16
+        for _ in keys:
+            page = int(rng.choice([per, 3 * per, 32, 5 * per, 8 * per * int(rng.integers(1, 40)), per * int(rng.integers(1, 50)) + per // 2]))
+            npg = 32 // math.gcd(page, 32) * int(rng.integers(1, max(2, 6000 // page)))  # a whole number of MX blocks
+            if rng.random() < 0.08:
+                npg += 1  # unless that makes a partial block
+            skew = b if rng.random() < 0.12 else 0  # one page off 16-byte alignment
+            stride = (page * b + 15) // 16 * 16 + 32
+            offs = [cur + int(j) * stride for j in rng.permutation(npg)]
+            if skew:
+                offs[int(rng.integers(0, npg))] += skew
+            cur += npg * stride + 32
+            specs.append((page, offs))
+        buf = np.full(cur + 64, GUARD, dtype=np.uint8)
+        xs = []
+        for page, offs in specs:
+            x = _wide(rng, page * len(offs) // 32 * 32 + 32, w)[:page * len(offs)]
+            buf[pages_at(x.size * b, offs, page * b, 0)] = x.view(np.uint8)
+            xs.append(x)
+        src = torch.from_numpy(buf).cuda()
+        lists = [[src.data_ptr() + o for o in offs] for _, offs in specs]
+        ecs = self.cl.client.batch_put_device_fp8_paged(keys, lists, [s[0] for s in specs], _cfg(bb, "BBH64", 1, tier), _stream(),
+                                                        wide=_mx(bb, w))
+        torch.cuda.synchronize()
+        for i, (k, (page, offs), x) in enumerate(zip(keys, specs, xs)):
+            desc = f"{k} page={page} pages={len(offs)} n={x.size}"
+            if x.size % 32:
+                exp = E.INVALID_ARGUMENT
+            elif not pages_coaligned(lists[i], page * b, 0, x.size * b):
+                exp = E.NOT_IMPLEMENTED
+            else:
+                exp = E.OK
+                self.objs[k] = Obj(_pack_model(x, w), "BBH64", 1, tier, x, w)
+            assert ecs[i] == exp, f"{self.where(i, desc)}: {ecs[i]}, want {exp}"
+            self.outcomes[str(exp).split(".")[-1]] += 1
+
+    def _fp8_usable(self, k):
+        return any(len(shs) == 1 and self.fabric(shs[0]) for shs in self.shards(k))
+
+    def get_fp8_paged(self, keys=None, scatter=False):
+        """Gets of packed objects into pages (or, scatter=True, into rows), in a type drawn per call."""
+        bb, rng = self.bb, self.rng
+        E = bb.ErrorCode
+        keys = keys or self.pick(True, int(rng.integers(1, 5)), gone=0.3)
+        if not keys:
+            return
+        gw = str(rng.choice(WIDES))
+        gb, per = WB[gw], 16 // WB[gw]
+        specs, cur = [], 16  # in elements
+        for k in keys:
+            o = self.objs.get(k)
+            n = o.x.size if o else 64
+            skew = int(rng.choice([1, per // 2])) if rng.random() < 0.15 else 0
+            if scatter:
+                width = 32 * int(rng.choice([d for d in (1, 2, 3, 4, 8, 16) if (n // 32) % d == 0]))
+                width = n if rng.random() < 0.1 else width
+                pitch = width + int(rng.choice([0, per, per * int(rng.integers(1, 30)), int(rng.integers(1, 100))]))
+                rows = n // width - (1 if o is not None and n > width and rng.random() < 0.05 else 0)
+                at = (cur + per - 1) // per * per + skew
+                cur = at + max(rows - 1, 0) * pitch + width + 32
+                specs.append((k, o, (width, pitch, rows), at))
+            else:
+                page = int(rng.choice([d for d in (per, 3 * per, 32, 5 * per, 8 * per, 40 * per, n) if n % d == 0]))
+                if o is not None and rng.random() < 0.08:
+                    page += 1  # pages * page may no longer be the object's element count
+                npg = -(-n // page)
+                stride = (page + per - 1) // per * per + 2 * per
+                offs = [cur + int(j) * stride for j in rng.permutation(npg)]
+                if skew:
+                    offs[int(rng.integers(0, npg))] += skew
+                cur += npg * stride + 32
+                specs.append((k, o, page, offs))
+        out = torch.full((cur + 64,), WGUARD[gb], dtype=torch.int16 if gb == 2 else torch.int32, device="cuda")
+        p = out.data_ptr()
+        self.what = f"fp8 {'scattered' if scatter else 'paged'} get of {len(keys)} as {gw}"
+        ref0, fo0 = self.counter("get_placement_refresh_total"), self.counter("replica_failover_total")
+        ns = [s[1].x.size if s[1] is not None else 64 for s in specs]
+        if scatter:
+            ecs = self.cl.client.batch_get_device_fp8_scatter(keys, [p + gb * s[3] for s in specs], ns, [s[2][0] for s in specs],
+                                                              [s[2][1] for s in specs], [s[2][2] for s in specs], _stream(), wide=_mx(bb, gw))
+        else:
+            ecs = self.cl.client.batch_get_device_fp8_paged(keys, [[p + gb * a for a in s[3]] for s in specs], [s[2] for s in specs], _stream(),
+                                                            wide=_mx(bb, gw))
+        torch.cuda.synchronize()
+        got = out.cpu().numpy().view(np.uint16 if gb == 2 else np.uint32)
+        written = np.zeros(got.size, dtype=bool)
+        mismatches = 0
+        for i, (k, o, shape, at) in enumerate(specs):
+            desc = f"{k} {'rows (width, pitch, rows)' if scatter else 'page'}={shape} {'at' if scatter else 'pages'}={at if scatter else len(at)}"
+            if o is None:
+                exp = E.OBJECT_NOT_FOUND
+            else:
+                n = o.x.size
+                desc += f" n={n} packed as {o.w} {o.tier}"
+                if scatter:
+                    width, pitch, rows = shape
+                    ds = at + rows_at(n, pitch if rows > 1 else width, width, 0)
+                    count_ok = rows * width == n
+                    aligned = (p + gb * at) % 16 == 0 and not (rows > 1 and width < pitch and (pitch - width) % per)
+                else:
+                    ds = pages_at(n, at, shape, 0) if len(at) * shape >= n else np.zeros(0, dtype=np.int64)
+                    count_ok = len(at) * shape == n
+                    addrs = [p + gb * a for a in at]
+                    aligned = not (len(at) > 1 and (shape * gb) % 16) and pages_coaligned(addrs, shape * gb, 0, n * gb)
+                if not count_ok:
+                    exp = E.INVALID_ARGUMENT
+                elif not self._fp8_usable(k) or not aligned:
+                    exp = E.NOT_IMPLEMENTED
+                elif self.mismatch(k, o, 0, o.data.size, o.data.size, 1):
+                    exp = E.CHECKSUM_MISMATCH
+                    written[ds] = True  # unspecified, nothing around them
+                else:
+                    exp = E.OK
+                    written[ds] = True
+                    _same(got[ds], o.back(gw), gw, self.where(i, desc))
+                    self.outcomes["cross-type read"] += gw != o.w
+            assert ecs[i] == exp, f"{self.where(i, desc)}: {ecs[i]}, want {exp}"
+            mismatches += exp == E.CHECKSUM_MISMATCH
+            self.outcomes[str(exp).split(".")[-1]] += 1
+            self.outcomes["fused"] += exp == E.OK
+        bad = np.nonzero(~written & (got != WGUARD[gb]))[0]
+        assert bad.size == 0, f"{self.where()}: {bad.size} elements written outside the results, first at {bad[:4].tolist()}"
+        assert self.counter("get_placement_refresh_total") - ref0 == mismatches, f"{self.where()}: placement refreshes"
+        self.outcomes["fail-over"] += self.counter("replica_failover_total") - fo0
+
+    def get_fp8_scatter(self, keys=None):
+        self.get_fp8_paged(keys, scatter=True)
 
     def migrate(self):
         keys = [k for k in self.objs]
@@ -446,9 +828,12 @@ class Model:
         keys = [k for k, o in self.objs.items() if o.algo != "NONE" and all(self.fabric(sh) for shs in self.shards(k) for sh in shs)]
         if not keys:
             return
+        everyone = rng.random() < 0.5
+        replicated = [k for k in keys if self.objs[k].copies > 1]
+        if not everyone and replicated and rng.random() < 0.7:  # one corrupt copy of several: the gets fail over
+            keys = replicated
         k = str(rng.choice(keys))
         o = self.objs[k]
-        everyone = rng.random() < 0.5
         placed = self.shards(k)
         flips = []
         for c, shs in enumerate(placed):
@@ -463,8 +848,10 @@ class Model:
         o.flips = {(c, s) for c, s, _ in flips}
         others = self.pick(o.fp8, 2)
         try:
-            for _ in range(2):  # two gets: the shapes are drawn anew each time
-                (self.get_fp8 if o.fp8 else self.get)([k] + others)
+            # a get of a shape drawn anew each time, then a get into pages or into rows
+            calls = [self.get_fp8, self.get_fp8_paged, self.get_fp8_scatter] if o.fp8 else [self.get, self.get_paged, self.get_scatter]
+            calls[0]([k] + others)
+            calls[int(rng.integers(1, 3))]([k] + others)
         finally:
             for c, s, pos in flips:
                 self.store.flip(placed[c][s], pos)
@@ -482,7 +869,7 @@ class Model:
             self.gone.add(k)
 
     def run(self, steps):
-        weights = np.array([3, 2, 4, 4, 2, 1, 3, 1], dtype=float)
+        weights = np.array([3, 2, 4, 4, 2, 1, 3, 1, 2, 3, 3, 2, 2, 2], dtype=float)
         for self.step in range(steps):
             op = OPS[int(self.rng.choice(len(OPS), p=weights / weights.sum()))] if self.step >= 4 else ["put", "put_fp8"][self.step % 2]
             self.ops[op] += 1
@@ -497,7 +884,8 @@ def test_random_operation_sequences(bb, tmp_path, seed):
         m = Model(bb, cl, seed)
         m.run(STEPS)
         print(f"\nseed {seed}: operations {dict(m.ops)}; outcomes {dict(m.outcomes)}")
-        for o in ("fused", "staged", "NOT_IMPLEMENTED", "CHECKSUM_MISMATCH", "fail-over", "OBJECT_NOT_FOUND"):
+        for o in ("fused", "staged", "NOT_IMPLEMENTED", "CHECKSUM_MISMATCH", "fail-over", "OBJECT_NOT_FOUND", "BUFFER_OVERFLOW",
+                  "INVALID_ARGUMENT", "cross-type read", "paged fused", "put staged"):
             assert m.outcomes[o] > 0, f"seed {seed}: no {o} outcome in {STEPS} steps: {dict(m.outcomes)}"
     finally:
         cl.stop()
