@@ -160,8 +160,8 @@ int main(int argc, char** argv) {
     std::vector<uint8_t> h1(65536), h2(65536);
     bool same = true;
     for (size_t off : {size_t{0}, nobj * osz - 65536}) {
-      fab.value()->copy_d2h(h1.data(), static_cast<uint8_t*>(src) + off, 65536, nullptr);
-      fab.value()->copy_d2h(h2.data(), static_cast<uint8_t*>(dst) + off, 65536, nullptr);
+      fab.value()->copy_from_device(h1.data(), static_cast<uint8_t*>(src) + off, {}, 65536, nullptr);
+      fab.value()->copy_from_device(h2.data(), static_cast<uint8_t*>(dst) + off, {}, 65536, nullptr);
       same &= h1 == h2;
     }
     auto avg = [](const std::vector<double>& v) { return v.empty() ? 0.0 : std::accumulate(v.begin(), v.end(), 0.0) / static_cast<double>(v.size()); };

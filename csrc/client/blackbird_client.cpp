@@ -682,23 +682,23 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::
   const size_t n = keys.size();
   const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<uint64_t> elems(n);
-  std::vector<SourceRows> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_put_fp8_strided", true, n, bf16_ptrs.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
       [&](size_t i, uint64_t* wide_bytes) {
-        SourceRows bytes;
+        DeviceLayout bytes;
         uint64_t extent = 0;
-        const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems[i], &extent);
+        const ErrorCode ec = DeviceLayout::from_rows(elem_widths[i], elem_pitches[i], rows[i], &mems[i], &elems[i], &extent);
         *wide_bytes = b * elems[i];
         if (ec != ErrorCode::OK) return ec;
-        if (extent > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        if (extent > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
         // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
         if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &p, cfg, stream, wide);
+        const auto m = pick(mems, idx);
+        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &m, cfg, stream, wide);
       });
 }
 
@@ -708,36 +708,33 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_paged(const std::ve
   const size_t n = keys.size();
   const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<uint64_t> elems(n);
-  std::vector<SourcePages> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_put_fp8_paged", true, n, pages.size() == n && page_elems.size() == n,
       [&](size_t i, uint64_t* wide_bytes) {
-        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &pats[i], &elems[i]);
+        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &mems[i], &elems[i]);
         if (ec != ErrorCode::OK) return ec;
         if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks
-        SourcePages bytes;
-        if (elems[i] > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        DeviceLayout bytes;
+        if (elems[i] > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
         *wide_bytes = b * elems[i];
         // the engine's rule for a paged pack, checked once: there is no host-staged path for packed puts
-        if (!bytes.coaligned(b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
+        if (!bytes.coaligned(0, b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), nullptr, cfg, stream, wide, &p);
+        const auto m = pick(mems, idx);
+        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), &m, cfg, stream, wide);
       });
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
-                                                       const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows,
-                                                       const WorkerConfig& cfg, void* stream, mxfp8::Wide wide,
-                                                       const std::vector<SourcePages>* pages) {
+                                                       const std::vector<uint64_t>& n_elems, const std::vector<DeviceLayout>* mem,
+                                                       const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (rows && rows->size() != keys.size()) ||
-      (pages && (rows || pages->size() != keys.size())))
-    return out;
+  if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (mem && mem->size() != keys.size())) return out;
   BB_TRACE_SPAN("batch_put_device_fp8", keys.size());
   WorkerConfig c = cfg;
   c.replication_factor = std::max<size_t>(1, std::min<size_t>(cfg.replication_factor, 3));  // one tile pass fans out to <= 3 copies
@@ -767,8 +764,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
       continue;
     }
     DeviceFp8Op op{&copies[0].shards[0], const_cast<void*>(bf16_ptrs[i]), n_elems[i], {}};
-    if (rows) op.rows = (*rows)[i];
-    if (pages) op.pages = (*pages)[i];
+    if (mem) op.mem = (*mem)[i];
     op.wide_type = wide;
     for (size_t cidx = 1; cidx < copies.size(); ++cidx) op.replicas.push_back(&copies[cidx].shards[0]);
     ops.push_back(std::move(op));
@@ -808,23 +804,23 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_scatter(const std::
                                                                      void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
   const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<SourceRows> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_get_fp8_scatter", false, n,
       bf16_ptrs.size() == n && n_elems.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
       [&](size_t i, uint64_t* wide_bytes) {
-        SourceRows bytes;
+        DeviceLayout bytes;
         uint64_t elems = 0, extent = 0;
-        const ErrorCode ec = SourceRows::from_rows(elem_widths[i], elem_pitches[i], rows[i], &pats[i], &elems, &extent);
+        const ErrorCode ec = DeviceLayout::from_rows(elem_widths[i], elem_pitches[i], rows[i], &mems[i], &elems, &extent);
         if (ec != ErrorCode::OK) return ec;
         if (elems != n_elems[i]) return ErrorCode::INVALID_ARGUMENT;
-        if (extent > UINT64_MAX / b || !pats[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        if (extent > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
         *wide_bytes = b * elems;
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &p, stream, wide);
+        const auto m = pick(mems, idx);
+        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &m, stream, wide);
       });
 }
 
@@ -866,11 +862,11 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::ve
   const size_t n = keys.size();
   const uint64_t b = mxfp8::wide_bytes(wide);
   std::vector<uint64_t> elems(n);
-  std::vector<SourcePages> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_get_fp8_paged", false, n, pages.size() == n && page_elems.size() == n,
       [&](size_t i, uint64_t* wide_bytes) {
-        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &pats[i], &elems[i]);
+        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &mems[i], &elems[i]);
         if (ec != ErrorCode::OK) return ec;
         if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
         if (elems[i] > UINT64_MAX / b) return ErrorCode::VALUE_OUT_OF_RANGE;
@@ -878,22 +874,22 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::ve
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, nullptr, stream, wide, &p);
+        const auto m = pick(mems, idx);
+        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, &m, stream, wide);
       });
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                                       const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide,
-                                                       const std::vector<SourcePages>* pages) {
+                                                       const std::vector<DeviceLayout>* mem, void* stream, mxfp8::Wide wide) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   const uint64_t b = mxfp8::wide_bytes(wide);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (rows && (ranges || rows->size() != keys.size())) || (pages && (ranges || rows || pages->size() != keys.size())))
+      (mem && (ranges || mem->size() != keys.size())))
     return out;
+  auto mem_of = [&](size_t i) { return mem ? (*mem)[i] : DeviceLayout{}; };
   BB_TRACE_SPAN("batch_get_device_fp8", keys.size());
   auto placed = keystone_->batch_get_workers(keys);
   std::vector<std::vector<size_t>> candidates(keys.size());
@@ -919,7 +915,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
-    if (pages && !copies.empty()) {  // the pages must hold exactly the stored object's elements
+    if (mem_of(i).kind() == DeviceLayout::PAGES && !copies.empty()) {  // the pages must hold exactly the stored object's elements
       uint64_t stored = 0;
       for (const auto& sh : copies[0].shards) stored += sh.length;
       if (stored != packed) {
@@ -943,21 +939,14 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
       out[i] = ErrorCode::NOT_IMPLEMENTED;  // demoted to a host tier, striped, other digest: caller gets + unpacks instead
       continue;
     }
-    // a range the kernel cannot store (StoreWindow::fused_get_aligned) fails alone, so that the rest of the batch still
-    // takes the fused launch; the caller reads it whole and slices instead.  A whole tensor is left to the engine.
+    // a range or a layout the kernel cannot store into (DeviceLayout::fused_get_aligned) fails alone, so that the rest of
+    // the batch still takes the fused launch; the caller reads it whole and slices instead.  A whole tensor of a plain get
+    // is left to the engine.
     StoreWindow bytes;
-    if (ranges && (!w.to_wide_bytes(b, &bytes) || !bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, b * n_elems[i]))) {
-      out[i] = ErrorCode::NOT_IMPLEMENTED;
-      continue;
-    }
-    SourceRows dst_bytes;  // so do destination rows the kernel cannot store into
-    if (rows && (!(*rows)[i].to_wide_bytes(b, &dst_bytes) ||
-                 !dst_bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, b * n_elems[i]))) {
-      out[i] = ErrorCode::NOT_IMPLEMENTED;
-      continue;
-    }
-    SourcePages dst_pages;  // and destination pages
-    if (pages && (!(*pages)[i].to_wide_bytes(b, &dst_pages) || !dst_pages.fused_get_aligned(0, b * n_elems[i]))) {
+    DeviceLayout dst_bytes;
+    if ((ranges || mem) &&
+        (!w.to_wide_bytes(b, &bytes) || !mem_of(i).to_wide_bytes(b, &dst_bytes) ||
+         !dst_bytes.fused_get_aligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), 0, b * n_elems[i], bytes))) {
       out[i] = ErrorCode::NOT_IMPLEMENTED;
       continue;
     }
@@ -974,8 +963,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ErrorCode::CHECKSUM_MISMATCH;
         continue;
       }
-      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], rows ? (*rows)[i] : SourceRows{}, wide,
-                     pages ? (*pages)[i] : SourcePages{}});
+      ops.push_back({&placed[i].value()[candidates[i][attempt]].shards[0], bases[i], n_elems[i], {}, wins[i], mem_of(i), wide});
       cur.push_back(i);
     }
     if (ops.empty()) break;
@@ -992,10 +980,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   // a key that moved to a non-fusable placement comes back NOT_IMPLEMENTED from the refresh, i.e. "get + unpack instead"
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
-    const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
-    const auto rpages = pages ? pick(*pages, r) : std::vector<SourcePages>();
-    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr, stream,
-                          wide, pages ? &rpages : nullptr);
+    const auto rmem = mem ? pick(*mem, r) : std::vector<DeviceLayout>();
+    return get_device_fp8(pick(keys, r), pick(bf16_ptrs, r), pick(n_elems, r), ranges ? &rranges : nullptr, mem ? &rmem : nullptr, stream,
+                          wide);
   });
   metrics_.inc("device_get_fp8_batches_total");
   return out;
@@ -1137,8 +1124,8 @@ static void ewma_update(std::atomic<double>& v, double sample) {
 
 // The fused kernels move 16-byte aligned buffers only (XferEngine::submit refuses a whole batch otherwise).  An object
 // whose caller buffer is not aligned with one of its shards is staged through host memory instead, so that it does not
-// fail its neighbours: a put's source where every shard starts (for a strided or paged source, every shard co-aligned), a
-// get's destination by StoreWindow::fused_get_aligned (SourceRows's or SourcePages's for a get into rows or pages).  Whether ok(off, len) holds for the shard [off, off + len) of every copy.
+// fail its neighbours: a put's source by DeviceLayout::coaligned from every shard's start, a get's destination by
+// DeviceLayout::fused_get_aligned.  Whether ok(off, len) holds for the shard [off, off + len) of every copy.
 template <class F>
 static bool fabric_aligned(const std::vector<CopyPlacement>& copies, F&& ok) {
   for (const auto& c : copies) {
@@ -1161,20 +1148,20 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vect
                                                                  const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
   std::vector<size_t> sizes(n);
-  std::vector<SourceRows> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_put_strided", true, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
       [&](size_t i, uint64_t* size) {
         uint64_t extent = 0;
-        const ErrorCode ec = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pats[i], size, &extent);
+        const ErrorCode ec = DeviceLayout::from_rows(widths[i], pitches[i], rows[i], &mems[i], size, &extent);
         if (ec != ErrorCode::OK) return ec;
         if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
         sizes[i] = static_cast<size_t>(*size);
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return put_device(pick(keys, idx), pick(dev_ptrs, idx), pick(sizes, idx), &p, cfg, stream);
+        const auto m = pick(mems, idx);
+        return put_device(pick(keys, idx), pick(dev_ptrs, idx), pick(sizes, idx), &m, cfg, stream);
       });
 }
 
@@ -1182,33 +1169,30 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector
                                                                const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
   std::vector<size_t> sizes(n);
-  std::vector<SourcePages> pats(n);
+  std::vector<DeviceLayout> mems(n);
   return shaped_batch(
       "device_put_paged", true, n, pages.size() == n && page_bytes.size() == n,
       [&](size_t i, uint64_t* size) {
-        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &pats[i], size);
+        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &mems[i], size);
         if (ec != ErrorCode::OK) return ec;
         if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
         sizes[i] = static_cast<size_t>(*size);
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
-        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), nullptr, cfg, stream, &p);
+        const auto m = pick(mems, idx);
+        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), &m, cfg, stream);
       });
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
-                                                   const std::vector<size_t>& sizes, const std::vector<SourceRows>* rows,
-                                                   const WorkerConfig& cfg, void* stream, const std::vector<SourcePages>* pages) {
+                                                   const std::vector<size_t>& sizes, const std::vector<DeviceLayout>* mem,
+                                                   const WorkerConfig& cfg, void* stream) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
-  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size() || (rows && rows->size() != keys.size()) ||
-      (pages && pages->size() != keys.size()))
-    return out;
-  auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
-  auto pages_of = [&](size_t i) { return pages ? (*pages)[i] : SourcePages{}; };
+  if (dev_ptrs.size() != keys.size() || sizes.size() != keys.size() || (mem && mem->size() != keys.size())) return out;
+  auto mem_of = [&](size_t i) { return mem ? (*mem)[i] : DeviceLayout{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_put_device", keys.size());
 
@@ -1250,13 +1234,11 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
       if (copies.empty()) continue;
       // placements on host tiers (DRAM / CXL / NVMe) and unaligned caller buffers: stage through host memory and use the
       // data servers
-      const SourceRows pat = rows_of(i);
-      const SourcePages pg = pages_of(i);
+      const DeviceLayout m = mem_of(i);
       const auto src = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
       bool on_fabric = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
-        if (pg.paged()) return pg.rebase(off).coaligned(len);
         uint64_t at = 0;
-        return pat.rebase(off, &at).coaligned(src + at, len);
+        return m.rebase(off, &at).coaligned(src + at, len);
       });
       for (const auto& c : copies)
         for (const auto& sh : c.shards) {
@@ -1283,9 +1265,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
           op.copy = c;
           op.shard = s;
           op.placement = &copies[c].shards[s];
-          op.obj_offset = off;
-          op.rows = pat.rebase(off, &op.rows_at);
-          op.pages = pg.rebase(off);
+          op.mem = m.rebase(off, &op.mem_at);
           for (size_t r = 1; same_layout && r < copies.size(); ++r) op.replicas.push_back(&copies[r].shards[s]);
           ch.ops.push_back(std::move(op));
           off += copies[c].shards[s].length;
@@ -1360,22 +1340,10 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
     start_chunk(chunks[c]);
   }
   while (finished < chunks.size()) finish_chunk(chunks[finished++]);
-  // host-tier placements: D2H into a staging buffer, then the TCP data path (checksums on the CPU).  A strided source is
-  // copied as its whole extent in one D2H, and its rows compacted here; a paged one with one D2H per run of pages.
+  // host-tier placements: D2H into a staging buffer, then the TCP data path (checksums on the CPU)
   for (size_t i : host_put) {
     std::vector<uint8_t> stage(sizes[i]);
-    const SourceRows pat = rows_of(i);
-    const SourcePages pg = pages_of(i);
-    ErrorCode ec;
-    if (pg.paged()) {
-      ec = device_->copy_d2h_pages(stage.data(), pg, sizes[i], stream);
-    } else if (pat.strided()) {
-      std::vector<uint8_t> extent(pat.extent(sizes[i]));
-      ec = device_->copy_d2h(extent.data(), dev_ptrs[i], extent.size(), stream);
-      pat.for_each_run(sizes[i], [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(stage.data() + x, extent.data() + at, n); });
-    } else {
-      ec = device_->copy_d2h(stage.data(), dev_ptrs[i], sizes[i], stream);
-    }
+    ErrorCode ec = device_->copy_from_device(stage.data(), dev_ptrs[i], mem_of(i), sizes[i], stream);
     ShardChecksums sums;
     if (ec == ErrorCode::OK) ec = transfer_put(host_placed[i], stage.data(), cfg.checksum, &sums);
     if (ec == ErrorCode::OK) ec = keystone_->put_complete(keys[i], sums);
@@ -1400,22 +1368,22 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_scatter(const std::vect
                                                                  const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes) {
   const size_t n = keys.size();
   std::vector<size_t> caps(n);
-  std::vector<SourceRows> pats(n);
+  std::vector<DeviceLayout> mems(n);
   if (out_sizes) out_sizes->assign(n, 0);
   return shaped_batch(
       "device_get_scatter", false, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
       [&](size_t i, uint64_t* size) {
         uint64_t extent = 0;
-        const ErrorCode ec = SourceRows::from_rows(widths[i], pitches[i], rows[i], &pats[i], size, &extent);
+        const ErrorCode ec = DeviceLayout::from_rows(widths[i], pitches[i], rows[i], &mems[i], size, &extent);
         if (ec != ErrorCode::OK) return ec;
         if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
         caps[i] = static_cast<size_t>(*size);
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
+        const auto m = pick(mems, idx);
         std::vector<size_t> sizes;
-        auto ecs = get_device(pick(keys, idx), pick(dev_ptrs, idx), pick(caps, idx), nullptr, &p, stream, &sizes);
+        auto ecs = get_device(pick(keys, idx), pick(dev_ptrs, idx), pick(caps, idx), nullptr, &m, stream, &sizes);
         for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
         return ecs;
       });
@@ -1425,21 +1393,21 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector
                                                                const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes) {
   const size_t n = keys.size();
   std::vector<size_t> caps(n);
-  std::vector<SourcePages> pats(n);
+  std::vector<DeviceLayout> mems(n);
   if (out_sizes) out_sizes->assign(n, 0);
   return shaped_batch(
       "device_get_paged", false, n, pages.size() == n && page_bytes.size() == n,
       [&](size_t i, uint64_t* size) {
-        const ErrorCode ec = SourcePages::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &pats[i], size);
+        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &mems[i], size);
         if (ec != ErrorCode::OK) return ec;
         if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
         caps[i] = static_cast<size_t>(*size);
         return ErrorCode::OK;
       },
       [&](const std::vector<size_t>& idx) {
-        const auto p = pick(pats, idx);
+        const auto m = pick(mems, idx);
         std::vector<size_t> sizes;
-        auto ecs = get_device(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(caps, idx), nullptr, nullptr, stream, &sizes, &p);
+        auto ecs = get_device(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(caps, idx), nullptr, &m, stream, &sizes);
         for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
         return ecs;
       });
@@ -1483,16 +1451,14 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
 
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                    const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges,
-                                                   const std::vector<SourceRows>* rows, void* stream, std::vector<size_t>* out_sizes,
-                                                   const std::vector<SourcePages>* pages) {
+                                                   const std::vector<DeviceLayout>* mem, void* stream, std::vector<size_t>* out_sizes) {
   std::vector<ErrorCode> out(keys.size(), ErrorCode::INVALID_PARAMETERS);
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (rows && (ranges || rows->size() != keys.size())) || (pages && (ranges || rows || pages->size() != keys.size())))
+      (mem && (ranges || mem->size() != keys.size())))
     return out;
-  auto rows_of = [&](size_t i) { return rows ? (*rows)[i] : SourceRows{}; };
-  auto pages_of = [&](size_t i) { return pages ? (*pages)[i] : SourcePages{}; };
+  auto mem_of = [&](size_t i) { return mem ? (*mem)[i] : DeviceLayout{}; };
   const TimePoint t_all = Clock::now();
   BB_TRACE_SPAN("batch_get_device", keys.size());
   if (out_sizes) out_sizes->assign(keys.size(), 0);
@@ -1523,10 +1489,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           op.copy = copy_choice[i] % copies.size();
           op.shard = s;
           op.placement = &copy.shards[s];
-          op.obj_offset = off;
           if (!whole) op.win = sp.rebase(off, len);
-          if (rows) op.rows = (*rows)[i].rebase(off, &op.rows_at);  // a scattered get: the shard's destination rows
-          if (pages) op.pages = (*pages)[i].rebase(off);            // a paged get: the shard's destination pages
+          op.mem = mem_of(i).rebase(off, &op.mem_at);
           ops.push_back(std::move(op));
         }
         off += len;
@@ -1639,12 +1603,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       const size_t start = copies.size() > 1 ? std::hash<std::string>{}(opts_.node_id + keys[i]) % copies.size() : 0;
       // an unaligned caller buffer is staged through the host whatever the replicas (see fabric_aligned)
       const auto dst = reinterpret_cast<uintptr_t>(dev_ptrs[i]);
-      const SourceRows pat = rows_of(i);
-      const SourcePages pg = pages_of(i);
-      const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) {
-        if (pages) return pg.fused_get_aligned(off, len);
-        return rows ? pat.fused_get_aligned(dst, off, len) : sp.fused_get_aligned(dst, off, len);
-      });
+      const DeviceLayout m = mem_of(i);
+      const bool aligned = fabric_aligned(copies, [&](uint64_t off, uint64_t len) { return m.fused_get_aligned(dst, off, len, sp); });
       bool found = false;
       for (size_t k = 0; aligned && k < copies.size() && !found; ++k) {
         bool local = true;
@@ -1673,20 +1633,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
         ErrorCode ec = transfer_get(copies, stage.data(), size, sp);
-        if (ec == ErrorCode::OK && pages) {  // into the pages: one H2D copy per run of pages
-          ec = device_->copy_h2d_pages(pg, stage.data(), size, stream);
-        } else if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
+        if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
           std::vector<uint8_t> dense(capacity[i]);
           sp.for_each_run(size, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + at, stage.data() + x, n); });
-          ec = device_->copy_h2d(dev_ptrs[i], dense.data(), dense.size(), stream);
-        } else if (ec == ErrorCode::OK && pat.strided()) {
-          // into the destination rows: one 2-D H2D copy of the whole rows, then the object's part of the next row
-          const uint64_t full = size / pat.width, part = size % pat.width;
-          ec = device_->copy_h2d_rows(dev_ptrs[i], pat.pitch, stage.data(), pat.width, full, stream);
-          if (ec == ErrorCode::OK && part)
-            ec = device_->copy_h2d(static_cast<uint8_t*>(dev_ptrs[i]) + full * pat.pitch, stage.data() + full * pat.width, part, stream);
-        } else if (ec == ErrorCode::OK) {
-          ec = device_->copy_h2d(dev_ptrs[i], stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
+          ec = device_->copy_to_device(dev_ptrs[i], DeviceLayout{}, dense.data(), dense.size(), stream);
+        } else if (ec == ErrorCode::OK) {  // the range, or the whole object into its layout
+          ec = device_->copy_to_device(dev_ptrs[i], m, stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
         }
         out[i] = ec;
         metrics_.inc("device_get_host_staged_total");
@@ -1767,11 +1719,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   if (n_dram_direct) metrics_.inc("device_get_dram_direct_total", n_dram_direct);
   refresh_placements(keys, placed, out, [&](const std::vector<size_t>& r) {
     const auto rranges = ranges ? pick(*ranges, r) : std::vector<ByteRange>();
-    const auto rrows = rows ? pick(*rows, r) : std::vector<SourceRows>();
-    const auto rpages = pages ? pick(*pages, r) : std::vector<SourcePages>();
+    const auto rmem = mem ? pick(*mem, r) : std::vector<DeviceLayout>();
     std::vector<size_t> rsizes;
-    auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, rows ? &rrows : nullptr,
-                           stream, &rsizes, pages ? &rpages : nullptr);
+    auto recs = get_device(pick(keys, r), pick(dev_ptrs, r), pick(capacity, r), ranges ? &rranges : nullptr, mem ? &rmem : nullptr,
+                           stream, &rsizes);
     for (size_t k = 0; out_sizes && k < r.size() && k < rsizes.size(); ++k) (*out_sizes)[r[k]] = rsizes[k];
     return recs;
   });
@@ -1795,17 +1746,10 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
     const DeviceShardOp& op = ops[k];
     const auto* src = static_cast<const uint8_t*>(op.src(dev_ptrs[op.item]));
     std::vector<uint8_t> dense;
-    if (op.pages.paged()) {  // as the kernel's paged gathering load: the shard's bytes, compacted from its pages
-      if (!op.pages.valid(op.placement->length) || op.rows.strided()) return ErrorCode::INVALID_ARGUMENT;
+    if (!op.mem.contiguous()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows or pages
+      if (!op.mem.valid(op.placement->length)) return ErrorCode::INVALID_ARGUMENT;
       dense.resize(op.placement->length);
-      op.pages.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) {
-        std::memcpy(dense.data() + x, reinterpret_cast<const void*>(at), n);
-      });
-      src = dense.data();
-    } else if (op.rows.strided()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows
-      if (!op.rows.valid()) return ErrorCode::INVALID_ARGUMENT;
-      dense.resize(op.placement->length);
-      op.rows.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, src + at, n); });
+      copy_from_device(dense.data(), src, op.mem, dense.size(), nullptr);
       src = dense.data();
     }
     ErrorCode ec = io_->write_shard(*op.placement, src, &digests[k], algo);
@@ -1823,27 +1767,17 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     ErrorCode ec;
-    if (op.pages.paged()) {  // as the kernel's paged scattering store: the whole shard, read and verified, stored into its pages
-      if (!op.pages.valid(op.placement->length) || op.rows.strided() || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
+    auto* dst = static_cast<uint8_t*>(op.dst(dev_ptrs[op.item]));
+    if (!op.mem.contiguous()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows or pages
+      if (!op.mem.valid(op.placement->length) || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      if (ec == ErrorCode::OK)
-        op.pages.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) {
-          std::memcpy(reinterpret_cast<void*>(at), whole.data() + x, n);
-        });
-    } else if (op.rows.strided()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows
-      if (!op.rows.valid() || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
-      std::vector<uint8_t> whole(op.placement->length);
-      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      auto* dst = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.rows_at;
-      if (ec == ErrorCode::OK)
-        op.rows.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + at, whole.data() + x, n); });
+      if (ec == ErrorCode::OK) copy_to_device(dst, op.mem, whole.data(), whole.size(), nullptr);
     } else if (op.win.covers(op.placement->length)) {
-      ec = io_->read_shard(*op.placement, static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset, op.placement->checksum_algo);
+      ec = io_->read_shard(*op.placement, dst, op.placement->checksum_algo);
     } else {  // as the kernel does: read and verify the whole shard, store only the window (only it is real memory)
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      auto* dst = static_cast<uint8_t*>(op.dst(dev_ptrs[op.item]));
       if (ec == ErrorCode::OK)
         op.win.for_each_run(whole.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + at, whole.data() + x, n); });
     }
@@ -1885,20 +1819,12 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
     if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
     const auto* src = static_cast<const uint8_t*>(op.wide);
     std::vector<uint8_t> dense;
-    if (op.pages.paged()) {  // as the engine and the kernel's paged gathering load: the elements, from their pages
-      SourcePages b;
-      if (op.rows.strided() || !op.win.whole() || !op.pages.valid(op.n_elems) || !op.pages.to_wide_bytes(eb, &b))
-        return ErrorCode::INVALID_ARGUMENT;
-      if (!b.coaligned(eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
-      dense.resize(eb * op.n_elems);
-      b.for_each_run(dense.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + x, reinterpret_cast<const void*>(at), n); });
-      src = dense.data();
-    } else if (op.rows.strided()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows
-      SourceRows b;
-      if (!op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+    if (!op.mem.contiguous()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows or pages
+      DeviceLayout b;
+      if (!op.win.whole() || !op.mem.valid(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
       dense.resize(eb * op.n_elems);
-      op.rows.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + eb * x, src + eb * at, eb * n); });
+      copy_from_device(dense.data(), op.wide, b, dense.size(), nullptr);
       src = dense.data();
     }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
@@ -1920,16 +1846,10 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
     const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
     if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
     if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
-    SourceRows b;
-    if (op.rows.strided()) {  // as the engine: destination rows, never with a window, co-aligned in wide bytes
-      if (!op.win.whole() || !op.rows.valid() || !op.rows.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+    DeviceLayout b;
+    if (!op.mem.contiguous()) {  // as the engine: destination rows or pages, never with a window, co-aligned in wide bytes
+      if (!op.win.whole() || !op.mem.valid(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
-    }
-    SourcePages pb;
-    if (op.pages.paged()) {  // as the engine: destination pages, never with rows or a window, co-aligned in wide bytes
-      if (op.rows.strided() || !op.win.whole() || !op.pages.valid(op.n_elems) || !op.pages.to_wide_bytes(eb, &pb))
-        return ErrorCode::INVALID_ARGUMENT;
-      if (!pb.coaligned(eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
     }
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
@@ -1939,19 +1859,18 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
     }
     if (ec != ErrorCode::OK) return ec;
     auto* dst = static_cast<uint8_t*>(op.wide);
-    if (op.win.whole() && !op.rows.strided() && !op.pages.paged()) {
+    if (op.win.whole() && op.mem.contiguous()) {
       mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, dst);
       continue;
     }
     std::vector<uint8_t> wide(eb * op.n_elems);
     mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, wide.data());
-    if (op.pages.paged()) {  // as the kernel's paged scattering store: the unpacked object into its pages
-      pb.for_each_run(wide.size(), [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(reinterpret_cast<void*>(at), wide.data() + x, n); });
+    if (!op.mem.contiguous()) {  // as the kernel's scattering store: the unpacked object into its rows or pages
+      copy_to_device(dst, b, wide.data(), wide.size(), nullptr);
       continue;
     }
-    auto store = [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + eb * at, wide.data() + eb * x, eb * n); };
-    if (op.rows.strided()) op.rows.for_each_run(op.n_elems, store);  // as the kernel's scattering store: into the rows
-    else op.win.for_each_run(op.n_elems, store);  // as the kernel does: the whole object read and verified, only the window stored
+    // as the kernel does: the whole object read and verified, only the window stored
+    op.win.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + eb * at, wide.data() + eb * x, eb * n); });
   }
   return ErrorCode::OK;
 }

@@ -56,25 +56,18 @@ struct DeviceShardOp {
   size_t copy = 0, shard = 0;
   const ShardPlacement* placement = nullptr;
   std::vector<const ShardPlacement*> replicas;  // same shard on the other copies (put fan-out)
-  uint64_t obj_offset = 0;    // byte offset of this shard inside the object
   // Get: the shard bytes that are stored (common/store_window.h); the whole shard is still read and verified.  An op whose
   // window covers the shard, the default included, is a whole-shard op.
   StoreWindow win;
-  // The base `win` goes with, given the object's: dev_ptrs[item] is where object byte 0 lands, or for a strided get where
-  // the result's row 0 lands.
-  void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(obj_offset); }
-  // Where the shard's bytes sit in the caller's strided memory (common/store_window.h): a put's source rows, or a get's
-  // destination rows (a get into a sliced tensor), the object's rows rebased to obj_offset; rows_at is where the shard's
-  // pattern row 0 starts relative to dev_ptrs[item].  The default is contiguous memory.  A get op never has both a
-  // pattern and a window.
-  SourceRows rows;
-  uint64_t rows_at = 0;
-  // A put's source pages or a get's destination pages (common/store_window.h), the object's table rebased to obj_offset;
-  // dev_ptrs[item] is not used then.  Never together with rows or a window.
-  SourcePages pages;
-  const void* src(const void* obj_base) const {
-    return static_cast<const uint8_t*>(obj_base) + (rows.strided() ? rows_at : obj_offset);
-  }
+  // Where the shard's bytes sit in the caller's memory (common/store_window.h): a put's source or a get's destination,
+  // the object's layout rebased to the shard's first byte, with its base mem_at bytes from dev_ptrs[item].  Never
+  // together with a window unless contiguous.
+  DeviceLayout mem;
+  uint64_t mem_at = 0;
+  // The base of `mem` given the object's; a get's also the base `win` goes with (a strided window's base is where the
+  // result's row 0 lands, which does not move with the shard).
+  const void* src(const void* obj_base) const { return static_cast<const uint8_t*>(obj_base) + mem_at; }
+  void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(mem_at); }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
@@ -86,15 +79,11 @@ struct DeviceFp8Op {
   // Get: the elements that are stored (common/store_window.h); the whole packed object is still read and verified.  The
   // default is the whole object.
   StoreWindow win;
-  // The wide side's rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts: a put's source
-  // rows, or a get's destination rows (never together with a window).  The packed object is one shard, so the pattern is
-  // the object's own.  The default is contiguous memory.
-  SourceRows rows;
+  // The wide side's layout in elements (common/store_window.h) at `wide`: a put's source or a get's destination, never
+  // together with a window unless contiguous.  The packed object is one shard, so the layout is the object's own.
+  DeviceLayout mem;
   // The element type of `wide`: bf16, fp16 or fp32 (common/mxfp8.h).  Ops of one call share its size (2 or 4 bytes).
   mxfp8::Wide wide_type = mxfp8::Wide::BF16;
-  // The wide side's pages, page and phase in elements (SourcePages in common/store_window.h): a put's source pages or a
-  // get's destination pages; `wide` is not used then.  Never together with rows or a window.
-  SourcePages pages;
 };
 
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
@@ -122,17 +111,14 @@ class DeviceTransport {
   // object; status[i] != 0 = digest mismatch on get.  Objects must satisfy fp8_eligible().
   virtual ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) { return ErrorCode::NOT_IMPLEMENTED; }
   virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
-  // Staging copies for objects (or shards) that live on host tiers: device <-> host buffer, synchronous.
-  virtual ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
-  // `rows` rows of `width` bytes, packed back to back at `host`, into row r = dev + r * pitch: one copy however many rows.
-  virtual ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) {
+  // Staging copies for objects (or shards) that live on host tiers, synchronous: object bytes [0, n) laid out by `layout`
+  // at `base` (common/store_window.h) from / to n bytes packed back to back at `host`.
+  virtual ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
     return ErrorCode::NOT_IMPLEMENTED;
   }
-  virtual ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
-  // Object bytes [0, n) of `pages` (common/store_window.h) from / to n bytes packed back to back at `host`: one copy per
-  // run of pages (SourcePages::for_each_run), synchronous.
-  virtual ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
-  virtual ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) { return ErrorCode::NOT_IMPLEMENTED; }
+  virtual ErrorCode copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void* stream) {
+    return ErrorCode::NOT_IMPLEMENTED;
+  }
 };
 
 class HostLoopbackTransport;
@@ -352,40 +338,33 @@ class BlackbirdClient {
   // Reads the object into dst[0, size) from the first copy that verifies: every shard, or with a window only those that
   // hold a byte it stores (whole, and verified).  The other bytes of dst are left as they are.
   ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, const StoreWindow& win = {});
-  // batch_get_device, batch_get_device_range, batch_get_device_strided and batch_get_device_scatter: `ranges` null = whole
-  // objects into buffers of `capacity`, else object i's rows into dev_ptrs[i] (capacity[i] = rows * length, for the chunk
-  // plan).  A range is the single row `rows == 1`.  `rows` (whole objects only) null = contiguous buffers, else object i
-  // lands in (*rows)[i], row 0 at dev_ptrs[i].
+  // batch_get_device, batch_get_device_range, batch_get_device_strided, batch_get_device_scatter and
+  // batch_get_device_paged: `ranges` null = whole objects into buffers of `capacity`, else object i's rows into dev_ptrs[i]
+  // (capacity[i] = rows * length, for the chunk plan).  A range is the single row `rows == 1`.  `mem` (whole objects
+  // only) null = contiguous buffers, else object i lands by (*mem)[i] at dev_ptrs[i].
   struct ByteRange {
     uint64_t offset = 0, length = 0;
     uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)
   };
-  // batch_put_device, batch_put_device_strided and batch_put_device_paged: `rows` null = contiguous sources, else object i
-  // is read by (*rows)[i]; `pages` non-null = object i is read from the pages (*pages)[i] wherever they are paged (dev_ptrs
-  // are then not read).
+  // batch_put_device, batch_put_device_strided and batch_put_device_paged: `mem` null = contiguous sources, else object i
+  // is read by (*mem)[i] at dev_ptrs[i].
   std::vector<ErrorCode> put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs, const std::vector<size_t>& sizes,
-                                    const std::vector<SourceRows>* rows, const WorkerConfig& cfg, void* stream,
-                                    const std::vector<SourcePages>* pages = nullptr);
-  // `pages` (whole objects only, never with `rows`) non-null = object i lands in the pages (*pages)[i] wherever they are
-  // paged.
+                                    const std::vector<DeviceLayout>* mem, const WorkerConfig& cfg, void* stream);
   std::vector<ErrorCode> get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs, const std::vector<size_t>& capacity,
-                                    const std::vector<ByteRange>* ranges, const std::vector<SourceRows>* rows, void* stream,
-                                    std::vector<size_t>* out_sizes, const std::vector<SourcePages>* pages = nullptr);
-  // batch_put_device_fp8, batch_put_device_fp8_strided and batch_put_device_fp8_paged: `rows` null = contiguous tensors,
-  // else object i is read by (*rows)[i], in elements; `pages` (never with `rows`) non-null = object i is read from the
-  // pages (*pages)[i], in elements (bf16_ptrs are then not read).
+                                    const std::vector<ByteRange>* ranges, const std::vector<DeviceLayout>* mem, void* stream,
+                                    std::vector<size_t>* out_sizes);
+  // batch_put_device_fp8, batch_put_device_fp8_strided and batch_put_device_fp8_paged: `mem` null = contiguous tensors,
+  // else object i is read by (*mem)[i] at bf16_ptrs[i], in elements.
   std::vector<ErrorCode> put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
-                                        const std::vector<uint64_t>& n_elems, const std::vector<SourceRows>* rows, const WorkerConfig& cfg,
-                                        void* stream, mxfp8::Wide wide, const std::vector<SourcePages>* pages = nullptr);
+                                        const std::vector<uint64_t>& n_elems, const std::vector<DeviceLayout>* mem, const WorkerConfig& cfg,
+                                        void* stream, mxfp8::Wide wide);
   // batch_get_device_fp8, batch_get_device_fp8_range, batch_get_device_fp8_strided, batch_get_device_fp8_scatter and
   // batch_get_device_fp8_paged: `ranges` null = whole tensors, else object i's rows (offset, length and pitch in elements)
-  // into bf16_ptrs[i]; `rows` (whole tensors only) null = contiguous destinations, else object i lands in (*rows)[i], in
-  // elements; `pages` (whole tensors only, never with `rows`) non-null = object i, which must hold exactly n_elems[i]
-  // elements, lands in the pages (*pages)[i], in elements.
+  // into bf16_ptrs[i]; `mem` (whole tensors only) null = contiguous destinations, else object i lands by (*mem)[i] at
+  // bf16_ptrs[i], in elements.  An object laid out in pages must hold exactly n_elems[i] elements.
   std::vector<ErrorCode> get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                         const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
-                                        const std::vector<SourceRows>* rows, void* stream, mxfp8::Wide wide,
-                                        const std::vector<SourcePages>* pages = nullptr);
+                                        const std::vector<DeviceLayout>* mem, void* stream, mxfp8::Wide wide);
   // The shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
   template <class Shape, class Run>
   std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);
@@ -439,27 +418,15 @@ class HostLoopbackTransport : public DeviceTransport {
   ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
   bool can_reach(const ShardPlacement& s) const override;
   uint64_t launches() const override { return launches_; }
-  ErrorCode copy_h2d(void* dev, const void* host, size_t n, void*) override {
-    std::memcpy(dev, host, n);
-    return ErrorCode::OK;
-  }
-  ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void*) override {
-    for (size_t r = 0; r < rows; ++r) std::memcpy(static_cast<uint8_t*>(dev) + r * pitch, static_cast<const uint8_t*>(host) + r * width, width);
-    return ErrorCode::OK;
-  }
-  ErrorCode copy_d2h(void* host, const void* dev, size_t n, void*) override {
-    std::memcpy(host, dev, n);
-    return ErrorCode::OK;
-  }
-  ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void*) override {
-    pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
-      std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(at), len);
+  ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void*) override {
+    layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+      std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(addr), len);
     });
     return ErrorCode::OK;
   }
-  ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void*) override {
-    pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
-      std::memcpy(reinterpret_cast<void*>(at), static_cast<const uint8_t*>(host) + x, len);
+  ErrorCode copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void*) override {
+    layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+      std::memcpy(reinterpret_cast<void*>(addr), static_cast<const uint8_t*>(host) + x, len);
     });
     return ErrorCode::OK;
   }

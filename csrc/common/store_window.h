@@ -12,7 +12,8 @@
 // The default window, [0, UINT64_MAX) without a pattern, is the whole object.
 //
 // SourceRows, below, maps a dense object onto strided memory instead: where a put reads each byte from, or where a get into
-// a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses.
+// a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses.  DeviceLayout, at the end, is
+// the one type the other layers hold for either of them.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -335,6 +336,92 @@ struct SourcePages {
     }
     if (run_n) f(run_x, run_at, run_n);
   }
+};
+
+// DeviceLayout: where the caller's units of one object sit on the device side of a transfer, relative to a base address:
+// contiguous (unit x at base + x, the default), in rows (SourceRows, with row 0 at the base) or in pages (SourcePages,
+// whose addresses are absolute: the base is not used).  It is the source of a put and the destination of a get, in bytes,
+// or for an MXFP8 transfer in elements of the wide side until to_wide_bytes().  This is the one place that knows the three
+// kinds; the transfer engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the
+// transports all hold one of these.  A StoreWindow only ever goes with a contiguous layout.
+class DeviceLayout {
+ public:
+  enum Kind { CONTIGUOUS, ROWS, PAGES };
+
+  DeviceLayout() = default;
+  // Rows without a pattern, and a table without pages, are contiguous.
+  explicit DeviceLayout(const SourceRows& r) : kind_(r.strided() ? ROWS : CONTIGUOUS), rows_(r) {}
+  explicit DeviceLayout(const SourcePages& p) : kind_(p.paged() ? PAGES : CONTIGUOUS), pages_(p) {}
+
+  // The layouts of SourceRows::from_rows and SourcePages::from_pages, with their object size and error rules.
+  static ErrorCode from_rows(uint64_t width, uint64_t pitch, uint64_t rows, DeviceLayout* out, uint64_t* size, uint64_t* extent) {
+    SourceRows r;
+    const ErrorCode ec = SourceRows::from_rows(width, pitch, rows, &r, size, extent);
+    *out = DeviceLayout(r);
+    return ec;
+  }
+  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, DeviceLayout* out, uint64_t* size) {
+    SourcePages p;
+    const ErrorCode ec = SourcePages::from_pages(npages, page, addrs, &p, size);
+    *out = DeviceLayout(p);
+    return ec;
+  }
+
+  Kind kind() const { return kind_; }
+  bool contiguous() const { return kind_ == CONTIGUOUS; }
+  const SourceRows& rows() const { return rows_; }     // the pattern of a ROWS layout
+  const SourcePages& pages() const { return pages_; }  // the table of a PAGES layout
+
+  // The INVALID_ARGUMENT rules against an object of len units: a valid pattern, or a table that holds every page.
+  bool valid(uint64_t len) const {
+    return kind_ == ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : true;
+  }
+
+  // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
+  // when the byte arithmetic could overflow.
+  bool to_wide_bytes(uint64_t b, DeviceLayout* out) const {
+    *out = *this;
+    return kind_ == ROWS ? rows_.to_wide_bytes(b, &out->rows_) : kind_ == PAGES ? pages_.to_wide_bytes(b, &out->pages_) : true;
+  }
+
+  // The layout seen from object unit `off`: unit x of the result is unit off + x here, relative to a base that has moved
+  // by *shift (off when contiguous, to where the new pattern's row 0 starts for rows, 0 for pages).
+  DeviceLayout rebase(uint64_t off, uint64_t* shift) const {
+    DeviceLayout l = *this;
+    *shift = off;
+    if (kind_ == ROWS) l.rows_ = rows_.rebase(off, shift);
+    if (kind_ == PAGES) l.pages_ = pages_.rebase(off), *shift = 0;
+    return l;
+  }
+
+  // Whether object bytes [0, len) at `base` are co-aligned with the tiles, so that the kernels only move 16-byte congruent
+  // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned or SourcePages::coaligned.
+  bool coaligned(uintptr_t base, uint64_t len) const {
+    return kind_ == ROWS ? rows_.coaligned(base, len) : kind_ == PAGES ? pages_.coaligned(len) : base % 16 == 0;
+  }
+
+  // The client's rule for whether a device get into this layout at `base` may take the fused path as far as the shard
+  // [off, off + len) of a copy goes: a contiguous get by its store window (StoreWindow::fused_get_aligned; the default is
+  // the whole object), rows and pages by SourceRows::fused_get_aligned and SourcePages::fused_get_aligned.
+  bool fused_get_aligned(uintptr_t base, uint64_t off, uint64_t len, const StoreWindow& win = {}) const {
+    if (kind_ == ROWS) return rows_.fused_get_aligned(base, off, len);
+    if (kind_ == PAGES) return pages_.fused_get_aligned(off, len);
+    return win.fused_get_aligned(base, off, len);
+  }
+
+  // Calls f(x, addr, n) for every run of n contiguous bytes of object bytes [0, len) at `base`: object bytes [x, x + n)
+  // live at [addr, addr + n), in order.
+  template <class F>
+  void for_each_run(uintptr_t base, uint64_t len, F&& f) const {
+    if (kind_ == ROWS) rows_.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { f(x, base + at, n); });
+    else if (kind_ == PAGES) pages_.for_each_run(len, f);
+    else if (len) f(uint64_t{0}, static_cast<uint64_t>(base), len);
+  }
+
+ private:
+  Kind kind_ = CONTIGUOUS;
+  SourceRows rows_;
+  SourcePages pages_;
 };
 
 }  // namespace bb

@@ -506,53 +506,47 @@ Result<void*> GpuFabric::resolve(const ShardPlacement& s) {
   return ErrorCode::MEMORY_POOL_NOT_FOUND;
 }
 
-ErrorCode GpuFabric::copy_h2d(void* dev, const void* host, size_t n, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice") || !cuda_ok(cudaMemcpyAsync(dev, host, n, cudaMemcpyHostToDevice, st), "H2D") ||
-      !cuda_ok(cudaStreamSynchronize(st), "sync"))
-    return ErrorCode::FABRIC_ERROR;
-  return ErrorCode::OK;
-}
-
-ErrorCode GpuFabric::copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) {
-  if (rows == 0 || width == 0) return ErrorCode::OK;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice") ||
-      !cuda_ok(cudaMemcpy2DAsync(dev, pitch, host, width, width, rows, cudaMemcpyHostToDevice, st), "H2D rows") ||
-      !cuda_ok(cudaStreamSynchronize(st), "sync"))
-    return ErrorCode::FABRIC_ERROR;
-  return ErrorCode::OK;
-}
-
-ErrorCode GpuFabric::copy_d2h(void* host, const void* dev, size_t n, void* stream) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice") || !cuda_ok(cudaMemcpyAsync(host, dev, n, cudaMemcpyDeviceToHost, st), "D2H") ||
-      !cuda_ok(cudaStreamSynchronize(st), "sync"))
-    return ErrorCode::FABRIC_ERROR;
-  return ErrorCode::OK;
-}
-
-// One async copy per run of pages, then one synchronise.
-ErrorCode GpuFabric::copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) {
+ErrorCode GpuFabric::copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
+  if (!layout.valid(n)) return ErrorCode::INVALID_ARGUMENT;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
+  const bool rows = layout.kind() == DeviceLayout::ROWS;
+  std::vector<uint8_t> extent(rows ? layout.rows().extent(n) : 0);
   bool ok = true;
-  pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
-    ok = ok && cuda_ok(cudaMemcpyAsync(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(at), len, cudaMemcpyDeviceToHost, st),
-                       "D2H pages");
+  auto d2h = [&](void* dst, const void* src, size_t len) { ok = ok && cuda_ok(cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, st), "D2H"); };
+  if (rows) d2h(extent.data(), base, extent.size());
+  else layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+    d2h(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(addr), len);
   });
   if (!cuda_ok(cudaStreamSynchronize(st), "sync") || !ok) return ErrorCode::FABRIC_ERROR;
+  if (rows)  // compact the rows here
+    layout.for_each_run(reinterpret_cast<uintptr_t>(extent.data()), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+      std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(addr), len);
+    });
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) {
+ErrorCode GpuFabric::copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void* stream) {
+  if (!layout.valid(n)) return ErrorCode::INVALID_ARGUMENT;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
+  const auto* h = static_cast<const uint8_t*>(host);
   bool ok = true;
-  pages.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t len) {
-    ok = ok && cuda_ok(cudaMemcpyAsync(reinterpret_cast<void*>(at), static_cast<const uint8_t*>(host) + x, len, cudaMemcpyHostToDevice, st),
-                       "H2D pages");
-  });
+  auto h2d = [&](void* dst, const void* src, size_t len) { ok = ok && cuda_ok(cudaMemcpyAsync(dst, src, len, cudaMemcpyHostToDevice, st), "H2D"); };
+  if (layout.kind() == DeviceLayout::ROWS) {  // the first row from the phase, one 2-D copy of the whole rows, the last row's part
+    const SourceRows& r = layout.rows();
+    auto* d = static_cast<uint8_t*>(base);
+    uint64_t x = r.phase ? std::min<uint64_t>(n, r.width - r.phase) : 0;
+    if (x) h2d(d + r.phase, h, x), d += r.pitch;
+    const uint64_t full = (n - x) / r.width;
+    if (full) ok = ok && cuda_ok(cudaMemcpy2DAsync(d, r.pitch, h + x, r.width, r.width, full, cudaMemcpyHostToDevice, st), "H2D rows");
+    x += full * r.width, d += full * r.pitch;
+    if (x < n) h2d(d, h + x, n - x);
+  } else {
+    layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+      h2d(reinterpret_cast<void*>(addr), h + x, len);
+    });
+  }
   if (!cuda_ok(cudaStreamSynchronize(st), "sync") || !ok) return ErrorCode::FABRIC_ERROR;
   return ErrorCode::OK;
 }
@@ -565,14 +559,9 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
     XferItem it;
     it.src = op.src(dev_ptrs[op.item]);
     it.nbytes = op.placement->length;
-    if (op.rows.strided()) {  // a gathered put: every pass and the multicast item read the same rows
-      it.rows = op.rows;
+    if (!op.mem.contiguous()) {  // a gathered put: every pass and the multicast item read the same rows or pages
+      it.mem = op.mem;
       it.flags |= XFER_GATHER;
-    }
-    if (op.pages.paged()) {  // a paged put: the same, from the shard's pages
-      it.src = nullptr;
-      it.pages = op.pages;
-      it.flags |= XFER_GATHER | XFER_PAGED;
     }
     // NVLS: the replica set is one whole multicast group at one offset -> a single multimem.st stream
     if (arena_ && !op.replicas.empty() && (it.nbytes & 15) == 0) {
@@ -615,9 +604,8 @@ ErrorCode GpuFabric::build_put_items(const std::vector<client::DeviceShardOp>& o
       XferItem more;
       more.src = it.src;
       more.nbytes = it.nbytes;
-      more.rows = it.rows;
-      more.pages = it.pages;
-      more.flags = it.flags & (XFER_GATHER | XFER_PAGED);
+      more.mem = it.mem;
+      more.flags = it.flags & XFER_GATHER;
       more.ndst = 0;
       for (; r < op.replicas.size() && more.ndst < kMaxDst; ++r) {
         auto d = resolve(*op.replicas[r]);
@@ -684,8 +672,7 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     it.n_elems = op.n_elems;
     it.wide_type = op.wide_type;
     it.win = op.win;  // a window on a put is refused by the engine
-    if (unpack) it.dst_rows = op.rows, it.dst_pages = op.pages;  // rows and pages are the destination's on a get,
-    else it.rows = op.rows, it.pages = op.pages;                 // the source's on a put
+    it.mem = op.mem;
     if (unpack) {  // get: read the chosen copy and verify it against the digest recorded at put time
       it.expect = op.placement->checksum;
       it.verify = true;
@@ -733,26 +720,19 @@ ErrorCode GpuFabric::build_get_items(const std::vector<client::DeviceShardOp>& o
     if (!s.ok()) return s.error();
     XferItem it;
     it.src = s.value();
-    it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.obj_offset;
+    it.dst[0] = op.dst(dev_ptrs[op.item]);
     it.ndst = 1;
     it.nbytes = op.placement->length;
     it.expect = op.placement->checksum;
     it.flags = algo == ChecksumAlgo::NONE ? 0u : static_cast<uint32_t>(XFER_VERIFY);
     if (!op.win.covers(it.nbytes)) {  // whole-shard ops keep exactly the descriptors they always had
       it.flags |= op.win.strided() ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
-      it.dst[0] = op.dst(dev_ptrs[op.item]);
       it.win = op.win;
       it.win.hi = std::min(op.win.hi, it.nbytes);
     }
-    if (op.rows.strided()) {  // a get into a strided destination: the shard's rows start at rows_at
+    if (!op.mem.contiguous()) {  // a get into rows or pages: the shard's, rebased to its first byte
       it.flags |= XFER_SCATTER;
-      it.dst[0] = static_cast<uint8_t*>(dev_ptrs[op.item]) + op.rows_at;
-      it.dst_rows = op.rows;
-    }
-    if (op.pages.paged()) {  // a get into pages: the shard's table, rebased to its first byte
-      it.flags |= XFER_SCATTER | XFER_PAGED;
-      it.dst[0] = nullptr;
-      it.dst_pages = op.pages;
+      it.mem = op.mem;
     }
     items->push_back(it);
     op_of_item->push_back(k);

@@ -85,11 +85,10 @@ class GpuFabric : public client::DeviceTransport {
   bool fp8_eligible(uint64_t n_elems) const override { return XferEngine::fp8_eligible(n_elems); }
   ErrorCode put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override;
   ErrorCode get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override;
-  ErrorCode copy_h2d(void* dev, const void* host, size_t n, void* stream) override;
-  ErrorCode copy_h2d_rows(void* dev, size_t pitch, const void* host, size_t width, size_t rows, void* stream) override;
-  ErrorCode copy_d2h(void* host, const void* dev, size_t n, void* stream) override;
-  ErrorCode copy_d2h_pages(void* host, const SourcePages& pages, size_t n, void* stream) override;
-  ErrorCode copy_h2d_pages(const SourcePages& pages, const void* host, size_t n, void* stream) override;
+  // One async copy per call (rows: the extent from the device, compacted on the host, or one 2-D copy of the whole rows
+  // to it; pages: one per run of pages), then one synchronise.
+  ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) override;
+  ErrorCode copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void* stream) override;
 
   // Re-reads the pool registry from the keystone and maps any new GPU slab.
   ErrorCode refresh_pools();

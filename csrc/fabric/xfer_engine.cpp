@@ -87,7 +87,6 @@ struct XferEngine::Slot {
     strides[k] = e;
   }
   void set_stride(uint32_t k, const StoreWindow& w) { set_stride(k, XferStride{w.pitch, w.width, w.phase}); }
-  void set_stride(uint32_t k, const SourceRows& r) { set_stride(k, XferStride{r.pitch, r.width, r.phase}); }
   // Writes the stride table behind tile_start when the batch has a strided descriptor, and returns the bytes of the
   // table to copy to the device: [descs | tile_start | strides], or without the strides.
   size_t write_strides(uint32_t nd) {
@@ -100,10 +99,18 @@ struct XferEngine::Slot {
   // first entry here until write_pages() turns it into a device address.
   std::vector<uint64_t> pages;
   std::vector<uint32_t> paged_descs;
-  void add_pages(uint32_t k, const SourcePages& p, uint64_t nbytes) {
+  // The table entry of descriptor k's gathered or scattered layout (in bytes, over nbytes): its pattern, or its page
+  // entries.  Returns the XFER_PAGED flag for pages, 0 for rows.
+  uint32_t set_layout(uint32_t k, const DeviceLayout& m, uint64_t nbytes) {
+    if (m.kind() != DeviceLayout::PAGES) {
+      set_stride(k, XferStride{m.rows().pitch, m.rows().width, m.rows().phase});
+      return 0;
+    }
+    const SourcePages& p = m.pages();
     set_stride(k, XferStride{{pages.size()}, p.page, p.phase});
     paged_descs.push_back(k);
     pages.insert(pages.end(), p.addrs, p.addrs + p.pages_for(nbytes));
+    return XFER_PAGED;
   }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
@@ -373,21 +380,13 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const bool strided = it.flags & XFER_STRIDED;
     const bool gather = it.flags & XFER_GATHER;
     const bool scatter = it.flags & XFER_SCATTER;
-    const bool src_paged = it.pages.paged(), dst_paged = it.dst_pages.paged();
     if ((strided && !win) || (win && (strided != it.win.strided() || !it.win.valid(it.nbytes) || it.ndst != 1 ||
                                       (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
-    // pages are the gathering load's source or the scattering store's destination, instead of rows on the same side
-    if (static_cast<bool>(it.flags & XFER_PAGED) != (src_paged || dst_paged) || (src_paged && (dst_paged || it.rows.strided())) ||
-        (dst_paged && it.dst_rows.strided()) || (src_paged && !it.pages.valid(it.nbytes)) ||
-        (dst_paged && !it.dst_pages.valid(it.nbytes)))
-      return ErrorCode::INVALID_ARGUMENT;
-    if (gather != (it.rows.strided() || src_paged) ||
-        (gather && ((!src_paged && !it.rows.valid()) || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM)))))
-      return ErrorCode::INVALID_ARGUMENT;
-    if (scatter != (it.dst_rows.strided() || dst_paged) ||
-        (scatter && ((!dst_paged && !it.dst_rows.valid()) || it.ndst != 1 ||
-                     (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
+    // a layout is the gathering load's source or the scattering store's destination, the side its flag names
+    if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES) ||
+        !it.mem.valid(it.nbytes) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
+        (scatter && (it.ndst != 1 || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
@@ -401,12 +400,11 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     // kernel nor the mailbox has a store window, a gathering load or a scattering store
     all_small = all_small && nbytes <= kSmallBytes && !(it.flags & (XFER_RAW_SUM | XFER_WINDOW | XFER_GATHER | XFER_SCATTER)) && it.ndst >= 1;
     if (it.ndst > kMaxDst || (it.ndst == 0 && !(it.flags & XFER_RAW_SUM))) return ErrorCode::INVALID_ARGUMENT;
-    uintptr_t al = gather ? 0 : reinterpret_cast<uintptr_t>(it.src);  // gathered: source rows instead
-    // strided and scattered: rows instead
+    uintptr_t al = gather ? 0 : reinterpret_cast<uintptr_t>(it.src);  // gathered: the source layout instead
+    // strided: the window instead; scattered: the destination layout instead
     for (uint32_t r = strided || scatter ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
     if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]))) ||
-        (gather && !(src_paged ? it.pages.coaligned(it.nbytes) : it.rows.coaligned(reinterpret_cast<uintptr_t>(it.src), it.nbytes))) ||
-        (scatter && !(dst_paged ? it.dst_pages.coaligned(it.nbytes) : it.dst_rows.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]), it.nbytes))))
+        ((gather || scatter) && !it.mem.coaligned(reinterpret_cast<uintptr_t>(gather ? it.src : it.dst[0]), it.nbytes)))
       return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
@@ -419,14 +417,11 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       d.win.hi = w.hi;
       if (strided) s->set_stride(nd, w);
     }
-    if (src_paged) s->add_pages(nd, it.pages, nbytes);
-    else if (dst_paged) s->add_pages(nd, it.dst_pages, nbytes);
-    else if (gather) s->set_stride(nd, it.rows);
-    else if (scatter) s->set_stride(nd, it.dst_rows);
     d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;
     d.flags = it.flags;
+    if (gather || scatter) d.flags |= s->set_layout(nd, it.mem, nbytes);
     d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
     if (algo == ChecksumAlgo::CRC32C) {
       d.expect = (static_cast<uint64_t>(crc_init_term_for(nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
@@ -642,29 +637,16 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
-    const bool src_paged = it.pages.paged(), dst_paged = it.dst_pages.paged();
-    const bool gather = it.rows.strided() || src_paged;
-    const bool scatter = it.dst_rows.strided() || dst_paged;
+    const bool shaped = !it.mem.contiguous();
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
     if (it.wide_type != mxfp8::Wide::BF16 && it.wide_type != mxfp8::Wide::F16 && it.wide_type != mxfp8::Wide::F32)
       return ErrorCode::INVALID_ARGUMENT;
     if (mxfp8::wide_bytes(it.wide_type) != eb) return ErrorCode::INVALID_ARGUMENT;  // mixes 2- and 4-byte wide types
-    SourceRows rows;  // a gathered put's source rows, or a scattered get's destination rows, in wide bytes
-    if (gather && (unpack || !it.rows.valid() || !it.rows.to_wide_bytes(eb, &rows))) return ErrorCode::INVALID_ARGUMENT;
-    if (scatter && (!unpack || gather || !it.win.whole() || !it.dst_rows.valid() || !it.dst_rows.to_wide_bytes(eb, &rows)))
-      return ErrorCode::INVALID_ARGUMENT;
-    // pages replace the rows on their side: the source of a pack or the destination of an unpack, never with a window
-    const bool paged = src_paged || dst_paged;
-    const SourcePages& pg = src_paged ? it.pages : it.dst_pages;
-    SourcePages pages;  // the table in wide bytes
-    if (paged && ((src_paged && it.rows.strided()) || (dst_paged && it.dst_rows.strided()) || !it.win.whole() ||
-                  !pg.valid(it.n_elems) || !pg.to_wide_bytes(eb, &pages)))
-      return ErrorCode::INVALID_ARGUMENT;
-    // a strided item's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
-    // first element after row 0's start): the rows are checked instead, and a paged item's pages
-    if (((strided || gather || scatter ? 0 : reinterpret_cast<uintptr_t>(it.wide)) | reinterpret_cast<uintptr_t>(it.packed)) & 15 ||
-        ((gather || scatter) &&
-         !(paged ? pages.coaligned(eb * it.n_elems) : rows.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems))))
+    DeviceLayout mem;  // a gathered put's source, or a scattered get's destination, in wide bytes; never with a window
+    if (shaped && (!it.win.whole() || !it.mem.valid(it.n_elems) || !it.mem.to_wide_bytes(eb, &mem))) return ErrorCode::INVALID_ARGUMENT;
+    // a strided window's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
+    // first element after row 0's start): the window is checked instead, below
+    if ((reinterpret_cast<uintptr_t>(it.packed) & 15) || (!strided && !mem.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
       return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
@@ -696,15 +678,8 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       d.flags |= XFER_STRIDED;
       s->set_stride(i, w);
     }
-    if (gather || scatter) {  // d.src (gather) or d.dst[0] (scatter) is the pattern's row 0, or not read when paged
-      d.flags |= gather ? XFER_GATHER : XFER_SCATTER;
-      if (paged) {
-        d.flags |= XFER_PAGED;
-        s->add_pages(i, pages, eb * it.n_elems);
-      } else {
-        s->set_stride(i, rows);
-      }
-    }
+    if (shaped)  // d.src (gather) or d.dst[0] (scatter) is the layout's base
+      d.flags |= (unpack ? XFER_SCATTER : XFER_GATHER) | s->set_layout(i, mem, eb * it.n_elems);
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
     const uint64_t nt_full = it.n_elems / kTileBytes;

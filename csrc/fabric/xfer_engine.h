@@ -31,24 +31,14 @@ struct XferItem {
   // win.coaligned(dst[0]).  The whole object is still read and hashed, except with ChecksumAlgo::NONE, where the engine
   // reads only the 16-byte aligned span of the window (see window_read_bytes).
   StoreWindow win;
-  // Put of a strided source (common/store_window.h): src is where the pattern's row 0 starts; XFER_GATHER exactly when it
-  // has a pattern.  INVALID_ARGUMENT for an invalid pattern, or one with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM;
-  // INVALID_ADDRESS unless rows.coaligned(src, nbytes), which replaces the 16-byte alignment check of src.
-  SourceRows rows;
-  // Get into a strided destination, the same rule on the other side: dst[0] is where the pattern's row 0 starts;
-  // XFER_SCATTER exactly when it has a pattern.  INVALID_ARGUMENT for an invalid pattern, or one with XFER_WINDOW,
-  // XFER_STRIDED, XFER_GATHER, XFER_MULTIMEM, XFER_RAW_SUM or ndst != 1; INVALID_ADDRESS unless
-  // dst_rows.coaligned(dst[0], nbytes), which replaces the 16-byte alignment check of dst[0].
-  SourceRows dst_rows;
-  // Paged put source (with XFER_GATHER) or paged get destination (with XFER_SCATTER), XFER_PAGED exactly when one of them
-  // is set (common/store_window.h): object byte x at addrs[(x + phase) / page] + (x + phase) % page; src, or dst[0], is
-  // not read.  The page entries are copied into the batch's device table by submit(), so the host array need only live
-  // until submit() returns.  INVALID_ARGUMENT for both at once, a table too short for nbytes or phase >= page, pages
-  // together with a SourceRows pattern on the same side, or XFER_PAGED without its XFER_GATHER / XFER_SCATTER, with
-  // XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM; the destination rules are those of rows / dst_rows.  INVALID_ADDRESS
-  // unless the pages are coaligned(nbytes).
-  SourcePages pages;
-  SourcePages dst_pages;
+  // Rows or pages (common/store_window.h) on one side of the transfer, which its flag names: a put's source with
+  // XFER_GATHER (src is the layout's base), or a get's destination with XFER_SCATTER (dst[0] is).  A page table's base is
+  // not read, and its entries are copied into the batch's device table by submit(), so the host array need only live
+  // until submit() returns; submit() sets XFER_PAGED for it.  INVALID_ARGUMENT for a side flag without a layout or a
+  // layout without one, XFER_PAGED without pages, !mem.valid(nbytes), XFER_GATHER with XFER_WINDOW, XFER_STRIDED or
+  // XFER_RAW_SUM, and XFER_SCATTER with those, XFER_GATHER, XFER_MULTIMEM or ndst != 1.  INVALID_ADDRESS unless
+  // mem.coaligned(base, nbytes), which replaces the 16-byte alignment check of the base.
+  DeviceLayout mem;
 };
 
 // Bytes the kernel reads for `it` under `algo`: nbytes, or for a windowed item without a checksum the trimmed span
@@ -76,27 +66,14 @@ struct Fp8Item {
   // the whole object.  The whole packed object is still read and verified.  INVALID_ARGUMENT unless valid against
   // n_elems; INVALID_ADDRESS unless a strided window is co-aligned in bf16 bytes, as XferItem's.
   StoreWindow win;
-  // Put only: the source rows in elements (common/store_window.h), `wide` being where the pattern's row 0 starts; the
-  // default is a contiguous source.  run_fp8 sets XFER_GATHER exactly when it has a pattern.  INVALID_ARGUMENT for a
-  // pattern on an unpack, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned
-  // in bf16 bytes, which replaces the 16-byte alignment check of `wide`.
-  SourceRows rows;
-  // Unpack only: the destination rows in elements, `wide` being where the pattern's row 0 starts; the default is a
-  // contiguous destination.  run_fp8 sets XFER_SCATTER exactly when it has a pattern.  INVALID_ARGUMENT for a pattern on a
-  // pack, with a window, an invalid one, or one whose bf16 byte count overflows; INVALID_ADDRESS unless it is co-aligned in
-  // bf16 bytes, which replaces the 16-byte alignment check of `wide`.
-  SourceRows dst_rows;
-  // Paged source (pack only, `pages`) or paged destination (unpack only, `dst_pages`), page and phase in elements, the
-  // addresses in bytes (SourcePages in common/store_window.h): element x at addrs[(x + phase) / page] + b * ((x + phase)
-  // % page) for b-byte elements; `wide` is not read.  run_fp8 sets XFER_GATHER | XFER_PAGED or XFER_SCATTER | XFER_PAGED
-  // exactly when one is set, and copies the page entries into the batch's device table, so the host array need only live
-  // until run_fp8 returns.  An MX block may straddle two pages.  INVALID_ARGUMENT for source pages on an unpack,
-  // destination pages on a pack, pages together with rows or a window, a table too short for n_elems, phase >= page, or a
-  // page whose wide-byte size overflows; INVALID_ADDRESS unless the table is co-aligned in wide bytes
-  // (SourcePages::coaligned of b * n_elems: addrs[k] + b * phase 16-byte aligned, and b * page % 16 == 0 for more than
-  // one page), which replaces the 16-byte alignment check of `wide`.
-  SourcePages pages;
-  SourcePages dst_pages;
+  // The wide side's rows or pages in elements, the page addresses in bytes (common/store_window.h), `wide` being the
+  // layout's base (not read for pages): a pack's source or an unpack's destination.  The default is contiguous.  run_fp8
+  // sets XFER_GATHER or XFER_SCATTER for it, with XFER_PAGED for pages whose entries it copies into the batch's device
+  // table, so the host array need only live until run_fp8 returns.  An MX block may straddle two pages.
+  // INVALID_ARGUMENT with a window, unless mem.valid(n_elems), or when its wide-byte arithmetic overflows;
+  // INVALID_ADDRESS unless it is co-aligned in wide bytes (DeviceLayout::coaligned of b * n_elems), which replaces the
+  // 16-byte alignment check of `wide`.
+  DeviceLayout mem;
 };
 
 struct XferResult {

@@ -46,25 +46,35 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
-// A gather or scatter pattern (common/store_window.h) given as (pitch, width, phase).
-SourceRows to_rows(const py::handle& h) {
-  auto g = h.cast<std::vector<uint64_t>>();
-  if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
-  return {g[0], g[1], g[2]};
-}
-// A page table (common/store_window.h) given as (addrs, page, phase); the addresses are kept in `keep` until the batch
-// has been submitted.
-SourcePages to_pages(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
-  auto t = py::cast<py::tuple>(h);
-  if (t.size() != 3) throw py::value_error("pages = (addrs, page, phase)");
-  keep.push_back(t[0].cast<std::vector<uint64_t>>());
-  return {keep.back().data(), keep.back().size(), t[1].cast<uint64_t>(), t[2].cast<uint64_t>()};
+// The layout slots of an item tuple (common/store_window.h), first to last: gather rows, scatter rows, source pages and
+// destination pages.  Rows are given as (pitch, width, phase), pages as (addrs, page, phase), whose addresses are kept in
+// `keep` until the batch has been submitted.  Returns the slot set, -1 for none; an item takes one layout, so a second
+// slot is the engine's INVALID_ARGUMENT, raised as `what`.
+int to_layout(const py::tuple& t, const size_t (&slots)[4], std::deque<std::vector<uint64_t>>& keep, DeviceLayout* out, const char* what) {
+  int set = -1;
+  for (int k = 0; k < 4; ++k) {
+    if (t.size() <= slots[k] || t[slots[k]].is_none()) continue;
+    if (set >= 0) check(ErrorCode::INVALID_ARGUMENT, what);
+    set = k;
+    if (k < 2) {
+      auto g = t[slots[k]].cast<std::vector<uint64_t>>();
+      if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
+      *out = DeviceLayout(SourceRows{g[0], g[1], g[2]});
+    } else {
+      auto p = py::cast<py::tuple>(t[slots[k]]);
+      if (p.size() != 3) throw py::value_error("pages = (addrs, page, phase)");
+      keep.push_back(p[0].cast<std::vector<uint64_t>>());
+      *out = DeviceLayout(SourcePages{keep.back().data(), keep.back().size(), p[1].cast<uint64_t>(), p[2].cast<uint64_t>()});
+    }
+  }
+  return set;
 }
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None,
-// src_pages=None, dst_pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
+// source pages=None, destination pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
 // it without that flag).  A window sets XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern
 // (pitch, width, phase) sets XFER_GATHER, with src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.  Source
-// pages (addrs, page, phase) set XFER_GATHER | XFER_PAGED, destination pages XFER_SCATTER | XFER_PAGED.
+// pages (addrs, page, phase) set XFER_GATHER | XFER_PAGED, destination pages XFER_SCATTER | XFER_PAGED.  At most one of
+// the four.
 XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   py::tuple t = py::cast<py::tuple>(h);
   if (t.size() < 3 || t.size() > 11)
@@ -79,22 +89,9 @@ XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
-  if (t.size() > 7 && !t[7].is_none()) {
-    it.rows = to_rows(t[7]);
-    it.flags |= XFER_GATHER;
-  }
-  if (t.size() > 8 && !t[8].is_none()) {
-    it.dst_rows = to_rows(t[8]);
-    it.flags |= XFER_SCATTER;
-  }
-  if (t.size() > 9 && !t[9].is_none()) {
-    it.pages = to_pages(t[9], keep);
-    it.flags |= XFER_GATHER | XFER_PAGED;
-  }
-  if (t.size() > 10 && !t[10].is_none()) {
-    it.dst_pages = to_pages(t[10], keep);
-    it.flags |= XFER_SCATTER | XFER_PAGED;
-  }
+  static const uint32_t side[4] = {XFER_GATHER, XFER_SCATTER, XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED};
+  const int k = to_layout(t, {7, 8, 9, 10}, keep, &it.mem, "XferEngine.submit");
+  if (k >= 0) it.flags |= side[k];
   return it;
 }
 }  // namespace
@@ -173,11 +170,10 @@ void bind_gpu(py::module_& m) {
                      "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
-               if (t.size() > 5 && !t[5].is_none()) it.rows = to_rows(t[5]);
-               if (t.size() > 6 && !t[6].is_none()) it.dst_rows = to_rows(t[6]);
                if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
-               if (t.size() > 8 && !t[8].is_none()) it.pages = to_pages(t[8], keep);
-               if (t.size() > 9 && !t[9].is_none()) it.dst_pages = to_pages(t[9], keep);
+               // the gather slots are a pack's, the scatter slots an unpack's
+               const int k = to_layout(t, {5, 6, 8, 9}, keep, &it.mem, "XferEngine.run_fp8");
+               if (k >= 0 && (k % 2 == 1) != unpack) check(ErrorCode::INVALID_ARGUMENT, "XferEngine.run_fp8");
                v.push_back(it);
              }
              XferResult res;
