@@ -47,6 +47,29 @@ def _by_dtype(idx, dtype_of) -> dict:
     return groups
 
 
+def _check(what: str, keys, ecs, fallback: bool = False) -> None:
+    """RuntimeError naming the first items whose code is not OK; with `fallback`, NOT_IMPLEMENTED is no error either
+    (the packed calls refuse with it what a fallback route then takes)."""
+    bad = [(k, e) for k, e in zip(keys, ecs) if e != _bb.ErrorCode.OK and not (fallback and e == _bb.ErrorCode.NOT_IMPLEMENTED)]
+    if bad:
+        raise RuntimeError(f"{what} failed: {bad[:3]}")
+
+
+def _meta(dtype: torch.dtype, shape, packed: bool) -> bytes:
+    """The `#meta` record of a tensor; a packed one also records its element count padded to whole 32-element MX blocks."""
+    n = torch.Size(shape).numel()
+    meta = {"dtype": str(dtype).replace("torch.", ""), "shape": list(shape), "packed": "mxfp8" if packed else None, "numel": n}
+    if packed:
+        meta["padded_numel"] = (n + 31) // 32 * 32
+    return json.dumps(meta).encode()
+
+
+def _elem_rows(es: int, rows, n: int):
+    """(width, pitch, rows) in elements of `es` bytes: byte rows (see TensorStore._source_rows), or n contiguous elements
+    as one row when rows is None."""
+    return (rows[0] // es, rows[1] // es, rows[2]) if rows is not None else (n, n, 1)
+
+
 class TensorStore:
     def __init__(self, client, config: Optional["_bb.WorkerConfig"] = None):
         self.client = client
@@ -60,6 +83,33 @@ class TensorStore:
     def _meta_cfg(self):
         return _bb.WorkerConfig(replication_factor=self.config.replication_factor, max_workers_per_copy=1, ttl_ms=self.config.ttl_ms,
                                 enable_soft_pin=self.config.enable_soft_pin, checksum=_bb.ChecksumAlgo.CRC32C)
+
+    def _put_metas(self, keys: list, metas: list) -> None:
+        ecs = self.client.batch_put([k + "#meta" for k in keys], metas, self._meta_cfg())
+        if any(e != _bb.ErrorCode.OK for e in ecs):
+            raise RuntimeError("meta put failed")
+
+    def _packed(self, what: str, keys: list, idx: list, dtype_of, call) -> list:
+        """One native call per dtype for the packed items idx: call(group, element size, wide) returns the group's error
+        codes.  RuntimeError for a code other than OK or NOT_IMPLEMENTED; returns the items refused with NOT_IMPLEMENTED,
+        in call order, for the caller's fallback."""
+        refused = []
+        for dt, grp in _by_dtype(idx, dtype_of).items():
+            ecs = call(grp, dt.itemsize, _MX_WIDE[dt])
+            _check(what, [keys[i] for i in grp], ecs, fallback=True)
+            refused += [i for i, e in zip(grp, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
+        return refused
+
+    def _whole(self, keys: list, idx: list, device, fn) -> None:
+        """fn(i, t) for each item of idx with its whole stored tensor t from batch_get: the route of the items no device
+        call above took."""
+        if idx:
+            for i, t in zip(idx, self.batch_get([keys[i] for i in idx], device)):
+                fn(i, t)
+
+    def _fp8_whole(self, m) -> bool:
+        """A packed object the fused unpack reads: unpadded, a whole number of 32-element MX blocks."""
+        return m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"] and self.client.device_fp8_eligible(m["numel"])
 
     # ------------------------------------------------------------------ put
     @staticmethod
@@ -121,48 +171,34 @@ class TensorStore:
         if pack_fp8:  # only slices the fused pack kernel can take are gathered
             rows = [r if r is not None and self._fused_fp8_ok(t, cfg) else None for t, r in zip(tensors, rows)]
         tensors = [t if r is not None else t.contiguous() for t, r in zip(tensors, rows)]
-        if pack_fp8:
-            # objects the fused kernel can take go through batch_put_device_fp8 (bf16 read once, packed bytes on the
-            # wire, digest of the packed object from the tensor cores); the rest are packed first (unfused path below)
-            fused_all = [i for i, t in enumerate(tensors) if t.is_cuda and self._fused_fp8_ok(t, cfg)]
-            done = []
-            for dt, fused in _by_dtype(fused_all, lambda i: tensors[i].dtype).items():
-                fk = [keys[i] for i in fused]
-                ptrs = [tensors[i].data_ptr() for i in fused]
-                es, wide = tensors[fused[0]].element_size(), _MX_WIDE[dt]
-                if any(rows[i] is not None for i in fused):
-                    # one call and one launch: contiguous tensors go as one row each; widths and pitches in elements
-                    shapes = [(rows[i][0] // es, rows[i][1] // es, rows[i][2]) if rows[i] is not None else (tensors[i].numel(),) * 2 + (1,)
-                              for i in fused]
-                    ecs = self.client.batch_put_device_fp8_strided(fk, ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
-                                                                   [s[2] for s in shapes], cfg, self._stream(), wide=wide)
-                else:
-                    ecs = self.client.batch_put_device_fp8(fk, ptrs, [tensors[i].numel() for i in fused], cfg, self._stream(), wide=wide)
-                done += [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.OK]
-                bad = [(keys[i], e) for i, e in zip(fused, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
-                if bad:
-                    raise RuntimeError(f"fused fp8 put failed: {bad[:3]}")
-            if fused_all:
-                metas = []
-                for i in done:
-                    t = tensors[i]
-                    metas.append(json.dumps({"dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape), "packed": "mxfp8",
-                                             "numel": t.numel(), "padded_numel": t.numel()}).encode())
-                if done:
-                    ecs = self.client.batch_put([keys[i] + "#meta" for i in done], metas, self._meta_cfg())
-                    if any(e != _bb.ErrorCode.OK for e in ecs):
-                        raise RuntimeError("meta put failed")
-                rest = [i for i in range(len(keys)) if i not in set(done)]
-                # a gathered slice the fused put refused (its placement is not one GPU-fabric shard per copy) is made
-                # contiguous and packed first, like any other
-                keys, tensors = [keys[i] for i in rest], [tensors[i].contiguous() for i in rest]
-                rows = [None] * len(keys)
-                if not keys:
-                    return
+        # objects the fused kernel can take go through batch_put_device_fp8 (bf16 read once, packed bytes on the wire,
+        # digest of the packed object from the tensor cores); the rest are packed first (unfused path below)
+        fused = [i for i, t in enumerate(tensors) if t.is_cuda and self._fused_fp8_ok(t, cfg)] if pack_fp8 else []
+        if fused:
+            def call(grp, es, wide):
+                fk, ptrs = [keys[i] for i in grp], [tensors[i].data_ptr() for i in grp]
+                if any(rows[i] is not None for i in grp):
+                    # one call and one launch: contiguous tensors go as one row each
+                    shapes = [_elem_rows(es, rows[i], tensors[i].numel()) for i in grp]
+                    return self.client.batch_put_device_fp8_strided(fk, ptrs, *map(list, zip(*shapes)), cfg, self._stream(), wide=wide)
+                return self.client.batch_put_device_fp8(fk, ptrs, [tensors[i].numel() for i in grp], cfg, self._stream(), wide=wide)
+
+            refused = set(self._packed("fused fp8 put", keys, fused, lambda i: tensors[i].dtype, call))
+            done = [i for grp in _by_dtype(fused, lambda i: tensors[i].dtype).values() for i in grp if i not in refused]
+            if done:
+                self._put_metas([keys[i] for i in done], [_meta(tensors[i].dtype, tensors[i].shape, True) for i in done])
+            done = set(done)
+            rest = [i for i in range(len(keys)) if i not in done]
+            # a gathered slice the fused put refused (its placement is not one GPU-fabric shard per copy) is made
+            # contiguous and packed first, like any other
+            keys, tensors = [keys[i] for i in rest], [tensors[i].contiguous() for i in rest]
+            rows = [None] * len(keys)
+            if not keys:
+                return
         payloads, metas, keep = [], [], []
         for t in tensors:
             assert t.is_cuda, "TensorStore moves CUDA tensors (host data: use client.put)"
-            meta = {"dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape), "packed": None, "numel": t.numel()}
+            metas.append(_meta(t.dtype, t.shape, pack_fp8))
             if pack_fp8:
                 n = t.numel()
                 npad = (n + 31) // 32 * 32
@@ -172,26 +208,18 @@ class TensorStore:
                 packed = torch.empty(_bb.mxfp8_packed_bytes(npad), dtype=torch.uint8, device=t.device)
                 _bb.mxfp8_pack(src.data_ptr(), npad, packed.data_ptr(), self._stream(), wide=_MX_WIDE[t.dtype])
                 keep.append(src)
-                meta["packed"] = "mxfp8"
-                meta["padded_numel"] = npad
                 t = packed
             assert t.data_ptr() % 16 == 0, "tensor storage must be 16-byte aligned"
             payloads.append(t)
-            metas.append(json.dumps(meta).encode())
         ptrs, sizes = [p.data_ptr() for p in payloads], [p.numel() * p.element_size() for p in payloads]
         if any(r is not None for r in rows):
             # one call and one launch for the whole batch: the other tensors go as one row each (pack_fp8 has no rows)
-            shapes = [r if r is not None else (n, n, 1) for r, n in zip(rows, sizes)]
-            ecs = self.client.batch_put_device_strided(list(keys), ptrs, [s[0] for s in shapes], [s[1] for s in shapes],
-                                                       [s[2] for s in shapes], cfg, self._stream())
+            shapes = [_elem_rows(1, r, n) for r, n in zip(rows, sizes)]
+            ecs = self.client.batch_put_device_strided(list(keys), ptrs, *map(list, zip(*shapes)), cfg, self._stream())
         else:
             ecs = self.client.batch_put_device(list(keys), ptrs, sizes, cfg, self._stream())
-        bad = [(k, e) for k, e in zip(keys, ecs) if e != _bb.ErrorCode.OK]
-        if bad:
-            raise RuntimeError(f"put failed: {bad[:3]}")
-        ecs = self.client.batch_put([k + "#meta" for k in keys], metas, self._meta_cfg())
-        if any(e != _bb.ErrorCode.OK for e in ecs):
-            raise RuntimeError("meta put failed")
+        _check("put", keys, ecs)
+        self._put_metas(keys, metas)
 
     def put(self, key: str, tensor: torch.Tensor, pack_fp8: bool = False, config=None) -> None:
         self.batch_put([key], [tensor], pack_fp8, config)
@@ -301,34 +329,20 @@ class TensorStore:
                      for p, s in zip(pages, shapes)]
         paged = [i for i, p in enumerate(pages) if p is not None]
         if paged and pack_fp8:
-            done = []
-            for dt, grp in _by_dtype(paged, lambda i: caches[i].dtype).items():
-                es = caches[grp[0]].element_size()
-                ecs = self.client.batch_put_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
-                                                             cfg, self._stream(), wide=_MX_WIDE[dt])
-                bad = [(keys[i], e) for i, e in zip(grp, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
-                if bad:
-                    raise RuntimeError(f"paged fp8 put failed: {bad[:3]}")
-                done += [i for i, e in zip(grp, ecs) if e == _bb.ErrorCode.OK]
-            paged = done
+            def call(grp, es, wide):
+                return self.client.batch_put_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp],
+                                                              [pages[i][1] // es for i in grp], cfg, self._stream(), wide=wide)
+
+            refused = set(self._packed("paged fp8 put", keys, paged, lambda i: caches[i].dtype, call))
+            paged = [i for grp in _by_dtype(paged, lambda i: caches[i].dtype).values() for i in grp if i not in refused]
         elif paged:
             ecs = self.client.batch_put_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged], [pages[i][1] for i in paged],
                                                      cfg, self._stream())
-            bad = [(keys[i], e) for i, e in zip(paged, ecs) if e != _bb.ErrorCode.OK]
-            if bad:
-                raise RuntimeError(f"paged put failed: {bad[:3]}")
+            _check("paged put", [keys[i] for i in paged], ecs)
         if paged:
-            metas = []
-            for i in paged:
-                n = torch.Size(shapes[i]).numel()
-                meta = {"dtype": str(caches[i].dtype).replace("torch.", ""), "shape": shapes[i], "packed": None, "numel": n}
-                if pack_fp8:
-                    meta.update(packed="mxfp8", padded_numel=n)
-                metas.append(json.dumps(meta).encode())
-            ecs = self.client.batch_put([keys[i] + "#meta" for i in paged], metas, self._meta_cfg())
-            if any(e != _bb.ErrorCode.OK for e in ecs):
-                raise RuntimeError("meta put failed")
-        rest = [i for i in range(len(keys)) if i not in set(paged)]
+            self._put_metas([keys[i] for i in paged], [_meta(caches[i].dtype, shapes[i], pack_fp8) for i in paged])
+        done = set(paged)
+        rest = [i for i in range(len(keys)) if i not in done]
         if rest:
             self.batch_put([keys[i] for i in rest], [caches[i].index_select(dims[i], torch.from_numpy(idx[i]).to(caches[i].device)) for i in rest],
                            pack_fp8, config)
@@ -372,34 +386,27 @@ class TensorStore:
                 raise ValueError(f"{k}: duplicate block ids")
             idx.append(t)
         # packed whole-block objects take the paged unpack; padded ones cannot fill whole pages
-        fp8 = [m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"] and self.client.device_fp8_eligible(m["numel"]) for m in metas]
+        fp8 = [self._fp8_whole(m) for m in metas]
         pages = [self._block_pages(c, d, b, FP8_PAGED_MIN_PAGE_BYTES if f else PAGED_MIN_PAGE_BYTES) if f or not m["packed"] else None
                  for m, f, c, d, b in zip(metas, fp8, caches, dims, idx)]
-        unpacked = [i for i, p in enumerate(pages) if p is not None and not fp8[i]]
-        for dt, grp in _by_dtype([i for i, p in enumerate(pages) if p is not None and fp8[i]], lambda i: caches[i].dtype).items():
-            es = caches[grp[0]].element_size()
-            ecs = self.client.batch_get_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
-                                                         self._stream(), wide=_MX_WIDE[dt])
-            bad = [(keys[i], e) for i, e in zip(grp, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
-            if bad:
-                raise RuntimeError(f"paged fp8 get failed: {bad[:3]}")
-            for i, e in zip(grp, ecs):
-                if e == _bb.ErrorCode.NOT_IMPLEMENTED:
-                    pages[i] = None  # get + index_copy_ below
-        paged = unpacked
+
+        def call(grp, es, wide):
+            return self.client.batch_get_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
+                                                          self._stream(), wide=wide)
+
+        for i in self._packed("paged fp8 get", keys, [i for i, p in enumerate(pages) if p is not None and fp8[i]], lambda i: caches[i].dtype, call):
+            pages[i] = None  # get + index_copy_ below
+        paged = [i for i, p in enumerate(pages) if p is not None and not fp8[i]]
         if paged:
             ecs, sizes = self.client.batch_get_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged],
                                                             [pages[i][1] for i in paged], self._stream())
-            bad = [(keys[i], e) for i, e in zip(paged, ecs) if e != _bb.ErrorCode.OK]
-            # the stored object must fill every page: a shorter one would leave the last blocks as they were
-            bad += [(keys[i], f"{n} bytes stored, {pages[i][0].size * pages[i][1]} selected") for i, e, n in zip(paged, ecs, sizes)
-                    if e == _bb.ErrorCode.OK and n != pages[i][0].size * pages[i][1]]
-            if bad:
-                raise RuntimeError(f"paged get failed: {bad[:3]}")
-        rest = [i for i, p in enumerate(pages) if p is None]
-        if rest:
-            for i, t in zip(rest, self.batch_get([keys[i] for i in rest], caches[rest[0]].device)):
-                caches[i].index_copy_(dims[i], torch.from_numpy(idx[i]).to(caches[i].device), t)
+            # the stored object must fill every page: a shorter one would leave the last blocks as they were; those are
+            # named after the items that failed
+            short = [f"{n} bytes stored, {pages[i][0].size * pages[i][1]} selected" if e == _bb.ErrorCode.OK and n != pages[i][0].size * pages[i][1]
+                     else _bb.ErrorCode.OK for i, e, n in zip(paged, ecs, sizes)]
+            _check("paged get", [keys[i] for i in paged] * 2, list(ecs) + short)
+        self._whole(keys, [i for i, p in enumerate(pages) if p is None], None,
+                    lambda i, t: caches[i].index_copy_(dims[i], torch.from_numpy(idx[i]).to(caches[i].device), t))
         return caches
 
     def get_blocks_into(self, key: str, cache: torch.Tensor, ids, dim: int = 0) -> torch.Tensor:
@@ -422,17 +429,15 @@ class TensorStore:
         result = [None] * len(keys)
         # MXFP8 objects made of whole tiles: unpack fused into the get kernel (falls through when the object is not a
         # single GPU-fabric shard any more, e.g. after demotion to a host tier)
-        fused_all = [i for i, m in enumerate(metas) if m["packed"] == "mxfp8" and m["padded_numel"] == m["numel"]
-                     and self.client.device_fp8_eligible(m["numel"])]
-        for dt, fused in _by_dtype(fused_all, lambda i: _stored_dtype(metas[i])).items():
-            outs = [torch.empty(metas[i]["numel"], dtype=dt, device=device) for i in fused]
-            ecs = self.client.batch_get_device_fp8([keys[i] for i in fused], [o.data_ptr() for o in outs], [metas[i]["numel"] for i in fused],
-                                                   self._stream(), wide=_MX_WIDE[dt])
-            for i, o, e in zip(fused, outs, ecs):
-                if e == _bb.ErrorCode.OK:
-                    result[i] = o.view(metas[i]["shape"])
-                elif e != _bb.ErrorCode.NOT_IMPLEMENTED:
-                    raise RuntimeError(f"fused fp8 get failed: {keys[i]}: {e}")
+        def call(grp, es, wide):
+            for i in grp:
+                result[i] = torch.empty(metas[i]["shape"], dtype=_stored_dtype(metas[i]), device=device)
+            return self.client.batch_get_device_fp8([keys[i] for i in grp], [result[i].data_ptr() for i in grp],
+                                                    [metas[i]["numel"] for i in grp], self._stream(), wide=wide)
+
+        fused = [i for i, m in enumerate(metas) if self._fp8_whole(m)]
+        for i in self._packed("fused fp8 get", keys, fused, lambda i: _stored_dtype(metas[i]), call):
+            result[i] = None
         rest = [i for i in range(len(keys)) if result[i] is None]
         if not rest:
             return result
@@ -446,9 +451,7 @@ class TensorStore:
                 bufs.append(torch.empty(m["shape"], dtype=_DTYPES[m["dtype"]], device=device))
         ecs, sizes = self.client.batch_get_device(list(keys), [b.data_ptr() for b in bufs], [b.numel() * b.element_size() for b in bufs],
                                                   self._stream())
-        bad = [(k, e) for k, e in zip(keys, ecs) if e != _bb.ErrorCode.OK]
-        if bad:
-            raise RuntimeError(f"get failed: {bad[:3]}")
+        _check("get", keys, ecs)
         out = []
         for m, b in zip(metas, bufs):
             if m["packed"] == "mxfp8":
@@ -497,47 +500,34 @@ class TensorStore:
             if not o.is_cuda or o.device.index != dev:
                 raise ValueError(f"{k}: out must be a CUDA tensor on cuda:{dev}, not {o.device}")
         rows = [None if o.is_contiguous() else self._source_rows(o) for o in outs]
-        rest = []  # route 4
-
-        def check(name, idx, ecs):
-            bad = [(keys[i], e) for i, e in zip(idx, ecs) if e != _bb.ErrorCode.OK]
-            if bad:
-                raise RuntimeError(f"{name} failed: {bad[:3]}")
-
         plain = [i for i, m in enumerate(metas) if not m["packed"]]
         dense = [i for i in plain if outs[i].is_contiguous()]
         if dense:
             ecs, _ = self.client.batch_get_device([keys[i] for i in dense], [outs[i].data_ptr() for i in dense],
                                                   [outs[i].numel() * outs[i].element_size() for i in dense], self._stream())
-            check("get", dense, ecs)
-        scattered = [i for i in plain if not outs[i].is_contiguous() and rows[i] is not None]
+            _check("get", [keys[i] for i in dense], ecs)
+        scattered = [i for i in plain if rows[i] is not None]
         if scattered:
             ecs, _ = self.client.batch_get_device_scatter([keys[i] for i in scattered], [outs[i].data_ptr() for i in scattered],
                                                           [rows[i][0] for i in scattered], [rows[i][1] for i in scattered],
                                                           [rows[i][2] for i in scattered], self._stream())
-            check("scattered get", scattered, ecs)
-        rest += [i for i in plain if not outs[i].is_contiguous() and rows[i] is None]
+            _check("scattered get", [keys[i] for i in scattered], ecs)
+        rest = [i for i in plain if not outs[i].is_contiguous() and rows[i] is None]  # route 4
         packed = [i for i, m in enumerate(metas) if m["packed"]]
-        fused = [i for i in packed if metas[i]["padded_numel"] == metas[i]["numel"] and self.client.device_fp8_eligible(metas[i]["numel"])
-                 and (outs[i].is_contiguous() or rows[i] is not None)]
-        rest += [i for i in packed if i not in set(fused)]
-        for dt, fused in _by_dtype(fused, lambda i: outs[i].dtype).items():
-            fk, ptrs = [keys[i] for i in fused], [outs[i].data_ptr() for i in fused]
-            es, wide = outs[fused[0]].element_size(), _MX_WIDE[dt]
-            if any(rows[i] is not None for i in fused):
-                # widths and pitches in elements; contiguous outs go as one row each
-                shapes = [(rows[i][0] // es, rows[i][1] // es, rows[i][2]) if rows[i] is not None else (outs[i].numel(),) * 2 + (1,)
-                          for i in fused]
-                ecs = self.client.batch_get_device_fp8_scatter(fk, ptrs, [outs[i].numel() for i in fused], [s[0] for s in shapes],
-                                                               [s[1] for s in shapes], [s[2] for s in shapes], self._stream(), wide=wide)
-            else:
-                ecs = self.client.batch_get_device_fp8(fk, ptrs, [outs[i].numel() for i in fused], self._stream(), wide=wide)
-            check("fused fp8 get", [i for i, e in zip(fused, ecs) if e != _bb.ErrorCode.NOT_IMPLEMENTED],
-                  [e for e in ecs if e != _bb.ErrorCode.NOT_IMPLEMENTED])
-            rest += [i for i, e in zip(fused, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
-        if rest:
-            for i, t in zip(rest, self.batch_get([keys[i] for i in rest], outs[rest[0]].device)):
-                outs[i].copy_(t)
+        fused = [i for i in packed if self._fp8_whole(metas[i]) and (outs[i].is_contiguous() or rows[i] is not None)]
+        take = set(fused)
+        rest += [i for i in packed if i not in take]
+
+        def call(grp, es, wide):
+            fk, ptrs, n = [keys[i] for i in grp], [outs[i].data_ptr() for i in grp], [outs[i].numel() for i in grp]
+            if any(rows[i] is not None for i in grp):
+                # contiguous outs go as one row each
+                shapes = [_elem_rows(es, rows[i], outs[i].numel()) for i in grp]
+                return self.client.batch_get_device_fp8_scatter(fk, ptrs, n, *map(list, zip(*shapes)), self._stream(), wide=wide)
+            return self.client.batch_get_device_fp8(fk, ptrs, n, self._stream(), wide=wide)
+
+        rest += self._packed("fused fp8 get", keys, fused, lambda i: outs[i].dtype, call)
+        self._whole(keys, rest, None, lambda i, t: outs[i].copy_(t))
         return outs
 
     def get_into(self, key: str, out: torch.Tensor) -> torch.Tensor:
@@ -563,49 +553,51 @@ class TensorStore:
                 raise IndexError(f"{k}: a 0-d tensor has no rows")
             if not 0 <= a <= b <= m["shape"][0]:
                 raise IndexError(f"{k}: rows [{a}, {b}) outside [0, {m['shape'][0]}]")
-        return self._get_rows(keys, metas, starts, stops, device)
+        return self._get_windows(keys, metas, [0] * len(keys), starts, stops, device)
 
-    def _get_rows(self, keys: list, metas: list, starts: list, stops: list, device: torch.device) -> list:
-        result = [None] * len(keys)
-        packed_all = [i for i, m in enumerate(metas) if m["packed"]]
-        for dt, packed in _by_dtype(packed_all, lambda i: _stored_dtype(metas[i])).items():
-            # Elements [lo, hi) of the (padded) packed object; their window ends before any pad.  Each result sits at
-            # element lo % (16 / element size) of its own allocation, so that the virtual base ptr - size * lo is 16-byte
-            # aligned and every row size takes the fused path.
-            per = 16 // torch.empty((), dtype=dt).element_size()
-            los, counts, ptrs = [], [], []
-            for i in packed:
-                m = metas[i]
-                row = torch.Size(m["shape"][1:]).numel()
-                lo, count = starts[i] * row, (stops[i] - starts[i]) * row
-                buf = torch.empty(count + lo % per, dtype=dt, device=device)
-                result[i] = buf[lo % per:].view([stops[i] - starts[i]] + m["shape"][1:])
-                los.append(lo), counts.append(count), ptrs.append(result[i].data_ptr())
-            ecs = self.client.batch_get_device_fp8_range([keys[i] for i in packed], ptrs, [metas[i]["padded_numel"] for i in packed], los,
-                                                         counts, self._stream(), wide=_MX_WIDE[dt])
-            bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
-            if bad:
-                raise RuntimeError(f"fused fp8 range get failed: {bad[:3]}")
-            unfused = [i for i, e in zip(packed, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
-            if unfused:
-                whole = self.batch_get([keys[i] for i in unfused], device)
-                for i, t in zip(unfused, whole):
-                    result[i] = t[starts[i]:stops[i]].clone()
-        ranged = [i for i, m in enumerate(metas) if not m["packed"]]
-        if ranged:
-            offsets, lengths = [], []
-            for i in ranged:
-                m = metas[i]
-                dtype = _DTYPES[m["dtype"]]
-                row = torch.Size(m["shape"][1:]).numel() * torch.empty((), dtype=dtype).element_size()
-                result[i] = torch.empty([stops[i] - starts[i]] + m["shape"][1:], dtype=dtype, device=device)
-                offsets.append(starts[i] * row)
-                lengths.append((stops[i] - starts[i]) * row)
-            ecs = self.client.batch_get_device_range([keys[i] for i in ranged], [result[i].data_ptr() for i in ranged], offsets,
-                                                     lengths, self._stream())
-            bad = [(keys[i], e) for i, e in zip(ranged, ecs) if e != _bb.ErrorCode.OK]
-            if bad:
-                raise RuntimeError(f"range get failed: {bad[:3]}")
+    def _get_windows(self, keys: list, metas: list, dims: list, starts: list, stops: list, device: torch.device) -> list:
+        """`t.narrow(dims[i], starts[i], stops[i] - starts[i])` of each stored tensor, as new contiguous tensors.  The
+        window is `rows` = prod(shape[:dim]) runs of `width` elements every `pitch` from element `offset`; the packed calls
+        count elements, the others bytes.  Along dim 0 (one run) the range calls read it, along other dims the strided
+        calls, one call per kind for all such items (packed: per dtype).  Packed items the fused kernel refuses are read
+        whole and narrowed."""
+        result, win = [None] * len(keys), [None] * len(keys)
+        for i, (m, d, a, b) in enumerate(zip(metas, dims, starts, stops)):
+            shape, dt = m["shape"], _stored_dtype(m)
+            inner = torch.Size(shape[d + 1:]).numel()
+            rows, offset, width = torch.Size(shape[:d]).numel(), a * inner, (b - a) * inner
+            # Each result but an unpacked dim-0 one sits at element offset % (16 / element size) of its own allocation,
+            # so that its virtual base (ptr - element size * offset) is 16-byte aligned and the window takes the fused
+            # kernel whenever its row gap allows.
+            skew = offset % (16 // dt.itemsize) if m["packed"] or d else 0
+            result[i] = torch.empty(rows * width + skew, dtype=dt, device=device)[skew:].view(shape[:d] + [b - a] + shape[d + 1:])
+            es = 1 if m["packed"] else dt.itemsize
+            win[i] = (offset * es, width * es, shape[d] * inner * es, rows)
+
+        def narrowed(i, t):
+            result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).clone(memory_format=torch.contiguous_format)
+
+        for along0 in (True, False):
+            idx = [i for i, d in enumerate(dims) if (d == 0) == along0]
+            n = 2 if along0 else 4  # (offset, width) or (offset, width, pitch, rows)
+            fp8_call, call, what = ((self.client.batch_get_device_fp8_range, self.client.batch_get_device_range, "range get") if along0 else
+                                    (self.client.batch_get_device_fp8_strided, self.client.batch_get_device_strided, "strided get"))
+
+            def fp8(grp, es, wide):
+                return fp8_call([keys[i] for i in grp], [result[i].data_ptr() for i in grp], [metas[i]["padded_numel"] for i in grp],
+                                *[[win[i][k] for i in grp] for k in range(n)], self._stream(), wide=wide)
+
+            def dtype_of(i):
+                return result[i].dtype
+
+            # the items one dtype's call refuses are read whole before the next dtype's call
+            for grp in _by_dtype([i for i in idx if metas[i]["packed"]], dtype_of).values():
+                self._whole(keys, self._packed(f"fused fp8 {what}", keys, grp, dtype_of, fp8), device, narrowed)
+            plain = [i for i in idx if not metas[i]["packed"]]
+            if plain:
+                ecs = call([keys[i] for i in plain], [result[i].data_ptr() for i in plain], *[[win[i][k] for i in plain] for k in range(n)],
+                           self._stream())
+                _check(what, [keys[i] for i in plain], ecs)
         return result
 
     def get_rows(self, key: str, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
@@ -644,53 +636,7 @@ class TensorStore:
             dims[j] %= len(shape)
             if not 0 <= a <= b <= shape[dims[j]]:
                 raise IndexError(f"{k}: [{a}, {b}) outside [0, {shape[dims[j]]}] along dim {dims[j]}")
-        result = [None] * len(keys)
-        first = [i for i, d in enumerate(dims) if d == 0]
-        if first:
-            rows = self._get_rows([keys[i] for i in first], [metas[i] for i in first], [starts[i] for i in first],
-                                  [stops[i] for i in first], device)
-            for i, t in zip(first, rows):
-                result[i] = t
-        packed_all = [i for i, m in enumerate(metas) if dims[i] != 0 and m["packed"]]
-        for dt, packed in _by_dtype(packed_all, lambda i: _stored_dtype(metas[i])).items():
-            # prod(shape[:dim]) rows of (stop - start) * inner elements every shape[dim] * inner elements
-            per = 16 // torch.empty((), dtype=dt).element_size()
-            offsets, widths, pitches, nrows = [], [], [], []
-            for i in packed:
-                shape, d = metas[i]["shape"], dims[i]
-                inner = torch.Size(shape[d + 1:]).numel()
-                offset, width = starts[i] * inner, (stops[i] - starts[i]) * inner
-                rows = torch.Size(shape[:d]).numel()
-                buf = torch.empty(rows * width + offset % per, dtype=dt, device=device)
-                result[i] = buf[offset % per:].view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
-                offsets.append(offset), widths.append(width), pitches.append(shape[d] * inner), nrows.append(rows)
-            ecs = self.client.batch_get_device_fp8_strided([keys[i] for i in packed], [result[i].data_ptr() for i in packed],
-                                                           [metas[i]["padded_numel"] for i in packed], offsets, widths, pitches,
-                                                           nrows, self._stream(), wide=_MX_WIDE[dt])
-            bad = [(keys[i], e) for i, e in zip(packed, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
-            if bad:
-                raise RuntimeError(f"fused fp8 strided get failed: {bad[:3]}")
-            unfused = [i for i, e in zip(packed, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
-            if unfused:
-                for i, t in zip(unfused, self.batch_get([keys[i] for i in unfused], device)):
-                    result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).contiguous()
-        strided = [i for i, m in enumerate(metas) if dims[i] != 0 and not m["packed"]]
-        if strided:
-            offsets, widths, pitches, nrows = [], [], [], []
-            for i in strided:
-                shape, d, dtype = metas[i]["shape"], dims[i], _DTYPES[metas[i]["dtype"]]
-                inner = torch.Size(shape[d + 1:]).numel() * torch.empty((), dtype=dtype).element_size()
-                offset, width = starts[i] * inner, (stops[i] - starts[i]) * inner
-                rows = torch.Size(shape[:d]).numel()
-                buf = torch.empty(rows * width + offset % 16, dtype=torch.uint8, device=device)
-                result[i] = buf[offset % 16:].view(dtype).view(shape[:d] + [stops[i] - starts[i]] + shape[d + 1:])
-                offsets.append(offset), widths.append(width), pitches.append(shape[d] * inner), nrows.append(rows)
-            ecs = self.client.batch_get_device_strided([keys[i] for i in strided], [result[i].data_ptr() for i in strided], offsets,
-                                                       widths, pitches, nrows, self._stream())
-            bad = [(keys[i], e) for i, e in zip(strided, ecs) if e != _bb.ErrorCode.OK]
-            if bad:
-                raise RuntimeError(f"strided get failed: {bad[:3]}")
-        return result
+        return self._get_windows(keys, metas, dims, starts, stops, device)
 
     def get_slice(self, key: str, dim: int, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
         """`t.narrow(dim, start, stop - start).contiguous()` of the tensor stored under `key` (see batch_get_slices)."""
@@ -727,83 +673,51 @@ class AsyncTensorStore(TensorStore):
     def _stream(self) -> int:  # every native call of this store is issued on the side stream
         return self._side.cuda_stream
 
-    def put_async(self, keys: Sequence[str], tensors: Sequence[torch.Tensor], pack_fp8: bool = False, config=None):
-        ready = torch.cuda.Event()
-        ready.record(torch.cuda.current_stream())  # the tensors' producers
-        tensors = list(tensors)  # keep them alive until the transfer is done
+    def _on_side(self, after_caller: bool, fn, *args, result=None):
+        """A future of fn(*args) run on the side stream from the worker thread, after the work already queued on the
+        caller's stream when `after_caller`; it yields `result` (fn's own result when None) once the side stream is done."""
+        ready = None
+        if after_caller:
+            ready = torch.cuda.Event()
+            ready.record(torch.cuda.current_stream())
 
         def run():
             torch.cuda.set_device(self._device)
-            self._side.wait_event(ready)
+            if ready is not None:
+                self._side.wait_event(ready)
             with torch.cuda.stream(self._side):
-                self.batch_put(keys, tensors, pack_fp8, config)
+                out = fn(*args)
             self._side.synchronize()
-            return len(tensors)
+            return out if result is None else result
 
         return self._pool.submit(run)
+
+    def put_async(self, keys: Sequence[str], tensors: Sequence[torch.Tensor], pack_fp8: bool = False, config=None):
+        tensors = list(tensors)  # keep them alive until the transfer is done
+        return self._on_side(True, self.batch_put, keys, tensors, pack_fp8, config, result=len(tensors))
 
     def get_async(self, keys: Sequence[str]):
-        def run():
-            torch.cuda.set_device(self._device)
-            with torch.cuda.stream(self._side):
-                out = self.batch_get(keys)
-            self._side.synchronize()
-            return out
-
-        return self._pool.submit(run)
+        return self._on_side(False, self.batch_get, keys)
 
     def get_into_async(self, keys: Sequence[str], outs: Sequence[torch.Tensor]):
         """batch_get_into on the side stream; the future yields `outs`, already synchronised with it.  The side stream
         first waits for the work already queued on the caller's stream, so the get does not overtake the caller's earlier
         reads or writes of the outs."""
-        ready = torch.cuda.Event()
-        ready.record(torch.cuda.current_stream())
-        keys, outs = list(keys), list(outs)
-
-        def run():
-            torch.cuda.set_device(self._device)
-            self._side.wait_event(ready)
-            with torch.cuda.stream(self._side):
-                self.batch_get_into(keys, outs)
-            self._side.synchronize()
-            return outs
-
-        return self._pool.submit(run)
+        outs = list(outs)
+        return self._on_side(True, self.batch_get_into, list(keys), outs, result=outs)
 
     def put_blocks_async(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0, pack_fp8: bool = False,
                          config=None):
         """batch_put_blocks on the side stream, ordered after the work already queued on the caller's stream; the future
         yields the number of objects stored."""
-        ready = torch.cuda.Event()
-        ready.record(torch.cuda.current_stream())
-        keys, caches, ids = list(keys), list(caches), list(ids)
-
-        def run():
-            torch.cuda.set_device(self._device)
-            self._side.wait_event(ready)
-            with torch.cuda.stream(self._side):
-                self.batch_put_blocks(keys, caches, ids, dim, pack_fp8, config)
-            self._side.synchronize()
-            return len(keys)
-
-        return self._pool.submit(run)
+        keys = list(keys)
+        return self._on_side(True, self.batch_put_blocks, keys, list(caches), list(ids), dim, pack_fp8, config, result=len(keys))
 
     def get_blocks_into_async(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0):
         """batch_get_blocks_into on the side stream, ordered after the work already queued on the caller's stream; the
         future yields `caches`, already synchronised with the side stream."""
-        ready = torch.cuda.Event()
-        ready.record(torch.cuda.current_stream())
-        keys, caches, ids = list(keys), list(caches), list(ids)
-
-        def run():
-            torch.cuda.set_device(self._device)
-            self._side.wait_event(ready)
-            with torch.cuda.stream(self._side):
-                self.batch_get_blocks_into(keys, caches, ids, dim)
-            self._side.synchronize()
-            return caches
-
-        return self._pool.submit(run)
+        caches = list(caches)
+        return self._on_side(True, self.batch_get_blocks_into, list(keys), caches, list(ids), dim, result=caches)
 
     def close(self):
         self._pool.shutdown(wait=True)
