@@ -97,15 +97,21 @@ class GpuFabric : public client::DeviceTransport {
   // NVLS replica arenas: pools named mc<g>@gpu<r> resolve through the arena; a put whose replica set is
   // exactly one multicast group (same offset everywhere) becomes ONE multimem.st stream.
   void set_arena(std::shared_ptr<NvlsArena> a) { arena_ = std::move(a); }
-  uint64_t multicast_puts() const { return multicast_puts_; }
+  uint64_t multicast_puts() const { return multicast_puts_.load(std::memory_order_relaxed); }
   uint64_t remaps() const { return remaps_; }
   // Payload bytes moved by the fused kernels, by direction and path: "hbm" (slab on this client's own GPU), "nvlink"
   // (peer slab over NVSwitch; multicast puts count one egress stream), "pcie" (pinned / shared DRAM pool).
   std::string metrics_text() const override;
   uint64_t path_bytes(bool put, int path) const { return bytes_[put ? 0 : 1][path].load(std::memory_order_relaxed); }  // mappings dropped because their pool was re-registered under a new key
   XferEngine& engine() { return *engine_; }
-  float last_device_ms() const { return last_ms_; }
-  double total_device_ms() const { return total_ms_; }  // sum of kernel times of all finished batches
+  float last_device_ms() const {
+    std::lock_guard<std::mutex> lk(mu_);
+    return last_ms_;
+  }
+  double total_device_ms() const {  // sum of kernel times of all finished batches
+    std::lock_guard<std::mutex> lk(mu_);
+    return total_ms_;
+  }
 
  private:
   GpuFabric() = default;
@@ -141,6 +147,7 @@ class GpuFabric : public client::DeviceTransport {
   ErrorCode finish(uint64_t ticket, InFlight* fl, XferResult* res);
   ErrorCode transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, XferResult* res);
   void note_device_ms(float ms) {
+    std::lock_guard<std::mutex> lk(mu_);
     last_ms_ = ms;
     total_ms_ += ms;
   }
@@ -153,14 +160,14 @@ class GpuFabric : public client::DeviceTransport {
   std::map<std::string, HostCandidate> host_candidates_;
   std::set<std::string> host_unreachable_;
   std::shared_ptr<NvlsArena> arena_;
-  uint64_t multicast_puts_ = 0;
+  std::atomic<uint64_t> multicast_puts_{0};
   std::atomic<uint64_t> remaps_{0};
   enum Path : int { PATH_HBM = 0, PATH_NVLINK = 1, PATH_PCIE = 2, PATH_MULTICAST = 3, kNumPaths = 4 };
   Path classify(const ShardPlacement& s) const;
   void count(bool put, Path p, uint64_t bytes) { bytes_[put ? 0 : 1][p].fetch_add(bytes, std::memory_order_relaxed); }
   std::atomic<uint64_t> bytes_[2][kNumPaths] = {};
-  float last_ms_ = 0.f;
-  double total_ms_ = 0.0;
+  float last_ms_ = 0.f;    // guarded by mu_
+  double total_ms_ = 0.0;  // guarded by mu_
 };
 
 // Process-local slab registry (in-process workers + clients share pointers directly; CUDA IPC

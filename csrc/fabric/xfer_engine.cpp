@@ -27,17 +27,11 @@ static ErrorCode cuda_failed(int code, const char* what) {
 }
 
 ErrorCode XferEngine::cuda_failed(int code, const char* what) {
-  last_cuda_error_ = code;
+  last_cuda_error_.store(code, std::memory_order_relaxed);
   return gpu::cuda_failed(code, what);
 }
 
 namespace {
-// Frees a slot when the call that holds it returns, whichever way it returns.
-struct SlotRelease {
-  uint64_t& ticket;
-  ~SlotRelease() { ticket = 0; }
-};
-
 // A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items |
 // page entries, only for batches with paged items].
 size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
@@ -119,41 +113,98 @@ struct XferEngine::Slot {
     uint64_t expect;
   };
   std::vector<Empty> empties;
+
+  ~Slot() {
+    if (ev_done) cudaEventSynchronize(ev_done);
+    cudaFreeHost(h_tab);
+    cudaFreeHost(h_res);
+    cudaFree(d_tab);
+    cudaFree(d_sum);
+    cudaFree(d_done);
+    cudaFree(d_digest);
+    cudaFree(d_status);
+    if (d_debug) cudaFree(d_debug);
+    if (d_trace) cudaFree(d_trace);
+    if (ev_start) cudaEventDestroy(ev_start);
+    if (ev_stop) cudaEventDestroy(ev_stop);
+    if (ev_done) cudaEventDestroy(ev_done);
+  }
 };
+
+// Releases a claimed slot when the call that holds it returns, whichever way it returns, unless the slot was kept (a
+// submitted batch holds it until wait()).  Work the call queued on a stream before it failed is finished first, so
+// that the next batch in the slot, maybe another thread's on another stream, cannot race it for the slot's tables.
+class XferEngine::SlotHold {
+ public:
+  SlotHold(XferEngine* e, Slot* s) : e_(e), s_(s) {}
+  ~SlotHold() {
+    if (!s_) return;
+    if (queued_) cudaStreamSynchronize(stream_);
+    e_->release_slot(s_);
+  }
+  SlotHold(const SlotHold&) = delete;
+  SlotHold& operator=(const SlotHold&) = delete;
+  void queued(cudaStream_t st) {
+    queued_ = true;
+    stream_ = st;
+  }
+  void settled() { queued_ = false; }
+  void keep() { s_ = nullptr; }
+
+ private:
+  XferEngine* e_;
+  Slot* s_;
+  bool queued_ = false;
+  cudaStream_t stream_ = nullptr;
+};
+
+// Allocates one slot for batches of up to `max_items` objects on the current device.  Its digest workspace is zeroed
+// on a stream of its own that does not synchronise with the legacy default stream: a slot added for a concurrent caller
+// must not wait for other threads' batches.
+Result<std::unique_ptr<XferEngine::Slot>> XferEngine::new_slot(uint32_t max_items) {
+  const size_t tab_bytes = stride_table_offset(max_items) + static_cast<size_t>(max_items) * sizeof(XferStride);
+  const size_t res_bytes = static_cast<size_t>(max_items) * 12;
+  auto s = std::make_unique<Slot>();
+  cudaStream_t zero = nullptr;
+  bool ok = cudaMallocHost(reinterpret_cast<void**>(&s->h_tab), tab_bytes) == cudaSuccess;
+  ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_res), res_bytes) == cudaSuccess;
+  ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_tab), tab_bytes) == cudaSuccess;
+  s->tab_bytes = tab_bytes;
+  ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_sum), static_cast<size_t>(max_items) * 8) == cudaSuccess;
+  ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_done), static_cast<size_t>(max_items) * 4) == cudaSuccess;
+  ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_digest), static_cast<size_t>(max_items) * 8) == cudaSuccess;
+  ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_status), static_cast<size_t>(max_items) * 4) == cudaSuccess;
+  ok = ok && cudaStreamCreateWithFlags(&zero, cudaStreamNonBlocking) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(s->d_sum, 0, static_cast<size_t>(max_items) * 8, zero) == cudaSuccess;
+  ok = ok && cudaMemsetAsync(s->d_done, 0, static_cast<size_t>(max_items) * 4, zero) == cudaSuccess;
+  ok = ok && cudaStreamSynchronize(zero) == cudaSuccess;
+  if (zero) cudaStreamDestroy(zero);
+  ok = ok && cudaEventCreate(&s->ev_start) == cudaSuccess;
+  ok = ok && cudaEventCreate(&s->ev_stop) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&s->ev_done, cudaEventDisableTiming) == cudaSuccess;
+  if (!ok) {
+    BB_LOG(ERROR) << "XferEngine: device allocation failed: " << cudaGetErrorString(cudaGetLastError());
+    return ErrorCode::OUT_OF_MEMORY;  // the slot's destructor frees what was allocated
+  }
+  return s;
+}
 
 Result<std::unique_ptr<XferEngine>> XferEngine::create(int device, uint32_t max_items, int slots) {
   std::unique_ptr<XferEngine> e(new XferEngine());
   e->device_ = device;
   e->max_items_ = max_items;
+  if (slots < 1 || slots > kMaxSlots) return ErrorCode::INVALID_ARGUMENT;
   int prev = 0;
   if (cudaGetDevice(&prev) != cudaSuccess) return ErrorCode::FABRIC_ERROR;
   if (cudaSetDevice(device) != cudaSuccess) return ErrorCode::FABRIC_ERROR;
-  const size_t tab_bytes = stride_table_offset(max_items) + static_cast<size_t>(max_items) * sizeof(XferStride);
-  const size_t res_bytes = static_cast<size_t>(max_items) * 12;
-  bool ok = true;
-  for (int i = 0; i < slots && ok; ++i) {
-    auto s = std::make_unique<Slot>();
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_tab), tab_bytes) == cudaSuccess;
-    ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_res), res_bytes) == cudaSuccess;
-    ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_tab), tab_bytes) == cudaSuccess;
-    s->tab_bytes = tab_bytes;
-    ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_sum), static_cast<size_t>(max_items) * 8) == cudaSuccess;
-    ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_done), static_cast<size_t>(max_items) * 4) == cudaSuccess;
-    ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_digest), static_cast<size_t>(max_items) * 8) == cudaSuccess;
-    ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_status), static_cast<size_t>(max_items) * 4) == cudaSuccess;
-    ok = ok && cudaMemset(s->d_sum, 0, static_cast<size_t>(max_items) * 8) == cudaSuccess;
-    ok = ok && cudaMemset(s->d_done, 0, static_cast<size_t>(max_items) * 4) == cudaSuccess;
-    ok = ok && cudaEventCreate(&s->ev_start) == cudaSuccess;
-    ok = ok && cudaEventCreate(&s->ev_stop) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&s->ev_done, cudaEventDisableTiming) == cudaSuccess;
-    e->slots_.push_back(std::move(s));
+  ErrorCode ec = ErrorCode::OK;
+  for (int i = 0; i < slots && ec == ErrorCode::OK; ++i) {
+    auto s = new_slot(max_items);
+    if (s.ok()) e->slots_.push_back(std::move(s).value());
+    else ec = s.error();
   }
-  ok = ok && cudaDeviceSynchronize() == cudaSuccess;
   cudaSetDevice(prev);
-  if (!ok) {
-    BB_LOG(ERROR) << "XferEngine: device allocation failed: " << cudaGetErrorString(cudaGetLastError());
-    return ErrorCode::OUT_OF_MEMORY;
-  }
+  if (ec != ErrorCode::OK) return ec;
   return e;
 }
 
@@ -161,21 +212,7 @@ XferEngine::~XferEngine() {
   int prev = 0;
   cudaGetDevice(&prev);
   cudaSetDevice(device_);
-  for (auto& s : slots_) {
-    if (s->ev_done) cudaEventSynchronize(s->ev_done);
-    cudaFreeHost(s->h_tab);
-    cudaFreeHost(s->h_res);
-    cudaFree(s->d_tab);
-    cudaFree(s->d_sum);
-    cudaFree(s->d_done);
-    cudaFree(s->d_digest);
-    cudaFree(s->d_status);
-    if (s->d_debug) cudaFree(s->d_debug);
-    if (s->d_trace) cudaFree(s->d_trace);
-    if (s->ev_start) cudaEventDestroy(s->ev_start);
-    if (s->ev_stop) cudaEventDestroy(s->ev_stop);
-    if (s->ev_done) cudaEventDestroy(s->ev_done);
-  }
+  slots_.clear();
   cudaSetDevice(prev);
 }
 
@@ -212,8 +249,8 @@ ErrorCode XferEngine::mailbox_launch_locked(uint32_t first_seq) {
   ++m.epoch;
   const int rc = launch_mailbox(m.slots, m.results, m.ctl, first_seq, m.epoch, m.linger_ns, m.max_ns, m.stream);
   if (rc != 0) return cuda_failed(rc, "launch_mailbox");
-  ++mailbox_launches_;
-  ++launches_;
+  mailbox_launches_.fetch_add(1, std::memory_order_relaxed);
+  launches_.fetch_add(1, std::memory_order_relaxed);
   return ErrorCode::OK;
 }
 
@@ -249,7 +286,7 @@ ErrorCode XferEngine::mailbox_post(Slot* s, const XferDesc* descs, uint32_t nd, 
     *reinterpret_cast<volatile uint32_t*>(&q.seq) = seq;
   }
   m.outstanding += nd;
-  mailbox_requests_ += nd;
+  mailbox_requests_.fetch_add(nd, std::memory_order_relaxed);
   // is anybody polling?  (exit_epoch == epoch: the last incarnation has announced its exit; epoch 0: never launched)
   if (m.epoch == 0 || *reinterpret_cast<volatile uint32_t*>(&m.ctl->exit_epoch) == m.epoch) {
     const uint32_t first = m.epoch == 0 ? s->mail_first : *reinterpret_cast<volatile uint32_t*>(&m.ctl->next_seq);
@@ -270,6 +307,7 @@ ErrorCode XferEngine::mailbox_wait(Slot* s) {
     uint32_t spins = 0;
     while (r->seq != seq) {
       if ((++spins & 0x3Fu) != 0) continue;
+      std::lock_guard<std::mutex> lk(mu_);
       // the warp may have left just before our request landed (it lingers only so long): start the next incarnation
       if (*reinterpret_cast<volatile uint32_t*>(&m.ctl->exit_epoch) == m.epoch && r->seq != seq) {
         BB_CUDA(cudaSetDevice(device_));
@@ -286,6 +324,7 @@ ErrorCode XferEngine::mailbox_wait(Slot* s) {
     dg[i] = r->digest;
     stt[i] = r->status;
   }
+  std::lock_guard<std::mutex> lk(mu_);
   m.outstanding -= std::min(m.outstanding, nd);
   return ErrorCode::OK;
 }
@@ -306,10 +345,32 @@ bool XferEngine::small_path_enabled() {
   return on && small_path_;
 }
 
-XferEngine::Slot* XferEngine::free_slot() {
-  for (auto& c : slots_)
-    if (c->ticket == 0) return c.get();
-  return nullptr;
+Result<XferEngine::Slot*> XferEngine::claim_slot() {
+  {
+    std::lock_guard<std::mutex> lk(mu_);
+    for (auto& c : slots_)
+      if (c->ticket == 0) {
+        c->ticket = next_ticket_++;
+        return c.get();
+      }
+    if (static_cast<int>(slots_.size()) + growing_ >= kMaxSlots) return ErrorCode::RESOURCE_EXHAUSTED;
+    ++growing_;
+  }
+  // Every slot is held by a batch of another thread, or of this one: a pipelined caller, or run_fp8 asking for its
+  // scales batch, holds one slot while it asks for the next, so waiting for a free one could wait forever.
+  auto fresh = new_slot(max_items_);
+  std::lock_guard<std::mutex> lk(mu_);
+  --growing_;
+  if (!fresh.ok()) return fresh.error();
+  Slot* s = fresh.value().get();
+  s->ticket = next_ticket_++;
+  slots_.push_back(std::move(fresh).value());
+  return s;
+}
+
+void XferEngine::release_slot(Slot* s) {
+  std::lock_guard<std::mutex> lk(mu_);
+  s->ticket = 0;
 }
 
 // Completes the slot's pinned table for the `nd` descriptors at its start, [descs | tile_start]: every descriptor's
@@ -363,9 +424,12 @@ ErrorCode XferEngine::write_pages(Slot* s, uint32_t nd, size_t* tab) {
 Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream,
                                     bool capture_debug) {
   if (items.size() > max_items_) return ErrorCode::RESOURCE_EXHAUSTED;
-  Slot* s = free_slot();
-  if (!s) return ErrorCode::RESOURCE_EXHAUSTED;  // caller must wait() on outstanding tickets
   BB_CUDA(cudaSetDevice(device_));
+  auto claimed = claim_slot();
+  if (!claimed.ok()) return claimed.error();
+  Slot* s = claimed.value();
+  const uint64_t ticket = s->ticket;
+  SlotHold hold(this, s);
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   s->item_to_desc.assign(items.size(), -1);
   s->empties.clear();
@@ -450,28 +514,36 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   // costs about as much GPU time as the kernel): the resident mailbox warp serves it without any launch, or else it
   // completes by flag and the launch is the ONLY stream operation.  The mailbox request bypasses `stream`, so
   // everything already queued there must have finished (the caller's source data is ready), and only one mailed batch
-  // is in flight at a time.
+  // is in flight at a time (across all threads: checked again under mu_ where the batch is posted).
   using Completion = Slot::Completion;
   s->completion = Completion::EVENTS;
   if (nd && all_small && direct && !capture_debug && !tile_trace_) {
-    if (nd <= kMailSlots / 2 && mailbox_enabled() && (!mb_ || mb_->outstanding == 0)) {
+    bool mail = nd <= kMailSlots / 2 && mailbox_enabled();
+    if (mail) {
+      std::lock_guard<std::mutex> lk(mu_);
+      mail = !mb_ || mb_->outstanding == 0;
+    }
+    if (mail) {
       bool simple = true;
       for (uint32_t i = 0; i < nd; ++i) simple = simple && descs[i].ndst == 1 && !(descs[i].flags & (XFER_MULTIMEM | XFER_WINDOW));
-      if (simple && cudaStreamQuery(st) == cudaSuccess)
-        s->completion = Completion::MAILBOX;
-      else
-        cudaGetLastError();  // cudaErrorNotReady is not sticky, but keep the error state clean
+      mail = simple && cudaStreamQuery(st) == cudaSuccess;
+      if (!mail) cudaGetLastError();  // cudaErrorNotReady is not sticky, but keep the error state clean
     }
-    if (s->completion == Completion::EVENTS && flag_completion_enabled()) s->completion = Completion::FLAG;
+    if (mail) {
+      std::lock_guard<std::mutex> lk(mu_);
+      if (!mb_ || mb_->outstanding == 0) {
+        s->completion = Completion::MAILBOX;
+        BB_TRY(mailbox_post(s, descs, nd, xalgo));
+        hold.keep();
+        return ticket;
+      }
+    }
+    if (flag_completion_enabled()) s->completion = Completion::FLAG;
   }
 
-  if (s->completion == Completion::MAILBOX) {
-    BB_TRY(mailbox_post(s, descs, nd, xalgo));
-    s->ticket = next_ticket_++;
-    return s->ticket;
-  }
   if (nd) {
     const bool inline_tab = nd <= kInlineDescs && s->pages.empty();  // page entries live in the device table only
+    hold.queued(st);
     if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
     if (capture_debug) {
       const size_t need = static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN * 4;
@@ -523,8 +595,8 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     }
     const int rc = launch_xfer(l);
     if (rc != 0) return cuda_failed(rc, "launch_xfer");
-    ++launches_;
-    if (all_small && !capture_debug && !tile_trace_) ++small_launches_;
+    launches_.fetch_add(1, std::memory_order_relaxed);
+    if (all_small && !capture_debug && !tile_trace_) small_launches_.fetch_add(1, std::memory_order_relaxed);
     if (s->completion == Completion::EVENTS) {
       BB_CUDA(cudaEventRecord(s->ev_stop, st));
       if (algo != ChecksumAlgo::NONE && !direct) {
@@ -535,16 +607,19 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     }
   }
   if (s->completion == Completion::EVENTS) BB_CUDA(cudaEventRecord(s->ev_done, st));
-  s->ticket = next_ticket_++;
-  return s->ticket;
+  hold.keep();
+  return ticket;
 }
 
 ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
   Slot* s = nullptr;
-  for (auto& c : slots_)
-    if (c->ticket == ticket) { s = c.get(); break; }
+  {
+    std::lock_guard<std::mutex> lk(mu_);
+    for (auto& c : slots_)
+      if (ticket != 0 && c->ticket == ticket) { s = c.get(); break; }
+  }
   if (!s) return ErrorCode::NOT_FOUND;
-  SlotRelease release{s->ticket};
+  SlotHold release(this, s);
   const uint32_t nd = s->ndesc;
   switch (s->completion) {
     case Slot::Completion::MAILBOX:
@@ -604,12 +679,16 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
     if (nd && s->completion == Slot::Completion::EVENTS) cudaEventElapsedTime(&out->device_ms, s->ev_start, s->ev_stop);
   }
   if (s->debug && nd) {
-    debug_host_.resize(static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN);
-    BB_CUDA(cudaMemcpy(debug_host_.data(), s->d_debug, debug_host_.size() * 4, cudaMemcpyDeviceToHost));
+    std::vector<uint32_t> acc(static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN);
+    BB_CUDA(cudaMemcpy(acc.data(), s->d_debug, acc.size() * 4, cudaMemcpyDeviceToHost));
+    std::lock_guard<std::mutex> lk(mu_);
+    debug_host_ = std::move(acc);
   }
   if (s->traced && nd) {
-    trace_host_.resize(static_cast<size_t>(s->total_tiles) * 4);
-    BB_CUDA(cudaMemcpy(trace_host_.data(), s->d_trace, trace_host_.size() * 8, cudaMemcpyDeviceToHost));
+    std::vector<uint64_t> trace(static_cast<size_t>(s->total_tiles) * 4);
+    BB_CUDA(cudaMemcpy(trace.data(), s->d_trace, trace.size() * 8, cudaMemcpyDeviceToHost));
+    std::lock_guard<std::mutex> lk(mu_);
+    trace_host_ = std::move(trace);
   }
   return ErrorCode::OK;
 }
@@ -622,10 +701,10 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // The fused kernel's batch holds this slot for the whole call; the scales batch below takes a second one.  The slot's
   // d_digest collects the payload sums (d_sum must stay zero between batches for bb_xfer).
-  Slot* s = free_slot();
-  if (!s) return ErrorCode::RESOURCE_EXHAUSTED;
-  s->ticket = next_ticket_++;
-  SlotRelease release{s->ticket};
+  auto claimed = claim_slot();
+  if (!claimed.ok()) return claimed.error();
+  Slot* s = claimed.value();
+  SlotHold release(this, s);
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
   // as submit() does: nothing of the slot's last batch (a paged bb_xfer batch's page entries included) carries over
@@ -695,6 +774,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   size_t tab = 0;
   if (s->pages.empty()) tab = s->write_strides(n);
   else BB_TRY(write_pages(s, n, &tab));  // may move the table: the launch's pointers are taken below
+  release.queued(st);
   BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
   BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;
@@ -709,13 +789,14 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   BB_CUDA(cudaEventRecord(s->ev_start, st));
   const int rc = launch_xfer_fp8(l, unpack, eb);
   if (rc != 0) return cuda_failed(rc, "launch_xfer_fp8");
-  ++launches_;
+  launches_.fetch_add(1, std::memory_order_relaxed);
   BB_CUDA(cudaEventRecord(s->ev_stop, st));
   BB_CUDA(cudaMemcpyAsync(s->h_res, s->d_digest, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, st));
   // scales: for a put they were just written by the kernel above (same stream), for a get they are read twice
   XferResult sres;
   BB_TRY(run(scale_items, ChecksumAlgo::BBH64, stream, &sres));  // waits for the stream up to here
   BB_CUDA(cudaStreamSynchronize(st));
+  release.settled();
   if (out) {
     const auto* sums = reinterpret_cast<const uint64_t*>(s->h_res);
     out->digest.assign(n, 0);

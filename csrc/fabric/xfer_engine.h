@@ -6,8 +6,10 @@
 // client's per-shard `UcxContext` + endpoint create/destroy + `ucp_put_nbx` + busy-poll
 // (blackbird_client.cpp:204-274, 276-351): zero per-object setup, zero per-object launches.
 #pragma once
+#include <atomic>
 #include <cstdint>
 #include <memory>
+#include <mutex>
 #include <vector>
 
 #include "common/checksum.h"
@@ -82,16 +84,21 @@ struct XferResult {
   float device_ms = 0.f;         // kernel time (CUDA events) of the batch
 };
 
+// One engine may be shared by many host threads: submit, wait, run and run_fp8 may be called concurrently, each thread
+// with its own stream.  A batch holds one slot (pinned and device descriptor table, digest workspace) from submit() to
+// wait(); the setters below are configuration, to be called before the engine is shared.
 class XferEngine {
  public:
-  // `device` is the CUDA ordinal the kernels run on; `max_items` bounds one batch.
+  // `device` is the CUDA ordinal the kernels run on; `max_items` bounds one batch.  `slots` are allocated up front; when
+  // concurrent callers hold all of them, a batch adds one more, up to kMaxSlots.
   static Result<std::unique_ptr<XferEngine>> create(int device, uint32_t max_items = 1u << 16, int slots = 4);
+  static constexpr int kMaxSlots = 64;
   ~XferEngine();
   XferEngine(const XferEngine&) = delete;
   XferEngine& operator=(const XferEngine&) = delete;
 
-  // Enqueues the whole batch on `stream` (cudaStream_t, nullptr = legacy default stream) and
-  // returns a ticket.  Does not block (unless all slots are in flight).
+  // Enqueues the whole batch on `stream` (cudaStream_t, nullptr = legacy default stream) and returns a ticket.  Does not
+  // block.  RESOURCE_EXHAUSTED when kMaxSlots batches are in flight.
   Result<uint64_t> submit(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream,
                           bool capture_debug = false);
   // Blocks until the ticket's batch has finished on the device and fills `out`.
@@ -100,12 +107,13 @@ class XferEngine {
   ErrorCode run(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream, XferResult* out);
   // Fused MXFP8 put (pack = wide -> slab) or get (unpack = slab -> wide): the wide side is read / written once, the
   // E4M3 payload is hashed on the tensor cores while it sits in shared memory, and the digest returned is the
-  // BBH64 of the stored packed object (identical to hashing the output of mxfp8_pack).  Synchronous; needs two free
-  // slots (the fused kernel's batch and the batch that hashes the scales).
+  // BBH64 of the stored packed object (identical to hashing the output of mxfp8_pack).  Synchronous; holds two slots
+  // (the fused kernel's batch and the batch that hashes the scales).
   ErrorCode run_fp8(const std::vector<Fp8Item>& items, bool unpack, void* stream, XferResult* out);
   static bool fp8_eligible(uint64_t n_elems) { return n_elems != 0 && n_elems % 32 == 0; }  // whole MX blocks
 
-  // Raw accumulators of the last capture_debug batch: [total_tiles][128][16] (tests only).
+  // Raw accumulators of the last capture_debug batch: [total_tiles][128][16] (tests only; not to be read while another
+  // thread waits for a capture_debug or traced batch).
   const std::vector<uint32_t>& debug_accumulators() const { return debug_host_; }
   // Diagnostics: when on, every batch records per-tile pipeline timestamps (globaltimer ns):
   // [tile][4] = load issued, landed in shared memory, store issued, slot released.  Read after wait().
@@ -113,8 +121,13 @@ class XferEngine {
   const std::vector<uint64_t>& tile_trace() const { return trace_host_; }
 
   int device() const { return device_; }
-  uint64_t launches() const { return launches_; }  // kernels launched so far
-  uint64_t small_launches() const { return small_launches_; }  // of which warp-per-object launches (xfer_small.cu)
+  uint64_t launches() const { return launches_.load(std::memory_order_relaxed); }  // kernels launched so far
+  // of which warp-per-object launches (xfer_small.cu)
+  uint64_t small_launches() const { return small_launches_.load(std::memory_order_relaxed); }
+  size_t slots() const {  // allocated slots: create()'s, plus those added for concurrent callers
+    std::lock_guard<std::mutex> lk(mu_);
+    return slots_.size();
+  }
   // Batches made only of objects <= kSmallBytes take the warp-per-object kernel (default on; BB_XFER_SMALL=0 disables).
   void set_small_path(bool on) { small_path_ = on; }
   // Small batches (<= kDirectResults objects on the warp path) complete by a flag in pinned memory instead of CUDA
@@ -124,38 +137,50 @@ class XferEngine {
   // warp (xfer_small.cu) instead of being launched: no cudaLaunchKernel in the steady state.  Default on;
   // BB_XFER_MAILBOX=0 disables; BB_MAILBOX_LINGER_US (default 200) = how long the warp waits for the next request.
   void set_mailbox(bool on) { mailbox_on_ = on; }
-  uint64_t mailbox_requests() const { return mailbox_requests_; }   // objects served by the resident warp
-  uint64_t mailbox_launches() const { return mailbox_launches_; }   // incarnations of the mailbox kernel
+  // objects served by the resident warp
+  uint64_t mailbox_requests() const { return mailbox_requests_.load(std::memory_order_relaxed); }
+  // incarnations of the mailbox kernel
+  uint64_t mailbox_launches() const { return mailbox_launches_.load(std::memory_order_relaxed); }
   void set_max_ctas(int n) { max_ctas_ = n; }
-  int last_cuda_error() const { return last_cuda_error_; }
+  int last_cuda_error() const { return last_cuda_error_.load(std::memory_order_relaxed); }
 
  private:
   struct Slot;
+  class SlotHold;
   XferEngine() = default;
-  Slot* free_slot();
+  static Result<std::unique_ptr<Slot>> new_slot(uint32_t max_items);
+  // Takes a free slot, or adds one, and gives it a fresh ticket: from here on no other batch can take it.
+  Result<Slot*> claim_slot();
+  void release_slot(Slot* s);
   ErrorCode write_tile_table(Slot* s, uint32_t nd);
   ErrorCode write_pages(Slot* s, uint32_t nd, size_t* tab);
   ErrorCode cuda_failed(int code, const char* what);
   int device_ = 0;
   uint32_t max_items_ = 0;
+  // Guards the slot table (slots_, every slot's ticket), next_ticket_, the mailbox (mb_) and debug_host_ / trace_host_.
+  // Held only for that bookkeeping (and the mailbox kernel's launch): never across a descriptor-table write, a batch's
+  // launch or a wait.  A claimed slot's other fields belong to the thread that claimed it.
+  mutable std::mutex mu_;
   std::vector<std::unique_ptr<Slot>> slots_;
+  int growing_ = 0;  // slots being allocated outside mu_, counted against kMaxSlots
   uint64_t next_ticket_ = 1;
-  uint64_t launches_ = 0;
-  uint64_t small_launches_ = 0;
+  std::atomic<uint64_t> launches_{0};
+  std::atomic<uint64_t> small_launches_{0};
   bool small_path_ = true;
   bool flag_completion_ = true;
   bool mailbox_on_ = true;
   bool mailbox_enabled();
   struct Mailbox;
   std::unique_ptr<Mailbox> mb_;
+  // mailbox_post and mailbox_launch_locked are called with mu_ held
   ErrorCode mailbox_post(Slot* s, const XferDesc* descs, uint32_t nd, int algo);
   ErrorCode mailbox_wait(Slot* s);
   ErrorCode mailbox_launch_locked(uint32_t first_seq);
-  uint64_t mailbox_requests_ = 0, mailbox_launches_ = 0;
+  std::atomic<uint64_t> mailbox_requests_{0}, mailbox_launches_{0};
   bool small_path_enabled();
   bool flag_completion_enabled();
   int max_ctas_ = 0;
-  int last_cuda_error_ = 0;
+  std::atomic<int> last_cuda_error_{0};
   std::vector<uint32_t> debug_host_;
   bool tile_trace_ = false;
   std::vector<uint64_t> trace_host_;

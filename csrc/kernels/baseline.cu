@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(1024) crc_combine_kernel(uint32_t* arr, uint64
   if (threadIdx.x == 0) *out = arr[0] ^ k.init_term ^ 0xFFFFFFFFu;
 }
 
-bool g_crc_table_init[16] = {false};
+PerDeviceOnce g_crc_table_once;  // c_crc_table upload
 
 }  // namespace
 
@@ -152,12 +152,10 @@ int launch_random_fill(void* dst, uint64_t nbytes, uint64_t seed, void* stream) 
 
 int launch_crc32c_simt(const void* data, uint64_t nbytes, uint32_t* out, uint32_t* scratch, void* stream) {
   int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev >= 0 && dev < 16 && !g_crc_table_init[dev]) {
+  if (const cudaError_t e = current_device(&dev); e != cudaSuccess) return static_cast<int>(e);
+  const cudaError_t e = g_crc_table_once.run(dev, [] {
     uint32_t t[4][256];
     // byte-step tables: T[k][b] = remainder of byte b followed by k zero bytes
-    uint32_t shift1[4][256];
-    (void)shift1;
     for (uint32_t b = 0; b < 256; ++b) {
       uint32_t c = b;
       for (int i = 0; i < 8; ++i) c = (c & 1) ? (c >> 1) ^ 0x82F63B78u : c >> 1;
@@ -165,10 +163,9 @@ int launch_crc32c_simt(const void* data, uint64_t nbytes, uint32_t* out, uint32_
     }
     for (uint32_t b = 0; b < 256; ++b)
       for (int k = 1; k < 4; ++k) t[k][b] = (t[k - 1][b] >> 8) ^ t[0][t[k - 1][b] & 0xFF];
-    cudaError_t e = cudaMemcpyToSymbol(c_crc_table, t, sizeof t);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    g_crc_table_init[dev] = true;
-  }
+    return cudaMemcpyToSymbol(c_crc_table, t, sizeof t);
+  });
+  if (e != cudaSuccess) return static_cast<int>(e);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (nbytes == 0) {
     const uint32_t zero = 0;

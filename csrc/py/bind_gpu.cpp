@@ -240,6 +240,7 @@ void bind_gpu(py::module_& m) {
       .def("set_tile_trace", &XferEngine::set_tile_trace)
       .def("tile_trace", [](XferEngine& e) { return e.tile_trace(); }, "[tile][4] globaltimer ns: load issued, landed, store issued, slot released")
       .def_property_readonly("launches", &XferEngine::launches)
+      .def_property_readonly("slots", &XferEngine::slots, "allocated slots: create()'s, plus those added for concurrent callers")
       .def_property_readonly("device", &XferEngine::device);
 
   m.def("copy_simt", [](uintptr_t dst, uintptr_t src, uint64_t n, uintptr_t stream) {

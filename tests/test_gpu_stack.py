@@ -482,8 +482,8 @@ def test_fused_fp8_put_fans_out_to_replicas_and_get_fails_over(bb, torch_cuda):
             bb.mxfp8_unpack(ref.data_ptr(), n, unp.data_ptr(), s)
             torch.cuda.synchronize()
             assert torch.equal(o.view(torch.int16), unp.view(torch.int16))
-        # all three corrupt -> CHECKSUM_MISMATCH
-        be.write(copies[2].shards[0].offset + 5, b"\xee")
+        # all three corrupt -> CHECKSUM_MISMATCH (a flipped byte: writing a constant leaves a copy intact whose byte holds it)
+        _flip_byte(be, copies[2].shards[0].offset + 5)
         ecs = cl.client.batch_get_device_fp8([keys[1]], [outs[1].data_ptr()], [n], s)
         assert ecs == [bb.ErrorCode.CHECKSUM_MISMATCH]
     finally:

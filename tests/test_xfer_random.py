@@ -664,6 +664,8 @@ def _other_side(rng, side):
 
 
 def fp8_round(bb, eng, seed, rnd):
+    """One fp8 round on the current stream; it waits for that stream only, so test_device_threads.py runs rounds from
+    several threads at once."""
     rng = np.random.default_rng([seed, rnd, 8])
     mx = {"bf16": bb.MxWide.BF16, "f16": bb.MxWide.F16, "f32": bb.MxWide.F32}
     grid = _grid(rng)
@@ -724,11 +726,11 @@ def fp8_round(bb, eng, seed, rnd):
         with pytest.raises(RuntimeError, match="INVALID_ARGUMENT"):
             eng.run_fp8(items[:pos] + [odd] + items[pos:], False, _stream(), wide=mx[types[0]])
         assert (eng.launches, eng.small_launches) == before, f"{where}: a batch of {other} at {pos} among {side} items launched"
-        torch.cuda.synchronize()
+        torch.cuda.current_stream().synchronize()
         assert all(bool((r == GUARD).all()) for r in reps) and bool((odd_out == GUARD).all()), f"{where}: a refused batch wrote bytes"
         SEEN["fp8-rejected"] += 1
     dg, st, _ = eng.run_fp8(items, False, _stream(), wide=mx[types[0]])
-    torch.cuda.synchronize()
+    torch.cuda.current_stream().synchronize()
     SEEN["fp8-pack"] += 1
     assert st == [0] * count, f"{where}: pack status {st}"
     for i, (p, d) in enumerate(zip(packed, dg)):
@@ -797,7 +799,7 @@ def fp8_round(bb, eng, seed, rnd):
         pg_ = None if pages is None else ([optr + gb * int(v) for v in pages[0]], pages[1], pages[2])
         gets.append((optr + gb * at, reps[0].data_ptr() + lay.offs[i], sizes[i], dg[i] ^ int(wrong[i]), win, None, scat, mx[gtypes[i]], None, pg_))
     dg2, st2, _ = eng.run_fp8(gets, True, _stream(), wide=mx[gtypes[0]])
-    torch.cuda.synchronize()
+    torch.cuda.current_stream().synchronize()
     SEEN["fp8-unpack"] += 1
     udesc = [f"{descs[i]}; get as {gtypes[i]}: {plan[i][6]} window={plan[i][1]} scatter={plan[i][2]}" for i in range(count)]
     for i in range(count):
