@@ -32,6 +32,15 @@ PAGED_MIN_PAGE_BYTES = 32 << 10
 # median ms: the paged calls win at 32 KiB pages (put 1.19 vs 1.81, get 1.30 vs 1.76, and no 512 MiB temporary) and at
 # 16 KiB (put 0.96 vs 1.02, get 0.99 vs 1.10), and lose from 8 KiB down (put 0.98 vs 0.80, get 0.92 vs 0.84).
 FP8_PAGED_MIN_PAGE_BYTES = 16 << 10
+# The same for partial restores of packed objects (get_blocks_into with `blocks`), whose alternative route also runs a
+# whole-object index_select.  bench/paged_partial_bench.py, 256 stored blocks of a cache [32, 2, 2048, h, 8, 128] on one
+# H100 80GB HBM3 at 700 W, median ms of the paged unpack vs get + index_select + index_copy_: at 32 KiB pages it wins from
+# k = 128 restored blocks on (bf16 1.16 vs 1.70, fp32 1.24 vs 1.32; k = 256: 1.41 vs 2.61) and is within 0.15 ms at
+# k = 16 (bf16 0.89 vs 0.94, fp32 1.02 vs 0.88); at 16 KiB it loses at k = 16 in every dtype (bf16 1.04 vs 0.81, fp32
+# 1.07 vs 0.78) and for fp32 also at k = 128 (1.27 vs 1.14), so the crossover is 32 KiB, not FP8_PAGED_MIN_PAGE_BYTES.
+# Unpacked partial restores keep PAGED_MIN_PAGE_BYTES: the same run shows them winning at 32 KiB (XXH3 k = 128: 1.30 vs
+# 1.80 ms) and losing at 16 KiB for k = 16 and at 8 KiB and below for every k.
+FP8_PARTIAL_MIN_PAGE_BYTES = 32 << 10
 
 
 def _stored_dtype(m) -> torch.dtype:
@@ -233,24 +242,24 @@ class TensorStore:
         return dim % cache.dim()
 
     @staticmethod
-    def _block_ids(key: str, ids, size: int) -> np.ndarray:
+    def _block_ids(key: str, ids, size: int, what: str = "block ids") -> np.ndarray:
         """`ids` (a list or an integer tensor) as a 1-D int64 numpy array; a CUDA tensor is copied to the host once, which
-        synchronises with its stream.  IndexError for an id outside [0, size)."""
+        synchronises with its stream.  IndexError for an id outside [0, size); `what` names the argument in errors."""
         if isinstance(ids, torch.Tensor):
             if ids.dtype.is_floating_point or ids.dtype.is_complex or ids.dtype == torch.bool:
-                raise TypeError(f"{key}: ids must be a 1-D integer list or tensor")
+                raise TypeError(f"{key}: {what} must be a 1-D integer list or tensor")
             a = ids.to(device="cpu", dtype=torch.int64).numpy()
         else:
             a = np.asarray(list(ids))
             if a.size == 0:
                 a = a.astype(np.int64)
             if a.dtype.kind not in "iu":
-                raise TypeError(f"{key}: ids must be a 1-D integer list or tensor")
+                raise TypeError(f"{key}: {what} must be a 1-D integer list or tensor")
             a = a.astype(np.int64)
         if a.ndim != 1:
-            raise TypeError(f"{key}: ids must be a 1-D integer list or tensor")
+            raise TypeError(f"{key}: {what} must be a 1-D integer list or tensor")
         if a.size and (a.min() < 0 or a.max() >= size):
-            raise IndexError(f"{key}: block ids must lie in [0, {size})")
+            raise IndexError(f"{key}: {what} must lie in [0, {size})")
         return a
 
     @staticmethod
@@ -351,44 +360,87 @@ class TensorStore:
         """Stores `cache.index_select(dim, ids)` under `key` (see batch_put_blocks)."""
         self.batch_put_blocks([key], [cache], [ids], dim, pack_fp8, config)
 
-    def batch_get_blocks_into(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0) -> list:
+    @staticmethod
+    def _sparse_table(addrs: np.ndarray, blocks: np.ndarray, n_stored: int) -> np.ndarray:
+        """The page table over the whole stored object of a partial restore: `addrs` are the pages of the cache blocks the
+        selected stored blocks land in (_block_pages, outer index major, blocks.size per outer index), placed at those
+        blocks' positions among the n_stored blocks per outer index; every other entry is 0, a page the get does not
+        store."""
+        table = np.zeros((addrs.size // blocks.size, n_stored), dtype=np.int64)
+        table[:, blocks] = addrs.reshape(-1, blocks.size)
+        return table.reshape(-1)
+
+    def batch_get_blocks_into(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0,
+                              blocks: Optional[Sequence] = None) -> list:
         """`caches[i].index_copy_(dim, ids[i], stored)` for the tensor stored under keys[i]: restores a request's KV blocks
         into whatever free blocks the allocator handed out.  No element of a cache outside the selected blocks is written.
         Returns `caches`.
 
-        Every check comes before any transfer: KeyError for a missing key, TypeError unless the cache dtype is the stored
-        dtype, ValueError unless the stored shape is the index_select shape, for a cache that is not a CUDA tensor on the
-        current device and for duplicate ids, IndexError for an id or a dim out of range.  Caches of the layout
-        batch_put_blocks reads in place take the paged get (batch_get_device_paged), which stores each tile straight into
-        its pages (RuntimeError unless the stored object fills every selected block); packed whole-block tensors with
-        pages of at least FP8_PAGED_MIN_PAGE_BYTES take the paged unpack (batch_get_device_fp8_paged), which unpacks each
-        tile straight into its pages.  Other layouts, padded packed tensors, and packed objects the fused kernel refuses
-        (NOT_IMPLEMENTED: an unfusable placement) take a get followed by index_copy_.  A CUDA `ids` tensor is copied to
-        the host once, which synchronises."""
+        With `blocks`, only some stored blocks are restored: `caches[i].index_copy_(dim, ids[i], stored.index_select(dim,
+        blocks[i]))`, blocks[i] indexing the stored tensor's `dim` -- a new request reusing the first k blocks of a stored
+        prefix (blocks=range(k)), or the evicted blocks of a request refilled while the rest stay resident.  blocks=None is
+        every stored block in order.
+
+        Every check comes before any transfer, so a cache is untouched after an error: KeyError for a missing key,
+        TypeError unless the cache dtype is the stored dtype or for ids or blocks that are not integers, ValueError unless
+        the stored shape is the index_select shape (with blocks: unless it equals the cache shape outside `dim` and
+        len(blocks[i]) == len(ids[i])), for a cache that is not a CUDA tensor on the current device and for duplicate ids
+        or blocks, IndexError for an id, a block or a dim out of range.  An empty selection with blocks moves nothing.
+
+        Caches of the layout batch_put_blocks reads in place take the paged get (batch_get_device_paged), which stores
+        each tile straight into its pages (RuntimeError unless the stored object fills the table); packed whole-block
+        tensors with pages of at least FP8_PAGED_MIN_PAGE_BYTES (FP8_PARTIAL_MIN_PAGE_BYTES with blocks) take the paged
+        unpack (batch_get_device_fp8_paged), which unpacks each tile straight into its pages.  With blocks, the table covers the whole stored object and the pages of
+        the stored blocks not selected are 0 (not stored): the whole object is still read and verified, but there is no
+        temporary and no index_select.  Other layouts, padded packed tensors, and packed objects the fused kernel refuses
+        (NOT_IMPLEMENTED: an unfusable placement) take a get followed by index_select and index_copy_.  CUDA `ids` or
+        `blocks` tensors are copied to the host once, which synchronises."""
         keys, caches, ids = list(keys), list(caches), list(ids)
         if not len(keys) == len(caches) == len(ids):
             raise ValueError("keys, caches and ids differ in length")
+        if blocks is not None:
+            blocks = list(blocks)
+            if len(blocks) != len(keys):
+                raise ValueError("keys and blocks differ in length")
         metas = self._metas(keys)
         dev = torch.cuda.current_device()
         dims = [self._block_dim(k, c, dim) for k, c in zip(keys, caches)]
-        idx = []
-        for k, m, c, b, d in zip(keys, metas, caches, ids, dims):
+        idx, sel = [], []  # sel[i]: the selected stored blocks, None for all of them
+        for j, (k, m, c, b, d) in enumerate(zip(keys, metas, caches, ids, dims)):
             if c.dtype != _stored_dtype(m):
                 raise TypeError(f"{k}: cache is {c.dtype}, the stored tensor {_stored_dtype(m)}")
             t = self._block_ids(k, b, c.shape[d])
-            shape = list(c.shape)
-            shape[d] = t.size
-            if shape != m["shape"]:
-                raise ValueError(f"{k}: the stored tensor has shape {m['shape']}, the selected blocks {shape}")
+            s = None
+            if blocks is None:
+                shape = list(c.shape)
+                shape[d] = t.size
+                if shape != m["shape"]:
+                    raise ValueError(f"{k}: the stored tensor has shape {m['shape']}, the selected blocks {shape}")
+            else:
+                stored = m["shape"]
+                if len(stored) != c.dim() or any(a != n for e, (a, n) in enumerate(zip(stored, c.shape)) if e != d):
+                    raise ValueError(f"{k}: the stored tensor has shape {stored}, the cache {list(c.shape)}: they differ outside dim {d}")
+                s = self._block_ids(k, blocks[j], stored[d], "blocks")
+                if s.size != t.size:
+                    raise ValueError(f"{k}: {s.size} blocks for {t.size} ids")
             if not c.is_cuda or c.device.index != dev:
                 raise ValueError(f"{k}: cache must be a CUDA tensor on cuda:{dev}, not {c.device}")
             if np.unique(t).size != t.size:
                 raise ValueError(f"{k}: duplicate block ids")
+            if s is not None and np.unique(s).size != s.size:
+                raise ValueError(f"{k}: duplicate blocks")
             idx.append(t)
+            sel.append(s)
+        live = [i for i in range(len(keys)) if sel[i] is None or sel[i].size]  # an empty selection moves nothing
         # packed whole-block objects take the paged unpack; padded ones cannot fill whole pages
         fp8 = [self._fp8_whole(m) for m in metas]
-        pages = [self._block_pages(c, d, b, FP8_PAGED_MIN_PAGE_BYTES if f else PAGED_MIN_PAGE_BYTES) if f or not m["packed"] else None
-                 for m, f, c, d, b in zip(metas, fp8, caches, dims, idx)]
+        pages = [None] * len(keys)
+        for i in live:
+            if fp8[i] or not metas[i]["packed"]:
+                fp8_min = FP8_PAGED_MIN_PAGE_BYTES if sel[i] is None else FP8_PARTIAL_MIN_PAGE_BYTES
+                pages[i] = self._block_pages(caches[i], dims[i], idx[i], fp8_min if fp8[i] else PAGED_MIN_PAGE_BYTES)
+            if pages[i] is not None and sel[i] is not None:
+                pages[i] = (self._sparse_table(pages[i][0], sel[i], metas[i]["shape"][dims[i]]), pages[i][1])
 
         def call(grp, es, wide):
             return self.client.batch_get_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
@@ -400,18 +452,24 @@ class TensorStore:
         if paged:
             ecs, sizes = self.client.batch_get_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged],
                                                             [pages[i][1] for i in paged], self._stream())
-            # the stored object must fill every page: a shorter one would leave the last blocks as they were; those are
+            # the stored object must fill the table: a shorter one would leave the last blocks as they were; those are
             # named after the items that failed
             short = [f"{n} bytes stored, {pages[i][0].size * pages[i][1]} selected" if e == _bb.ErrorCode.OK and n != pages[i][0].size * pages[i][1]
                      else _bb.ErrorCode.OK for i, e, n in zip(paged, ecs, sizes)]
             _check("paged get", [keys[i] for i in paged] * 2, list(ecs) + short)
-        self._whole(keys, [i for i, p in enumerate(pages) if p is None], None,
-                    lambda i, t: caches[i].index_copy_(dims[i], torch.from_numpy(idx[i]).to(caches[i].device), t))
+
+        def restore(i, t):
+            if sel[i] is not None:
+                t = t.index_select(dims[i], torch.from_numpy(sel[i]).to(t.device))
+            caches[i].index_copy_(dims[i], torch.from_numpy(idx[i]).to(caches[i].device), t)
+
+        self._whole(keys, [i for i in live if pages[i] is None], None, restore)
         return caches
 
-    def get_blocks_into(self, key: str, cache: torch.Tensor, ids, dim: int = 0) -> torch.Tensor:
-        """`cache.index_copy_(dim, ids, stored)` for the tensor stored under `key` (see batch_get_blocks_into)."""
-        return self.batch_get_blocks_into([key], [cache], [ids], dim)[0]
+    def get_blocks_into(self, key: str, cache: torch.Tensor, ids, dim: int = 0, blocks=None) -> torch.Tensor:
+        """`cache.index_copy_(dim, ids, stored)`, or with `blocks` `cache.index_copy_(dim, ids, stored.index_select(dim,
+        blocks))`, for the tensor stored under `key` (see batch_get_blocks_into)."""
+        return self.batch_get_blocks_into([key], [cache], [ids], dim, None if blocks is None else [blocks])[0]
 
     # ------------------------------------------------------------------ get
     def _metas(self, keys: Sequence[str]) -> list:
@@ -713,11 +771,13 @@ class AsyncTensorStore(TensorStore):
         keys = list(keys)
         return self._on_side(True, self.batch_put_blocks, keys, list(caches), list(ids), dim, pack_fp8, config, result=len(keys))
 
-    def get_blocks_into_async(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0):
-        """batch_get_blocks_into on the side stream, ordered after the work already queued on the caller's stream; the
-        future yields `caches`, already synchronised with the side stream."""
+    def get_blocks_into_async(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0,
+                              blocks: Optional[Sequence] = None):
+        """batch_get_blocks_into (with `blocks`, a partial restore) on the side stream, ordered after the work already
+        queued on the caller's stream; the future yields `caches`, already synchronised with the side stream."""
         caches = list(caches)
-        return self._on_side(True, self.batch_get_blocks_into, list(keys), caches, list(ids), dim, result=caches)
+        return self._on_side(True, self.batch_get_blocks_into, list(keys), caches, list(ids), dim,
+                             None if blocks is None else list(blocks), result=caches)
 
     def close(self):
         self._pool.shutdown(wait=True)

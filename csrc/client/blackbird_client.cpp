@@ -715,6 +715,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_paged(const std::ve
         const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &mems[i], &elems[i]);
         if (ec != ErrorCode::OK) return ec;
         if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks
+        if (!mems[i].valid_source(elems[i])) return ErrorCode::INVALID_ARGUMENT;  // a null page: a put reads every element
         DeviceLayout bytes;
         if (elems[i] > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
         *wide_bytes = b * elems[i];
@@ -1175,6 +1176,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector
       [&](size_t i, uint64_t* size) {
         const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &mems[i], size);
         if (ec != ErrorCode::OK) return ec;
+        if (!mems[i].valid_source(*size)) return ErrorCode::INVALID_ARGUMENT;  // a null page: a put reads every byte
         if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
         sizes[i] = static_cast<size_t>(*size);
         return ErrorCode::OK;
@@ -1747,7 +1749,7 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
     const auto* src = static_cast<const uint8_t*>(op.src(dev_ptrs[op.item]));
     std::vector<uint8_t> dense;
     if (!op.mem.contiguous()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows or pages
-      if (!op.mem.valid(op.placement->length)) return ErrorCode::INVALID_ARGUMENT;
+      if (!op.mem.valid_source(op.placement->length)) return ErrorCode::INVALID_ARGUMENT;
       dense.resize(op.placement->length);
       copy_from_device(dense.data(), src, op.mem, dense.size(), nullptr);
       src = dense.data();
@@ -1821,7 +1823,7 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
     std::vector<uint8_t> dense;
     if (!op.mem.contiguous()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows or pages
       DeviceLayout b;
-      if (!op.win.whole() || !op.mem.valid(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+      if (!op.win.whole() || !op.mem.valid_source(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
       dense.resize(eb * op.n_elems);
       copy_from_device(dense.data(), op.wide, b, dense.size(), nullptr);

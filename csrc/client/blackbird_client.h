@@ -112,7 +112,8 @@ class DeviceTransport {
   virtual ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) { return ErrorCode::NOT_IMPLEMENTED; }
   virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
   // Staging copies for objects (or shards) that live on host tiers, synchronous: object bytes [0, n) laid out by `layout`
-  // at `base` (common/store_window.h) from / to n bytes packed back to back at `host`.
+  // at `base` (common/store_window.h) from / to n bytes packed back to back at `host`.  copy_to_device skips null pages;
+  // copy_from_device refuses them (INVALID_ARGUMENT).
   virtual ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
     return ErrorCode::NOT_IMPLEMENTED;
   }
@@ -218,13 +219,16 @@ class BlackbirdClient {
   // or an element count that is not a positive whole number of MX blocks; VALUE_OUT_OF_RANGE when the count or its wide
   // bytes overflow; NOT_IMPLEMENTED unless the table is co-aligned in wide bytes (every page 16-byte aligned and, for
   // several pages, page_elems[i] % 8 == 0) -- there is no host-staged path; the rest of the batch keeps its launch.
+  // INVALID_ARGUMENT, also before anything is allocated, for a zero page address: a put reads every page.
   std::vector<ErrorCode> batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                     const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
                                                     mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Gets of packed tensors into pages, the mirror: object i is unpacked into the pages pages[i] of page_elems[i] elements,
   // element x in page x / page_elems[i] at element x % page_elems[i], by the paged scattering store of the fused unpack.
-  // Only the object's elements are written; pages of one get must not overlap (not checked).  Fail-over and the placement
-  // refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT for page_elems[i] == 0 with pages, or unless the
+  // Only the object's elements are written; pages of one get must not overlap (not checked).  A zero page address is a
+  // page that is not stored (SourcePages' null page): a partial restore names only the pages it wants and leaves the
+  // others 0.  The table still covers the whole object, which is still read whole and verified, so a corrupt copy fails
+  // over even when no page is stored.  Fail-over and the placement refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT for page_elems[i] == 0 with pages, or unless the
   // stored object holds exactly pages[i].size() * page_elems[i] elements (a positive whole number of MX blocks);
   // VALUE_OUT_OF_RANGE when that count or its wide bytes overflow; NOT_IMPLEMENTED when the object is not fusable (as
   // batch_get_device_fp8) or the pages fail SourcePages::fused_get_aligned in wide bytes -- there is no host-staged path;
@@ -303,14 +307,16 @@ class BlackbirdClient {
   // the put kernel; it needs every shard of every copy co-aligned (SourcePages::coaligned: 16-byte aligned pages and shard starts and, for
   // several pages, page_bytes[i] % 16 == 0).  Any other item, and every placement the fabric cannot reach, is staged
   // through the host (one D2H copy per run of pages) while the rest of the batch keeps the fused launch.  Per object,
-  // before anything is allocated: INVALID_ARGUMENT for page_bytes[i] == 0 with pages; VALUE_OUT_OF_RANGE when the size
-  // overflows.  No pages is a zero-byte object.
+  // before anything is allocated: INVALID_ARGUMENT for page_bytes[i] == 0 with pages or for a zero page address (a put
+  // reads every page); VALUE_OUT_OF_RANGE when the size overflows.  No pages is a zero-byte object.
   std::vector<ErrorCode> batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                 const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream);
   // Paged gets, the mirror: object i lands in the pages pages[i] of page_bytes[i] bytes, object byte x in page
   // x / page_bytes[i] at offset x % page_bytes[i].  The capacity is pages[i].size() * page_bytes[i]: a larger object is
   // BUFFER_OVERFLOW, a shorter one fills its bytes in page order; out_sizes[i] receives the size.  Only the object's bytes
-  // are written.  Pages of one get must not overlap (not checked).  Every shard is read whole and verified, with the
+  // are written.  Pages of one get must not overlap (not checked).  A zero page address is a page that is not stored
+  // (SourcePages' null page): a partial restore names only the pages it wants and leaves the others 0; the capacity and
+  // out_sizes rules do not change.  Every shard is read whole and verified, stored pages or not, with the
   // fail-over and placement refresh of batch_get_device.  The fused path scatters the pages in the get kernel; it needs
   // SourcePages::fused_get_aligned for every shard of every copy.  Any other item, and every placement the fabric cannot
   // reach, is staged through the host (one H2D copy per run of pages).  Per object: INVALID_ARGUMENT for
@@ -419,6 +425,7 @@ class HostLoopbackTransport : public DeviceTransport {
   bool can_reach(const ShardPlacement& s) const override;
   uint64_t launches() const override { return launches_; }
   ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void*) override {
+    if (!layout.valid_source(n)) return ErrorCode::INVALID_ARGUMENT;
     layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
       std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(addr), len);
     });

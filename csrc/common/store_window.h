@@ -259,6 +259,12 @@ struct SourceRows {
 // XFER_PAGED descriptors (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.  The unit of `page` and
 // `phase` is a byte, or for an MXFP8 transfer an element of the wide side (to_wide_bytes() turns elements into bytes);
 // the addresses are byte addresses either way.
+//
+// An address of 0 is a null page: on the get side, the object bytes that fall in it are not stored (a partial restore
+// into some of a cache's blocks).  No CUDA allocation or host buffer lives at address 0, so the marker cannot collide
+// with a real page.  Null pages start and extend no run (for_each_run) and are exempt from the alignment rules
+// (coaligned, fused_get_aligned); the table still covers the whole object.  A put must read every byte, so its table may
+// hold no null page (has_null, DeviceLayout::valid_source).
 struct SourcePages {
   const uint64_t* addrs = nullptr;
   uint64_t npages = 0, page = 0, phase = 0;
@@ -276,6 +282,13 @@ struct SourcePages {
   uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
   // Whether the table holds every page of an object of `len` bytes, with phase < page.
   bool valid(uint64_t len) const { return paged() && phase < page && pages_for(len) <= npages; }
+  // Whether a page that object bytes [0, len) touch is null.
+  bool has_null(uint64_t len) const {
+    const uint64_t n = pages_for(len);
+    for (uint64_t k = 0; k < n; ++k)
+      if (addrs[k] == 0) return true;
+    return false;
+  }
 
   // The table of `npages` pages of `page` bytes at addrs: an object of *size = npages * page bytes.  INVALID_ARGUMENT for
   // page == 0 with pages; VALUE_OUT_OF_RANGE when the product overflows.  No pages is a zero-byte object (no table).
@@ -299,13 +312,13 @@ struct SourcePages {
 
   // Whether object bytes [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by
   // TMA: byte x of page k lives at addrs[k] + phase - k * page + x, so addrs[k] + phase must be 16-byte aligned for every
-  // page touched, and the page a multiple of 16 bytes when more than one page is touched.  (With phase % 16 == 0, as for
-  // a table cut at 16-byte shard starts, that is every page 16-byte aligned.)
+  // non-null page touched, and the page a multiple of 16 bytes when more than one page is touched.  (With phase % 16 == 0,
+  // as for a table cut at 16-byte shard starts, that is every page 16-byte aligned.)
   bool coaligned(uint64_t len) const {
     const uint64_t n = pages_for(len);
     if (n > 1 && page % 16) return false;
     for (uint64_t k = 0; k < n; ++k)
-      if ((addrs[k] + phase) % 16) return false;
+      if (addrs[k] != 0 && (addrs[k] + phase) % 16) return false;
     return true;
   }
 
@@ -320,13 +333,17 @@ struct SourcePages {
   }
 
   // Calls f(x, addr, n) for every run of n contiguous bytes of object bytes [0, len): object bytes [x, x + n) live at
-  // [addr, addr + n), in order.  Pages that follow one another in memory make one run.
+  // [addr, addr + n), in order.  Pages that follow one another in memory make one run; null pages make none and end the
+  // run before them.
   template <class F>
   void for_each_run(uint64_t len, F&& f) const {
     uint64_t x = 0, run_x = 0, run_at = 0, run_n = 0;
     for (uint64_t k = 0; x < len; ++k) {
       const uint64_t c = k == 0 ? phase : 0, n = std::min(page - c, len - x), at = addrs[k] + c;
-      if (run_n && run_at + run_n == at) {
+      if (addrs[k] == 0) {
+        if (run_n) f(run_x, run_at, run_n);
+        run_n = 0;
+      } else if (run_n && run_at + run_n == at) {
         run_n += n;
       } else {
         if (run_n) f(run_x, run_at, run_n);
@@ -376,6 +393,8 @@ class DeviceLayout {
   bool valid(uint64_t len) const {
     return kind_ == ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : true;
   }
+  // The same for a put's source, which must read every unit: valid(len), and no null page.
+  bool valid_source(uint64_t len) const { return valid(len) && !(kind_ == PAGES && pages_.has_null(len)); }
 
   // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
   // when the byte arithmetic could overflow.

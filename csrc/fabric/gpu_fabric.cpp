@@ -507,7 +507,7 @@ Result<void*> GpuFabric::resolve(const ShardPlacement& s) {
 }
 
 ErrorCode GpuFabric::copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
-  if (!layout.valid(n)) return ErrorCode::INVALID_ARGUMENT;
+  if (!layout.valid_source(n)) return ErrorCode::INVALID_ARGUMENT;  // every byte is read: no null page
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
   const bool rows = layout.kind() == DeviceLayout::ROWS;

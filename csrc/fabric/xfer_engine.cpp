@@ -449,7 +449,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       return ErrorCode::INVALID_ARGUMENT;
     // a layout is the gathering load's source or the scattering store's destination, the side its flag names
     if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES) ||
-        !it.mem.valid(it.nbytes) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
+        !(gather ? it.mem.valid_source(it.nbytes) : it.mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
         (scatter && (it.ndst != 1 || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
@@ -722,7 +722,8 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       return ErrorCode::INVALID_ARGUMENT;
     if (mxfp8::wide_bytes(it.wide_type) != eb) return ErrorCode::INVALID_ARGUMENT;  // mixes 2- and 4-byte wide types
     DeviceLayout mem;  // a gathered put's source, or a scattered get's destination, in wide bytes; never with a window
-    if (shaped && (!it.win.whole() || !it.mem.valid(it.n_elems) || !it.mem.to_wide_bytes(eb, &mem))) return ErrorCode::INVALID_ARGUMENT;
+    if (shaped && (!it.win.whole() || !(unpack ? it.mem.valid(it.n_elems) : it.mem.valid_source(it.n_elems)) || !it.mem.to_wide_bytes(eb, &mem)))
+      return ErrorCode::INVALID_ARGUMENT;
     // a strided window's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
     // first element after row 0's start): the window is checked instead, below
     if ((reinterpret_cast<uintptr_t>(it.packed) & 15) || (!strided && !mem.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))

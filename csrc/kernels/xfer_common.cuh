@@ -164,9 +164,12 @@ __device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t
 }
 // The same for a paged descriptor (XFER_PAGED, entry {pages, page, phase}): row r of the dense layout is page r, which
 // starts at pages[r], so tile byte o of it sits at pages[r] + off + phase - r * page + o.  `base` is ignored.
+__device__ __forceinline__ uint64_t page_entry(const XferStride& st, uint64_t r) {
+  return __ldg(reinterpret_cast<const unsigned long long*>(st.pages) + r);
+}
 template <bool PAGED>
 __device__ __forceinline__ uint64_t row_addr(uint64_t base, uint64_t off, uint64_t r, const XferStride& st) {
-  if constexpr (PAGED) return __ldg(reinterpret_cast<const unsigned long long*>(st.pages) + r) + off + st.phase - r * st.width;
+  if constexpr (PAGED) return page_entry(st, r) + off + st.phase - r * st.width;
   else return row_src(base, off, r, st);
 }
 // The producer's part of a gathered tile: the row segments of the tile, one per lane, the middle bulk-loaded into `tile`
@@ -192,11 +195,13 @@ __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t*
 // tile's `bytes` object bytes from `off`, in the object's dense layout {width, width, phase}, one row segment per lane,
 // each stored at row_src(dst0, ...) as a TMA middle plus a byte-wise head and tail.  dst0 is the descriptor's dst[0], where
 // the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.  PAGED: the rows are
-// the pages of an XFER_PAGED descriptor (row_addr), dst0 is not read.
+// the pages of an XFER_PAGED descriptor (row_addr), dst0 is not read, and a page whose entry is 0 is not stored (the null
+// page of SourcePages): its lane stores nothing and still commits its empty bulk group.
 template <bool PAGED = false>
 __device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t bytes,
                                                      const XferStride& st, uint32_t lane) {
   for_row_segments(off, 0, bytes, XferStride{{st.width}, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    if (PAGED && page_entry(st, r) == 0) return;
     store_segment(reinterpret_cast<uint8_t*>(row_addr<PAGED>(dst0, off, r, st)), tile, g);
   });
 }

@@ -418,6 +418,8 @@ void bind_control(py::module_& m) {
       .def_property_readonly("addrs", [](const PyPages& t) { return std::vector<uint64_t>(t.p.addrs, t.p.addrs + t.p.npages); })
       .def("paged", [](const PyPages& t) { return t.p.paged(); })
       .def("valid", [](const PyPages& t, uint64_t len) { return t.p.valid(len); }, py::arg("len"))
+      .def("has_null", [](const PyPages& t, uint64_t len) { return t.p.has_null(len); }, py::arg("len"),
+           "whether a page that object bytes [0, len) touch has address 0 (not stored by a get, refused by a put)")
       .def_static("from_pages",
                   [](const py::handle& addrs, uint64_t page) {
                     auto v = std::make_shared<const std::vector<uint64_t>>(to_page_addrs(addrs));
@@ -1383,7 +1385,7 @@ void bind_control(py::module_& m) {
       }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
          "Object i = the len(pages[i]) pages of page_bytes[i] bytes at the device addresses pages[i] (each a 1-D integer "
          "array-like: list, numpy array or CPU tensor), concatenated in order; stored as a put of the concatenation would "
-         "store it; returns one ErrorCode per object.")
+         "store it; a zero page address is INVALID_ARGUMENT for that object; returns one ErrorCode per object.")
       .def("batch_get_device_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
                                         const std::vector<uint64_t>& page_bytes, uintptr_t stream) {
         const auto lists = to_page_lists(pages);
@@ -1392,8 +1394,9 @@ void bind_control(py::module_& m) {
         return py::make_tuple(ecs_to_py(ecs), sizes);
       }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("stream") = 0,
          "Object i into the pages pages[i] of page_bytes[i] bytes, byte x in page x // page_bytes[i] (capacity len(pages[i]) "
-         "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; pages of one get "
-         "must not overlap (not checked); returns (one ErrorCode per object, object sizes).")
+         "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; a page address "
+         "of 0 is not stored (a partial restore: the table still covers the whole object); pages of one get must not "
+         "overlap (not checked); returns (one ErrorCode per object, object sizes).")
       .def("batch_put_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
                                             const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, uintptr_t stream,
                                             mxfp8::Wide wide) {
@@ -1403,8 +1406,8 @@ void bind_control(py::module_& m) {
          py::arg("wide") = mxfp8::Wide::BF16,
          "Packed tensor i = the len(pages[i]) pages of page_elems[i] elements of type `wide` at the device addresses pages[i] "
          "(each a 1-D integer array-like), concatenated in order; packed in the put kernel and stored as "
-         "batch_put_device_fp8 of the concatenation would store it; returns one ErrorCode per object (NOT_IMPLEMENTED: "
-         "gather the pages and put that).")
+         "batch_put_device_fp8 of the concatenation would store it; a zero page address is INVALID_ARGUMENT for that "
+         "object; returns one ErrorCode per object (NOT_IMPLEMENTED: gather the pages and put that).")
       .def("batch_get_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
                                             const std::vector<uint64_t>& page_elems, uintptr_t stream, mxfp8::Wide wide) {
         const auto lists = to_page_lists(pages);
@@ -1412,8 +1415,8 @@ void bind_control(py::module_& m) {
       }, py::arg("keys"), py::arg("pages"), py::arg("page_elems"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
          "Packed tensor i, which must hold len(pages[i]) * page_elems[i] elements, unpacked to type `wide` into the pages "
          "pages[i] of page_elems[i] elements, element x in page x // page_elems[i]; the whole packed object is read and "
-         "verified, only its elements are written; returns one ErrorCode per object (NOT_IMPLEMENTED: get it whole and "
-         "copy).")
+         "verified, only its elements are written; a page address of 0 is not stored (a partial restore); returns one "
+         "ErrorCode per object (NOT_IMPLEMENTED: get it whole and copy).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)
