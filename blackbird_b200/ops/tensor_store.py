@@ -41,6 +41,18 @@ FP8_PAGED_MIN_PAGE_BYTES = 16 << 10
 # Unpacked partial restores keep PAGED_MIN_PAGE_BYTES: the same run shows them winning at 32 KiB (XXH3 k = 128: 1.30 vs
 # 1.80 ms) and losing at 16 KiB for k = 16 and at 8 KiB and below for every k.
 FP8_PARTIAL_MIN_PAGE_BYTES = 32 << 10
+# Smallest page that put_layer_blocks / get_layer_blocks_into move with block ids that stay on the device
+# (batch_put_device_blocks / batch_get_device_blocks); smaller pages take index_select + stack + put and get +
+# index_copy_.  bench/layer_blocks_bench.py, 32 per-layer bf16 caches [2, 2048, h, 8, 128] with 256 blocks selected, on
+# one H100 80GB HBM3 at 700 W, two runs: the device route beats index_select + stack + put / get + index_copy_ at every
+# page size measured, 32, 16, 8 and 4 KiB, with XXH3 and without a checksum (4 KiB put 0.80-0.86 vs 1.49-2.24 ms
+# median, get 0.86-1.00 vs 1.47-1.70).  Smaller pages were not measured, so they keep the other route.  DESIGN.md
+# section 5 has the numbers.
+LAYER_BLOCKS_MIN_PAGE_BYTES = 4 << 10
+# The same for packed (MXFP8) objects (batch_put_device_fp8_blocks / batch_get_device_fp8_blocks), whose other route runs
+# the pack or unpack kernel as well.  The same benchmark, packed bf16 (every page size) and fp16 / fp32 (32 KiB): the
+# device route wins everywhere measured too (bf16 4 KiB put 0.78-0.95 vs 1.83-2.03 ms, get 0.95-0.97 vs 1.59-1.74).
+FP8_LAYER_BLOCKS_MIN_PAGE_BYTES = 4 << 10
 
 
 def _stored_dtype(m) -> torch.dtype:
@@ -471,6 +483,247 @@ class TensorStore:
         blocks))`, for the tensor stored under `key` (see batch_get_blocks_into)."""
         return self.batch_get_blocks_into([key], [cache], [ids], dim, None if blocks is None else [blocks])[0]
 
+    # ------------------------------------------------------------------ blocks of per-layer caches, ids on the device
+    @staticmethod
+    def _layers(key: str, caches) -> tuple:
+        """(list of caches, stacked): one tensor, or a list of same-shape, same-dtype tensors on one device (one per layer,
+        stacked along a new dim 0).  ValueError otherwise."""
+        if isinstance(caches, torch.Tensor):
+            return [caches], False
+        caches = list(caches)
+        if not caches or any(c.shape != caches[0].shape or c.dtype != caches[0].dtype or c.device != caches[0].device for c in caches):
+            raise ValueError(f"{key}: caches must be one tensor or a non-empty list of same-shape, same-dtype tensors on one device")
+        return caches, True
+
+    @staticmethod
+    def _device_ids(t, device) -> bool:
+        """Whether `t` is a 1-D CUDA int32 or int64 tensor on `device`: ids the device route reads where they are."""
+        return isinstance(t, torch.Tensor) and t.is_cuda and t.device == device and t.dim() == 1 and t.dtype in (torch.int32, torch.int64)
+
+    def _device_blocks(self, layers: list, dim: int, ids: torch.Tensor, sel: Optional[torch.Tensor], n_stored: int, packed: bool = False):
+        """The DeviceBlocks of `layers` (index_select(dim, ids) of each, layer-major), with the id tensors it points to, or
+        None when the device route should not move them: the layout batch_put_blocks reads in place, pages of at least
+        LAYER_BLOCKS_MIN_PAGE_BYTES (FP8_LAYER_BLOCKS_MIN_PAGE_BYTES when `packed`, whose pages are then counted in
+        elements), a block stride of a multiple of 16 bytes, and layers that do not overlap one another (a get into
+        aliased layers would store two blocks into one page at once; the fallback's per-layer index_copy_ is ordered).
+        The slice addresses are computed from the shapes and strides alone; the ids are never read here."""
+        if ids.numel() == 0:
+            return None
+        # the layers share shape and dtype; those that share strides too differ only in their base address
+        es = layers[0].element_size()
+        first = self._block_pages(layers[0], dim, np.zeros(1, dtype=np.int64), FP8_LAYER_BLOCKS_MIN_PAGE_BYTES if packed else LAYER_BLOCKS_MIN_PAGE_BYTES)
+        stride = layers[0].stride(dim) * es
+        if first is None or stride % 16 or any(c.stride() != layers[0].stride() or c.data_ptr() % 16 for c in layers):
+            return None
+        extent = (1 + sum((n - 1) * st for n, st in zip(layers[0].shape, layers[0].stride()))) * es
+        starts = sorted(c.data_ptr() for c in layers)
+        if any(a + extent > b for a, b in zip(starts, starts[1:])):
+            return None
+        base = layers[0].data_ptr()
+        pages = [(first[0] + (c.data_ptr() - base), first[1]) for c in layers]
+        wide = ids.dtype == torch.int64 or (sel is not None and sel.dtype == torch.int64)
+        dt = torch.int64 if wide else torch.int32
+        ids = ids.to(dt).contiguous()
+        sel = None if sel is None else sel.to(dt).contiguous()
+        outer = np.concatenate([p[0] for p in pages])
+        page = pages[0][1] // es if packed else pages[0][1]
+        b = _bb.DeviceBlocks(outer, ids.data_ptr(), ids.numel(), layers[0].shape[dim], stride, page, id_bytes=dt.itemsize,
+                             sel=0 if sel is None else sel.data_ptr(), n_stored=n_stored if sel is not None else 0)
+        return b, (ids, sel)
+
+    @staticmethod
+    def _verdicts(keys: list, items: list, ecs: list) -> None:
+        """Raises for the items the device refused on their ids: IndexError for an id or block out of range, ValueError for
+        a repeated one (a get's); RuntimeError for any other code but OK."""
+        for i, e in zip(items, ecs):
+            if e == _bb.ErrorCode.VALUE_OUT_OF_RANGE:
+                raise IndexError(f"{keys[i]}: block ids or blocks out of range")
+            if e == _bb.ErrorCode.INVALID_ARGUMENT:
+                raise ValueError(f"{keys[i]}: duplicate block ids or blocks")
+        _check("layer blocks transfer", [keys[i] for i in items], ecs)
+
+    def batch_put_layer_blocks(self, keys: Sequence[str], caches: Sequence, ids: Sequence, dim: int = 0, pack_fp8: bool = False,
+                               config=None) -> None:
+        """Stores `torch.stack([c.index_select(dim, ids[i]) for c in caches[i]])` under keys[i] -- one object for a
+        request's blocks in every layer of an engine that keeps one KV tensor per layer -- with the usual `#meta`, so get,
+        get_rows, get_slice, and get_blocks_into on a stacked cache read it unchanged.  caches[i] may also be a single
+        tensor, stored as `index_select(dim, ids[i])` alone.  ValueError for caches of different shapes, dtypes or
+        devices, IndexError for a dim out of range, TypeError for pack_fp8 with a dtype other than bf16, fp16 or fp32,
+        all before anything is stored.
+
+        CUDA int32 or int64 `ids` on the caches' device stay there: when every cache has the layout batch_put_blocks
+        reads in place with pages of at least LAYER_BLOCKS_MIN_PAGE_BYTES, the transfer engine builds the page table on
+        the device from the ids (batch_put_device_blocks) and the put kernel reads the blocks in place, with no host
+        synchronisation.  With pack_fp8, caches of that layout with pages of at least FP8_LAYER_BLOCKS_MIN_PAGE_BYTES,
+        whose selected element count is a whole number of MX blocks, under a fusable config (as put_blocks), are packed as
+        the pages are read (batch_put_device_fp8_blocks, one call per dtype).  Then an id out of range is found on the
+        device, after the transfer: IndexError is raised after the call, that key stores nothing (no object, no `#meta`),
+        and the other keys of the batch complete.  This differs from put_blocks, which checks ids before any transfer.
+        Layers that overlap one another take the fallback.
+
+        Every other case -- host ids, other layouts, smaller pages, and placements the device route cannot take
+        (NOT_IMPLEMENTED) -- checks the ids on the host first (IndexError before that key is stored; a CUDA ids tensor is
+        copied to the host, which synchronises) and takes index_select + stack + batch_put."""
+        keys, caches, ids = list(keys), list(caches), list(ids)
+        if not len(keys) == len(caches) == len(ids):
+            raise ValueError("keys, caches and ids differ in length")
+        cfg = config or self.config
+        layers = [self._layers(k, c) for k, c in zip(keys, caches)]
+        if pack_fp8:
+            bad = [(k, ls[0].dtype) for k, (ls, _) in zip(keys, layers) if ls[0].dtype not in _MX_WIDE]
+            if bad:
+                raise TypeError(f"MXFP8 packing takes bfloat16, float16 and float32 tensors, not {bad[:3]}")
+        dims = [self._block_dim(k, ls[0], dim) for k, (ls, _) in zip(keys, layers)]
+        def shape(i):
+            s = list(layers[i][0][0].shape)
+            s[dims[i]] = len(ids[i]) if not isinstance(ids[i], torch.Tensor) else ids[i].numel()
+            return [len(layers[i][0])] + s if layers[i][1] else s
+
+        blocks, dev = [None] * len(keys), []
+        for i, ((ls, _), d) in enumerate(zip(layers, dims)):
+            # packed: the fused pack takes whole MX blocks under a fusable config, as put_blocks
+            if ls[0].is_cuda and self._device_ids(ids[i], ls[0].device) and (
+                    not pack_fp8 or (self._fusable_fp8_cfg(cfg) and self.client.device_fp8_eligible(torch.Size(shape(i)).numel()))):
+                blocks[i] = self._device_blocks(ls, d, ids[i], None, 0, pack_fp8)
+            if blocks[i] is not None:
+                dev.append(i)
+        rest = [i for i in range(len(keys)) if blocks[i] is None]
+        refused = []
+        if dev:
+            ecs = {}
+            if pack_fp8:  # one call per wide type
+                for dt, grp in _by_dtype(dev, lambda i: layers[i][0][0].dtype).items():
+                    got = self.client.batch_put_device_fp8_blocks([keys[i] for i in grp], [blocks[i][0] for i in grp], cfg, self._stream(),
+                                                                  wide=_MX_WIDE[dt])
+                    ecs.update(zip(grp, got))
+            else:
+                ecs.update(zip(dev, self.client.batch_put_device_blocks([keys[i] for i in dev], [blocks[i][0] for i in dev], cfg, self._stream())))
+            ok = [i for i in dev if ecs[i] == _bb.ErrorCode.OK]
+            rest += [i for i in dev if ecs[i] == _bb.ErrorCode.NOT_IMPLEMENTED]
+            refused = [(i, ecs[i]) for i in dev if ecs[i] not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+            if ok:
+                self._put_metas([keys[i] for i in ok], [_meta(layers[i][0][0].dtype, shape(i), pack_fp8) for i in ok])
+        if rest:
+            sel = {i: torch.from_numpy(self._block_ids(keys[i], ids[i], layers[i][0][0].shape[dims[i]])) for i in rest}
+            picked = []
+            for i in rest:
+                ls, stacked = layers[i]
+                t = [c.index_select(dims[i], sel[i].to(c.device)) for c in ls]
+                picked.append(torch.stack(t) if stacked else t[0])
+            self.batch_put([keys[i] for i in rest], picked, pack_fp8, config)
+        self._verdicts(keys, [i for i, _ in refused], [e for _, e in refused])
+
+    def put_layer_blocks(self, key: str, caches, ids, dim: int = 0, pack_fp8: bool = False, config=None) -> None:
+        """Stores `torch.stack([c.index_select(dim, ids) for c in caches])` under `key` (see batch_put_layer_blocks)."""
+        self.batch_put_layer_blocks([key], [caches], [ids], dim, pack_fp8, config)
+
+    def batch_get_layer_blocks_into(self, keys: Sequence[str], caches: Sequence, ids: Sequence, dim: int = 0,
+                                    blocks: Optional[Sequence] = None) -> list:
+        """The mirror of batch_put_layer_blocks: `c.index_copy_(dim, ids[i], stored[l])` for every layer l, c =
+        caches[i][l], of the tensor stored under keys[i] (a single tensor: `caches[i].index_copy_(dim, ids[i], stored)`).
+        With `blocks`, a partial restore: `stored[l].index_select(dim, blocks[i])` is copied instead.  Returns `caches`.
+
+        Errors that need no ids come first, before any transfer: KeyError for a missing key, TypeError for a dtype other
+        than the stored one, ValueError for a stored shape other than the selection's (with blocks: other than the
+        caches' outside `dim`, or len(blocks[i]) != len(ids[i])) or for caches not on the current CUDA device.
+
+        CUDA int32 or int64 `ids` (and `blocks`) on the caches' device stay there when every cache has the layout
+        get_blocks_into stores into in place, with pages of at least LAYER_BLOCKS_MIN_PAGE_BYTES, and the layers do not
+        overlap: the transfer engine builds the page table from them on the device (batch_get_device_blocks), with no host
+        synchronisation.  A packed whole-block object takes batch_get_device_fp8_blocks (pages of at least
+        FP8_LAYER_BLOCKS_MIN_PAGE_BYTES, one call per dtype), which unpacks each tile straight into its pages.  Then an id or block out of range (IndexError) or a repeated one (ValueError) is found on the
+        device and raised after the call: no byte of that key's caches is written, and the other keys complete.  This
+        differs from get_blocks_into, which checks before any transfer.  Every other case checks the ids on the host first
+        (copying CUDA tensors there, which synchronises) and takes a whole get + index_copy_ per layer."""
+        keys, caches, ids = list(keys), list(caches), list(ids)
+        if not len(keys) == len(caches) == len(ids):
+            raise ValueError("keys, caches and ids differ in length")
+        if blocks is not None:
+            blocks = list(blocks)
+            if len(blocks) != len(keys):
+                raise ValueError("keys and blocks differ in length")
+        metas = self._metas(keys)
+        dev = torch.cuda.current_device()
+        layers = [self._layers(k, c) for k, c in zip(keys, caches)]
+        dims = [self._block_dim(k, ls[0], dim) for k, (ls, _) in zip(keys, layers)]
+        n_stored = []
+        for j, (k, m, (ls, stacked), d) in enumerate(zip(keys, metas, layers, dims)):
+            c = ls[0]
+            if c.dtype != _stored_dtype(m):
+                raise TypeError(f"{k}: cache is {c.dtype}, the stored tensor {_stored_dtype(m)}")
+            if not c.is_cuda or c.device.index != dev:
+                raise ValueError(f"{k}: caches must be CUDA tensors on cuda:{dev}, not {c.device}")
+            stored = m["shape"][1:] if stacked else m["shape"]
+            if stacked and (not m["shape"] or m["shape"][0] != len(ls)):
+                raise ValueError(f"{k}: the stored tensor has shape {m['shape']}, for {len(ls)} layers")
+            n = len(ids[j]) if not isinstance(ids[j], torch.Tensor) else ids[j].numel()
+            if len(stored) != c.dim() or any(a != s for e, (a, s) in enumerate(zip(stored, c.shape)) if e != d):
+                raise ValueError(f"{k}: the stored tensor has shape {m['shape']}, the caches {list(c.shape)}: they differ outside dim {d}")
+            if blocks is None and stored[d] != n:
+                raise ValueError(f"{k}: {stored[d]} blocks stored, {n} ids")
+            if blocks is not None:
+                nb = len(blocks[j]) if not isinstance(blocks[j], torch.Tensor) else blocks[j].numel()
+                if nb != n:
+                    raise ValueError(f"{k}: {nb} blocks for {n} ids")
+            n_stored.append(stored[d])
+        live = [i for i in range(len(keys)) if blocks is None or (len(blocks[i]) if not isinstance(blocks[i], torch.Tensor) else blocks[i].numel())]
+        tables = [None] * len(keys)
+        for i in live:
+            ls = layers[i][0]
+            sel = None if blocks is None else blocks[i]
+            # packed objects the fused unpack reads (whole MX blocks) take the fp8 call; padded ones the fallback
+            fp8 = metas[i]["packed"] is not None
+            if (fp8 and not self._fp8_whole(metas[i])) or not self._device_ids(ids[i], ls[0].device) or (
+                    sel is not None and not self._device_ids(sel, ls[0].device)):
+                continue
+            tables[i] = self._device_blocks(ls, dims[i], ids[i], sel, n_stored[i], fp8)
+        on_dev = [i for i in live if tables[i] is not None and not metas[i]["packed"]]
+        packed = [i for i in live if tables[i] is not None and metas[i]["packed"]]
+        rest = [i for i in live if tables[i] is None]
+        refused = []
+        for dt, grp in _by_dtype(packed, lambda i: layers[i][0][0].dtype).items():  # one call per wide type
+            ecs = self.client.batch_get_device_fp8_blocks([keys[i] for i in grp], [tables[i][0] for i in grp], self._stream(), wide=_MX_WIDE[dt])
+            rest += [i for i, e in zip(grp, ecs) if e == _bb.ErrorCode.NOT_IMPLEMENTED]
+            refused += [(i, e) for i, e in zip(grp, ecs) if e not in (_bb.ErrorCode.OK, _bb.ErrorCode.NOT_IMPLEMENTED)]
+        if on_dev:
+            ecs, sizes = self.client.batch_get_device_blocks([keys[i] for i in on_dev], [tables[i][0] for i in on_dev], self._stream())
+            for i, e, n in zip(on_dev, ecs, sizes):
+                want = int(np.prod(metas[i]["shape"], dtype=np.int64)) * layers[i][0][0].element_size()
+                if e == _bb.ErrorCode.NOT_IMPLEMENTED:
+                    rest.append(i)
+                elif e == _bb.ErrorCode.OK and n != want:
+                    raise RuntimeError(f"{keys[i]}: {n} bytes stored, {want} expected")
+                elif e != _bb.ErrorCode.OK:
+                    refused.append((i, e))
+        if rest:
+            idx, sel = {}, {}
+            for i in rest:
+                c = layers[i][0][0]
+                idx[i] = self._block_ids(keys[i], ids[i], c.shape[dims[i]])
+                if np.unique(idx[i]).size != idx[i].size:
+                    raise ValueError(f"{keys[i]}: duplicate block ids")
+                if blocks is not None:
+                    sel[i] = self._block_ids(keys[i], blocks[i], n_stored[i], "blocks")
+                    if np.unique(sel[i]).size != sel[i].size:
+                        raise ValueError(f"{keys[i]}: duplicate blocks")
+
+            def restore(i, t):
+                ls, stacked = layers[i]
+                for l, c in enumerate(ls):
+                    s = t[l] if stacked else t
+                    if i in sel:
+                        s = s.index_select(dims[i], torch.from_numpy(sel[i]).to(s.device))
+                    c.index_copy_(dims[i], torch.from_numpy(idx[i]).to(c.device), s)
+
+            self._whole(keys, rest, None, restore)
+        self._verdicts(keys, [i for i, _ in refused], [e for _, e in refused])
+        return caches
+
+    def get_layer_blocks_into(self, key: str, caches, ids, dim: int = 0, blocks=None):
+        """The tensor stored under `key` copied into the blocks `ids` of every layer's cache (see
+        batch_get_layer_blocks_into)."""
+        return self.batch_get_layer_blocks_into([key], [caches], [ids], dim, None if blocks is None else [blocks])[0]
+
     # ------------------------------------------------------------------ get
     def _metas(self, keys: Sequence[str]) -> list:
         metas = []
@@ -777,6 +1030,21 @@ class AsyncTensorStore(TensorStore):
         queued on the caller's stream; the future yields `caches`, already synchronised with the side stream."""
         caches = list(caches)
         return self._on_side(True, self.batch_get_blocks_into, list(keys), caches, list(ids), dim,
+                             None if blocks is None else list(blocks), result=caches)
+
+    def put_layer_blocks_async(self, keys: Sequence[str], caches: Sequence, ids: Sequence, dim: int = 0, pack_fp8: bool = False,
+                               config=None):
+        """batch_put_layer_blocks on the side stream, ordered after the work already queued on the caller's stream (which
+        may be writing the ids); the future yields the number of objects stored, or raises the call's error."""
+        keys = list(keys)
+        return self._on_side(True, self.batch_put_layer_blocks, keys, list(caches), list(ids), dim, pack_fp8, config, result=len(keys))
+
+    def get_layer_blocks_into_async(self, keys: Sequence[str], caches: Sequence, ids: Sequence, dim: int = 0,
+                                    blocks: Optional[Sequence] = None):
+        """batch_get_layer_blocks_into on the side stream, ordered after the work already queued on the caller's stream;
+        the future yields `caches`, already synchronised with the side stream."""
+        caches = list(caches)
+        return self._on_side(True, self.batch_get_layer_blocks_into, list(keys), caches, list(ids), dim,
                              None if blocks is None else list(blocks), result=caches)
 
     def close(self):

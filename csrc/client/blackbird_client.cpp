@@ -772,13 +772,15 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
     idx.push_back(i);
   }
   std::vector<uint64_t> digests;
-  ErrorCode ec = ops.empty() ? ErrorCode::OK : device_->put_fp8(ops, stream, &digests);
+  std::vector<ErrorCode> verdicts;
+  ErrorCode ec = ops.empty() ? ErrorCode::OK : device_->put_fp8_verdicts(ops, stream, &digests, &verdicts);
   std::vector<ObjectKey> done;
   std::vector<ShardChecksums> sums;
   for (size_t k = 0; k < idx.size(); ++k) {
-    if (ec != ErrorCode::OK || digests.size() != idx.size()) {
+    const ErrorCode v = k < verdicts.size() ? verdicts[k] : ErrorCode::OK;  // refused ids: the answer, and no digest
+    if (ec != ErrorCode::OK || digests.size() != idx.size() || v != ErrorCode::OK) {
       keystone_->put_cancel(keys[idx[k]]);
-      out[idx[k]] = ec != ErrorCode::OK ? ec : ErrorCode::INTERNAL_ERROR;
+      out[idx[k]] = ec != ErrorCode::OK ? ec : v != ErrorCode::OK ? v : ErrorCode::INTERNAL_ERROR;
       continue;
     }
     done.push_back(keys[idx[k]]);
@@ -880,6 +882,58 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::ve
       });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                                    const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
+  std::vector<uint64_t> elems(n);
+  std::vector<DeviceLayout> mems(n);
+  return shaped_batch(
+      "device_put_fp8_blocks", true, n, blocks.size() == n,
+      [&](size_t i, uint64_t* wide_bytes) {
+        SourceBlocks sb;
+        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &sb, &elems[i]);
+        if (ec != ErrorCode::OK) return ec;
+        if (elems[i] == 0 || elems[i] % 32 || sb.has_null()) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks; a put reads every page
+        mems[i] = DeviceLayout(sb);
+        DeviceLayout bytes;
+        if (elems[i] > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *wide_bytes = b * elems[i];
+        // the engine's rule for a pack from blocks, checked once: there is no host-staged path for packed puts
+        if (!bytes.coaligned(0, b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto m = pick(mems, idx);
+        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), &m, cfg, stream, wide);
+      });
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                                    void* stream, mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
+  std::vector<uint64_t> elems(n);
+  std::vector<DeviceLayout> mems(n);
+  return shaped_batch(
+      "device_get_fp8_blocks", false, n, blocks.size() == n,
+      [&](size_t i, uint64_t* wide_bytes) {
+        SourceBlocks sb;
+        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &sb, &elems[i]);
+        if (ec != ErrorCode::OK) return ec;
+        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
+        if (elems[i] > UINT64_MAX / b) return ErrorCode::VALUE_OUT_OF_RANGE;
+        if (!sb.distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // the resolve kernel's duplicate bitmap is bounded
+        mems[i] = DeviceLayout(sb);
+        *wide_bytes = b * elems[i];
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto m = pick(mems, idx);
+        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, &m, stream, wide);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
                                                        const std::vector<DeviceLayout>* mem, void* stream, mxfp8::Wide wide) {
@@ -916,7 +970,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
-    if (mem_of(i).kind() == DeviceLayout::PAGES && !copies.empty()) {  // the pages must hold exactly the stored object's elements
+    const DeviceLayout::Kind kind = mem_of(i).kind();
+    if ((kind == DeviceLayout::PAGES || kind == DeviceLayout::BLOCKS) && !copies.empty()) {  // the pages must hold exactly the stored object's elements
       uint64_t stored = 0;
       for (const auto& sh : copies[0].shards) stored += sh.length;
       if (stored != packed) {
@@ -970,10 +1025,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     if (ops.empty()) break;
     if (attempt > 0) metrics_.inc("replica_failover_total");
     std::vector<uint32_t> status;
-    ErrorCode ec = device_->get_fp8(ops, stream, &status);
+    std::vector<ErrorCode> verdicts;
+    ErrorCode ec = device_->get_fp8_verdicts(ops, stream, &status, &verdicts);
     todo.clear();
     for (size_t k = 0; k < cur.size(); ++k) {
       if (ec != ErrorCode::OK || status.size() != cur.size()) out[cur[k]] = ec != ErrorCode::OK ? ec : ErrorCode::INTERNAL_ERROR;
+      else if (k < verdicts.size() && verdicts[k] != ErrorCode::OK) out[cur[k]] = verdicts[k];  // its ids, not its copy: no fail-over
       else if (status[k]) todo.push_back(cur[k]);
       else out[cur[k]] = ErrorCode::OK;
     }
@@ -1211,6 +1268,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
   std::vector<Chunk> chunks(plan.size());
   std::vector<size_t> host_put;                      // objects whose placement is not on the GPU fabric
   std::map<size_t, std::vector<CopyPlacement>> host_placed;
+  std::vector<bool> refused(keys.size(), false);     // blocks off the fabric (no host-staged path), or refused ids
 
   std::string reach_pool;
   bool reach_answer = false;
@@ -1251,6 +1309,11 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
           }
           on_fabric &= reach_answer;
         }
+      if (!on_fabric && m.kind() == DeviceLayout::BLOCKS) {  // the host cannot read the ids without a sync
+        out[i] = ErrorCode::NOT_IMPLEMENTED;
+        refused[i] = true;
+        continue;
+      }
       if (!on_fabric) {
         host_put.push_back(i);
         host_placed[i] = copies;
@@ -1288,9 +1351,12 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
   auto finish_chunk = [&](Chunk& ch) {
     BB_TRACE_SPAN("finish_chunk", ch.end - ch.begin);
     std::vector<uint64_t> digests;
+    std::vector<ErrorCode> verdicts;
     ErrorCode ec = ch.submit_error;
     const TimePoint t1 = Clock::now();
-    if (ch.submitted) ec = device_->wait_put(ch.ticket, &digests);
+    if (ch.submitted) ec = device_->wait_put_verdicts(ch.ticket, &digests, &verdicts);
+    for (size_t k = 0; ec == ErrorCode::OK && k < verdicts.size(); ++k)  // refused ids: the item's answer, and no digest
+      if (verdicts[k] != ErrorCode::OK && !refused[ch.ops[k].item]) out[ch.ops[k].item] = verdicts[k], refused[ch.ops[k].item] = true;
     metrics_.observe("phase_put_wait_us", us_since(t1));
     const TimePoint t2 = Clock::now();
     std::vector<ObjectKey> done_keys, cancel_keys;
@@ -1299,10 +1365,12 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
     if (ec != ErrorCode::OK) {
       for (size_t i = ch.begin; i < ch.end; ++i)
         if (ch.placed[i - ch.begin].ok()) {
-          out[i] = ec;
+          if (!refused[i]) out[i] = ec;
           cancel_keys.push_back(keys[i]);
         }
     } else {
+      for (size_t i = ch.begin; i < ch.end; ++i)
+        if (refused[i]) cancel_keys.push_back(keys[i]);
       std::vector<ShardChecksums> sums(ch.end - ch.begin);
       for (size_t i = ch.begin; i < ch.end; ++i) {
         const auto& pr = ch.placed[i - ch.begin];
@@ -1318,7 +1386,7 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
         for (size_t r = 0; r < op.replicas.size(); ++r) sm[r + 1][op.shard] = digests[k];
       }
       for (size_t i = ch.begin; i < ch.end; ++i)
-        if (ch.placed[i - ch.begin].ok() && !host_placed.count(i)) {
+        if (ch.placed[i - ch.begin].ok() && !host_placed.count(i) && !refused[i]) {
           done_keys.push_back(keys[i]);
           done_sums.push_back(std::move(sums[i - ch.begin]));
           done_idx.push_back(i);
@@ -1415,6 +1483,66 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector
       });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                                const WorkerConfig& cfg, void* stream) {
+  const size_t n = keys.size();
+  std::vector<size_t> sizes(n);
+  std::vector<DeviceLayout> mems(n);
+  return shaped_batch(
+      "device_put_blocks", true, n, blocks.size() == n,
+      [&](size_t i, uint64_t* size) {
+        SourceBlocks b;
+        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &b, size);
+        if (ec != ErrorCode::OK) return ec;
+        if (b.has_null()) return ErrorCode::INVALID_ARGUMENT;  // a selection: a put reads every page
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        mems[i] = DeviceLayout(b);
+        sizes[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto m = pick(mems, idx);
+        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), &m, cfg, stream);
+      });
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                                void* stream, std::vector<size_t>* out_sizes) {
+  const size_t n = keys.size();
+  std::vector<size_t> caps(n);
+  std::vector<DeviceLayout> mems(n);
+  std::vector<bool> checkable(n, true);
+  if (out_sizes) out_sizes->assign(n, 0);
+  return shaped_batch(
+      "device_get_blocks", false, n, blocks.size() == n,
+      [&](size_t i, uint64_t* size) {
+        SourceBlocks b;
+        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &b, size);
+        if (ec != ErrorCode::OK) return ec;
+        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        mems[i] = DeviceLayout(b);
+        caps[i] = static_cast<size_t>(*size);
+        return ErrorCode::OK;
+      },
+      [&](const std::vector<size_t>& idx) {
+        // the resolve kernel checks a get's ids for duplicates in a bitmap of bounded size: larger caches are the caller's
+        std::vector<size_t> run;
+        std::vector<ErrorCode> ecs(idx.size(), ErrorCode::NOT_IMPLEMENTED);
+        for (size_t i : idx)
+          if (mems[i].blocks().distinct_checkable()) run.push_back(i);
+        const auto m = pick(mems, run);
+        std::vector<size_t> sizes;
+        const auto got = get_device(pick(keys, run), std::vector<void*>(run.size(), nullptr), pick(caps, run), nullptr, &m, stream, &sizes);
+        for (size_t k = 0, j = 0; k < idx.size() && j < run.size(); ++k)
+          if (idx[k] == run[j]) {
+            ecs[k] = got[j];
+            if (out_sizes && j < sizes.size()) (*out_sizes)[idx[k]] = sizes[j];
+            ++j;
+          }
+        return ecs;
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                                const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& lengths,
                                                                void* stream) {
@@ -1499,11 +1627,17 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
       }
     }
   };
-  auto apply_status = [&](const std::vector<DeviceShardOp>& ops, const std::vector<uint32_t>& status, std::vector<size_t>* retry) {
+  // A verdict on an item's block ids answers it, ahead of its digests: its ids, not its copy, are wrong.
+  auto apply_status = [&](const std::vector<DeviceShardOp>& ops, const std::vector<uint32_t>& status, const std::vector<ErrorCode>& verdicts,
+                          std::vector<size_t>* retry) {
     std::vector<bool> bad(keys.size(), false), seen(keys.size(), false);
     for (size_t k = 0; k < ops.size(); ++k) {
       seen[ops[k].item] = true;
       if (status[k] != 0) bad[ops[k].item] = true;
+      if (k < verdicts.size() && verdicts[k] != ErrorCode::OK && pending[ops[k].item]) {
+        out[ops[k].item] = verdicts[k];
+        pending[ops[k].item] = false;
+      }
     }
     for (size_t i = 0; i < keys.size(); ++i) {
       if (!seen[i] || !pending[i]) continue;
@@ -1631,6 +1765,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           }
         }
       }
+      if (!found && m.kind() == DeviceLayout::BLOCKS) {  // no host-staged path: the host cannot read the ids without a sync
+        out[i] = ErrorCode::NOT_IMPLEMENTED;
+        continue;
+      }
       if (!found) {
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
@@ -1664,9 +1802,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
     BB_TRACE_SPAN("finish_chunk", ch.end - ch.begin);
     if (ch.ops.empty()) return;
     std::vector<uint32_t> status;
+    std::vector<ErrorCode> verdicts;
     ErrorCode ec = ch.err;
     const TimePoint t1 = Clock::now();
-    if (ch.submitted) ec = device_->wait_get(ch.ticket, &status);
+    if (ch.submitted) ec = device_->wait_get_verdicts(ch.ticket, &status, &verdicts);
     metrics_.observe("phase_get_wait_us", us_since(t1));
     if (ec != ErrorCode::OK) {
       for (size_t i = ch.begin; i < ch.end; ++i)
@@ -1676,7 +1815,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         }
       return;
     }
-    apply_status(ch.ops, status, &retry);
+    apply_status(ch.ops, status, verdicts, &retry);
   };
   const size_t depth = std::max<size_t>(1, std::min<size_t>(2, device_->max_in_flight()));
   size_t finished = 0;
@@ -1702,8 +1841,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
     if (ops.empty()) break;
     metrics_.inc("replica_failover_total");
     std::vector<uint32_t> status;
+    std::vector<ErrorCode> verdicts;
     auto t = device_->submit_get(ops, bases, stream);
-    ErrorCode ec = t.ok() ? device_->wait_get(t.value(), &status) : t.error();
+    ErrorCode ec = t.ok() ? device_->wait_get_verdicts(t.value(), &status, &verdicts) : t.error();
     if (ec != ErrorCode::OK) {
       for (size_t i = 0; i < keys.size(); ++i)
         if (pending[i]) {
@@ -1712,7 +1852,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         }
       break;
     }
-    apply_status(ops, status, &still);
+    apply_status(ops, status, verdicts, &still);
     retry.swap(still);
   }
   for (size_t i = 0; i < keys.size(); ++i)
@@ -1744,14 +1884,18 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
                                                    ChecksumAlgo algo, void*) {
   ++launches_;  // one "launch" per batch, like the fused kernel
   std::vector<uint64_t> digests(ops.size(), 0);
+  std::vector<ErrorCode> verdicts(ops.size(), ErrorCode::OK);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     const auto* src = static_cast<const uint8_t*>(op.src(dev_ptrs[op.item]));
     std::vector<uint8_t> dense;
     if (!op.mem.contiguous()) {  // as the kernel's gathering load: the shard's bytes, compacted from its rows or pages
       if (!op.mem.valid_source(op.placement->length)) return ErrorCode::INVALID_ARGUMENT;
+      if (op.mem.kind() == DeviceLayout::BLOCKS && !op.mem.coaligned(0, op.placement->length)) return ErrorCode::INVALID_ADDRESS;
+      std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table reads block 0 of every slice
+      const DeviceLayout m = op.mem.resolved(op.placement->length, false, &table, &verdicts[k]);
       dense.resize(op.placement->length);
-      copy_from_device(dense.data(), src, op.mem, dense.size(), nullptr);
+      copy_from_device(dense.data(), src, m, dense.size(), nullptr);
       src = dense.data();
     }
     ErrorCode ec = io_->write_shard(*op.placement, src, &digests[k], algo);
@@ -1759,22 +1903,27 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
     if (ec != ErrorCode::OK) return ec;
   }
   std::lock_guard<std::mutex> lk(done_mu_);
-  done_[next_ticket_].first = std::move(digests);
+  done_[next_ticket_] = {std::move(digests), {}, std::move(verdicts)};
   return next_ticket_++;
 }
 
 Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void*) {
   ++launches_;
   std::vector<uint32_t> status(ops.size(), 0);
+  std::vector<ErrorCode> verdicts(ops.size(), ErrorCode::OK);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceShardOp& op = ops[k];
     ErrorCode ec;
     auto* dst = static_cast<uint8_t*>(op.dst(dev_ptrs[op.item]));
     if (!op.mem.contiguous()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows or pages
       if (!op.mem.valid(op.placement->length) || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
+      if (op.mem.kind() == DeviceLayout::BLOCKS && !op.mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // as the engine
+      if (op.mem.kind() == DeviceLayout::BLOCKS && !op.mem.coaligned(0, op.placement->length)) return ErrorCode::INVALID_ADDRESS;
+      std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table is all null pages
+      const DeviceLayout m = op.mem.resolved(op.placement->length, true, &table, &verdicts[k]);
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
-      if (ec == ErrorCode::OK) copy_to_device(dst, op.mem, whole.data(), whole.size(), nullptr);
+      if (ec == ErrorCode::OK) copy_to_device(dst, m, whole.data(), whole.size(), nullptr);
     } else if (op.win.covers(op.placement->length)) {
       ec = io_->read_shard(*op.placement, dst, op.placement->checksum_algo);
     } else {  // as the kernel does: read and verify the whole shard, store only the window (only it is real memory)
@@ -1790,31 +1939,45 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
     }
   }
   std::lock_guard<std::mutex> lk(done_mu_);
-  done_[next_ticket_].second = std::move(status);
+  done_[next_ticket_] = {{}, std::move(status), std::move(verdicts)};
   return next_ticket_++;
 }
 
 ErrorCode HostLoopbackTransport::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
-  std::lock_guard<std::mutex> lk(done_mu_);
-  auto it = done_.find(ticket);
-  if (it == done_.end()) return ErrorCode::NOT_FOUND;
-  if (digests) *digests = std::move(it->second.first);
-  done_.erase(it);
-  return ErrorCode::OK;
+  std::vector<ErrorCode> verdicts;
+  return wait_put_verdicts(ticket, digests, &verdicts);
 }
 
 ErrorCode HostLoopbackTransport::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
+  std::vector<ErrorCode> verdicts;
+  return wait_get_verdicts(ticket, status, &verdicts);
+}
+
+ErrorCode HostLoopbackTransport::wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
   std::lock_guard<std::mutex> lk(done_mu_);
   auto it = done_.find(ticket);
   if (it == done_.end()) return ErrorCode::NOT_FOUND;
-  if (status) *status = std::move(it->second.second);
+  if (digests) *digests = std::move(it->second.digests);
+  *verdicts = std::move(it->second.verdicts);
   done_.erase(it);
   return ErrorCode::OK;
 }
 
-ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint64_t>* digests) {
+ErrorCode HostLoopbackTransport::wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
+  std::lock_guard<std::mutex> lk(done_mu_);
+  auto it = done_.find(ticket);
+  if (it == done_.end()) return ErrorCode::NOT_FOUND;
+  if (status) *status = std::move(it->second.status);
+  *verdicts = std::move(it->second.verdicts);
+  done_.erase(it);
+  return ErrorCode::OK;
+}
+
+ErrorCode HostLoopbackTransport::put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint64_t>* digests,
+                                                  std::vector<ErrorCode>* verdicts) {
   ++launches_;
   if (digests) digests->assign(ops.size(), 0);
+  verdicts->assign(ops.size(), ErrorCode::OK);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
     const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
@@ -1825,6 +1988,8 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
       DeviceLayout b;
       if (!op.win.whole() || !op.mem.valid_source(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table reads block 0 of every slice
+      b = b.resolved(eb * op.n_elems, false, &table, &(*verdicts)[k]);
       dense.resize(eb * op.n_elems);
       copy_from_device(dense.data(), op.wide, b, dense.size(), nullptr);
       src = dense.data();
@@ -1840,9 +2005,11 @@ ErrorCode HostLoopbackTransport::put_fp8(const std::vector<DeviceFp8Op>& ops, vo
   return ErrorCode::OK;
 }
 
-ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint32_t>* status) {
+ErrorCode HostLoopbackTransport::get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint32_t>* status,
+                                                  std::vector<ErrorCode>* verdicts) {
   ++launches_;
   if (status) status->assign(ops.size(), 0);
+  verdicts->assign(ops.size(), ErrorCode::OK);
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
     const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
@@ -1852,7 +2019,10 @@ ErrorCode HostLoopbackTransport::get_fp8(const std::vector<DeviceFp8Op>& ops, vo
     if (!op.mem.contiguous()) {  // as the engine: destination rows or pages, never with a window, co-aligned in wide bytes
       if (!op.win.whole() || !op.mem.valid(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      if (b.kind() == DeviceLayout::BLOCKS && !b.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // as the engine
     }
+    std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table is all null pages
+    b = b.resolved(eb * op.n_elems, true, &table, &(*verdicts)[k]);
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {

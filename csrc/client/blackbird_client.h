@@ -101,6 +101,17 @@ class DeviceTransport {
   virtual ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) = 0;
   virtual Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) = 0;
   virtual ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) = 0;
+  // wait_put and wait_get with each op's verdict on the block ids of a BLOCKS layout (SourceBlocks in
+  // common/store_window.h): empty, or one per op, OK or the refusal.  A refused op's transfer touched nothing outside the
+  // caller's memory, and its digest or status means nothing.  A transport that takes no BLOCKS layout returns none.
+  virtual ErrorCode wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
+    verdicts->clear();
+    return wait_put(ticket, digests);
+  }
+  virtual ErrorCode wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
+    verdicts->clear();
+    return wait_get(ticket, status);
+  }
   // True when the shard lives in this client's own device memory (a get from it never leaves the GPU).
   virtual bool is_local(const ShardPlacement& s) const { return false; }
   virtual size_t max_in_flight() const { return 1; }
@@ -111,9 +122,21 @@ class DeviceTransport {
   // object; status[i] != 0 = digest mismatch on get.  Objects must satisfy fp8_eligible().
   virtual ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) { return ErrorCode::NOT_IMPLEMENTED; }
   virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
+  // put_fp8 and get_fp8 with each op's verdict on the block ids of a BLOCKS layout, as wait_put_verdicts.
+  virtual ErrorCode put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
+                                     std::vector<ErrorCode>* verdicts) {
+    verdicts->clear();
+    return put_fp8(ops, stream, digests);
+  }
+  virtual ErrorCode get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
+                                     std::vector<ErrorCode>* verdicts) {
+    verdicts->clear();
+    return get_fp8(ops, stream, status);
+  }
   // Staging copies for objects (or shards) that live on host tiers, synchronous: object bytes [0, n) laid out by `layout`
   // at `base` (common/store_window.h) from / to n bytes packed back to back at `host`.  copy_to_device skips null pages;
-  // copy_from_device refuses them (INVALID_ARGUMENT).
+  // copy_from_device refuses them (INVALID_ARGUMENT).  A BLOCKS layout is NOT_IMPLEMENTED on a GPU: the host cannot read
+  // its ids without synchronising.
   virtual ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
     return ErrorCode::NOT_IMPLEMENTED;
   }
@@ -235,6 +258,18 @@ class BlackbirdClient {
   // the rest of the batch keeps the fused launch.
   std::vector<ErrorCode> batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                     const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+  // Packed puts and gets from block ids that stay on the device: batch_put_device_blocks and batch_get_device_blocks for
+  // packed tensors, `page` counted in elements of `wide` (the stride and slice addresses in bytes), with the rules of
+  // batch_put_device_fp8_paged and batch_get_device_fp8_paged.  Per object, before anything is allocated: INVALID_ARGUMENT
+  // for the shape errors of the byte calls or an element count that is not a positive whole number of MX blocks (on a
+  // get: not exactly the stored object's); VALUE_OUT_OF_RANGE when the count or its wide bytes overflow; NOT_IMPLEMENTED
+  // when the table is not co-aligned in wide bytes, the object is not fusable, or (a get) n_blocks or n_stored exceeds
+  // SourceBlocks::kMaxDistinct -- there is no host-staged path.  After the transfer the device's verdict on the ids
+  // answers the object as for the byte calls: a refused put is cancelled, a refused get stores nothing and is not retried.
+  std::vector<ErrorCode> batch_put_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                     const WorkerConfig& cfg, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+  std::vector<ErrorCode> batch_get_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
+                                                     mxfp8::Wide wide = mxfp8::Wide::BF16);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);
@@ -323,6 +358,29 @@ class BlackbirdClient {
   // page_bytes[i] == 0 with pages; VALUE_OUT_OF_RANGE when the capacity overflows.
   std::vector<ErrorCode> batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                 const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes);
+  // Paged puts from block ids that stay on the device: object i is the pages of blocks[i] (SourceBlocks in
+  // common/store_window.h: outer slice q, block ids[k], page r = q * n_ids + k at outer[q] + ids[k] * stride), in page
+  // order, as batch_put_device_paged of that table would store it.  The ids are read on `stream` by the transfer
+  // engine's resolve kernel, after the work queued there before the call; the host never reads them, and no host work
+  // depends on their number beyond the small outer array.  Placement, replica fan-out and digests are
+  // batch_put_device_paged's.  Per object, before anything is allocated: INVALID_ARGUMENT for page == 0 with pages, a
+  // selection (a put reads every page) or ids other than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the size overflows.
+  // After the transfer, from the device: VALUE_OUT_OF_RANGE for an id outside [0, n_blocks); the put is then cancelled,
+  // nothing is stored and the rest of the batch carries on.  NOT_IMPLEMENTED when the table is not co-aligned
+  // (SourceBlocks::coaligned) or a placement is not on the GPU fabric: there is no host-staged path; the put is cancelled.
+  std::vector<ErrorCode> batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
+                                                 const WorkerConfig& cfg, void* stream);
+  // Paged gets into blocks named by device-resident ids, the mirror: object i lands in the pages of blocks[i], with a
+  // selection (sel, n_stored) as a partial restore: only the pages of the stored blocks sel[m] land, in block ids[m], and
+  // the others are not stored.  The capacity is the table's size; out_sizes[i] receives the object's size.  Every shard
+  // is read whole and verified, with the fail-over and placement refresh of batch_get_device.  Per object: INVALID_ARGUMENT
+  // for page == 0 with pages or ids other than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the capacity overflows;
+  // BUFFER_OVERFLOW for a larger object; NOT_IMPLEMENTED when n_blocks or n_stored exceeds SourceBlocks::kMaxDistinct, the
+  // table fails SourceBlocks::fused_get_aligned or no copy is on the GPU fabric.  After the transfer, from the device:
+  // VALUE_OUT_OF_RANGE for an id (or selection entry) out of range, INVALID_ARGUMENT for a repeated one; then nothing
+  // of the object is stored, it is not retried on another replica, and the rest of the batch carries on.
+  std::vector<ErrorCode> batch_get_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
+                                                 std::vector<size_t>* out_sizes);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }
@@ -422,17 +480,24 @@ class HostLoopbackTransport : public DeviceTransport {
   ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override;
   Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) override;
   ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
+  ErrorCode wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) override;
+  ErrorCode wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) override;
   bool can_reach(const ShardPlacement& s) const override;
   uint64_t launches() const override { return launches_; }
+  // A BLOCKS layout is resolved on the host (SourceBlocks::resolve): here the "device" ids are host memory.
   ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void*) override {
     if (!layout.valid_source(n)) return ErrorCode::INVALID_ARGUMENT;
-    layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+    std::vector<uint64_t> table;
+    ErrorCode v;
+    layout.resolved(n, false, &table, &v).for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
       std::memcpy(static_cast<uint8_t*>(host) + x, reinterpret_cast<const void*>(addr), len);
     });
     return ErrorCode::OK;
   }
   ErrorCode copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void*) override {
-    layout.for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
+    std::vector<uint64_t> table;
+    ErrorCode v;
+    layout.resolved(n, true, &table, &v).for_each_run(reinterpret_cast<uintptr_t>(base), n, [&](uint64_t x, uint64_t addr, uint64_t len) {
       std::memcpy(reinterpret_cast<void*>(addr), static_cast<const uint8_t*>(host) + x, len);
     });
     return ErrorCode::OK;
@@ -441,8 +506,18 @@ class HostLoopbackTransport : public DeviceTransport {
   // MXFP8 through the CPU reference codec (common/mxfp8.h): the stored object and its digest are the ones the fused
   // kernels produce, so the fp8 client logic (replica fan-out, fail-over between replicas) is testable on CPU too.
   bool fp8_eligible(uint64_t n_elems) const override { return n_elems != 0 && n_elems % 32 == 0; }
-  ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override;
-  ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override;
+  ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override {
+    std::vector<ErrorCode> verdicts;
+    return put_fp8_verdicts(ops, stream, digests, &verdicts);
+  }
+  ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override {
+    std::vector<ErrorCode> verdicts;
+    return get_fp8_verdicts(ops, stream, status, &verdicts);
+  }
+  ErrorCode put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
+                             std::vector<ErrorCode>* verdicts) override;
+  ErrorCode get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
+                             std::vector<ErrorCode>* verdicts) override;
 
  private:
   std::shared_ptr<BlackbirdClient> io_;
@@ -450,7 +525,12 @@ class HostLoopbackTransport : public DeviceTransport {
   std::atomic<uint64_t> launches_{0};
   std::mutex done_mu_;
   uint64_t next_ticket_ = 1;
-  std::map<uint64_t, std::pair<std::vector<uint64_t>, std::vector<uint32_t>>> done_;  // ticket -> (put digests, get status)
+  struct Done {
+    std::vector<uint64_t> digests;  // put
+    std::vector<uint32_t> status;   // get
+    std::vector<ErrorCode> verdicts;
+  };
+  std::map<uint64_t, Done> done_;
 };
 
 }  // namespace bb::client

@@ -12,11 +12,12 @@
 // The default window, [0, UINT64_MAX) without a pattern, is the whole object.
 //
 // SourceRows, below, maps a dense object onto strided memory instead: where a put reads each byte from, or where a get into
-// a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses.  DeviceLayout, at the end, is
-// the one type the other layers hold for either of them.
+// a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses, SourceBlocks onto pages named
+// by block ids in device memory.  DeviceLayout, at the end, is the one type the other layers hold for any of them.
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <vector>
 
 #include "common/error.h"
 
@@ -355,20 +356,157 @@ struct SourcePages {
   }
 };
 
+// SourceBlocks: the pages of a paged KV cache picked by block ids that stay in device memory, on either side of a
+// transfer.  The cache is n_outer outer slices (for one tensor per layer: layer-major, then each layer's outer index),
+// slice q starting at the byte address outer[q]; block b of a slice lies `stride` bytes after block b - 1.  Without a
+// selection the object has n_outer * n_ids pages, page r = q * n_ids + k at
+//   outer[q] + ids[k] * stride
+// With a selection `sel` (a partial restore, gets only) it has n_outer * n_stored pages: page q * n_stored + sel[m] is at
+// outer[q] + ids[m] * stride and every other page is a null page (not stored, as SourcePages').  Object bytes then map
+// onto the pages exactly as SourcePages maps them, with `page` and `phase` in its units; `first` is the table's first page
+// after rebase().  `outer` is a small host array, one entry per slice; `ids` and `sel` are n_ids integers of id_bytes (4
+// or 8, signed) that the host never reads on the device route: the transfer engine's resolve kernel builds the page
+// table on the device (kernels/resolve_blocks.cu) and the host loopback transport calls resolve() below, the reference.
+//
+// The ids decide the verdict: every id in [0, n_blocks) or VALUE_OUT_OF_RANGE; for a get, ids pairwise distinct or
+// INVALID_ARGUMENT; a selection's entries in [0, n_stored) and pairwise distinct, under the same two codes.  A refused
+// table never leads a transfer outside the caller's cache: a get's entries are all null (nothing is stored) and a put's
+// are all block 0 of their slice, outer[q] (the put is then cancelled).  Co-alignment needs no id: every address is
+// outer[q] + a multiple of the stride, so coaligned() is a closed form over outer[], stride and page.
+struct SourceBlocks {
+  const uint64_t* outer = nullptr;
+  uint64_t n_outer = 0;
+  const void* ids = nullptr;
+  uint64_t n_ids = 0;
+  const void* sel = nullptr;  // null: no selection
+  uint64_t n_stored = 0;
+  uint32_t id_bytes = 4;
+  uint64_t n_blocks = 0, stride = 0, page = 0, phase = 0, first = 0;
+
+  // Gets check duplicates in a bitmap of this many bits over n_blocks (and n_stored) in the resolve kernel's shared
+  // memory; a larger bound is NOT_IMPLEMENTED on the device route.
+  static constexpr uint64_t kMaxDistinct = uint64_t{1} << 18;
+
+  bool paged() const { return page != 0; }
+  uint64_t per_outer() const { return sel ? n_stored : n_ids; }
+  uint64_t npages() const { return n_outer * per_outer(); }
+  uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
+  // Whether the table holds every page of an object of `len` units from page `first`, with phase < page.
+  bool valid(uint64_t len) const {
+    return paged() && phase < page && (id_bytes == 4 || id_bytes == 8) && first + pages_for(len) <= npages() &&
+           (n_ids == 0 || (ids && n_blocks != 0)) && (n_outer == 0 || outer);
+  }
+  // A put reads every unit: no selection, whose pages may be null.
+  bool has_null() const { return sel != nullptr; }
+  // Whether the device route can check a get's ids for duplicates (kMaxDistinct).
+  bool distinct_checkable() const { return n_blocks <= kMaxDistinct && (!sel || n_stored <= kMaxDistinct); }
+
+  // The table of ids.size() blocks of every slice in outer[], pages of `page` units: an object of *size = n_outer *
+  // per_outer() * page units.  INVALID_ARGUMENT for page == 0 with pages, a selection without stored blocks or ids of
+  // another width than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the size overflows.  No pages is a zero-unit object.
+  static ErrorCode from_blocks(const SourceBlocks& b, SourceBlocks* out, uint64_t* size) {
+    *out = b;
+    out->first = 0, out->phase = 0;
+    *size = 0;
+    if ((b.id_bytes != 4 && b.id_bytes != 8) || (b.sel && b.n_stored == 0)) return ErrorCode::INVALID_ARGUMENT;
+    uint64_t pages = 0;
+    if (__builtin_mul_overflow(b.n_outer, out->per_outer(), &pages)) return ErrorCode::VALUE_OUT_OF_RANGE;
+    if (pages == 0) return ErrorCode::OK;
+    if (b.page == 0) return ErrorCode::INVALID_ARGUMENT;
+    if (__builtin_mul_overflow(pages, b.page, size)) return ErrorCode::VALUE_OUT_OF_RANGE;
+    return ErrorCode::OK;
+  }
+
+  // The table in bytes of elements of `b` bytes (an MXFP8 transfer's wide side): page and phase times b, the same
+  // addresses and stride.  False when either product overflows.
+  bool to_wide_bytes(uint64_t b, SourceBlocks* out) const {
+    *out = *this;
+    return !__builtin_mul_overflow(page, b, &out->page) && !__builtin_mul_overflow(phase, b, &out->phase);
+  }
+  // The table seen from object unit `off`: unit x of the result is unit off + x here (as SourcePages::rebase).
+  SourceBlocks rebase(uint64_t off) const {
+    SourceBlocks r = *this;
+    if (!paged()) return r;
+    r.first = first + (phase + off) / page;
+    r.phase = (phase + off) % page;
+    return r;
+  }
+  // SourcePages::coaligned for every table the ids could make: the stride a multiple of 16 bytes, every outer[q] + phase
+  // 16-byte aligned, and the page a multiple of 16 when object units [0, len) touch more than one page.
+  bool coaligned(uint64_t len) const {
+    const uint64_t n = pages_for(len);
+    if (n == 0) return true;
+    if ((n > 1 && page % 16) || stride % 16) return false;
+    for (uint64_t q = 0; q < n_outer; ++q)
+      if ((outer[q] + phase) % 16) return false;
+    return true;
+  }
+  // The client's fused-get rule, as SourcePages::fused_get_aligned: the page a multiple of 16 whenever the object has
+  // more than one page, and the shard [off, off + len) co-aligned.
+  bool fused_get_aligned(uint64_t off, uint64_t len) const {
+    if (npages() > 1 && page % 16) return false;
+    return rebase(off).coaligned(len);
+  }
+
+  int64_t id_at(const void* p, uint64_t k) const {
+    return id_bytes == 8 ? static_cast<const int64_t*>(p)[k] : static_cast<const int32_t*>(p)[k];
+  }
+  // The reference resolve, with ids and sel in host memory: writes the `count` page entries from page `first` into
+  // table[0, count) and returns the verdict (OK, VALUE_OUT_OF_RANGE or INVALID_ARGUMENT, see above).  `get` refuses
+  // duplicate ids.  Every id is checked, not only those of the pages written, so every shard of an object reaches the
+  // same verdict.
+  ErrorCode verdict(bool get) const {
+    auto in_range = [&](const void* p, uint64_t bound) {
+      for (uint64_t k = 0; k < n_ids; ++k)
+        if (id_at(p, k) < 0 || static_cast<uint64_t>(id_at(p, k)) >= bound) return false;
+      return true;
+    };
+    auto distinct = [&](const void* p, uint64_t bound) {
+      std::vector<bool> seen(bound);
+      for (uint64_t k = 0; k < n_ids; ++k) {
+        if (seen[id_at(p, k)]) return false;
+        seen[id_at(p, k)] = true;
+      }
+      return true;
+    };
+    if (!in_range(ids, n_blocks) || (sel && !in_range(sel, n_stored))) return ErrorCode::VALUE_OUT_OF_RANGE;
+    if (get && (!distinct(ids, n_blocks) || (sel && !distinct(sel, n_stored)))) return ErrorCode::INVALID_ARGUMENT;
+    return ErrorCode::OK;
+  }
+  ErrorCode resolve(uint64_t* table, uint64_t count, bool get) const {
+    const ErrorCode v = verdict(get);
+    const uint64_t per = per_outer();
+    for (uint64_t t = 0; t < count; ++t) {
+      const uint64_t r = first + t, q = r / per;
+      table[t] = v != ErrorCode::OK ? (get ? 0 : outer[q]) : sel ? 0 : outer[q] + static_cast<uint64_t>(id_at(ids, r % per)) * stride;
+    }
+    if (v == ErrorCode::OK && sel)
+      for (uint64_t q = 0; q < n_outer; ++q)
+        for (uint64_t m = 0; m < n_ids; ++m) {
+          const uint64_t r = q * n_stored + static_cast<uint64_t>(id_at(sel, m));
+          if (r >= first && r - first < count) table[r - first] = outer[q] + static_cast<uint64_t>(id_at(ids, m)) * stride;
+        }
+    return v;
+  }
+};
+
 // DeviceLayout: where the caller's units of one object sit on the device side of a transfer, relative to a base address:
-// contiguous (unit x at base + x, the default), in rows (SourceRows, with row 0 at the base) or in pages (SourcePages,
-// whose addresses are absolute: the base is not used).  It is the source of a put and the destination of a get, in bytes,
-// or for an MXFP8 transfer in elements of the wide side until to_wide_bytes().  This is the one place that knows the three
-// kinds; the transfer engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the
-// transports all hold one of these.  A StoreWindow only ever goes with a contiguous layout.
+// contiguous (unit x at base + x, the default), in rows (SourceRows, with row 0 at the base), in pages (SourcePages,
+// whose addresses are absolute: the base is not used) or in blocks picked by device-resident ids (SourceBlocks, absolute
+// too).  It is the source of a put and the destination of a get, in bytes, or for an MXFP8 transfer in elements of the
+// wide side until to_wide_bytes().  This is the one place that knows the four kinds; the transfer engine (XferItem,
+// Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the transports all hold one of these.  A
+// StoreWindow only ever goes with a contiguous layout.  A BLOCKS layout has no host copy runs (for_each_run does nothing
+// for it) until resolved() has turned it into pages.
 class DeviceLayout {
  public:
-  enum Kind { CONTIGUOUS, ROWS, PAGES };
+  enum Kind { CONTIGUOUS, ROWS, PAGES, BLOCKS };
 
   DeviceLayout() = default;
   // Rows without a pattern, and a table without pages, are contiguous.
   explicit DeviceLayout(const SourceRows& r) : kind_(r.strided() ? ROWS : CONTIGUOUS), rows_(r) {}
   explicit DeviceLayout(const SourcePages& p) : kind_(p.paged() ? PAGES : CONTIGUOUS), pages_(p) {}
+  explicit DeviceLayout(const SourceBlocks& b) : kind_(b.paged() ? BLOCKS : CONTIGUOUS), blocks_(b) {}
 
   // The layouts of SourceRows::from_rows and SourcePages::from_pages, with their object size and error rules.
   static ErrorCode from_rows(uint64_t width, uint64_t pitch, uint64_t rows, DeviceLayout* out, uint64_t* size, uint64_t* extent) {
@@ -388,35 +526,46 @@ class DeviceLayout {
   bool contiguous() const { return kind_ == CONTIGUOUS; }
   const SourceRows& rows() const { return rows_; }     // the pattern of a ROWS layout
   const SourcePages& pages() const { return pages_; }  // the table of a PAGES layout
+  const SourceBlocks& blocks() const { return blocks_; }  // the description of a BLOCKS layout
 
   // The INVALID_ARGUMENT rules against an object of len units: a valid pattern, or a table that holds every page.
   bool valid(uint64_t len) const {
-    return kind_ == ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : true;
+    return kind_ == ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : kind_ == BLOCKS ? blocks_.valid(len) : true;
   }
-  // The same for a put's source, which must read every unit: valid(len), and no null page.
-  bool valid_source(uint64_t len) const { return valid(len) && !(kind_ == PAGES && pages_.has_null(len)); }
+  // The same for a put's source, which must read every unit: valid(len), and no null page (nor a selection of blocks).
+  bool valid_source(uint64_t len) const {
+    return valid(len) && !(kind_ == PAGES && pages_.has_null(len)) && !(kind_ == BLOCKS && blocks_.has_null());
+  }
 
   // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
   // when the byte arithmetic could overflow.
   bool to_wide_bytes(uint64_t b, DeviceLayout* out) const {
     *out = *this;
-    return kind_ == ROWS ? rows_.to_wide_bytes(b, &out->rows_) : kind_ == PAGES ? pages_.to_wide_bytes(b, &out->pages_) : true;
+    return kind_ == ROWS     ? rows_.to_wide_bytes(b, &out->rows_)
+           : kind_ == PAGES  ? pages_.to_wide_bytes(b, &out->pages_)
+           : kind_ == BLOCKS ? blocks_.to_wide_bytes(b, &out->blocks_)
+                             : true;
   }
 
   // The layout seen from object unit `off`: unit x of the result is unit off + x here, relative to a base that has moved
-  // by *shift (off when contiguous, to where the new pattern's row 0 starts for rows, 0 for pages).
+  // by *shift (off when contiguous, to where the new pattern's row 0 starts for rows, 0 for pages and blocks).
   DeviceLayout rebase(uint64_t off, uint64_t* shift) const {
     DeviceLayout l = *this;
     *shift = off;
     if (kind_ == ROWS) l.rows_ = rows_.rebase(off, shift);
     if (kind_ == PAGES) l.pages_ = pages_.rebase(off), *shift = 0;
+    if (kind_ == BLOCKS) l.blocks_ = blocks_.rebase(off), *shift = 0;
     return l;
   }
 
   // Whether object bytes [0, len) at `base` are co-aligned with the tiles, so that the kernels only move 16-byte congruent
-  // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned or SourcePages::coaligned.
+  // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned, SourcePages::coaligned or
+  // SourceBlocks::coaligned.
   bool coaligned(uintptr_t base, uint64_t len) const {
-    return kind_ == ROWS ? rows_.coaligned(base, len) : kind_ == PAGES ? pages_.coaligned(len) : base % 16 == 0;
+    return kind_ == ROWS     ? rows_.coaligned(base, len)
+           : kind_ == PAGES  ? pages_.coaligned(len)
+           : kind_ == BLOCKS ? blocks_.coaligned(len)
+                             : base % 16 == 0;
   }
 
   // The client's rule for whether a device get into this layout at `base` may take the fused path as far as the shard
@@ -425,6 +574,7 @@ class DeviceLayout {
   bool fused_get_aligned(uintptr_t base, uint64_t off, uint64_t len, const StoreWindow& win = {}) const {
     if (kind_ == ROWS) return rows_.fused_get_aligned(base, off, len);
     if (kind_ == PAGES) return pages_.fused_get_aligned(off, len);
+    if (kind_ == BLOCKS) return blocks_.fused_get_aligned(off, len);
     return win.fused_get_aligned(base, off, len);
   }
 
@@ -434,13 +584,24 @@ class DeviceLayout {
   void for_each_run(uintptr_t base, uint64_t len, F&& f) const {
     if (kind_ == ROWS) rows_.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { f(x, base + at, n); });
     else if (kind_ == PAGES) pages_.for_each_run(len, f);
-    else if (len) f(uint64_t{0}, static_cast<uint64_t>(base), len);
+    else if (len && kind_ == CONTIGUOUS) f(uint64_t{0}, static_cast<uint64_t>(base), len);
+  }
+
+  // The layout with host-resident ids resolved (SourceBlocks::resolve) into pages over *table, for object units
+  // [0, len) of a get or a put; *verdict receives the verdict.  Other kinds come back as they are, with OK.
+  DeviceLayout resolved(uint64_t len, bool get, std::vector<uint64_t>* table, ErrorCode* verdict) const {
+    *verdict = ErrorCode::OK;
+    if (kind_ != BLOCKS) return *this;
+    table->assign(blocks_.pages_for(len), 0);
+    *verdict = blocks_.resolve(table->data(), table->size(), get);
+    return DeviceLayout(SourcePages{table->data(), table->size(), blocks_.page, blocks_.phase});
   }
 
  private:
   Kind kind_ = CONTIGUOUS;
   SourceRows rows_;
   SourcePages pages_;
+  SourceBlocks blocks_;
 };
 
 }  // namespace bb

@@ -507,6 +507,7 @@ Result<void*> GpuFabric::resolve(const ShardPlacement& s) {
 }
 
 ErrorCode GpuFabric::copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) {
+  if (layout.kind() == DeviceLayout::BLOCKS) return ErrorCode::NOT_IMPLEMENTED;  // the ids are device memory
   if (!layout.valid_source(n)) return ErrorCode::INVALID_ARGUMENT;  // every byte is read: no null page
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
@@ -527,6 +528,7 @@ ErrorCode GpuFabric::copy_from_device(void* host, const void* base, const Device
 }
 
 ErrorCode GpuFabric::copy_to_device(void* base, const DeviceLayout& layout, const void* host, size_t n, void* stream) {
+  if (layout.kind() == DeviceLayout::BLOCKS) return ErrorCode::NOT_IMPLEMENTED;  // the ids are device memory
   if (!layout.valid(n)) return ErrorCode::INVALID_ARGUMENT;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (!cuda_ok(cudaSetDevice(device_), "cudaSetDevice")) return ErrorCode::FABRIC_ERROR;
@@ -649,6 +651,17 @@ ErrorCode GpuFabric::finish(uint64_t ticket, InFlight* fl, XferResult* res) {
 }
 
 ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
+  std::vector<ErrorCode> verdicts;
+  return wait_put_verdicts(ticket, digests, &verdicts);
+}
+
+// An op's verdict is the first refusal among its items (the extra fan-out passes of a put resolve the same ids).
+static void op_verdicts(const std::vector<size_t>& op_of_item, const std::vector<ErrorCode>& item_verdicts, std::vector<ErrorCode>* out) {
+  for (size_t i = 0; i < op_of_item.size() && i < item_verdicts.size(); ++i)
+    if ((*out)[op_of_item[i]] == ErrorCode::OK) (*out)[op_of_item[i]] = item_verdicts[i];
+}
+
+ErrorCode GpuFabric::wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
   BB_TRACE_SPAN("fabric.wait_put");
   InFlight fl;
   XferResult res;
@@ -657,6 +670,8 @@ ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
     digests->assign(fl.nops, 0);
     for (size_t i = fl.op_of_item.size(); i-- > 0;) (*digests)[fl.op_of_item[i]] = res.digest[i];
   }
+  verdicts->assign(fl.nops, ErrorCode::OK);
+  op_verdicts(fl.op_of_item, res.verdict, verdicts);
   return ErrorCode::OK;
 }
 
@@ -693,18 +708,32 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
 }
 
 ErrorCode GpuFabric::put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) {
+  std::vector<ErrorCode> verdicts;
+  return put_fp8_verdicts(ops, stream, digests, &verdicts);
+}
+
+ErrorCode GpuFabric::get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) {
+  std::vector<ErrorCode> verdicts;
+  return get_fp8_verdicts(ops, stream, status, &verdicts);
+}
+
+ErrorCode GpuFabric::put_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
+                                      std::vector<ErrorCode>* verdicts) {
   BB_TRACE_SPAN("fabric.put_fp8", ops.size());
   XferResult res;
   BB_TRY(transfer_fp8(ops, false, stream, &res));
   if (digests) *digests = std::move(res.digest);
+  *verdicts = std::move(res.verdict);  // one item per op
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) {
+ErrorCode GpuFabric::get_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
+                                      std::vector<ErrorCode>* verdicts) {
   BB_TRACE_SPAN("fabric.get_fp8", ops.size());
   XferResult res;
   BB_TRY(transfer_fp8(ops, true, stream, &res));
   if (status) *status = std::move(res.status);
+  *verdicts = std::move(res.verdict);
   return ErrorCode::OK;
 }
 
@@ -766,10 +795,17 @@ Result<uint64_t> GpuFabric::submit_get(const std::vector<client::DeviceShardOp>&
     note_device_ms(res.device_ms);
     fl.status.resize(ops.size(), 0);
     for (size_t i = 0; i < fl.op_of_item.size(); ++i) fl.status[fl.op_of_item[i]] = res.status[i];
+    fl.verdicts.resize(ops.size(), ErrorCode::OK);
+    op_verdicts(fl.op_of_item, res.verdict, &fl.verdicts);
   }
 }
 
 ErrorCode GpuFabric::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
+  std::vector<ErrorCode> verdicts;
+  return wait_get_verdicts(ticket, status, &verdicts);
+}
+
+ErrorCode GpuFabric::wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
   BB_TRACE_SPAN("fabric.wait_get");
   InFlight fl;
   XferResult res;
@@ -779,6 +815,9 @@ ErrorCode GpuFabric::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
     status->resize(fl.nops, 0);
     for (size_t i = 0; i < fl.op_of_item.size(); ++i) (*status)[fl.op_of_item[i]] = res.status[i];
   }
+  *verdicts = std::move(fl.verdicts);
+  verdicts->resize(fl.nops, ErrorCode::OK);
+  op_verdicts(fl.op_of_item, res.verdict, verdicts);
   return ErrorCode::OK;
 }
 

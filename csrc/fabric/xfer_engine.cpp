@@ -33,7 +33,9 @@ ErrorCode XferEngine::cuda_failed(int code, const char* what) {
 
 namespace {
 // A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items |
-// page entries, only for batches with paged items].
+// page entries and BLOCKS items' slice addresses, only for batches with paged items | resolve jobs, only for batches
+// with BLOCKS items], and in the device copy only, behind it, the BLOCKS items' page entries, which the resolve kernel
+// writes: the host neither fills nor copies them.
 size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
 size_t page_table_offset(size_t nd) { return stride_table_offset(nd) + nd * sizeof(XferStride); }
 }  // namespace
@@ -45,16 +47,16 @@ struct XferEngine::Slot {
     FLAG,     // the kernel's status words in pinned memory; no event on the stream (small-object latency path)
     MAILBOX,  // served by the resident mailbox warp: results arrive in the mailbox's result ring
   };
-  // host (pinned): [descs | tile_start | strides | pages], tab_bytes each way
+  // host (pinned): [descs | tile_start | strides | pages | jobs], tab_bytes
   uint8_t* h_tab = nullptr;
-  // device
+  // device: the same, then the BLOCKS items' page entries, dtab_bytes
   uint8_t* d_tab = nullptr;
-  size_t tab_bytes = 0;
+  size_t tab_bytes = 0, dtab_bytes = 0;
   uint64_t* d_sum = nullptr;
   uint32_t* d_done = nullptr;
   uint64_t* d_digest = nullptr;
   uint32_t* d_status = nullptr;
-  // host (pinned) results: [digest | status]
+  // host (pinned) results: [digest | status | verdict], max_items each
   uint8_t* h_res = nullptr;
   uint32_t* d_debug = nullptr;
   size_t d_debug_bytes = 0;
@@ -93,17 +95,49 @@ struct XferEngine::Slot {
   // first entry here until write_pages() turns it into a device address.
   std::vector<uint64_t> pages;
   std::vector<uint32_t> paged_descs;
+  // The resolve jobs of the batch's BLOCKS descriptors; their outer pointers hold indices into `pages`, their entries
+  // (like the stride entries of blocks_descs) indices into the `reserved` device-only entries, and their verdict pointers
+  // descriptor indices, until write_pages() turns them into addresses.
+  std::vector<BlocksJob> jobs;
+  std::vector<uint32_t> blocks_descs;
+  uint64_t reserved = 0;
+  void clear_layouts() {
+    strides.clear();
+    pages.clear();
+    paged_descs.clear();
+    jobs.clear();
+    blocks_descs.clear();
+    reserved = 0;
+  }
   // The table entry of descriptor k's gathered or scattered layout (in bytes, over nbytes): its pattern, or its page
-  // entries.  Returns the XFER_PAGED flag for pages, 0 for rows.
-  uint32_t set_layout(uint32_t k, const DeviceLayout& m, uint64_t nbytes) {
-    if (m.kind() != DeviceLayout::PAGES) {
+  // entries, or for blocks room for them and a resolve job (`get`: the scattering side).  Returns the XFER_PAGED flag for
+  // pages and blocks, 0 for rows.
+  uint32_t set_layout(uint32_t k, const DeviceLayout& m, uint64_t nbytes, bool get) {
+    if (m.kind() == DeviceLayout::ROWS) {
       set_stride(k, XferStride{m.rows().pitch, m.rows().width, m.rows().phase});
       return 0;
     }
-    const SourcePages& p = m.pages();
-    set_stride(k, XferStride{{pages.size()}, p.page, p.phase});
-    paged_descs.push_back(k);
-    pages.insert(pages.end(), p.addrs, p.addrs + p.pages_for(nbytes));
+    if (m.kind() == DeviceLayout::PAGES) {
+      const SourcePages& p = m.pages();
+      paged_descs.push_back(k);
+      set_stride(k, XferStride{{pages.size()}, p.page, p.phase});
+      pages.insert(pages.end(), p.addrs, p.addrs + p.pages_for(nbytes));
+      return XFER_PAGED;
+    }
+    const SourceBlocks& b = m.blocks();
+    BlocksJob j{};
+    blocks_descs.push_back(k);
+    set_stride(k, XferStride{{reserved}, b.page, b.phase});
+    j.entries = reinterpret_cast<uint64_t*>(reserved);
+    j.count = b.pages_for(nbytes);
+    reserved += j.count;
+    j.outer = reinterpret_cast<const uint64_t*>(pages.size());
+    pages.insert(pages.end(), b.outer, b.outer + b.n_outer);
+    j.ids = b.ids, j.sel = b.sel;
+    j.n_outer = b.n_outer, j.n_ids = b.n_ids, j.n_stored = b.n_stored, j.n_blocks = b.n_blocks;
+    j.stride = b.stride, j.first = b.first, j.id_bytes = b.id_bytes, j.get = get;
+    j.verdict = reinterpret_cast<uint32_t*>(static_cast<uintptr_t>(k));
+    jobs.push_back(j);
     return XFER_PAGED;
   }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
@@ -163,13 +197,13 @@ class XferEngine::SlotHold {
 // must not wait for other threads' batches.
 Result<std::unique_ptr<XferEngine::Slot>> XferEngine::new_slot(uint32_t max_items) {
   const size_t tab_bytes = stride_table_offset(max_items) + static_cast<size_t>(max_items) * sizeof(XferStride);
-  const size_t res_bytes = static_cast<size_t>(max_items) * 12;
+  const size_t res_bytes = static_cast<size_t>(max_items) * 16;
   auto s = std::make_unique<Slot>();
   cudaStream_t zero = nullptr;
   bool ok = cudaMallocHost(reinterpret_cast<void**>(&s->h_tab), tab_bytes) == cudaSuccess;
   ok = ok && cudaMallocHost(reinterpret_cast<void**>(&s->h_res), res_bytes) == cudaSuccess;
   ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_tab), tab_bytes) == cudaSuccess;
-  s->tab_bytes = tab_bytes;
+  s->tab_bytes = s->dtab_bytes = tab_bytes;
   ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_sum), static_cast<size_t>(max_items) * 8) == cudaSuccess;
   ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_done), static_cast<size_t>(max_items) * 4) == cudaSuccess;
   ok = ok && cudaMalloc(reinterpret_cast<void**>(&s->d_digest), static_cast<size_t>(max_items) * 8) == cudaSuccess;
@@ -390,35 +424,79 @@ ErrorCode XferEngine::write_tile_table(Slot* s, uint32_t nd) {
   return ErrorCode::OK;
 }
 
-// Appends the batch's page entries to the slot's table of `nd` descriptors (written up to tile_start), growing both
-// copies of the table first when they are too small (the slot is idle: nothing reads them), and points every paged
-// descriptor's stride entry at its first entry in the device copy.  *tab: the bytes of the table to copy to the device.
+// Appends the batch's page entries, slice addresses and resolve jobs to the slot's table of `nd` descriptors (written up
+// to tile_start), growing the table first when it is too small (the slot is idle: nothing reads it), and points every
+// paged descriptor's stride entry at its first entry in the device copy.  The device copy also holds the BLOCKS items'
+// page entries behind the jobs, which only the resolve kernel writes.  *tab: the bytes of the table to copy to the
+// device.
 ErrorCode XferEngine::write_pages(Slot* s, uint32_t nd, size_t* tab) {
-  const size_t off = page_table_offset(nd), need = off + s->pages.size() * sizeof(uint64_t);
-  if (need > s->tab_bytes) {
-    // both new buffers first: on a failure the slot keeps its old, still valid pair
+  const size_t off = page_table_offset(nd), filled = jobs_offset(s, nd) + s->jobs.size() * sizeof(BlocksJob);
+  const size_t need = filled + s->reserved * sizeof(uint64_t);
+  if (filled > s->tab_bytes || need > s->dtab_bytes) {
+    // the new buffers first: on a failure the slot keeps its old, still valid pair
     uint8_t *h = nullptr, *d = nullptr;
-    const cudaError_t eh = cudaMallocHost(reinterpret_cast<void**>(&h), need);
-    const cudaError_t ed = eh == cudaSuccess ? cudaMalloc(reinterpret_cast<void**>(&d), need) : eh;
-    if (ed != cudaSuccess) {
+    cudaError_t e = filled > s->tab_bytes ? cudaMallocHost(reinterpret_cast<void**>(&h), filled) : cudaSuccess;
+    if (e == cudaSuccess && need > s->dtab_bytes) e = cudaMalloc(reinterpret_cast<void**>(&d), need);
+    if (e != cudaSuccess) {
       if (h) cudaFreeHost(h);
       cudaGetLastError();
-      BB_LOG(ERROR) << "XferEngine: growing a descriptor table to " << need << " bytes failed: " << cudaGetErrorString(ed);
+      BB_LOG(ERROR) << "XferEngine: growing a descriptor table to " << need << " bytes failed: " << cudaGetErrorString(e);
       return ErrorCode::OUT_OF_MEMORY;
     }
-    std::memcpy(h, s->h_tab, stride_table_offset(nd));
-    cudaFreeHost(s->h_tab);
-    cudaFree(s->d_tab);
-    s->h_tab = h;
-    s->d_tab = d;
-    s->tab_bytes = need;
+    if (h) {
+      std::memcpy(h, s->h_tab, stride_table_offset(nd));
+      cudaFreeHost(s->h_tab);
+      s->h_tab = h;
+      s->tab_bytes = filled;
+    }
+    if (d) {
+      cudaFree(s->d_tab);
+      s->d_tab = d;
+      s->dtab_bytes = need;
+    }
   }
   const auto d_pages = reinterpret_cast<uint64_t>(s->d_tab + off);
+  const auto d_reserved = reinterpret_cast<uint64_t>(s->d_tab + filled);
   for (uint32_t k : s->paged_descs) s->strides[k].pages = d_pages + s->strides[k].pages * sizeof(uint64_t);
+  for (uint32_t k : s->blocks_descs) s->strides[k].pages = d_reserved + s->strides[k].pages * sizeof(uint64_t);
   s->write_strides(nd);
   std::memcpy(s->h_tab + off, s->pages.data(), s->pages.size() * sizeof(uint64_t));
-  *tab = need;
+  auto* verdicts = reinterpret_cast<uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 12);
+  for (BlocksJob& j : s->jobs) {
+    j.entries = reinterpret_cast<uint64_t*>(d_reserved + reinterpret_cast<uintptr_t>(j.entries) * sizeof(uint64_t));
+    j.outer = reinterpret_cast<const uint64_t*>(d_pages + reinterpret_cast<uintptr_t>(j.outer) * sizeof(uint64_t));
+    j.verdict = verdicts + reinterpret_cast<uintptr_t>(j.verdict);
+    *j.verdict = kBlocksOk;
+  }
+  std::memcpy(s->h_tab + jobs_offset(s, nd), s->jobs.data(), s->jobs.size() * sizeof(BlocksJob));
+  *tab = filled;
   return ErrorCode::OK;
+}
+
+// Queues the resolve kernel of the batch's BLOCKS descriptors on stream `st`, after the copy of the table it reads.
+ErrorCode XferEngine::launch_resolve(Slot* s, uint32_t nd, void* st) {
+  if (s->jobs.empty()) return ErrorCode::OK;
+  const int rc = launch_resolve_blocks(reinterpret_cast<const BlocksJob*>(s->d_tab + jobs_offset(s, nd)), static_cast<uint32_t>(s->jobs.size()), st);
+  if (rc != 0) return cuda_failed(rc, "launch_resolve_blocks");
+  launches_.fetch_add(1, std::memory_order_relaxed);
+  return ErrorCode::OK;
+}
+
+size_t XferEngine::jobs_offset(const Slot* s, uint32_t nd) {
+  return page_table_offset(nd) + s->pages.size() * sizeof(uint64_t);
+}
+
+// The verdict of every item of the slot's last batch: OK, or the resolve kernel's for a BLOCKS item (read once the
+// batch has finished).
+void XferEngine::read_verdicts(const Slot* s, uint32_t nitems, const std::vector<int32_t>& item_to_desc, std::vector<ErrorCode>* out) const {
+  out->assign(nitems, ErrorCode::OK);
+  if (s->jobs.empty()) return;
+  const auto* v = reinterpret_cast<const volatile uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 12);
+  for (uint32_t i = 0; i < nitems; ++i) {
+    const int32_t d = item_to_desc[i];
+    if (d < 0) continue;
+    (*out)[i] = v[d] == kBlocksOutOfRange ? ErrorCode::VALUE_OUT_OF_RANGE : v[d] == kBlocksDuplicate ? ErrorCode::INVALID_ARGUMENT : ErrorCode::OK;
+  }
 }
 
 Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, ChecksumAlgo algo, void* stream,
@@ -433,9 +511,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   s->item_to_desc.assign(items.size(), -1);
   s->empties.clear();
-  s->strides.clear();
-  s->pages.clear();
-  s->paged_descs.clear();
+  s->clear_layouts();
   uint32_t nd = 0;
   bool all_small = small_path_enabled();
   for (size_t i = 0; i < items.size(); ++i) {
@@ -448,10 +524,12 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
                                       (it.flags & (XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
     // a layout is the gathering load's source or the scattering store's destination, the side its flag names
-    if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES) ||
+    const bool blocks = it.mem.kind() == DeviceLayout::BLOCKS;
+    if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES && !blocks) ||
         !(gather ? it.mem.valid_source(it.nbytes) : it.mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
         (scatter && (it.ndst != 1 || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
       return ErrorCode::INVALID_ARGUMENT;
+    if (blocks && scatter && !it.mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
     // below the window and ends with it (an empty window reads nothing).  A verified window reads the whole object.
     const uint64_t nbytes = window_read_bytes(it, algo);
@@ -485,7 +563,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     d.ndst = it.ndst;
     d.expect = it.expect;
     d.flags = it.flags;
-    if (gather || scatter) d.flags |= s->set_layout(nd, it.mem, nbytes);
+    if (gather || scatter) d.flags |= s->set_layout(nd, it.mem, nbytes, scatter);
     d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
     if (algo == ChecksumAlgo::CRC32C) {
       d.expect = (static_cast<uint64_t>(crc_init_term_for(nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
@@ -545,6 +623,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const bool inline_tab = nd <= kInlineDescs && s->pages.empty();  // page entries live in the device table only
     hold.queued(st);
     if (!inline_tab) BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
+    BB_TRY(launch_resolve(s, nd, st));
     if (capture_debug) {
       const size_t need = static_cast<size_t>(s->total_tiles) * tchash::kRows * tchash::kN * 4;
       if (need > s->d_debug_bytes) {
@@ -675,6 +754,7 @@ ErrorCode XferEngine::wait(uint64_t ticket, XferResult* out) {
         out->status[e.item] = ((e.flags & XFER_VERIFY) && digest != want) ? 1u : 0u;
       }
     }
+    read_verdicts(s, s->nitems, s->item_to_desc, &out->verdict);
     out->device_ms = 0.f;
     if (nd && s->completion == Slot::Completion::EVENTS) cudaEventElapsedTime(&out->device_ms, s->ev_start, s->ev_stop);
   }
@@ -708,9 +788,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   auto* descs = reinterpret_cast<XferDesc*>(s->h_tab);
   std::vector<XferItem> scale_items(n);  // scales region of every object, hashed as a RAW_SUM slice by bb_xfer
   // as submit() does: nothing of the slot's last batch (a paged bb_xfer batch's page entries included) carries over
-  s->strides.clear();
-  s->pages.clear();
-  s->paged_descs.clear();
+  s->clear_layouts();
   // one kernel instantiation per launch: bf16 and fp16 items share the 2-byte one, fp32 items take the 4-byte one
   const uint32_t eb = mxfp8::wide_bytes(items[0].wide_type);
   for (uint32_t i = 0; i < n; ++i) {
@@ -724,6 +802,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
     DeviceLayout mem;  // a gathered put's source, or a scattered get's destination, in wide bytes; never with a window
     if (shaped && (!it.win.whole() || !(unpack ? it.mem.valid(it.n_elems) : it.mem.valid_source(it.n_elems)) || !it.mem.to_wide_bytes(eb, &mem)))
       return ErrorCode::INVALID_ARGUMENT;
+    if (unpack && mem.kind() == DeviceLayout::BLOCKS && !mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;
     // a strided window's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
     // first element after row 0's start): the window is checked instead, below
     if ((reinterpret_cast<uintptr_t>(it.packed) & 15) || (!strided && !mem.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
@@ -759,7 +838,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       s->set_stride(i, w);
     }
     if (shaped)  // d.src (gather) or d.dst[0] (scatter) is the layout's base
-      d.flags |= (unpack ? XFER_SCATTER : XFER_GATHER) | s->set_layout(i, mem, eb * it.n_elems);
+      d.flags |= (unpack ? XFER_SCATTER : XFER_GATHER) | s->set_layout(i, mem, eb * it.n_elems, unpack);
     // the fused kernel hashes the whole payload tiles; everything past them (payload tail + scales) is hashed from the
     // stored bytes as a slice
     const uint64_t nt_full = it.n_elems / kTileBytes;
@@ -777,6 +856,7 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   else BB_TRY(write_pages(s, n, &tab));  // may move the table: the launch's pointers are taken below
   release.queued(st);
   BB_CUDA(cudaMemcpyAsync(s->d_tab, s->h_tab, tab, cudaMemcpyHostToDevice, st));
+  BB_TRY(launch_resolve(s, n, st));
   BB_CUDA(cudaMemsetAsync(s->d_digest, 0, static_cast<size_t>(n) * 8, st));
   XferLaunch l;
   l.descs = reinterpret_cast<const XferDesc*>(s->d_tab);
@@ -807,6 +887,9 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       out->digest[i] = tchash::finalize(sums[i] + sres.digest[i], total);
       if (items[i].verify && out->digest[i] != items[i].expect) out->status[i] = 1;
     }
+    std::vector<int32_t> ident(n);
+    for (uint32_t i = 0; i < n; ++i) ident[i] = static_cast<int32_t>(i);
+    read_verdicts(s, n, ident, &out->verdict);
     float ms = 0.f;
     cudaEventElapsedTime(&ms, s->ev_start, s->ev_stop);
     out->device_ms = ms + sres.device_ms;

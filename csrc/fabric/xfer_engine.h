@@ -41,7 +41,10 @@ struct XferItem {
   // (!mem.valid_source(nbytes)), with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM, and XFER_SCATTER with those, XFER_GATHER,
   // XFER_MULTIMEM or ndst != 1.  A scattering store's table may hold null pages: the bytes that fall in them are read and
   // hashed but not stored.  INVALID_ADDRESS unless mem.coaligned(base, nbytes), which replaces the 16-byte alignment check
-  // of the base.
+  // of the base.  Blocks (SourceBlocks) take XFER_PAGED too: their ids stay on the device, the resolve kernel builds the
+  // page entries on `stream` before the transfer kernel, and its verdict comes back in XferResult::verdict; a
+  // scattering store's n_blocks (and n_stored) beyond SourceBlocks::kMaxDistinct is NOT_IMPLEMENTED.  The ids must be
+  // ready on `stream` (stream order), and the outer array need only live until submit() returns.
   DeviceLayout mem;
 };
 
@@ -78,7 +81,7 @@ struct Fp8Item {
   // INVALID_ARGUMENT with a window, unless mem.valid(n_elems) (a pack: mem.valid_source(n_elems)), or when its wide-byte
   // arithmetic overflows;
   // INVALID_ADDRESS unless it is co-aligned in wide bytes (DeviceLayout::coaligned of b * n_elems), which replaces the
-  // 16-byte alignment check of `wide`.
+  // 16-byte alignment check of `wide`.  Blocks as XferItem's, the verdict in XferResult::verdict.
   DeviceLayout mem;
 };
 
@@ -86,6 +89,10 @@ struct XferResult {
   std::vector<uint64_t> digest;  // per item
   std::vector<uint32_t> status;  // per item: 0 ok, 1 checksum mismatch
   float device_ms = 0.f;         // kernel time (CUDA events) of the batch
+  // per item: OK, or for an item laid out in blocks the resolve kernel's verdict on its ids (SourceBlocks):
+  // VALUE_OUT_OF_RANGE or INVALID_ARGUMENT.  A refused item moved nothing outside the caller's tensors: a get stored
+  // nothing, a put read block 0 of every slice instead of the blocks named (its digest must not be recorded).
+  std::vector<ErrorCode> verdict;
 };
 
 // One engine may be shared by many host threads: submit, wait, run and run_fp8 may be called concurrently, each thread
@@ -158,6 +165,9 @@ class XferEngine {
   void release_slot(Slot* s);
   ErrorCode write_tile_table(Slot* s, uint32_t nd);
   ErrorCode write_pages(Slot* s, uint32_t nd, size_t* tab);
+  ErrorCode launch_resolve(Slot* s, uint32_t nd, void* stream);
+  static size_t jobs_offset(const Slot* s, uint32_t nd);
+  void read_verdicts(const Slot* s, uint32_t nitems, const std::vector<int32_t>& item_to_desc, std::vector<ErrorCode>* out) const;
   ErrorCode cuda_failed(int code, const char* what);
   int device_ = 0;
   uint32_t max_items_ = 0;

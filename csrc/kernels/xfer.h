@@ -198,6 +198,29 @@ int launch_xfer_fp8(const XferLaunch& l, bool unpack, uint32_t wide_bytes = 2);
 // Dynamic shared memory of the instantiation for `wide_bytes`-byte elements (its ring stage counts differ).
 int xfer_fp8_smem_bytes(uint32_t wide_bytes = 2);
 
+// ---- page tables from device-resident block ids (resolve_blocks.cu; the rule is SourceBlocks in common/store_window.h)
+// One job fills the page entries of one XFER_PAGED descriptor whose layout is a SourceBlocks: entries[t] is page first + t
+// of the object, t < count.  Every id (and selection entry) of the object is checked first, so that every shard of it
+// reaches the same verdict, which the job writes to *verdict: kBlocksOk, kBlocksOutOfRange or kBlocksDuplicate (a get's
+// repeated id or selection entry).  A refused get's entries are all 0 (null pages: nothing is stored), a refused put's
+// all outer[q] (block 0 of the page's slice, inside the caller's cache).  n_blocks and, with a selection, n_stored are
+// at most kBlocksMaxDistinct for a get.
+constexpr uint32_t kBlocksOk = 0, kBlocksOutOfRange = 1, kBlocksDuplicate = 2;
+constexpr uint64_t kBlocksMaxDistinct = uint64_t{1} << 18;
+struct BlocksJob {
+  uint64_t* entries;
+  const uint64_t* outer;  // device copy of the n_outer slice addresses
+  const void* ids;
+  const void* sel;  // null: no selection
+  uint64_t n_outer, n_ids, n_stored, n_blocks, stride, first, count;
+  uint32_t id_bytes;  // 4 or 8, for ids and sel alike
+  uint32_t get;       // refuse duplicates; a refused table is all null
+  uint32_t* verdict;  // pinned host memory
+  uint32_t pad;
+};
+// Launches one CTA per job of the device table `jobs` on `stream`.  Returns 0 or a cudaError_t value.
+int launch_resolve_blocks(const BlocksJob* jobs, uint32_t njobs, void* stream);
+
 // CRC32C per-object constants (host): un-padding multiplier and the init-register term.
 uint32_t crc_unpad_for(uint64_t nbytes);
 uint32_t crc_init_term_for(uint64_t nbytes);

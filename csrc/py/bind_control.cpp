@@ -13,6 +13,7 @@
 #include "coord/etcd_coord.h"
 #include "coord/coord.h"
 #include "keystone/keystone_service.h"
+#include "py/py_blocks.h"
 #include "rpc/rpc_service.h"
 #include "rpc/wire.h"
 #include "worker/worker_service.h"
@@ -66,7 +67,8 @@ std::vector<std::vector<uint64_t>> to_page_lists(const py::sequence& s) {
   for (auto h : s) out.push_back(to_page_addrs(h));
   return out;
 }
-// SourcePages for Python: the table owns its page addresses (a rebased table shares them).
+// SourcePages for Python: the table owns its page addresses (a rebased table shares them).  SourceBlocks is PyBlocks
+// (py/py_blocks.h), shared with the engine's bindings.
 struct PyPages {
   std::shared_ptr<const std::vector<uint64_t>> addrs;
   SourcePages p;
@@ -449,6 +451,60 @@ void bind_control(py::module_& m) {
              return out;
            },
            py::arg("len"), "[(x, addr, n)]: object bytes [x, x + n) live at [addr, addr + n); adjacent pages make one run");
+
+  py::class_<PyBlocks>(m, "DeviceBlocks",
+                       "Pages of a paged KV cache named by block ids that stay on the device (SourceBlocks, common/store_window.h): "
+                       "page r = q * n_ids + k of the object is at outer[q] + ids[k] * stride.  With a selection (sel, n_stored), "
+                       "a partial restore, the object has n_outer * n_stored pages: page q * n_stored + sel[m] is at outer[q] + "
+                       "ids[m] * stride and the others are not stored.  ids and sel are pointers to n_ids int32 (id_bytes=4) or "
+                       "int64 (id_bytes=8) values; the device route never reads them on the host.")
+      .def(py::init([](const py::handle& outer, uintptr_t ids, uint64_t n_ids, uint64_t n_blocks, uint64_t stride, uint64_t page,
+                       uint32_t id_bytes, uintptr_t sel, uint64_t n_stored) {
+             auto v = std::make_shared<const std::vector<uint64_t>>(to_page_addrs(outer));
+             SourceBlocks b;
+             b.outer = v->data(), b.n_outer = v->size();
+             b.ids = reinterpret_cast<const void*>(ids), b.n_ids = n_ids;
+             b.sel = reinterpret_cast<const void*>(sel), b.n_stored = n_stored;
+             b.id_bytes = id_bytes, b.n_blocks = n_blocks, b.stride = stride, b.page = page;
+             return PyBlocks{v, b};
+           }),
+           py::arg("outer"), py::arg("ids"), py::arg("n_ids"), py::arg("n_blocks"), py::arg("stride"), py::arg("page"),
+           py::arg("id_bytes") = 4, py::arg("sel") = 0, py::arg("n_stored") = 0)
+      .def_property_readonly("outer", [](const PyBlocks& t) { return *t.outer; })
+      .def_property_readonly("page", [](const PyBlocks& t) { return t.b.page; })
+      .def_property_readonly("phase", [](const PyBlocks& t) { return t.b.phase; })
+      .def_property_readonly("first", [](const PyBlocks& t) { return t.b.first; })
+      .def_property_readonly("npages", [](const PyBlocks& t) { return t.b.npages(); })
+      .def("size", [](const PyBlocks& t) {
+             SourceBlocks b;
+             uint64_t size = 0;
+             const ErrorCode ec = SourceBlocks::from_blocks(t.b, &b, &size);
+             return py::make_tuple(ec, size);
+           }, "(ErrorCode, object units) of SourceBlocks::from_blocks")
+      .def("valid", [](const PyBlocks& t, uint64_t len) { return t.b.valid(len); }, py::arg("len"))
+      .def("has_null", [](const PyBlocks& t) { return t.b.has_null(); })
+      .def("distinct_checkable", [](const PyBlocks& t) { return t.b.distinct_checkable(); })
+      .def("rebase", [](const PyBlocks& t, uint64_t off) { return PyBlocks{t.outer, t.b.rebase(off)}; }, py::arg("off"))
+      .def("to_wide_bytes",
+           [](const PyBlocks& t, uint64_t b) {
+             PyBlocks w{t.outer, {}};
+             const bool ok = t.b.to_wide_bytes(b, &w.b);
+             w.b.outer = t.outer->data();
+             return py::make_tuple(ok, w);
+           },
+           py::arg("b"))
+      .def("coaligned", [](const PyBlocks& t, uint64_t len) { return t.b.coaligned(len); }, py::arg("len"))
+      .def("fused_get_aligned", [](const PyBlocks& t, uint64_t off, uint64_t len) { return t.b.fused_get_aligned(off, len); },
+           py::arg("off"), py::arg("len"))
+      .def("resolve",
+           [](const PyBlocks& t, uint64_t count, bool get) {
+             std::vector<uint64_t> table(count);
+             const ErrorCode v = t.b.resolve(table.data(), count, get);
+             return py::make_tuple(v, table);
+           },
+           py::arg("count"), py::arg("get"),
+           "(verdict, entries): the host reference resolve, reading ids and sel as HOST pointers; entries of pages first.. "
+           "first + count");
 
   using alloc::PoolAllocator;
   using alloc::Range;
@@ -1397,6 +1453,42 @@ void bind_control(py::module_& m) {
          "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; a page address "
          "of 0 is not stored (a partial restore: the table still covers the whole object); pages of one get must not "
          "overlap (not checked); returns (one ErrorCode per object, object sizes).")
+      .def("batch_put_device_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
+                                         const WorkerConfig& cfg, uintptr_t stream) {
+        std::vector<SourceBlocks> bs;
+        for (const auto& b : blocks) bs.push_back(b.b);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_blocks(keys, bs, cfg, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("blocks"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
+         "Object i = the pages of blocks[i] (DeviceBlocks), in page order, the page table built on the device from ids that "
+         "stay there; an id out of range is VALUE_OUT_OF_RANGE for that object, whose put is cancelled; returns one "
+         "ErrorCode per object.")
+      .def("batch_get_device_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
+                                         uintptr_t stream) {
+        std::vector<SourceBlocks> bs;
+        for (const auto& b : blocks) bs.push_back(b.b);
+        std::vector<size_t> sizes;
+        const auto ecs = nogil([&] { return c.batch_get_device_blocks(keys, bs, reinterpret_cast<void*>(stream), &sizes); });
+        return py::make_tuple(ecs_to_py(ecs), sizes);
+      }, py::arg("keys"), py::arg("blocks"), py::arg("stream") = 0,
+         "Object i into the pages of blocks[i] (DeviceBlocks; with a selection only the selected stored blocks land); an id "
+         "out of range is VALUE_OUT_OF_RANGE, a repeated one INVALID_ARGUMENT, and then nothing of that object is stored; "
+         "returns (one ErrorCode per object, object sizes).")
+      .def("batch_put_device_fp8_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
+                                             const WorkerConfig& cfg, uintptr_t stream, mxfp8::Wide wide) {
+        std::vector<SourceBlocks> bs;
+        for (const auto& b : blocks) bs.push_back(b.b);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_fp8_blocks(keys, bs, cfg, reinterpret_cast<void*>(stream), wide); }));
+      }, py::arg("keys"), py::arg("blocks"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         "batch_put_device_blocks of packed tensors: object i = the pages of blocks[i] (DeviceBlocks, page in elements of "
+         "`wide`), packed to MXFP8 as the pages are read; returns one ErrorCode per object.")
+      .def("batch_get_device_fp8_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
+                                             uintptr_t stream, mxfp8::Wide wide) {
+        std::vector<SourceBlocks> bs;
+        for (const auto& b : blocks) bs.push_back(b.b);
+        return ecs_to_py(nogil([&] { return c.batch_get_device_fp8_blocks(keys, bs, reinterpret_cast<void*>(stream), wide); }));
+      }, py::arg("keys"), py::arg("blocks"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         "batch_get_device_blocks of packed tensors: object i unpacked into the pages of blocks[i] (page in elements of "
+         "`wide`; with a selection only the selected stored blocks land); returns one ErrorCode per object.")
       .def("batch_put_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
                                             const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, uintptr_t stream,
                                             mxfp8::Wide wide) {

@@ -10,6 +10,7 @@
 #include "fabric/gpu_fabric.h"
 #include "fabric/xfer_engine.h"
 #include "kernels/xfer.h"
+#include "py/py_blocks.h"
 
 namespace py = pybind11;
 using namespace bb;
@@ -46,13 +47,14 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
-// The layout slots of an item tuple (common/store_window.h), first to last: gather rows, scatter rows, source pages and
-// destination pages.  Rows are given as (pitch, width, phase), pages as (addrs, page, phase), whose addresses are kept in
-// `keep` until the batch has been submitted.  Returns the slot set, -1 for none; an item takes one layout, so a second
-// slot is the engine's INVALID_ARGUMENT, raised as `what`.
-int to_layout(const py::tuple& t, const size_t (&slots)[4], std::deque<std::vector<uint64_t>>& keep, DeviceLayout* out, const char* what) {
+// The layout slots of an item tuple (common/store_window.h), first to last: gather rows, scatter rows, source pages,
+// destination pages, source blocks and destination blocks.  Rows are given as (pitch, width, phase), pages as (addrs,
+// page, phase), whose addresses are kept in `keep` until the batch has been submitted, blocks as a DeviceBlocks.  Returns
+// the slot set, -1 for none (even: the source side); an item takes one layout, so a second slot is the engine's
+// INVALID_ARGUMENT, raised as `what`.
+int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vector<uint64_t>>& keep, DeviceLayout* out, const char* what) {
   int set = -1;
-  for (int k = 0; k < 4; ++k) {
+  for (int k = 0; k < 6; ++k) {
     if (t.size() <= slots[k] || t[slots[k]].is_none()) continue;
     if (set >= 0) check(ErrorCode::INVALID_ARGUMENT, what);
     set = k;
@@ -60,6 +62,8 @@ int to_layout(const py::tuple& t, const size_t (&slots)[4], std::deque<std::vect
       auto g = t[slots[k]].cast<std::vector<uint64_t>>();
       if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
       *out = DeviceLayout(SourceRows{g[0], g[1], g[2]});
+    } else if (k >= 4) {
+      *out = DeviceLayout(t[slots[k]].cast<PyBlocks>().b);  // the outer array lives in the Python object until the call returns
     } else {
       auto p = py::cast<py::tuple>(t[slots[k]]);
       if (p.size() != 3) throw py::value_error("pages = (addrs, page, phase)");
@@ -77,7 +81,7 @@ int to_layout(const py::tuple& t, const size_t (&slots)[4], std::deque<std::vect
 // the four.
 XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 11)
+  if (t.size() < 3 || t.size() > 13)
     throw py::value_error(
         "xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, gather (pitch, width, phase)[, scatter "
         "(pitch, width, phase)[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]]])");
@@ -89,10 +93,18 @@ XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
-  static const uint32_t side[4] = {XFER_GATHER, XFER_SCATTER, XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED};
-  const int k = to_layout(t, {7, 8, 9, 10}, keep, &it.mem, "XferEngine.submit");
+  static const uint32_t side[6] = {XFER_GATHER, XFER_SCATTER, XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED,
+                                   XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED};
+  const int k = to_layout(t, {7, 8, 9, 10, 11, 12}, keep, &it.mem, "XferEngine.submit");
   if (k >= 0) it.flags |= side[k];
   return it;
+}
+// (digests, status, device_ms), with the verdicts behind them when an item is laid out in blocks.
+template <class Item>
+py::tuple results(const std::vector<Item>& items, const XferResult& res) {
+  for (const Item& it : items)
+    if (it.mem.kind() == DeviceLayout::BLOCKS) return py::make_tuple(res.digest, res.status, res.device_ms, res.verdict);
+  return py::make_tuple(res.digest, res.status, res.device_ms);
 }
 }  // namespace
 
@@ -132,7 +144,7 @@ void bind_gpu(py::module_& m) {
                if (!t.ok()) check(t.error(), "XferEngine.submit");
                check(e.wait(t.value(), &res), "XferEngine.wait");
              }
-             return py::make_tuple(res.digest, res.status, res.device_ms);
+             return results(v, res);
            },
            py::arg("items"), py::arg("algo") = ChecksumAlgo::BBH64, py::arg("stream") = 0, py::arg("debug") = false,
            "Runs one fused batch; items = (src, dst | [dst, ...], nbytes[, expect[, flags[, tile_base[, (lo, hi)]]]]), where [] "
@@ -147,7 +159,10 @@ void bind_gpu(py::module_& m) {
            "phase) // width) * pitch + (x + phase) % width.  Source pages (addrs, page, phase) as the tenth element set "
            "XFER_GATHER | XFER_PAGED: object byte x is read from addrs[(x + phase) // page] + (x + phase) % page (src is "
            "not read); destination pages as the eleventh set XFER_SCATTER | XFER_PAGED and store by the same rule (dst is "
-           "not read); returns (digests, status, device_ms).")
+           "not read); source blocks (a DeviceBlocks, ids on the device) as the twelfth and destination blocks as the "
+           "thirteenth do the same with a page table the resolve kernel builds on the stream; returns (digests, status, "
+           "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item (VALUE_OUT_OF_RANGE or "
+           "INVALID_ARGUMENT for refused ids).")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream, mxfp8::Wide wide) {
              std::vector<gpu::Fp8Item> v;
@@ -164,7 +179,7 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 10)
+               if (t.size() < 3 || t.size() > 12)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
                      "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
@@ -172,7 +187,7 @@ void bind_gpu(py::module_& m) {
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
                // the gather slots are a pack's, the scatter slots an unpack's
-               const int k = to_layout(t, {5, 6, 8, 9}, keep, &it.mem, "XferEngine.run_fp8");
+               const int k = to_layout(t, {5, 6, 8, 9, 10, 11}, keep, &it.mem, "XferEngine.run_fp8");
                if (k >= 0 && (k % 2 == 1) != unpack) check(ErrorCode::INVALID_ARGUMENT, "XferEngine.run_fp8");
                v.push_back(it);
              }
@@ -181,7 +196,7 @@ void bind_gpu(py::module_& m) {
                py::gil_scoped_release rel;
                check(e.run_fp8(v, unpack, reinterpret_cast<void*>(stream), &res), "XferEngine.run_fp8");
              }
-             return py::make_tuple(res.digest, res.status, res.device_ms);
+             return results(v, res);
            },
            py::arg("items"), py::arg("unpack"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
            "`wide` (MxWide) is the element type of every item's wide side: bf16, fp16 or fp32, unless an item gives its own as "
@@ -206,8 +221,10 @@ void bind_gpu(py::module_& m) {
            "elements, as the ninth element read element x from addrs[(x + phase) // page] + 2 * ((x + phase) % page) "
            "(bf16_ptr is not read); a get's destination pages as the tenth store by the same rule.  INVALID_ARGUMENT for "
            "pages on the wrong side, with rows or a window, phase >= page or a table too short; INVALID_ADDRESS unless "
-           "every page touched is co-aligned in wide bytes and, for several pages, page % 8 == 0.  Returns (digests of the "
-           "packed objects, status, device_ms).")
+           "every page touched is co-aligned in wide bytes and, for several pages, page % 8 == 0.  A put's source blocks "
+           "(DeviceBlocks, page in elements) as the eleventh element and a get's destination blocks as the twelfth take a "
+           "page table the resolve kernel builds on the stream.  Returns (digests of the packed objects, status, "
+           "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item.")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
