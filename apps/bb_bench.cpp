@@ -180,20 +180,18 @@ int main(int argc, char** argv) {
     // reaches it over the same-host shared-memory channel), synthetic GPU pools, and a transport whose transfers are free.
     // What is left is exactly what bounds batches of small objects: Keystone round trips + the client's own per-object work.
     struct NullTransport : client::DeviceTransport {
-      // ticket = launch number; the batch's op count is all wait_* needs
+      // ticket = launch number; the batch's op count is all wait needs
       Result<uint64_t> submit_put(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>&, ChecksumAlgo,
                                   void*) override {
         return submit(ops.size());
       }
-      ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override {
-        if (digests) digests->assign(take(ticket), 0x1234);
-        return ErrorCode::OK;
-      }
       Result<uint64_t> submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>&, void*) override {
         return submit(ops.size());
       }
-      ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override {
-        if (status) status->assign(take(ticket), 0);
+      ErrorCode wait(uint64_t ticket, client::DeviceBatchResult* res) override {
+        const size_t nops = nops_of[ticket];
+        nops_of.erase(ticket);
+        *res = {std::vector<uint64_t>(nops, 0x1234), std::vector<uint32_t>(nops, 0), std::vector<ErrorCode>(nops, ErrorCode::OK)};
         return ErrorCode::OK;
       }
       bool can_reach(const ShardPlacement&) const override { return true; }
@@ -201,11 +199,6 @@ int main(int argc, char** argv) {
       uint64_t submit(size_t nops) {
         nops_of[++n] = nops;
         return n;
-      }
-      size_t take(uint64_t ticket) {
-        const size_t nops = nops_of[ticket];
-        nops_of.erase(ticket);
-        return nops;
       }
       uint64_t n = 0;
       std::map<uint64_t, size_t> nops_of;

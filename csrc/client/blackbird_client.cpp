@@ -609,12 +609,11 @@ static std::vector<T> pick(const std::vector<T>& v, const std::vector<size_t>& i
   return out;
 }
 
-// The shaped calls (strided puts; range and strided gets; bytes and MXFP8) over put_device, put_device_fp8, get_device and
-// get_device_fp8.  Unless `arity_ok`, every item is INVALID_PARAMETERS (CLIENT_DISCONNECTED without a Keystone).  Then
-// shape(i, &bytes) records item i's shape and returns its error.  For a put (`admit`) an item with an error fails here,
-// before the Keystone allocates anything for it, and run(idx) puts the others as one batch, or nothing runs when there
-// are none.  A get refuses no item here (the Keystone's answer comes first), and run(idx) gets them all, an empty batch
-// included.  <name>_total and <name>_bytes_total count the OK items and their `bytes`.
+// The shaped calls over put_device, put_device_fp8, get_device and get_device_fp8.  Unless `arity_ok`, every item is
+// INVALID_PARAMETERS (CLIENT_DISCONNECTED without a Keystone).  Then shape(i, &bytes) records item i's shape and returns
+// its error.  For a put (`admit`) an item with an error fails here, before the Keystone allocates anything for it, and
+// run(idx) puts the others as one batch, or nothing runs when there are none.  A get runs run(idx) for the others, an
+// empty batch included.  <name>_total and <name>_bytes_total count the OK items and their `bytes`.
 template <class Shape, class Run>
 std::vector<ErrorCode> BlackbirdClient::shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run) {
   if (!arity_ok) return std::vector<ErrorCode>(n, keystone_ ? ErrorCode::INVALID_PARAMETERS : ErrorCode::CLIENT_DISCONNECTED);
@@ -636,6 +635,101 @@ std::vector<ErrorCode> BlackbirdClient::shaped_batch(std::string_view name, bool
   metrics_.inc(std::string(name) + "_total", done);
   metrics_.inc(std::string(name) + "_bytes_total", total);
   return out;
+}
+
+// What the builder of a shaped put or get makes of item i: the layout of the caller's side and the object's size, in
+// bytes or, for MXFP8, in elements of the wide side.  `table`: the size is that of a page table (pages or blocks), not of
+// rows.
+struct ShapedItem {
+  DeviceLayout mem;
+  uint64_t units = 0;
+  bool table = false;
+};
+
+static ErrorCode rows_item(uint64_t width, uint64_t pitch, uint64_t rows, ShapedItem* it) {
+  uint64_t extent = 0;  // admit_shaped has it from the layout
+  return DeviceLayout::from_rows(width, pitch, rows, &it->mem, &it->units, &extent);
+}
+
+static ErrorCode pages_item(const std::vector<uint64_t>& pages, uint64_t page, ShapedItem* it) {
+  it->table = true;
+  return DeviceLayout::from_pages(pages.size(), page, pages.data(), &it->mem, &it->units);
+}
+
+static ErrorCode blocks_item(const SourceBlocks& blocks, ShapedItem* it) {
+  SourceBlocks b;
+  const ErrorCode ec = SourceBlocks::from_blocks(blocks, &b, &it->units);
+  it->mem = DeviceLayout(b);
+  it->table = true;
+  return ec;
+}
+
+// The admission rule of the shaped calls (blackbird_client.h), in this order: an item of a put or a get of units of b
+// bytes (`packed`: MXFP8 elements), its layout at `base`.
+static ErrorCode admit_shaped(const ShapedItem& it, bool put, uint64_t b, bool packed, const void* base) {
+  const DeviceLayout& m = it.mem;
+  const uint64_t u = it.units;
+  if (packed && it.table && (u == 0 || u % 32)) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
+  if (put && (m.pages().has_null(u) || m.blocks().has_null())) return ErrorCode::INVALID_ARGUMENT;  // a put reads every unit
+  if (u > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+  DeviceLayout bytes;
+  const uint64_t extent = m.kind() == DeviceLayout::ROWS ? m.rows().extent(u) : u;
+  if (packed && (extent > UINT64_MAX / b || !m.to_wide_bytes(b, &bytes))) return ErrorCode::VALUE_OUT_OF_RANGE;
+  // the engine's rule for a gathering pack, checked once: there is no host-staged path for packed puts
+  if (packed && put && !bytes.coaligned(reinterpret_cast<uintptr_t>(base), b * u)) return ErrorCode::NOT_IMPLEMENTED;
+  // the resolve kernel checks a get's ids for duplicates in a bitmap of bounded size: larger caches are the caller's
+  if (!put && !m.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;
+  return ErrorCode::OK;
+}
+
+template <class Build>
+std::vector<ErrorCode> BlackbirdClient::shaped_put(std::string_view name, const std::vector<ObjectKey>& keys, const std::vector<const void*>& ptrs,
+                                                   bool arity_ok, std::optional<mxfp8::Wide> fp8, Build&& build, const WorkerConfig& cfg,
+                                                   void* stream) {
+  const uint64_t b = fp8 ? mxfp8::wide_bytes(*fp8) : 1;
+  std::vector<ShapedItem> items(keys.size());
+  return shaped_batch(
+      name, true, keys.size(), arity_ok,
+      [&](size_t i, uint64_t* bytes) {
+        ErrorCode ec = build(i, &items[i]);
+        if (ec == ErrorCode::OK) ec = admit_shaped(items[i], true, b, fp8.has_value(), ptrs[i]);
+        *bytes = b * items[i].units;
+        return ec;
+      },
+      [&](const std::vector<size_t>& idx) {
+        std::vector<DeviceLayout> mems;
+        std::vector<uint64_t> units;
+        for (size_t i : idx) mems.push_back(items[i].mem), units.push_back(items[i].units);
+        if (fp8) return put_device_fp8(pick(keys, idx), pick(ptrs, idx), units, &mems, cfg, stream, *fp8);
+        return put_device(pick(keys, idx), pick(ptrs, idx), std::vector<size_t>(units.begin(), units.end()), &mems, cfg, stream);
+      });
+}
+
+template <class Build>
+std::vector<ErrorCode> BlackbirdClient::shaped_get(std::string_view name, const std::vector<ObjectKey>& keys, const std::vector<void*>& ptrs,
+                                                   bool arity_ok, std::optional<mxfp8::Wide> fp8, Build&& build, void* stream,
+                                                   std::vector<size_t>* out_sizes) {
+  const uint64_t b = fp8 ? mxfp8::wide_bytes(*fp8) : 1;
+  std::vector<ShapedItem> items(keys.size());
+  if (out_sizes) out_sizes->assign(keys.size(), 0);
+  return shaped_batch(
+      name, false, keys.size(), arity_ok,
+      [&](size_t i, uint64_t* bytes) {
+        ErrorCode ec = build(i, &items[i]);
+        if (ec == ErrorCode::OK) ec = admit_shaped(items[i], false, b, fp8.has_value(), ptrs[i]);
+        *bytes = b * items[i].units;
+        return ec;
+      },
+      [&](const std::vector<size_t>& idx) {
+        std::vector<DeviceLayout> mems;
+        std::vector<uint64_t> units;
+        for (size_t i : idx) mems.push_back(items[i].mem), units.push_back(items[i].units);
+        if (fp8) return get_device_fp8(pick(keys, idx), pick(ptrs, idx), units, nullptr, &mems, stream, *fp8);
+        std::vector<size_t> sizes;
+        auto ecs = get_device(pick(keys, idx), pick(ptrs, idx), std::vector<size_t>(units.begin(), units.end()), nullptr, &mems, stream, &sizes);
+        for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
+        return ecs;
+      });
 }
 
 // A digest mismatch on every replica can also mean that the Keystone moved the object under us (tier move, compaction,
@@ -680,53 +774,19 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::
                                                                      const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream,
                                                                      mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<uint64_t> elems(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_fp8_strided", true, n, bf16_ptrs.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        DeviceLayout bytes;
-        uint64_t extent = 0;
-        const ErrorCode ec = DeviceLayout::from_rows(elem_widths[i], elem_pitches[i], rows[i], &mems[i], &elems[i], &extent);
-        *wide_bytes = b * elems[i];
-        if (ec != ErrorCode::OK) return ec;
-        if (extent > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
-        // the engine's rule for a gathered put, checked once: there is no host-staged path for packed puts
-        if (!bytes.coaligned(reinterpret_cast<uintptr_t>(bf16_ptrs[i]), b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(elems, idx), &m, cfg, stream, wide);
-      });
+  return shaped_put(
+      "device_put_fp8_strided", keys, bf16_ptrs,
+      bf16_ptrs.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return rows_item(elem_widths[i], elem_pitches[i], rows[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                    const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
                                                                    mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<uint64_t> elems(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_fp8_paged", true, n, pages.size() == n && page_elems.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &mems[i], &elems[i]);
-        if (ec != ErrorCode::OK) return ec;
-        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks
-        if (!mems[i].valid_source(elems[i])) return ErrorCode::INVALID_ARGUMENT;  // a null page: a put reads every element
-        DeviceLayout bytes;
-        if (elems[i] > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
-        *wide_bytes = b * elems[i];
-        // the engine's rule for a paged pack, checked once: there is no host-staged path for packed puts
-        if (!bytes.coaligned(0, b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), &m, cfg, stream, wide);
-      });
+  return shaped_put(
+      "device_put_fp8_paged", keys, std::vector<const void*>(n), pages.size() == n && page_elems.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
@@ -771,20 +831,19 @@ std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectK
     ops.push_back(std::move(op));
     idx.push_back(i);
   }
-  std::vector<uint64_t> digests;
-  std::vector<ErrorCode> verdicts;
-  ErrorCode ec = ops.empty() ? ErrorCode::OK : device_->put_fp8_verdicts(ops, stream, &digests, &verdicts);
+  DeviceBatchResult res;
+  ErrorCode ec = ops.empty() ? ErrorCode::OK : device_->run_fp8(ops, false, stream, &res);
   std::vector<ObjectKey> done;
   std::vector<ShardChecksums> sums;
   for (size_t k = 0; k < idx.size(); ++k) {
-    const ErrorCode v = k < verdicts.size() ? verdicts[k] : ErrorCode::OK;  // refused ids: the answer, and no digest
-    if (ec != ErrorCode::OK || digests.size() != idx.size() || v != ErrorCode::OK) {
+    const ErrorCode v = ec != ErrorCode::OK ? ec : res.verdicts[k];  // refused ids: the answer, and no digest
+    if (v != ErrorCode::OK || res.digests.size() != idx.size()) {
       keystone_->put_cancel(keys[idx[k]]);
-      out[idx[k]] = ec != ErrorCode::OK ? ec : v != ErrorCode::OK ? v : ErrorCode::INTERNAL_ERROR;
+      out[idx[k]] = v != ErrorCode::OK ? v : ErrorCode::INTERNAL_ERROR;
       continue;
     }
     done.push_back(keys[idx[k]]);
-    sums.push_back(ShardChecksums(placed[idx[k]].value().size(), std::vector<uint64_t>{digests[k]}));  // same bytes in every copy
+    sums.push_back(ShardChecksums(placed[idx[k]].value().size(), std::vector<uint64_t>{res.digests[k]}));  // same bytes in every copy
   }
   if (!done.empty()) {
     auto r = keystone_->batch_put_complete(done, sums);
@@ -806,25 +865,14 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_scatter(const std::
                                                                      const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
                                                                      void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_get_fp8_scatter", false, n,
-      bf16_ptrs.size() == n && n_elems.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        DeviceLayout bytes;
-        uint64_t elems = 0, extent = 0;
-        const ErrorCode ec = DeviceLayout::from_rows(elem_widths[i], elem_pitches[i], rows[i], &mems[i], &elems, &extent);
-        if (ec != ErrorCode::OK) return ec;
-        if (elems != n_elems[i]) return ErrorCode::INVALID_ARGUMENT;
-        if (extent > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
-        *wide_bytes = b * elems;
-        return ErrorCode::OK;
+  return shaped_get(
+      "device_get_fp8_scatter", keys, bf16_ptrs,
+      bf16_ptrs.size() == n && n_elems.size() == n && elem_widths.size() == n && elem_pitches.size() == n && rows.size() == n, wide,
+      [&](size_t i, ShapedItem* it) {
+        const ErrorCode ec = rows_item(elem_widths[i], elem_pitches[i], rows[i], it);
+        return ec != ErrorCode::OK || it->units == n_elems[i] ? ec : ErrorCode::INVALID_ARGUMENT;
       },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), nullptr, &m, stream, wide);
-      });
+      stream, nullptr);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -863,75 +911,25 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                    const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<uint64_t> elems(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_get_fp8_paged", false, n, pages.size() == n && page_elems.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_elems[i], pages[i].data(), &mems[i], &elems[i]);
-        if (ec != ErrorCode::OK) return ec;
-        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
-        if (elems[i] > UINT64_MAX / b) return ErrorCode::VALUE_OUT_OF_RANGE;
-        *wide_bytes = b * elems[i];
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, &m, stream, wide);
-      });
+  return shaped_get(
+      "device_get_fp8_paged", keys, std::vector<void*>(n), pages.size() == n && page_elems.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], it); }, stream, nullptr);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                                     const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<uint64_t> elems(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_fp8_blocks", true, n, blocks.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        SourceBlocks sb;
-        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &sb, &elems[i]);
-        if (ec != ErrorCode::OK) return ec;
-        if (elems[i] == 0 || elems[i] % 32 || sb.has_null()) return ErrorCode::INVALID_ARGUMENT;  // whole MX blocks; a put reads every page
-        mems[i] = DeviceLayout(sb);
-        DeviceLayout bytes;
-        if (elems[i] > UINT64_MAX / b || !mems[i].to_wide_bytes(b, &bytes)) return ErrorCode::VALUE_OUT_OF_RANGE;
-        *wide_bytes = b * elems[i];
-        // the engine's rule for a pack from blocks, checked once: there is no host-staged path for packed puts
-        if (!bytes.coaligned(0, b * elems[i])) return ErrorCode::NOT_IMPLEMENTED;
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device_fp8(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(elems, idx), &m, cfg, stream, wide);
-      });
+  return shaped_put(
+      "device_put_fp8_blocks", keys, std::vector<const void*>(n), blocks.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return blocks_item(blocks[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                                     void* stream, mxfp8::Wide wide) {
   const size_t n = keys.size();
-  const uint64_t b = mxfp8::wide_bytes(wide);
-  std::vector<uint64_t> elems(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_get_fp8_blocks", false, n, blocks.size() == n,
-      [&](size_t i, uint64_t* wide_bytes) {
-        SourceBlocks sb;
-        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &sb, &elems[i]);
-        if (ec != ErrorCode::OK) return ec;
-        if (elems[i] == 0 || elems[i] % 32) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
-        if (elems[i] > UINT64_MAX / b) return ErrorCode::VALUE_OUT_OF_RANGE;
-        if (!sb.distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // the resolve kernel's duplicate bitmap is bounded
-        mems[i] = DeviceLayout(sb);
-        *wide_bytes = b * elems[i];
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return get_device_fp8(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(elems, idx), nullptr, &m, stream, wide);
-      });
+  return shaped_get(
+      "device_get_fp8_blocks", keys, std::vector<void*>(n), blocks.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return blocks_item(blocks[i], it); }, stream, nullptr);
 }
 
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
@@ -1024,14 +1022,13 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     }
     if (ops.empty()) break;
     if (attempt > 0) metrics_.inc("replica_failover_total");
-    std::vector<uint32_t> status;
-    std::vector<ErrorCode> verdicts;
-    ErrorCode ec = device_->get_fp8_verdicts(ops, stream, &status, &verdicts);
+    DeviceBatchResult res;
+    ErrorCode ec = device_->run_fp8(ops, true, stream, &res);
     todo.clear();
     for (size_t k = 0; k < cur.size(); ++k) {
-      if (ec != ErrorCode::OK || status.size() != cur.size()) out[cur[k]] = ec != ErrorCode::OK ? ec : ErrorCode::INTERNAL_ERROR;
-      else if (k < verdicts.size() && verdicts[k] != ErrorCode::OK) out[cur[k]] = verdicts[k];  // its ids, not its copy: no fail-over
-      else if (status[k]) todo.push_back(cur[k]);
+      if (ec != ErrorCode::OK || res.status.size() != cur.size()) out[cur[k]] = ec != ErrorCode::OK ? ec : ErrorCode::INTERNAL_ERROR;
+      else if (res.verdicts[k] != ErrorCode::OK) out[cur[k]] = res.verdicts[k];  // its ids, not its copy: no fail-over
+      else if (res.status[k]) todo.push_back(cur[k]);
       else out[cur[k]] = ErrorCode::OK;
     }
   }
@@ -1205,43 +1202,17 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vect
                                                                  const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                                  const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
-  std::vector<size_t> sizes(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_strided", true, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* size) {
-        uint64_t extent = 0;
-        const ErrorCode ec = DeviceLayout::from_rows(widths[i], pitches[i], rows[i], &mems[i], size, &extent);
-        if (ec != ErrorCode::OK) return ec;
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        sizes[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device(pick(keys, idx), pick(dev_ptrs, idx), pick(sizes, idx), &m, cfg, stream);
-      });
+  return shaped_put(
+      "device_put_strided", keys, dev_ptrs, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
+      std::nullopt, [&](size_t i, ShapedItem* it) { return rows_item(widths[i], pitches[i], rows[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
-  std::vector<size_t> sizes(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_paged", true, n, pages.size() == n && page_bytes.size() == n,
-      [&](size_t i, uint64_t* size) {
-        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &mems[i], size);
-        if (ec != ErrorCode::OK) return ec;
-        if (!mems[i].valid_source(*size)) return ErrorCode::INVALID_ARGUMENT;  // a null page: a put reads every byte
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        sizes[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), &m, cfg, stream);
-      });
+  return shaped_put(
+      "device_put_paged", keys, std::vector<const void*>(n), pages.size() == n && page_bytes.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
@@ -1350,13 +1321,12 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
 
   auto finish_chunk = [&](Chunk& ch) {
     BB_TRACE_SPAN("finish_chunk", ch.end - ch.begin);
-    std::vector<uint64_t> digests;
-    std::vector<ErrorCode> verdicts;
+    DeviceBatchResult res;
     ErrorCode ec = ch.submit_error;
     const TimePoint t1 = Clock::now();
-    if (ch.submitted) ec = device_->wait_put_verdicts(ch.ticket, &digests, &verdicts);
-    for (size_t k = 0; ec == ErrorCode::OK && k < verdicts.size(); ++k)  // refused ids: the item's answer, and no digest
-      if (verdicts[k] != ErrorCode::OK && !refused[ch.ops[k].item]) out[ch.ops[k].item] = verdicts[k], refused[ch.ops[k].item] = true;
+    if (ch.submitted) ec = device_->wait(ch.ticket, &res);
+    for (size_t k = 0; ec == ErrorCode::OK && k < ch.ops.size(); ++k)  // refused ids: the item's answer, and no digest
+      if (res.verdicts[k] != ErrorCode::OK && !refused[ch.ops[k].item]) out[ch.ops[k].item] = res.verdicts[k], refused[ch.ops[k].item] = true;
     metrics_.observe("phase_put_wait_us", us_since(t1));
     const TimePoint t2 = Clock::now();
     std::vector<ObjectKey> done_keys, cancel_keys;
@@ -1382,8 +1352,8 @@ std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>&
       for (size_t k = 0; k < ch.ops.size(); ++k) {
         const auto& op = ch.ops[k];
         auto& sm = sums[op.item - ch.begin];
-        sm[op.copy][op.shard] = digests[k];
-        for (size_t r = 0; r < op.replicas.size(); ++r) sm[r + 1][op.shard] = digests[k];
+        sm[op.copy][op.shard] = res.digests[k];
+        for (size_t r = 0; r < op.replicas.size(); ++r) sm[r + 1][op.shard] = res.digests[k];
       }
       for (size_t i = ch.begin; i < ch.end; ++i)
         if (ch.placed[i - ch.begin].ok() && !host_placed.count(i) && !refused[i]) {
@@ -1437,110 +1407,33 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_scatter(const std::vect
                                                                  const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                                  const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes) {
   const size_t n = keys.size();
-  std::vector<size_t> caps(n);
-  std::vector<DeviceLayout> mems(n);
-  if (out_sizes) out_sizes->assign(n, 0);
-  return shaped_batch(
-      "device_get_scatter", false, n, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
-      [&](size_t i, uint64_t* size) {
-        uint64_t extent = 0;
-        const ErrorCode ec = DeviceLayout::from_rows(widths[i], pitches[i], rows[i], &mems[i], size, &extent);
-        if (ec != ErrorCode::OK) return ec;
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        caps[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        std::vector<size_t> sizes;
-        auto ecs = get_device(pick(keys, idx), pick(dev_ptrs, idx), pick(caps, idx), nullptr, &m, stream, &sizes);
-        for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
-        return ecs;
-      });
+  return shaped_get(
+      "device_get_scatter", keys, dev_ptrs, dev_ptrs.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n,
+      std::nullopt, [&](size_t i, ShapedItem* it) { return rows_item(widths[i], pitches[i], rows[i], it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes) {
   const size_t n = keys.size();
-  std::vector<size_t> caps(n);
-  std::vector<DeviceLayout> mems(n);
-  if (out_sizes) out_sizes->assign(n, 0);
-  return shaped_batch(
-      "device_get_paged", false, n, pages.size() == n && page_bytes.size() == n,
-      [&](size_t i, uint64_t* size) {
-        const ErrorCode ec = DeviceLayout::from_pages(pages[i].size(), page_bytes[i], pages[i].data(), &mems[i], size);
-        if (ec != ErrorCode::OK) return ec;
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        caps[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        std::vector<size_t> sizes;
-        auto ecs = get_device(pick(keys, idx), std::vector<void*>(idx.size(), nullptr), pick(caps, idx), nullptr, &m, stream, &sizes);
-        for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
-        return ecs;
-      });
+  return shaped_get(
+      "device_get_paged", keys, std::vector<void*>(n), pages.size() == n && page_bytes.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                                 const WorkerConfig& cfg, void* stream) {
   const size_t n = keys.size();
-  std::vector<size_t> sizes(n);
-  std::vector<DeviceLayout> mems(n);
-  return shaped_batch(
-      "device_put_blocks", true, n, blocks.size() == n,
-      [&](size_t i, uint64_t* size) {
-        SourceBlocks b;
-        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &b, size);
-        if (ec != ErrorCode::OK) return ec;
-        if (b.has_null()) return ErrorCode::INVALID_ARGUMENT;  // a selection: a put reads every page
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        mems[i] = DeviceLayout(b);
-        sizes[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        const auto m = pick(mems, idx);
-        return put_device(pick(keys, idx), std::vector<const void*>(idx.size(), nullptr), pick(sizes, idx), &m, cfg, stream);
-      });
+  return shaped_put(
+      "device_put_blocks", keys, std::vector<const void*>(n), blocks.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return blocks_item(blocks[i], it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                                 void* stream, std::vector<size_t>* out_sizes) {
   const size_t n = keys.size();
-  std::vector<size_t> caps(n);
-  std::vector<DeviceLayout> mems(n);
-  std::vector<bool> checkable(n, true);
-  if (out_sizes) out_sizes->assign(n, 0);
-  return shaped_batch(
-      "device_get_blocks", false, n, blocks.size() == n,
-      [&](size_t i, uint64_t* size) {
-        SourceBlocks b;
-        const ErrorCode ec = SourceBlocks::from_blocks(blocks[i], &b, size);
-        if (ec != ErrorCode::OK) return ec;
-        if (*size > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
-        mems[i] = DeviceLayout(b);
-        caps[i] = static_cast<size_t>(*size);
-        return ErrorCode::OK;
-      },
-      [&](const std::vector<size_t>& idx) {
-        // the resolve kernel checks a get's ids for duplicates in a bitmap of bounded size: larger caches are the caller's
-        std::vector<size_t> run;
-        std::vector<ErrorCode> ecs(idx.size(), ErrorCode::NOT_IMPLEMENTED);
-        for (size_t i : idx)
-          if (mems[i].blocks().distinct_checkable()) run.push_back(i);
-        const auto m = pick(mems, run);
-        std::vector<size_t> sizes;
-        const auto got = get_device(pick(keys, run), std::vector<void*>(run.size(), nullptr), pick(caps, run), nullptr, &m, stream, &sizes);
-        for (size_t k = 0, j = 0; k < idx.size() && j < run.size(); ++k)
-          if (idx[k] == run[j]) {
-            ecs[k] = got[j];
-            if (out_sizes && j < sizes.size()) (*out_sizes)[idx[k]] = sizes[j];
-            ++j;
-          }
-        return ecs;
-      });
+  return shaped_get(
+      "device_get_blocks", keys, std::vector<void*>(n), blocks.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return blocks_item(blocks[i], it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_range(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
@@ -1628,14 +1521,13 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
     }
   };
   // A verdict on an item's block ids answers it, ahead of its digests: its ids, not its copy, are wrong.
-  auto apply_status = [&](const std::vector<DeviceShardOp>& ops, const std::vector<uint32_t>& status, const std::vector<ErrorCode>& verdicts,
-                          std::vector<size_t>* retry) {
+  auto apply_status = [&](const std::vector<DeviceShardOp>& ops, const DeviceBatchResult& res, std::vector<size_t>* retry) {
     std::vector<bool> bad(keys.size(), false), seen(keys.size(), false);
     for (size_t k = 0; k < ops.size(); ++k) {
       seen[ops[k].item] = true;
-      if (status[k] != 0) bad[ops[k].item] = true;
-      if (k < verdicts.size() && verdicts[k] != ErrorCode::OK && pending[ops[k].item]) {
-        out[ops[k].item] = verdicts[k];
+      if (res.status[k] != 0) bad[ops[k].item] = true;
+      if (res.verdicts[k] != ErrorCode::OK && pending[ops[k].item]) {
+        out[ops[k].item] = res.verdicts[k];
         pending[ops[k].item] = false;
       }
     }
@@ -1801,11 +1693,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   auto finish_chunk = [&](Chunk& ch) {
     BB_TRACE_SPAN("finish_chunk", ch.end - ch.begin);
     if (ch.ops.empty()) return;
-    std::vector<uint32_t> status;
-    std::vector<ErrorCode> verdicts;
+    DeviceBatchResult res;
     ErrorCode ec = ch.err;
     const TimePoint t1 = Clock::now();
-    if (ch.submitted) ec = device_->wait_get_verdicts(ch.ticket, &status, &verdicts);
+    if (ch.submitted) ec = device_->wait(ch.ticket, &res);
     metrics_.observe("phase_get_wait_us", us_since(t1));
     if (ec != ErrorCode::OK) {
       for (size_t i = ch.begin; i < ch.end; ++i)
@@ -1815,7 +1706,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         }
       return;
     }
-    apply_status(ch.ops, status, verdicts, &retry);
+    apply_status(ch.ops, res, &retry);
   };
   const size_t depth = std::max<size_t>(1, std::min<size_t>(2, device_->max_in_flight()));
   size_t finished = 0;
@@ -1840,10 +1731,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
     build_ops(0, keys.size(), ops);
     if (ops.empty()) break;
     metrics_.inc("replica_failover_total");
-    std::vector<uint32_t> status;
-    std::vector<ErrorCode> verdicts;
+    DeviceBatchResult res;
     auto t = device_->submit_get(ops, bases, stream);
-    ErrorCode ec = t.ok() ? device_->wait_get_verdicts(t.value(), &status, &verdicts) : t.error();
+    ErrorCode ec = t.ok() ? device_->wait(t.value(), &res) : t.error();
     if (ec != ErrorCode::OK) {
       for (size_t i = 0; i < keys.size(); ++i)
         if (pending[i]) {
@@ -1852,7 +1742,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         }
       break;
     }
-    apply_status(ops, status, verdicts, &still);
+    apply_status(ops, res, &still);
     retry.swap(still);
   }
   for (size_t i = 0; i < keys.size(); ++i)
@@ -1903,7 +1793,7 @@ Result<uint64_t> HostLoopbackTransport::submit_put(const std::vector<DeviceShard
     if (ec != ErrorCode::OK) return ec;
   }
   std::lock_guard<std::mutex> lk(done_mu_);
-  done_[next_ticket_] = {std::move(digests), {}, std::move(verdicts)};
+  done_[next_ticket_] = {std::move(digests), std::vector<uint32_t>(ops.size(), 0), std::move(verdicts)};
   return next_ticket_++;
 }
 
@@ -1939,81 +1829,46 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
     }
   }
   std::lock_guard<std::mutex> lk(done_mu_);
-  done_[next_ticket_] = {{}, std::move(status), std::move(verdicts)};
+  done_[next_ticket_] = {std::vector<uint64_t>(ops.size(), 0), std::move(status), std::move(verdicts)};
   return next_ticket_++;
 }
 
-ErrorCode HostLoopbackTransport::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
-  std::vector<ErrorCode> verdicts;
-  return wait_put_verdicts(ticket, digests, &verdicts);
-}
-
-ErrorCode HostLoopbackTransport::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
-  std::vector<ErrorCode> verdicts;
-  return wait_get_verdicts(ticket, status, &verdicts);
-}
-
-ErrorCode HostLoopbackTransport::wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
+ErrorCode HostLoopbackTransport::wait(uint64_t ticket, DeviceBatchResult* res) {
   std::lock_guard<std::mutex> lk(done_mu_);
   auto it = done_.find(ticket);
   if (it == done_.end()) return ErrorCode::NOT_FOUND;
-  if (digests) *digests = std::move(it->second.digests);
-  *verdicts = std::move(it->second.verdicts);
+  *res = std::move(it->second);
   done_.erase(it);
   return ErrorCode::OK;
 }
 
-ErrorCode HostLoopbackTransport::wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
-  std::lock_guard<std::mutex> lk(done_mu_);
-  auto it = done_.find(ticket);
-  if (it == done_.end()) return ErrorCode::NOT_FOUND;
-  if (status) *status = std::move(it->second.status);
-  *verdicts = std::move(it->second.verdicts);
-  done_.erase(it);
-  return ErrorCode::OK;
-}
-
-ErrorCode HostLoopbackTransport::put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint64_t>* digests,
-                                                  std::vector<ErrorCode>* verdicts) {
+ErrorCode HostLoopbackTransport::run_fp8(const std::vector<DeviceFp8Op>& ops, bool unpack, void*, DeviceBatchResult* res) {
   ++launches_;
-  if (digests) digests->assign(ops.size(), 0);
-  verdicts->assign(ops.size(), ErrorCode::OK);
+  *res = {std::vector<uint64_t>(ops.size(), 0), std::vector<uint32_t>(ops.size(), 0), std::vector<ErrorCode>(ops.size(), ErrorCode::OK)};
   for (size_t k = 0; k < ops.size(); ++k) {
     const DeviceFp8Op& op = ops[k];
     const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
     if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
-    const auto* src = static_cast<const uint8_t*>(op.wide);
-    std::vector<uint8_t> dense;
-    if (!op.mem.contiguous()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows or pages
-      DeviceLayout b;
-      if (!op.win.whole() || !op.mem.valid_source(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
-      if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
-      std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table reads block 0 of every slice
-      b = b.resolved(eb * op.n_elems, false, &table, &(*verdicts)[k]);
-      dense.resize(eb * op.n_elems);
-      copy_from_device(dense.data(), op.wide, b, dense.size(), nullptr);
-      src = dense.data();
+    if (!unpack) {
+      const auto* src = static_cast<const uint8_t*>(op.wide);
+      std::vector<uint8_t> dense;
+      if (!op.mem.contiguous()) {  // as the engine and the kernel's gathering load: the elements, compacted from their rows or pages
+        DeviceLayout b;
+        if (!op.win.whole() || !op.mem.valid_source(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+        if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+        std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table reads block 0 of every slice
+        b = b.resolved(eb * op.n_elems, false, &table, &res->verdicts[k]);
+        dense.resize(eb * op.n_elems);
+        copy_from_device(dense.data(), op.wide, b, dense.size(), nullptr);
+        src = dense.data();
+      }
+      std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
+      mxfp8::pack(src, op.wide_type, op.n_elems, packed.data());
+      ErrorCode ec = io_->write_shard(*op.placement, packed.data(), &res->digests[k], ChecksumAlgo::BBH64);
+      for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], packed.data(), nullptr, ChecksumAlgo::NONE);
+      if (ec != ErrorCode::OK) return ec;
+      continue;
     }
-    std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
-    mxfp8::pack(src, op.wide_type, op.n_elems, packed.data());
-    uint64_t d = 0;
-    ErrorCode ec = io_->write_shard(*op.placement, packed.data(), &d, ChecksumAlgo::BBH64);
-    for (size_t r = 0; r < op.replicas.size() && ec == ErrorCode::OK; ++r) ec = io_->write_shard(*op.replicas[r], packed.data(), nullptr, ChecksumAlgo::NONE);
-    if (ec != ErrorCode::OK) return ec;
-    if (digests) (*digests)[k] = d;
-  }
-  return ErrorCode::OK;
-}
-
-ErrorCode HostLoopbackTransport::get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void*, std::vector<uint32_t>* status,
-                                                  std::vector<ErrorCode>* verdicts) {
-  ++launches_;
-  if (status) status->assign(ops.size(), 0);
-  verdicts->assign(ops.size(), ErrorCode::OK);
-  for (size_t k = 0; k < ops.size(); ++k) {
-    const DeviceFp8Op& op = ops[k];
-    const uint64_t eb = mxfp8::wide_bytes(op.wide_type);
-    if (eb != mxfp8::wide_bytes(ops[0].wide_type)) return ErrorCode::INVALID_ARGUMENT;  // as the engine: one element size
     if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
     DeviceLayout b;
     if (!op.mem.contiguous()) {  // as the engine: destination rows or pages, never with a window, co-aligned in wide bytes
@@ -2022,11 +1877,11 @@ ErrorCode HostLoopbackTransport::get_fp8_verdicts(const std::vector<DeviceFp8Op>
       if (b.kind() == DeviceLayout::BLOCKS && !b.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // as the engine
     }
     std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table is all null pages
-    b = b.resolved(eb * op.n_elems, true, &table, &(*verdicts)[k]);
+    b = b.resolved(eb * op.n_elems, true, &table, &res->verdicts[k]);
     std::vector<uint8_t> packed(mxfp8::packed_bytes(op.n_elems));
     const ErrorCode ec = io_->read_shard(*op.placement, packed.data(), ChecksumAlgo::BBH64);
     if (ec == ErrorCode::CHECKSUM_MISMATCH) {
-      if (status) (*status)[k] = 1;
+      res->status[k] = 1;
       continue;
     }
     if (ec != ErrorCode::OK) return ec;

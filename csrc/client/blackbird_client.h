@@ -17,6 +17,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -86,6 +87,15 @@ struct DeviceFp8Op {
   mxfp8::Wide wide_type = mxfp8::Wide::BF16;
 };
 
+// What a device batch did, one entry per op in every field.
+struct DeviceBatchResult {
+  std::vector<uint64_t> digests;   // put: the digest of the op's shard (MXFP8: BBH64 of the stored packed object)
+  std::vector<uint32_t> status;    // get: 0 = the shard verified against its placement's digest, else a mismatch
+  // OK, or the refusal of the block ids of a BLOCKS layout (SourceBlocks in common/store_window.h).  A refused op's
+  // transfer touched nothing outside the caller's memory, and its digest or status means nothing.
+  std::vector<ErrorCode> verdicts;
+};
+
 // Implemented by the GPU fabric: moves shards between client device buffers and worker slabs
 // with the fused kernels.  Returns per-op digests (put) or verifies them (get).
 class DeviceTransport {
@@ -94,44 +104,22 @@ class DeviceTransport {
   virtual bool can_reach(const ShardPlacement& s) const = 0;
   virtual uint64_t launches() const = 0;
   // submit_* enqueues a batch and returns a ticket, so the caller can overlap control-plane round trips of the next chunk
-  // with this one's transfer; wait_* blocks until it is done.  dev_ptrs[item] is the device buffer of object `item`.  A
-  // put returns one digest per op; a get verifies each shard with its placement's algorithm (status per op, 0 = ok).
+  // with this one's transfer; wait() blocks until it is done and fills its result.  dev_ptrs[item] is the device buffer of
+  // object `item`.  A put digests every op; a get verifies each shard with its placement's algorithm.
   virtual Result<uint64_t> submit_put(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
                                       void* stream) = 0;
-  virtual ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) = 0;
   virtual Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) = 0;
-  virtual ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) = 0;
-  // wait_put and wait_get with each op's verdict on the block ids of a BLOCKS layout (SourceBlocks in
-  // common/store_window.h): empty, or one per op, OK or the refusal.  A refused op's transfer touched nothing outside the
-  // caller's memory, and its digest or status means nothing.  A transport that takes no BLOCKS layout returns none.
-  virtual ErrorCode wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
-    verdicts->clear();
-    return wait_put(ticket, digests);
-  }
-  virtual ErrorCode wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
-    verdicts->clear();
-    return wait_get(ticket, status);
-  }
+  virtual ErrorCode wait(uint64_t ticket, DeviceBatchResult* res) = 0;
   // True when the shard lives in this client's own device memory (a get from it never leaves the GPU).
   virtual bool is_local(const ShardPlacement& s) const { return false; }
   virtual size_t max_in_flight() const { return 1; }
   // Prometheus lines of the transport's own counters (bytes per path, launches, ...); appended to the client's metrics.
   virtual std::string metrics_text() const { return {}; }
   virtual bool fp8_eligible(uint64_t n_elems) const { return false; }
-  // Fused MXFP8 put / get (pack / unpack inside the transfer kernel).  digests[i] = BBH64 of the stored packed
-  // object; status[i] != 0 = digest mismatch on get.  Objects must satisfy fp8_eligible().
-  virtual ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) { return ErrorCode::NOT_IMPLEMENTED; }
-  virtual ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) { return ErrorCode::NOT_IMPLEMENTED; }
-  // put_fp8 and get_fp8 with each op's verdict on the block ids of a BLOCKS layout, as wait_put_verdicts.
-  virtual ErrorCode put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
-                                     std::vector<ErrorCode>* verdicts) {
-    verdicts->clear();
-    return put_fp8(ops, stream, digests);
-  }
-  virtual ErrorCode get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
-                                     std::vector<ErrorCode>* verdicts) {
-    verdicts->clear();
-    return get_fp8(ops, stream, status);
+  // Fused MXFP8 put (pack inside the transfer kernel) or, with `unpack`, get, synchronous.  Objects must satisfy
+  // fp8_eligible().
+  virtual ErrorCode run_fp8(const std::vector<DeviceFp8Op>& ops, bool unpack, void* stream, DeviceBatchResult* res) {
+    return ErrorCode::NOT_IMPLEMENTED;
   }
   // Staging copies for objects (or shards) that live on host tiers, synchronous: object bytes [0, n) laid out by `layout`
   // at `base` (common/store_window.h) from / to n bytes packed back to back at `host`.  copy_to_device skips null pages;
@@ -186,10 +174,9 @@ class BlackbirdClient {
   // elem_pitches[i] (SourceRows in common/store_window.h, in elements).  The put kernel gathers the rows while it packs, so
   // no contiguous copy is made; the stored packed object and its digest are byte for byte those of batch_put_device_fp8
   // of the compacted rows, so every fp8 get reads it.  Placement, replica fan-out and errors are batch_put_device_fp8's.
-  // Per object, before anything is allocated: INVALID_ARGUMENT for elem_widths[i] > elem_pitches[i] with rows[i] > 1;
-  // VALUE_OUT_OF_RANGE when the element count or the source extent overflows; NOT_IMPLEMENTED unless bf16_ptrs[i] is
-  // 16-byte aligned and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is no host-staged path;
-  // the rest of the batch keeps its single launch.  rows[i] == 1 or elem_widths[i] == elem_pitches[i] is exactly
+  // Per object, the shaped calls' admission (shaped_put) of SourceRows::from_rows: INVALID_ARGUMENT for elem_widths[i] >
+  // elem_pitches[i] with rows[i] > 1; co-aligned means bf16_ptrs[i] 16-byte aligned and, for rows[i] > 1,
+  // (elem_pitches[i] - elem_widths[i]) % 8 == 0.  rows[i] == 1 or elem_widths[i] == elem_pitches[i] is exactly
   // batch_put_device_fp8 of one contiguous tensor.
   std::vector<ErrorCode> batch_put_device_fp8_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
@@ -224,11 +211,12 @@ class BlackbirdClient {
   // Gets of packed tensors into sliced bf16 tensors the caller owns: object i (n_elems[i] elements) is unpacked into rows[i]
   // rows of elem_widths[i] elements, row r at bf16_ptrs[i] + 2 * r * elem_pitches[i] (SourceRows in common/store_window.h,
   // in elements), by the scattering store of the fused unpack.  No element outside the rows is ever written.  Fail-over
-  // and the placement refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT unless rows[i] * elem_widths[i] ==
-  // n_elems[i], or for elem_widths[i] > elem_pitches[i] with rows[i] > 1; VALUE_OUT_OF_RANGE when a product overflows;
-  // NOT_IMPLEMENTED when the object is not fusable (as batch_get_device_fp8), or unless bf16_ptrs[i] is 16-byte aligned
-  // and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is no host-staged path; the rest of the
-  // batch keeps the fused launch.  rows[i] == 1 or elem_widths[i] == elem_pitches[i] is batch_get_device_fp8.
+  // and the placement refresh are batch_get_device_fp8's.  Per object, the shaped calls' admission (shaped_get) of
+  // SourceRows::from_rows: INVALID_ARGUMENT for elem_widths[i] > elem_pitches[i] with rows[i] > 1 or unless rows[i] *
+  // elem_widths[i] == n_elems[i].  Then NOT_IMPLEMENTED when the object is not fusable (as batch_get_device_fp8), or
+  // unless bf16_ptrs[i] is 16-byte aligned and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is
+  // no host-staged path; the rest of the batch keeps the fused launch.  rows[i] == 1 or elem_widths[i] ==
+  // elem_pitches[i] is batch_get_device_fp8.
   std::vector<ErrorCode> batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
                                                       const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
@@ -238,11 +226,9 @@ class BlackbirdClient {
   // (SourcePages in common/store_window.h, page size in elements, addresses in bytes).  The pack kernel reads each page in
   // place; an MX block may straddle two pages.  The stored packed object and its digest are byte for byte those of
   // batch_put_device_fp8 of the concatenation, so every fp8 get reads it.  Placement, replica fan-out and errors are
-  // batch_put_device_fp8's.  Per object, before anything is allocated: INVALID_ARGUMENT for page_elems[i] == 0 with pages,
-  // or an element count that is not a positive whole number of MX blocks; VALUE_OUT_OF_RANGE when the count or its wide
-  // bytes overflow; NOT_IMPLEMENTED unless the table is co-aligned in wide bytes (every page 16-byte aligned and, for
-  // several pages, page_elems[i] % 8 == 0) -- there is no host-staged path; the rest of the batch keeps its launch.
-  // INVALID_ARGUMENT, also before anything is allocated, for a zero page address: a put reads every page.
+  // batch_put_device_fp8's.  Per object, the shaped calls' admission (shaped_put) of SourcePages::from_pages:
+  // INVALID_ARGUMENT for page_elems[i] == 0 with pages; co-aligned means every page 16-byte aligned and, for several
+  // pages, page_elems[i] % 8 == 0.
   std::vector<ErrorCode> batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                     const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
                                                     mxfp8::Wide wide = mxfp8::Wide::BF16);
@@ -251,21 +237,22 @@ class BlackbirdClient {
   // Only the object's elements are written; pages of one get must not overlap (not checked).  A zero page address is a
   // page that is not stored (SourcePages' null page): a partial restore names only the pages it wants and leaves the
   // others 0.  The table still covers the whole object, which is still read whole and verified, so a corrupt copy fails
-  // over even when no page is stored.  Fail-over and the placement refresh are batch_get_device_fp8's.  Per object: INVALID_ARGUMENT for page_elems[i] == 0 with pages, or unless the
-  // stored object holds exactly pages[i].size() * page_elems[i] elements (a positive whole number of MX blocks);
-  // VALUE_OUT_OF_RANGE when that count or its wide bytes overflow; NOT_IMPLEMENTED when the object is not fusable (as
-  // batch_get_device_fp8) or the pages fail SourcePages::fused_get_aligned in wide bytes -- there is no host-staged path;
-  // the rest of the batch keeps the fused launch.
+  // over even when no page is stored.  Fail-over and the placement refresh are batch_get_device_fp8's.  Per object, the
+  // shaped calls' admission (shaped_get) of SourcePages::from_pages: INVALID_ARGUMENT for page_elems[i] == 0 with pages.
+  // Then INVALID_ARGUMENT unless the stored object holds exactly pages[i].size() * page_elems[i] elements;
+  // NOT_IMPLEMENTED when the object is not fusable (as batch_get_device_fp8) or the pages fail
+  // SourcePages::fused_get_aligned in wide bytes -- there is no host-staged path; the rest of the batch keeps the fused
+  // launch.
   std::vector<ErrorCode> batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                     const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   // Packed puts and gets from block ids that stay on the device: batch_put_device_blocks and batch_get_device_blocks for
   // packed tensors, `page` counted in elements of `wide` (the stride and slice addresses in bytes), with the rules of
-  // batch_put_device_fp8_paged and batch_get_device_fp8_paged.  Per object, before anything is allocated: INVALID_ARGUMENT
-  // for the shape errors of the byte calls or an element count that is not a positive whole number of MX blocks (on a
-  // get: not exactly the stored object's); VALUE_OUT_OF_RANGE when the count or its wide bytes overflow; NOT_IMPLEMENTED
-  // when the table is not co-aligned in wide bytes, the object is not fusable, or (a get) n_blocks or n_stored exceeds
-  // SourceBlocks::kMaxDistinct -- there is no host-staged path.  After the transfer the device's verdict on the ids
-  // answers the object as for the byte calls: a refused put is cancelled, a refused get stores nothing and is not retried.
+  // batch_put_device_fp8_paged and batch_get_device_fp8_paged.  Per object, the shaped calls' admission (shaped_put,
+  // shaped_get) of SourceBlocks::from_blocks, whose shape errors are the byte calls'.  Then, on a get, INVALID_ARGUMENT
+  // unless the element count is exactly the stored object's, and NOT_IMPLEMENTED when the object is not fusable or the
+  // table fails SourceBlocks::fused_get_aligned in wide bytes -- there is no host-staged path.  After the transfer the
+  // device's verdict on the ids answers the object as for the byte calls: a refused put is cancelled, a refused get
+  // stores nothing and is not retried.
   std::vector<ErrorCode> batch_put_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                      const WorkerConfig& cfg, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   std::vector<ErrorCode> batch_get_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
@@ -291,10 +278,10 @@ class BlackbirdClient {
   // every get reads it.  The fused path gathers the rows in the put kernel; it needs dev_ptrs[i] 16-byte aligned, for
   // rows[i] > 1 (pitches[i] - widths[i]) % 16 == 0, and every shard start 16-byte aligned.  Any other item, and every
   // placement the fabric cannot reach, is staged through the host (one copy of the source extent, rows compacted there)
-  // while the rest of the batch keeps the fused launch.  Per object, before anything is allocated: INVALID_ARGUMENT for
-  // widths[i] > pitches[i] with rows[i] > 1; VALUE_OUT_OF_RANGE when the size or the extent overflows.  rows[i] == 1 or
-  // widths[i] == pitches[i] is exactly batch_put_device of one contiguous block, rows[i] == 0 or widths[i] == 0 that of a
-  // zero-byte object.
+  // while the rest of the batch keeps the fused launch.  Per object, the shaped calls' admission (shaped_put) of
+  // SourceRows::from_rows: INVALID_ARGUMENT for widths[i] > pitches[i] with rows[i] > 1.  rows[i] == 1 or widths[i] ==
+  // pitches[i] is exactly batch_put_device of one contiguous block, rows[i] == 0 or widths[i] == 0 that of a zero-byte
+  // object.
   std::vector<ErrorCode> batch_put_device_strided(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                                   const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                   const std::vector<uint64_t>& rows, const WorkerConfig& cfg, void* stream);
@@ -329,9 +316,9 @@ class BlackbirdClient {
   // refresh of batch_get_device.  The fused path scatters the rows in the get kernel; it needs dev_ptrs[i] 16-byte aligned,
   // for rows[i] > 1 (pitches[i] - widths[i]) % 16 == 0, and every shard start 16-byte aligned.  Any other item, and every
   // placement the fabric cannot reach, is staged through the host (one 2-D H2D copy of the rows) while the rest of the
-  // batch keeps the fused launch.  Per object, before anything is read: INVALID_ARGUMENT for widths[i] > pitches[i] with
-  // rows[i] > 1; VALUE_OUT_OF_RANGE when the size or the extent overflows.  rows[i] == 1 or widths[i] == pitches[i] is
-  // exactly batch_get_device with capacity rows[i] * widths[i].
+  // batch keeps the fused launch.  Per object, the shaped calls' admission (shaped_get) of SourceRows::from_rows:
+  // INVALID_ARGUMENT for widths[i] > pitches[i] with rows[i] > 1.  rows[i] == 1 or widths[i] == pitches[i] is exactly
+  // batch_get_device with capacity rows[i] * widths[i].
   std::vector<ErrorCode> batch_get_device_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                   const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                   const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes);
@@ -341,9 +328,9 @@ class BlackbirdClient {
   // those of batch_put_device of the concatenation, so every get reads it.  The fused path reads each page in place in
   // the put kernel; it needs every shard of every copy co-aligned (SourcePages::coaligned: 16-byte aligned pages and shard starts and, for
   // several pages, page_bytes[i] % 16 == 0).  Any other item, and every placement the fabric cannot reach, is staged
-  // through the host (one D2H copy per run of pages) while the rest of the batch keeps the fused launch.  Per object,
-  // before anything is allocated: INVALID_ARGUMENT for page_bytes[i] == 0 with pages or for a zero page address (a put
-  // reads every page); VALUE_OUT_OF_RANGE when the size overflows.  No pages is a zero-byte object.
+  // through the host (one D2H copy per run of pages) while the rest of the batch keeps the fused launch.  Per object, the
+  // shaped calls' admission (shaped_put) of SourcePages::from_pages: INVALID_ARGUMENT for page_bytes[i] == 0 with pages.
+  // No pages is a zero-byte object.
   std::vector<ErrorCode> batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                 const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream);
   // Paged gets, the mirror: object i lands in the pages pages[i] of page_bytes[i] bytes, object byte x in page
@@ -354,8 +341,8 @@ class BlackbirdClient {
   // out_sizes rules do not change.  Every shard is read whole and verified, stored pages or not, with the
   // fail-over and placement refresh of batch_get_device.  The fused path scatters the pages in the get kernel; it needs
   // SourcePages::fused_get_aligned for every shard of every copy.  Any other item, and every placement the fabric cannot
-  // reach, is staged through the host (one H2D copy per run of pages).  Per object: INVALID_ARGUMENT for
-  // page_bytes[i] == 0 with pages; VALUE_OUT_OF_RANGE when the capacity overflows.
+  // reach, is staged through the host (one H2D copy per run of pages).  Per object, the shaped calls' admission
+  // (shaped_get) of SourcePages::from_pages: INVALID_ARGUMENT for page_bytes[i] == 0 with pages.
   std::vector<ErrorCode> batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                 const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes);
   // Paged puts from block ids that stay on the device: object i is the pages of blocks[i] (SourceBlocks in
@@ -363,20 +350,20 @@ class BlackbirdClient {
   // order, as batch_put_device_paged of that table would store it.  The ids are read on `stream` by the transfer
   // engine's resolve kernel, after the work queued there before the call; the host never reads them, and no host work
   // depends on their number beyond the small outer array.  Placement, replica fan-out and digests are
-  // batch_put_device_paged's.  Per object, before anything is allocated: INVALID_ARGUMENT for page == 0 with pages, a
-  // selection (a put reads every page) or ids other than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the size overflows.
-  // After the transfer, from the device: VALUE_OUT_OF_RANGE for an id outside [0, n_blocks); the put is then cancelled,
-  // nothing is stored and the rest of the batch carries on.  NOT_IMPLEMENTED when the table is not co-aligned
-  // (SourceBlocks::coaligned) or a placement is not on the GPU fabric: there is no host-staged path; the put is cancelled.
+  // batch_put_device_paged's.  Per object, the shaped calls' admission (shaped_put) of SourceBlocks::from_blocks:
+  // INVALID_ARGUMENT for page == 0 with pages or ids other than 4 or 8 bytes.  After the transfer, from the device:
+  // VALUE_OUT_OF_RANGE for an id outside [0, n_blocks); the put is then cancelled, nothing is stored and the rest of the
+  // batch carries on.  NOT_IMPLEMENTED when the table is not co-aligned (SourceBlocks::coaligned) or a placement is not on
+  // the GPU fabric: there is no host-staged path; the put is cancelled.
   std::vector<ErrorCode> batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
                                                  const WorkerConfig& cfg, void* stream);
   // Paged gets into blocks named by device-resident ids, the mirror: object i lands in the pages of blocks[i], with a
   // selection (sel, n_stored) as a partial restore: only the pages of the stored blocks sel[m] land, in block ids[m], and
   // the others are not stored.  The capacity is the table's size; out_sizes[i] receives the object's size.  Every shard
-  // is read whole and verified, with the fail-over and placement refresh of batch_get_device.  Per object: INVALID_ARGUMENT
-  // for page == 0 with pages or ids other than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the capacity overflows;
-  // BUFFER_OVERFLOW for a larger object; NOT_IMPLEMENTED when n_blocks or n_stored exceeds SourceBlocks::kMaxDistinct, the
-  // table fails SourceBlocks::fused_get_aligned or no copy is on the GPU fabric.  After the transfer, from the device:
+  // is read whole and verified, with the fail-over and placement refresh of batch_get_device.  Per object, the shaped
+  // calls' admission (shaped_get) of SourceBlocks::from_blocks: INVALID_ARGUMENT for page == 0 with pages or ids other
+  // than 4 or 8 bytes.  Then BUFFER_OVERFLOW for a larger object; NOT_IMPLEMENTED when the table fails
+  // SourceBlocks::fused_get_aligned or no copy is on the GPU fabric.  After the transfer, from the device:
   // VALUE_OUT_OF_RANGE for an id (or selection entry) out of range, INVALID_ARGUMENT for a repeated one; then nothing
   // of the object is stored, it is not retried on another replica, and the rest of the batch carries on.
   std::vector<ErrorCode> batch_get_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
@@ -432,6 +419,27 @@ class BlackbirdClient {
   // The shaped batch_*_device_* calls over the four above, and the placement refresh of get_device and get_device_fp8.
   template <class Shape, class Run>
   std::vector<ErrorCode> shaped_batch(std::string_view name, bool admit, size_t n, bool arity_ok, Shape&& shape, Run&& run);
+  // The strided, scatter, paged and blocks puts and gets, bytes and MXFP8 (`fp8`: the wide type).  build(i, &item) makes
+  // item i's layout and size from the call's own arguments, in bytes or elements of the wide type:
+  // SourceRows::from_rows, SourcePages::from_pages or SourceBlocks::from_blocks, with their errors (INVALID_ARGUMENT for
+  // a shape, VALUE_OUT_OF_RANGE for an overflow).  Then one admission rule, in this order:
+  //   - MXFP8 from a page table (pages, blocks): INVALID_ARGUMENT unless a positive whole number of MX blocks.  Rows
+  //     are left to put_device_fp8 and get_device_fp8, which answer for a count that is not fusable;
+  //   - a put: INVALID_ARGUMENT for a null page or a selection of blocks (a put reads every unit);
+  //   - VALUE_OUT_OF_RANGE when the size does not fit in size_t, or for MXFP8 when the source extent or the layout
+  //     overflows in wide bytes;
+  //   - an MXFP8 put: NOT_IMPLEMENTED unless the layout at ptrs[i] is co-aligned in wide bytes (DeviceLayout::coaligned),
+  //     as there is no host-staged path for packed puts;
+  //   - a get: NOT_IMPLEMENTED when n_blocks or n_stored exceeds SourceBlocks::kMaxDistinct.
+  // A refused put item never reaches the Keystone and a refused get item is not looked up; the rest of the batch goes on
+  // through put_device, get_device, put_device_fp8 or get_device_fp8 (dev_ptrs[i] = ptrs[i]), whose own rules follow.
+  // out_sizes, when given, is the get's, 0 for a refused item; the metrics are shaped_batch's, in wide bytes for MXFP8.
+  template <class Build>
+  std::vector<ErrorCode> shaped_put(std::string_view name, const std::vector<ObjectKey>& keys, const std::vector<const void*>& ptrs,
+                                    bool arity_ok, std::optional<mxfp8::Wide> fp8, Build&& build, const WorkerConfig& cfg, void* stream);
+  template <class Build>
+  std::vector<ErrorCode> shaped_get(std::string_view name, const std::vector<ObjectKey>& keys, const std::vector<void*>& ptrs,
+                                    bool arity_ok, std::optional<mxfp8::Wide> fp8, Build&& build, void* stream, std::vector<size_t>* out_sizes);
   template <class Reissue>
   void refresh_placements(const std::vector<ObjectKey>& keys, const std::vector<Result<std::vector<CopyPlacement>>>& placed,
                           std::vector<ErrorCode>& out, Reissue&& reissue);
@@ -477,11 +485,8 @@ class HostLoopbackTransport : public DeviceTransport {
   // Synchronous: submit_* moves the shards and keeps the result under the ticket it returns.
   Result<uint64_t> submit_put(const std::vector<DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
                               void* stream) override;
-  ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override;
   Result<uint64_t> submit_get(const std::vector<DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) override;
-  ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
-  ErrorCode wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) override;
-  ErrorCode wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) override;
+  ErrorCode wait(uint64_t ticket, DeviceBatchResult* res) override;
   bool can_reach(const ShardPlacement& s) const override;
   uint64_t launches() const override { return launches_; }
   // A BLOCKS layout is resolved on the host (SourceBlocks::resolve): here the "device" ids are host memory.
@@ -506,18 +511,7 @@ class HostLoopbackTransport : public DeviceTransport {
   // MXFP8 through the CPU reference codec (common/mxfp8.h): the stored object and its digest are the ones the fused
   // kernels produce, so the fp8 client logic (replica fan-out, fail-over between replicas) is testable on CPU too.
   bool fp8_eligible(uint64_t n_elems) const override { return n_elems != 0 && n_elems % 32 == 0; }
-  ErrorCode put_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override {
-    std::vector<ErrorCode> verdicts;
-    return put_fp8_verdicts(ops, stream, digests, &verdicts);
-  }
-  ErrorCode get_fp8(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override {
-    std::vector<ErrorCode> verdicts;
-    return get_fp8_verdicts(ops, stream, status, &verdicts);
-  }
-  ErrorCode put_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
-                             std::vector<ErrorCode>* verdicts) override;
-  ErrorCode get_fp8_verdicts(const std::vector<DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
-                             std::vector<ErrorCode>* verdicts) override;
+  ErrorCode run_fp8(const std::vector<DeviceFp8Op>& ops, bool unpack, void* stream, DeviceBatchResult* res) override;
 
  private:
   std::shared_ptr<BlackbirdClient> io_;
@@ -525,12 +519,7 @@ class HostLoopbackTransport : public DeviceTransport {
   std::atomic<uint64_t> launches_{0};
   std::mutex done_mu_;
   uint64_t next_ticket_ = 1;
-  struct Done {
-    std::vector<uint64_t> digests;  // put
-    std::vector<uint32_t> status;   // get
-    std::vector<ErrorCode> verdicts;
-  };
-  std::map<uint64_t, Done> done_;
+  std::map<uint64_t, DeviceBatchResult> done_;
 };
 
 }  // namespace bb::client

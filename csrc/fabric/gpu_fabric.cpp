@@ -650,32 +650,34 @@ ErrorCode GpuFabric::finish(uint64_t ticket, InFlight* fl, XferResult* res) {
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::wait_put(uint64_t ticket, std::vector<uint64_t>* digests) {
-  std::vector<ErrorCode> verdicts;
-  return wait_put_verdicts(ticket, digests, &verdicts);
+// The engine's per-item results of a batch as its `nops` ops': a put op's digest is its first item's (the extra fan-out
+// passes of a put come after it), and its verdict is the first refusal among its items (they resolve the same ids).  A
+// get op has one item.  Entries of ops without an item are kept (a get's from the groups of a mixed batch that finished
+// in submit_get), or zero / OK.
+static void to_ops(size_t nops, const std::vector<size_t>& op_of_item, const XferResult& res, client::DeviceBatchResult* out) {
+  out->digests.resize(nops, 0);
+  out->status.resize(nops, 0);
+  out->verdicts.resize(nops, ErrorCode::OK);
+  for (size_t i = op_of_item.size(); i-- > 0;) {
+    out->digests[op_of_item[i]] = res.digest[i];
+    out->status[op_of_item[i]] = res.status[i];
+  }
+  for (size_t i = 0; i < op_of_item.size(); ++i)
+    if (out->verdicts[op_of_item[i]] == ErrorCode::OK) out->verdicts[op_of_item[i]] = res.verdict[i];
 }
 
-// An op's verdict is the first refusal among its items (the extra fan-out passes of a put resolve the same ids).
-static void op_verdicts(const std::vector<size_t>& op_of_item, const std::vector<ErrorCode>& item_verdicts, std::vector<ErrorCode>* out) {
-  for (size_t i = 0; i < op_of_item.size() && i < item_verdicts.size(); ++i)
-    if ((*out)[op_of_item[i]] == ErrorCode::OK) (*out)[op_of_item[i]] = item_verdicts[i];
-}
-
-ErrorCode GpuFabric::wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) {
-  BB_TRACE_SPAN("fabric.wait_put");
+ErrorCode GpuFabric::wait(uint64_t ticket, client::DeviceBatchResult* out) {
+  BB_TRACE_SPAN("fabric.wait");
   InFlight fl;
   XferResult res;
   BB_TRY(finish(ticket, &fl, &res));
-  if (digests) {
-    digests->assign(fl.nops, 0);
-    for (size_t i = fl.op_of_item.size(); i-- > 0;) (*digests)[fl.op_of_item[i]] = res.digest[i];
-  }
-  verdicts->assign(fl.nops, ErrorCode::OK);
-  op_verdicts(fl.op_of_item, res.verdict, verdicts);
+  *out = std::move(fl.done);
+  to_ops(fl.nops, fl.op_of_item, res, out);
   return ErrorCode::OK;
 }
 
-ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, XferResult* res) {
+ErrorCode GpuFabric::run_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, client::DeviceBatchResult* out) {
+  BB_TRACE_SPAN(unpack ? "fabric.get_fp8" : "fabric.put_fp8", ops.size());
   std::vector<Fp8Item> items;
   items.reserve(ops.size());
   for (const auto& op : ops) {
@@ -702,38 +704,10 @@ ErrorCode GpuFabric::transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, b
     }
     items.push_back(it);
   }
-  BB_TRY(engine_->run_fp8(items, unpack, stream, res));
-  note_device_ms(res->device_ms);
-  return ErrorCode::OK;
-}
-
-ErrorCode GpuFabric::put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) {
-  std::vector<ErrorCode> verdicts;
-  return put_fp8_verdicts(ops, stream, digests, &verdicts);
-}
-
-ErrorCode GpuFabric::get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) {
-  std::vector<ErrorCode> verdicts;
-  return get_fp8_verdicts(ops, stream, status, &verdicts);
-}
-
-ErrorCode GpuFabric::put_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
-                                      std::vector<ErrorCode>* verdicts) {
-  BB_TRACE_SPAN("fabric.put_fp8", ops.size());
   XferResult res;
-  BB_TRY(transfer_fp8(ops, false, stream, &res));
-  if (digests) *digests = std::move(res.digest);
-  *verdicts = std::move(res.verdict);  // one item per op
-  return ErrorCode::OK;
-}
-
-ErrorCode GpuFabric::get_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
-                                      std::vector<ErrorCode>* verdicts) {
-  BB_TRACE_SPAN("fabric.get_fp8", ops.size());
-  XferResult res;
-  BB_TRY(transfer_fp8(ops, true, stream, &res));
-  if (status) *status = std::move(res.status);
-  *verdicts = std::move(res.verdict);
+  BB_TRY(engine_->run_fp8(items, unpack, stream, &res));
+  note_device_ms(res.device_ms);
+  *out = {std::move(res.digest), std::move(res.status), std::move(res.verdict)};  // one item per op
   return ErrorCode::OK;
 }
 
@@ -793,32 +767,8 @@ Result<uint64_t> GpuFabric::submit_get(const std::vector<client::DeviceShardOp>&
     XferResult res;
     BB_TRY(engine_->wait(t.value(), &res));
     note_device_ms(res.device_ms);
-    fl.status.resize(ops.size(), 0);
-    for (size_t i = 0; i < fl.op_of_item.size(); ++i) fl.status[fl.op_of_item[i]] = res.status[i];
-    fl.verdicts.resize(ops.size(), ErrorCode::OK);
-    op_verdicts(fl.op_of_item, res.verdict, &fl.verdicts);
+    to_ops(ops.size(), fl.op_of_item, res, &fl.done);
   }
-}
-
-ErrorCode GpuFabric::wait_get(uint64_t ticket, std::vector<uint32_t>* status) {
-  std::vector<ErrorCode> verdicts;
-  return wait_get_verdicts(ticket, status, &verdicts);
-}
-
-ErrorCode GpuFabric::wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) {
-  BB_TRACE_SPAN("fabric.wait_get");
-  InFlight fl;
-  XferResult res;
-  BB_TRY(finish(ticket, &fl, &res));
-  if (status) {
-    *status = std::move(fl.status);
-    status->resize(fl.nops, 0);
-    for (size_t i = 0; i < fl.op_of_item.size(); ++i) (*status)[fl.op_of_item[i]] = res.status[i];
-  }
-  *verdicts = std::move(fl.verdicts);
-  verdicts->resize(fl.nops, ErrorCode::OK);
-  op_verdicts(fl.op_of_item, res.verdict, verdicts);
-  return ErrorCode::OK;
 }
 
 }  // namespace bb::gpu

@@ -76,21 +76,13 @@ class GpuFabric : public client::DeviceTransport {
   uint64_t launches() const override { return engine_->launches(); }
   Result<uint64_t> submit_put(const std::vector<client::DeviceShardOp>& ops, const std::vector<const void*>& dev_ptrs, ChecksumAlgo algo,
                               void* stream) override;
-  ErrorCode wait_put(uint64_t ticket, std::vector<uint64_t>* digests) override;
-  ErrorCode wait_put_verdicts(uint64_t ticket, std::vector<uint64_t>* digests, std::vector<ErrorCode>* verdicts) override;
   // One engine batch per checksum algorithm in `ops` (normally exactly one).  A batch that mixes algorithms runs all
   // groups but the last to completion before returning, so it never holds more than one engine slot.
   Result<uint64_t> submit_get(const std::vector<client::DeviceShardOp>& ops, const std::vector<void*>& dev_ptrs, void* stream) override;
-  ErrorCode wait_get(uint64_t ticket, std::vector<uint32_t>* status) override;
-  ErrorCode wait_get_verdicts(uint64_t ticket, std::vector<uint32_t>* status, std::vector<ErrorCode>* verdicts) override;
+  ErrorCode wait(uint64_t ticket, client::DeviceBatchResult* res) override;
   size_t max_in_flight() const override { return 3; }
   bool fp8_eligible(uint64_t n_elems) const override { return XferEngine::fp8_eligible(n_elems); }
-  ErrorCode put_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests) override;
-  ErrorCode get_fp8(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status) override;
-  ErrorCode put_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint64_t>* digests,
-                             std::vector<ErrorCode>* verdicts) override;
-  ErrorCode get_fp8_verdicts(const std::vector<client::DeviceFp8Op>& ops, void* stream, std::vector<uint32_t>* status,
-                             std::vector<ErrorCode>* verdicts) override;
+  ErrorCode run_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, client::DeviceBatchResult* res) override;
   // One async copy per call (rows: the extent from the device, compacted on the host, or one 2-D copy of the whole rows
   // to it; pages: one per run of pages), then one synchronise.
   ErrorCode copy_from_device(void* host, const void* base, const DeviceLayout& layout, size_t n, void* stream) override;
@@ -148,11 +140,9 @@ class GpuFabric : public client::DeviceTransport {
   struct InFlight {
     size_t nops = 0;
     std::vector<size_t> op_of_item;  // item -> op
-    std::vector<uint32_t> status;    // get: per op, from the groups of a mixed batch that finished in submit_get
-    std::vector<ErrorCode> verdicts;  // the same for the groups' block-id verdicts
+    client::DeviceBatchResult done;  // get: per op, from the groups of a mixed batch that finished in submit_get
   };
   ErrorCode finish(uint64_t ticket, InFlight* fl, XferResult* res);
-  ErrorCode transfer_fp8(const std::vector<client::DeviceFp8Op>& ops, bool unpack, void* stream, XferResult* res);
   void note_device_ms(float ms) {
     std::lock_guard<std::mutex> lk(mu_);
     last_ms_ = ms;
