@@ -80,7 +80,7 @@ def main():
             ids_d, new_d = ids.cuda(), new_ids.cuda()
             sel = cache.index_select(2, ids_d)
             nbytes = sel.numel() * sel.element_size()
-            _, page = TensorStore._block_pages(cache, 2, ids.numpy(), 0)
+            _, page, _ = TensorStore._block_pages(cache, 2, ids.numpy(), 0)
             store.put("ref", sel, pack_fp8=True)
             want = store.get("ref")  # the unpacked blocks every get must store
             store.remove(["ref"])

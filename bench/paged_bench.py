@@ -82,8 +82,8 @@ def main():
                                        preferred_classes=[_bb.StorageClass.RAM_GPU])
                 store = TensorStore(cl.client, cfg)
                 tensor_store.PAGED_MIN_PAGE_BYTES = 0
-                src_pages, page = TensorStore._block_pages(cache, 2, ids.numpy())
-                dst_pages, _ = TensorStore._block_pages(cache, 2, new_ids.numpy())
+                src_pages, page, _ = TensorStore._block_pages(cache, 2, ids.numpy())
+                dst_pages, _, _ = TensorStore._block_pages(cache, 2, new_ids.numpy())
                 page_keys = [f"pp/{k}" for k in range(src_pages.size)]
                 src_list, dst_list = src_pages.tolist(), dst_pages.tolist()
                 tensor_store.PAGED_MIN_PAGE_BYTES = shipped

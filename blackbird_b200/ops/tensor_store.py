@@ -53,6 +53,18 @@ LAYER_BLOCKS_MIN_PAGE_BYTES = 4 << 10
 # the pack or unpack kernel as well.  The same benchmark, packed bf16 (every page size) and fp16 / fp32 (32 KiB): the
 # device route wins everywhere measured too (bf16 4 KiB put 0.78-0.95 vs 1.83-2.03 ms, get 0.95-0.97 vs 1.59-1.74).
 FP8_LAYER_BLOCKS_MIN_PAGE_BYTES = 4 << 10
+# Shortest in-page row that the paged and block-id calls move when a block's page is rows inside it (a head slice of a
+# KV cache, _block_pages); shorter rows take index_select + put and get + index_copy_.  bench/sliced_blocks_bench.py,
+# 256 blocks of bf16 NHD / HND caches (2-32 MiB objects) on one H100 80GB HBM3 at 700 W, 15 calls: the transfer kernel
+# with rows of 256 bytes and more takes 0.9-1.2x the time of a contiguous paged transfer of the same bytes (1 head,
+# 256 B rows: put 0.029 vs 0.024 ms, get 0.027 vs 0.027), with 128 B rows 1.2-1.4x (put 0.030 vs 0.022, get 0.029 vs
+# 0.025), and at 128 B the call loses to index_select + put by more than at 256 B (median put 0.62 vs 0.44 ms, get 0.73
+# vs 0.53).  At these object sizes every route is host-bound (~0.5 ms a call) and the min-max spreads overlap, but the
+# row route's median is 0.05-0.25 ms above index_select + put / get + index_copy_ at every row size measured, 256 B and
+# more included: below this threshold it loses by more, above it it still does not win on time, only in memory (no
+# temporary as large as the selection).  Where that host time goes was not measured, nor were objects large enough for
+# the paged route to win on time (the 512 MiB workloads of PAGED_MIN_PAGE_BYTES).
+PAGED_MIN_ROW_BYTES = 256
 
 
 def _stored_dtype(m) -> torch.dtype:
@@ -276,21 +288,31 @@ class TensorStore:
 
     @staticmethod
     def _block_pages(cache: torch.Tensor, dim: int, ids: np.ndarray, min_page: Optional[int] = None):
-        """(page addresses, page bytes) of cache.index_select(dim, ids) for the paged device calls, or None when they should
-        not move it.  Page (o, k) is cache[o..., ids[k]] over the dims after `dim`, in index_select order (outer index
-        major): those dims must form one contiguous block of a multiple of 16 bytes, the outer dims must collapse to one
-        positive stride, the blocks must not overlap one another (no zero or negative strides: an expanded cache takes
-        the fallback), every page must be 16-byte aligned, and the page at least `min_page` bytes (by default
-        PAGED_MIN_PAGE_BYTES; FP8_PAGED_MIN_PAGE_BYTES for packed objects).  The addresses are a numpy int64 array, built without a loop per
-        page."""
+        """(page addresses, page bytes, rows) of cache.index_select(dim, ids) for the paged device calls, or None when they
+        should not move it.  Page (o, k) is cache[o..., ids[k]] over the dims after `dim`, in index_select order (outer
+        index major): those dims must be one contiguous block (rows None), or rows inside the block, rows =
+        (row_width, row_pitch) in bytes as _source_rows gives them for one block (a head slice of a KV cache: a trailing
+        contiguous block gives the width, the other dims collapse to one pitch), with rows of at least PAGED_MIN_ROW_BYTES
+        and a gap between them of a multiple of 16 bytes.  The page (its dense bytes) must be a multiple of 16 bytes and at
+        least `min_page` bytes (by default PAGED_MIN_PAGE_BYTES; FP8_PAGED_MIN_PAGE_BYTES for packed objects), the outer dims
+        must collapse to one positive stride, the blocks must not overlap one another over their true extent (no zero or
+        negative strides: an expanded cache takes the fallback) and every page must be 16-byte aligned.  The addresses are
+        a numpy int64 array, built without a loop per page."""
         if not cache.is_cuda or cache.numel() == 0 or ids.size == 0:
             return None
         es, shape, stride = cache.element_size(), cache.shape, cache.stride()
-        page = es
-        for n, s in reversed([(n, s) for n, s in zip(shape[dim + 1:], stride[dim + 1:]) if n != 1]):
-            if s * es != page:
+        inner = [(n, s) for n, s in zip(shape[dim + 1:], stride[dim + 1:]) if n != 1]
+        width = es
+        while inner and inner[-1][1] * es == width:  # the trailing contiguous block
+            width *= inner.pop()[0]
+        page, extent, rows = width, width, None
+        if inner:  # rows inside the block: the other dims must collapse to one pitch
+            if any(s != s2 * n2 for (_, s), (n2, s2) in zip(inner, inner[1:])):
                 return None
-            page *= n
+            n, pitch = int(np.prod([n for n, _ in inner], dtype=np.int64)), inner[-1][1] * es
+            if pitch <= width or (pitch - width) % 16 or width < PAGED_MIN_ROW_BYTES:
+                return None
+            page, extent, rows = n * width, (n - 1) * pitch + width, (width, pitch)
         if page % 16 or page < (PAGED_MIN_PAGE_BYTES if min_page is None else min_page):
             return None
         outer = [(n, s) for n, s in zip(shape[:dim], stride[:dim]) if n != 1]
@@ -300,7 +322,6 @@ class TensorStore:
         o_step = outer[-1][1] * es if outer else 0
         b_step = stride[dim] * es
         # disjoint blocks: every (outer, block) step positive and at least the extent of the smaller steps' blocks
-        extent = page
         for n, step in sorted([(n, st) for n, st in ((n_outer, o_step), (shape[dim], b_step)) if n > 1], key=lambda t: t[1]):
             if step < extent:
                 return None
@@ -308,7 +329,12 @@ class TensorStore:
         addrs = (cache.data_ptr() + np.arange(n_outer, dtype=np.int64)[:, None] * o_step + ids[None, :] * b_step).reshape(-1)
         if (addrs & 15).any():
             return None
-        return addrs, page
+        return addrs, page, rows
+
+    @staticmethod
+    def _rows_in(rows, es: int):
+        """A _block_pages row pattern in elements of `es` bytes (the packed calls count in elements), None kept."""
+        return None if rows is None else (rows[0] // es, rows[1] // es)
 
     def batch_put_blocks(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0, pack_fp8: bool = False,
                          config=None) -> None:
@@ -352,13 +378,14 @@ class TensorStore:
         if paged and pack_fp8:
             def call(grp, es, wide):
                 return self.client.batch_put_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp],
-                                                              [pages[i][1] // es for i in grp], cfg, self._stream(), wide=wide)
+                                                              [pages[i][1] // es for i in grp], cfg, self._stream(), wide=wide,
+                                                              rows=[self._rows_in(pages[i][2], es) for i in grp])
 
             refused = set(self._packed("paged fp8 put", keys, paged, lambda i: caches[i].dtype, call))
             paged = [i for grp in _by_dtype(paged, lambda i: caches[i].dtype).values() for i in grp if i not in refused]
         elif paged:
             ecs = self.client.batch_put_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged], [pages[i][1] for i in paged],
-                                                     cfg, self._stream())
+                                                     cfg, self._stream(), rows=[pages[i][2] for i in paged])
             _check("paged put", [keys[i] for i in paged], ecs)
         if paged:
             self._put_metas([keys[i] for i in paged], [_meta(caches[i].dtype, shapes[i], pack_fp8) for i in paged])
@@ -452,18 +479,18 @@ class TensorStore:
                 fp8_min = FP8_PAGED_MIN_PAGE_BYTES if sel[i] is None else FP8_PARTIAL_MIN_PAGE_BYTES
                 pages[i] = self._block_pages(caches[i], dims[i], idx[i], fp8_min if fp8[i] else PAGED_MIN_PAGE_BYTES)
             if pages[i] is not None and sel[i] is not None:
-                pages[i] = (self._sparse_table(pages[i][0], sel[i], metas[i]["shape"][dims[i]]), pages[i][1])
+                pages[i] = (self._sparse_table(pages[i][0], sel[i], metas[i]["shape"][dims[i]]), pages[i][1], pages[i][2])
 
         def call(grp, es, wide):
             return self.client.batch_get_device_fp8_paged([keys[i] for i in grp], [pages[i][0] for i in grp], [pages[i][1] // es for i in grp],
-                                                          self._stream(), wide=wide)
+                                                          self._stream(), wide=wide, rows=[self._rows_in(pages[i][2], es) for i in grp])
 
         for i in self._packed("paged fp8 get", keys, [i for i, p in enumerate(pages) if p is not None and fp8[i]], lambda i: caches[i].dtype, call):
             pages[i] = None  # get + index_copy_ below
         paged = [i for i, p in enumerate(pages) if p is not None and not fp8[i]]
         if paged:
             ecs, sizes = self.client.batch_get_device_paged([keys[i] for i in paged], [pages[i][0] for i in paged],
-                                                            [pages[i][1] for i in paged], self._stream())
+                                                            [pages[i][1] for i in paged], self._stream(), rows=[pages[i][2] for i in paged])
             # the stored object must fill the table: a shorter one would leave the last blocks as they were; those are
             # named after the items that failed
             short = [f"{n} bytes stored, {pages[i][0].size * pages[i][1]} selected" if e == _bb.ErrorCode.OK and n != pages[i][0].size * pages[i][1]
@@ -520,15 +547,16 @@ class TensorStore:
         if any(a + extent > b for a, b in zip(starts, starts[1:])):
             return None
         base = layers[0].data_ptr()
-        pages = [(first[0] + (c.data_ptr() - base), first[1]) for c in layers]
         wide = ids.dtype == torch.int64 or (sel is not None and sel.dtype == torch.int64)
         dt = torch.int64 if wide else torch.int32
         ids = ids.to(dt).contiguous()
         sel = None if sel is None else sel.to(dt).contiguous()
-        outer = np.concatenate([p[0] for p in pages])
-        page = pages[0][1] // es if packed else pages[0][1]
-        b = _bb.DeviceBlocks(outer, ids.data_ptr(), ids.numel(), layers[0].shape[dim], stride, page, id_bytes=dt.itemsize,
-                             sel=0 if sel is None else sel.data_ptr(), n_stored=n_stored if sel is not None else 0)
+        outer = np.concatenate([first[0] + (c.data_ptr() - base) for c in layers])
+        unit = es if packed else 1
+        rows = self._rows_in(first[2], unit) or (0, 0)
+        b = _bb.DeviceBlocks(outer, ids.data_ptr(), ids.numel(), layers[0].shape[dim], stride, first[1] // unit, id_bytes=dt.itemsize,
+                             sel=0 if sel is None else sel.data_ptr(), n_stored=n_stored if sel is not None else 0,
+                             row_width=rows[0], row_pitch=rows[1])
         return b, (ids, sel)
 
     @staticmethod

@@ -651,9 +651,12 @@ static ErrorCode rows_item(uint64_t width, uint64_t pitch, uint64_t rows, Shaped
   return DeviceLayout::from_rows(width, pitch, rows, &it->mem, &it->units, &extent);
 }
 
-static ErrorCode pages_item(const std::vector<uint64_t>& pages, uint64_t page, ShapedItem* it) {
+// Item i of a paged call: its pages, with the in-page row pattern page_rows[i] when the call has one ((0, 0): none).
+static ErrorCode pages_item(const std::vector<uint64_t>& pages, uint64_t page, const std::vector<PageRows>& page_rows, size_t i,
+                            ShapedItem* it) {
   it->table = true;
-  return DeviceLayout::from_pages(pages.size(), page, pages.data(), &it->mem, &it->units);
+  const PageRows r = page_rows.empty() ? PageRows{} : page_rows[i];
+  return DeviceLayout::from_pages(pages.size(), page, pages.data(), &it->mem, &it->units, r.first, r.second);
 }
 
 static ErrorCode blocks_item(const SourceBlocks& blocks, ShapedItem* it) {
@@ -782,11 +785,11 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_strided(const std::
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                    const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
-                                                                   mxfp8::Wide wide) {
+                                                                   mxfp8::Wide wide, const std::vector<PageRows>& page_rows) {
   const size_t n = keys.size();
   return shaped_put(
-      "device_put_fp8_paged", keys, std::vector<const void*>(n), pages.size() == n && page_elems.size() == n, wide,
-      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], it); }, cfg, stream);
+      "device_put_fp8_paged", keys, std::vector<const void*>(n), pages.size() == n && page_elems.size() == n && (page_rows.empty() || page_rows.size() == n), wide,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], page_rows, i, it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<const void*>& bf16_ptrs,
@@ -909,11 +912,12 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                                   const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide) {
+                                                                   const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide,
+                                                                   const std::vector<PageRows>& page_rows) {
   const size_t n = keys.size();
   return shaped_get(
-      "device_get_fp8_paged", keys, std::vector<void*>(n), pages.size() == n && page_elems.size() == n, wide,
-      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], it); }, stream, nullptr);
+      "device_get_fp8_paged", keys, std::vector<void*>(n), pages.size() == n && page_elems.size() == n && (page_rows.empty() || page_rows.size() == n), wide,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_elems[i], page_rows, i, it); }, stream, nullptr);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,
@@ -1208,11 +1212,12 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_strided(const std::vect
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                               const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream) {
+                                                               const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream,
+                                                               const std::vector<PageRows>& page_rows) {
   const size_t n = keys.size();
   return shaped_put(
-      "device_put_paged", keys, std::vector<const void*>(n), pages.size() == n && page_bytes.size() == n, std::nullopt,
-      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], it); }, cfg, stream);
+      "device_put_paged", keys, std::vector<const void*>(n), pages.size() == n && page_bytes.size() == n && (page_rows.empty() || page_rows.size() == n), std::nullopt,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], page_rows, i, it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
@@ -1413,11 +1418,12 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_scatter(const std::vect
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                               const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes) {
+                                                               const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes,
+                                                               const std::vector<PageRows>& page_rows) {
   const size_t n = keys.size();
   return shaped_get(
-      "device_get_paged", keys, std::vector<void*>(n), pages.size() == n && page_bytes.size() == n, std::nullopt,
-      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], it); }, stream, out_sizes);
+      "device_get_paged", keys, std::vector<void*>(n), pages.size() == n && page_bytes.size() == n && (page_rows.empty() || page_rows.size() == n), std::nullopt,
+      [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], page_rows, i, it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,

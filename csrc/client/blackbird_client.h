@@ -19,6 +19,7 @@
 #include <mutex>
 #include <optional>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "common/metrics.h"
@@ -28,6 +29,9 @@
 #include "rpc/rpc_service.h"
 
 namespace bb::client {
+
+// The in-page row pattern of one paged object, (row_width, row_pitch) in its units (SourcePages); (0, 0): one row per page.
+using PageRows = std::pair<uint64_t, uint64_t>;
 
 struct BlackbirdClientOptions {
   std::string keystone_host = "127.0.0.1";
@@ -231,7 +235,7 @@ class BlackbirdClient {
   // pages, page_elems[i] % 8 == 0.
   std::vector<ErrorCode> batch_put_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                     const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, void* stream,
-                                                    mxfp8::Wide wide = mxfp8::Wide::BF16);
+                                                    mxfp8::Wide wide = mxfp8::Wide::BF16, const std::vector<PageRows>& page_rows = {});
   // Gets of packed tensors into pages, the mirror: object i is unpacked into the pages pages[i] of page_elems[i] elements,
   // element x in page x / page_elems[i] at element x % page_elems[i], by the paged scattering store of the fused unpack.
   // Only the object's elements are written; pages of one get must not overlap (not checked).  A zero page address is a
@@ -244,7 +248,8 @@ class BlackbirdClient {
   // SourcePages::fused_get_aligned in wide bytes -- there is no host-staged path; the rest of the batch keeps the fused
   // launch.
   std::vector<ErrorCode> batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                    const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+                                                    const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16,
+                                                    const std::vector<PageRows>& page_rows = {});
   // Packed puts and gets from block ids that stay on the device: batch_put_device_blocks and batch_get_device_blocks for
   // packed tensors, `page` counted in elements of `wide` (the stride and slice addresses in bytes), with the rules of
   // batch_put_device_fp8_paged and batch_get_device_fp8_paged.  Per object, the shaped calls' admission (shaped_put,
@@ -330,9 +335,13 @@ class BlackbirdClient {
   // several pages, page_bytes[i] % 16 == 0).  Any other item, and every placement the fabric cannot reach, is staged
   // through the host (one D2H copy per run of pages) while the rest of the batch keeps the fused launch.  Per object, the
   // shaped calls' admission (shaped_put) of SourcePages::from_pages: INVALID_ARGUMENT for page_bytes[i] == 0 with pages.
-  // No pages is a zero-byte object.
+  // No pages is a zero-byte object.  page_rows (PageRows), empty or one per object, makes every page of object i rows of
+  // page_rows[i].first bytes every page_rows[i].second bytes inside its block (a head slice of a KV block; (0, 0): one
+  // row), under the from_pages rules of the pattern; co-aligned then also needs a gap between rows that is a multiple
+  // of 16 bytes.  The four paged calls, byte and MXFP8, take it alike (MXFP8 in elements); SourceBlocks carries its own.
   std::vector<ErrorCode> batch_put_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream);
+                                                const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, void* stream,
+                                                const std::vector<PageRows>& page_rows = {});
   // Paged gets, the mirror: object i lands in the pages pages[i] of page_bytes[i] bytes, object byte x in page
   // x / page_bytes[i] at offset x % page_bytes[i].  The capacity is pages[i].size() * page_bytes[i]: a larger object is
   // BUFFER_OVERFLOW, a shorter one fills its bytes in page order; out_sizes[i] receives the size.  Only the object's bytes
@@ -344,7 +353,8 @@ class BlackbirdClient {
   // reach, is staged through the host (one H2D copy per run of pages).  Per object, the shaped calls' admission
   // (shaped_get) of SourcePages::from_pages: INVALID_ARGUMENT for page_bytes[i] == 0 with pages.
   std::vector<ErrorCode> batch_get_device_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
-                                                const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes);
+                                                const std::vector<uint64_t>& page_bytes, void* stream, std::vector<size_t>* out_sizes,
+                                                const std::vector<PageRows>& page_rows = {});
   // Paged puts from block ids that stay on the device: object i is the pages of blocks[i] (SourceBlocks in
   // common/store_window.h: outer slice q, block ids[k], page r = q * n_ids + k at outer[q] + ids[k] * stride), in page
   // order, as batch_put_device_paged of that table would store it.  The ids are read on `stream` by the transfer

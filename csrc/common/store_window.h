@@ -252,14 +252,19 @@ struct SourceRows {
 
 // SourcePages: a dense object cut into equal pages of `page` bytes that sit at arbitrary addresses (the blocks of a paged
 // KV cache), on either side of a transfer: the source a device put reads from, or the destination a device get stores
-// into.  Object byte x lives at
-//   addrs[(x + phase) / page] + (x + phase) % page
+// into.  A page may itself be rows inside its block (a head slice of a KV block): `row_width` bytes every `row_pitch`
+// bytes, n = page / row_width rows per page.  With k = (x + phase) / page and c = (x + phase) % page, object byte x lives at
+//   addrs[k] + c                                            row_width == 0 (one row per page, the default)
+//   addrs[k] + (c / row_width) * row_pitch + c % row_width  an in-page row pattern
 // `addrs` is a host array of npages page addresses owned by the caller.  SourceRows is the special case
 // addrs[k] = src + k * pitch (with page = width).  This is the one statement of the rule; the transfer engine (XferItem,
 // Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client, the host loopback transport and the kernels'
-// XFER_PAGED descriptors (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.  The unit of `page` and
-// `phase` is a byte, or for an MXFP8 transfer an element of the wide side (to_wide_bytes() turns elements into bytes);
-// the addresses are byte addresses either way.
+// XFER_PAGED descriptors (kernels/xfer.h) all follow it.  page == 0 (the default) is no table.  The unit of `page`,
+// `phase`, `row_width` and `row_pitch` is a byte, or for an MXFP8 transfer an element of the wide side (to_wide_bytes()
+// turns elements into bytes); the addresses are byte addresses either way.  `page` stays the dense bytes of a page, so
+// the pattern changes neither the object's size nor where its shards are cut.  A pattern is 0 < row_width < row_pitch
+// with page % row_width == 0 and more than one row per page; from_pages() drops one whose rows touch or that has one row
+// per page, which is the same memory as no pattern.
 //
 // An address of 0 is a null page: on the get side, the object bytes that fall in it are not stored (a partial restore
 // into some of a cache's blocks).  No CUDA allocation or host buffer lives at address 0, so the marker cannot collide
@@ -269,20 +274,43 @@ struct SourceRows {
 struct SourcePages {
   const uint64_t* addrs = nullptr;
   uint64_t npages = 0, page = 0, phase = 0;
+  uint64_t row_width = 0, row_pitch = 0;  // in-page row pattern; 0 / 0: one row per page
 
   bool paged() const { return page != 0; }
-  // The table of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4): page and
-  // phase times b, the same addresses.  False when either product overflows.
+  bool has_rows() const { return row_width != 0; }
+  // The in-page pattern of pages of `page` units, checked and normalised: INVALID_ARGUMENT when exactly one of *width and
+  // *pitch is 0, *width > *pitch or page % *width != 0; VALUE_OUT_OF_RANGE when a page's extent,
+  // (page / *width - 1) * *pitch + *width, overflows.  A pattern with one row per page or rows that touch becomes 0 / 0.  SourceBlocks::from_blocks applies it too.
+  static ErrorCode page_rows(uint64_t page, uint64_t* width, uint64_t* pitch) {
+    if ((*width == 0) != (*pitch == 0)) return ErrorCode::INVALID_ARGUMENT;
+    if (*width == 0) return ErrorCode::OK;
+    if (*width > *pitch || page % *width) return ErrorCode::INVALID_ARGUMENT;
+    uint64_t e = 0;
+    if (__builtin_mul_overflow(page / *width - 1, *pitch, &e) || __builtin_add_overflow(e, *width, &e)) return ErrorCode::VALUE_OUT_OF_RANGE;
+    if (*width == page || *width == *pitch) *width = *pitch = 0;
+    return ErrorCode::OK;
+  }
+  // Where in-page unit c of a page lies from the page's address.
+  uint64_t in_page(uint64_t c) const { return has_rows() ? c / row_width * row_pitch + c % row_width : c; }
+  // The table of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4): page,
+  // phase and the row pattern times b, the same addresses.  False when a product overflows.
   bool to_wide_bytes(uint64_t b, SourcePages* out) const {
-    uint64_t pb = 0, fb = 0;
-    if (__builtin_mul_overflow(page, b, &pb) || __builtin_mul_overflow(phase, b, &fb)) return false;
-    *out = {addrs, npages, pb, fb};
-    return true;
+    *out = *this;
+    return !__builtin_mul_overflow(page, b, &out->page) && !__builtin_mul_overflow(phase, b, &out->phase) &&
+           !__builtin_mul_overflow(row_width, b, &out->row_width) && !__builtin_mul_overflow(row_pitch, b, &out->row_pitch);
   }
   // Pages that object bytes [0, len) touch.
   uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
-  // Whether the table holds every page of an object of `len` bytes, with phase < page.
-  bool valid(uint64_t len) const { return paged() && phase < page && pages_for(len) <= npages; }
+  // Whether the table holds every page of an object of `len` bytes, with phase < page, and its pattern is one
+  // page_rows() keeps.
+  bool valid(uint64_t len) const {
+    return paged() && phase < page && pages_for(len) <= npages && rows_valid(page, row_width, row_pitch);
+  }
+  // Whether (width, pitch) is a pattern page_rows() keeps for pages of `page` units: 0 / 0, or more than one row per page
+  // with gaps between them.
+  static bool rows_valid(uint64_t page, uint64_t width, uint64_t pitch) {
+    return width == 0 ? pitch == 0 : width < pitch && width < page && page % width == 0;
+  }
   // Whether a page that object bytes [0, len) touch is null.
   bool has_null(uint64_t len) const {
     const uint64_t n = pages_for(len);
@@ -291,15 +319,19 @@ struct SourcePages {
     return false;
   }
 
-  // The table of `npages` pages of `page` bytes at addrs: an object of *size = npages * page bytes.  INVALID_ARGUMENT for
-  // page == 0 with pages; VALUE_OUT_OF_RANGE when the product overflows.  No pages is a zero-byte object (no table).
-  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, SourcePages* out, uint64_t* size) {
+  // The table of `npages` pages of `page` bytes at addrs, each page rows of row_width bytes every row_pitch bytes (0 / 0:
+  // one row): an object of *size = npages * page bytes.  INVALID_ARGUMENT for page == 0 with pages and for a pattern
+  // page_rows() refuses; VALUE_OUT_OF_RANGE when the product or a page's extent overflows.  No pages is a zero-byte object
+  // (no table).
+  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, SourcePages* out, uint64_t* size,
+                              uint64_t row_width = 0, uint64_t row_pitch = 0) {
     *out = {};
     *size = 0;
     if (npages == 0) return ErrorCode::OK;
     if (page == 0) return ErrorCode::INVALID_ARGUMENT;
+    if (const ErrorCode ec = page_rows(page, &row_width, &row_pitch); ec != ErrorCode::OK) return ec;
     if (__builtin_mul_overflow(npages, page, size)) return ErrorCode::VALUE_OUT_OF_RANGE;
-    *out = {addrs, npages, page, 0};
+    *out = {addrs, npages, page, 0, row_width, row_pitch};
     return ErrorCode::OK;
   }
 
@@ -308,16 +340,18 @@ struct SourcePages {
   SourcePages rebase(uint64_t off) const {
     if (!paged()) return *this;
     const uint64_t k = (phase + off) / page;
-    return {addrs + std::min(k, npages), npages - std::min(k, npages), page, (phase + off) % page};
+    return {addrs + std::min(k, npages), npages - std::min(k, npages), page, (phase + off) % page, row_width, row_pitch};
   }
 
   // Whether object bytes [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by
-  // TMA: byte x of page k lives at addrs[k] + phase - k * page + x, so addrs[k] + phase must be 16-byte aligned for every
-  // non-null page touched, and the page a multiple of 16 bytes when more than one page is touched.  (With phase % 16 == 0,
-  // as for a table cut at 16-byte shard starts, that is every page 16-byte aligned.)
+  // TMA: byte x of in-page row j of page k lives at addrs[k] + phase - k * page + j * (row_pitch - row_width) + x, so
+  // addrs[k] + phase must be 16-byte aligned for every non-null page touched, the page a multiple of 16 bytes when more
+  // than one page is touched, and with a pattern the gap between rows a multiple of 16 (decided by the pattern, not by
+  // how many rows the span touches, as SourceRows::fused_get_aligned).  (With phase % 16 == 0, as for a table cut at
+  // 16-byte shard starts, that is every page 16-byte aligned.)
   bool coaligned(uint64_t len) const {
     const uint64_t n = pages_for(len);
-    if (n > 1 && page % 16) return false;
+    if ((n > 1 && page % 16) || (n > 0 && has_rows() && (row_pitch - row_width) % 16)) return false;
     for (uint64_t k = 0; k < n; ++k)
       if (addrs[k] != 0 && (addrs[k] + phase) % 16) return false;
     return true;
@@ -334,23 +368,26 @@ struct SourcePages {
   }
 
   // Calls f(x, addr, n) for every run of n contiguous bytes of object bytes [0, len): object bytes [x, x + n) live at
-  // [addr, addr + n), in order.  Pages that follow one another in memory make one run; null pages make none and end the
-  // run before them.
+  // [addr, addr + n), in order.  One segment per page, or per in-page row with a pattern; segments that follow one
+  // another in memory make one run; null pages make none and end the run before them.
   template <class F>
   void for_each_run(uint64_t len, F&& f) const {
+    const uint64_t w = has_rows() ? row_width : page;
     uint64_t x = 0, run_x = 0, run_at = 0, run_n = 0;
     for (uint64_t k = 0; x < len; ++k) {
-      const uint64_t c = k == 0 ? phase : 0, n = std::min(page - c, len - x), at = addrs[k] + c;
-      if (addrs[k] == 0) {
-        if (run_n) f(run_x, run_at, run_n);
-        run_n = 0;
-      } else if (run_n && run_at + run_n == at) {
-        run_n += n;
-      } else {
-        if (run_n) f(run_x, run_at, run_n);
-        run_x = x, run_at = at, run_n = n;
+      for (uint64_t c = k == 0 ? phase : 0; c < page && x < len;) {
+        const uint64_t n = std::min(w - c % w, len - x), at = addrs[k] + in_page(c);
+        if (addrs[k] == 0) {
+          if (run_n) f(run_x, run_at, run_n);
+          run_n = 0;
+        } else if (run_n && run_at + run_n == at) {
+          run_n += n;
+        } else {
+          if (run_n) f(run_x, run_at, run_n);
+          run_x = x, run_at = at, run_n = n;
+        }
+        x += n, c += n;
       }
-      x += n;
     }
     if (run_n) f(run_x, run_at, run_n);
   }
@@ -363,8 +400,8 @@ struct SourcePages {
 //   outer[q] + ids[k] * stride
 // With a selection `sel` (a partial restore, gets only) it has n_outer * n_stored pages: page q * n_stored + sel[m] is at
 // outer[q] + ids[m] * stride and every other page is a null page (not stored, as SourcePages').  Object bytes then map
-// onto the pages exactly as SourcePages maps them, with `page` and `phase` in its units; `first` is the table's first page
-// after rebase().  `outer` is a small host array, one entry per slice; `ids` and `sel` are n_ids integers of id_bytes (4
+// onto the pages exactly as SourcePages maps them, with `page`, `phase` and the in-page row pattern (row_width,
+// row_pitch: a head slice of each block) in its units; `first` is the table's first page after rebase().  `outer` is a small host array, one entry per slice; `ids` and `sel` are n_ids integers of id_bytes (4
 // or 8, signed) that the host never reads on the device route: the transfer engine's resolve kernel builds the page
 // table on the device (kernels/resolve_blocks.cu) and the host loopback transport calls resolve() below, the reference.
 //
@@ -372,7 +409,7 @@ struct SourcePages {
 // INVALID_ARGUMENT; a selection's entries in [0, n_stored) and pairwise distinct, under the same two codes.  A refused
 // table never leads a transfer outside the caller's cache: a get's entries are all null (nothing is stored) and a put's
 // are all block 0 of their slice, outer[q] (the put is then cancelled).  Co-alignment needs no id: every address is
-// outer[q] + a multiple of the stride, so coaligned() is a closed form over outer[], stride and page.
+// outer[q] + a multiple of the stride, so coaligned() is a closed form over outer[], stride, page and the pattern.
 struct SourceBlocks {
   const uint64_t* outer = nullptr;
   uint64_t n_outer = 0;
@@ -382,6 +419,7 @@ struct SourceBlocks {
   uint64_t n_stored = 0;
   uint32_t id_bytes = 4;
   uint64_t n_blocks = 0, stride = 0, page = 0, phase = 0, first = 0;
+  uint64_t row_width = 0, row_pitch = 0;  // in-page row pattern, as SourcePages'
 
   // Gets check duplicates in a bitmap of this many bits over n_blocks (and n_stored) in the resolve kernel's shared
   // memory; a larger bound is NOT_IMPLEMENTED on the device route.
@@ -391,10 +429,11 @@ struct SourceBlocks {
   uint64_t per_outer() const { return sel ? n_stored : n_ids; }
   uint64_t npages() const { return n_outer * per_outer(); }
   uint64_t pages_for(uint64_t len) const { return len == 0 || !paged() ? 0 : (len - 1 + phase) / page + 1; }
-  // Whether the table holds every page of an object of `len` units from page `first`, with phase < page.
+  // Whether the table holds every page of an object of `len` units from page `first`, with phase < page, and its pattern
+  // is one SourcePages::page_rows keeps.
   bool valid(uint64_t len) const {
     return paged() && phase < page && (id_bytes == 4 || id_bytes == 8) && first + pages_for(len) <= npages() &&
-           (n_ids == 0 || (ids && n_blocks != 0)) && (n_outer == 0 || outer);
+           (n_ids == 0 || (ids && n_blocks != 0)) && (n_outer == 0 || outer) && SourcePages::rows_valid(page, row_width, row_pitch);
   }
   // A put reads every unit: no selection, whose pages may be null.
   bool has_null() const { return sel != nullptr; }
@@ -402,8 +441,9 @@ struct SourceBlocks {
   bool distinct_checkable() const { return n_blocks <= kMaxDistinct && (!sel || n_stored <= kMaxDistinct); }
 
   // The table of ids.size() blocks of every slice in outer[], pages of `page` units: an object of *size = n_outer *
-  // per_outer() * page units.  INVALID_ARGUMENT for page == 0 with pages, a selection without stored blocks or ids of
-  // another width than 4 or 8 bytes; VALUE_OUT_OF_RANGE when the size overflows.  No pages is a zero-unit object.
+  // per_outer() * page units.  INVALID_ARGUMENT for page == 0 with pages, a selection without stored blocks, ids of
+  // another width than 4 or 8 bytes or a pattern SourcePages::page_rows refuses (which also normalises it);
+  // VALUE_OUT_OF_RANGE when the size or a page's extent overflows.  No pages is a zero-unit object.
   static ErrorCode from_blocks(const SourceBlocks& b, SourceBlocks* out, uint64_t* size) {
     *out = b;
     out->first = 0, out->phase = 0;
@@ -413,15 +453,18 @@ struct SourceBlocks {
     if (__builtin_mul_overflow(b.n_outer, out->per_outer(), &pages)) return ErrorCode::VALUE_OUT_OF_RANGE;
     if (pages == 0) return ErrorCode::OK;
     if (b.page == 0) return ErrorCode::INVALID_ARGUMENT;
+    if (const ErrorCode ec = SourcePages::page_rows(b.page, &out->row_width, &out->row_pitch); ec != ErrorCode::OK) return ec;
     if (__builtin_mul_overflow(pages, b.page, size)) return ErrorCode::VALUE_OUT_OF_RANGE;
     return ErrorCode::OK;
   }
+  bool has_rows() const { return row_width != 0; }
 
-  // The table in bytes of elements of `b` bytes (an MXFP8 transfer's wide side): page and phase times b, the same
-  // addresses and stride.  False when either product overflows.
+  // The table in bytes of elements of `b` bytes (an MXFP8 transfer's wide side): page, phase and the row pattern times b,
+  // the same addresses and stride.  False when a product overflows.
   bool to_wide_bytes(uint64_t b, SourceBlocks* out) const {
     *out = *this;
-    return !__builtin_mul_overflow(page, b, &out->page) && !__builtin_mul_overflow(phase, b, &out->phase);
+    return !__builtin_mul_overflow(page, b, &out->page) && !__builtin_mul_overflow(phase, b, &out->phase) &&
+           !__builtin_mul_overflow(row_width, b, &out->row_width) && !__builtin_mul_overflow(row_pitch, b, &out->row_pitch);
   }
   // The table seen from object unit `off`: unit x of the result is unit off + x here (as SourcePages::rebase).
   SourceBlocks rebase(uint64_t off) const {
@@ -432,11 +475,12 @@ struct SourceBlocks {
     return r;
   }
   // SourcePages::coaligned for every table the ids could make: the stride a multiple of 16 bytes, every outer[q] + phase
-  // 16-byte aligned, and the page a multiple of 16 when object units [0, len) touch more than one page.
+  // 16-byte aligned, the page a multiple of 16 when object units [0, len) touch more than one page, and with a pattern
+  // the gap between rows a multiple of 16.
   bool coaligned(uint64_t len) const {
     const uint64_t n = pages_for(len);
     if (n == 0) return true;
-    if ((n > 1 && page % 16) || stride % 16) return false;
+    if ((n > 1 && page % 16) || stride % 16 || (has_rows() && (row_pitch - row_width) % 16)) return false;
     for (uint64_t q = 0; q < n_outer; ++q)
       if ((outer[q] + phase) % 16) return false;
     return true;
@@ -515,9 +559,10 @@ class DeviceLayout {
     *out = DeviceLayout(r);
     return ec;
   }
-  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, DeviceLayout* out, uint64_t* size) {
+  static ErrorCode from_pages(uint64_t npages, uint64_t page, const uint64_t* addrs, DeviceLayout* out, uint64_t* size,
+                              uint64_t row_width = 0, uint64_t row_pitch = 0) {
     SourcePages p;
-    const ErrorCode ec = SourcePages::from_pages(npages, page, addrs, &p, size);
+    const ErrorCode ec = SourcePages::from_pages(npages, page, addrs, &p, size, row_width, row_pitch);
     *out = DeviceLayout(p);
     return ec;
   }
@@ -594,7 +639,7 @@ class DeviceLayout {
     if (kind_ != BLOCKS) return *this;
     table->assign(blocks_.pages_for(len), 0);
     *verdict = blocks_.resolve(table->data(), table->size(), get);
-    return DeviceLayout(SourcePages{table->data(), table->size(), blocks_.page, blocks_.phase});
+    return DeviceLayout(SourcePages{table->data(), table->size(), blocks_.page, blocks_.phase, blocks_.row_width, blocks_.row_pitch});
   }
 
  private:

@@ -110,8 +110,8 @@ struct XferEngine::Slot {
     reserved = 0;
   }
   // The table entry of descriptor k's gathered or scattered layout (in bytes, over nbytes): its pattern, or its page
-  // entries, or for blocks room for them and a resolve job (`get`: the scattering side).  Returns the XFER_PAGED flag for
-  // pages and blocks, 0 for rows.
+  // entries, or for blocks room for them and a resolve job (`get`: the scattering side), with the in-page row pattern of
+  // either.  Returns the XFER_PAGED flag for pages and blocks (and XFER_PAGE_ROWS with a pattern), 0 for rows.
   uint32_t set_layout(uint32_t k, const DeviceLayout& m, uint64_t nbytes, bool get) {
     if (m.kind() == DeviceLayout::ROWS) {
       set_stride(k, XferStride{m.rows().pitch, m.rows().width, m.rows().phase});
@@ -120,14 +120,14 @@ struct XferEngine::Slot {
     if (m.kind() == DeviceLayout::PAGES) {
       const SourcePages& p = m.pages();
       paged_descs.push_back(k);
-      set_stride(k, XferStride{{pages.size()}, p.page, p.phase});
+      set_stride(k, XferStride{{pages.size()}, p.page, p.phase, p.row_width, p.row_pitch});
       pages.insert(pages.end(), p.addrs, p.addrs + p.pages_for(nbytes));
-      return XFER_PAGED;
+      return p.has_rows() ? XFER_PAGED | XFER_PAGE_ROWS : XFER_PAGED;
     }
     const SourceBlocks& b = m.blocks();
     BlocksJob j{};
     blocks_descs.push_back(k);
-    set_stride(k, XferStride{{reserved}, b.page, b.phase});
+    set_stride(k, XferStride{{reserved}, b.page, b.phase, b.row_width, b.row_pitch});
     j.entries = reinterpret_cast<uint64_t*>(reserved);
     j.count = b.pages_for(nbytes);
     reserved += j.count;
@@ -138,7 +138,7 @@ struct XferEngine::Slot {
     j.stride = b.stride, j.first = b.first, j.id_bytes = b.id_bytes, j.get = get;
     j.verdict = reinterpret_cast<uint32_t*>(static_cast<uintptr_t>(k));
     jobs.push_back(j);
-    return XFER_PAGED;
+    return b.has_rows() ? XFER_PAGED | XFER_PAGE_ROWS : XFER_PAGED;
   }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
@@ -525,6 +525,9 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       return ErrorCode::INVALID_ARGUMENT;
     // a layout is the gathering load's source or the scattering store's destination, the side its flag names
     const bool blocks = it.mem.kind() == DeviceLayout::BLOCKS;
+    // XFER_PAGE_ROWS is the engine's to set, from the layout's pattern (set_layout): a caller's flag would send a
+    // descriptor without a pattern down the in-page row walk
+    if (it.flags & XFER_PAGE_ROWS) return ErrorCode::INVALID_ARGUMENT;
     if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES && !blocks) ||
         !(gather ? it.mem.valid_source(it.nbytes) : it.mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
         (scatter && (it.ndst != 1 || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))

@@ -36,7 +36,9 @@ struct XferItem {
   // Rows or pages (common/store_window.h) on one side of the transfer, which its flag names: a put's source with
   // XFER_GATHER (src is the layout's base), or a get's destination with XFER_SCATTER (dst[0] is).  A page table's base is
   // not read, and its entries are copied into the batch's device table by submit(), so the host array need only live
-  // until submit() returns; submit() sets XFER_PAGED for it.  INVALID_ARGUMENT for a side flag without a layout or a
+  // until submit() returns; submit() sets XFER_PAGED for it, and XFER_PAGE_ROWS when its pages are in-page rows (the
+  // pattern is checked by mem.valid and mem.coaligned); XFER_PAGE_ROWS among the caller's flags is INVALID_ARGUMENT.
+  // INVALID_ARGUMENT for a side flag without a layout or a
   // layout without one, XFER_PAGED without pages, !mem.valid(nbytes), XFER_GATHER with a null page
   // (!mem.valid_source(nbytes)), with XFER_WINDOW, XFER_STRIDED or XFER_RAW_SUM, and XFER_SCATTER with those, XFER_GATHER,
   // XFER_MULTIMEM or ndst != 1.  A scattering store's table may hold null pages: the bytes that fall in them are read and
@@ -76,7 +78,8 @@ struct Fp8Item {
   // The wide side's rows or pages in elements, the page addresses in bytes (common/store_window.h), `wide` being the
   // layout's base (not read for pages): a pack's source or an unpack's destination.  The default is contiguous.  run_fp8
   // sets XFER_GATHER or XFER_SCATTER for it, with XFER_PAGED for pages whose entries it copies into the batch's device
-  // table, so the host array need only live until run_fp8 returns.  An MX block may straddle two pages.  An unpack's table
+  // table (and XFER_PAGE_ROWS for in-page rows), so the host array need only live until run_fp8 returns.  An MX block may
+  // straddle two pages or two in-page rows.  An unpack's table
   // may hold null pages, whose elements are not stored; a pack's may not.
   // INVALID_ARGUMENT with a window, unless mem.valid(n_elems) (a pack: mem.valid_source(n_elems)), or when its wide-byte
   // arithmetic overflows;

@@ -57,6 +57,11 @@ enum XferFlags : uint32_t {
   // XFER_STRIDED or XFER_RAW_SUM.  The tile in shared memory is the dense object's tile, so the digest, the verify and
   // the stored bytes are those of a contiguous put or get.
   XFER_PAGED = 1u << 8,
+  // With XFER_PAGED only: every page is rows inside its block, the in-page row pattern of SourcePages: with the entry's
+  // row_width and row_pitch, c = (x + phase) % page and k = (x + phase) / page, object byte x is at
+  // pages[k] + (c / row_width) * row_pitch + c % row_width.  The kernels then move the dense object's rows of row_width
+  // bytes one per lane instead of whole pages; the tile is still the dense object's tile.
+  XFER_PAGE_ROWS = 1u << 9,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -91,13 +96,15 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 // congruent to x mod 16 (SourceRows::coaligned).  An XFER_SCATTER descriptor's entry is its destination rows, under the
 // same rules.  An XFER_PAGED descriptor's entry is {pages, page, phase}: `pages` the device address of the first of its
 // page entries (uint64_t addresses, one per page the descriptor touches), `page` in `width`, phase < page, every page
-// co-aligned: pages[k] + phase 16-byte aligned (SourcePages::coaligned).
+// co-aligned: pages[k] + phase 16-byte aligned (SourcePages::coaligned).  row_width and row_pitch are read only for
+// XFER_PAGE_ROWS descriptors: 0 < row_width < row_pitch, page % row_width == 0, (row_pitch - row_width) % 16 == 0.
 struct XferStride {
   union {
     uint64_t pitch;
     uint64_t pages;  // XFER_PAGED
   };
   uint64_t width, phase;
+  uint64_t row_width = 0, row_pitch = 0;  // XFER_PAGE_ROWS
 };
 
 constexpr uint32_t kSmallBytes = 4096;     // objects up to this size may take the warp-per-object path (xfer_small.cu)
@@ -124,7 +131,7 @@ struct XferLaunch {
   const XferDesc* host_descs = nullptr;
   const uint32_t* host_tile_start = nullptr;
   // Row patterns of the XFER_STRIDED, XFER_GATHER and XFER_SCATTER descriptors, one entry per descriptor (the entries of unflagged
-  // descriptors are never read); null when the batch has none.  host_strides is their copy for the kernel parameters of an
+  // descriptors are never read, nor row_width / row_pitch of descriptors without XFER_PAGE_ROWS); null when the batch has none.  host_strides is their copy for the kernel parameters of an
   // inline batch; a batch with XFER_PAGED descriptors has no inline copy (their entries point into device memory).
   const XferStride* strides = nullptr;
   const XferStride* host_strides = nullptr;

@@ -163,25 +163,42 @@ __device__ __forceinline__ uint64_t row_src(uint64_t src, uint64_t off, uint64_t
   return src + off + st.phase + r * (st.pitch - st.width);
 }
 // The same for a paged descriptor (XFER_PAGED, entry {pages, page, phase}): row r of the dense layout is page r, which
-// starts at pages[r], so tile byte o of it sits at pages[r] + off + phase - r * page + o.  `base` is ignored.
+// starts at pages[r], so tile byte o of it sits at pages[r] + off + phase - r * page + o.  `base` is ignored.  ROWS
+// (XFER_PAGE_ROWS): the dense layout's rows are the row_width-byte in-page rows instead, n = page / row_width per page,
+// row r being in-page row r % n of page r / n: tile byte o of it sits at
+// pages[r / n] + (r % n) * row_pitch + off + phase - r * row_width + o.
 __device__ __forceinline__ uint64_t page_entry(const XferStride& st, uint64_t r) {
   return __ldg(reinterpret_cast<const unsigned long long*>(st.pages) + r);
 }
-template <bool PAGED>
+template <bool PAGED, bool ROWS = false>
 __device__ __forceinline__ uint64_t row_addr(uint64_t base, uint64_t off, uint64_t r, const XferStride& st) {
-  if constexpr (PAGED) return page_entry(st, r) + off + st.phase - r * st.width;
-  else return row_src(base, off, r, st);
+  if constexpr (PAGED && ROWS) {
+    const uint64_t n = st.width / st.row_width;
+    return page_entry(st, r / n) + (r % n) * st.row_pitch + off + st.phase - r * st.row_width;
+  } else if constexpr (PAGED) {
+    return page_entry(st, r) + off + st.phase - r * st.width;
+  } else {
+    return row_src(base, off, r, st);
+  }
+}
+// The width of the dense layout's rows whose segments the gathering load and scattering store move: a page, or with
+// ROWS an in-page row.
+template <bool PAGED, bool ROWS>
+__device__ __forceinline__ uint64_t dense_row(const XferStride& st) {
+  return PAGED && ROWS ? st.row_width : st.width;
 }
 // The producer's part of a gathered tile: the row segments of the tile, one per lane, the middle bulk-loaded into `tile`
 // with completion on `bar`, head and tail by plain loads and shared stores.  Returns the bytes this lane's bulk loads
 // deliver; the caller sums them over the warp for the stage's expect_tx, and the calling lane still has to fence its
-// shared stores for the async proxy.  PAGED: the rows are the pages of an XFER_PAGED descriptor (row_addr).
-template <bool PAGED = false>
+// shared stores for the async proxy.  PAGED: the rows are the pages of an XFER_PAGED descriptor (row_addr), or with ROWS
+// their in-page rows.
+template <bool PAGED = false, bool ROWS = false>
 __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t* bar, uint64_t src, uint64_t off, uint32_t bytes,
                                                         const XferStride& st, uint32_t lane) {
   uint32_t tx = 0;
-  for_row_segments(off, 0, bytes, XferStride{{st.width}, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
-    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_addr<PAGED>(src, off, r, st));
+  const uint64_t w = dense_row<PAGED, ROWS>(st);
+  for_row_segments(off, 0, bytes, XferStride{{w}, w, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_addr<PAGED, ROWS>(src, off, r, st));
     if (g.a1 > g.a0) {
       ptx::bulk_g2s(tile + g.a0, s + g.a0, g.a1 - g.a0, bar);
       tx += g.a1 - g.a0;
@@ -196,18 +213,22 @@ __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t*
 // each stored at row_src(dst0, ...) as a TMA middle plus a byte-wise head and tail.  dst0 is the descriptor's dst[0], where
 // the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.  PAGED: the rows are
 // the pages of an XFER_PAGED descriptor (row_addr), dst0 is not read, and a page whose entry is 0 is not stored (the null
-// page of SourcePages): its lane stores nothing and still commits its empty bulk group.
-template <bool PAGED = false>
+// page of SourcePages): its lane stores nothing and still commits its empty bulk group.  ROWS: the segments are the
+// pages' in-page rows, and row r's page is r / (page / row_width).
+template <bool PAGED = false, bool ROWS = false>
 __device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t bytes,
                                                      const XferStride& st, uint32_t lane) {
-  for_row_segments(off, 0, bytes, XferStride{{st.width}, st.width, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
-    if (PAGED && page_entry(st, r) == 0) return;
-    store_segment(reinterpret_cast<uint8_t*>(row_addr<PAGED>(dst0, off, r, st)), tile, g);
+  const uint64_t w = dense_row<PAGED, ROWS>(st);
+  for_row_segments(off, 0, bytes, XferStride{{w}, w, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+    if (PAGED && page_entry(st, ROWS ? r / (st.width / st.row_width) : r) == 0) return;
+    store_segment(reinterpret_cast<uint8_t*>(row_addr<PAGED, ROWS>(dst0, off, r, st)), tile, g);
   });
 }
-// The row pattern of descriptor `i` from a device table (read-only path).
-__device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i) {
+// The row pattern of descriptor `i` from a device table (read-only path); `rows`: with the in-page row pattern of an
+// XFER_PAGE_ROWS descriptor, else without (those words are not read).
+__device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i, bool rows = false) {
   const uint64_t* e = reinterpret_cast<const uint64_t*>(&table[i]);
+  if (rows) return {__ldg(e), __ldg(e + 1), __ldg(e + 2), __ldg(e + 3), __ldg(e + 4)};
   return {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
 }
 

@@ -300,9 +300,13 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
             if (p.use_inline) gst = p.inl_strides[g_desc];
             else gst = load_stride(p.strides, g_desc);
           }
-          const uint32_t seg_tx = (e.m.ndst_flags >> 8) & XFER_PAGED
-                                      ? gather_row_segments<true>(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane)
-                                      : gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane);
+          // in-page rows (XFER_PAGE_ROWS, never inline): their pattern is read here, so that `gst` stays three words
+          const uint32_t gfl = e.m.ndst_flags >> 8;
+          const uint32_t seg_tx =
+              gfl & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.tile[stage], &s.full[stage], src_i, off, bytes,
+                                                                     load_stride(p.strides, g_desc, true), lane)
+              : gfl & XFER_PAGED   ? gather_row_segments<true>(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane)
+                                   : gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane);
           tx = __reduce_add_sync(0xffffffffu, seg_tx);
           wrote = true;
         } else if (lane < tail) {
@@ -354,7 +358,8 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
           if (p.use_inline) st = p.inl_strides[st_desc];
           else st = load_stride(p.strides, st_desc);
         }
-        if (flags & XFER_PAGED) scatter_row_segments<true>(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
+        if (flags & XFER_PAGE_ROWS) scatter_row_segments<true, true>(s.tile[stage], m.dst[0], off, m.bytes, load_stride(p.strides, st_desc, true), lane);
+        else if (flags & XFER_PAGED) scatter_row_segments<true>(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
         else if (flags & XFER_SCATTER) scatter_row_segments(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
         else store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);
       } else if (flags & XFER_MULTIMEM) {

@@ -77,7 +77,8 @@ struct FpMeta {            // 64 bytes
   uint32_t valid;          // payload bytes (= elements) of this tile: 16384, or the multiple-of-32 tail of the object
   uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
                            // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
-                           // FpParams::strides either way); XFER_PAGED as well when those rows are pages
+                           // FpParams::strides either way); XFER_PAGED as well when those rows are pages,
+                           // and XFER_PAGE_ROWS when the pages are in-page rows
   uint32_t f16;            // XFER_WIDE_F16: the wide side is fp16 (2-byte instantiation only)
   uint32_t pad;
 };
@@ -172,7 +173,7 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED : XFER_GATHER | XFER_PAGED);
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED | XFER_PAGE_ROWS : XFER_GATHER | XFER_PAGED | XFER_PAGE_ROWS);
         e.m.f16 = d.flags & XFER_WIDE_F16;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
@@ -233,9 +234,12 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             }
             // XFER_PAGED: the rows are the pages of the table in gst, e.src is not read
             const uint64_t off = static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes;
-            const uint32_t seg_tx = e.m.strided & XFER_PAGED
-                                        ? gather_row_segments<true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane)
-                                        : gather_row_segments(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane);
+            // XFER_PAGE_ROWS: their in-page rows, whose pattern is read here so that `gst` stays three words
+            const uint32_t seg_tx =
+                e.m.strided & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid,
+                                                                               load_stride(p.strides, g_desc, true), lane)
+                : e.m.strided & XFER_PAGED   ? gather_row_segments<true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane)
+                                             : gather_row_segments(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane);
             tx = __reduce_add_sync(0xffffffffu, seg_tx);
           }
           __syncwarp();
@@ -273,7 +277,9 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           }
           // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile.  A paged one stores
           // into the pages of the table in `pat` and does not read dst[0].
-          if (m.strided & XFER_PAGED) scatter_row_segments<true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
+          if (m.strided & XFER_PAGE_ROWS)
+            scatter_row_segments<true, true>(s.wide[st], m.dst[0] - off, off, x1, load_stride(p.strides, pat_desc, true), lane);
+          else if (m.strided & XFER_PAGED) scatter_row_segments<true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
           else if (m.strided & XFER_SCATTER) scatter_row_segments(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
           else store_row_segments(s.wide[st], m.dst[0] - off, off, x0, x1, pat, lane);
         } else {

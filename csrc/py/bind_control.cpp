@@ -67,6 +67,13 @@ std::vector<std::vector<uint64_t>> to_page_lists(const py::sequence& s) {
   for (auto h : s) out.push_back(to_page_addrs(h));
   return out;
 }
+// The `rows` argument of the paged calls: None (no pattern), or one (row_width, row_pitch) or None per object.
+std::vector<client::PageRows> to_page_rows(const py::object& rows) {
+  std::vector<client::PageRows> out;
+  if (rows.is_none()) return out;
+  for (auto h : py::cast<py::sequence>(rows)) out.push_back(h.is_none() ? client::PageRows{} : h.cast<client::PageRows>());
+  return out;
+}
 // SourcePages for Python: the table owns its page addresses (a rebased table shares them).  SourceBlocks is PyBlocks
 // (py/py_blocks.h), shared with the engine's bindings.
 struct PyPages {
@@ -413,24 +420,30 @@ void bind_control(py::module_& m) {
            py::arg("len"), "[(x, at, n)]: object bytes [x, x + n) are read from source bytes [at, at + n)");
   py::class_<PyPages>(m, "SourcePages",
                       "A dense object cut into equal pages at arbitrary addresses: a paged device put's source, or a paged get's "
-                      "destination (common/store_window.h).  Object byte x lives at addrs[(x + phase) // page] + (x + phase) % page.")
+                      "destination (common/store_window.h).  With k = (x + phase) // page and c = (x + phase) % page, object byte x "
+                      "lives at addrs[k] + c, or with an in-page row pattern at addrs[k] + (c // row_width) * row_pitch + "
+                      "c % row_width.")
       .def_property_readonly("npages", [](const PyPages& t) { return t.p.npages; })
       .def_property_readonly("page", [](const PyPages& t) { return t.p.page; })
       .def_property_readonly("phase", [](const PyPages& t) { return t.p.phase; })
+      .def_property_readonly("row_width", [](const PyPages& t) { return t.p.row_width; })
+      .def_property_readonly("row_pitch", [](const PyPages& t) { return t.p.row_pitch; })
       .def_property_readonly("addrs", [](const PyPages& t) { return std::vector<uint64_t>(t.p.addrs, t.p.addrs + t.p.npages); })
       .def("paged", [](const PyPages& t) { return t.p.paged(); })
       .def("valid", [](const PyPages& t, uint64_t len) { return t.p.valid(len); }, py::arg("len"))
       .def("has_null", [](const PyPages& t, uint64_t len) { return t.p.has_null(len); }, py::arg("len"),
            "whether a page that object bytes [0, len) touch has address 0 (not stored by a get, refused by a put)")
       .def_static("from_pages",
-                  [](const py::handle& addrs, uint64_t page) {
+                  [](const py::handle& addrs, uint64_t page, uint64_t row_width, uint64_t row_pitch) {
                     auto v = std::make_shared<const std::vector<uint64_t>>(to_page_addrs(addrs));
                     PyPages t{v, {}};
                     uint64_t size = 0;
-                    const ErrorCode ec = SourcePages::from_pages(v->size(), page, v->data(), &t.p, &size);
+                    const ErrorCode ec = SourcePages::from_pages(v->size(), page, v->data(), &t.p, &size, row_width, row_pitch);
                     return py::make_tuple(ec, t, size);
                   },
-                  py::arg("addrs"), py::arg("page"), "(ErrorCode, SourcePages, object bytes)")
+                  py::arg("addrs"), py::arg("page"), py::arg("row_width") = 0, py::arg("row_pitch") = 0,
+                  "(ErrorCode, SourcePages, object bytes); row_width / row_pitch: each page is rows of row_width bytes every "
+                  "row_pitch bytes (0 / 0: one row)")
       .def("rebase", [](const PyPages& t, uint64_t off) { return PyPages{t.addrs, t.p.rebase(off)}; }, py::arg("off"),
            "the table seen from object byte off")
       .def("to_wide_bytes",
@@ -450,26 +463,32 @@ void bind_control(py::module_& m) {
              t.p.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { out.emplace_back(x, at, n); });
              return out;
            },
-           py::arg("len"), "[(x, addr, n)]: object bytes [x, x + n) live at [addr, addr + n); adjacent pages make one run");
+           py::arg("len"),
+           "[(x, addr, n)]: object bytes [x, x + n) live at [addr, addr + n); one per page or in-page row, adjacent ones make "
+           "one run");
 
   py::class_<PyBlocks>(m, "DeviceBlocks",
                        "Pages of a paged KV cache named by block ids that stay on the device (SourceBlocks, common/store_window.h): "
                        "page r = q * n_ids + k of the object is at outer[q] + ids[k] * stride.  With a selection (sel, n_stored), "
                        "a partial restore, the object has n_outer * n_stored pages: page q * n_stored + sel[m] is at outer[q] + "
                        "ids[m] * stride and the others are not stored.  ids and sel are pointers to n_ids int32 (id_bytes=4) or "
-                       "int64 (id_bytes=8) values; the device route never reads them on the host.")
+                       "int64 (id_bytes=8) values; the device route never reads them on the host.  row_width / row_pitch: each page "
+                       "is rows of row_width units every row_pitch units inside its block, as SourcePages' (0 / 0: one row).")
       .def(py::init([](const py::handle& outer, uintptr_t ids, uint64_t n_ids, uint64_t n_blocks, uint64_t stride, uint64_t page,
-                       uint32_t id_bytes, uintptr_t sel, uint64_t n_stored) {
+                       uint32_t id_bytes, uintptr_t sel, uint64_t n_stored, uint64_t row_width, uint64_t row_pitch) {
              auto v = std::make_shared<const std::vector<uint64_t>>(to_page_addrs(outer));
              SourceBlocks b;
              b.outer = v->data(), b.n_outer = v->size();
              b.ids = reinterpret_cast<const void*>(ids), b.n_ids = n_ids;
              b.sel = reinterpret_cast<const void*>(sel), b.n_stored = n_stored;
              b.id_bytes = id_bytes, b.n_blocks = n_blocks, b.stride = stride, b.page = page;
+             b.row_width = row_width, b.row_pitch = row_pitch;
              return PyBlocks{v, b};
            }),
            py::arg("outer"), py::arg("ids"), py::arg("n_ids"), py::arg("n_blocks"), py::arg("stride"), py::arg("page"),
-           py::arg("id_bytes") = 4, py::arg("sel") = 0, py::arg("n_stored") = 0)
+           py::arg("id_bytes") = 4, py::arg("sel") = 0, py::arg("n_stored") = 0, py::arg("row_width") = 0, py::arg("row_pitch") = 0)
+      .def_property_readonly("row_width", [](const PyBlocks& t) { return t.b.row_width; })
+      .def_property_readonly("row_pitch", [](const PyBlocks& t) { return t.b.row_pitch; })
       .def_property_readonly("outer", [](const PyBlocks& t) { return *t.outer; })
       .def_property_readonly("page", [](const PyBlocks& t) { return t.b.page; })
       .def_property_readonly("phase", [](const PyBlocks& t) { return t.b.phase; })
@@ -1435,24 +1454,31 @@ void bind_control(py::module_& m) {
          "widths[i]); every shard is read whole and verified, no byte outside the rows is written; returns (one ErrorCode "
          "per object, object sizes).")
       .def("batch_put_device_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
-                                        const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, uintptr_t stream) {
+                                        const std::vector<uint64_t>& page_bytes, const WorkerConfig& cfg, uintptr_t stream,
+                                        const py::object& rows) {
         const auto lists = to_page_lists(pages);
-        return ecs_to_py(nogil([&] { return c.batch_put_device_paged(keys, lists, page_bytes, cfg, reinterpret_cast<void*>(stream)); }));
+        const auto pr = to_page_rows(rows);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_paged(keys, lists, page_bytes, cfg, reinterpret_cast<void*>(stream), pr); }));
       }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
+         py::arg("rows") = py::none(),
          "Object i = the len(pages[i]) pages of page_bytes[i] bytes at the device addresses pages[i] (each a 1-D integer "
          "array-like: list, numpy array or CPU tensor), concatenated in order; stored as a put of the concatenation would "
-         "store it; a zero page address is INVALID_ARGUMENT for that object; returns one ErrorCode per object.")
+         "store it; a zero page address is INVALID_ARGUMENT for that object; rows[i] = (row_width, row_pitch) makes each page "
+         "of object i rows of row_width bytes every row_pitch bytes (a head slice of each block; None: one row); returns "
+         "one ErrorCode per object.")
       .def("batch_get_device_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
-                                        const std::vector<uint64_t>& page_bytes, uintptr_t stream) {
+                                        const std::vector<uint64_t>& page_bytes, uintptr_t stream, const py::object& rows) {
         const auto lists = to_page_lists(pages);
+        const auto pr = to_page_rows(rows);
         std::vector<size_t> sizes;
-        const auto ecs = nogil([&] { return c.batch_get_device_paged(keys, lists, page_bytes, reinterpret_cast<void*>(stream), &sizes); });
+        const auto ecs = nogil([&] { return c.batch_get_device_paged(keys, lists, page_bytes, reinterpret_cast<void*>(stream), &sizes, pr); });
         return py::make_tuple(ecs_to_py(ecs), sizes);
-      }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("stream") = 0,
+      }, py::arg("keys"), py::arg("pages"), py::arg("page_bytes"), py::arg("stream") = 0, py::arg("rows") = py::none(),
          "Object i into the pages pages[i] of page_bytes[i] bytes, byte x in page x // page_bytes[i] (capacity len(pages[i]) "
          "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; a page address "
          "of 0 is not stored (a partial restore: the table still covers the whole object); pages of one get must not "
-         "overlap (not checked); returns (one ErrorCode per object, object sizes).")
+         "overlap (not checked); rows as batch_put_device_paged's, and then no byte outside the rows is written; returns "
+         "(one ErrorCode per object, object sizes).")
       .def("batch_put_device_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
                                          const WorkerConfig& cfg, uintptr_t stream) {
         std::vector<SourceBlocks> bs;
@@ -1491,23 +1517,29 @@ void bind_control(py::module_& m) {
          "`wide`; with a selection only the selected stored blocks land); returns one ErrorCode per object.")
       .def("batch_put_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
                                             const std::vector<uint64_t>& page_elems, const WorkerConfig& cfg, uintptr_t stream,
-                                            mxfp8::Wide wide) {
+                                            mxfp8::Wide wide, const py::object& rows) {
         const auto lists = to_page_lists(pages);
-        return ecs_to_py(nogil([&] { return c.batch_put_device_fp8_paged(keys, lists, page_elems, cfg, reinterpret_cast<void*>(stream), wide); }));
+        const auto pr = to_page_rows(rows);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_fp8_paged(keys, lists, page_elems, cfg, reinterpret_cast<void*>(stream), wide, pr); }));
       }, py::arg("keys"), py::arg("pages"), py::arg("page_elems"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
-         py::arg("wide") = mxfp8::Wide::BF16,
+         py::arg("wide") = mxfp8::Wide::BF16, py::arg("rows") = py::none(),
          "Packed tensor i = the len(pages[i]) pages of page_elems[i] elements of type `wide` at the device addresses pages[i] "
          "(each a 1-D integer array-like), concatenated in order; packed in the put kernel and stored as "
          "batch_put_device_fp8 of the concatenation would store it; a zero page address is INVALID_ARGUMENT for that "
-         "object; returns one ErrorCode per object (NOT_IMPLEMENTED: gather the pages and put that).")
+         "object; rows as batch_put_device_paged's, in elements; returns one ErrorCode per object (NOT_IMPLEMENTED: gather "
+         "the pages and put that).")
       .def("batch_get_device_fp8_paged", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& pages,
-                                            const std::vector<uint64_t>& page_elems, uintptr_t stream, mxfp8::Wide wide) {
+                                            const std::vector<uint64_t>& page_elems, uintptr_t stream, mxfp8::Wide wide,
+                                            const py::object& rows) {
         const auto lists = to_page_lists(pages);
-        return ecs_to_py(nogil([&] { return c.batch_get_device_fp8_paged(keys, lists, page_elems, reinterpret_cast<void*>(stream), wide); }));
+        const auto pr = to_page_rows(rows);
+        return ecs_to_py(nogil([&] { return c.batch_get_device_fp8_paged(keys, lists, page_elems, reinterpret_cast<void*>(stream), wide, pr); }));
       }, py::arg("keys"), py::arg("pages"), py::arg("page_elems"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         py::arg("rows") = py::none(),
          "Packed tensor i, which must hold len(pages[i]) * page_elems[i] elements, unpacked to type `wide` into the pages "
          "pages[i] of page_elems[i] elements, element x in page x // page_elems[i]; the whole packed object is read and "
-         "verified, only its elements are written; a page address of 0 is not stored (a partial restore); returns one "
+         "verified, only its elements are written; a page address of 0 is not stored (a partial restore); rows as "
+         "batch_put_device_fp8_paged's; returns one "
          "ErrorCode per object (NOT_IMPLEMENTED: get it whole and copy).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)

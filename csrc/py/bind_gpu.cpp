@@ -66,9 +66,10 @@ int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vect
       *out = DeviceLayout(t[slots[k]].cast<PyBlocks>().b);  // the outer array lives in the Python object until the call returns
     } else {
       auto p = py::cast<py::tuple>(t[slots[k]]);
-      if (p.size() != 3) throw py::value_error("pages = (addrs, page, phase)");
+      if (p.size() != 3 && p.size() != 5) throw py::value_error("pages = (addrs, page, phase[, row_width, row_pitch])");
       keep.push_back(p[0].cast<std::vector<uint64_t>>());
-      *out = DeviceLayout(SourcePages{keep.back().data(), keep.back().size(), p[1].cast<uint64_t>(), p[2].cast<uint64_t>()});
+      *out = DeviceLayout(SourcePages{keep.back().data(), keep.back().size(), p[1].cast<uint64_t>(), p[2].cast<uint64_t>(),
+                                      p.size() == 5 ? p[3].cast<uint64_t>() : 0, p.size() == 5 ? p[4].cast<uint64_t>() : 0});
     }
   }
   return set;
@@ -77,8 +78,8 @@ int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vect
 // source pages=None, destination pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
 // it without that flag).  A window sets XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern
 // (pitch, width, phase) sets XFER_GATHER, with src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.  Source
-// pages (addrs, page, phase) set XFER_GATHER | XFER_PAGED, destination pages XFER_SCATTER | XFER_PAGED.  At most one of
-// the four.
+// pages (addrs, page, phase[, row_width, row_pitch]) set XFER_GATHER | XFER_PAGED, destination pages
+// XFER_SCATTER | XFER_PAGED (with an in-page row pattern also XFER_PAGE_ROWS).  At most one of the four.
 XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   py::tuple t = py::cast<py::tuple>(h);
   if (t.size() < 3 || t.size() > 13)
@@ -118,6 +119,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_GATHER") = static_cast<uint32_t>(XFER_GATHER);
   m.attr("XFER_SCATTER") = static_cast<uint32_t>(XFER_SCATTER);
   m.attr("XFER_PAGED") = static_cast<uint32_t>(XFER_PAGED);
+  m.attr("XFER_PAGE_ROWS") = static_cast<uint32_t>(XFER_PAGE_ROWS);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -159,7 +161,8 @@ void bind_gpu(py::module_& m) {
            "phase) // width) * pitch + (x + phase) % width.  Source pages (addrs, page, phase) as the tenth element set "
            "XFER_GATHER | XFER_PAGED: object byte x is read from addrs[(x + phase) // page] + (x + phase) % page (src is "
            "not read); destination pages as the eleventh set XFER_SCATTER | XFER_PAGED and store by the same rule (dst is "
-           "not read); source blocks (a DeviceBlocks, ids on the device) as the twelfth and destination blocks as the "
+           "not read); pages (addrs, page, phase, row_width, row_pitch) are in-page rows (SourcePages), c = (x + phase) % "
+           "page at addrs[...] + (c // row_width) * row_pitch + c % row_width; source blocks (a DeviceBlocks, ids on the device) as the twelfth and destination blocks as the "
            "thirteenth do the same with a page table the resolve kernel builds on the stream; returns (digests, status, "
            "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item (VALUE_OUT_OF_RANGE or "
            "INVALID_ARGUMENT for refused ids).")
