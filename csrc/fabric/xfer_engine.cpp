@@ -2,6 +2,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cstdlib>
@@ -461,12 +462,14 @@ ErrorCode XferEngine::write_pages(Slot* s, uint32_t nd, size_t* tab) {
   for (uint32_t k : s->blocks_descs) s->strides[k].pages = d_reserved + s->strides[k].pages * sizeof(uint64_t);
   s->write_strides(nd);
   std::memcpy(s->h_tab + off, s->pages.data(), s->pages.size() * sizeof(uint64_t));
+  // read_verdicts() reads the word of every descriptor of a batch with jobs: a descriptor without one must not report
+  // the verdict a refused BLOCKS item left at its index in an earlier batch of this slot
   auto* verdicts = reinterpret_cast<uint32_t*>(s->h_res + static_cast<size_t>(max_items_) * 12);
+  if (!s->jobs.empty()) std::fill(verdicts, verdicts + nd, kBlocksOk);
   for (BlocksJob& j : s->jobs) {
     j.entries = reinterpret_cast<uint64_t*>(d_reserved + reinterpret_cast<uintptr_t>(j.entries) * sizeof(uint64_t));
     j.outer = reinterpret_cast<const uint64_t*>(d_pages + reinterpret_cast<uintptr_t>(j.outer) * sizeof(uint64_t));
     j.verdict = verdicts + reinterpret_cast<uintptr_t>(j.verdict);
-    *j.verdict = kBlocksOk;
   }
   std::memcpy(s->h_tab + jobs_offset(s, nd), s->jobs.data(), s->jobs.size() * sizeof(BlocksJob));
   *tab = filled;
