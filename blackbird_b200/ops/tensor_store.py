@@ -894,13 +894,26 @@ class TensorStore:
                 raise IndexError(f"{k}: rows [{a}, {b}) outside [0, {m['shape'][0]}]")
         return self._get_windows(keys, metas, [0] * len(keys), starts, stops, device)
 
+    @staticmethod
+    def _windows(metas: list, dims: list, starts: list, stops: list) -> list:
+        """(offset, width, pitch, rows) of `t.narrow(dims[i], starts[i], stops[i] - starts[i])` of each stored tensor:
+        `rows` = prod(shape[:dim]) runs of `width` units every `pitch` units from unit `offset`, the units elements for
+        packed tensors, else bytes."""
+        win = []
+        for m, d, a, b in zip(metas, dims, starts, stops):
+            shape = m["shape"]
+            inner = torch.Size(shape[d + 1:]).numel()
+            es = 1 if m["packed"] else _stored_dtype(m).itemsize
+            win.append((a * inner * es, (b - a) * inner * es, shape[d] * inner * es, torch.Size(shape[:d]).numel()))
+        return win
+
     def _get_windows(self, keys: list, metas: list, dims: list, starts: list, stops: list, device: torch.device) -> list:
         """`t.narrow(dims[i], starts[i], stops[i] - starts[i])` of each stored tensor, as new contiguous tensors.  The
         window is `rows` = prod(shape[:dim]) runs of `width` elements every `pitch` from element `offset`; the packed calls
         count elements, the others bytes.  Along dim 0 (one run) the range calls read it, along other dims the strided
         calls, one call per kind for all such items (packed: per dtype).  Packed items the fused kernel refuses are read
         whole and narrowed."""
-        result, win = [None] * len(keys), [None] * len(keys)
+        result, win = [None] * len(keys), self._windows(metas, dims, starts, stops)
         for i, (m, d, a, b) in enumerate(zip(metas, dims, starts, stops)):
             shape, dt = m["shape"], _stored_dtype(m)
             inner = torch.Size(shape[d + 1:]).numel()
@@ -910,8 +923,6 @@ class TensorStore:
             # kernel whenever its row gap allows.
             skew = offset % (16 // dt.itemsize) if m["packed"] or d else 0
             result[i] = torch.empty(rows * width + skew, dtype=dt, device=device)[skew:].view(shape[:d] + [b - a] + shape[d + 1:])
-            es = 1 if m["packed"] else dt.itemsize
-            win[i] = (offset * es, width * es, shape[d] * inner * es, rows)
 
         def narrowed(i, t):
             result[i] = t.narrow(dims[i], starts[i], stops[i] - starts[i]).clone(memory_format=torch.contiguous_format)
@@ -966,6 +977,16 @@ class TensorStore:
         if not len(keys) == len(dims) == len(starts) == len(stops):
             raise ValueError("keys, dims, starts and stops differ in length")
         metas = self._metas(keys)
+        self._slice_checks(keys, metas, dims, starts, stops)
+        return self._get_windows(keys, metas, dims, starts, stops, device)
+
+    def get_slice(self, key: str, dim: int, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
+        """`t.narrow(dim, start, stop - start).contiguous()` of the tensor stored under `key` (see batch_get_slices)."""
+        return self.batch_get_slices([key], [dim], [start], [stop], device)[0]
+
+    def _slice_checks(self, keys: list, metas: list, dims: list, starts: list, stops: list) -> None:
+        """IndexError for a 0-d tensor, a dim out of range or bounds outside 0 <= start <= stop <= shape[dim]; dims are
+        normalised in place (negative dims count from the end)."""
         for j, (k, m, a, b) in enumerate(zip(keys, metas, starts, stops)):
             shape = m["shape"]
             if not shape:
@@ -975,11 +996,98 @@ class TensorStore:
             dims[j] %= len(shape)
             if not 0 <= a <= b <= shape[dims[j]]:
                 raise IndexError(f"{k}: [{a}, {b}) outside [0, {shape[dims[j]]}] along dim {dims[j]}")
-        return self._get_windows(keys, metas, dims, starts, stops, device)
 
-    def get_slice(self, key: str, dim: int, start: int, stop: int, device: Optional[torch.device] = None) -> torch.Tensor:
-        """`t.narrow(dim, start, stop - start).contiguous()` of the tensor stored under `key` (see batch_get_slices)."""
-        return self.batch_get_slices([key], [dim], [start], [stop], device)[0]
+    def batch_get_slices_into(self, keys: Sequence[str], outs: Sequence[torch.Tensor], dims: Sequence[int], starts: Sequence[int],
+                              stops: Sequence[int]) -> list:
+        """Loads `t.narrow(dim, start, stop - start)` of each stored tensor into an existing CUDA tensor and returns `outs`:
+        a tensor-parallel rank loads its shard of a stored weight into its place in a fused parameter
+        (`W_fused[:, a:b]`), a reader restores heads `kv[:, h0:h1, :]` of a stored layer into the same heads of a live
+        buffer, a job refreshes a slice of a model buffer in place.  No slice-sized temporary is made on the fused routes,
+        and no element of an out's storage outside the view is written.  The outs must not overlap one another (not
+        checked).
+
+        Every check comes before any transfer: KeyError for a missing key; IndexError for a 0-d tensor, a dim out of
+        range or bounds outside 0 <= start <= stop <= shape[dim] (negative dims count from the end); TypeError unless
+        out.dtype is the stored dtype; ValueError unless out.shape is the narrowed shape and out is a CUDA tensor on the
+        current device.  Then each route is one call for all the slices that take it (packed: one per dtype):
+          1. a contiguous out: the range get (dim 0) or the strided get of batch_get_slices, at out's pointer;
+          2. an out whose elements are rows (see _source_rows: `narrow` along any dim, `t[::k]`):
+             batch_get_device_strided_scatter (packed: batch_get_device_fp8_strided_scatter), whose kernel stores the
+             slice's pieces straight into the rows;
+          3. everything else -- transposed or overlapping outs, and packed slices the fused kernels refuse
+             (NOT_IMPLEMENTED: misaligned rows, unfusable placements) -- batch_get_slices into a temporary, then
+             out.copy_().  Unpacked slices the fused kernels cannot store are staged through the host by the client."""
+        keys, outs, dims, starts, stops = list(keys), list(outs), list(dims), list(starts), list(stops)
+        if not len(keys) == len(outs) == len(dims) == len(starts) == len(stops):
+            raise ValueError("keys, outs, dims, starts and stops differ in length")
+        metas = self._metas(keys)
+        self._slice_checks(keys, metas, dims, starts, stops)
+        for k, m, o, d, a, b in zip(keys, metas, outs, dims, starts, stops):
+            want = _stored_dtype(m)
+            if o.dtype != want:
+                raise TypeError(f"{k}: out is {o.dtype}, the stored tensor {want}")
+            shape = m["shape"][:d] + [b - a] + m["shape"][d + 1:]
+            if list(o.shape) != shape:
+                raise ValueError(f"{k}: out has shape {list(o.shape)}, the slice {shape}")
+            if not o.is_cuda or o.device.index != torch.cuda.current_device():
+                raise ValueError(f"{k}: out must be a CUDA tensor on the current device, not {o.device}")
+        win = self._windows(metas, dims, starts, stops)
+        rows = [None if o.is_contiguous() else self._source_rows(o) for o in outs]
+        n = len(keys)
+        rest = [i for i in range(n) if not outs[i].is_contiguous() and rows[i] is None]  # route 3
+        for along0 in (True, False):  # route 1: (offset, width) or (offset, width, pitch, rows) at out's pointer
+            idx = [i for i in range(n) if outs[i].is_contiguous() and (dims[i] == 0) == along0]
+            k = 2 if along0 else 4
+            fp8_call, call, what = ((self.client.batch_get_device_fp8_range, self.client.batch_get_device_range, "range get") if along0 else
+                                    (self.client.batch_get_device_fp8_strided, self.client.batch_get_device_strided, "strided get"))
+
+            def fp8(grp, es, wide):
+                return fp8_call([keys[i] for i in grp], [outs[i].data_ptr() for i in grp], [metas[i]["padded_numel"] for i in grp],
+                                *[[win[i][j] for i in grp] for j in range(k)], self._stream(), wide=wide)
+
+            rest += self._packed(f"fused fp8 {what}", keys, [i for i in idx if metas[i]["packed"]], lambda i: outs[i].dtype, fp8)
+            plain = [i for i in idx if not metas[i]["packed"]]
+            if plain:
+                ecs = call([keys[i] for i in plain], [outs[i].data_ptr() for i in plain], *[[win[i][j] for i in plain] for j in range(k)],
+                           self._stream())
+                _check(what, [keys[i] for i in plain], ecs)
+        idx = [i for i in range(n) if not outs[i].is_contiguous() and rows[i] is not None]  # route 2
+
+        def dst_rows(grp, es):
+            return [rows[i][0] // es for i in grp], [rows[i][1] // es for i in grp]
+
+        def fp8_rows(grp, es, wide):
+            return self.client.batch_get_device_fp8_strided_scatter(
+                [keys[i] for i in grp], [outs[i].data_ptr() for i in grp], [metas[i]["padded_numel"] for i in grp],
+                *[[win[i][j] for i in grp] for j in range(4)], *dst_rows(grp, es), self._stream(), wide=wide)
+
+        rest += self._packed("fused fp8 slice get", keys, [i for i in idx if metas[i]["packed"]], lambda i: outs[i].dtype, fp8_rows)
+        plain = [i for i in idx if not metas[i]["packed"]]
+        if plain:
+            ecs = self.client.batch_get_device_strided_scatter([keys[i] for i in plain], [outs[i].data_ptr() for i in plain],
+                                                               *[[win[i][j] for i in plain] for j in range(4)], *dst_rows(plain, 1),
+                                                               self._stream())
+            _check("slice get", [keys[i] for i in plain], ecs)
+        if rest:
+            got = self._get_windows([keys[i] for i in rest], [metas[i] for i in rest], [dims[i] for i in rest], [starts[i] for i in rest],
+                                    [stops[i] for i in rest], outs[rest[0]].device)
+            for i, t in zip(rest, got):
+                outs[i].copy_(t)
+        return outs
+
+    def get_slice_into(self, key: str, out: torch.Tensor, dim: int, start: int, stop: int) -> torch.Tensor:
+        """Loads `t.narrow(dim, start, stop - start)` of the tensor stored under `key` into `out` and returns it (see
+        batch_get_slices_into)."""
+        return self.batch_get_slices_into([key], [out], [dim], [start], [stop])[0]
+
+    def batch_get_rows_into(self, keys: Sequence[str], outs: Sequence[torch.Tensor], starts: Sequence[int], stops: Sequence[int]) -> list:
+        """Rows [start, stop) along dim 0 of each stored tensor into existing tensors: batch_get_slices_into with dim 0."""
+        keys = list(keys)
+        return self.batch_get_slices_into(keys, outs, [0] * len(keys), starts, stops)
+
+    def get_rows_into(self, key: str, out: torch.Tensor, start: int, stop: int) -> torch.Tensor:
+        """`t[start:stop]` of the tensor stored under `key` into `out` (see batch_get_slices_into)."""
+        return self.batch_get_slices_into([key], [out], [0], [start], [stop])[0]
 
     def remove(self, keys: Sequence[str]) -> None:
         self.client.batch_remove(list(keys) + [k + "#meta" for k in keys])
@@ -1044,6 +1152,13 @@ class AsyncTensorStore(TensorStore):
         reads or writes of the outs."""
         outs = list(outs)
         return self._on_side(True, self.batch_get_into, list(keys), outs, result=outs)
+
+    def get_slices_into_async(self, keys: Sequence[str], outs: Sequence[torch.Tensor], dims: Sequence[int], starts: Sequence[int],
+                              stops: Sequence[int]):
+        """batch_get_slices_into on the side stream, ordered after the work already queued on the caller's stream; the
+        future yields `outs`, already synchronised with the side stream, or raises the call's error."""
+        outs = list(outs)
+        return self._on_side(True, self.batch_get_slices_into, list(keys), outs, list(dims), list(starts), list(stops), result=outs)
 
     def put_blocks_async(self, keys: Sequence[str], caches: Sequence[torch.Tensor], ids: Sequence, dim: int = 0, pack_fp8: bool = False,
                          config=None):

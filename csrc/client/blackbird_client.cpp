@@ -911,6 +911,47 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided(const std::
       [&](const std::vector<size_t>&) { return get_device_fp8(keys, bf16_ptrs, n_elems, &ranges, nullptr, stream, wide); });
 }
 
+// The destination of a slice get's result of `units` units: rows of dst_width units every dst_pitch units, as many as the
+// result fills (the last one possibly in part), with SourceRows::from_rows' errors; INVALID_ARGUMENT for a zero width with
+// a result.
+static ErrorCode result_rows(uint64_t units, uint64_t dst_width, uint64_t dst_pitch, DeviceLayout* out) {
+  *out = {};
+  if (units == 0) return ErrorCode::OK;
+  if (dst_width == 0) return ErrorCode::INVALID_ARGUMENT;
+  SourceRows r;
+  uint64_t size = 0, extent = 0;
+  const ErrorCode ec = SourceRows::from_rows(dst_width, dst_pitch, (units - 1) / dst_width + 1, &r, &size, &extent);
+  *out = DeviceLayout::window_rows(r);
+  return ec;
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_strided_scatter(
+    const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs, const std::vector<uint64_t>& n_elems,
+    const std::vector<uint64_t>& elem_offsets, const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
+    const std::vector<uint64_t>& rows, const std::vector<uint64_t>& dst_widths, const std::vector<uint64_t>& dst_pitches, void* stream,
+    mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  const uint64_t b = mxfp8::wide_bytes(wide);
+  std::vector<ByteRange> ranges(n);
+  std::vector<DeviceLayout> mem(n);
+  return shaped_batch(
+      "device_get_fp8_strided_scatter", false, n,
+      bf16_ptrs.size() == n && n_elems.size() == n && elem_offsets.size() == n && elem_widths.size() == n && elem_pitches.size() == n &&
+          rows.size() == n && dst_widths.size() == n && dst_pitches.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {elem_offsets[i], elem_widths[i], elem_pitches[i], rows[i]};
+        uint64_t total = 0;
+        if (__builtin_mul_overflow(rows[i], elem_widths[i], &total)) return ErrorCode::VALUE_OUT_OF_RANGE;
+        *bytes = b * total;  // counted for OK items only, whose rows lie inside the object
+        return result_rows(total, dst_widths[i], dst_pitches[i], &mem[i]);
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto rr = pick(ranges, idx);
+        const auto rm = pick(mem, idx);
+        return get_device_fp8(pick(keys, idx), pick(bf16_ptrs, idx), pick(n_elems, idx), &rr, &rm, stream, wide);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_paged(const std::vector<ObjectKey>& keys, const std::vector<std::vector<uint64_t>>& pages,
                                                                    const std::vector<uint64_t>& page_elems, void* stream, mxfp8::Wide wide,
                                                                    const std::vector<PageRows>& page_rows) {
@@ -944,7 +985,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (bf16_ptrs.size() != keys.size() || n_elems.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (mem && (ranges || mem->size() != keys.size())))
+      (mem && mem->size() != keys.size()))
     return out;
   auto mem_of = [&](size_t i) { return mem ? (*mem)[i] : DeviceLayout{}; };
   BB_TRACE_SPAN("batch_get_device_fp8", keys.size());
@@ -968,7 +1009,9 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
         out[i] = ec;
         continue;
       }
-      bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - b * w.base_shift(w.lo));
+      // rows of the result (WINDOW_ROWS) start at the caller's pointer
+      if (mem_of(i).kind() != DeviceLayout::WINDOW_ROWS)
+        bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(bf16_ptrs[i]) - b * w.base_shift(w.lo));
     }
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
@@ -1478,6 +1521,34 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided(const std::vect
       [&](const std::vector<size_t>&) { return get_device(keys, dev_ptrs, lens, &ranges, nullptr, stream, nullptr); });
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_strided_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                                         const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                                                         const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows,
+                                                                         const std::vector<uint64_t>& dst_widths,
+                                                                         const std::vector<uint64_t>& dst_pitches, void* stream) {
+  const size_t n = keys.size();
+  std::vector<ByteRange> ranges(n);
+  std::vector<DeviceLayout> mem(n);
+  std::vector<size_t> lens(n);
+  return shaped_batch(
+      "device_get_strided_scatter", false, n,
+      dev_ptrs.size() == n && offsets.size() == n && widths.size() == n && pitches.size() == n && rows.size() == n &&
+          dst_widths.size() == n && dst_pitches.size() == n,
+      [&](size_t i, uint64_t* bytes) {
+        ranges[i] = {offsets[i], widths[i], pitches[i], rows[i]};
+        uint64_t total = 0;
+        if (__builtin_mul_overflow(rows[i], widths[i], &total) || total > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
+        lens[i] = static_cast<size_t>(total);
+        *bytes = total;
+        return result_rows(total, dst_widths[i], dst_pitches[i], &mem[i]);
+      },
+      [&](const std::vector<size_t>& idx) {
+        const auto rr = pick(ranges, idx);
+        const auto rm = pick(mem, idx);
+        return get_device(pick(keys, idx), pick(dev_ptrs, idx), pick(lens, idx), &rr, &rm, stream, nullptr);
+      });
+}
+
 std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                    const std::vector<size_t>& capacity, const std::vector<ByteRange>* ranges,
                                                    const std::vector<DeviceLayout>* mem, void* stream, std::vector<size_t>* out_sizes) {
@@ -1485,7 +1556,7 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
   if (!keystone_) return std::vector<ErrorCode>(keys.size(), ErrorCode::CLIENT_DISCONNECTED);
   if (!device_) return std::vector<ErrorCode>(keys.size(), ErrorCode::NOT_IMPLEMENTED);
   if (dev_ptrs.size() != keys.size() || capacity.size() != keys.size() || (ranges && ranges->size() != keys.size()) ||
-      (mem && (ranges || mem->size() != keys.size())))
+      (mem && mem->size() != keys.size()))
     return out;
   auto mem_of = [&](size_t i) { return mem ? (*mem)[i] : DeviceLayout{}; };
   const TimePoint t_all = Clock::now();
@@ -1518,8 +1589,12 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           op.copy = copy_choice[i] % copies.size();
           op.shard = s;
           op.placement = &copy.shards[s];
+          const DeviceLayout m = mem_of(i);
           if (!whole) op.win = sp.rebase(off, len);
-          op.mem = mem_of(i).rebase(off, &op.mem_at);
+          if (m.kind() == DeviceLayout::WINDOW_ROWS)  // the rows move on with the shard's first stored unit
+            op.mem = DeviceLayout::window_rows(WindowRows{sp, m.rows()}.rebase(off, len, &op.mem_at).rows);
+          else
+            op.mem = m.rebase(off, &op.mem_at);
           ops.push_back(std::move(op));
         }
         off += len;
@@ -1615,7 +1690,10 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
           out[i] = ec;
           continue;
         }
-        range_bases[i] = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.base_shift(sp.lo));
+        // rows of the result (WINDOW_ROWS) start at the caller's pointer
+        range_bases[i] = mem_of(i).kind() == DeviceLayout::WINDOW_ROWS
+                             ? dev_ptrs[i]
+                             : reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(dev_ptrs[i]) - sp.base_shift(sp.lo));
       } else if (size > capacity[i]) {
         out[i] = ErrorCode::BUFFER_OVERFLOW;
         continue;
@@ -1671,12 +1749,14 @@ std::vector<ErrorCode> BlackbirdClient::get_device(const std::vector<ObjectKey>&
         std::vector<uint8_t> stage(size);
         // data servers + CPU checksum + replica fail-over, over the shards the get reads
         ErrorCode ec = transfer_get(copies, stage.data(), size, sp);
-        if (ec == ErrorCode::OK && sp.strided()) {  // compact the rows on the host: one H2D copy of rows * width bytes
+        // compact the rows on the host: one H2D copy of rows * width bytes, into the result's rows for WINDOW_ROWS
+        if (ec == ErrorCode::OK && sp.strided()) {
           std::vector<uint8_t> dense(capacity[i]);
           sp.for_each_run(size, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dense.data() + at, stage.data() + x, n); });
-          ec = device_->copy_to_device(dev_ptrs[i], DeviceLayout{}, dense.data(), dense.size(), stream);
+          ec = device_->copy_to_device(dev_ptrs[i], m.kind() == DeviceLayout::WINDOW_ROWS ? m.as_rows() : DeviceLayout{}, dense.data(),
+                                       dense.size(), stream);
         } else if (ec == ErrorCode::OK) {  // the range, or the whole object into its layout
-          ec = device_->copy_to_device(dev_ptrs[i], m, stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
+          ec = device_->copy_to_device(dev_ptrs[i], m.as_rows(), stage.data() + sp.lo, std::min<uint64_t>(sp.hi, size) - sp.lo, stream);
         }
         out[i] = ec;
         metrics_.inc("device_get_host_staged_total");
@@ -1811,12 +1891,21 @@ Result<uint64_t> HostLoopbackTransport::submit_get(const std::vector<DeviceShard
     const DeviceShardOp& op = ops[k];
     ErrorCode ec;
     auto* dst = static_cast<uint8_t*>(op.dst(dev_ptrs[op.item]));
-    if (!op.mem.contiguous()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows or pages
-      if (!op.mem.valid(op.placement->length) || !op.win.whole()) return ErrorCode::INVALID_ARGUMENT;
+    const uint64_t len = op.placement->length;
+    if (op.mem.kind() == DeviceLayout::WINDOW_ROWS && !op.win.covers(len)) {
+      // as the kernel's windowed scattering store: the whole shard read and verified, the window's units stored into the
+      // rows of its result
+      const WindowRows wr{op.win, op.mem.rows()};
+      if (!wr.valid(len)) return ErrorCode::INVALID_ARGUMENT;
+      std::vector<uint8_t> whole(len);
+      ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
+      if (ec == ErrorCode::OK) wr.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + at, whole.data() + x, n); });
+    } else if (!op.mem.contiguous()) {  // as the kernel's scattering store: the whole shard, read and verified, stored into its rows or pages
+      if (!op.mem.valid(op.placement->length) || (!op.win.whole() && op.mem.kind() != DeviceLayout::WINDOW_ROWS)) return ErrorCode::INVALID_ARGUMENT;
       if (op.mem.kind() == DeviceLayout::BLOCKS && !op.mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // as the engine
       if (op.mem.kind() == DeviceLayout::BLOCKS && !op.mem.coaligned(0, op.placement->length)) return ErrorCode::INVALID_ADDRESS;
       std::vector<uint64_t> table;  // blocks: as the resolve kernel, a refused table is all null pages
-      const DeviceLayout m = op.mem.resolved(op.placement->length, true, &table, &verdicts[k]);
+      const DeviceLayout m = op.mem.as_rows().resolved(op.placement->length, true, &table, &verdicts[k]);
       std::vector<uint8_t> whole(op.placement->length);
       ec = io_->read_shard(*op.placement, whole.data(), op.placement->checksum_algo);
       if (ec == ErrorCode::OK) copy_to_device(dst, m, whole.data(), whole.size(), nullptr);
@@ -1876,9 +1965,21 @@ ErrorCode HostLoopbackTransport::run_fp8(const std::vector<DeviceFp8Op>& ops, bo
       continue;
     }
     if (!op.win.over(op.n_elems).valid(op.n_elems)) return ErrorCode::INVALID_ARGUMENT;  // as the engine
+    // as the engine: rows of the window's result (WindowRows), co-aligned in wide bytes, unless the window stores the
+    // whole object in place, where they are the object's own rows
+    const bool wrows = op.mem.kind() == DeviceLayout::WINDOW_ROWS && !op.win.covers(op.n_elems);
+    const WindowRows wr{op.win.over(op.n_elems), op.mem.rows()};
+    if (wrows) {
+      WindowRows wb;
+      if (!op.mem.rows().valid() || !wr.to_wide_bytes(eb, &wb)) return ErrorCode::INVALID_ARGUMENT;
+      if (!wb.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
+    }
+    const DeviceLayout lay = wrows ? DeviceLayout{} : op.mem.as_rows();
     DeviceLayout b;
-    if (!op.mem.contiguous()) {  // as the engine: destination rows or pages, never with a window, co-aligned in wide bytes
-      if (!op.win.whole() || !op.mem.valid(op.n_elems) || !op.mem.to_wide_bytes(eb, &b)) return ErrorCode::INVALID_ARGUMENT;
+    if (!lay.contiguous()) {  // as the engine: destination rows or pages, never with a window, co-aligned in wide bytes
+      // with rows of a window's result, the window stores the whole object in place (wrows is false)
+      if ((!op.win.whole() && op.mem.kind() != DeviceLayout::WINDOW_ROWS) || !lay.valid(op.n_elems) || !lay.to_wide_bytes(eb, &b))
+        return ErrorCode::INVALID_ARGUMENT;
       if (!b.coaligned(reinterpret_cast<uintptr_t>(op.wide), eb * op.n_elems)) return ErrorCode::INVALID_ADDRESS;
       if (b.kind() == DeviceLayout::BLOCKS && !b.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;  // as the engine
     }
@@ -1892,14 +1993,18 @@ ErrorCode HostLoopbackTransport::run_fp8(const std::vector<DeviceFp8Op>& ops, bo
     }
     if (ec != ErrorCode::OK) return ec;
     auto* dst = static_cast<uint8_t*>(op.wide);
-    if (op.win.whole() && op.mem.contiguous()) {
+    if (op.win.whole() && lay.contiguous()) {
       mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, dst);
       continue;
     }
     std::vector<uint8_t> wide(eb * op.n_elems);
     mxfp8::unpack(packed.data(), op.n_elems, op.wide_type, wide.data());
-    if (!op.mem.contiguous()) {  // as the kernel's scattering store: the unpacked object into its rows or pages
+    if (!lay.contiguous()) {  // as the kernel's scattering store: the unpacked object into its rows or pages
       copy_to_device(dst, b, wide.data(), wide.size(), nullptr);
+      continue;
+    }
+    if (wrows) {  // as the kernel's windowed scattering store: the window's elements into the rows of its result
+      wr.for_each_run(op.n_elems, [&](uint64_t x, uint64_t at, uint64_t n) { std::memcpy(dst + eb * at, wide.data() + eb * x, eb * n); });
       continue;
     }
     // as the kernel does: the whole object read and verified, only the window stored

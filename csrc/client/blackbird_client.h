@@ -66,13 +66,15 @@ struct DeviceShardOp {
   StoreWindow win;
   // Where the shard's bytes sit in the caller's memory (common/store_window.h): a put's source or a get's destination,
   // the object's layout rebased to the shard's first byte, with its base mem_at bytes from dev_ptrs[item].  Never
-  // together with a window unless contiguous.
+  // together with a window unless contiguous or WINDOW_ROWS (the rows of the window's result, WindowRows::rebase).
   DeviceLayout mem;
   uint64_t mem_at = 0;
   // The base of `mem` given the object's; a get's also the base `win` goes with (a strided window's base is where the
-  // result's row 0 lands, which does not move with the shard).
+  // result's row 0 lands, which does not move with the shard, unless the result lands in rows).
   const void* src(const void* obj_base) const { return static_cast<const uint8_t*>(obj_base) + mem_at; }
-  void* dst(void* obj_base) const { return static_cast<uint8_t*>(obj_base) + win.base_shift(mem_at); }
+  void* dst(void* obj_base) const {
+    return static_cast<uint8_t*>(obj_base) + (mem.kind() == DeviceLayout::WINDOW_ROWS ? mem_at : win.base_shift(mem_at));
+  }
 };
 
 // One object of a fused MXFP8 transfer: the whole packed object ([E4M3 payload][E8M0 scales]) is a single shard.
@@ -221,6 +223,24 @@ class BlackbirdClient {
   // unless bf16_ptrs[i] is 16-byte aligned and, for rows[i] > 1, (elem_pitches[i] - elem_widths[i]) % 8 == 0 -- there is
   // no host-staged path; the rest of the batch keeps the fused launch.  rows[i] == 1 or elem_widths[i] ==
   // elem_pitches[i] is batch_get_device_fp8.
+  // Strided or range gets of packed tensors into slices of tensors the caller owns (a TP rank's shard of a stored weight
+  // into its place in a fused parameter): the window of batch_get_device_fp8_strided (rows[i] rows of elem_widths[i]
+  // elements every elem_pitches[i] from elem_offsets[i]; a range is one row), whose dense result lands in rows of
+  // dst_widths[i] elements every dst_pitches[i] elements from bf16_ptrs[i] (WindowRows in common/store_window.h, in
+  // elements): result element p at bf16_ptrs[i] + 2 * ((p / dst_widths[i]) * dst_pitches[i] + p % dst_widths[i]).  The
+  // whole packed object is read and verified, only the window is unpacked into the rows, and no element outside them is
+  // ever written.  Per object, the window's errors as batch_get_device_fp8_strided; INVALID_ARGUMENT for dst_widths[i]
+  // == 0 with a non-empty result or dst_widths[i] > dst_pitches[i] when the result spans several rows; NOT_IMPLEMENTED
+  // when the object is not fusable or the item fails WindowRows::fused_get_aligned in wide bytes (the first stored
+  // element's destination congruent to twice its index mod 16, and (pitches - widths) % 8 == 0 for both patterns) --
+  // there is no host-staged path; the rest of the batch keeps the fused launch.  dst_widths[i] == dst_pitches[i] is
+  // batch_get_device_fp8_strided.
+  std::vector<ErrorCode> batch_get_device_fp8_strided_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
+                                                              const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_offsets,
+                                                              const std::vector<uint64_t>& elem_widths, const std::vector<uint64_t>& elem_pitches,
+                                                              const std::vector<uint64_t>& rows, const std::vector<uint64_t>& dst_widths,
+                                                              const std::vector<uint64_t>& dst_pitches, void* stream,
+                                                              mxfp8::Wide wide = mxfp8::Wide::BF16);
   std::vector<ErrorCode> batch_get_device_fp8_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                       const std::vector<uint64_t>& n_elems, const std::vector<uint64_t>& elem_widths,
                                                       const std::vector<uint64_t>& elem_pitches, const std::vector<uint64_t>& rows,
@@ -324,6 +344,23 @@ class BlackbirdClient {
   // batch keeps the fused launch.  Per object, the shaped calls' admission (shaped_get) of SourceRows::from_rows:
   // INVALID_ARGUMENT for widths[i] > pitches[i] with rows[i] > 1.  rows[i] == 1 or widths[i] == pitches[i] is exactly
   // batch_get_device with capacity rows[i] * widths[i].
+  // Strided or range gets into slices of tensors the caller owns (`out[:, h0:h1, :]`, a TP shard into a fused
+  // parameter): the window of batch_get_device_strided (rows[i] rows of widths[i] bytes every pitches[i] from
+  // offsets[i]; a range is one row), whose dense result lands in rows of dst_widths[i] bytes every dst_pitches[i] bytes
+  // from dev_ptrs[i] (WindowRows in common/store_window.h): result byte p at dev_ptrs[i] + (p / dst_widths[i]) *
+  // dst_pitches[i] + p % dst_widths[i].  Shards are read and verified as for batch_get_device_strided, with its
+  // fail-over and placement refresh, and no byte outside the destination rows is ever written.  The fused path stores
+  // the window's pieces in the get kernel; it needs WindowRows::fused_get_aligned for every shard of every copy (both
+  // gaps multiples of 16 bytes, each shard's first stored byte at an address congruent to its offset mod 16).  Any other
+  // item, and every placement the fabric cannot reach, is staged through the host (the window compacted there, one 2-D
+  // H2D copy into the rows).  Per object, the window's errors as batch_get_device_strided; INVALID_ARGUMENT for
+  // dst_widths[i] == 0 with a non-empty result or dst_widths[i] > dst_pitches[i] when the result spans several rows.
+  // dst_widths[i] == dst_pitches[i] is batch_get_device_strided.
+  std::vector<ErrorCode> batch_get_device_strided_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
+                                                          const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                                          const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows,
+                                                          const std::vector<uint64_t>& dst_widths, const std::vector<uint64_t>& dst_pitches,
+                                                          void* stream);
   std::vector<ErrorCode> batch_get_device_scatter(const std::vector<ObjectKey>& keys, const std::vector<void*>& dev_ptrs,
                                                   const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                                   const std::vector<uint64_t>& rows, void* stream, std::vector<size_t>* out_sizes);
@@ -401,8 +438,9 @@ class BlackbirdClient {
   ErrorCode transfer_get(const std::vector<CopyPlacement>& copies, uint8_t* dst, size_t size, const StoreWindow& win = {});
   // batch_get_device, batch_get_device_range, batch_get_device_strided, batch_get_device_scatter and
   // batch_get_device_paged: `ranges` null = whole objects into buffers of `capacity`, else object i's rows into dev_ptrs[i]
-  // (capacity[i] = rows * length, for the chunk plan).  A range is the single row `rows == 1`.  `mem` (whole objects
-  // only) null = contiguous buffers, else object i lands by (*mem)[i] at dev_ptrs[i].
+  // (capacity[i] = rows * length, for the chunk plan).  A range is the single row `rows == 1`.  `mem` null = contiguous
+  // buffers, else object i lands by (*mem)[i] at dev_ptrs[i]: with `ranges` only a WINDOW_ROWS layout (the rows of the
+  // range's result) or a contiguous one.
   struct ByteRange {
     uint64_t offset = 0, length = 0;
     uint64_t pitch = 0, rows = 1;  // row r = bytes [offset + r * pitch, + length)

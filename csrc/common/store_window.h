@@ -250,6 +250,126 @@ struct SourceRows {
   }
 };
 
+// WindowRows: a store window whose result lands in rows of a larger tensor the caller owns (a slice of a stored tensor
+// read into a slice of a live one).  The units `win` selects keep their dense result index p, the position the window's
+// own get gives them in a contiguous result:
+//   p = x - lo                                              contiguous window
+//   p = (row + (x + phase) / pitch) * width + (x + phase) % pitch   strided window
+// and unit p lands at
+//   dst + ((p + rows.phase) / rows.width) * rows.pitch + (p + rows.phase) % rows.width
+// which is SourceRows applied to the result.  Without a pattern in `rows` the result is contiguous at dst: the window's
+// own get.  This is the one statement of the rule; the transfer engine (XferItem, Fp8Item with a WINDOW_ROWS layout),
+// the fabric's ops, the client, the host loopback transport and the kernels' XFER_WINDOW_ROWS descriptors
+// (kernels/xfer.h) all follow it.  The unit is a byte, or for an MXFP8 get an element of the wide side until
+// to_wide_bytes().
+struct WindowRows {
+  StoreWindow win;
+  SourceRows rows;
+
+  // The INVALID_ARGUMENT rules against an object of n units: StoreWindow::valid and SourceRows::valid.
+  bool valid(uint64_t n) const { return win.valid(n) && rows.valid(); }
+
+  // The dense result index of stored unit x.
+  uint64_t index(uint64_t x) const {
+    if (!win.strided()) return x - win.lo;
+    const uint64_t y = x + win.phase;
+    return (static_cast<uint64_t>(win.row) + y / win.pitch) * win.width + y % win.pitch;
+  }
+  // Where result unit p lands relative to dst.
+  uint64_t at(uint64_t p) const {
+    if (!rows.strided()) return p;
+    const uint64_t q = p + rows.phase;
+    return q / rows.width * rows.pitch + q % rows.width;
+  }
+  // The first and the last stored unit of an object of n units; false when the window stores none.
+  bool stored_bounds(uint64_t n, uint64_t* first, uint64_t* last) const {
+    const uint64_t hi = std::min(win.hi, n);
+    if (win.lo >= hi) return false;
+    uint64_t a = win.lo, b = hi - 1;
+    if (win.strided()) {
+      const uint64_t ca = (a + win.phase) % win.pitch, cb = (b + win.phase) % win.pitch;
+      if (ca >= win.width) a += win.pitch - ca;
+      if (cb >= win.width) {
+        if (b < cb - win.width + 1) return false;
+        b -= cb - win.width + 1;
+      }
+      if (a > b || a >= hi) return false;
+    }
+    *first = a, *last = b;
+    return true;
+  }
+
+  // Whether every stored unit of an object of n units (in bytes) lands at an address congruent mod 16 to its object
+  // offset, so that the kernels only bulk-store 16-byte congruent spans, a TMA middle plus a byte-wise head and tail per
+  // segment.  The closed form: the first stored byte congruent; the gap between window rows a multiple of 16 when the
+  // stored bytes span more than one window row, and the gap between destination rows when they span more than one
+  // destination row.  With both gaps multiples of 16 that is exact; otherwise it may refuse a shape whose rows happen to
+  // line up, which then takes the host-staged path.
+  bool coaligned(uintptr_t dst, uint64_t n) const {
+    uint64_t a = 0, b = 0;
+    if (!stored_bounds(n, &a, &b)) return true;
+    if (win.strided() && (a + win.phase) / win.pitch != (b + win.phase) / win.pitch && (win.pitch - win.width) % 16) return false;
+    const uint64_t pa = index(a), pb = index(b);
+    if (rows.strided() && (pa + rows.phase) / rows.width != (pb + rows.phase) / rows.width && (rows.pitch - rows.width) % 16)
+      return false;
+    return (dst + at(pa) - a) % 16 == 0;
+  }
+
+  // The window seen from unit `off` (off <= win.hi), clipped to [off, off + len), with its rows: unit x of the result is
+  // unit off + x here and lands at the same address once dst has moved by *shift.  A contiguous window's dense index
+  // starts again at the shard's first stored unit, so the rows move on by the units stored before it; a strided
+  // window's index does not change.
+  WindowRows rebase(uint64_t off, uint64_t len, uint64_t* shift) const {
+    const uint64_t d = win.strided() ? 0 : std::min(std::max(win.lo, off), win.hi) - win.lo;
+    WindowRows r{win.rebase(off, len), rows};
+    r.rows = rows.rebase(d, shift);
+    return r;
+  }
+
+  // The client's rule for whether a device get of this window into these rows at dst (in bytes; an MXFP8 get's after
+  // to_wide_bytes()) may take the fused path as far as the shard [off, off + len) of a copy goes; the get is fused only
+  // if every shard of every copy passes.  Both gaps must be multiples of 16 bytes whatever the shard holds, so that
+  // whether a get is fused depends on the call's own shape and pointer, not on where the placement cut the object (as
+  // StoreWindow::fused_get_aligned); then the shard must be coaligned().
+  bool fused_get_aligned(uintptr_t dst, uint64_t off, uint64_t len) const {
+    if ((win.strided() && (win.pitch - win.width) % 16) || (rows.strided() && (rows.pitch - rows.width) % 16)) return false;
+    if (!win.touches(off, len)) return true;
+    uint64_t shift = 0;
+    const WindowRows r = rebase(off, len, &shift);
+    return r.coaligned(dst + shift, len);
+  }
+
+  // Calls f(x, at, n) for every run of n stored units from unit x of an object of n_units that land contiguously at
+  // dst + at, in order: the window's runs cut at the destination rows.
+  template <class F>
+  void for_each_run(uint64_t n_units, F&& f) const {
+    win.for_each_run(n_units, [&](uint64_t x, uint64_t a, uint64_t n) {
+      uint64_t p = win.strided() ? a : a - win.lo;
+      while (n) {
+        const uint64_t k = rows.strided() ? std::min(n, rows.width - (p + rows.phase) % rows.width) : n;
+        f(x, at(p), k);
+        x += k, p += k, n -= k;
+      }
+    });
+  }
+
+  // The rule in bytes of elements of `b` bytes (an MXFP8 get's wide side); false when the arithmetic could overflow.
+  bool to_wide_bytes(uint64_t b, WindowRows* out) const { return win.to_wide_bytes(b, &out->win) && rows.to_wide_bytes(b, &out->rows); }
+
+  // The rows as the kernels see them: their dense index of a strided window counts from pattern row 0, which is result
+  // row `row`, so the rows move back by row * width units; *shift receives how far dst moves (modulo 2^64: the kernels
+  // never dereference an address outside the rows).
+  SourceRows kernel_rows(uint64_t* shift) const {
+    *shift = 0;
+    if (!win.strided() || !rows.strided()) return rows;
+    const int64_t k = win.row * static_cast<int64_t>(win.width) + static_cast<int64_t>(rows.phase);
+    const int64_t w = static_cast<int64_t>(rows.width);
+    const int64_t j = k >= 0 ? k / w : -((-k + w - 1) / w);  // floor(k / w)
+    *shift = static_cast<uint64_t>(j) * rows.pitch;
+    return {rows.pitch, rows.width, static_cast<uint64_t>(k - j * w)};
+  }
+};
+
 // SourcePages: a dense object cut into equal pages of `page` bytes that sit at arbitrary addresses (the blocks of a paged
 // KV cache), on either side of a transfer: the source a device put reads from, or the destination a device get stores
 // into.  A page may itself be rows inside its block (a head slice of a KV block): `row_width` bytes every `row_pitch`
@@ -540,17 +660,28 @@ struct SourceBlocks {
 // too).  It is the source of a put and the destination of a get, in bytes, or for an MXFP8 transfer in elements of the
 // wide side until to_wide_bytes().  This is the one place that knows the four kinds; the transfer engine (XferItem,
 // Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the transports all hold one of these.  A
-// StoreWindow only ever goes with a contiguous layout.  A BLOCKS layout has no host copy runs (for_each_run does nothing
-// for it) until resolved() has turned it into pages.
+// StoreWindow goes with a contiguous layout, or with WINDOW_ROWS: rows of the window's dense result (WindowRows), which
+// only a get's destination has and only the calls that take both a window and destination rows build (window_rows()).
+// Its rows() are the WindowRows' rows, and the functions below that have no window treat it as the rows of a whole-object
+// get (the window [0, n) without a pattern, where p = x).  A BLOCKS layout has no host copy runs (for_each_run does
+// nothing for it) until resolved() has turned it into pages.
 class DeviceLayout {
  public:
-  enum Kind { CONTIGUOUS, ROWS, PAGES, BLOCKS };
+  enum Kind { CONTIGUOUS, ROWS, PAGES, BLOCKS, WINDOW_ROWS };
 
   DeviceLayout() = default;
   // Rows without a pattern, and a table without pages, are contiguous.
   explicit DeviceLayout(const SourceRows& r) : kind_(r.strided() ? ROWS : CONTIGUOUS), rows_(r) {}
   explicit DeviceLayout(const SourcePages& p) : kind_(p.paged() ? PAGES : CONTIGUOUS), pages_(p) {}
   explicit DeviceLayout(const SourceBlocks& b) : kind_(b.paged() ? BLOCKS : CONTIGUOUS), blocks_(b) {}
+  // Rows of a windowed get's result; rows without a pattern are contiguous (the window's own get).
+  static DeviceLayout window_rows(const SourceRows& r) {
+    DeviceLayout l(r);
+    if (r.strided()) l.kind_ = WINDOW_ROWS;
+    return l;
+  }
+  // The same rows as the destination of a whole object, where the result index is the object offset.
+  DeviceLayout as_rows() const { return kind_ == WINDOW_ROWS ? DeviceLayout(rows_) : *this; }
 
   // The layouts of SourceRows::from_rows and SourcePages::from_pages, with their object size and error rules.
   static ErrorCode from_rows(uint64_t width, uint64_t pitch, uint64_t rows, DeviceLayout* out, uint64_t* size, uint64_t* extent) {
@@ -569,24 +700,25 @@ class DeviceLayout {
 
   Kind kind() const { return kind_; }
   bool contiguous() const { return kind_ == CONTIGUOUS; }
-  const SourceRows& rows() const { return rows_; }     // the pattern of a ROWS layout
+  const SourceRows& rows() const { return rows_; }     // the pattern of a ROWS or WINDOW_ROWS layout
   const SourcePages& pages() const { return pages_; }  // the table of a PAGES layout
   const SourceBlocks& blocks() const { return blocks_; }  // the description of a BLOCKS layout
 
   // The INVALID_ARGUMENT rules against an object of len units: a valid pattern, or a table that holds every page.
   bool valid(uint64_t len) const {
-    return kind_ == ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : kind_ == BLOCKS ? blocks_.valid(len) : true;
+    return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : kind_ == BLOCKS ? blocks_.valid(len) : true;
   }
-  // The same for a put's source, which must read every unit: valid(len), and no null page (nor a selection of blocks).
+  // The same for a put's source, which must read every unit: valid(len), no null page (nor a selection of blocks), and not
+  // the rows of a get's result.
   bool valid_source(uint64_t len) const {
-    return valid(len) && !(kind_ == PAGES && pages_.has_null(len)) && !(kind_ == BLOCKS && blocks_.has_null());
+    return valid(len) && kind_ != WINDOW_ROWS && !(kind_ == PAGES && pages_.has_null(len)) && !(kind_ == BLOCKS && blocks_.has_null());
   }
 
   // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
   // when the byte arithmetic could overflow.
   bool to_wide_bytes(uint64_t b, DeviceLayout* out) const {
     *out = *this;
-    return kind_ == ROWS     ? rows_.to_wide_bytes(b, &out->rows_)
+    return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.to_wide_bytes(b, &out->rows_)
            : kind_ == PAGES  ? pages_.to_wide_bytes(b, &out->pages_)
            : kind_ == BLOCKS ? blocks_.to_wide_bytes(b, &out->blocks_)
                              : true;
@@ -597,7 +729,7 @@ class DeviceLayout {
   DeviceLayout rebase(uint64_t off, uint64_t* shift) const {
     DeviceLayout l = *this;
     *shift = off;
-    if (kind_ == ROWS) l.rows_ = rows_.rebase(off, shift);
+    if (kind_ == ROWS || kind_ == WINDOW_ROWS) l.rows_ = rows_.rebase(off, shift);
     if (kind_ == PAGES) l.pages_ = pages_.rebase(off), *shift = 0;
     if (kind_ == BLOCKS) l.blocks_ = blocks_.rebase(off), *shift = 0;
     return l;
@@ -607,7 +739,7 @@ class DeviceLayout {
   // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned, SourcePages::coaligned or
   // SourceBlocks::coaligned.
   bool coaligned(uintptr_t base, uint64_t len) const {
-    return kind_ == ROWS     ? rows_.coaligned(base, len)
+    return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.coaligned(base, len)
            : kind_ == PAGES  ? pages_.coaligned(len)
            : kind_ == BLOCKS ? blocks_.coaligned(len)
                              : base % 16 == 0;
@@ -615,8 +747,10 @@ class DeviceLayout {
 
   // The client's rule for whether a device get into this layout at `base` may take the fused path as far as the shard
   // [off, off + len) of a copy goes: a contiguous get by its store window (StoreWindow::fused_get_aligned; the default is
-  // the whole object), rows and pages by SourceRows::fused_get_aligned and SourcePages::fused_get_aligned.
+  // the whole object), rows and pages by SourceRows::fused_get_aligned and SourcePages::fused_get_aligned, rows of the
+  // window's result by WindowRows::fused_get_aligned.
   bool fused_get_aligned(uintptr_t base, uint64_t off, uint64_t len, const StoreWindow& win = {}) const {
+    if (kind_ == WINDOW_ROWS) return WindowRows{win, rows_}.fused_get_aligned(base, off, len);
     if (kind_ == ROWS) return rows_.fused_get_aligned(base, off, len);
     if (kind_ == PAGES) return pages_.fused_get_aligned(off, len);
     if (kind_ == BLOCKS) return blocks_.fused_get_aligned(off, len);
@@ -627,7 +761,7 @@ class DeviceLayout {
   // live at [addr, addr + n), in order.
   template <class F>
   void for_each_run(uintptr_t base, uint64_t len, F&& f) const {
-    if (kind_ == ROWS) rows_.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { f(x, base + at, n); });
+    if (kind_ == ROWS || kind_ == WINDOW_ROWS) rows_.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { f(x, base + at, n); });
     else if (kind_ == PAGES) pages_.for_each_run(len, f);
     else if (len && kind_ == CONTIGUOUS) f(uint64_t{0}, static_cast<uint64_t>(base), len);
   }

@@ -141,6 +141,18 @@ struct XferEngine::Slot {
     jobs.push_back(j);
     return b.has_rows() ? XFER_PAGED | XFER_PAGE_ROWS : XFER_PAGED;
   }
+  // The table entry of descriptor k whose window's result lands in rows (WindowRows, in bytes; the descriptor's byte 0
+  // is unit `trim`): the window pattern, if any, then the rows as the kernels count them.  *base receives the
+  // descriptor's dst[0], from the rows' base `dst`.  Returns XFER_WINDOW_ROWS.
+  uint32_t set_window_rows(uint32_t k, const WindowRows& wr, uint64_t trim, uintptr_t dst, void** base) {
+    uint64_t shift = 0, kshift = 0;
+    const WindowRows r = wr.rebase(trim, UINT64_MAX, &shift);
+    const SourceRows kr = r.kernel_rows(&kshift);
+    const StoreWindow& w = r.win;
+    set_stride(k, XferStride{{w.strided() ? w.pitch : 1}, w.strided() ? w.width : 1, w.phase, kr.width, kr.pitch, kr.phase});
+    *base = reinterpret_cast<void*>(dst + shift + kshift);
+    return XFER_WINDOW_ROWS;
+  }
   // Zero-size items get no descriptor: wait() reports their digest and checks their `expect` itself.
   struct Empty {
     uint32_t item;
@@ -528,12 +540,17 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       return ErrorCode::INVALID_ARGUMENT;
     // a layout is the gathering load's source or the scattering store's destination, the side its flag names
     const bool blocks = it.mem.kind() == DeviceLayout::BLOCKS;
-    // XFER_PAGE_ROWS is the engine's to set, from the layout's pattern (set_layout): a caller's flag would send a
-    // descriptor without a pattern down the in-page row walk
-    if (it.flags & XFER_PAGE_ROWS) return ErrorCode::INVALID_ARGUMENT;
-    if ((gather || scatter) == it.mem.contiguous() || ((it.flags & XFER_PAGED) && it.mem.kind() != DeviceLayout::PAGES && !blocks) ||
-        !(gather ? it.mem.valid_source(it.nbytes) : it.mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
-        (scatter && (it.ndst != 1 || (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM)))))
+    // XFER_PAGE_ROWS and XFER_WINDOW_ROWS are the engine's to set, from the layout (set_layout, and a WINDOW_ROWS layout
+    // below): a caller's flag would send a descriptor without its pattern down the in-page row walk or the windowed store
+    if (it.flags & (XFER_PAGE_ROWS | XFER_WINDOW_ROWS)) return ErrorCode::INVALID_ARGUMENT;
+    // The one scattering store with a window: into rows of the window's result (WindowRows).  Without a window those are
+    // the object's own rows.
+    const bool wrows = scatter && win && it.mem.kind() == DeviceLayout::WINDOW_ROWS;
+    const DeviceLayout mem = scatter && !win ? it.mem.as_rows() : it.mem;
+    const uint32_t scatter_excl = (wrows ? 0u : XFER_WINDOW | XFER_STRIDED) | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM;
+    if ((gather || scatter) == mem.contiguous() || ((it.flags & XFER_PAGED) && mem.kind() != DeviceLayout::PAGES && !blocks) ||
+        !(gather ? mem.valid_source(it.nbytes) : mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
+        (scatter && (it.ndst != 1 || (it.flags & scatter_excl))))
       return ErrorCode::INVALID_ARGUMENT;
     if (blocks && scatter && !it.mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;
     // Without a checksum nothing outside the window has to be read: the descriptor starts at the 16-byte boundary at or
@@ -551,8 +568,10 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     uintptr_t al = gather ? 0 : reinterpret_cast<uintptr_t>(it.src);  // gathered: the source layout instead
     // strided: the window instead; scattered: the destination layout instead
     for (uint32_t r = strided || scatter ? 1 : 0; r < it.ndst; ++r) al |= reinterpret_cast<uintptr_t>(it.dst[r]);
-    if ((al & 15) || (strided && !it.win.coaligned(reinterpret_cast<uintptr_t>(it.dst[0]))) ||
-        ((gather || scatter) && !it.mem.coaligned(reinterpret_cast<uintptr_t>(gather ? it.src : it.dst[0]), it.nbytes)))
+    const auto dst0 = reinterpret_cast<uintptr_t>(it.dst[0]);
+    const WindowRows wr{it.win, mem.rows()};
+    if ((al & 15) || (strided && !wrows && !it.win.coaligned(dst0)) || (wrows && !wr.coaligned(dst0, it.nbytes)) ||
+        ((gather || scatter) && !wrows && !mem.coaligned(reinterpret_cast<uintptr_t>(gather ? it.src : it.dst[0]), it.nbytes)))
       return ErrorCode::INVALID_ADDRESS;
     if ((it.flags & XFER_MULTIMEM) && (it.nbytes & 15)) return ErrorCode::INVALID_ARGUMENT;
     XferDesc& d = descs[nd];
@@ -560,16 +579,17 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     for (uint32_t r = 0; r < kMaxDst; ++r) d.dst[r] = r < it.ndst ? it.dst[r] : nullptr;
     if (win) {  // the descriptor's byte 0 is object byte `trim`
       const StoreWindow w = it.win.rebase(trim);
-      d.win.base = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(it.dst[0]) + w.base_shift(trim) + w.origin());
+      d.win.base = reinterpret_cast<void*>(dst0 + w.base_shift(trim) + w.origin());
       d.win.lo = w.lo;
       d.win.hi = w.hi;
-      if (strided) s->set_stride(nd, w);
+      if (strided && !wrows) s->set_stride(nd, w);
     }
     d.nbytes = nbytes;
     d.ndst = it.ndst;
     d.expect = it.expect;
     d.flags = it.flags;
-    if (gather || scatter) d.flags |= s->set_layout(nd, it.mem, nbytes, scatter);
+    if (wrows) d.flags = (d.flags & ~XFER_SCATTER) | s->set_window_rows(nd, wr, trim, dst0, &d.win.base);
+    else if (gather || scatter) d.flags |= s->set_layout(nd, mem, nbytes, scatter);
     d.reserved = (it.flags & XFER_RAW_SUM) ? it.tile_base : 0;
     if (algo == ChecksumAlgo::CRC32C) {
       d.expect = (static_cast<uint64_t>(crc_init_term_for(nbytes)) << 32) | (it.expect & 0xFFFFFFFFull);
@@ -800,18 +820,24 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
   for (uint32_t i = 0; i < n; ++i) {
     const Fp8Item& it = items[i];
     const bool strided = it.win.strided();
-    const bool shaped = !it.mem.contiguous();
+    // an unpack into rows of the window's result (WindowRows); with a window that stores the whole object in place those
+    // are the object's own rows
+    const bool wrows = unpack && it.mem.kind() == DeviceLayout::WINDOW_ROWS && !it.win.covers(it.n_elems);
+    const DeviceLayout lay = wrows ? DeviceLayout{} : unpack ? it.mem.as_rows() : it.mem;
+    const bool shaped = !lay.contiguous();
+    // the window a shaped layout may go with: none, or for rows of a window's result one that stores the whole object
+    const bool in_place = it.win.whole() || (unpack && it.mem.kind() == DeviceLayout::WINDOW_ROWS && it.win.covers(it.n_elems));
     if (!fp8_eligible(it.n_elems)) return ErrorCode::INVALID_ARGUMENT;
     if (it.wide_type != mxfp8::Wide::BF16 && it.wide_type != mxfp8::Wide::F16 && it.wide_type != mxfp8::Wide::F32)
       return ErrorCode::INVALID_ARGUMENT;
     if (mxfp8::wide_bytes(it.wide_type) != eb) return ErrorCode::INVALID_ARGUMENT;  // mixes 2- and 4-byte wide types
     DeviceLayout mem;  // a gathered put's source, or a scattered get's destination, in wide bytes; never with a window
-    if (shaped && (!it.win.whole() || !(unpack ? it.mem.valid(it.n_elems) : it.mem.valid_source(it.n_elems)) || !it.mem.to_wide_bytes(eb, &mem)))
+    if (shaped && (!in_place || !(unpack ? lay.valid(it.n_elems) : lay.valid_source(it.n_elems)) || !lay.to_wide_bytes(eb, &mem)))
       return ErrorCode::INVALID_ARGUMENT;
     if (unpack && mem.kind() == DeviceLayout::BLOCKS && !mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;
     // a strided window's rows need not start at `wide` (row 0 of the pattern may lie before the window, or the object's
     // first element after row 0's start): the window is checked instead, below
-    if ((reinterpret_cast<uintptr_t>(it.packed) & 15) || (!strided && !mem.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
+    if ((reinterpret_cast<uintptr_t>(it.packed) & 15) || (!strided && !wrows && !mem.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)))
       return ErrorCode::INVALID_ADDRESS;
     const uint32_t nrep = unpack ? 1u : it.nreplicas;
     if (nrep < 1 || nrep > kMaxDst) return ErrorCode::INVALID_ARGUMENT;
@@ -837,7 +863,13 @@ ErrorCode XferEngine::run_fp8(const std::vector<Fp8Item>& items, bool unpack, vo
       d.win.lo = w.lo;
       d.win.hi = w.hi;
     }
-    if (strided) {  // held to the rule submit() applies to a strided XferItem
+    if (wrows) {  // held to the rule submit() applies to an XferItem with a WINDOW_ROWS layout, in wide bytes
+      WindowRows wr{w, it.mem.rows()};
+      if (!it.mem.rows().valid() || !it.mem.rows().to_wide_bytes(eb, &wr.rows)) return ErrorCode::INVALID_ARGUMENT;
+      if (!wr.coaligned(reinterpret_cast<uintptr_t>(it.wide), eb * it.n_elems)) return ErrorCode::INVALID_ADDRESS;
+      if (strided) d.flags |= XFER_STRIDED;
+      d.flags |= s->set_window_rows(i, wr, 0, reinterpret_cast<uintptr_t>(it.wide), &d.win.base);
+    } else if (strided) {  // held to the rule submit() applies to a strided XferItem
       if (!w.coaligned(reinterpret_cast<uintptr_t>(it.wide))) return ErrorCode::INVALID_ADDRESS;
       d.win.base = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(it.wide) + w.origin());
       d.flags |= XFER_STRIDED;

@@ -62,6 +62,15 @@ enum XferFlags : uint32_t {
   // pages[k] + (c / row_width) * row_pitch + c % row_width.  The kernels then move the dense object's rows of row_width
   // bytes one per lane instead of whole pages; the tile is still the dense object's tile.
   XFER_PAGE_ROWS = 1u << 9,
+  // With XFER_WINDOW (and XFER_STRIDED for a strided window) only, one destination: the window's dense result lands in
+  // rows (WindowRows, common/store_window.h).  Stored unit x has the dense index p = x - lo (a range window) or
+  // p = ((x + phase) / pitch) * width + (x + phase) % pitch (a strided window, the descriptor's pattern), and lands at
+  // dst[0] + ((p + row_phase) / row_width) * row_pitch + (p + row_phase) % row_width.  The window pattern is the entry's
+  // pitch / width / phase as for XFER_STRIDED; the destination rows are its row_width / row_pitch / row_phase words,
+  // which XFER_PAGE_ROWS uses for in-page rows and which no other descriptor reads.  Only the engine sets it (from a
+  // WINDOW_ROWS layout); never with XFER_SCATTER, XFER_GATHER, XFER_PAGED, XFER_MULTIMEM or XFER_RAW_SUM.  Every tile
+  // is still loaded and hashed, so the digest and the verify are those of a plain get.
+  XFER_WINDOW_ROWS = 1u << 10,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -97,14 +106,18 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 // same rules.  An XFER_PAGED descriptor's entry is {pages, page, phase}: `pages` the device address of the first of its
 // page entries (uint64_t addresses, one per page the descriptor touches), `page` in `width`, phase < page, every page
 // co-aligned: pages[k] + phase 16-byte aligned (SourcePages::coaligned).  row_width and row_pitch are read only for
-// XFER_PAGE_ROWS descriptors: 0 < row_width < row_pitch, page % row_width == 0, (row_pitch - row_width) % 16 == 0.
+// XFER_PAGE_ROWS descriptors: 0 < row_width < row_pitch, page % row_width == 0, (row_pitch - row_width) % 16 == 0.  An
+// XFER_WINDOW_ROWS descriptor's entry holds its window pattern (XFER_STRIDED only) in the first three words and its
+// destination rows in the last three: 0 < row_width < row_pitch, row_phase < row_width, and every stored byte's
+// destination congruent to its object offset mod 16 (WindowRows::coaligned).
 struct XferStride {
   union {
     uint64_t pitch;
     uint64_t pages;  // XFER_PAGED
   };
   uint64_t width, phase;
-  uint64_t row_width = 0, row_pitch = 0;  // XFER_PAGE_ROWS
+  uint64_t row_width = 0, row_pitch = 0;  // XFER_PAGE_ROWS, XFER_WINDOW_ROWS
+  uint64_t row_phase = 0;                 // XFER_WINDOW_ROWS
 };
 
 constexpr uint32_t kSmallBytes = 4096;     // objects up to this size may take the warp-per-object path (xfer_small.cu)
@@ -131,7 +144,7 @@ struct XferLaunch {
   const XferDesc* host_descs = nullptr;
   const uint32_t* host_tile_start = nullptr;
   // Row patterns of the XFER_STRIDED, XFER_GATHER and XFER_SCATTER descriptors, one entry per descriptor (the entries of unflagged
-  // descriptors are never read, nor row_width / row_pitch of descriptors without XFER_PAGE_ROWS); null when the batch has none.  host_strides is their copy for the kernel parameters of an
+  // descriptors are never read, nor row_width / row_pitch / row_phase of descriptors without XFER_PAGE_ROWS or XFER_WINDOW_ROWS); null when the batch has none.  host_strides is their copy for the kernel parameters of an
   // inline batch; a batch with XFER_PAGED descriptors has no inline copy (their entries point into device memory).
   const XferStride* strides = nullptr;
   const XferStride* host_strides = nullptr;

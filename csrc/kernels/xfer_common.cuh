@@ -225,11 +225,68 @@ __device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64
   });
 }
 // The row pattern of descriptor `i` from a device table (read-only path); `rows`: with the in-page row pattern of an
-// XFER_PAGE_ROWS descriptor, else without (those words are not read).
+// XFER_PAGE_ROWS descriptor or the destination rows of an XFER_WINDOW_ROWS one, else without (those words are not read).
 __device__ __forceinline__ XferStride load_stride(const XferStride* table, uint32_t i, bool rows = false) {
   const uint64_t* e = reinterpret_cast<const uint64_t*>(&table[i]);
-  if (rows) return {__ldg(e), __ldg(e + 1), __ldg(e + 2), __ldg(e + 3), __ldg(e + 4)};
+  if (rows) return {__ldg(e), __ldg(e + 1), __ldg(e + 2), __ldg(e + 3), __ldg(e + 4), __ldg(e + 5)};
   return {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
+}
+// The store warp's part of a windowed scattering store (XFER_WINDOW_ROWS, entry `st`): the window's segments of the tile
+// at object offset `off` -- the span [x0, x1) of a range window whose lower bound is `lo`, or with `strided` the row
+// segments of the window pattern -- each cut at the destination rows (row_width / row_pitch / row_phase) and stored as a
+// TMA middle plus a byte-wise head and tail.  Tile byte o of a segment has the dense index poff + o (poff = off - lo, or
+// row_dst(0, ...) of its window row), and lands in destination row j = (poff + o + row_phase) / row_width at
+// row_src(dst0, poff, j, rows) + o.  Every piece (a segment's part in one destination row) goes to its own lane: a range
+// window's pieces directly, a strided window's through a warp prefix sum of its segments' piece counts, 32 segments at
+// a time, so that neither many short window rows nor a few window rows cut into many destination rows leave lanes idle.
+// The calling lane still has to commit its bulk group and wait on it.
+__device__ __forceinline__ void store_window_rows(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t x0, uint32_t x1, uint64_t lo,
+                                                  bool strided, const XferStride& st, uint32_t lane) {
+  const XferStride rows{{st.row_pitch}, st.row_width, st.row_phase};
+  const XferStride dense{{st.row_width}, st.row_width, st.row_phase};
+  if (!strided) {
+    const uint64_t poff = off - lo;
+    for_row_segments(poff, x0, x1, dense, lane, [&](uint64_t j, const TileSpan& g) {
+      store_segment(reinterpret_cast<uint8_t*>(row_src(dst0, poff, j, rows)), tile, g);
+    });
+    return;
+  }
+  constexpr uint32_t kAll = 0xffffffffu;
+  auto shfl64 = [](uint64_t v, uint32_t src) {
+    return (static_cast<uint64_t>(__shfl_sync(kAll, static_cast<uint32_t>(v >> 32), src)) << 32) | __shfl_sync(kAll, static_cast<uint32_t>(v), src);
+  };
+  const uint64_t r0 = first_row(off, x0, st);
+  const uint32_t nseg = row_count(off, x0, x1, st);
+  for (uint32_t base = 0; base < nseg; base += 32) {
+    // lane k describes segment base + k: its span, dense offset, first destination row and piece count
+    uint32_t s0 = 0, s1 = 0, cnt = 0;
+    uint64_t poff = 0, j0 = 0;
+    if (base + lane < nseg) {
+      const uint64_t r = r0 + base + lane;
+      const TileSpan g = segment_span(off, x0, x1, r, st);
+      s0 = g.x0, s1 = g.x1, poff = row_dst(0, off, r, st);
+      cnt = row_count(poff, s0, s1, dense);
+      j0 = first_row(poff, s0, dense);
+    }
+    uint32_t incl = cnt;  // inclusive prefix sum of the piece counts
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+      const uint32_t v = __shfl_up_sync(kAll, incl, d);
+      if (lane >= d) incl += v;
+    }
+    const uint32_t total = __shfl_sync(kAll, incl, 31), excl = incl - cnt;
+    for (uint32_t t0 = 0; t0 < total; t0 += 32) {
+      const uint32_t t = t0 + lane;
+      uint32_t k = 0;  // the segment of piece t: how many segments end at or before it
+      for (uint32_t b = 16; b; b >>= 1)
+        if (__shfl_sync(kAll, incl, k + b - 1) <= t) k += b;
+      const uint32_t ks0 = __shfl_sync(kAll, s0, k), ks1 = __shfl_sync(kAll, s1, k), before = __shfl_sync(kAll, excl, k);
+      const uint64_t kpoff = shfl64(poff, k), kj0 = shfl64(j0, k);
+      if (t < total) {
+        const uint64_t j = kj0 + (t - before);
+        store_segment(reinterpret_cast<uint8_t*>(row_src(dst0, kpoff, j, rows)), tile, segment_span(kpoff, ks0, ks1, j, dense));
+      }
+    }
+  }
 }
 
 // ---------------------------------------------------------------- warp helpers

@@ -17,7 +17,8 @@
 //                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.  A
 //                      scattering store (XFER_SCATTER: a get into a strided destination) stores the whole tile as
 //                      the row segments of the destination rows, one per lane; a paged one (XFER_PAGED) as the
-//                      segments of its pages.
+//                      segments of its pages.  A windowed one (XFER_WINDOW_ROWS) cuts the window's segments at the
+//                      destination rows of the dense result.
 //   warp 3  finalizer: folds the per-tile partials into per-object digests in registers; an
 //                      object that lives entirely inside this CTA's run is finalised with no
 //                      global atomics; only the <=2 objects straddling a CTA boundary use them.
@@ -347,10 +348,14 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
       const uint64_t off = static_cast<uint64_t>(m.tile_in_obj) * kTileBytes;
       const uint32_t ndst = m.ndst_flags & 0xFFu;
       const uint32_t flags = m.ndst_flags >> 8;
-      const bool strided = flags & (XFER_STRIDED | XFER_SCATTER);
+      const bool strided = flags & (XFER_STRIDED | XFER_SCATTER | XFER_WINDOW_ROWS);
       // the whole tile, or its part inside the window [dst[1], dst[2]) (object offsets)
       const auto [x0, x1, a0, a1, h1, tb] = tile_span(off, m.bytes, flags & XFER_WINDOW, m.dst[1], m.dst[2]);
-      if (strided) {
+      if (flags & XFER_WINDOW_ROWS) {
+        // the window's segments cut at the destination rows, whose words follow the window pattern's in the entry
+        const XferStride e = p.use_inline ? p.inl_strides[m.desc] : load_stride(p.strides, m.desc, true);
+        store_window_rows(s.tile[stage], m.dst[0], off, x0, x1, m.dst[1], flags & XFER_STRIDED, e, lane);
+      } else if (strided) {
         // one row segment per lane (a tile can hold thousands of short rows): TMA middle, head and tail byte-wise; a
         // strided window's rows, or the destination rows of a scattering store
         if (m.desc != st_desc) {

@@ -78,7 +78,8 @@ struct FpMeta {            // 64 bytes
   uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
                            // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
                            // FpParams::strides either way); XFER_PAGED as well when those rows are pages,
-                           // and XFER_PAGE_ROWS when the pages are in-page rows
+                           // and XFER_PAGE_ROWS when the pages are in-page rows; unpack: XFER_WINDOW_ROWS when the
+                           // window's result lands in rows (with XFER_STRIDED for a strided window)
   uint32_t f16;            // XFER_WIDE_F16: the wide side is fp16 (2-byte instantiation only)
   uint32_t pad;
 };
@@ -173,7 +174,8 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED | XFER_PAGE_ROWS : XFER_GATHER | XFER_PAGED | XFER_PAGE_ROWS);
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED | XFER_PAGE_ROWS | XFER_WINDOW_ROWS
+                                        : XFER_GATHER | XFER_PAGED | XFER_PAGE_ROWS);
         e.m.f16 = d.flags & XFER_WIDE_F16;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
@@ -277,7 +279,10 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
           }
           // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile.  A paged one stores
           // into the pages of the table in `pat` and does not read dst[0].
-          if (m.strided & XFER_PAGE_ROWS)
+          if (m.strided & XFER_WINDOW_ROWS)  // the window's segments cut at the destination rows of the dense result
+            store_window_rows(s.wide[st], m.dst[0] - off, off, x0, x1, m.dst[1], m.strided & XFER_STRIDED,
+                              load_stride(p.strides, m.desc, true), lane);
+          else if (m.strided & XFER_PAGE_ROWS)
             scatter_row_segments<true, true>(s.wide[st], m.dst[0] - off, off, x1, load_stride(p.strides, pat_desc, true), lane);
           else if (m.strided & XFER_PAGED) scatter_row_segments<true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
           else if (m.strided & XFER_SCATTER) scatter_row_segments(s.wide[st], m.dst[0] - off, off, x1, pat, lane);

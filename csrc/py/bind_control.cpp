@@ -418,6 +418,60 @@ void bind_control(py::module_& m) {
              return out;
            },
            py::arg("len"), "[(x, at, n)]: object bytes [x, x + n) are read from source bytes [at, at + n)");
+  py::class_<WindowRows>(m, "WindowRows",
+                         "A store window whose dense result lands in rows (common/store_window.h): stored unit x has the result "
+                         "index p = x - lo (a range) or (row + (x + phase) // pitch) * width + (x + phase) % pitch (strided), and "
+                         "lands at dst + ((p + rows.phase) // rows.width) * rows.pitch + (p + rows.phase) % rows.width.")
+      .def(py::init([](uint64_t lo, uint64_t hi, uint64_t pitch, uint64_t width, uint64_t phase, int64_t row, const SourceRows& rows) {
+             return WindowRows{{lo, hi, pitch, width, phase, row}, rows};
+           }),
+           py::arg("lo"), py::arg("hi"), py::arg("pitch") = 0, py::arg("width") = 0, py::arg("phase") = 0, py::arg("row") = 0,
+           py::arg("rows") = SourceRows{})
+      .def_static("from_rows",
+                  [](uint64_t offset, uint64_t width, uint64_t pitch, uint64_t rows, uint64_t size, const SourceRows& dst_rows) {
+                    WindowRows w{{}, dst_rows};
+                    const ErrorCode ec = StoreWindow::from_rows(offset, width, pitch, rows, size, &w.win);
+                    return py::make_tuple(ec, w);
+                  },
+                  py::arg("offset"), py::arg("width"), py::arg("pitch"), py::arg("rows"), py::arg("size"), py::arg("dst_rows"),
+                  "(ErrorCode, WindowRows): the window of a strided get (StoreWindow::from_rows) with these destination rows")
+      .def_property_readonly("window", [](const WindowRows& w) {
+        return py::make_tuple(w.win.lo, w.win.hi, w.win.pitch, w.win.width, w.win.phase, w.win.row);
+      }, "(lo, hi, pitch, width, phase, row)")
+      .def_property_readonly("rows", [](const WindowRows& w) { return w.rows; })
+      .def("valid", &WindowRows::valid, py::arg("n"))
+      .def("index", &WindowRows::index, py::arg("x"), "the dense result index of stored unit x")
+      .def("at", &WindowRows::at, py::arg("p"), "where result unit p lands, from dst")
+      .def("coaligned", &WindowRows::coaligned, py::arg("dst"), py::arg("n"))
+      .def("fused_get_aligned", &WindowRows::fused_get_aligned, py::arg("dst"), py::arg("off"), py::arg("len"))
+      .def("rebase",
+           [](const WindowRows& w, uint64_t off, uint64_t len) {
+             uint64_t shift = 0;
+             const WindowRows r = w.rebase(off, len, &shift);
+             return py::make_tuple(r, shift);
+           },
+           py::arg("off"), py::arg("len"), "(the rule seen from unit off, clipped to len units; how far dst moves)")
+      .def("runs",
+           [](const WindowRows& w, uint64_t n) {
+             std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> out;
+             w.for_each_run(n, [&](uint64_t x, uint64_t at, uint64_t k) { out.emplace_back(x, at, k); });
+             return out;
+           },
+           py::arg("n"), "[(x, at, k)]: stored units [x, x + k) land at [dst + at, dst + at + k)")
+      .def("to_wide_bytes",
+           [](const WindowRows& w, uint64_t b) -> py::object {
+             WindowRows r;
+             if (!w.to_wide_bytes(b, &r)) return py::none();
+             return py::cast(r);
+           },
+           py::arg("b"))
+      .def("kernel_rows",
+           [](const WindowRows& w) {
+             uint64_t shift = 0;
+             const SourceRows r = w.kernel_rows(&shift);
+             return py::make_tuple(r, shift);
+           },
+           "(the rows as the kernels count the dense index, how far dst moves modulo 2**64)");
   py::class_<PyPages>(m, "SourcePages",
                       "A dense object cut into equal pages at arbitrary addresses: a paged device put's source, or a paged get's "
                       "destination (common/store_window.h).  With k = (x + phase) // page and c = (x + phase) % page, object byte x "
@@ -1347,6 +1401,20 @@ void bind_control(py::module_& m) {
            "Elements [elem_offsets[i], elem_offsets[i] + elem_counts[i]) of packed tensor i (n_elems[i] elements), unpacked to "
            "bf16 at bf16_ptrs[i]; the whole packed object is read and verified; returns one ErrorCode per object "
            "(NOT_IMPLEMENTED: read it whole and slice).")
+      .def("batch_get_device_fp8_strided_scatter",
+           [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
+              const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
+              const std::vector<uint64_t>& rows, const std::vector<uint64_t>& dst_widths, const std::vector<uint64_t>& dst_pitches,
+              uintptr_t stream, mxfp8::Wide wide) {
+             return ecs_to_py(nogil([&] {
+               return c.batch_get_device_fp8_strided_scatter(keys, to_ptrs<void*>(ptrs), n_elems, offsets, widths, pitches, rows, dst_widths,
+                                                             dst_pitches, reinterpret_cast<void*>(stream), wide);
+             }));
+           },
+           py::arg("keys"), py::arg("bf16_ptrs"), py::arg("n_elems"), py::arg("elem_offsets"), py::arg("elem_widths"), py::arg("elem_pitches"),
+           py::arg("rows"), py::arg("dst_widths"), py::arg("dst_pitches"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+           "The window of batch_get_device_fp8_strided, in elements, unpacked into rows of dst_widths[i] elements every "
+           "dst_pitches[i] elements from bf16_ptrs[i]; returns one ErrorCode per object (NOT_IMPLEMENTED: read whole and slice).")
       .def("batch_get_device_fp8_strided",
            [](BlackbirdClient& c, const std::vector<ObjectKey>& keys, const std::vector<uintptr_t>& ptrs, const std::vector<uint64_t>& n_elems,
               const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
@@ -1441,6 +1509,20 @@ void bind_control(py::module_& m) {
          "rows[i] rows of widths[i] bytes of object i, row r = bytes [offsets[i] + r * pitches[i], + widths[i]), densely into "
          "dev_ptrs[i] (row r at dev_ptrs[i] + r * widths[i]); every shard holding a stored byte is read whole and verified; "
          "returns one ErrorCode per object.")
+      .def("batch_get_device_strided_scatter", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
+                                                  const std::vector<uint64_t>& offsets, const std::vector<uint64_t>& widths,
+                                                  const std::vector<uint64_t>& pitches, const std::vector<uint64_t>& rows,
+                                                  const std::vector<uint64_t>& dst_widths, const std::vector<uint64_t>& dst_pitches,
+                                                  uintptr_t stream) {
+        return ecs_to_py(nogil([&] {
+          return c.batch_get_device_strided_scatter(keys, to_ptrs<void*>(ptrs), offsets, widths, pitches, rows, dst_widths, dst_pitches,
+                                                    reinterpret_cast<void*>(stream));
+        }));
+      }, py::arg("keys"), py::arg("dev_ptrs"), py::arg("offsets"), py::arg("widths"), py::arg("pitches"), py::arg("rows"),
+         py::arg("dst_widths"), py::arg("dst_pitches"), py::arg("stream") = 0,
+         "The window of batch_get_device_strided (rows[i] rows of widths[i] bytes every pitches[i] from offsets[i]) into "
+         "rows of dst_widths[i] bytes every dst_pitches[i] bytes from dev_ptrs[i]: result byte p at dev_ptrs[i] + "
+         "(p // dst_widths[i]) * dst_pitches[i] + p % dst_widths[i]; returns one ErrorCode per object.")
       .def("batch_get_device_scatter", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<uintptr_t>& ptrs,
                                           const std::vector<uint64_t>& widths, const std::vector<uint64_t>& pitches,
                                           const std::vector<uint64_t>& rows, uintptr_t stream) {

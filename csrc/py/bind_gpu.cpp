@@ -74,6 +74,17 @@ int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vect
   }
   return set;
 }
+// The fourteenth (run) or thirteenth (run_fp8) slot of an item tuple: the rows (pitch, width, phase) that a windowed
+// get's dense result lands in, a WINDOW_ROWS layout (WindowRows).  An item takes one layout: with another one (k >= 0) it
+// is INVALID_ARGUMENT.  Returns whether the slot is set.
+bool to_window_rows(const py::tuple& t, size_t slot, int k, DeviceLayout* out) {
+  if (t.size() <= slot || t[slot].is_none()) return false;
+  if (k >= 0) check(ErrorCode::INVALID_ARGUMENT, "XferEngine: one layout per item");
+  auto g = t[slot].cast<std::vector<uint64_t>>();
+  if (g.size() != 3) throw py::value_error("window rows = (pitch, width, phase)");
+  *out = DeviceLayout::window_rows(SourceRows{g[0], g[1], g[2]});
+  return true;
+}
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None,
 // source pages=None, destination pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
 // it without that flag).  A window sets XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern
@@ -82,7 +93,7 @@ int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vect
 // XFER_SCATTER | XFER_PAGED (with an in-page row pattern also XFER_PAGE_ROWS).  At most one of the four.
 XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 13)
+  if (t.size() < 3 || t.size() > 14)
     throw py::value_error(
         "xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, gather (pitch, width, phase)[, scatter "
         "(pitch, width, phase)[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]]])");
@@ -98,6 +109,7 @@ XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
                                    XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED};
   const int k = to_layout(t, {7, 8, 9, 10, 11, 12}, keep, &it.mem, "XferEngine.submit");
   if (k >= 0) it.flags |= side[k];
+  if (to_window_rows(t, 13, k, &it.mem)) it.flags |= XFER_SCATTER;
   return it;
 }
 // (digests, status, device_ms), with the verdicts behind them when an item is laid out in blocks.
@@ -120,6 +132,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_SCATTER") = static_cast<uint32_t>(XFER_SCATTER);
   m.attr("XFER_PAGED") = static_cast<uint32_t>(XFER_PAGED);
   m.attr("XFER_PAGE_ROWS") = static_cast<uint32_t>(XFER_PAGE_ROWS);
+  m.attr("XFER_WINDOW_ROWS") = static_cast<uint32_t>(XFER_WINDOW_ROWS);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -163,7 +176,10 @@ void bind_gpu(py::module_& m) {
            "not read); destination pages as the eleventh set XFER_SCATTER | XFER_PAGED and store by the same rule (dst is "
            "not read); pages (addrs, page, phase, row_width, row_pitch) are in-page rows (SourcePages), c = (x + phase) % "
            "page at addrs[...] + (c // row_width) * row_pitch + c % row_width; source blocks (a DeviceBlocks, ids on the device) as the twelfth and destination blocks as the "
-           "thirteenth do the same with a page table the resolve kernel builds on the stream; returns (digests, status, "
+           "thirteenth do the same with a page table the resolve kernel builds on the stream.  Window rows (pitch, width, "
+           "phase) as the fourteenth element, with a window, set XFER_SCATTER with a WINDOW_ROWS layout: the window's dense "
+           "result (p = x - lo, or the strided window's result index) lands at dst + ((p + phase) // width) * pitch + (p + "
+           "phase) % width, which the engine marks XFER_WINDOW_ROWS; returns (digests, status, "
            "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item (VALUE_OUT_OF_RANGE or "
            "INVALID_ARGUMENT for refused ids).")
       .def("run_fp8",
@@ -182,7 +198,7 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 12)
+               if (t.size() < 3 || t.size() > 13)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
                      "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
@@ -192,6 +208,7 @@ void bind_gpu(py::module_& m) {
                // the gather slots are a pack's, the scatter slots an unpack's
                const int k = to_layout(t, {5, 6, 8, 9, 10, 11}, keep, &it.mem, "XferEngine.run_fp8");
                if (k >= 0 && (k % 2 == 1) != unpack) check(ErrorCode::INVALID_ARGUMENT, "XferEngine.run_fp8");
+               to_window_rows(t, 12, k, &it.mem);
                v.push_back(it);
              }
              XferResult res;
@@ -226,7 +243,9 @@ void bind_gpu(py::module_& m) {
            "pages on the wrong side, with rows or a window, phase >= page or a table too short; INVALID_ADDRESS unless "
            "every page touched is co-aligned in wide bytes and, for several pages, page % 8 == 0.  A put's source blocks "
            "(DeviceBlocks, page in elements) as the eleventh element and a get's destination blocks as the twelfth take a "
-           "page table the resolve kernel builds on the stream.  Returns (digests of the packed objects, status, "
+           "page table the resolve kernel builds on the stream.  A get's window rows (pitch, width, phase), in elements, as the "
+           "thirteenth element store the window's dense result into rows by the rule of WindowRows.  Returns (digests of the "
+           "packed objects, status, "
            "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item.")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
