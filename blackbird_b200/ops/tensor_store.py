@@ -5,6 +5,9 @@
     store.put("kv/layer3", kv_fp16, pack_fp8=True)                  # block-scaled MXFP8 on the wire / in the slab
     t = store.get("kv/layer3")                                      # verified + unpacked fp16 tensor
 
+    store.put_bundle("ckpt/step100", model.state_dict())            # many tensors, one object and one `#meta`
+    store.get_bundle_into("ckpt/step100", model.state_dict())       # loaded in place into the parameters
+
 Tensor metadata (dtype, shape, packing) travels in a small side object `<key>#meta`.
 """
 from __future__ import annotations
@@ -753,12 +756,18 @@ class TensorStore:
         return self.batch_get_layer_blocks_into([key], [caches], [ids], dim, None if blocks is None else [blocks])[0]
 
     # ------------------------------------------------------------------ get
-    def _metas(self, keys: Sequence[str]) -> list:
+    def _metas(self, keys: Sequence[str], bundle: bool = False) -> list:
+        """The `#meta` records of keys: KeyError for a missing one, TypeError for a bundle where a tensor is wanted or the
+        other way round (`bundle`)."""
         metas = []
-        for ec, blob in self.client.batch_get([k + "#meta" for k in keys]):
+        for k, (ec, blob) in zip(keys, self.client.batch_get([k + "#meta" for k in keys])):
             if ec != _bb.ErrorCode.OK:
                 raise KeyError(f"object metadata missing: {ec}")
-            metas.append(json.loads(blob))
+            m = json.loads(blob)
+            if ("bundle" in m) != bundle:
+                have, want = ("bundle", "tensor") if "bundle" in m else ("tensor", "bundle")
+                raise TypeError(f"{k} holds a {have}, not a {want}: use the {want} calls")
+            metas.append(m)
         return metas
 
     def batch_get(self, keys: Sequence[str], device: Optional[torch.device] = None) -> list:
@@ -1089,6 +1098,169 @@ class TensorStore:
         """`t[start:stop]` of the tensor stored under `key` into `out` (see batch_get_slices_into)."""
         return self.batch_get_slices_into([key], [out], [0], [start], [stop])[0]
 
+    # ------------------------------------------------------------------ bundles
+    def _gap_zeros(self, device: torch.device) -> torch.Tensor:
+        """32 zero bytes at a 16-byte aligned address on `device`: the source of every gap between a bundle's tensors."""
+        cache = self.__dict__.setdefault("_gap_zero_bufs", {})
+        if device not in cache:
+            cache[device] = torch.zeros(32, dtype=torch.uint8, device=device)
+        return cache[device]
+
+    @staticmethod
+    def _bundle_items(bundle, what: str) -> tuple:
+        """(container kind, [(name, value)]) of a mapping (a state_dict) or a sequence, whose names are its indices."""
+        if isinstance(bundle, dict) or hasattr(bundle, "items"):
+            return "dict", [(str(k), v) for k, v in bundle.items()]
+        if isinstance(bundle, (list, tuple)):
+            return "list", [(str(i), v) for i, v in enumerate(bundle)]
+        raise TypeError(f"{what}: a bundle is a mapping of names to tensors or a sequence of tensors, not {type(bundle).__name__}")
+
+    def batch_put_bundles(self, keys: Sequence[str], bundles: Sequence, config=None) -> None:
+        """Stores each bundle -- a mapping of names to CUDA tensors, such as a `state_dict`, or a sequence of them -- as
+        ONE object under its key, with one `#meta`: the tensors back to back, each at a 16-byte aligned offset, read in
+        place by the fused put kernel from a segment list (batch_put_device_segments), one native call for the batch.  A
+        bundle costs one object's control-plane work instead of two per tensor, and it is stored whole or not at all.
+
+        The gaps between tensors are read from a small zeroed device buffer at an address congruent to the gap's offset,
+        so a bundle of 16-byte aligned contiguous tensors is read wholly in place; a tensor that is not contiguous or not
+        16-byte aligned is copied into an aligned temporary first.  Every dtype TensorStore knows is accepted, 0-d and
+        zero-element tensors included.  TypeError for another dtype or a value that is not a tensor, ValueError for a
+        tensor that is not a CUDA tensor on the current device; both before anything is stored.  The `#meta` records
+        each entry's name, dtype, shape, offset and bytes and the total."""
+        cfg = config or self.config
+        keys, bundles = list(keys), list(bundles)
+        if len(keys) != len(bundles):
+            raise ValueError("keys and bundles differ in length")
+        plans = []
+        for k, b in zip(keys, bundles):
+            kind, items = self._bundle_items(b, k)
+            for name, t in items:
+                if not isinstance(t, torch.Tensor):
+                    raise TypeError(f"{k}[{name}]: not a tensor but {type(t).__name__}")
+                if t.dtype not in _DTYPES.values():
+                    raise TypeError(f"{k}[{name}]: dtype {t.dtype} is not one TensorStore stores")
+                if not t.is_cuda or t.device.index != torch.cuda.current_device():
+                    raise ValueError(f"{k}[{name}]: must be a CUDA tensor on the current device, not {t.device}")
+            plans.append((kind, items))
+        zeros = self._gap_zeros(torch.device("cuda", torch.cuda.current_device())).data_ptr()
+        segments, metas, keep = [], [], []
+        for kind, items in plans:
+            segs, entries, off = [], [], 0
+            for name, t in items:
+                nbytes = t.numel() * t.element_size()
+                if nbytes and (not t.is_contiguous() or t.data_ptr() % 16):
+                    t = t.clone(memory_format=torch.contiguous_format) if t.is_contiguous() else t.contiguous()
+                    if t.data_ptr() % 16:  # a fresh allocation is aligned; this is a guard, not a route
+                        t = torch.empty_like(t).copy_(t)
+                    keep.append(t)
+                gap = -off % 16
+                if gap:
+                    segs.append((zeros + off % 16, gap))
+                    off += gap
+                if nbytes:
+                    segs.append((t.data_ptr(), nbytes))
+                entries.append({"name": name, "dtype": str(t.dtype).replace("torch.", ""), "shape": list(t.shape), "offset": off,
+                                "bytes": nbytes})
+                off += nbytes
+            segments.append(np.array(segs, dtype=np.uint64).reshape(-1, 2))
+            metas.append(json.dumps({"bundle": kind, "entries": entries, "total": off}).encode())
+        ecs = self.client.batch_put_device_segments(keys, segments, cfg, self._stream())
+        _check("bundle put", keys, ecs)
+        self._put_metas(keys, metas)
+
+    def put_bundle(self, key: str, tensors, config=None) -> None:
+        """Stores the mapping or sequence of CUDA tensors `tensors` as one object (see batch_put_bundles)."""
+        self.batch_put_bundles([key], [tensors], config)
+
+    @staticmethod
+    def _entry_view(buf: torch.Tensor, e: dict) -> torch.Tensor:
+        dt = _DTYPES[e["dtype"]]
+        return buf[e["offset"]: e["offset"] + e["bytes"]].view(dt).view(e["shape"])
+
+    def batch_get_bundles(self, keys: Sequence[str], device: Optional[torch.device] = None) -> list:
+        """Each stored bundle in the container type it was stored as (a dict, or a list for a sequence), its tensors views
+        of ONE aligned allocation per bundle that a single plain device get (batch_get_device) filled and verified: the
+        views share that storage, so resizing one or keeping one alive keeps the whole bundle's allocation.  TypeError
+        for a key that holds a tensor, KeyError for a missing one."""
+        device = device or torch.device("cuda", torch.cuda.current_device())
+        keys = list(keys)
+        metas = self._metas(keys, bundle=True)
+        bufs = [torch.empty(max(m["total"], 1), dtype=torch.uint8, device=device) for m in metas]
+        idx = [i for i, m in enumerate(metas) if m["total"]]
+        if idx:
+            ecs, _ = self.client.batch_get_device([keys[i] for i in idx], [bufs[i].data_ptr() for i in idx], [metas[i]["total"] for i in idx],
+                                                  self._stream())
+            _check("bundle get", [keys[i] for i in idx], ecs)
+        out = []
+        for m, b in zip(metas, bufs):
+            views = [(e["name"], self._entry_view(b, e)) for e in m["entries"]]
+            out.append(dict(views) if m["bundle"] == "dict" else [v for _, v in views])
+        return out
+
+    def get_bundle(self, key: str, device: Optional[torch.device] = None):
+        """The bundle stored under `key` (see batch_get_bundles)."""
+        return self.batch_get_bundles([key], device)[0]
+
+    def batch_get_bundles_into(self, keys: Sequence[str], outs: Sequence) -> list:
+        """Loads stored bundles into existing CUDA tensors in place -- a checkpoint into a module's parameters -- and
+        returns `outs`.  outs[i] maps entry names to tensors (a sequence stands for names 0, 1, ...) and may name a subset:
+        the entries it does not name, and the gaps, are not stored.  Every bundle is one segment list of ONE
+        batch_get_device_segments call: a contiguous 16-byte aligned out is a segment itself, any other out gets a
+        contiguous temporary segment and then out.copy_(tmp).  Every shard of the object is still read whole and
+        verified.
+
+        Every check comes before any transfer: KeyError for a missing key or name, TypeError for a key that holds a
+        tensor or an out of another dtype than its entry, ValueError for another shape or an out that is not a CUDA
+        tensor on the current device."""
+        keys, outs = list(keys), list(outs)
+        if len(keys) != len(outs):
+            raise ValueError("keys and outs differ in length")
+        metas = self._metas(keys, bundle=True)
+        dev = torch.cuda.current_device()
+        named = []
+        for k, m, o in zip(keys, metas, outs):
+            _, items = self._bundle_items(o, k)
+            entries = {e["name"]: e for e in m["entries"]}
+            for name, t in items:
+                if name not in entries:
+                    raise KeyError(f"{k}: the bundle has no entry {name!r}")
+                e = entries[name]
+                if not isinstance(t, torch.Tensor):
+                    raise TypeError(f"{k}[{name}]: not a tensor but {type(t).__name__}")
+                if t.dtype != _DTYPES[e["dtype"]]:
+                    raise TypeError(f"{k}[{name}]: out is {t.dtype}, the stored tensor {e['dtype']}")
+                if list(t.shape) != e["shape"]:
+                    raise ValueError(f"{k}[{name}]: out has shape {list(t.shape)}, the stored tensor {e['shape']}")
+                if not t.is_cuda or t.device.index != dev:
+                    raise ValueError(f"{k}[{name}]: out must be a CUDA tensor on cuda:{dev}, not {t.device}")
+            named.append(dict(items))
+        segments, copies = [], []
+        for m, want in zip(metas, named):
+            segs, off = [], 0
+            for e in m["entries"]:
+                if e["offset"] > off:
+                    segs.append((0, e["offset"] - off))
+                t = want.get(e["name"])
+                if e["bytes"] and t is None:
+                    segs.append((0, e["bytes"]))
+                elif e["bytes"]:
+                    if not t.is_contiguous() or t.data_ptr() % 16:
+                        tmp = torch.empty(e["shape"], dtype=t.dtype, device=t.device)
+                        copies.append((t, tmp))
+                        t = tmp
+                    segs.append((t.data_ptr(), e["bytes"]))
+                off = e["offset"] + e["bytes"]
+            segments.append(np.array(segs, dtype=np.uint64).reshape(-1, 2))
+        ecs, _ = self.client.batch_get_device_segments(keys, segments, self._stream())
+        _check("bundle get", keys, ecs)
+        for t, tmp in copies:
+            t.copy_(tmp)
+        return outs
+
+    def get_bundle_into(self, key: str, outs):
+        """Loads the bundle stored under `key` into the tensors `outs` names (see batch_get_bundles_into)."""
+        return self.batch_get_bundles_into([key], [outs])[0]
+
     def remove(self, keys: Sequence[str]) -> None:
         self.client.batch_remove(list(keys) + [k + "#meta" for k in keys])
 
@@ -1189,6 +1361,18 @@ class AsyncTensorStore(TensorStore):
         caches = list(caches)
         return self._on_side(True, self.batch_get_layer_blocks_into, list(keys), caches, list(ids), dim,
                              None if blocks is None else list(blocks), result=caches)
+
+    def put_bundles_async(self, keys: Sequence[str], bundles: Sequence, config=None):
+        """batch_put_bundles on the side stream, ordered after the work already queued on the caller's stream; the future
+        yields the number of bundles stored, or raises the call's error."""
+        keys, bundles = list(keys), list(bundles)  # keep the tensors alive until the transfer is done
+        return self._on_side(True, self.batch_put_bundles, keys, bundles, config, result=len(keys))
+
+    def get_bundles_into_async(self, keys: Sequence[str], outs: Sequence):
+        """batch_get_bundles_into on the side stream, ordered after the work already queued on the caller's stream; the
+        future yields `outs`, already synchronised with the side stream."""
+        outs = list(outs)
+        return self._on_side(True, self.batch_get_bundles_into, list(keys), outs, result=outs)
 
     def close(self):
         self._pool.shutdown(wait=True)

@@ -644,6 +644,7 @@ struct ShapedItem {
   DeviceLayout mem;
   uint64_t units = 0;
   bool table = false;
+  std::vector<SegmentEntry> segments;  // the table a SEGMENTS layout points into
 };
 
 static ErrorCode rows_item(uint64_t width, uint64_t pitch, uint64_t rows, ShapedItem* it) {
@@ -667,13 +668,20 @@ static ErrorCode blocks_item(const SourceBlocks& blocks, ShapedItem* it) {
   return ec;
 }
 
+static ErrorCode segments_item(const std::vector<SourceSegments::Segment>& segs, ShapedItem* it) {
+  SourceSegments g;
+  const ErrorCode ec = SourceSegments::from_segments(segs.data(), segs.size(), &it->segments, &g, &it->units);
+  it->mem = DeviceLayout(g);
+  return ec;
+}
+
 // The admission rule of the shaped calls (blackbird_client.h), in this order: an item of a put or a get of units of b
 // bytes (`packed`: MXFP8 elements), its layout at `base`.
 static ErrorCode admit_shaped(const ShapedItem& it, bool put, uint64_t b, bool packed, const void* base) {
   const DeviceLayout& m = it.mem;
   const uint64_t u = it.units;
   if (packed && it.table && (u == 0 || u % 32)) return ErrorCode::INVALID_ARGUMENT;  // no packed object has that many elements
-  if (put && (m.pages().has_null(u) || m.blocks().has_null())) return ErrorCode::INVALID_ARGUMENT;  // a put reads every unit
+  if (put && (m.pages().has_null(u) || m.blocks().has_null() || m.segments().has_null(u))) return ErrorCode::INVALID_ARGUMENT;  // a put reads every unit
   if (u > SIZE_MAX) return ErrorCode::VALUE_OUT_OF_RANGE;
   DeviceLayout bytes;
   const uint64_t extent = m.kind() == DeviceLayout::ROWS ? m.rows().extent(u) : u;
@@ -1263,6 +1271,15 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_paged(const std::vector
       [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], page_rows, i, it); }, cfg, stream);
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_segments(const std::vector<ObjectKey>& keys,
+                                                                  const std::vector<std::vector<SourceSegments::Segment>>& segments,
+                                                                  const WorkerConfig& cfg, void* stream) {
+  const size_t n = keys.size();
+  return shaped_put(
+      "device_put_segments", keys, std::vector<const void*>(n), segments.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], it); }, cfg, stream);
+}
+
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
                                                    const std::vector<size_t>& sizes, const std::vector<DeviceLayout>* mem,
                                                    const WorkerConfig& cfg, void* stream) {
@@ -1467,6 +1484,15 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_paged(const std::vector
   return shaped_get(
       "device_get_paged", keys, std::vector<void*>(n), pages.size() == n && page_bytes.size() == n && (page_rows.empty() || page_rows.size() == n), std::nullopt,
       [&](size_t i, ShapedItem* it) { return pages_item(pages[i], page_bytes[i], page_rows, i, it); }, stream, out_sizes);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_segments(const std::vector<ObjectKey>& keys,
+                                                                  const std::vector<std::vector<SourceSegments::Segment>>& segments, void* stream,
+                                                                  std::vector<size_t>* out_sizes) {
+  const size_t n = keys.size();
+  return shaped_get(
+      "device_get_segments", keys, std::vector<void*>(n), segments.size() == n, std::nullopt,
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,

@@ -415,6 +415,27 @@ class BlackbirdClient {
   // of the object is stored, it is not retried on another replica, and the rest of the batch carries on.
   std::vector<ErrorCode> batch_get_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
                                                  std::vector<size_t>* out_sizes);
+  // Segment-list puts (the tensors of a state_dict, a request's per-layer state of several sizes, as one object):
+  // object i is the concatenation of the segments segments[i], each a (device address, bytes) pair, in list order
+  // (SourceSegments in common/store_window.h); one object, one metadata record, one digest set, one placement.  The stored
+  // object and its digests are those of batch_put_device of the concatenation, so every get reads it.  The fused path
+  // reads each segment in place in the put kernel; it needs every shard of every copy co-aligned (SourceSegments::
+  // coaligned: address = object offset mod 16 for every segment, with shards cut at 16-byte multiples).  Any other item,
+  // and every placement the fabric cannot reach, is staged through the host (one D2H copy per run of segments) while the
+  // rest of the batch keeps the fused launch.  Per object, the shaped calls' admission (shaped_put) of
+  // SourceSegments::from_segments: zero-length segments are dropped, VALUE_OUT_OF_RANGE when the total overflows,
+  // INVALID_ARGUMENT for a segment at address 0.  No segments is a zero-byte object.
+  std::vector<ErrorCode> batch_put_device_segments(const std::vector<ObjectKey>& keys, const std::vector<std::vector<SourceSegments::Segment>>& segments,
+                                                   const WorkerConfig& cfg, void* stream);
+  // Segment-list gets, the mirror: object i lands in the segments segments[i] in list order.  The capacity is the sum of
+  // the lengths, null segments included: a larger object is BUFFER_OVERFLOW, a shorter one fills its bytes in list order;
+  // out_sizes[i] receives the size.  A segment at address 0 is not stored (a null segment): a partial restore names only
+  // the segments it wants.  Every shard is read whole and verified, with the fail-over and placement refresh of
+  // batch_get_device.  The fused path scatters the segments in the get kernel; it needs SourceSegments::fused_get_aligned
+  // for every shard of every copy.  Any other item, and every placement the fabric cannot reach, is staged through the
+  // host (one H2D copy per run of segments).  Admission as batch_put_device_segments', null segments allowed.
+  std::vector<ErrorCode> batch_get_device_segments(const std::vector<ObjectKey>& keys, const std::vector<std::vector<SourceSegments::Segment>>& segments,
+                                                   void* stream, std::vector<size_t>* out_sizes);
 
   Result<ClusterStats> cluster_stats();
   rpc::KeystoneApi& keystone() { return *keystone_; }

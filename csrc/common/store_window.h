@@ -13,10 +13,12 @@
 //
 // SourceRows, below, maps a dense object onto strided memory instead: where a put reads each byte from, or where a get into
 // a sliced destination stores it.  SourcePages maps it onto pages at arbitrary addresses, SourceBlocks onto pages named
-// by block ids in device memory.  DeviceLayout, at the end, is the one type the other layers hold for any of them.
+// by block ids in device memory, SourceSegments onto a list of segments of any sizes.  DeviceLayout, at the end, is the
+// one type the other layers hold for any of them.
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 #include "common/error.h"
@@ -654,11 +656,145 @@ struct SourceBlocks {
   }
 };
 
+// One segment of a SourceSegments table as the kernels load it, 16 bytes: the object offset of its first byte and its
+// address.
+struct SegmentEntry {
+  uint64_t start, addr;
+};
+static_assert(sizeof(SegmentEntry) == 16, "one uint4 load per segment entry");
+
+// SourceSegments: an object that is the concatenation of a list of segments of any sizes at arbitrary addresses (the
+// tensors of a state_dict, a request's KV pages and SSM state), on either side of a transfer: the source a device put
+// reads from, or the destination a device get stores into.  Segment k is (addr[k], len[k]) and holds object bytes
+// [start[k], start[k] + len[k]), start being the exclusive prefix sum of the lengths, so object byte x lives at
+//   addr[k] + (x - start[k])    for the k with start[k] <= x < start[k + 1]
+// The table is `nseg` SegmentEntry {start, addr} followed by the end sentinel {total, 0}, so that entry k + 1 gives the
+// end of segment k; from_segments() builds it (zero-length segments dropped, starts strictly increasing).  `phase` is
+// the object offset of byte 0 as the holder sees it (rebase()): byte x of a rebased table is object byte phase + x.  This
+// is the one statement of the rule; the transfer engine (XferItem), the fabric's ops (DeviceShardOp), the client, the
+// host loopback transport and the kernels' XFER_SEGMENTS descriptors (kernels/xfer.h) all follow it.  The unit is a byte
+// (there are no MXFP8 segment transfers).
+//
+// An address of 0 is a null segment, as SourcePages' null page: on the get side its bytes are read and verified but not
+// stored (a partial restore of some tensors of a bundle); a put refuses it (has_null, DeviceLayout::valid_source).  Null
+// segments start and extend no run and are exempt from the alignment rules.
+struct SourceSegments {
+  using Segment = std::pair<uint64_t, uint64_t>;  // (address, bytes)
+
+  const SegmentEntry* entries = nullptr;  // nseg entries, then the sentinel
+  uint64_t nseg = 0, phase = 0;
+
+  bool segmented() const { return entries != nullptr; }
+  // The object's size: the sentinel's start.
+  uint64_t total() const { return entries ? entries[nseg].start : 0; }
+
+  // The table of the `count` segments at segs into *table (which the result points into): an object of *size bytes.
+  // Zero-length segments are dropped.  VALUE_OUT_OF_RANGE when the total overflows.  No segment (or only empty ones) is
+  // a zero-byte object, with no table.
+  static ErrorCode from_segments(const Segment* segs, uint64_t count, std::vector<SegmentEntry>* table, SourceSegments* out, uint64_t* size) {
+    *out = {};
+    *size = 0;
+    table->clear();
+    uint64_t total = 0;
+    for (uint64_t k = 0; k < count; ++k) {
+      if (segs[k].second == 0) continue;
+      table->push_back({total, segs[k].first});
+      if (__builtin_add_overflow(total, segs[k].second, &total)) {
+        table->clear();
+        return ErrorCode::VALUE_OUT_OF_RANGE;
+      }
+    }
+    if (table->empty()) return ErrorCode::OK;
+    const uint64_t n = table->size();
+    table->push_back({total, 0});
+    *out = {table->data(), n, 0};
+    *size = total;
+    return ErrorCode::OK;
+  }
+
+  // The segment holding byte x (x < total() - phase): the last entry starting at or before phase + x.
+  uint64_t seg_of(uint64_t x) const {
+    const uint64_t g = phase + x;
+    const SegmentEntry* e = std::upper_bound(entries, entries + nseg, g, [](uint64_t v, const SegmentEntry& s) { return v < s.start; });
+    return e == entries ? 0 : static_cast<uint64_t>(e - entries) - 1;
+  }
+  // Whether the table holds bytes [0, len) with its entry 0 holding byte 0, the form from_segments() and rebase() keep
+  // (start[0] <= phase < start[1], or phase == total() for a table rebased to its end): the kernels search from entry 0
+  // and the engine copies the entries from there.
+  bool valid(uint64_t len) const {
+    if (!segmented() || entries[0].start > phase || phase > total() || len > total() - phase) return false;
+    return nseg == 0 ? phase == total() : phase < entries[1].start;
+  }
+  // Calls f(k) for every segment that bytes [0, len) touch, in order.
+  template <class F>
+  void for_each_touched(uint64_t len, F&& f) const {
+    if (len == 0 || !segmented()) return;
+    for (uint64_t k = seg_of(0); k < nseg && entries[k].start < phase + len; ++k) f(k);
+  }
+  // Segments that bytes [0, len) touch, the first being entry 0 of a rebased table.
+  uint64_t segments_for(uint64_t len) const {
+    uint64_t n = 0;
+    for_each_touched(len, [&](uint64_t) { ++n; });
+    return n;
+  }
+  // Whether a segment that bytes [0, len) touch is null.
+  bool has_null(uint64_t len) const {
+    bool null = false;
+    for_each_touched(len, [&](uint64_t k) { null = null || entries[k].addr == 0; });
+    return null;
+  }
+
+  // The table seen from byte `off` (off <= total() - phase): byte x of the result is byte off + x here.  Shards of a
+  // striped object may start inside a segment, which the new phase records; entry 0 of the result holds its byte 0.
+  SourceSegments rebase(uint64_t off) const {
+    if (!segmented()) return *this;
+    const uint64_t g = phase + off;
+    const uint64_t k = g < total() ? seg_of(off) : nseg;
+    return {entries + k, nseg - k, g};
+  }
+
+  // Whether bytes [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by TMA:
+  // byte x of segment k lives at addr[k] - start[k] + phase + x, so addr[k] + phase - start[k] must be 16-byte aligned
+  // for every non-null segment touched.  (For a shard cut at a multiple of 16 bytes that is addr[k] = start[k] mod 16.)
+  bool coaligned(uint64_t len) const {
+    bool ok = true;
+    for_each_touched(len, [&](uint64_t k) { ok = ok && (entries[k].addr == 0 || (entries[k].addr + phase - entries[k].start) % 16 == 0); });
+    return ok;
+  }
+  // The client's rule for whether a device get into these segments may take the fused path as far as the shard
+  // [off, off + len) of a copy goes; the get is fused only if every shard of every copy passes.  As for pages, the verdict
+  // is the segments' own, addr[k] = start[k] mod 16 where the object is cut at 16-byte multiples.
+  bool fused_get_aligned(uint64_t off, uint64_t len) const { return rebase(off).coaligned(len); }
+
+  // Calls f(x, addr, n) for every run of n contiguous bytes of bytes [0, len): bytes [x, x + n) live at [addr, addr + n),
+  // in order.  Segments that follow one another in memory make one run; null segments make none and end the run before
+  // them.
+  template <class F>
+  void for_each_run(uint64_t len, F&& f) const {
+    uint64_t run_x = 0, run_at = 0, run_n = 0;
+    for_each_touched(len, [&](uint64_t k) {
+      const uint64_t a = std::max(entries[k].start, phase), b = std::min(entries[k + 1].start, phase + len);
+      const uint64_t x = a - phase, n = b - a, at = entries[k].addr + (a - entries[k].start);
+      if (entries[k].addr == 0) {
+        if (run_n) f(run_x, run_at, run_n);
+        run_n = 0;
+      } else if (run_n && run_at + run_n == at) {
+        run_n += n;
+      } else {
+        if (run_n) f(run_x, run_at, run_n);
+        run_x = x, run_at = at, run_n = n;
+      }
+    });
+    if (run_n) f(run_x, run_at, run_n);
+  }
+};
+
 // DeviceLayout: where the caller's units of one object sit on the device side of a transfer, relative to a base address:
 // contiguous (unit x at base + x, the default), in rows (SourceRows, with row 0 at the base), in pages (SourcePages,
-// whose addresses are absolute: the base is not used) or in blocks picked by device-resident ids (SourceBlocks, absolute
-// too).  It is the source of a put and the destination of a get, in bytes, or for an MXFP8 transfer in elements of the
-// wide side until to_wide_bytes().  This is the one place that knows the four kinds; the transfer engine (XferItem,
+// whose addresses are absolute: the base is not used), in blocks picked by device-resident ids (SourceBlocks, absolute
+// too) or in segments of any sizes (SourceSegments, absolute too).  It is the source of a put and the destination of a
+// get, in bytes, or for an MXFP8 transfer in elements of the wide side until to_wide_bytes() (which refuses segments).
+// This is the one place that knows the kinds; the transfer engine (XferItem,
 // Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the transports all hold one of these.  A
 // StoreWindow goes with a contiguous layout, or with WINDOW_ROWS: rows of the window's dense result (WindowRows), which
 // only a get's destination has and only the calls that take both a window and destination rows build (window_rows()).
@@ -667,13 +803,14 @@ struct SourceBlocks {
 // nothing for it) until resolved() has turned it into pages.
 class DeviceLayout {
  public:
-  enum Kind { CONTIGUOUS, ROWS, PAGES, BLOCKS, WINDOW_ROWS };
+  enum Kind { CONTIGUOUS, ROWS, PAGES, BLOCKS, WINDOW_ROWS, SEGMENTS };
 
   DeviceLayout() = default;
   // Rows without a pattern, and a table without pages, are contiguous.
   explicit DeviceLayout(const SourceRows& r) : kind_(r.strided() ? ROWS : CONTIGUOUS), rows_(r) {}
   explicit DeviceLayout(const SourcePages& p) : kind_(p.paged() ? PAGES : CONTIGUOUS), pages_(p) {}
   explicit DeviceLayout(const SourceBlocks& b) : kind_(b.paged() ? BLOCKS : CONTIGUOUS), blocks_(b) {}
+  explicit DeviceLayout(const SourceSegments& s) : kind_(s.segmented() ? SEGMENTS : CONTIGUOUS), segments_(s) {}
   // Rows of a windowed get's result; rows without a pattern are contiguous (the window's own get).
   static DeviceLayout window_rows(const SourceRows& r) {
     DeviceLayout l(r);
@@ -703,21 +840,28 @@ class DeviceLayout {
   const SourceRows& rows() const { return rows_; }     // the pattern of a ROWS or WINDOW_ROWS layout
   const SourcePages& pages() const { return pages_; }  // the table of a PAGES layout
   const SourceBlocks& blocks() const { return blocks_; }  // the description of a BLOCKS layout
+  const SourceSegments& segments() const { return segments_; }  // the table of a SEGMENTS layout
 
   // The INVALID_ARGUMENT rules against an object of len units: a valid pattern, or a table that holds every page.
   bool valid(uint64_t len) const {
-    return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.valid() : kind_ == PAGES ? pages_.valid(len) : kind_ == BLOCKS ? blocks_.valid(len) : true;
+    return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.valid()
+           : kind_ == PAGES                      ? pages_.valid(len)
+           : kind_ == BLOCKS                     ? blocks_.valid(len)
+           : kind_ == SEGMENTS                   ? segments_.valid(len)
+                                                 : true;
   }
-  // The same for a put's source, which must read every unit: valid(len), no null page (nor a selection of blocks), and not
-  // the rows of a get's result.
+  // The same for a put's source, which must read every unit: valid(len), no null page or segment (nor a selection of
+  // blocks), and not the rows of a get's result.
   bool valid_source(uint64_t len) const {
-    return valid(len) && kind_ != WINDOW_ROWS && !(kind_ == PAGES && pages_.has_null(len)) && !(kind_ == BLOCKS && blocks_.has_null());
+    return valid(len) && kind_ != WINDOW_ROWS && !(kind_ == PAGES && pages_.has_null(len)) && !(kind_ == BLOCKS && blocks_.has_null()) &&
+           !(kind_ == SEGMENTS && segments_.has_null(len));
   }
 
   // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
-  // when the byte arithmetic could overflow.
+  // when the byte arithmetic could overflow, and for segments, which have no MXFP8 transfers.
   bool to_wide_bytes(uint64_t b, DeviceLayout* out) const {
     *out = *this;
+    if (kind_ == SEGMENTS) return false;
     return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.to_wide_bytes(b, &out->rows_)
            : kind_ == PAGES  ? pages_.to_wide_bytes(b, &out->pages_)
            : kind_ == BLOCKS ? blocks_.to_wide_bytes(b, &out->blocks_)
@@ -725,35 +869,38 @@ class DeviceLayout {
   }
 
   // The layout seen from object unit `off`: unit x of the result is unit off + x here, relative to a base that has moved
-  // by *shift (off when contiguous, to where the new pattern's row 0 starts for rows, 0 for pages and blocks).
+  // by *shift (off when contiguous, to where the new pattern's row 0 starts for rows, 0 for pages, blocks and segments).
   DeviceLayout rebase(uint64_t off, uint64_t* shift) const {
     DeviceLayout l = *this;
     *shift = off;
     if (kind_ == ROWS || kind_ == WINDOW_ROWS) l.rows_ = rows_.rebase(off, shift);
     if (kind_ == PAGES) l.pages_ = pages_.rebase(off), *shift = 0;
     if (kind_ == BLOCKS) l.blocks_ = blocks_.rebase(off), *shift = 0;
+    if (kind_ == SEGMENTS) l.segments_ = segments_.rebase(off), *shift = 0;
     return l;
   }
 
   // Whether object bytes [0, len) at `base` are co-aligned with the tiles, so that the kernels only move 16-byte congruent
-  // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned, SourcePages::coaligned or
-  // SourceBlocks::coaligned.
+  // spans: the base 16-byte aligned when contiguous, else SourceRows::coaligned, SourcePages::coaligned,
+  // SourceBlocks::coaligned or SourceSegments::coaligned.
   bool coaligned(uintptr_t base, uint64_t len) const {
     return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.coaligned(base, len)
-           : kind_ == PAGES  ? pages_.coaligned(len)
-           : kind_ == BLOCKS ? blocks_.coaligned(len)
-                             : base % 16 == 0;
+           : kind_ == PAGES    ? pages_.coaligned(len)
+           : kind_ == BLOCKS   ? blocks_.coaligned(len)
+           : kind_ == SEGMENTS ? segments_.coaligned(len)
+                               : base % 16 == 0;
   }
 
   // The client's rule for whether a device get into this layout at `base` may take the fused path as far as the shard
   // [off, off + len) of a copy goes: a contiguous get by its store window (StoreWindow::fused_get_aligned; the default is
-  // the whole object), rows and pages by SourceRows::fused_get_aligned and SourcePages::fused_get_aligned, rows of the
-  // window's result by WindowRows::fused_get_aligned.
+  // the whole object), rows, pages and segments by their own fused_get_aligned, rows of the window's result by
+  // WindowRows::fused_get_aligned.
   bool fused_get_aligned(uintptr_t base, uint64_t off, uint64_t len, const StoreWindow& win = {}) const {
     if (kind_ == WINDOW_ROWS) return WindowRows{win, rows_}.fused_get_aligned(base, off, len);
     if (kind_ == ROWS) return rows_.fused_get_aligned(base, off, len);
     if (kind_ == PAGES) return pages_.fused_get_aligned(off, len);
     if (kind_ == BLOCKS) return blocks_.fused_get_aligned(off, len);
+    if (kind_ == SEGMENTS) return segments_.fused_get_aligned(off, len);
     return win.fused_get_aligned(base, off, len);
   }
 
@@ -763,6 +910,7 @@ class DeviceLayout {
   void for_each_run(uintptr_t base, uint64_t len, F&& f) const {
     if (kind_ == ROWS || kind_ == WINDOW_ROWS) rows_.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { f(x, base + at, n); });
     else if (kind_ == PAGES) pages_.for_each_run(len, f);
+    else if (kind_ == SEGMENTS) segments_.for_each_run(len, f);
     else if (len && kind_ == CONTIGUOUS) f(uint64_t{0}, static_cast<uint64_t>(base), len);
   }
 
@@ -781,6 +929,7 @@ class DeviceLayout {
   SourceRows rows_;
   SourcePages pages_;
   SourceBlocks blocks_;
+  SourceSegments segments_;
 };
 
 }  // namespace bb

@@ -34,11 +34,12 @@ ErrorCode XferEngine::cuda_failed(int code, const char* what) {
 
 namespace {
 // A slot's table of nd descriptors is [descs | tile_start (nd + 1) | strides (nd), only for batches with strided items |
-// page entries and BLOCKS items' slice addresses, only for batches with paged items | resolve jobs, only for batches
-// with BLOCKS items], and in the device copy only, behind it, the BLOCKS items' page entries, which the resolve kernel
-// writes: the host neither fills nor copies them.
+// page entries, SEGMENTS items' segment entries and BLOCKS items' slice addresses, only for batches with paged or
+// segmented items | resolve jobs, only for batches with BLOCKS items], and in the device copy only, behind it, the BLOCKS
+// items' page entries, which the resolve kernel writes: the host neither fills nor copies them.  The page entries start
+// 16-byte aligned, so that the kernels load a segment entry as one uint4.
 size_t stride_table_offset(size_t nd) { return (nd * sizeof(XferDesc) + (nd + 1) * 4 + 7) & ~size_t{7}; }
-size_t page_table_offset(size_t nd) { return stride_table_offset(nd) + nd * sizeof(XferStride); }
+size_t page_table_offset(size_t nd) { return (stride_table_offset(nd) + nd * sizeof(XferStride) + 15) & ~size_t{15}; }
 }  // namespace
 
 struct XferEngine::Slot {
@@ -92,8 +93,9 @@ struct XferEngine::Slot {
     std::memcpy(h_tab + stride_table_offset(nd), strides.data(), static_cast<size_t>(nd) * sizeof(XferStride));
     return stride_table_offset(nd) + static_cast<size_t>(nd) * sizeof(XferStride);
   }
-  // The page entries of the batch's XFER_PAGED descriptors, back to back; each one's stride entry holds the index of its
-  // first entry here until write_pages() turns it into a device address.
+  // The page entries of the batch's XFER_PAGED descriptors and the segment entries of its XFER_SEGMENTS ones (two words
+  // each, at an even index), back to back; each one's stride entry holds the index of its first entry here until
+  // write_pages() turns it into a device address.
   std::vector<uint64_t> pages;
   std::vector<uint32_t> paged_descs;
   // The resolve jobs of the batch's BLOCKS descriptors; their outer pointers hold indices into `pages`, their entries
@@ -112,11 +114,21 @@ struct XferEngine::Slot {
   }
   // The table entry of descriptor k's gathered or scattered layout (in bytes, over nbytes): its pattern, or its page
   // entries, or for blocks room for them and a resolve job (`get`: the scattering side), with the in-page row pattern of
-  // either.  Returns the XFER_PAGED flag for pages and blocks (and XFER_PAGE_ROWS with a pattern), 0 for rows.
+  // either, or the segment entries its bytes touch and the sentinel after them.  Returns the XFER_PAGED flag for pages
+  // and blocks (and XFER_PAGE_ROWS with a pattern), XFER_SEGMENTS for segments, 0 for rows.  O(segments), not O(tiles).
   uint32_t set_layout(uint32_t k, const DeviceLayout& m, uint64_t nbytes, bool get) {
     if (m.kind() == DeviceLayout::ROWS) {
       set_stride(k, XferStride{m.rows().pitch, m.rows().width, m.rows().phase});
       return 0;
+    }
+    if (m.kind() == DeviceLayout::SEGMENTS) {
+      const SourceSegments& g = m.segments();  // rebased: entry 0 holds byte 0
+      const uint64_t n = g.segments_for(nbytes);
+      if (pages.size() % 2) pages.push_back(0);
+      paged_descs.push_back(k);
+      set_stride(k, XferStride{{pages.size()}, n, g.phase});
+      for (uint64_t j = 0; j <= n; ++j) pages.push_back(g.entries[j].start), pages.push_back(g.entries[j].addr);
+      return XFER_SEGMENTS;
     }
     if (m.kind() == DeviceLayout::PAGES) {
       const SourcePages& p = m.pages();
@@ -540,9 +552,10 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
       return ErrorCode::INVALID_ARGUMENT;
     // a layout is the gathering load's source or the scattering store's destination, the side its flag names
     const bool blocks = it.mem.kind() == DeviceLayout::BLOCKS;
-    // XFER_PAGE_ROWS and XFER_WINDOW_ROWS are the engine's to set, from the layout (set_layout, and a WINDOW_ROWS layout
-    // below): a caller's flag would send a descriptor without its pattern down the in-page row walk or the windowed store
-    if (it.flags & (XFER_PAGE_ROWS | XFER_WINDOW_ROWS)) return ErrorCode::INVALID_ARGUMENT;
+    // XFER_PAGE_ROWS, XFER_WINDOW_ROWS and XFER_SEGMENTS are the engine's to set, from the layout (set_layout, and a
+    // WINDOW_ROWS layout below): a caller's flag would send a descriptor without its table down the in-page row walk, the
+    // windowed store or the segment walk
+    if (it.flags & (XFER_PAGE_ROWS | XFER_WINDOW_ROWS | XFER_SEGMENTS)) return ErrorCode::INVALID_ARGUMENT;
     // The one scattering store with a window: into rows of the window's result (WindowRows).  Without a window those are
     // the object's own rows.
     const bool wrows = scatter && win && it.mem.kind() == DeviceLayout::WINDOW_ROWS;

@@ -46,7 +46,10 @@ struct XferItem {
   // of the base.  Blocks (SourceBlocks) take XFER_PAGED too: their ids stay on the device, the resolve kernel builds the
   // page entries on `stream` before the transfer kernel, and its verdict comes back in XferResult::verdict; a
   // scattering store's n_blocks (and n_stored) beyond SourceBlocks::kMaxDistinct is NOT_IMPLEMENTED.  The ids must be
-  // ready on `stream` (stream order), and the outer array need only live until submit() returns.
+  // ready on `stream` (stream order), and the outer array need only live until submit() returns.  Segments
+  // (SourceSegments) take XFER_SEGMENTS, which submit() sets (among the caller's flags it is INVALID_ARGUMENT): the entries
+  // the item's bytes touch are copied into the batch's device table like page entries, a get's null segments are read and
+  // hashed but not stored, a put's are INVALID_ARGUMENT.
   DeviceLayout mem;
 };
 
@@ -84,7 +87,8 @@ struct Fp8Item {
   // INVALID_ARGUMENT with a window, unless mem.valid(n_elems) (a pack: mem.valid_source(n_elems)), or when its wide-byte
   // arithmetic overflows;
   // INVALID_ADDRESS unless it is co-aligned in wide bytes (DeviceLayout::coaligned of b * n_elems), which replaces the
-  // 16-byte alignment check of `wide`.  Blocks as XferItem's, the verdict in XferResult::verdict.
+  // 16-byte alignment check of `wide`.  Blocks as XferItem's, the verdict in XferResult::verdict.  Segments are
+  // INVALID_ARGUMENT: there are no MXFP8 segment transfers.
   DeviceLayout mem;
 };
 

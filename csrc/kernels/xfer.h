@@ -71,6 +71,17 @@ enum XferFlags : uint32_t {
   // WINDOW_ROWS layout); never with XFER_SCATTER, XFER_GATHER, XFER_PAGED, XFER_MULTIMEM or XFER_RAW_SUM.  Every tile
   // is still loaded and hashed, so the digest and the verify are those of a plain get.
   XFER_WINDOW_ROWS = 1u << 10,
+  // Segmented source or destination (SourceSegments, common/store_window.h), in bb_xfer only, together with XFER_GATHER
+  // (a put reads its segments) or XFER_SCATTER (a get stores into them): the object is the concatenation of segments of
+  // any sizes, object byte x at addr[k] + (x - start[k]) for the segment k with start[k] <= x < start[k + 1].  The
+  // descriptor's XferStride entry is {device address of its first segment entry, number of segments, object offset of the
+  // descriptor's byte 0}; the entries are 16-byte SegmentEntry {start, addr} pairs followed by one whose start ends the
+  // last segment.  `src` (put) or dst[0] (get) is not read.  Per tile the walking warp finds the tile's first segment by a
+  // 32-way search and takes the segments that overlap the tile one per lane.  A get's segment whose address is 0 is not
+  // stored (a null segment).  Only the engine sets it (from a SEGMENTS layout); never with XFER_PAGED, XFER_PAGE_ROWS,
+  // XFER_WINDOW, XFER_STRIDED, XFER_WINDOW_ROWS or XFER_RAW_SUM.  The tile in shared memory is the dense object's tile,
+  // so the digest, the verify and the stored bytes are those of a contiguous put or get of the concatenation.
+  XFER_SEGMENTS = 1u << 11,
 };
 
 // 64-byte transfer descriptor, one per (object shard, direction).
@@ -109,11 +120,14 @@ static_assert(offsetof(XferDesc, win.lo) == offsetof(XferDesc, dst) + 8 && offse
 // XFER_PAGE_ROWS descriptors: 0 < row_width < row_pitch, page % row_width == 0, (row_pitch - row_width) % 16 == 0.  An
 // XFER_WINDOW_ROWS descriptor's entry holds its window pattern (XFER_STRIDED only) in the first three words and its
 // destination rows in the last three: 0 < row_width < row_pitch, row_phase < row_width, and every stored byte's
-// destination congruent to its object offset mod 16 (WindowRows::coaligned).
+// destination congruent to its object offset mod 16 (WindowRows::coaligned).  An XFER_SEGMENTS descriptor's entry is
+// {segs, nseg, phase}: `segs` (in `pages`) the 16-byte aligned device address of its first segment entry, `nseg` (in
+// `width`) the segments its bytes touch, `phase` the object offset of its byte 0, and every non-null segment co-aligned:
+// addr[k] + phase - start[k] 16-byte aligned (SourceSegments::coaligned).
 struct XferStride {
   union {
     uint64_t pitch;
-    uint64_t pages;  // XFER_PAGED
+    uint64_t pages;  // XFER_PAGED; XFER_SEGMENTS: the segment entries
   };
   uint64_t width, phase;
   uint64_t row_width = 0, row_pitch = 0;  // XFER_PAGE_ROWS, XFER_WINDOW_ROWS

@@ -187,25 +187,68 @@ template <bool PAGED, bool ROWS>
 __device__ __forceinline__ uint64_t dense_row(const XferStride& st) {
   return PAGED && ROWS ? st.row_width : st.width;
 }
+// Segments (XFER_SEGMENTS, entry {segs, nseg, phase}): entry k of the table is the 16-byte {start, addr} of segment k,
+// entry nseg's start ends the last one.
+__device__ __forceinline__ uint64_t seg_start(const XferStride& st, uint64_t k) {
+  return __ldg(reinterpret_cast<const unsigned long long*>(st.pages) + 2 * k);
+}
+// Calls f(a, g, null) for every segment of the segment table `st` that the tile of `bytes` bytes at descriptor offset
+// `off` overlaps: g is its tile-relative span, tile byte o of it lives at a + o (a = addr - start + phase + off), and
+// `null` marks a null segment (address 0).  The warp finds the segment holding the tile's first byte by a 32-way search (each lane loads one
+// start per step, a ballot picks the last one at or before the byte), then takes the overlapping segments one per lane,
+// so that a tile of thousands of short segments keeps every lane busy; a segment over many tiles is one span per tile.
+// The whole warp calls it.
+template <class F>
+__device__ __forceinline__ void for_table_segments(uint64_t off, uint32_t bytes, const XferStride& st, uint32_t lane, F&& f) {
+  constexpr uint32_t kAll = 0xffffffffu;
+  const uint64_t g0 = st.phase + off, g1 = g0 + bytes;
+  uint64_t k0 = 0, cnt = st.width;  // segment entries [k0, k0 + cnt) hold g0, the first at or before it
+  while (cnt > 1) {
+    const uint64_t step = (cnt + 31) / 32, k = k0 + lane * step;
+    const uint32_t le = __ballot_sync(kAll, k < k0 + cnt && seg_start(st, k) <= g0);
+    const uint32_t j = 31 - __clz(le);  // lane 0's entry always starts at or before g0
+    k0 += j * step;
+    cnt = min(step, cnt - j * step);
+  }
+  for (uint64_t b = k0;; b += 32) {
+    const uint64_t k = b + lane;
+    uint64_t s0 = 0;
+    const bool in = k < st.width && (s0 = seg_start(st, k)) < g1;
+    if (in) {
+      const uint4 e = __ldg(reinterpret_cast<const uint4*>(st.pages) + k);
+      const uint64_t addr = (static_cast<uint64_t>(e.w) << 32) | e.z, s1 = seg_start(st, k + 1);
+      const uint32_t x0 = s0 > g0 ? static_cast<uint32_t>(s0 - g0) : 0u;
+      const uint32_t x1 = static_cast<uint32_t>(min(s1, g1) - g0);
+      f(addr - s0 + g0, span_parts(x0, x1), addr == 0);
+    }
+    if (__ballot_sync(kAll, in) != kAll) break;
+  }
+}
 // The producer's part of a gathered tile: the row segments of the tile, one per lane, the middle bulk-loaded into `tile`
 // with completion on `bar`, head and tail by plain loads and shared stores.  Returns the bytes this lane's bulk loads
 // deliver; the caller sums them over the warp for the stage's expect_tx, and the calling lane still has to fence its
 // shared stores for the async proxy.  PAGED: the rows are the pages of an XFER_PAGED descriptor (row_addr), or with ROWS
-// their in-page rows.
-template <bool PAGED = false, bool ROWS = false>
+// their in-page rows.  SEGS: the segments of an XFER_SEGMENTS descriptor (for_table_segments) instead of rows.
+template <bool PAGED = false, bool ROWS = false, bool SEGS = false>
 __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t* bar, uint64_t src, uint64_t off, uint32_t bytes,
                                                         const XferStride& st, uint32_t lane) {
   uint32_t tx = 0;
-  const uint64_t w = dense_row<PAGED, ROWS>(st);
-  for_row_segments(off, 0, bytes, XferStride{{w}, w, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
-    const uint8_t* s = reinterpret_cast<const uint8_t*>(row_addr<PAGED, ROWS>(src, off, r, st));
+  auto load = [&](const uint8_t* s, const TileSpan& g) {
     if (g.a1 > g.a0) {
       ptx::bulk_g2s(tile + g.a0, s + g.a0, g.a1 - g.a0, bar);
       tx += g.a1 - g.a0;
     }
     for (uint32_t o = g.x0; o < g.h1; ++o) tile[o] = s[o];
     for (uint32_t o = g.tb; o < g.x1; ++o) tile[o] = s[o];
-  });
+  };
+  if constexpr (SEGS) {
+    for_table_segments(off, bytes, st, lane, [&](uint64_t a, const TileSpan& g, bool) { load(reinterpret_cast<const uint8_t*>(a), g); });
+  } else {
+    const uint64_t w = dense_row<PAGED, ROWS>(st);
+    for_row_segments(off, 0, bytes, XferStride{{w}, w, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
+      load(reinterpret_cast<const uint8_t*>(row_addr<PAGED, ROWS>(src, off, r, st)), g);
+    });
+  }
   return tx;
 }
 // The store warp's part of a scattered tile (XFER_SCATTER, destination rows `st`), the mirror of gather_row_segments: the
@@ -214,10 +257,17 @@ __device__ __forceinline__ uint32_t gather_row_segments(uint8_t* tile, uint64_t*
 // the pattern's row 0 starts.  The calling lane still has to commit its bulk group and wait on it.  PAGED: the rows are
 // the pages of an XFER_PAGED descriptor (row_addr), dst0 is not read, and a page whose entry is 0 is not stored (the null
 // page of SourcePages): its lane stores nothing and still commits its empty bulk group.  ROWS: the segments are the
-// pages' in-page rows, and row r's page is r / (page / row_width).
-template <bool PAGED = false, bool ROWS = false>
+// pages' in-page rows, and row r's page is r / (page / row_width).  SEGS: the segments of an XFER_SEGMENTS descriptor
+// (for_table_segments), a null segment's lane storing nothing as a null page's.
+template <bool PAGED = false, bool ROWS = false, bool SEGS = false>
 __device__ __forceinline__ void scatter_row_segments(const uint8_t* tile, uint64_t dst0, uint64_t off, uint32_t bytes,
                                                      const XferStride& st, uint32_t lane) {
+  if constexpr (SEGS) {
+    for_table_segments(off, bytes, st, lane, [&](uint64_t a, const TileSpan& g, bool null) {
+      if (!null) store_segment(reinterpret_cast<uint8_t*>(a), tile, g);
+    });
+    return;
+  }
   const uint64_t w = dense_row<PAGED, ROWS>(st);
   for_row_segments(off, 0, bytes, XferStride{{w}, w, st.phase}, lane, [&](uint64_t r, const TileSpan& g) {
     if (PAGED && page_entry(st, ROWS ? r / (st.width / st.row_width) : r) == 0) return;

@@ -10,14 +10,16 @@
 //                      The source may be local HBM (put) or a peer GPU's slab over NVLink (get).  A gathering load
 //                      (XFER_GATHER: a put of a strided source) fills the tile from its source row segments, one per
 //                      lane, so the tile is byte for byte the tile of the dense object.  A paged one (XFER_PAGED)
-//                      reads each row segment from its page, whose address it loads from the page table.
+//                      reads each row segment from its page, whose address it loads from the page table; a
+//                      segmented one (XFER_SEGMENTS) each segment overlapping the tile from the segment table.
 //   warp 2  store    : `cp.async.bulk` shared -> global to 1..3 destinations (local or
 //                      peer-mapped: replica fan-out with a single HBM read), or `multimem.st`
 //                      to an NVLS multicast address (one store, N replicas).  A store window (XFER_WINDOW) cuts
 //                      each tile to its span; a strided one (XFER_STRIDED) to its row segments, one per lane.  A
 //                      scattering store (XFER_SCATTER: a get into a strided destination) stores the whole tile as
 //                      the row segments of the destination rows, one per lane; a paged one (XFER_PAGED) as the
-//                      segments of its pages.  A windowed one (XFER_WINDOW_ROWS) cuts the window's segments at the
+//                      segments of its pages, a segmented one (XFER_SEGMENTS) as the tile's parts of its segments.
+//                      A windowed one (XFER_WINDOW_ROWS) cuts the window's segments at the
 //                      destination rows of the dense result.
 //   warp 3  finalizer: folds the per-tile partials into per-object digests in registers; an
 //                      object that lives entirely inside this CTA's run is finalised with no
@@ -304,7 +306,8 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
           // in-page rows (XFER_PAGE_ROWS, never inline): their pattern is read here, so that `gst` stays three words
           const uint32_t gfl = e.m.ndst_flags >> 8;
           const uint32_t seg_tx =
-              gfl & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.tile[stage], &s.full[stage], src_i, off, bytes,
+              gfl & XFER_SEGMENTS  ? gather_row_segments<false, false, true>(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane)
+              : gfl & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.tile[stage], &s.full[stage], src_i, off, bytes,
                                                                      load_stride(p.strides, g_desc, true), lane)
               : gfl & XFER_PAGED   ? gather_row_segments<true>(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane)
                                    : gather_row_segments(s.tile[stage], &s.full[stage], src_i, off, bytes, gst, lane);
@@ -363,7 +366,8 @@ __global__ void __launch_bounds__(kThreads, resident_ctas(kStages)) bb_xfer_kern
           if (p.use_inline) st = p.inl_strides[st_desc];
           else st = load_stride(p.strides, st_desc);
         }
-        if (flags & XFER_PAGE_ROWS) scatter_row_segments<true, true>(s.tile[stage], m.dst[0], off, m.bytes, load_stride(p.strides, st_desc, true), lane);
+        if (flags & XFER_SEGMENTS) scatter_row_segments<false, false, true>(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
+        else if (flags & XFER_PAGE_ROWS) scatter_row_segments<true, true>(s.tile[stage], m.dst[0], off, m.bytes, load_stride(p.strides, st_desc, true), lane);
         else if (flags & XFER_PAGED) scatter_row_segments<true>(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
         else if (flags & XFER_SCATTER) scatter_row_segments(s.tile[stage], m.dst[0], off, m.bytes, st, lane);
         else store_row_segments(s.tile[stage], m.dst[0], off, x0, x1, st, lane);

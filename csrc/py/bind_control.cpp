@@ -74,6 +74,29 @@ std::vector<client::PageRows> to_page_rows(const py::object& rows) {
   for (auto h : py::cast<py::sequence>(rows)) out.push_back(h.is_none() ? client::PageRows{} : h.cast<client::PageRows>());
   return out;
 }
+// A segment list given as (address, bytes) pairs: a list of pairs, or an (n, 2) integer numpy array or CPU tensor, copied
+// as a block.
+std::vector<SourceSegments::Segment> to_segments(const py::handle& h) {
+  auto a = py::array_t<uint64_t, py::array::c_style | py::array::forcecast>::ensure(h);
+  if (!a) throw py::type_error("a segment list is (address, bytes) pairs: a list of pairs or an (n, 2) integer array");
+  if (a.size() == 0) return {};
+  if (a.ndim() != 2 || a.shape(1) != 2) throw py::value_error("a segment list is (address, bytes) pairs, shape (n, 2)");
+  std::vector<SourceSegments::Segment> out(static_cast<size_t>(a.shape(0)));
+  for (size_t k = 0; k < out.size(); ++k) out[k] = {a.data()[2 * k], a.data()[2 * k + 1]};
+  return out;
+}
+std::vector<std::vector<SourceSegments::Segment>> to_segment_lists(const py::sequence& s) {
+  std::vector<std::vector<SourceSegments::Segment>> out;
+  out.reserve(s.size());
+  for (auto h : s) out.push_back(to_segments(h));
+  return out;
+}
+// SourceSegments for Python: the table owns its entries (a rebased table shares them).
+struct PySegments {
+  std::shared_ptr<const std::vector<SegmentEntry>> table;
+  SourceSegments g;
+};
+
 // SourcePages for Python: the table owns its page addresses (a rebased table shares them).  SourceBlocks is PyBlocks
 // (py/py_blocks.h), shared with the engine's bindings.
 struct PyPages {
@@ -520,6 +543,53 @@ void bind_control(py::module_& m) {
            py::arg("len"),
            "[(x, addr, n)]: object bytes [x, x + n) live at [addr, addr + n); one per page or in-page row, adjacent ones make "
            "one run");
+
+  py::class_<PySegments>(m, "SourceSegments",
+                         "An object that is the concatenation of segments of any sizes at arbitrary addresses: a segment put's "
+                         "source, or a segment get's destination (common/store_window.h).  Segment k holds object bytes "
+                         "[start[k], start[k] + len[k]), start the exclusive prefix sum, and object byte x lives at addr[k] + (x - "
+                         "start[k]).  Byte x of a rebased table is object byte phase + x.")
+      .def_property_readonly("nseg", [](const PySegments& t) { return t.g.nseg; })
+      .def_property_readonly("phase", [](const PySegments& t) { return t.g.phase; })
+      .def_property_readonly("total", [](const PySegments& t) { return t.g.total(); })
+      .def_property_readonly("entries",
+                             [](const PySegments& t) {
+                               std::vector<std::pair<uint64_t, uint64_t>> out;
+                               for (uint64_t k = 0; t.g.segmented() && k <= t.g.nseg; ++k) out.emplace_back(t.g.entries[k].start, t.g.entries[k].addr);
+                               return out;
+                             },
+                             "[(start, addr)] of the segments from entry 0, then the sentinel (total, 0)")
+      .def("segmented", [](const PySegments& t) { return t.g.segmented(); })
+      .def("valid", [](const PySegments& t, uint64_t len) { return t.g.valid(len); }, py::arg("len"))
+      .def("has_null", [](const PySegments& t, uint64_t len) { return t.g.has_null(len); }, py::arg("len"),
+           "whether a segment that bytes [0, len) touch has address 0 (not stored by a get, refused by a put)")
+      .def("segments_for", [](const PySegments& t, uint64_t len) { return t.g.segments_for(len); }, py::arg("len"))
+      .def_static("from_segments",
+                  [](const py::handle& segs) {
+                    const auto v = to_segments(segs);
+                    auto table = std::make_shared<std::vector<SegmentEntry>>();
+                    PySegments t;
+                    uint64_t size = 0;
+                    const ErrorCode ec = SourceSegments::from_segments(v.data(), v.size(), table.get(), &t.g, &size);
+                    t.table = table;
+                    return py::make_tuple(ec, t, size);
+                  },
+                  py::arg("segments"), "(ErrorCode, SourceSegments, object bytes) of (address, bytes) pairs")
+      .def("rebase", [](const PySegments& t, uint64_t off) { return PySegments{t.table, t.g.rebase(off)}; }, py::arg("off"),
+           "the table seen from byte off")
+      .def("coaligned", [](const PySegments& t, uint64_t len) { return t.g.coaligned(len); }, py::arg("len"))
+      .def("fused_get_aligned", [](const PySegments& t, uint64_t off, uint64_t len) { return t.g.fused_get_aligned(off, len); },
+           py::arg("off"), py::arg("len"))
+      .def("runs",
+           [](const PySegments& t, uint64_t len) {
+             if (len > 0 && !t.g.valid(len)) throw py::value_error("the table does not hold len bytes");
+             std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> out;
+             t.g.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { out.emplace_back(x, at, n); });
+             return out;
+           },
+           py::arg("len"),
+           "[(x, addr, n)]: bytes [x, x + n) live at [addr, addr + n); segments adjacent in memory make one run, null segments "
+           "none");
 
   py::class_<PyBlocks>(m, "DeviceBlocks",
                        "Pages of a paged KV cache named by block ids that stay on the device (SourceBlocks, common/store_window.h): "
@@ -1560,6 +1630,27 @@ void bind_control(py::module_& m) {
          "* page_bytes[i]); every shard is read whole and verified, only the object's bytes are written; a page address "
          "of 0 is not stored (a partial restore: the table still covers the whole object); pages of one get must not "
          "overlap (not checked); rows as batch_put_device_paged's, and then no byte outside the rows is written; returns "
+         "(one ErrorCode per object, object sizes).")
+      .def("batch_put_device_segments", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& segments,
+                                           const WorkerConfig& cfg, uintptr_t stream) {
+        const auto lists = to_segment_lists(segments);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_segments(keys, lists, cfg, reinterpret_cast<void*>(stream)); }));
+      }, py::arg("keys"), py::arg("segments"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0,
+         "Object i = the segments segments[i] concatenated in order, each an (address, bytes) pair (a list of pairs or an "
+         "(n, 2) integer array); one object and one digest set per list, stored as a put of the concatenation would store "
+         "it.  Zero-length segments are dropped; a segment at address 0 is INVALID_ARGUMENT and a total past 2**64 "
+         "VALUE_OUT_OF_RANGE for that object.  Segments whose address is congruent to their object offset mod 16 are read "
+         "in place by the fused put kernel, others are staged through the host; returns one ErrorCode per object.")
+      .def("batch_get_device_segments", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& segments,
+                                           uintptr_t stream) {
+        const auto lists = to_segment_lists(segments);
+        std::vector<size_t> sizes;
+        const auto ecs = nogil([&] { return c.batch_get_device_segments(keys, lists, reinterpret_cast<void*>(stream), &sizes); });
+        return py::make_tuple(ecs_to_py(ecs), sizes);
+      }, py::arg("keys"), py::arg("segments"), py::arg("stream") = 0,
+         "Object i into the segments segments[i] in order (capacity: the sum of the lengths, null segments included; a "
+         "larger object is BUFFER_OVERFLOW, a shorter one fills the segments in order); every shard is read whole and "
+         "verified, only the object's bytes are written; a segment at address 0 is not stored (a partial restore); returns "
          "(one ErrorCode per object, object sizes).")
       .def("batch_put_device_blocks", [](BlackbirdClient& c, const std::vector<std::string>& keys, const std::vector<PyBlocks>& blocks,
                                          const WorkerConfig& cfg, uintptr_t stream) {

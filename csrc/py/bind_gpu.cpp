@@ -47,18 +47,34 @@ bool to_window(const py::handle& h, StoreWindow* win) {
   win->phase = w[4];
   return true;
 }
+// What a batch's layouts point into until it has been submitted: page addresses and segment tables.
+struct Keep {
+  std::deque<std::vector<uint64_t>> pages;
+  std::deque<std::vector<SegmentEntry>> segments;
+};
 // The layout slots of an item tuple (common/store_window.h), first to last: gather rows, scatter rows, source pages,
-// destination pages, source blocks and destination blocks.  Rows are given as (pitch, width, phase), pages as (addrs,
-// page, phase), whose addresses are kept in `keep` until the batch has been submitted, blocks as a DeviceBlocks.  Returns
-// the slot set, -1 for none (even: the source side); an item takes one layout, so a second slot is the engine's
-// INVALID_ARGUMENT, raised as `what`.
-int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vector<uint64_t>>& keep, DeviceLayout* out, const char* what) {
+// destination pages, source blocks, destination blocks, source segments and destination segments.  Rows are given as
+// (pitch, width, phase), pages as (addrs, page, phase), whose addresses are kept in `keep` until the batch has been
+// submitted, blocks as a DeviceBlocks, segments as (segments, off): the (address, bytes) pairs of the whole object
+// (SourceSegments::from_segments, its table kept in `keep`) seen from object byte off (rebase).  Returns the slot set, -1
+// for none (even: the source side); an item takes one layout, so a second slot is the engine's INVALID_ARGUMENT, raised
+// as `what`.
+int to_layout(const py::tuple& t, const size_t (&slots)[8], Keep& keep, DeviceLayout* out, const char* what) {
   int set = -1;
-  for (int k = 0; k < 6; ++k) {
+  for (int k = 0; k < 8; ++k) {
     if (t.size() <= slots[k] || t[slots[k]].is_none()) continue;
     if (set >= 0) check(ErrorCode::INVALID_ARGUMENT, what);
     set = k;
-    if (k < 2) {
+    if (k >= 6) {
+      auto g = py::cast<py::tuple>(t[slots[k]]);
+      if (g.size() != 2) throw py::value_error("segments = ([(addr, bytes), ...], off)");
+      const auto pairs = g[0].cast<std::vector<std::pair<uint64_t, uint64_t>>>();
+      keep.segments.emplace_back();
+      SourceSegments seg;
+      uint64_t size = 0;
+      check(SourceSegments::from_segments(pairs.data(), pairs.size(), &keep.segments.back(), &seg, &size), what);
+      *out = DeviceLayout(seg.rebase(std::min(g[1].cast<uint64_t>(), size)));
+    } else if (k < 2) {
       auto g = t[slots[k]].cast<std::vector<uint64_t>>();
       if (g.size() != 3) throw py::value_error("gather / scatter = (pitch, width, phase)");
       *out = DeviceLayout(SourceRows{g[0], g[1], g[2]});
@@ -67,8 +83,8 @@ int to_layout(const py::tuple& t, const size_t (&slots)[6], std::deque<std::vect
     } else {
       auto p = py::cast<py::tuple>(t[slots[k]]);
       if (p.size() != 3 && p.size() != 5) throw py::value_error("pages = (addrs, page, phase[, row_width, row_pitch])");
-      keep.push_back(p[0].cast<std::vector<uint64_t>>());
-      *out = DeviceLayout(SourcePages{keep.back().data(), keep.back().size(), p[1].cast<uint64_t>(), p[2].cast<uint64_t>(),
+      keep.pages.push_back(p[0].cast<std::vector<uint64_t>>());
+      *out = DeviceLayout(SourcePages{keep.pages.back().data(), keep.pages.back().size(), p[1].cast<uint64_t>(), p[2].cast<uint64_t>(),
                                       p.size() == 5 ? p[3].cast<uint64_t>() : 0, p.size() == 5 ? p[4].cast<uint64_t>() : 0});
     }
   }
@@ -86,14 +102,16 @@ bool to_window_rows(const py::tuple& t, size_t slot, int k, DeviceLayout* out) {
   return true;
 }
 // item tuple: (src, dst | [dst...], nbytes, expect=0, flags=0, tile_base=0, window=None, gather=None, scatter=None,
-// source pages=None, destination pages=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
+// source pages=None, destination pages=None, source blocks=None, destination blocks=None, window rows=None, source
+// segments=None, destination segments=None).  An empty destination list makes a hash-only XFER_RAW_SUM descriptor (the engine rejects
 // it without that flag).  A window sets XFER_WINDOW, and one with a pattern XFER_STRIDED as well.  A gather pattern
 // (pitch, width, phase) sets XFER_GATHER, with src = row 0; a scatter pattern XFER_SCATTER, with dst = row 0.  Source
 // pages (addrs, page, phase[, row_width, row_pitch]) set XFER_GATHER | XFER_PAGED, destination pages
-// XFER_SCATTER | XFER_PAGED (with an in-page row pattern also XFER_PAGE_ROWS).  At most one of the four.
-XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
+// XFER_SCATTER | XFER_PAGED (with an in-page row pattern also XFER_PAGE_ROWS).  Source segments set XFER_GATHER,
+// destination segments XFER_SCATTER (the engine adds XFER_SEGMENTS).  At most one layout.
+XferItem to_item(const py::handle& h, Keep& keep) {
   py::tuple t = py::cast<py::tuple>(h);
-  if (t.size() < 3 || t.size() > 14)
+  if (t.size() < 3 || t.size() > 16)
     throw py::value_error(
         "xfer item = (src, dst|[dst..], nbytes[, expect[, flags[, tile_base[, (lo, hi)[, gather (pitch, width, phase)[, scatter "
         "(pitch, width, phase)[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]]])");
@@ -105,9 +123,9 @@ XferItem to_item(const py::handle& h, std::deque<std::vector<uint64_t>>& keep) {
   if (t.size() > 4) it.flags = t[4].cast<uint32_t>();
   if (t.size() > 5) it.tile_base = t[5].cast<uint32_t>();
   if (t.size() > 6 && !t[6].is_none()) it.flags |= to_window(t[6], &it.win) ? XFER_WINDOW | XFER_STRIDED : XFER_WINDOW;
-  static const uint32_t side[6] = {XFER_GATHER, XFER_SCATTER, XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED,
-                                   XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED};
-  const int k = to_layout(t, {7, 8, 9, 10, 11, 12}, keep, &it.mem, "XferEngine.submit");
+  static const uint32_t side[8] = {XFER_GATHER, XFER_SCATTER, XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED,
+                                   XFER_GATHER | XFER_PAGED, XFER_SCATTER | XFER_PAGED, XFER_GATHER, XFER_SCATTER};
+  const int k = to_layout(t, {7, 8, 9, 10, 11, 12, 14, 15}, keep, &it.mem, "XferEngine.submit");
   if (k >= 0) it.flags |= side[k];
   if (to_window_rows(t, 13, k, &it.mem)) it.flags |= XFER_SCATTER;
   return it;
@@ -133,6 +151,7 @@ void bind_gpu(py::module_& m) {
   m.attr("XFER_PAGED") = static_cast<uint32_t>(XFER_PAGED);
   m.attr("XFER_PAGE_ROWS") = static_cast<uint32_t>(XFER_PAGE_ROWS);
   m.attr("XFER_WINDOW_ROWS") = static_cast<uint32_t>(XFER_WINDOW_ROWS);
+  m.attr("XFER_SEGMENTS") = static_cast<uint32_t>(XFER_SEGMENTS);
   m.def("cuda_device_count", [] {
     int n = 0;
     device_count(&n);
@@ -149,7 +168,7 @@ void bind_gpu(py::module_& m) {
       .def("run",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream, bool debug) {
              std::vector<XferItem> v;
-             std::deque<std::vector<uint64_t>> keep;
+             Keep keep;
              v.reserve(items.size());
              for (auto h : items) v.push_back(to_item(h, keep));
              XferResult res;
@@ -181,11 +200,15 @@ void bind_gpu(py::module_& m) {
            "result (p = x - lo, or the strided window's result index) lands at dst + ((p + phase) // width) * pitch + (p + "
            "phase) % width, which the engine marks XFER_WINDOW_ROWS; returns (digests, status, "
            "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item (VALUE_OUT_OF_RANGE or "
-           "INVALID_ARGUMENT for refused ids).")
+           "INVALID_ARGUMENT for refused ids).  Source segments (pairs, off) as the fifteenth element set XFER_GATHER: "
+           "the object is the (address, bytes) pairs concatenated, seen from object byte off, and object byte x is read "
+           "from the segment holding off + x (src is not read); destination segments as the sixteenth set XFER_SCATTER "
+           "and store by the same rule, a segment at address 0 not stored (dst is not read).  The engine marks both "
+           "XFER_SEGMENTS.")
       .def("run_fp8",
            [](XferEngine& e, const py::list& items, bool unpack, uintptr_t stream, mxfp8::Wide wide) {
              std::vector<gpu::Fp8Item> v;
-             std::deque<std::vector<uint64_t>> keep;
+             Keep keep;
              for (auto h : items) {
                auto t = h.cast<py::tuple>();
                gpu::Fp8Item it;
@@ -198,7 +221,7 @@ void bind_gpu(py::module_& m) {
                it.more_packed[0] = packed[1];
                it.more_packed[1] = packed[2];
                it.n_elems = t[2].cast<uint64_t>();
-               if (t.size() < 3 || t.size() > 13)
+               if (t.size() < 3 || t.size() > 15)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
                      "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
@@ -206,7 +229,7 @@ void bind_gpu(py::module_& m) {
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
                // the gather slots are a pack's, the scatter slots an unpack's
-               const int k = to_layout(t, {5, 6, 8, 9, 10, 11}, keep, &it.mem, "XferEngine.run_fp8");
+               const int k = to_layout(t, {5, 6, 8, 9, 10, 11, 13, 14}, keep, &it.mem, "XferEngine.run_fp8");
                if (k >= 0 && (k % 2 == 1) != unpack) check(ErrorCode::INVALID_ARGUMENT, "XferEngine.run_fp8");
                to_window_rows(t, 12, k, &it.mem);
                v.push_back(it);
@@ -251,7 +274,7 @@ void bind_gpu(py::module_& m) {
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
              std::vector<XferItem> v;
-             std::deque<std::vector<uint64_t>> keep;
+             Keep keep;
              v.reserve(items.size());
              for (auto h : items) v.push_back(to_item(h, keep));
              auto t = e.submit(v, algo, reinterpret_cast<void*>(stream));
