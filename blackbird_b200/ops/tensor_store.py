@@ -1100,11 +1100,23 @@ class TensorStore:
 
     # ------------------------------------------------------------------ bundles
     def _gap_zeros(self, device: torch.device) -> torch.Tensor:
-        """32 zero bytes at a 16-byte aligned address on `device`: the source of every gap between a bundle's tensors."""
+        """144 zero bytes at a 16-byte aligned address on `device`: the source of every gap between a bundle's tensors, and
+        of a packed bundle's padding (up to 31 fp32 elements, 124 bytes, from an address up to 15 bytes in)."""
         cache = self.__dict__.setdefault("_gap_zero_bufs", {})
         if device not in cache:
-            cache[device] = torch.zeros(32, dtype=torch.uint8, device=device)
+            cache[device] = torch.zeros(144, dtype=torch.uint8, device=device)
         return cache[device]
+
+    @staticmethod
+    def _aligned(t: torch.Tensor, keep: list) -> torch.Tensor:
+        """t itself when it is contiguous and 16-byte aligned (or has no elements), else an aligned contiguous copy kept
+        alive in `keep`."""
+        if t.numel() and (not t.is_contiguous() or t.data_ptr() % 16):
+            t = t.clone(memory_format=torch.contiguous_format) if t.is_contiguous() else t.contiguous()
+            if t.data_ptr() % 16:  # a fresh allocation is aligned; this is a guard, not a route
+                t = torch.empty_like(t).copy_(t)
+            keep.append(t)
+        return t
 
     @staticmethod
     def _bundle_items(bundle, what: str) -> tuple:
@@ -1115,7 +1127,7 @@ class TensorStore:
             return "list", [(str(i), v) for i, v in enumerate(bundle)]
         raise TypeError(f"{what}: a bundle is a mapping of names to tensors or a sequence of tensors, not {type(bundle).__name__}")
 
-    def batch_put_bundles(self, keys: Sequence[str], bundles: Sequence, config=None) -> None:
+    def batch_put_bundles(self, keys: Sequence[str], bundles: Sequence, config=None, pack_fp8: bool = False) -> None:
         """Stores each bundle -- a mapping of names to CUDA tensors, such as a `state_dict`, or a sequence of them -- as
         ONE object under its key, with one `#meta`: the tensors back to back, each at a 16-byte aligned offset, read in
         place by the fused put kernel from a segment list (batch_put_device_segments), one native call for the batch.  A
@@ -1126,7 +1138,11 @@ class TensorStore:
         16-byte aligned is copied into an aligned temporary first.  Every dtype TensorStore knows is accepted, 0-d and
         zero-element tensors included.  TypeError for another dtype or a value that is not a tensor, ValueError for a
         tensor that is not a CUDA tensor on the current device; both before anything is stored.  The `#meta` records
-        each entry's name, dtype, shape, offset and bytes and the total."""
+        each entry's name, dtype, shape, offset and bytes and the total.
+
+        pack_fp8 stores each bundle as ONE MXFP8-packed object (see _put_packed_bundles): every entry of a bundle must
+        have the same dtype, bf16, fp16 or fp32 (TypeError otherwise), and a bundle needs at least one element
+        (ValueError), both before anything is stored."""
         cfg = config or self.config
         keys, bundles = list(keys), list(bundles)
         if len(keys) != len(bundles):
@@ -1134,6 +1150,9 @@ class TensorStore:
         plans = []
         for k, b in zip(keys, bundles):
             kind, items = self._bundle_items(b, k)
+            dts = {t.dtype for _, t in items if isinstance(t, torch.Tensor)}
+            if pack_fp8 and (len(dts) > 1 or not dts <= set(_MX_WIDE)):
+                raise TypeError(f"{k}: a packed bundle holds bfloat16, float16 or float32 tensors of one dtype, not {sorted(map(str, dts))}")
             for name, t in items:
                 if not isinstance(t, torch.Tensor):
                     raise TypeError(f"{k}[{name}]: not a tensor but {type(t).__name__}")
@@ -1141,18 +1160,19 @@ class TensorStore:
                     raise TypeError(f"{k}[{name}]: dtype {t.dtype} is not one TensorStore stores")
                 if not t.is_cuda or t.device.index != torch.cuda.current_device():
                     raise ValueError(f"{k}[{name}]: must be a CUDA tensor on the current device, not {t.device}")
+            if pack_fp8 and sum(t.numel() for _, t in items) == 0:
+                raise ValueError(f"{k}: a packed bundle needs at least one element")
             plans.append((kind, items))
+        if pack_fp8:
+            self._put_packed_bundles(keys, plans, cfg)
+            return
         zeros = self._gap_zeros(torch.device("cuda", torch.cuda.current_device())).data_ptr()
         segments, metas, keep = [], [], []
         for kind, items in plans:
             segs, entries, off = [], [], 0
             for name, t in items:
                 nbytes = t.numel() * t.element_size()
-                if nbytes and (not t.is_contiguous() or t.data_ptr() % 16):
-                    t = t.clone(memory_format=torch.contiguous_format) if t.is_contiguous() else t.contiguous()
-                    if t.data_ptr() % 16:  # a fresh allocation is aligned; this is a guard, not a route
-                        t = torch.empty_like(t).copy_(t)
-                    keep.append(t)
+                t = self._aligned(t, keep)
                 gap = -off % 16
                 if gap:
                     segs.append((zeros + off % 16, gap))
@@ -1168,25 +1188,104 @@ class TensorStore:
         _check("bundle put", keys, ecs)
         self._put_metas(keys, metas)
 
-    def put_bundle(self, key: str, tensors, config=None) -> None:
+    def _put_packed_bundles(self, keys: list, plans: list, cfg) -> None:
+        """The packed form of batch_put_bundles, for checked (kind, items) plans.  Each entry starts on a whole 32-element
+        MX block and is padded with zeros to a multiple of 32 elements, so its values never share a block scale with a
+        neighbour's: each entry decodes bit for bit to what put(k, t, pack_fp8=True) and get(k) give for it alone.  The
+        padding is read from the zeroed gap buffer at an address congruent to its wide-byte offset, and entries that are
+        not contiguous or not 16-byte aligned get an aligned temporary, so the fused pack reads the segment list in place
+        (batch_put_device_fp8_segments, one call per dtype) when the config is fusable.  Otherwise, and for bundles it
+        refuses with NOT_IMPLEMENTED, the entries are copied into a padded wide temporary, packed (mxfp8_pack) and put as
+        bytes: the stored object is byte for byte the same.  The `#meta` is the plain bundle's record, offsets and bytes in
+        wide bytes of the unpacked object, plus "packed", "dtype" and "numel", the padded element total."""
+        zeros = self._gap_zeros(torch.device("cuda", torch.cuda.current_device())).data_ptr()
+        segments, metas, dtypes, numels, keep = [], [], [], [], []
+        for kind, items in plans:
+            dt = items[0][1].dtype
+            es = dt.itemsize
+            segs, entries, off = [], [], 0  # off in elements
+            for name, t in items:
+                n = t.numel()
+                t = self._aligned(t, keep)
+                if n:
+                    segs.append((t.data_ptr(), n))
+                entries.append({"name": name, "dtype": str(dt).replace("torch.", ""), "shape": list(t.shape), "offset": es * off,
+                                "bytes": es * n})
+                off += n
+                pad = -off % 32
+                if pad:
+                    segs.append((zeros + es * off % 16, pad))
+                    off += pad
+            segments.append(np.array(segs, dtype=np.uint64).reshape(-1, 2))
+            metas.append({"bundle": kind, "entries": entries, "total": es * off, "packed": "mxfp8",
+                          "dtype": str(dt).replace("torch.", ""), "numel": off})
+            dtypes.append(dt)
+            numels.append(off)
+        idx = list(range(len(keys)))
+        if self._fusable_fp8_cfg(cfg):
+            def call(grp, es, wide):
+                return self.client.batch_put_device_fp8_segments([keys[i] for i in grp], [segments[i] for i in grp], cfg, self._stream(),
+                                                                 wide=wide)
+
+            idx = self._packed("packed bundle put", keys, idx, lambda i: dtypes[i], call)
+        if idx:
+            packed = []
+            for i in idx:
+                wide = torch.zeros(numels[i], dtype=dtypes[i], device=torch.device("cuda", torch.cuda.current_device()))
+                for (_, t), e in zip(plans[i][1], metas[i]["entries"]):
+                    if e["bytes"]:
+                        self._entry_view(wide.view(torch.uint8), e).copy_(t)
+                buf = torch.empty(_bb.mxfp8_packed_bytes(numels[i]), dtype=torch.uint8, device=wide.device)
+                _bb.mxfp8_pack(wide.data_ptr(), numels[i], buf.data_ptr(), self._stream(), wide=_MX_WIDE[dtypes[i]])
+                packed.append(buf)
+            ecs = self.client.batch_put_device([keys[i] for i in idx], [b.data_ptr() for b in packed], [b.numel() for b in packed], cfg,
+                                               self._stream())
+            _check("packed bundle put", [keys[i] for i in idx], ecs)
+        self._put_metas(keys, [json.dumps(m).encode() for m in metas])
+
+    def put_bundle(self, key: str, tensors, config=None, pack_fp8: bool = False) -> None:
         """Stores the mapping or sequence of CUDA tensors `tensors` as one object (see batch_put_bundles)."""
-        self.batch_put_bundles([key], [tensors], config)
+        self.batch_put_bundles([key], [tensors], config, pack_fp8)
 
     @staticmethod
     def _entry_view(buf: torch.Tensor, e: dict) -> torch.Tensor:
         dt = _DTYPES[e["dtype"]]
         return buf[e["offset"]: e["offset"] + e["bytes"]].view(dt).view(e["shape"])
 
+    def _packed_bundle_bufs(self, keys: list, metas: list, idx: list, bufs: list, device) -> None:
+        """Fills bufs[i], for each packed bundle i of idx, with its unpacked object as bytes: one fused unpack per dtype
+        (batch_get_device_fp8) into a wide allocation; a bundle it refuses with NOT_IMPLEMENTED is read packed
+        (batch_get_device) and unpacked by mxfp8_unpack."""
+        wides = {i: torch.empty(metas[i]["numel"], dtype=_stored_dtype(metas[i]), device=device) for i in idx}
+        for i in idx:
+            bufs[i] = wides[i].view(torch.uint8)
+
+        def call(grp, es, wide):
+            return self.client.batch_get_device_fp8([keys[i] for i in grp], [wides[i].data_ptr() for i in grp],
+                                                    [metas[i]["numel"] for i in grp], self._stream(), wide=wide)
+
+        rest = [i for i in idx if not self.client.device_fp8_eligible(metas[i]["numel"])]
+        rest += self._packed("packed bundle get", keys, [i for i in idx if i not in rest], lambda i: _stored_dtype(metas[i]), call)
+        if rest:
+            packed = [torch.empty(_bb.mxfp8_packed_bytes(metas[i]["numel"]), dtype=torch.uint8, device=device) for i in rest]
+            ecs, _ = self.client.batch_get_device([keys[i] for i in rest], [b.data_ptr() for b in packed], [b.numel() for b in packed],
+                                                  self._stream())
+            _check("packed bundle get", [keys[i] for i in rest], ecs)
+            for i, b in zip(rest, packed):
+                _bb.mxfp8_unpack(b.data_ptr(), metas[i]["numel"], wides[i].data_ptr(), self._stream(), wide=_MX_WIDE[_stored_dtype(metas[i])])
+
     def batch_get_bundles(self, keys: Sequence[str], device: Optional[torch.device] = None) -> list:
         """Each stored bundle in the container type it was stored as (a dict, or a list for a sequence), its tensors views
         of ONE aligned allocation per bundle that a single plain device get (batch_get_device) filled and verified: the
         views share that storage, so resizing one or keeping one alive keeps the whole bundle's allocation.  TypeError
-        for a key that holds a tensor, KeyError for a missing one."""
+        for a key that holds a tensor, KeyError for a missing one.  A packed bundle's allocation is its unpacked object,
+        filled by one fused unpack per dtype (see _packed_bundle_bufs); a batch may mix packed and plain bundles."""
         device = device or torch.device("cuda", torch.cuda.current_device())
         keys = list(keys)
         metas = self._metas(keys, bundle=True)
-        bufs = [torch.empty(max(m["total"], 1), dtype=torch.uint8, device=device) for m in metas]
-        idx = [i for i, m in enumerate(metas) if m["total"]]
+        bufs = [torch.empty(max(m["total"], 1), dtype=torch.uint8, device=device) if not m.get("packed") else None for m in metas]
+        self._packed_bundle_bufs(keys, metas, [i for i, m in enumerate(metas) if m.get("packed")], bufs, device)
+        idx = [i for i, m in enumerate(metas) if m["total"] and not m.get("packed")]
         if idx:
             ecs, _ = self.client.batch_get_device([keys[i] for i in idx], [bufs[i].data_ptr() for i in idx], [metas[i]["total"] for i in idx],
                                                   self._stream())
@@ -1207,7 +1306,9 @@ class TensorStore:
         the entries it does not name, and the gaps, are not stored.  Every bundle is one segment list of ONE
         batch_get_device_segments call: a contiguous 16-byte aligned out is a segment itself, any other out gets a
         contiguous temporary segment and then out.copy_(tmp).  Every shard of the object is still read whole and
-        verified.
+        verified.  Packed bundles take one batch_get_device_fp8_segments call per dtype instead, their segments in
+        elements (the padding is a null segment too); one it refuses with NOT_IMPLEMENTED is read whole (see
+        _packed_bundle_bufs) and copied into the outs.  A batch may mix packed and plain bundles.
 
         Every check comes before any transfer: KeyError for a missing key or name, TypeError for a key that holds a
         tensor or an out of another dtype than its entry, ValueError for another shape or an out that is not a CUDA
@@ -1235,26 +1336,46 @@ class TensorStore:
                     raise ValueError(f"{k}[{name}]: out must be a CUDA tensor on cuda:{dev}, not {t.device}")
             named.append(dict(items))
         segments, copies = [], []
-        for m, want in zip(metas, named):
+        for i, (m, want) in enumerate(zip(metas, named)):
+            es = _stored_dtype(m).itemsize if m.get("packed") else 1  # segments in elements of a packed bundle
             segs, off = [], 0
             for e in m["entries"]:
                 if e["offset"] > off:
-                    segs.append((0, e["offset"] - off))
+                    segs.append((0, (e["offset"] - off) // es))
                 t = want.get(e["name"])
                 if e["bytes"] and t is None:
-                    segs.append((0, e["bytes"]))
+                    segs.append((0, e["bytes"] // es))
                 elif e["bytes"]:
                     if not t.is_contiguous() or t.data_ptr() % 16:
                         tmp = torch.empty(e["shape"], dtype=t.dtype, device=t.device)
-                        copies.append((t, tmp))
+                        copies.append((i, t, tmp))
                         t = tmp
-                    segs.append((t.data_ptr(), e["bytes"]))
+                    segs.append((t.data_ptr(), e["bytes"] // es))
                 off = e["offset"] + e["bytes"]
+            if m["total"] > off:  # a packed bundle's last padding
+                segs.append((0, (m["total"] - off) // es))
             segments.append(np.array(segs, dtype=np.uint64).reshape(-1, 2))
-        ecs, _ = self.client.batch_get_device_segments(keys, segments, self._stream())
-        _check("bundle get", keys, ecs)
-        for t, tmp in copies:
-            t.copy_(tmp)
+        plain = [i for i, m in enumerate(metas) if not m.get("packed")]
+        if plain:
+            ecs, _ = self.client.batch_get_device_segments([keys[i] for i in plain], [segments[i] for i in plain], self._stream())
+            _check("bundle get", [keys[i] for i in plain], ecs)
+
+        def call(grp, es, wide):
+            ecs, _ = self.client.batch_get_device_fp8_segments([keys[i] for i in grp], [segments[i] for i in grp], self._stream(), wide=wide)
+            return ecs
+
+        packed = [i for i, m in enumerate(metas) if m.get("packed")]
+        rest = self._packed("packed bundle get", keys, packed, lambda i: _stored_dtype(metas[i]), call)
+        for i, t, tmp in copies:
+            if i not in rest:
+                t.copy_(tmp)
+        if rest:  # refused: the whole unpacked object, then each named entry copied out of it
+            bufs = [None] * len(keys)
+            self._packed_bundle_bufs(keys, metas, rest, bufs, torch.device("cuda", dev))
+            for i in rest:
+                for e in metas[i]["entries"]:
+                    if e["name"] in named[i] and e["bytes"]:
+                        named[i][e["name"]].copy_(self._entry_view(bufs[i], e))
         return outs
 
     def get_bundle_into(self, key: str, outs):
@@ -1362,11 +1483,11 @@ class AsyncTensorStore(TensorStore):
         return self._on_side(True, self.batch_get_layer_blocks_into, list(keys), caches, list(ids), dim,
                              None if blocks is None else list(blocks), result=caches)
 
-    def put_bundles_async(self, keys: Sequence[str], bundles: Sequence, config=None):
+    def put_bundles_async(self, keys: Sequence[str], bundles: Sequence, config=None, pack_fp8: bool = False):
         """batch_put_bundles on the side stream, ordered after the work already queued on the caller's stream; the future
         yields the number of bundles stored, or raises the call's error."""
         keys, bundles = list(keys), list(bundles)  # keep the tensors alive until the transfer is done
-        return self._on_side(True, self.batch_put_bundles, keys, bundles, config, result=len(keys))
+        return self._on_side(True, self.batch_put_bundles, keys, bundles, config, pack_fp8, result=len(keys))
 
     def get_bundles_into_async(self, keys: Sequence[str], outs: Sequence):
         """batch_get_bundles_into on the side stream, ordered after the work already queued on the caller's stream; the

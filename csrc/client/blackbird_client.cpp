@@ -638,8 +638,8 @@ std::vector<ErrorCode> BlackbirdClient::shaped_batch(std::string_view name, bool
 }
 
 // What the builder of a shaped put or get makes of item i: the layout of the caller's side and the object's size, in
-// bytes or, for MXFP8, in elements of the wide side.  `table`: the size is that of a page table (pages or blocks), not of
-// rows.
+// bytes or, for MXFP8, in elements of the wide side.  `table`: the size is that of a table (pages, blocks or segments),
+// not of rows.
 struct ShapedItem {
   DeviceLayout mem;
   uint64_t units = 0;
@@ -668,10 +668,12 @@ static ErrorCode blocks_item(const SourceBlocks& blocks, ShapedItem* it) {
   return ec;
 }
 
-static ErrorCode segments_item(const std::vector<SourceSegments::Segment>& segs, ShapedItem* it) {
+// Item i of a segment call, its segments in units of `unit` bytes (1, or for MXFP8 the wide type's).
+static ErrorCode segments_item(const std::vector<SourceSegments::Segment>& segs, uint64_t unit, ShapedItem* it) {
   SourceSegments g;
-  const ErrorCode ec = SourceSegments::from_segments(segs.data(), segs.size(), &it->segments, &g, &it->units);
+  const ErrorCode ec = SourceSegments::from_segments(segs.data(), segs.size(), &it->segments, &g, &it->units, unit);
   it->mem = DeviceLayout(g);
+  it->table = true;
   return ec;
 }
 
@@ -735,7 +737,11 @@ std::vector<ErrorCode> BlackbirdClient::shaped_get(std::string_view name, const 
         std::vector<DeviceLayout> mems;
         std::vector<uint64_t> units;
         for (size_t i : idx) mems.push_back(items[i].mem), units.push_back(items[i].units);
-        if (fp8) return get_device_fp8(pick(keys, idx), pick(ptrs, idx), units, nullptr, &mems, stream, *fp8);
+        if (fp8) {  // a fused get stores exactly the units its layout holds
+          auto ecs = get_device_fp8(pick(keys, idx), pick(ptrs, idx), units, nullptr, &mems, stream, *fp8);
+          for (size_t k = 0; out_sizes && k < idx.size(); ++k) (*out_sizes)[idx[k]] = ecs[k] == ErrorCode::OK ? units[k] : 0;
+          return ecs;
+        }
         std::vector<size_t> sizes;
         auto ecs = get_device(pick(keys, idx), pick(ptrs, idx), std::vector<size_t>(units.begin(), units.end()), nullptr, &mems, stream, &sizes);
         for (size_t k = 0; out_sizes && k < idx.size() && k < sizes.size(); ++k) (*out_sizes)[idx[k]] = sizes[k];
@@ -985,6 +991,24 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_blocks(const std::v
       [&](size_t i, ShapedItem* it) { return blocks_item(blocks[i], it); }, stream, nullptr);
 }
 
+std::vector<ErrorCode> BlackbirdClient::batch_put_device_fp8_segments(const std::vector<ObjectKey>& keys,
+                                                                      const std::vector<std::vector<SourceSegments::Segment>>& segments,
+                                                                      const WorkerConfig& cfg, void* stream, mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  return shaped_put(
+      "device_put_fp8_segments", keys, std::vector<const void*>(n), segments.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], mxfp8::wide_bytes(wide), it); }, cfg, stream);
+}
+
+std::vector<ErrorCode> BlackbirdClient::batch_get_device_fp8_segments(const std::vector<ObjectKey>& keys,
+                                                                      const std::vector<std::vector<SourceSegments::Segment>>& segments,
+                                                                      void* stream, std::vector<size_t>* out_sizes, mxfp8::Wide wide) {
+  const size_t n = keys.size();
+  return shaped_get(
+      "device_get_fp8_segments", keys, std::vector<void*>(n), segments.size() == n, wide,
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], mxfp8::wide_bytes(wide), it); }, stream, out_sizes);
+}
+
 std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectKey>& keys, const std::vector<void*>& bf16_ptrs,
                                                        const std::vector<uint64_t>& n_elems, const std::vector<ByteRange>* ranges,
                                                        const std::vector<DeviceLayout>* mem, void* stream, mxfp8::Wide wide) {
@@ -1024,7 +1048,8 @@ std::vector<ErrorCode> BlackbirdClient::get_device_fp8(const std::vector<ObjectK
     const auto& copies = placed[i].value();
     const uint64_t packed = n_elems[i] + n_elems[i] / 32;
     const DeviceLayout::Kind kind = mem_of(i).kind();
-    if ((kind == DeviceLayout::PAGES || kind == DeviceLayout::BLOCKS) && !copies.empty()) {  // the pages must hold exactly the stored object's elements
+    // the pages or segments must hold exactly the stored object's elements
+    if ((kind == DeviceLayout::PAGES || kind == DeviceLayout::BLOCKS || kind == DeviceLayout::SEGMENTS) && !copies.empty()) {
       uint64_t stored = 0;
       for (const auto& sh : copies[0].shards) stored += sh.length;
       if (stored != packed) {
@@ -1277,7 +1302,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_put_device_segments(const std::vec
   const size_t n = keys.size();
   return shaped_put(
       "device_put_segments", keys, std::vector<const void*>(n), segments.size() == n, std::nullopt,
-      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], it); }, cfg, stream);
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], 1, it); }, cfg, stream);
 }
 
 std::vector<ErrorCode> BlackbirdClient::put_device(const std::vector<ObjectKey>& keys, const std::vector<const void*>& dev_ptrs,
@@ -1492,7 +1517,7 @@ std::vector<ErrorCode> BlackbirdClient::batch_get_device_segments(const std::vec
   const size_t n = keys.size();
   return shaped_get(
       "device_get_segments", keys, std::vector<void*>(n), segments.size() == n, std::nullopt,
-      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], it); }, stream, out_sizes);
+      [&](size_t i, ShapedItem* it) { return segments_item(segments[i], 1, it); }, stream, out_sizes);
 }
 
 std::vector<ErrorCode> BlackbirdClient::batch_put_device_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks,

@@ -282,6 +282,29 @@ class BlackbirdClient {
                                                      const WorkerConfig& cfg, void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
   std::vector<ErrorCode> batch_get_device_fp8_blocks(const std::vector<ObjectKey>& keys, const std::vector<SourceBlocks>& blocks, void* stream,
                                                      mxfp8::Wide wide = mxfp8::Wide::BF16);
+  // Packed segment-list puts (a list of bf16, fp16 or fp32 tensors as one packed object): object i is the concatenation of
+  // the segments segments[i], each a (device address, elements of `wide`) pair, in list order (SourceSegments with the
+  // unit of the wide type, common/store_window.h).  The pack kernel reads each segment in place; an MX block may straddle
+  // two segments.  The stored packed object and its digest are byte for byte those of batch_put_device_fp8 of the
+  // concatenation, so every fp8 get reads it.  Placement, replica fan-out and errors are batch_put_device_fp8's.  Per
+  // object, the shaped calls' admission (shaped_put) of SourceSegments::from_segments: zero-length segments are dropped,
+  // VALUE_OUT_OF_RANGE when the total's bytes overflow, INVALID_ARGUMENT for a segment at address 0 and for an element
+  // total that is 0 or not a multiple of 32, NOT_IMPLEMENTED unless co-aligned in wide bytes (address = b * element
+  // offset mod 16 for every segment) -- there is no host-staged packed put.
+  std::vector<ErrorCode> batch_put_device_fp8_segments(const std::vector<ObjectKey>& keys,
+                                                       const std::vector<std::vector<SourceSegments::Segment>>& segments, const WorkerConfig& cfg,
+                                                       void* stream, mxfp8::Wide wide = mxfp8::Wide::BF16);
+  // Gets of packed objects into segments, the mirror: object i is unpacked into the segments segments[i] in list order,
+  // by the segmented scattering store of the fused unpack; out_sizes[i] receives its elements.  A segment at address 0
+  // is not stored (a null segment): its elements are still read, unpacked and verified, so a partial restore names only
+  // the segments it wants.  Fail-over and the placement refresh are batch_get_device_fp8's.  Admission as
+  // batch_put_device_fp8_segments', null segments allowed and co-alignment not checked there.  Then INVALID_ARGUMENT
+  // unless the stored object holds exactly the segments' element total, null segments counted; NOT_IMPLEMENTED when the
+  // object is not fusable (as batch_get_device_fp8) or the segments fail SourceSegments::fused_get_aligned in wide bytes
+  // -- there is no host-staged path; the rest of the batch keeps the fused launch.
+  std::vector<ErrorCode> batch_get_device_fp8_segments(const std::vector<ObjectKey>& keys,
+                                                       const std::vector<std::vector<SourceSegments::Segment>>& segments, void* stream,
+                                                       std::vector<size_t>* out_sizes, mxfp8::Wide wide = mxfp8::Wide::BF16);
   bool device_fp8_eligible(uint64_t n_elems) const { return device_ && device_->fp8_eligible(n_elems); }
   // Moves every copy of the object to `target` (promotion to the GPU tier, demotion to DRAM / NVMe ...).
   ErrorCode migrate(const ObjectKey& key, StorageClass target);

@@ -670,36 +670,45 @@ static_assert(sizeof(SegmentEntry) == 16, "one uint4 load per segment entry");
 //   addr[k] + (x - start[k])    for the k with start[k] <= x < start[k + 1]
 // The table is `nseg` SegmentEntry {start, addr} followed by the end sentinel {total, 0}, so that entry k + 1 gives the
 // end of segment k; from_segments() builds it (zero-length segments dropped, starts strictly increasing).  `phase` is
-// the object offset of byte 0 as the holder sees it (rebase()): byte x of a rebased table is object byte phase + x.  This
-// is the one statement of the rule; the transfer engine (XferItem), the fabric's ops (DeviceShardOp), the client, the
-// host loopback transport and the kernels' XFER_SEGMENTS descriptors (kernels/xfer.h) all follow it.  The unit is a byte
-// (there are no MXFP8 segment transfers).
+// the object byte offset of byte 0 as the holder sees it (rebase()): byte x of a rebased table is object byte phase + x.
+// This is the one statement of the rule; the transfer engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp,
+// DeviceFp8Op), the client, the host loopback transport and the kernels' XFER_SEGMENTS descriptors (kernels/xfer.h) all
+// follow it.
+//
+// Units.  The table (start, phase, total()) is always in bytes.  `unit` is the bytes per unit of its callers' lengths and
+// offsets: 1 for the byte calls, whose segments are (address, bytes), and b for an MXFP8 transfer, whose segments are
+// (address, elements) of its wide type of b bytes (2: bf16 / fp16, 4: fp32).  from_segments() scales the lengths once;
+// valid, rebase, has_null, segments_for, coaligned, fused_get_aligned and for_each_run take units; to_wide_bytes(b) is
+// the same table with unit 1, no copy.  So a packed segment transfer's wide bytes are co-aligned when
+// addr[k] = b * start_elem[k] (mod 16) for every non-null segment k, start_elem being its first element's object index.
 //
 // An address of 0 is a null segment, as SourcePages' null page: on the get side its bytes are read and verified but not
 // stored (a partial restore of some tensors of a bundle); a put refuses it (has_null, DeviceLayout::valid_source).  Null
 // segments start and extend no run and are exempt from the alignment rules.
 struct SourceSegments {
-  using Segment = std::pair<uint64_t, uint64_t>;  // (address, bytes)
+  using Segment = std::pair<uint64_t, uint64_t>;  // (address, units)
 
   const SegmentEntry* entries = nullptr;  // nseg entries, then the sentinel
   uint64_t nseg = 0, phase = 0;
+  uint64_t unit = 1;  // bytes per unit of the callers' lengths and offsets
 
   bool segmented() const { return entries != nullptr; }
-  // The object's size: the sentinel's start.
+  // The object's size in bytes: the sentinel's start.
   uint64_t total() const { return entries ? entries[nseg].start : 0; }
 
-  // The table of the `count` segments at segs into *table (which the result points into): an object of *size bytes.
-  // Zero-length segments are dropped.  VALUE_OUT_OF_RANGE when the total overflows.  No segment (or only empty ones) is
-  // a zero-byte object, with no table.
-  static ErrorCode from_segments(const Segment* segs, uint64_t count, std::vector<SegmentEntry>* table, SourceSegments* out, uint64_t* size) {
+  // The table of the `count` segments at segs, each (address, units of `unit` bytes), into *table (which the result points
+  // into): an object of *size units.  Zero-length segments are dropped.  VALUE_OUT_OF_RANGE when a segment's or the
+  // total's bytes overflow.  No segment (or only empty ones) is a zero-unit object, with no table.
+  static ErrorCode from_segments(const Segment* segs, uint64_t count, std::vector<SegmentEntry>* table, SourceSegments* out, uint64_t* size,
+                                 uint64_t unit = 1) {
     *out = {};
     *size = 0;
     table->clear();
-    uint64_t total = 0;
+    uint64_t total = 0, bytes = 0;
     for (uint64_t k = 0; k < count; ++k) {
       if (segs[k].second == 0) continue;
       table->push_back({total, segs[k].first});
-      if (__builtin_add_overflow(total, segs[k].second, &total)) {
+      if (__builtin_mul_overflow(segs[k].second, unit, &bytes) || __builtin_add_overflow(total, bytes, &total)) {
         table->clear();
         return ErrorCode::VALUE_OUT_OF_RANGE;
       }
@@ -707,53 +716,61 @@ struct SourceSegments {
     if (table->empty()) return ErrorCode::OK;
     const uint64_t n = table->size();
     table->push_back({total, 0});
-    *out = {table->data(), n, 0};
-    *size = total;
+    *out = {table->data(), n, 0, unit};
+    *size = total / unit;
     return ErrorCode::OK;
   }
 
-  // The segment holding byte x (x < total() - phase): the last entry starting at or before phase + x.
+  // The layout of an MXFP8 transfer's wide side, in bytes of elements of `b` bytes: the same table with unit 1.  False
+  // unless its unit is b (a table of bytes, or of another wide type).
+  bool to_wide_bytes(uint64_t b, SourceSegments* out) const {
+    *out = *this;
+    out->unit = 1;
+    return unit == b;
+  }
+
+  // The segment holding unit x (x < units left): the last entry starting at or before byte phase + unit * x.
   uint64_t seg_of(uint64_t x) const {
-    const uint64_t g = phase + x;
+    const uint64_t g = phase + unit * x;
     const SegmentEntry* e = std::upper_bound(entries, entries + nseg, g, [](uint64_t v, const SegmentEntry& s) { return v < s.start; });
     return e == entries ? 0 : static_cast<uint64_t>(e - entries) - 1;
   }
-  // Whether the table holds bytes [0, len) with its entry 0 holding byte 0, the form from_segments() and rebase() keep
+  // Whether the table holds units [0, len) with its entry 0 holding unit 0, the form from_segments() and rebase() keep
   // (start[0] <= phase < start[1], or phase == total() for a table rebased to its end): the kernels search from entry 0
   // and the engine copies the entries from there.
   bool valid(uint64_t len) const {
-    if (!segmented() || entries[0].start > phase || phase > total() || len > total() - phase) return false;
+    if (!segmented() || entries[0].start > phase || phase > total() || len > (total() - phase) / unit) return false;
     return nseg == 0 ? phase == total() : phase < entries[1].start;
   }
-  // Calls f(k) for every segment that bytes [0, len) touch, in order.
+  // Calls f(k) for every segment that units [0, len) touch, in order.
   template <class F>
   void for_each_touched(uint64_t len, F&& f) const {
     if (len == 0 || !segmented()) return;
-    for (uint64_t k = seg_of(0); k < nseg && entries[k].start < phase + len; ++k) f(k);
+    for (uint64_t k = seg_of(0); k < nseg && entries[k].start < phase + unit * len; ++k) f(k);
   }
-  // Segments that bytes [0, len) touch, the first being entry 0 of a rebased table.
+  // Segments that units [0, len) touch, the first being entry 0 of a rebased table.
   uint64_t segments_for(uint64_t len) const {
     uint64_t n = 0;
     for_each_touched(len, [&](uint64_t) { ++n; });
     return n;
   }
-  // Whether a segment that bytes [0, len) touch is null.
+  // Whether a segment that units [0, len) touch is null.
   bool has_null(uint64_t len) const {
     bool null = false;
     for_each_touched(len, [&](uint64_t k) { null = null || entries[k].addr == 0; });
     return null;
   }
 
-  // The table seen from byte `off` (off <= total() - phase): byte x of the result is byte off + x here.  Shards of a
-  // striped object may start inside a segment, which the new phase records; entry 0 of the result holds its byte 0.
+  // The table seen from unit `off` (off <= units left): unit x of the result is unit off + x here.  Shards of a striped
+  // object may start inside a segment, which the new phase records; entry 0 of the result holds its unit 0.
   SourceSegments rebase(uint64_t off) const {
     if (!segmented()) return *this;
-    const uint64_t g = phase + off;
+    const uint64_t g = phase + unit * off;
     const uint64_t k = g < total() ? seg_of(off) : nseg;
-    return {entries + k, nseg - k, g};
+    return {entries + k, nseg - k, g, unit};
   }
 
-  // Whether bytes [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by TMA:
+  // Whether units [0, len) are co-aligned with the tiles, so that the kernel only moves 16-byte congruent spans by TMA:
   // byte x of segment k lives at addr[k] - start[k] + phase + x, so addr[k] + phase - start[k] must be 16-byte aligned
   // for every non-null segment touched.  (For a shard cut at a multiple of 16 bytes that is addr[k] = start[k] mod 16.)
   bool coaligned(uint64_t len) const {
@@ -766,26 +783,29 @@ struct SourceSegments {
   // is the segments' own, addr[k] = start[k] mod 16 where the object is cut at 16-byte multiples.
   bool fused_get_aligned(uint64_t off, uint64_t len) const { return rebase(off).coaligned(len); }
 
-  // Calls f(x, addr, n) for every run of n contiguous bytes of bytes [0, len): bytes [x, x + n) live at [addr, addr + n),
-  // in order.  Segments that follow one another in memory make one run; null segments make none and end the run before
-  // them.
+  // Calls f(x, addr, n) for every run of n contiguous units of units [0, len): units [x, x + n) live at bytes
+  // [addr, addr + unit * n), in order.  Segments that follow one another in memory make one run; null segments make none
+  // and end the run before them.
   template <class F>
   void for_each_run(uint64_t len, F&& f) const {
     uint64_t run_x = 0, run_at = 0, run_n = 0;
+    auto emit = [&] {
+      if (run_n) f(run_x / unit, run_at, run_n / unit);
+    };
     for_each_touched(len, [&](uint64_t k) {
-      const uint64_t a = std::max(entries[k].start, phase), b = std::min(entries[k + 1].start, phase + len);
+      const uint64_t a = std::max(entries[k].start, phase), b = std::min(entries[k + 1].start, phase + unit * len);
       const uint64_t x = a - phase, n = b - a, at = entries[k].addr + (a - entries[k].start);
       if (entries[k].addr == 0) {
-        if (run_n) f(run_x, run_at, run_n);
+        emit();
         run_n = 0;
       } else if (run_n && run_at + run_n == at) {
         run_n += n;
       } else {
-        if (run_n) f(run_x, run_at, run_n);
+        emit();
         run_x = x, run_at = at, run_n = n;
       }
     });
-    if (run_n) f(run_x, run_at, run_n);
+    emit();
   }
 };
 
@@ -793,9 +813,8 @@ struct SourceSegments {
 // contiguous (unit x at base + x, the default), in rows (SourceRows, with row 0 at the base), in pages (SourcePages,
 // whose addresses are absolute: the base is not used), in blocks picked by device-resident ids (SourceBlocks, absolute
 // too) or in segments of any sizes (SourceSegments, absolute too).  It is the source of a put and the destination of a
-// get, in bytes, or for an MXFP8 transfer in elements of the wide side until to_wide_bytes() (which refuses segments).
-// This is the one place that knows the kinds; the transfer engine (XferItem,
-// Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the transports all hold one of these.  A
+// get, in bytes, or for an MXFP8 transfer in elements of the wide side until to_wide_bytes().  This is the one place
+// that knows the kinds; the transfer engine (XferItem, Fp8Item), the fabric's ops (DeviceShardOp, DeviceFp8Op), the client and the transports all hold one of these.  A
 // StoreWindow goes with a contiguous layout, or with WINDOW_ROWS: rows of the window's dense result (WindowRows), which
 // only a get's destination has and only the calls that take both a window and destination rows build (window_rows()).
 // Its rows() are the WindowRows' rows, and the functions below that have no window treat it as the rows of a whole-object
@@ -858,14 +877,14 @@ class DeviceLayout {
   }
 
   // The layout of an MXFP8 transfer's wide side, given in elements, in bytes of elements of `b` bytes (2 or 4).  False
-  // when the byte arithmetic could overflow, and for segments, which have no MXFP8 transfers.
+  // when the byte arithmetic could overflow, and for segments whose unit is not b.
   bool to_wide_bytes(uint64_t b, DeviceLayout* out) const {
     *out = *this;
-    if (kind_ == SEGMENTS) return false;
     return kind_ == ROWS || kind_ == WINDOW_ROWS ? rows_.to_wide_bytes(b, &out->rows_)
-           : kind_ == PAGES  ? pages_.to_wide_bytes(b, &out->pages_)
-           : kind_ == BLOCKS ? blocks_.to_wide_bytes(b, &out->blocks_)
-                             : true;
+           : kind_ == PAGES    ? pages_.to_wide_bytes(b, &out->pages_)
+           : kind_ == BLOCKS   ? blocks_.to_wide_bytes(b, &out->blocks_)
+           : kind_ == SEGMENTS ? segments_.to_wide_bytes(b, &out->segments_)
+                               : true;
   }
 
   // The layout seen from object unit `off`: unit x of the result is unit off + x here, relative to a base that has moved

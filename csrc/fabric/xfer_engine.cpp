@@ -563,6 +563,7 @@ Result<uint64_t> XferEngine::submit(const std::vector<XferItem>& items, Checksum
     const uint32_t scatter_excl = (wrows ? 0u : XFER_WINDOW | XFER_STRIDED) | XFER_GATHER | XFER_MULTIMEM | XFER_RAW_SUM;
     if ((gather || scatter) == mem.contiguous() || ((it.flags & XFER_PAGED) && mem.kind() != DeviceLayout::PAGES && !blocks) ||
         !(gather ? mem.valid_source(it.nbytes) : mem.valid(it.nbytes)) || (gather && (it.flags & (XFER_WINDOW | XFER_STRIDED | XFER_RAW_SUM))) ||
+        (mem.kind() == DeviceLayout::SEGMENTS && mem.segments().unit != 1) ||
         (scatter && (it.ndst != 1 || (it.flags & scatter_excl))))
       return ErrorCode::INVALID_ARGUMENT;
     if (blocks && scatter && !it.mem.blocks().distinct_checkable()) return ErrorCode::NOT_IMPLEMENTED;

@@ -49,7 +49,7 @@ struct XferItem {
   // ready on `stream` (stream order), and the outer array need only live until submit() returns.  Segments
   // (SourceSegments) take XFER_SEGMENTS, which submit() sets (among the caller's flags it is INVALID_ARGUMENT): the entries
   // the item's bytes touch are copied into the batch's device table like page entries, a get's null segments are read and
-  // hashed but not stored, a put's are INVALID_ARGUMENT.
+  // hashed but not stored, a put's are INVALID_ARGUMENT, and so is a table whose unit is not a byte.
   DeviceLayout mem;
 };
 
@@ -78,17 +78,18 @@ struct Fp8Item {
   // the whole object.  The whole packed object is still read and verified.  INVALID_ARGUMENT unless valid against
   // n_elems; INVALID_ADDRESS unless a strided window is co-aligned in bf16 bytes, as XferItem's.
   StoreWindow win;
-  // The wide side's rows or pages in elements, the page addresses in bytes (common/store_window.h), `wide` being the
-  // layout's base (not read for pages): a pack's source or an unpack's destination.  The default is contiguous.  run_fp8
-  // sets XFER_GATHER or XFER_SCATTER for it, with XFER_PAGED for pages whose entries it copies into the batch's device
-  // table (and XFER_PAGE_ROWS for in-page rows), so the host array need only live until run_fp8 returns.  An MX block may
-  // straddle two pages or two in-page rows.  An unpack's table
-  // may hold null pages, whose elements are not stored; a pack's may not.
+  // The wide side's rows, pages or segments in elements, the addresses in bytes (common/store_window.h), `wide` being the
+  // layout's base (not read for pages and segments): a pack's source or an unpack's destination.  The default is
+  // contiguous.  run_fp8 sets XFER_GATHER or XFER_SCATTER for it, with XFER_PAGED for pages whose entries it copies into
+  // the batch's device table (and XFER_PAGE_ROWS for in-page rows), or XFER_SEGMENTS for segments (a table whose unit is
+  // the wide type's bytes), whose entries it copies likewise, so the host array need only live until run_fp8 returns.  An
+  // MX block may straddle two pages, two in-page rows or two segments.  An unpack's table may hold null pages or
+  // segments, whose elements are not stored; a pack's may not.
   // INVALID_ARGUMENT with a window, unless mem.valid(n_elems) (a pack: mem.valid_source(n_elems)), or when its wide-byte
   // arithmetic overflows;
   // INVALID_ADDRESS unless it is co-aligned in wide bytes (DeviceLayout::coaligned of b * n_elems), which replaces the
-  // 16-byte alignment check of `wide`.  Blocks as XferItem's, the verdict in XferResult::verdict.  Segments are
-  // INVALID_ARGUMENT: there are no MXFP8 segment transfers.
+  // 16-byte alignment check of `wide`.  Blocks as XferItem's, the verdict in XferResult::verdict.  Segments whose unit is
+  // not the wide type's bytes are INVALID_ARGUMENT.
   DeviceLayout mem;
 };
 

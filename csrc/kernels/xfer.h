@@ -71,16 +71,17 @@ enum XferFlags : uint32_t {
   // WINDOW_ROWS layout); never with XFER_SCATTER, XFER_GATHER, XFER_PAGED, XFER_MULTIMEM or XFER_RAW_SUM.  Every tile
   // is still loaded and hashed, so the digest and the verify are those of a plain get.
   XFER_WINDOW_ROWS = 1u << 10,
-  // Segmented source or destination (SourceSegments, common/store_window.h), in bb_xfer only, together with XFER_GATHER
-  // (a put reads its segments) or XFER_SCATTER (a get stores into them): the object is the concatenation of segments of
-  // any sizes, object byte x at addr[k] + (x - start[k]) for the segment k with start[k] <= x < start[k + 1].  The
-  // descriptor's XferStride entry is {device address of its first segment entry, number of segments, object offset of the
+  // Segmented source or destination (SourceSegments, common/store_window.h), in bb_xfer and bb_xfer_fp8, together with
+  // XFER_GATHER (a put or a pack reads its segments) or XFER_SCATTER (a get or an unpack stores into them), in bytes (of
+  // the wide side for bb_xfer_fp8): the object is the concatenation of segments of any sizes, object byte x at
+  // addr[k] + (x - start[k]) for the segment k with start[k] <= x < start[k + 1].  The descriptor's XferStride entry is {device address of its first segment entry, number of segments, object offset of the
   // descriptor's byte 0}; the entries are 16-byte SegmentEntry {start, addr} pairs followed by one whose start ends the
   // last segment.  `src` (put) or dst[0] (get) is not read.  Per tile the walking warp finds the tile's first segment by a
   // 32-way search and takes the segments that overlap the tile one per lane.  A get's segment whose address is 0 is not
   // stored (a null segment).  Only the engine sets it (from a SEGMENTS layout); never with XFER_PAGED, XFER_PAGE_ROWS,
   // XFER_WINDOW, XFER_STRIDED, XFER_WINDOW_ROWS or XFER_RAW_SUM.  The tile in shared memory is the dense object's tile,
-  // so the digest, the verify and the stored bytes are those of a contiguous put or get of the concatenation.
+  // so the digest, the verify and the stored bytes are those of a contiguous put or get of the concatenation (for
+  // bb_xfer_fp8 the wide tile is the concatenation's, so an MX block may straddle two segments).
   XFER_SEGMENTS = 1u << 11,
 };
 

@@ -11,7 +11,10 @@
 //                   tile, the packed object and its digest are those of a put of the compacted rows.  With
 //                   XFER_GATHER | XFER_PAGED (puts of the blocks of a paged cache) the row segments are the pages of
 //                   SourcePages in wide bytes, each read from the address in the page table, so the tile is that
-//                   of the concatenated pages; an MX block may straddle two pages, the codec never sees it.
+//                   of the concatenated pages; an MX block may straddle two pages, the codec never sees it.  With
+//                   XFER_GATHER | XFER_SEGMENTS (puts of a list of tensors) the lanes take the segments of the
+//                   SourceSegments table that overlap the tile, in wide bytes, so the tile is that of the concatenated
+//                   segments and an MX block may straddle two segments the same way.
 //   get  (UNPACK) : TMA loads payload tile + scales from the slab -> tensor-core hash of the payload tile ->
 //                   8 unpack warps expand to bf16 in shared memory -> TMA stores the 32 KiB tile to the caller.
 //                   With XFER_WINDOW (element-range gets) only the bf16 bytes [win.lo, win.hi) of the object are
@@ -22,7 +25,8 @@
 //                   With XFER_SCATTER instead (gets into a sliced tensor) the store warp stores every 32 KiB bf16 tile
 //                   as the row segments of the destination rows, by the SourceRows rule in bf16 bytes, as bb_xfer does;
 //                   with XFER_SCATTER | XFER_PAGED (gets into the blocks of a paged cache) as the segments of the
-//                   destination pages, by the SourcePages rule in wide bytes.
+//                   destination pages, by the SourcePages rule in wide bytes; with XFER_SCATTER | XFER_SEGMENTS (gets
+//                   into a list of tensors) as the tile's parts of the destination segments, a null segment not stored.
 //
 // The stored object keeps the layout of the unfused path ([E4M3 payload n][E8M0 scales n/32], common/mxfp8.h), and so
 // does its digest: BBH64 is a sum of per-tile terms, this kernel accumulates the payload tiles (tile index 0..T-1)
@@ -78,8 +82,9 @@ struct FpMeta {            // 64 bytes
   uint32_t strided;        // unpack: XFER_STRIDED when the descriptor's window is strided, XFER_SCATTER when its
                            // destination is rows; pack: XFER_GATHER when its source is rows (the pattern in
                            // FpParams::strides either way); XFER_PAGED as well when those rows are pages,
-                           // and XFER_PAGE_ROWS when the pages are in-page rows; unpack: XFER_WINDOW_ROWS when the
-                           // window's result lands in rows (with XFER_STRIDED for a strided window)
+                           // and XFER_PAGE_ROWS when the pages are in-page rows, or XFER_SEGMENTS when they are the
+                           // segments of a table; unpack: XFER_WINDOW_ROWS when the window's result lands in rows
+                           // (with XFER_STRIDED for a strided window)
   uint32_t f16;            // XFER_WIDE_F16: the wide side is fp16 (2-byte instantiation only)
   uint32_t pad;
 };
@@ -174,8 +179,8 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
         e.m.desc = lo;
         e.m.tile_in_obj = ti;
         e.m.obj_ntiles = next - first;
-        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED | XFER_PAGE_ROWS | XFER_WINDOW_ROWS
-                                        : XFER_GATHER | XFER_PAGED | XFER_PAGE_ROWS);
+        e.m.strided = d.flags & (UNPACK ? XFER_STRIDED | XFER_SCATTER | XFER_PAGED | XFER_PAGE_ROWS | XFER_WINDOW_ROWS | XFER_SEGMENTS
+                                        : XFER_GATHER | XFER_PAGED | XFER_PAGE_ROWS | XFER_SEGMENTS);
         e.m.f16 = d.flags & XFER_WIDE_F16;
         e.m.pad = 0;
         e.m.valid = static_cast<uint32_t>(min(static_cast<uint64_t>(kTileBytes), nbytes - static_cast<uint64_t>(ti) * kTileBytes));
@@ -237,8 +242,10 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             // XFER_PAGED: the rows are the pages of the table in gst, e.src is not read
             const uint64_t off = static_cast<uint64_t>(e.m.tile_in_obj) * kWideBytes;
             // XFER_PAGE_ROWS: their in-page rows, whose pattern is read here so that `gst` stays three words
+            // XFER_SEGMENTS: the segments of the table in gst that overlap the tile
             const uint32_t seg_tx =
-                e.m.strided & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid,
+                e.m.strided & XFER_SEGMENTS    ? gather_row_segments<false, false, true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane)
+                : e.m.strided & XFER_PAGE_ROWS ? gather_row_segments<true, true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid,
                                                                                load_stride(p.strides, g_desc, true), lane)
                 : e.m.strided & XFER_PAGED   ? gather_row_segments<true>(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane)
                                              : gather_row_segments(s.wide[ws], &s.w_full[ws], e.src, off, WB * e.m.valid, gst, lane);
@@ -277,11 +284,12 @@ __global__ void __launch_bounds__(kFpThreads, 1) bb_xfer_fp8_kernel(const __grid
             pat_desc = m.desc;
             pat = load_stride(p.strides, pat_desc);
           }
-          // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile.  A paged one stores
-          // into the pages of the table in `pat` and does not read dst[0].
+          // m.dst[0] = dst[0] + off; a scattering store has no window, so [x0, x1) is the whole tile.  A paged or segmented
+          // one stores into the pages or segments of the table in `pat` and does not read dst[0].
           if (m.strided & XFER_WINDOW_ROWS)  // the window's segments cut at the destination rows of the dense result
             store_window_rows(s.wide[st], m.dst[0] - off, off, x0, x1, m.dst[1], m.strided & XFER_STRIDED,
                               load_stride(p.strides, m.desc, true), lane);
+          else if (m.strided & XFER_SEGMENTS) scatter_row_segments<false, false, true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);
           else if (m.strided & XFER_PAGE_ROWS)
             scatter_row_segments<true, true>(s.wide[st], m.dst[0] - off, off, x1, load_stride(p.strides, pat_desc, true), lane);
           else if (m.strided & XFER_PAGED) scatter_row_segments<true>(s.wide[st], m.dst[0] - off, off, x1, pat, lane);

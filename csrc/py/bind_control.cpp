@@ -548,8 +548,11 @@ void bind_control(py::module_& m) {
                          "An object that is the concatenation of segments of any sizes at arbitrary addresses: a segment put's "
                          "source, or a segment get's destination (common/store_window.h).  Segment k holds object bytes "
                          "[start[k], start[k] + len[k]), start the exclusive prefix sum, and object byte x lives at addr[k] + (x - "
-                         "start[k]).  Byte x of a rebased table is object byte phase + x.")
+                         "start[k]).  Byte x of a rebased table is object byte phase + x.  The table (entries, phase, total) is in "
+                         "bytes; lengths and offsets the methods take are in units of `unit` bytes (1, or an MXFP8 transfer's "
+                         "wide element size).")
       .def_property_readonly("nseg", [](const PySegments& t) { return t.g.nseg; })
+      .def_property_readonly("unit", [](const PySegments& t) { return t.g.unit; })
       .def_property_readonly("phase", [](const PySegments& t) { return t.g.phase; })
       .def_property_readonly("total", [](const PySegments& t) { return t.g.total(); })
       .def_property_readonly("entries",
@@ -565,31 +568,40 @@ void bind_control(py::module_& m) {
            "whether a segment that bytes [0, len) touch has address 0 (not stored by a get, refused by a put)")
       .def("segments_for", [](const PySegments& t, uint64_t len) { return t.g.segments_for(len); }, py::arg("len"))
       .def_static("from_segments",
-                  [](const py::handle& segs) {
+                  [](const py::handle& segs, uint64_t elem_bytes) {
+                    if (elem_bytes == 0) throw py::value_error("elem_bytes must be positive");
                     const auto v = to_segments(segs);
                     auto table = std::make_shared<std::vector<SegmentEntry>>();
                     PySegments t;
                     uint64_t size = 0;
-                    const ErrorCode ec = SourceSegments::from_segments(v.data(), v.size(), table.get(), &t.g, &size);
+                    const ErrorCode ec = SourceSegments::from_segments(v.data(), v.size(), table.get(), &t.g, &size, elem_bytes);
                     t.table = table;
                     return py::make_tuple(ec, t, size);
                   },
-                  py::arg("segments"), "(ErrorCode, SourceSegments, object bytes) of (address, bytes) pairs")
+                  py::arg("segments"), py::arg("elem_bytes") = 1,
+                  "(ErrorCode, SourceSegments, object units) of (address, units) pairs, a unit being elem_bytes bytes")
       .def("rebase", [](const PySegments& t, uint64_t off) { return PySegments{t.table, t.g.rebase(off)}; }, py::arg("off"),
-           "the table seen from byte off")
+           "the table seen from unit off")
+      .def("to_wide_bytes",
+           [](const PySegments& t, uint64_t b) -> py::object {
+             PySegments w{t.table, {}};
+             if (!t.g.to_wide_bytes(b, &w.g)) return py::none();
+             return py::cast(w);
+           },
+           py::arg("b"), "the same table with unit 1, or None unless its unit is b")
       .def("coaligned", [](const PySegments& t, uint64_t len) { return t.g.coaligned(len); }, py::arg("len"))
       .def("fused_get_aligned", [](const PySegments& t, uint64_t off, uint64_t len) { return t.g.fused_get_aligned(off, len); },
            py::arg("off"), py::arg("len"))
       .def("runs",
            [](const PySegments& t, uint64_t len) {
-             if (len > 0 && !t.g.valid(len)) throw py::value_error("the table does not hold len bytes");
+             if (len > 0 && !t.g.valid(len)) throw py::value_error("the table does not hold len units");
              std::vector<std::tuple<uint64_t, uint64_t, uint64_t>> out;
              t.g.for_each_run(len, [&](uint64_t x, uint64_t at, uint64_t n) { out.emplace_back(x, at, n); });
              return out;
            },
            py::arg("len"),
-           "[(x, addr, n)]: bytes [x, x + n) live at [addr, addr + n); segments adjacent in memory make one run, null segments "
-           "none");
+           "[(x, addr, n)]: units [x, x + n) live at bytes [addr, addr + unit * n); segments adjacent in memory make one run, "
+           "null segments none");
 
   py::class_<PyBlocks>(m, "DeviceBlocks",
                        "Pages of a paged KV cache named by block ids that stay on the device (SourceBlocks, common/store_window.h): "
@@ -1714,6 +1726,28 @@ void bind_control(py::module_& m) {
          "verified, only its elements are written; a page address of 0 is not stored (a partial restore); rows as "
          "batch_put_device_fp8_paged's; returns one "
          "ErrorCode per object (NOT_IMPLEMENTED: get it whole and copy).")
+      .def("batch_put_device_fp8_segments", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& segments,
+                                               const WorkerConfig& cfg, uintptr_t stream, mxfp8::Wide wide) {
+        const auto lists = to_segment_lists(segments);
+        return ecs_to_py(nogil([&] { return c.batch_put_device_fp8_segments(keys, lists, cfg, reinterpret_cast<void*>(stream), wide); }));
+      }, py::arg("keys"), py::arg("segments"), py::arg("config") = WorkerConfig{}, py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         "Packed tensor i = the segments segments[i] concatenated in order, each an (address, elements of `wide`) pair (a "
+         "list of pairs or an (n, 2) integer array); packed in the put kernel and stored as batch_put_device_fp8 of the "
+         "concatenation would store it.  Zero-length segments are dropped; a segment at address 0, or an element total "
+         "that is 0 or not a multiple of 32, is INVALID_ARGUMENT for that object; returns one ErrorCode per object "
+         "(NOT_IMPLEMENTED: a segment's address is not congruent to its element offset times the element size mod 16, or "
+         "the placement is not fusable -- pack a contiguous copy and put that).")
+      .def("batch_get_device_fp8_segments", [](BlackbirdClient& c, const std::vector<std::string>& keys, const py::sequence& segments,
+                                               uintptr_t stream, mxfp8::Wide wide) {
+        const auto lists = to_segment_lists(segments);
+        std::vector<size_t> sizes;
+        const auto ecs = nogil([&] { return c.batch_get_device_fp8_segments(keys, lists, reinterpret_cast<void*>(stream), &sizes, wide); });
+        return py::make_tuple(ecs_to_py(ecs), sizes);
+      }, py::arg("keys"), py::arg("segments"), py::arg("stream") = 0, py::arg("wide") = mxfp8::Wide::BF16,
+         "Packed tensor i, which must hold exactly the segments' element total (null segments included), unpacked to type "
+         "`wide` into the segments segments[i] in order; the whole packed object is read and verified, only its elements "
+         "are written; a segment at address 0 is not stored (a partial restore); returns (one ErrorCode per object, "
+         "elements per object) (NOT_IMPLEMENTED: get it whole and copy).")
       .def("cluster_stats", [](BlackbirdClient& c) { return unwrap(nogil([&] { return c.cluster_stats(); })); })
       .def("metrics_text", &BlackbirdClient::metrics_text)
       .def("set_device_pipeline_chunks", &BlackbirdClient::set_device_pipeline_chunks)

@@ -55,10 +55,10 @@ struct Keep {
 // The layout slots of an item tuple (common/store_window.h), first to last: gather rows, scatter rows, source pages,
 // destination pages, source blocks, destination blocks, source segments and destination segments.  Rows are given as
 // (pitch, width, phase), pages as (addrs, page, phase), whose addresses are kept in `keep` until the batch has been
-// submitted, blocks as a DeviceBlocks, segments as (segments, off): the (address, bytes) pairs of the whole object
-// (SourceSegments::from_segments, its table kept in `keep`) seen from object byte off (rebase).  Returns the slot set, -1
-// for none (even: the source side); an item takes one layout, so a second slot is the engine's INVALID_ARGUMENT, raised
-// as `what`.
+// submitted, blocks as a DeviceBlocks, segments as (segments, off[, unit]): the (address, units) pairs of the whole
+// object in units of `unit` bytes (1 unless given; an MXFP8 transfer's are elements of its wide type), seen from object
+// unit off (SourceSegments::from_segments and rebase, the table kept in `keep`).  Returns the slot set, -1 for none
+// (even: the source side); an item takes one layout, so a second slot is the engine's INVALID_ARGUMENT, raised as `what`.
 int to_layout(const py::tuple& t, const size_t (&slots)[8], Keep& keep, DeviceLayout* out, const char* what) {
   int set = -1;
   for (int k = 0; k < 8; ++k) {
@@ -67,12 +67,14 @@ int to_layout(const py::tuple& t, const size_t (&slots)[8], Keep& keep, DeviceLa
     set = k;
     if (k >= 6) {
       auto g = py::cast<py::tuple>(t[slots[k]]);
-      if (g.size() != 2) throw py::value_error("segments = ([(addr, bytes), ...], off)");
+      if (g.size() != 2 && g.size() != 3) throw py::value_error("segments = ([(addr, units), ...], off[, unit])");
+      const uint64_t unit = g.size() == 3 ? g[2].cast<uint64_t>() : 1;
+      if (unit == 0) throw py::value_error("segments: unit must be positive");
       const auto pairs = g[0].cast<std::vector<std::pair<uint64_t, uint64_t>>>();
       keep.segments.emplace_back();
       SourceSegments seg;
       uint64_t size = 0;
-      check(SourceSegments::from_segments(pairs.data(), pairs.size(), &keep.segments.back(), &seg, &size), what);
+      check(SourceSegments::from_segments(pairs.data(), pairs.size(), &keep.segments.back(), &seg, &size, unit), what);
       *out = DeviceLayout(seg.rebase(std::min(g[1].cast<uint64_t>(), size)));
     } else if (k < 2) {
       auto g = t[slots[k]].cast<std::vector<uint64_t>>();
@@ -224,7 +226,8 @@ void bind_gpu(py::module_& m) {
                if (t.size() < 3 || t.size() > 15)
                  throw py::value_error(
                      "fp8 item = (bf16_ptr, packed_ptr|[packed..], n_elems[, expect[, window[, gather (pitch, width, phase)[, "
-                     "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)]]]]]]])");
+                     "scatter (pitch, width, phase)[, wide[, src pages (addrs, page, phase)[, dst pages (addrs, page, phase)[, src "
+                     "blocks[, dst blocks[, window rows[, src segments ([(addr, elems)], off, elem_bytes)[, dst segments]]]]]]]]]]]])");
                if (t.size() > 3 && !t[3].is_none()) it.expect = t[3].cast<uint64_t>(), it.verify = true;
                if (t.size() > 4 && !t[4].is_none()) to_window(t[4], &it.win);
                if (t.size() > 7 && !t[7].is_none()) it.wide_type = t[7].cast<mxfp8::Wide>();
@@ -267,9 +270,14 @@ void bind_gpu(py::module_& m) {
            "every page touched is co-aligned in wide bytes and, for several pages, page % 8 == 0.  A put's source blocks "
            "(DeviceBlocks, page in elements) as the eleventh element and a get's destination blocks as the twelfth take a "
            "page table the resolve kernel builds on the stream.  A get's window rows (pitch, width, phase), in elements, as the "
-           "thirteenth element store the window's dense result into rows by the rule of WindowRows.  Returns (digests of the "
-           "packed objects, status, "
-           "device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item.")
+           "thirteenth element store the window's dense result into rows by the rule of WindowRows.  A put's source segments "
+           "(pairs, off, elem_bytes) as the fourteenth element read the (address, elements) pairs concatenated, seen from "
+           "element off: element x from the segment holding off + x (bf16_ptr is not read); a get's destination segments "
+           "as the fifteenth store by the same rule, a segment at address 0 not stored.  INVALID_ARGUMENT for segments on "
+           "the wrong side, with a window, null on a put, or whose unit is not the item's element size (elem_bytes 2 for "
+           "bf16 / fp16, 4 for fp32; (pairs, off) is a table of bytes, as run's); INVALID_ADDRESS unless every non-null "
+           "segment's address is congruent to elem_bytes times its first element's index mod 16.  Returns (digests of the packed objects, "
+           "status, device_ms), and for a batch with blocks also the verdicts, one ErrorCode per item.")
       .def_static("fp8_eligible", &XferEngine::fp8_eligible)
       .def("submit",
            [](XferEngine& e, const py::list& items, ChecksumAlgo algo, uintptr_t stream) {
